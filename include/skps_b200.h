@@ -264,6 +264,39 @@ SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot, const uint8_t* const* fr
 SKPS_API int skps_mpipe_wait(skps_mpipe* p, int slot, int32_t* n_faces, double* boxes, double* kps, float* scores,
                              int32_t* ran_detector);
 
+/* ---- Aligned face chips (csrc/align.cu; additive) -----------------------------------------------------------------------
+ * What a caller does with the 98 landmarks before a recognition / attribute model: estimate the least-squares similarity
+ * (rotation, uniform scale, translation; no reflection; Umeyama 1991) from landmarks [96, 97, 54, 76, 82] (pupils, nose tip,
+ * mouth corners) to the ArcFace 112x112 five-point template scaled by size/112, and warp a size x size chip with it.
+ * Replaces, per face on the host,
+ *     M = <similarity estimate>; chip = cv2.warpAffine(frame, M, (size, size), flags=cv2.INTER_LINEAR,
+ *                                                      borderMode=cv2.BORDER_CONSTANT, borderValue=0)
+ * byte for byte (OpenCV's fixed-point path).  M is (2,3) float64 frame -> chip, the matrix one passes to cv2.warpAffine.
+ * Chips are BGR like the frame.  size is 16..512. */
+
+/* Batched cv2.warpAffine of one [dev] HxWx3 uint8 frame (row pitch `pitch` bytes) with n arbitrary affine matrices
+ * M [dev] (n,2,3) float64 (shear included) -> out [dev] (n,out_h,out_w,3) uint8.  count [dev] or NULL: matrices i >= *count
+ * are skipped (their output is left as it was).  Asynchronous on `stream`. */
+SKPS_API int skps_warp_affine(const uint8_t* frame, int H, int W, int pitch, const double* M, const int32_t* count, int n,
+                              int out_h, int out_w, uint8_t* out, void* stream);
+/* Estimate + warp for n faces of one [dev] frame: kps [dev] (n,P,2) float64 with P >= 98 (WFLW-98 order) -> chips [dev]
+ * (n,size,size,3) uint8 and M [dev] (n,2,3) float64.  count [dev] or NULL as above.  Asynchronous on `stream`. */
+SKPS_API int skps_align_faces(const uint8_t* frame, int H, int W, int pitch, const double* kps, const int32_t* count, int n,
+                              int P, int size, uint8_t* chips, double* M, void* stream);
+/* skps_align_faces on the frame of the last skps_pipeline_run / skps_pipeline_commit_frame (still in HBM, not uploaded
+ * again) for FaceAna, whose landmarks are smoothed on the host: kps [host] (n,n_points,2) float64, chips [host]
+ * (n,size,size,3) uint8, M [host] (n,2,3) float64.  n <= top_k.  Synchronous. */
+SKPS_API int skps_pipeline_align(skps_pipeline* p, const double* kps, int n, int size, uint8_t* chips, double* M, void* stream);
+/* FaceAnaStreams: size > 0 makes every following skps_mpipe_submit warp one chip per returned face, from the smoothed
+ * float64 landmarks of the temporal layer and the frame in the stream's ring, on the compute stream without a host
+ * synchronisation; chips and matrices are copied back with the slot's other results.  size 0 switches it off and frees the
+ * buffers (n_streams x top_k x size^2 x 3 bytes on the device and twice that pinned on the host); an allocation failure is
+ * reported through skps_last_error.  No batch may be in flight. */
+SKPS_API int skps_mpipe_set_align(skps_mpipe* p, int size);
+/* After skps_mpipe_wait(slot), for a slot submitted with alignment on: chips [host] (n, top_k, size, size, 3) uint8 and
+ * M [host] (n, top_k, 2, 3) float64, n = that submit's stream count; entries i >= n_faces[s] are undefined. */
+SKPS_API int skps_mpipe_align_results(skps_mpipe* p, int slot, uint8_t* chips, double* M);
+
 #ifdef __cplusplus
 }
 #endif

@@ -18,6 +18,7 @@ from ...logger.logger import logger
 from ..smoother.lk import EmaFilter, GroupTrack
 from .face_detector import FaceDetector, letterbox_geometry
 from .face_landmark import FaceLandmark
+from .align import check_size
 
 
 def get_cfg():
@@ -28,7 +29,11 @@ def get_cfg():
 
 
 class FaceAna():
-    def __init__(self, verbose=False, top_k=None, max_frame_hw=(2160, 3840)):
+    def __init__(self, verbose=False, top_k=None, max_frame_hw=(2160, 3840), align=None):
+        """align: None, or a chip side in 16..512: every result dict then also carries 'chip' ((align, align, 3) uint8
+        BGR, the face warped to the ArcFace five-point template) and 'M' ((2, 3) float64, the frame -> chip matrix for
+        cv2.warpAffine), computed on the GPU from the returned 'kps' and the frame already in HBM (core/api/align.py)."""
+        self.align = None if align is None else check_size(align)
         if verbose:
             logger.setLevel(logging.DEBUG)
         cfg = get_cfg()
@@ -119,7 +124,22 @@ class FaceAna():
                           np.max(landmarks[i][:, 0]), np.max(landmarks[i][:, 1])])
         tmp_box = np.array(track)
         self.track_box = self.judge_boxs(boxes_return, tmp_box)
-        return self.to_dict(self.track_box, landmarks, states)
+        res = self.to_dict(self.track_box, landmarks, states)
+        if self.align is not None and res:
+            self._add_chips(res)
+        return res
+
+    def _add_chips(self, res):
+        """'chip' and 'M' for every face, from its returned 'kps' promoted to float64 (skps_pipeline_align)."""
+        n, size = len(res), self.align
+        kps = np.ascontiguousarray(np.stack([np.asarray(r['kps'], np.float64) for r in res]))
+        chips = np.empty((n, size, size, 3), np.uint8)
+        M = np.empty((n, 2, 3), np.float64)
+        rt.check(self.lib.skps_pipeline_align(self._pipe, kps.ctypes.data, n, size, chips.ctypes.data, M.ctypes.data,
+                                              self._stream.cuda_stream))
+        for i, r in enumerate(res):
+            r['chip'] = chips[i]
+            r['M'] = M[i]
 
     def to_dict(self, bboxes, kps, states):
         return [{'box': bboxes[i], 'kps': kps[i], 'scores': states[i]} for i in range(len(bboxes))]

@@ -7,6 +7,7 @@ device (csrc/mpipe.cu, csrc/temporal.cu) and two batches can be in flight so tha
 
     fa = FaceAnaStreams(n_streams=16, top_k=4)
     results = fa.run(frames)            # list of S lists of {'box','kps','scores'} - what S FaceAna.run calls return
+    # FaceAnaStreams(..., align=112): each dict also has 'chip' (112x112x3 uint8, aligned) and 'M' (2x3 float64)
     # or, overlapped:
     fa.submit(frames_t0); fa.submit(frames_t1); r0 = fa.collect(); fa.submit(frames_t2); r1 = fa.collect(); ...
 """
@@ -17,12 +18,16 @@ import pathlib
 import numpy as np
 
 from ... import runtime as rt
+from .align import check_size
 from .facer import get_cfg
 from .onnx_model_base import ONNXEngine
 
 
 class FaceAnaStreams:
-    def __init__(self, n_streams, top_k=None, max_frame_hw=(2160, 3840), device="cuda"):
+    def __init__(self, n_streams, top_k=None, max_frame_hw=(2160, 3840), device="cuda", align=None):
+        """align: None, or a chip side in 16..512: every result dict then also carries 'chip' and 'M' as FaceAna(align=...)
+        returns them, warped inside the same submit on the device from the smoothed landmarks and the frame in the ring."""
+        self.align = None if align is None else check_size(align)
         cfg = get_cfg()['Skps']
         det_cfg, kps_cfg, tr_cfg = cfg['Detect'], cfg['Keypoints'], cfg['Trace']
         self.n_streams = int(n_streams)
@@ -44,6 +49,11 @@ class FaceAnaStreams:
         S, K, P = self.n_streams, self.top_k, self.n_points
         self._out = [dict(n=np.zeros(S, np.int32), box=np.zeros((S, K, 4), np.float64), kps=np.zeros((S, K, P, 2), np.float64),
                           sc=np.zeros((S, K, P), np.float32), det=np.zeros(S, np.int32)) for _ in range(2)]
+        if self.align is not None:
+            rt.check(self.lib.skps_mpipe_set_align(h, self.align))
+            for o in self._out:
+                o["chips"] = np.zeros((S, K, self.align, self.align, 3), np.uint8)
+                o["M"] = np.zeros((S, K, 2, 3), np.float64)
         self._pending = []              # [(slot, n, keep-alive frames)]
         self._next = 0
         self.last_ran_detector = None
@@ -90,11 +100,17 @@ class FaceAnaStreams:
         rt.check(self.lib.skps_mpipe_wait(self._h, slot, o["n"].ctypes.data, o["box"].ctypes.data, o["kps"].ctypes.data,
                                           o["sc"].ctypes.data, o["det"].ctypes.data))
         self.last_ran_detector = o["det"][:n].astype(bool)
+        if self.align is not None:
+            rt.check(self.lib.skps_mpipe_align_results(self._h, slot, o["chips"].ctypes.data, o["M"].ctypes.data))
         res = []
         for s in range(n):
             k = int(o["n"][s])
             res.append([{'box': o["box"][s, i].copy(), 'kps': o["kps"][s, i].copy(), 'scores': o["sc"][s, i].copy()}
                         for i in range(k)])
+            if self.align is not None:
+                for i, r in enumerate(res[-1]):
+                    r['chip'] = o["chips"][s, i].copy()
+                    r['M'] = o["M"][s, i].copy()
         return res
 
     def run(self, frames):

@@ -39,10 +39,15 @@ struct skps_mpipe {
         MpStreamDesc* h_desc = nullptr;       // pinned: per-stream frame pointers + letterbox geometry of this batch
         int32_t* h_count = nullptr; int32_t* h_flag = nullptr; int32_t* h_det_count = nullptr;
         double* h_box = nullptr; double* h_kps = nullptr; float* h_scores = nullptr;
+        uint8_t* h_chips = nullptr; double* h_M = nullptr;     // pinned, only while alignment is on
         cudaEvent_t ev_in = nullptr, ev_done = nullptr;
         int n = 0;
+        int align = 0;                        // chip size this slot's batch was submitted with (0 = none)
         bool busy = false;
     } slot[2];
+    // aligned chips (skps_mpipe_set_align): [S][K][size][size][3] / [S][K][2][3], allocated only while align_size > 0
+    int align_size = 0;
+    uint8_t* d_chips = nullptr; double* d_align_M = nullptr;
     // device scratch (one set: batches are serialised on s_compute)
     int32_t *d_hw = nullptr, *d_have_prev = nullptr, *d_flag = nullptr, *d_det_count = nullptr, *d_det_idx = nullptr;
     int32_t *d_count = nullptr, *d_detail = nullptr;
@@ -72,14 +77,14 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
     for (uint8_t* f : p->d_frame) if (f) cudaFree(f);
     for (auto& sl : p->slot) {
         void* host[] = {sl.h_desc, sl.h_stage, sl.h_hw, sl.h_have_prev, sl.h_geom, sl.h_count, sl.h_flag, sl.h_det_count, sl.h_box,
-                        sl.h_kps, sl.h_scores};
+                        sl.h_kps, sl.h_scores, sl.h_chips, sl.h_M};
         for (void* q : host) if (q) cudaFreeHost(q);
         if (sl.ev_in) cudaEventDestroy(sl.ev_in);
         if (sl.ev_done) cudaEventDestroy(sl.ev_done);
     }
     void* dev[] = {p->d_desc, p->d_hw, p->d_have_prev, p->d_flag, p->d_det_count, p->d_det_idx, p->d_count, p->d_detail, p->d_diff,
                    p->d_det_rows, p->d_boxes, p->d_kps_now, p->d_prev_lm, p->d_prev_dx, p->d_track, p->d_out_kps,
-                   p->d_track_f32, p->d_n_prev, p->d_prev_f32, p->d_state_idx, p->d_n_track};
+                   p->d_track_f32, p->d_n_prev, p->d_prev_f32, p->d_state_idx, p->d_n_track, p->d_chips, p->d_align_M};
     for (void* q : dev) if (q) cudaFree(q);
     if (p->s_copy) cudaStreamDestroy(p->s_copy);
     if (p->s_compute) cudaStreamDestroy(p->s_compute);
@@ -251,6 +256,14 @@ extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8
     { const double r = a.two_pi * 1.0 * 1.0; a.a_d = r / (r + 1); a.one_minus_a_d = 1 - a.a_d; }
     a.min_cutoff = 0.15; a.beta = 0.8;
     if (launch_mp_temporal(a, n, sx)) return 1;
+    sl.align = p->align_size;
+    if (sl.align) {
+        // chips from the smoothed landmarks, on the frames still in the ring
+        const size_t chip_bytes = (size_t)sl.align * sl.align * 3;
+        if (launch_mp_align(p->d_desc, p->d_out_kps, p->d_count, K, P, sl.align, p->d_chips, p->d_align_M, n, sx)) return 1;
+        SKPS_CUDA(cudaMemcpyAsync(sl.h_chips, p->d_chips, chip_bytes * K * n, cudaMemcpyDeviceToHost, sx));
+        SKPS_CUDA(cudaMemcpyAsync(sl.h_M, p->d_align_M, 8 * 6 * (size_t)K * n, cudaMemcpyDeviceToHost, sx));
+    }
     SKPS_CUDA(cudaMemcpyAsync(sl.h_count, p->d_count, 4 * n, cudaMemcpyDeviceToHost, sx));
     SKPS_CUDA(cudaMemcpyAsync(sl.h_flag, p->d_flag, 4 * n, cudaMemcpyDeviceToHost, sx));
     SKPS_CUDA(cudaMemcpyAsync(sl.h_det_count, p->d_det_count, 4 * n, cudaMemcpyDeviceToHost, sx));
@@ -287,6 +300,53 @@ extern "C" SKPS_API int skps_mpipe_wait(skps_mpipe* p, int slot_i, int32_t* n_fa
     memcpy(boxes, sl.h_box, sizeof(double) * 4 * K * n);
     memcpy(kps, sl.h_kps, sizeof(double) * 2 * P * K * n);
     memcpy(scores, sl.h_scores, sizeof(float) * P * K * n);
+    return 0;
+}
+
+static void free_align(skps_mpipe* p) {
+    if (p->d_chips) cudaFree(p->d_chips);
+    if (p->d_align_M) cudaFree(p->d_align_M);
+    p->d_chips = nullptr; p->d_align_M = nullptr;
+    for (auto& sl : p->slot) {
+        if (sl.h_chips) cudaFreeHost(sl.h_chips);
+        if (sl.h_M) cudaFreeHost(sl.h_M);
+        sl.h_chips = nullptr; sl.h_M = nullptr; sl.align = 0;
+    }
+    p->align_size = 0;
+}
+
+extern "C" SKPS_API int skps_mpipe_set_align(skps_mpipe* p, int size) {
+    SKPS_CHECK(p && (size == 0 || (size >= 16 && size <= 512)), "mpipe_set_align: size %d is neither 0 nor in 16..512", size);
+    SKPS_CHECK(!p->slot[0].busy && !p->slot[1].busy, "mpipe_set_align: a batch is in flight (call skps_mpipe_wait first)");
+    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_CUDA(cudaStreamSynchronize(p->s_compute));
+    if (size == p->align_size) return 0;
+    free_align(p);
+    if (size == 0) return 0;
+    const size_t faces = (size_t)p->S * p->K, chip_bytes = (size_t)size * size * 3;
+    bool ok = cudaMalloc((void**)&p->d_chips, chip_bytes * faces) == cudaSuccess &&
+              cudaMalloc((void**)&p->d_align_M, 8 * 6 * faces) == cudaSuccess;
+    for (auto& sl : p->slot)
+        ok = ok && cudaMallocHost((void**)&sl.h_chips, chip_bytes * faces) == cudaSuccess &&
+             cudaMallocHost((void**)&sl.h_M, 8 * 6 * faces) == cudaSuccess;
+    if (!ok) {
+        cudaGetLastError();
+        free_align(p);
+        SKPS_CHECK(false, "mpipe_set_align: cannot allocate %zu chip bytes per buffer (%zu faces of %dx%d)", chip_bytes * faces,
+                   faces, size, size);
+    }
+    p->align_size = size;
+    return 0;
+}
+
+extern "C" SKPS_API int skps_mpipe_align_results(skps_mpipe* p, int slot_i, uint8_t* chips, double* M) {
+    SKPS_CHECK(p && (slot_i == 0 || slot_i == 1) && chips && M, "mpipe_align_results: bad arguments");
+    const skps_mpipe::Slot& sl = p->slot[slot_i];
+    SKPS_CHECK(!sl.busy, "mpipe_align_results: slot %d is in flight (call skps_mpipe_wait first)", slot_i);
+    SKPS_CHECK(sl.align > 0 && sl.n > 0, "mpipe_align_results: slot %d was not submitted with alignment on", slot_i);
+    const size_t faces = (size_t)sl.n * p->K;
+    memcpy(chips, sl.h_chips, faces * sl.align * sl.align * 3);
+    memcpy(M, sl.h_M, faces * 6 * sizeof(double));
     return 0;
 }
 

@@ -50,5 +50,9 @@ int launch_mp_select(const float* det_rows, const int* det_count, int max_det, c
                      int* count, int n_streams, cudaStream_t s);
 int launch_mp_decide(const unsigned long long* diff, const int* hw, const int* have_prev, int* flag, int n, cudaStream_t s);
 int launch_mp_temporal(const MpTemporalArgs& a, int n_streams, cudaStream_t s);
+// Aligned face chips (align.cu): per face of stream g < n with i < count[g], M = similarity of kps[g][i] (P x 2 float64) to the
+// ArcFace template at `size`, chips[g][i] = cv2.warpAffine(desc[g].cur, M, (size, size)); chips [n][K][size][size][3], M [n][K][2][3].
+int launch_mp_align(const MpStreamDesc* d, const double* kps, const int* count, int K, int P, int size, uint8_t* chips,
+                    double* M, int n, cudaStream_t s);
 
 }  // namespace skps

@@ -37,6 +37,9 @@ struct skps_pipeline {
     Host* h_res = nullptr;
     float* h_boxes = nullptr; float* h_kps = nullptr; float* h_scores = nullptr;
     int32_t* h_det_idx = nullptr; float* h_det_rows = nullptr; float* h_track = nullptr;
+    // aligned chips (skps_pipeline_align): allocated on first use, for top_k faces at align_size
+    int align_size = 0;
+    double* d_align_kps = nullptr; double* d_align_M = nullptr; uint8_t* d_chips = nullptr;
 };
 
 extern "C" SKPS_API void skps_pipeline_destroy(skps_pipeline* p) {
@@ -45,7 +48,7 @@ extern "C" SKPS_API void skps_pipeline_destroy(skps_pipeline* p) {
     for (int i = 0; i < 2; ++i) if (p->d_frame[i]) cudaFree(p->d_frame[i]);
     if (p->h_frame) cudaFreeHost(p->h_frame);
     void* dev[] = {p->d_det_rows, p->d_det_idx, p->d_det_count, p->d_track, p->d_boxes, p->d_count, p->d_detail,
-                   p->d_kps, p->d_diff};
+                   p->d_kps, p->d_diff, p->d_align_kps, p->d_align_M, p->d_chips};
     for (void* q : dev) if (q) cudaFree(q);
     void* host[] = {p->h_res, p->h_boxes, p->h_kps, p->h_scores, p->h_det_idx, p->h_det_rows, p->h_track};
     for (void* q : host) if (q) cudaFreeHost(q);
@@ -228,5 +231,37 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, const uint8_t* frame
     // the frame just processed becomes "previous" for the next frame_diff (facer.py:57,62)
     p->prev_h = H; p->prev_w = W;
     p->cur ^= 1;
+    return 0;
+}
+
+// Aligned chips from the frame of the last run / commit, which is d_frame[cur ^ 1] (prev_h x prev_w) until the next frame
+// is staged.  The landmarks were smoothed on the host (GroupTrack), so they come up; n x 98 x 2 doubles are tiny.
+extern "C" SKPS_API int skps_pipeline_align(skps_pipeline* p, const double* kps, int n, int size, uint8_t* chips, double* M,
+                                            void* stream) {
+    SKPS_CHECK(p && kps && chips && M, "pipeline_align: null argument");
+    SKPS_CHECK(n > 0 && n <= p->cfg.top_k, "pipeline_align: %d faces, expected 1..%d", n, p->cfg.top_k);
+    SKPS_CHECK(size >= 16 && size <= 512, "pipeline_align: size %d outside 16..512", size);
+    SKPS_CHECK(p->prev_h > 0 && p->prev_w > 0, "pipeline_align: no frame (run the pipeline first)");
+    cudaStream_t s = (cudaStream_t)stream;
+    SKPS_CUDA(cudaSetDevice(p->device));
+    const int K = p->cfg.top_k, P = p->n_points;
+    const size_t chip_bytes = (size_t)size * size * 3;
+    if (p->align_size != size) {
+        SKPS_CUDA(cudaStreamSynchronize(s));
+        void* old[] = {p->d_align_kps, p->d_align_M, p->d_chips};
+        for (void* q : old) if (q) cudaFree(q);
+        p->d_align_kps = p->d_align_M = nullptr; p->d_chips = nullptr; p->align_size = 0;
+        SKPS_CUDA(cudaMalloc((void**)&p->d_align_kps, sizeof(double) * 2 * P * K));
+        SKPS_CUDA(cudaMalloc((void**)&p->d_align_M, sizeof(double) * 6 * K));
+        SKPS_CUDA(cudaMalloc((void**)&p->d_chips, chip_bytes * K));
+        p->align_size = size;
+    }
+    const int H = p->prev_h, W = p->prev_w;
+    SKPS_CUDA(cudaMemcpyAsync(p->d_align_kps, kps, sizeof(double) * 2 * P * n, cudaMemcpyHostToDevice, s));
+    if (skps_align_faces(p->d_frame[p->cur ^ 1], H, W, W * 3, p->d_align_kps, nullptr, n, P, size, p->d_chips, p->d_align_M, s))
+        return 1;
+    SKPS_CUDA(cudaMemcpyAsync(chips, p->d_chips, chip_bytes * n, cudaMemcpyDeviceToHost, s));
+    SKPS_CUDA(cudaMemcpyAsync(M, p->d_align_M, sizeof(double) * 6 * n, cudaMemcpyDeviceToHost, s));
+    SKPS_CUDA(cudaStreamSynchronize(s));
     return 0;
 }

@@ -87,6 +87,12 @@ SIGNATURES = {
     "skps_mpipe_wait": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "skps_pipeline_commit_frame": (C.c_int, [c_vp, C.c_int, C.c_int]),
     "skps_pipeline_frame_diff": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double), c_vp]),
+    "skps_warp_affine": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
+    "skps_align_faces": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp,
+                                   c_vp]),
+    "skps_pipeline_align": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp]),
+    "skps_mpipe_set_align": (C.c_int, [c_vp, C.c_int]),
+    "skps_mpipe_align_results": (C.c_int, [c_vp, C.c_int, c_vp, c_vp]),
 }
 
 _lib = None

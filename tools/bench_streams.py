@@ -4,6 +4,12 @@ frame-difference gate re-runs the detector on every frame (the worst case for th
 host results out: every H2D / D2H is inside the timed region.
 
     python tools/bench_streams.py [--streams 16] [--batches 12] [--configs 1080p_4faces,4k_16faces] [--gather]
+    python tools/bench_streams.py --align 112 [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
+
+--align SIZE times every config with and without aligned face chips (FaceAnaStreams(align=SIZE)) in the same process,
+alternating the two over --rounds rounds, and reports the median ms_per_call of both.  At 4k_16faces it also times the
+alignment kernel alone with CUDA events (skps_align_faces on one 4K frame in HBM, the landmarks of every face of the last
+call) and reports the bytes it writes per second.  The GPU name and power limit are read in the same run.
 
 Under torchrun every rank drives its own S streams on its own GPU (streams shard across GPUs, no collective on the data
 path); time = max over ranks.  --gather adds one NCCL all_gather of the packed (box, landmarks, scores) rows per call."""
@@ -102,6 +108,108 @@ def run_config(name, n_streams=16, batches=12, warmup=3, gather=False, dist=None
             "gather_to_rank0": bool(rows is not None)}
 
 
+def gpu_info(torch):
+    """Name and power limit of the current GPU (read-only nvidia-smi query; None where it is not available)."""
+    import subprocess
+    idx = torch.cuda.current_device()
+    info = {"gpu": torch.cuda.get_device_name(idx), "power_limit_w": None, "max_sm_clock_mhz": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(idx), "--query-gpu=power.limit,clocks.max.sm",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30).stdout
+        pw, clk = [v.strip() for v in out.strip().splitlines()[0].split(",")]
+        info["power_limit_w"], info["max_sm_clock_mhz"] = float(pw), float(clk)
+    except Exception:
+        pass
+    return info
+
+
+HBM_PEAK_BPS = 3.35e12          # H100 SXM data sheet (HBM3)
+
+
+def time_align_kernel(torch, frame, kps, size, iters=200):
+    """CUDA-event time of one skps_align_faces launch (estimate + warp of len(kps) chips from one frame in HBM)."""
+    import ctypes as C
+    from peppa_pig_face_landmark_b200 import runtime as rt
+    lib = rt.load_library()
+    H, W = frame.shape[:2]
+    n = kps.shape[0]
+    d_frame = torch.from_numpy(np.ascontiguousarray(frame)).cuda()
+    d_kps = torch.from_numpy(np.ascontiguousarray(kps, dtype=np.float64)).cuda()
+    chips = torch.empty((n, size, size, 3), dtype=torch.uint8, device="cuda")
+    M = torch.empty((n, 2, 3), dtype=torch.float64, device="cuda")
+    stream = torch.cuda.current_stream()
+
+    def launch():
+        rt.check(lib.skps_align_faces(d_frame.data_ptr(), H, W, W * 3, d_kps.data_ptr(), None, n, kps.shape[1], size,
+                                      chips.data_ptr(), M.data_ptr(), C.c_void_p(stream.cuda_stream)))
+    for _ in range(20):
+        launch()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(iters):
+        launch()
+    e1.record()
+    torch.cuda.synchronize()
+    us = 1e3 * e0.elapsed_time(e1) / iters
+    written = n * size * size * 3
+    return {"chips": n, "size": size, "kernel_us": us, "bytes_written": written,
+            "written_GBps": written / (us * 1e-6) / 1e9, "written_share_of_hbm_peak": written / (us * 1e-6) / HBM_PEAK_BPS,
+            "timing": "CUDA events around %d back-to-back launches" % iters}
+
+
+def run_align_pair(name, size, n_streams=16, batches=12, warmup=3, rounds=5, length=6):
+    """The same config with and without alignment, alternating; median ms_per_call of each."""
+    import torch
+    import frames
+    from Skps import FaceAnaStreams
+    maker, topk = getattr(frames, CONFIGS[name][0]), CONFIGS[name][1]
+    seqs = make_streams(torch, frames, maker, n_streams, length=length)
+    H, W = seqs[0][0].shape[:2]
+    fas = {"off": FaceAnaStreams(n_streams=n_streams, top_k=topk, max_frame_hw=(H, W)),
+           "on": FaceAnaStreams(n_streams=n_streams, top_k=topk, max_frame_hw=(H, W), align=size)}
+    L = len(seqs[0])
+
+    def batch(t):
+        return [seqs[s][t % L] for s in range(n_streams)]
+    for fa in fas.values():
+        for t in range(warmup):
+            fa.run(batch(t))
+    times = {"off": [], "on": []}
+    faces, last = {}, None
+    for r in range(rounds):
+        for key in (("off", "on") if r % 2 == 0 else ("on", "off")):
+            fa = fas[key]
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            nf = 0
+            fa.submit(batch(0))
+            for t in range(1, batches):
+                fa.submit(batch(t))
+                nf += sum(len(x) for x in fa.collect())
+            res = fa.collect()
+            nf += sum(len(x) for x in res)
+            torch.cuda.synchronize()
+            times[key].append(time.perf_counter() - t0)
+            faces[key] = nf
+            if key == "on":
+                last = res
+    per_face = 32 + 98 * 2 * 8 + 98 * 4
+    out = {"config": name, "streams_per_gpu": n_streams, "calls": batches, "rounds": rounds, "align_size": size,
+           "ms_per_call": 1e3 * float(np.median(times["off"])) / batches,
+           "ms_per_call_align": 1e3 * float(np.median(times["on"])) / batches,
+           "ms_per_call_rounds": [1e3 * v / batches for v in times["off"]],
+           "ms_per_call_align_rounds": [1e3 * v / batches for v in times["on"]],
+           "faces_per_frame": faces["on"] / (n_streams * batches),
+           "d2h_bytes_per_frame": int(topk * per_face),
+           "d2h_bytes_per_frame_align": int(topk * (per_face + size * size * 3 + 6 * 8)),
+           "api": "FaceAnaStreams.submit/collect, pinned host frames, 2 calls in flight; align: chips warped in submit"}
+    del fas
+    if name == "4k_16faces":
+        kps = np.stack([f["kps"] for faces_s in last for f in faces_s])
+        out["align_kernel"] = time_align_kernel(torch, batch(batches - 1)[0], kps, size)
+    return out
+
+
 def main():
     import torch
     a = sys.argv[1:]
@@ -116,6 +224,13 @@ def main():
     if world > 1:
         import torch.distributed as dist
         dist.init_process_group("nccl", device_id=torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0"))))
+    if "--align" in a:
+        size, rounds = int(opt("--align", 112)), int(opt("--rounds", 5))
+        print(json.dumps(gpu_info(torch)))
+        for name in names:
+            print(json.dumps(run_align_pair(name, size, n_streams, batches, rounds=rounds)))
+            sys.stdout.flush()
+        return
     for name in names:
         r = run_config(name, n_streams, batches, gather="--gather" in a, dist=dist, rank=rank, world=world)
         if r is not None:
