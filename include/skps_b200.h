@@ -89,7 +89,7 @@ SKPS_API int skps_engine_buffer_dims(const skps_engine* e, int buf, int* h, int*
 SKPS_API int skps_engine_read_buffer(skps_engine* e, int buf, int batch, void* dst_host);
 /* Number of kernels one forward launches (for bench.py's gpu_launches). */
 SKPS_API int skps_engine_launches_per_forward(const skps_engine* e);
-/* Kernel launches of one forward at `batch` (segments sweep the batch in L2-sized chunks). */
+/* Kernel launches of one forward at `batch` (0 for batch <= 0). */
 SKPS_API int skps_engine_launches_for_batch(const skps_engine* e, int batch);
 /* Profiling: enqueue only op `op_index` of the plan on the buffers left by the last forward
  * (bench.py times the dominant kernel with CUDA events around this call). */

@@ -33,7 +33,7 @@ def split16_round(x, lo_scale=1.0):
 class PlanInterp:
     def __init__(self, plan, emulate_split=False, lo_scale=1.0):
         self.plan = plan
-        self.emulate_split = emulate_split      # tensor-core convs: operands rounded to the fp16 hi/lo format, fp64 accumulate
+        self.emulate_split = emulate_split      # tensor-core convs and OP_DWPW: operands rounded to fp16 hi/lo, fp64 accumulate
         self.lo_scale = lo_scale
 
     def run(self, x_nhwc, dump=None):
@@ -52,9 +52,13 @@ class PlanInterp:
         def wr(v, val):
             bufs[v.buf.idx][..., v.c_off: v.c_off + v.C * v.c_stride: v.c_stride] = val
 
-        ops = []
+        ops, fp32_dwpw = [], set()
         for op in pl.ops:                       # a fused stem block is executed as the layers it replaces
-            ops += op.sub_ops if op.type == P.OP_STEM_BLOCK else [op]
+            if op.type == P.OP_STEM_BLOCK:
+                ops += op.sub_ops
+                fp32_dwpw.add(id(op.sub_ops[1]))      # csrc/stem_block.cu runs its depthwise + 1x1 on the FP32 pipes
+            else:
+                ops.append(op)
         for op in ops:
             t = op.type
             if t == P.OP_CONV:
@@ -125,7 +129,14 @@ class PlanInterp:
                 wd = torch.from_numpy(op.dw_w).T.reshape(C, 1, 3, 3).contiguous()
                 y = _act(F.conv2d(x, wd, torch.from_numpy(op.dw_b), padding=1, groups=C), op.dw_act)
                 w = torch.from_numpy(op.w_ref).permute(0, 3, 1, 2).contiguous()
-                y = F.conv2d(y, w, torch.from_numpy(op.b) if op.b is not None else None).permute(0, 2, 3, 1)
+                bias = torch.from_numpy(op.b) if op.b is not None else None
+                if self.emulate_split and id(op) not in fp32_dwpw:     # the depthwise output enters the MMA as fp16 hi/lo
+                    sc = np.float32(1.0 / op.floats[0])
+                    y = F.conv2d(split16_round(y, self.lo_scale).double(), (split16_round(w * sc) / sc).double(),
+                                 bias.double() if bias is not None else None).float()
+                else:
+                    y = F.conv2d(y, w, bias)
+                y = y.permute(0, 2, 3, 1)
                 if op.ins[1] is not None and (op.flags & P.FLAG_RES_FIRST):
                     y = _act(y + rd(op.ins[1]), op.act)
                 else:

@@ -5,7 +5,6 @@ Here the graph is lowered to a fused plan and executed by hand-written sm_90a ke
 the C-ABI in include/skps_b200.h; PyTorch/numpy objects are only containers for memory.
 """
 import ctypes as C
-import os
 
 import numpy as np
 
@@ -15,7 +14,7 @@ from ...onnx_loader import load_onnx
 
 
 class ONNXEngine:
-    def __init__(self, onnx_f, device="cuda", max_batch=1, use_tc=None):
+    def __init__(self, onnx_f, device="cuda", max_batch=1, use_tc=True):
         if "cuda" not in str(device):
             raise RuntimeError("ONNXEngine: this build executes on a CUDA device only (got device=%r)" % (device,))
         torch = rt.require_cuda()
@@ -26,8 +25,6 @@ class ONNXEngine:
         if len(shp) != 4 or shp[1] != 3 or min(shp[2:]) <= 0:
             raise ValueError("ONNXEngine: unsupported input shape %s in %s" % (shp, onnx_f))
         self.in_hw = (int(shp[2]), int(shp[3]))
-        if use_tc is None:
-            use_tc = os.environ.get("SKPS_TC", "1") != "0"
         self.plan = lowering.lower(onnx_f, self.in_hw, name=str(onnx_f), use_tc=use_tc)
         words, blob = self.plan.serialize()
         self._words, self._blob = words, blob

@@ -182,22 +182,6 @@ conv_hm_kernel(const __grid_constant__ CUtensorMap tmX_hi, const __grid_constant
 }
 
 // ------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn hm_encode() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    }
-    return fn;
-}
-
 bool hm_shape_ok(int H, int W, int Cin, int Cout, int in_ld, int in_coff) {
     if (W < 8 || W > HM_N || HM_N % W || (H * W) % HM_N) return false;      // whole 256-pixel row blocks
     if (Cin % 8 || Cin > 128 || Cout > HM_M || (in_ld % 8) || (in_coff % 8)) return false;
@@ -205,7 +189,7 @@ bool hm_shape_ok(int H, int W, int Cin, int Cout, int in_ld, int in_coff) {
 }
 
 int hm_prepare(HmLayer& L, const TcSetup& s) {
-    EncodeTiledFn enc = hm_encode();
+    EncodeTiledFn enc = tensor_map_encoder();
     SKPS_CHECK(enc, "cuTensorMapEncodeTiled entry point not available");
     SKPS_CHECK(s.kh == 1 && s.kw == 1 && (s.stride <= 1) && s.act == ACT_NONE && !s.res && s.hm_val && s.hm_idx,
                "conv_hm: 1x1, linear, partial-maximum output only");
@@ -247,7 +231,7 @@ int hm_prepare(HmLayer& L, const TcSetup& s) {
     return 0;
 }
 
-int hm_launch(const HmLayer& L, int batch, int img0, int num_sms, cudaStream_t stream) {
+int hm_launch(const HmLayer& L, int batch, int num_sms, cudaStream_t stream) {
     static int attr_bytes = 0;
     if (L.smem_bytes > attr_bytes) {
         SKPS_CUDA(cudaFuncSetAttribute(conv_hm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
@@ -255,7 +239,6 @@ int hm_launch(const HmLayer& L, int batch, int img0, int num_sms, cudaStream_t s
     }
     HmK k = L.k;
     k.m_tiles = batch * k.tiles_per_img;
-    k.img0 = img0;
     const int grid = k.m_tiles < num_sms ? k.m_tiles : num_sms;
     conv_hm_kernel<<<grid, HM_THREADS, L.smem_bytes, stream>>>(L.x_hi, L.x_lo, L.w_hi, L.w_lo, k);
     SKPS_CUDA(cudaGetLastError());
@@ -313,7 +296,7 @@ extern "C" SKPS_API int skps_debug_conv_hm(const float* x, int N, int H, int W, 
     HmLayer L;
     int rc = hm_prepare(L, s);
     const int sms = sm_count();
-    if (!rc) rc = hm_launch(L, N, 0, sms, 0);
+    if (!rc) rc = hm_launch(L, N, sms, 0);
     if (!rc && cudaDeviceSynchronize() != cudaSuccess) { set_error("debug_conv_hm: kernel failed"); rc = 1; }
     if (!rc) {
         cudaMemcpy(val, d_val, (size_t)N * tiles * ld * 4, cudaMemcpyDeviceToHost);

@@ -235,28 +235,13 @@ conv_mma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant
 }
 
 // ------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn mma_get_encode() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    }
-    return fn;
-}
-
 bool conv_mma_supported(int cin, int cout, int kh, int kw, int stride, int dil, int pad) {
     return kh == 3 && kw == 3 && stride == 1 && dil == 1 && pad == 1 && cin == cout && (cin == 24 || cin == 40);
 }
 
 int conv_mma_prepare(ConvMmaLayer& L, const TView& in, const TView& out, const TView& res, int res_first, const void* w_packed,
                      const float* bias, float out_scale, int act, int max_batch) {
-    EncodeTiledFn enc = mma_get_encode();
+    EncodeTiledFn enc = tensor_map_encoder();
     SKPS_CHECK(enc, "cuTensorMapEncodeTiled entry point not available");
     SKPS_CHECK(conv_mma_supported(in.C, out.C, 3, 3, 1, 1, 1), "conv_mma: unsupported channels %d -> %d", in.C, out.C);
     SKPS_CHECK(in.fmt == DT_SPLIT16 && in.c_stride == 1 && ((in.ld | in.c_off) & 7) == 0, "conv_mma: input view");
@@ -309,9 +294,9 @@ static int mma_launch_t(const ConvMmaLayer& L, const ConvMmaK& k, cudaStream_t s
     return 0;
 }
 
-int conv_mma_launch(const ConvMmaLayer& L, int batch, int img0, cudaStream_t stream) {
+int conv_mma_launch(const ConvMmaLayer& L, int batch, cudaStream_t stream) {
     ConvMmaK k = L.k;
-    k.batch = batch; k.img0 = img0;
+    k.batch = batch;
     if (L.cin == 24) return mma_launch_t<24, 24>(L, k, stream);
     if (L.cin == 40) return mma_launch_t<40, 40>(L, k, stream);
     set_error("conv_mma: %d channels not instantiated", L.cin);
@@ -365,7 +350,7 @@ extern "C" SKPS_API int skps_debug_conv_mma(const float* x, int N, int H, int W,
     if (d_res) { r = in; r.base = d_res; r.fmt = DT_F32; r.plane = 0; }
     ConvMmaLayer L;
     if (conv_mma_prepare(L, in, o, r, res_first, d_w, d_bias, out_scale, act, N)) return 1;
-    if (conv_mma_launch(L, N, 0, 0)) return 1;
+    if (conv_mma_launch(L, N, 0)) return 1;
     SKPS_CUDA(cudaDeviceSynchronize());
     if (out_split) {
         __half* tmp = (__half*)malloc(n * 4);

@@ -28,6 +28,6 @@ struct ConvMmaLayer {
 bool conv_mma_supported(int cin, int cout, int kh, int kw, int stride, int dil, int pad);
 int conv_mma_prepare(ConvMmaLayer& L, const TView& in, const TView& out, const TView& res, int res_first, const void* w_packed,
                      const float* bias, float out_scale, int act, int max_batch);
-int conv_mma_launch(const ConvMmaLayer& L, int batch, int img0, cudaStream_t stream);
+int conv_mma_launch(const ConvMmaLayer& L, int batch, cudaStream_t stream);
 
 }  // namespace skps

@@ -16,15 +16,6 @@
 //   32-column chunks of the tile (the chunks alternate between them) and run the epilogue on them
 //   (registers -> bias/act/residual -> global).  Persistent CTAs, one per SM; the producer fills the next
 //   stages while the epilogue of a tile runs.
-//
-// Halo-row mode (k3) for 3x3 / stride 1 / dilation 1 convs on 64-wide maps (the decoder's conv2, 40 % of the student's MACs):
-// the per-tap pipeline above fetches every activation row once per tap - 9 x 64 KB of A tiles per 256 pixels, and the kernel
-// was L2->SM bound (lts 71-79 % of its cap, tensor pipe 53 %).  In k3 mode a pipeline stage is (kx, 32-channel half-chunk):
-// ONE 6-row x 64-pixel box (rows y0-1 .. y0+4, shifted by kx-1 in x; padding = TMA OOB fill) serves the three ky taps of a
-// 4-row x 64-pixel output group: tap ky of pixel tile u is the 128 rows that start (2u + ky) image rows into the box, i.e. a
-// shared-memory descriptor offset of (2u + ky) x 4 KB - the taps are addressed in place, nothing is copied.  64-byte rows
-// (SWIZZLE_64B) keep two 96 KB stages (A 48 KB + the three ky weight tiles 48 KB) inside shared memory.  L2->SM bytes per
-// 256 pixels: 1728 KB -> 1152 KB.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <stdlib.h>
@@ -45,8 +36,6 @@ constexpr int TC_THREADS = 384;        // warp 0: TMA; warps 4-11: MMA + epilogu
 constexpr int TC_XS_BYTES = 2 * 16384; // accumulator hand-off buffers of the two MMA warpgroups (wg_rows32)
 constexpr int TC_MAX_OWN = 4;          // 32-column chunks a warpgroup accumulates per tile (mt * n_tile <= 256)
 constexpr int MAX_STAGES = 4;
-constexpr int K3_ROWS = 6;                          // input rows per halo box: 4 output rows + 2
-constexpr int K3_A_PLANE = K3_ROWS * 64 * 64;       // 6 rows x 64 pixels x 64 B (32 fp16 channels) = 24 KB per plane
 
 // One level of a warp reduce-scatter of per-column (max, first arg-max): 2N column candidates per lane in, N out; after the
 // levels 16, 8, 4, 2, 1 lane L holds column L reduced over the warp's 32 rows.  Ties keep the smaller pixel index.
@@ -81,11 +70,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     const uint32_t n_pad = (uint32_t)((p.n_tile + 31) & ~31);
     const uint32_t b_tile_bytes = n_pad * TC_BK * 2;
     // stage = [A0_hi][A0_lo]([A1_hi][A1_lo])[B_hi][B_lo]: with mt = 2 two pixel tiles share one weight tile
-    // k3: stage = [A hi 24 KB][A lo 24 KB][ky = 0,1,2: B hi, B lo of n_tile x 64 B each]
-    const uint32_t b3_bytes = n_pad * 64u;
-    const uint32_t a_bytes = p.k3 ? 2u * K3_A_PLANE : (uint32_t)p.mt * 2u * A_TILE_BYTES;
-    const uint32_t stage_bytes = p.k3 ? a_bytes + 6u * b3_bytes : a_bytes + 2u * b_tile_bytes;
-    const uint32_t tx_bytes = p.k3 ? a_bytes + 6u * (uint32_t)p.n_tile * 64u : a_bytes + 4u * (uint32_t)p.n_tile * TC_BK;
+    const uint32_t a_bytes = (uint32_t)p.mt * 2u * A_TILE_BYTES;
+    const uint32_t stage_bytes = a_bytes + 2u * b_tile_bytes;
+    const uint32_t tx_bytes = a_bytes + 4u * (uint32_t)p.n_tile * TC_BK;
 
     if (warp == 0 && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA_hi) : "memory");
@@ -114,27 +101,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             int stage = 0;
             uint32_t phase = 0;
             const int tiles_x = (p.W + p.bw - 1) / p.bw;       // ragged maps: edge tiles hang over, TMA zero-fills / clips
-            if (p.k3) {
-                const int halves = p.Cin >> 5, gpi = p.tiles_per_img >> 1, K_row = p.cchunks * TC_BK;
-                for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                    const int img_l = tile / gpi, y0 = (tile - img_l * gpi) * 4;
-                    for (int kb = 0; kb < 3 * halves; ++kb) {
-                        const int kx = kb / halves, h = kb - kx * halves;
-                        mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1u);
-                        const uint32_t fb = smem_u32(&full_bar[stage]);
-                        mbar_expect_tx(fb, tx_bytes);
-                        const uint32_t sa = tile_base + (uint32_t)stage * stage_bytes;
-                        tma_load_4d(sa, &tmA_hi, fb, h * 32, kx - 1, y0 - 1, img_l + p.img0);
-                        tma_load_4d(sa + K3_A_PLANE, &tmA_lo, fb, h * 32, kx - 1, y0 - 1, img_l + p.img0);
-                        for (int ky = 0; ky < 3; ++ky) {
-                            const int kcol = (ky * 3 + kx) * K_row + h * 32;
-                            tma_load_2d(sa + a_bytes + (uint32_t)(2 * ky) * b3_bytes, &tmB_hi, fb, kcol, 0);
-                            tma_load_2d(sa + a_bytes + (uint32_t)(2 * ky + 1) * b3_bytes, &tmB_lo, fb, kcol, 0);
-                        }
-                        if (++stage == p.stages) { stage = 0; phase ^= 1u; }
-                    }
-                }
-            } else
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const int g_idx = tile / p.n_tiles, n_idx = tile - g_idx * p.n_tiles;
                 int img[2], y0[2], x0[2];
@@ -186,35 +152,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             for (int g = 0; g < p.mt * n_chunks_t && n_own < TC_MAX_OWN; ++g)
                 if (((chunk_ctr + g) & 1) == half_id) { own_u[n_own] = g / n_chunks_t; own_c[n_own] = g % n_chunks_t; ++n_own; }
             float accv[TC_MAX_OWN][32];
-            if (p.k3) {
-                const int nkb = 3 * (p.Cin >> 5);
-                for (int kb = 0; kb < nkb; ++kb) {
-                    mbar_wait(smem_u32(&full_bar[stage]), phase);
-                    const uint32_t sa = tile_base + (uint32_t)stage * stage_bytes;
-                    wg_fence();
-                    for (int ky = 0; ky < 3; ++ky) {
-                        const uint64_t b_hi = make_smem_desc_sw64(sa + a_bytes + (uint32_t)(2 * ky) * b3_bytes);
-                        const uint64_t b_lo = make_smem_desc_sw64(sa + a_bytes + (uint32_t)(2 * ky + 1) * b3_bytes);
-#pragma unroll
-                        for (int o = 0; o < TC_MAX_OWN; ++o) {
-                            if (o >= n_own) break;
-                            // pixel tile u, tap row ky: 128 box rows starting (2u + ky) image rows in = (2u + ky) * 4 KB
-                            const uint32_t ao = sa + (uint32_t)(2 * own_u[o] + ky) * 4096u;
-                            const uint64_t a_hi = make_smem_desc_sw64(ao), a_lo = make_smem_desc_sw64(ao + K3_A_PLANE);
-                            const uint64_t bo = (uint64_t)(own_c[o] * 32 * 64 >> 4);
-                            for (int k = 0; k < 2; ++k) {
-                                const uint64_t koff = (uint64_t)(k * 2);             // 16 fp16 = 32 bytes along K
-                                wg_mma3_128x32(accv[o], a_hi + koff, a_lo + koff, 64u * 64u, b_hi + bo + koff, b_lo + bo + koff,
-                                               (kb | ky | k) != 0);
-                            }
-                        }
-                    }
-                    wg_commit();
-                    wg_wait0();
-                    if (lane == 0) mbar_arrive(smem_u32(&empty_bar[stage]));
-                    if (++stage == p.stages) { stage = 0; phase ^= 1u; }
-                }
-            } else
             for (int kb = 0; kb < kblocks; ++kb) {
                 mbar_wait(smem_u32(&full_bar[stage]), phase);
                 const uint32_t sa = tile_base + (uint32_t)stage * stage_bytes;
@@ -463,22 +400,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
 }
 
 // ------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    }
-    return fn;
-}
-
 static const float* zero_bias() {
     static float* z = nullptr;       // 1024 zeros for bias-free layers (ASPP), per process/device
     if (!z) {
@@ -492,16 +413,10 @@ static const float* zero_bias() {
 // Maps whose width divides (or is a multiple of) 128 use row-block tiles (bw = min(W, 128)) that cover the map exactly.
 // Any other map (the detector's 48x80 / 24x40 / 12x20, re-targeted @192/@320 exports) gets the bw in {64,32,16,8} with the
 // fewest tiles, edge tiles hanging over the right/bottom border: the TMA loads zero-fill and the TMA stores clip what
-// lies outside, the direct-store path masks it.  SKPS_TC_ANY_W=0 restores the exact-cover-only rule.
+// lies outside, the direct-store path masks it.
 static int tc_pick_bw(int H, int W) {
-    static int any_w = -1;
-    if (any_w < 0) {
-        const char* e = getenv("SKPS_TC_ANY_W");
-        any_w = (e && e[0] == '0') ? 0 : 1;
-    }
     if (W >= TC_BM && W % TC_BM == 0) return TC_BM;
     if (W < TC_BM && TC_BM % W == 0 && H % (TC_BM / W) == 0) return W;
-    if (!any_w) return 0;
     int best = 0, best_tiles = 1 << 30;
     for (int bw = 64; bw >= 8; bw >>= 1) {
         const int bh = TC_BM / bw;
@@ -521,7 +436,7 @@ bool tc_shape_ok(int H, int W, int Cin, int in_ld, int in_coff) {
 }
 
 int tc_prepare(TcLayer& L, const TcSetup& s) {
-    EncodeTiledFn enc = get_encode();
+    EncodeTiledFn enc = tensor_map_encoder();
     SKPS_CHECK(enc, "cuTensorMapEncodeTiled entry point not available");
     const int stride = s.stride > 0 ? s.stride : 1;
     SKPS_CHECK((stride == 1 || stride == 2) && s.H % stride == 0 && s.W % stride == 0, "conv_tc: stride %d on %dx%d", stride,
@@ -544,34 +459,21 @@ int tc_prepare(TcLayer& L, const TcSetup& s) {
     SKPS_CHECK(s.n_tile >= 8 && s.n_tile <= 256 && s.n_tile % 8 == 0, "conv_tc: n_tile %d", s.n_tile);
     // two pixel tiles per weight-tile load when both accumulators fit the registers of the MMA warpgroups (N <= 128)
     // and two pipeline stages still fit in shared memory (checked below): halves the weight traffic from L2
-    k.mt = (s.n_tile <= 128 && s.mt_hint != 1) ? 2 : 1;
+    k.mt = s.n_tile <= 128 ? 2 : 1;
     const size_t n_pad = (size_t)((s.n_tile + 31) & ~31);
-    {
-        // halo-row mode (see the file header): 3x3 / stride 1 / dilation 1 on 64-wide maps, whole 4-row groups, one N tile
-        // Off by default (opt-in): it moves 33 % fewer bytes from L2 (1 152 vs 1 728 KB per 256
-        // pixels), but both operands of every MMA come from shared memory either way.  SKPS_TC_K3=1 enables it
-        // (tests/test_conv_tc_gpu.py does).
-        const char* e = getenv("SKPS_TC_K3");
-        const int k3_on = (e && e[0] == '1') ? 1 : 0;
-        k.k3 = (k3_on && s.kh == 3 && stride == 1 && s.dil == 1 && Wo == 64 && k.bw == 64 && Ho % 4 == 0 && s.Cin % 32 == 0 &&
-                s.n_tiles == 1 && k.mt == 2 && k.ipt == 1 && !s.hm_val) ? 1 : 0;
-        // only where two of its stages fit next to the hand-off and store buffers
-        const size_t k3_stage = (size_t)2 * K3_A_PLANE + 6 * n_pad * 64;
-        if (k.k3 && (227 * 1024 - 2048 - TC_XS_BYTES - 2 * 16384) / k3_stage < 2) k.k3 = 0;
-    }
     auto stage_size = [&]() {
-        return k.k3 ? (size_t)2 * K3_A_PLANE + 6 * n_pad * 64 : (size_t)k.mt * 2 * (size_t)A_TILE_BYTES + 2 * n_pad * TC_BK * 2;
+        return (size_t)k.mt * 2 * (size_t)A_TILE_BYTES + 2 * n_pad * TC_BK * 2;
     };
     size_t stage_bytes = stage_size();
     // TMA-store epilogue: full 128-byte lines instead of 16-byte pieces per thread.  Needs a unit-stride,
     // 16-byte aligned destination whose channel count is a multiple of 8 (the swizzle-free box clips at Cout).
     const int oes = s.out_fmt == DT_SPLIT16 ? 2 : 4;
     k.tma_store = (s.out_cstride == 1 && (s.Cout % 8) == 0 && ((size_t)s.out_ld * oes) % 16 == 0 &&
-                   ((size_t)s.out_coff * oes) % 16 == 0 && s.tma_store_hint != 1 && !s.hm_val) ? 1 : 0;
+                   ((size_t)s.out_coff * oes) % 16 == 0 && !s.hm_val) ? 1 : 0;
     // two staging buffers per epilogue warp group when the pipeline still gets its stages, else one
     const size_t budget = 227 * 1024 - 1024 - 1024 - TC_XS_BYTES;  // minus static smem slack, alignment pad, hand-off
     const size_t out_min = (k.tma_store || s.out_cstride != 1) ? (size_t)2 * 16384 : 0;
-    if (k.mt == 2 && !k.k3 && (budget - out_min) / stage_bytes < 2) {
+    if (k.mt == 2 && (budget - out_min) / stage_bytes < 2) {
         k.mt = 1;                                                    // two stages matter more than the shared weight tile
         stage_bytes = stage_size();
     }
@@ -580,7 +482,7 @@ int tc_prepare(TcLayer& L, const TcSetup& s) {
     k.out_bufs = (k.tma_store && (budget - 4 * 16384) / stage_bytes >= (size_t)want_stages) ? 2 : 1;
     const size_t out_stage = (k.tma_store || s.out_cstride != 1) ? (size_t)2 * k.out_bufs * 16384 : 0;   // strided outputs transpose through it
     int stages = (int)((budget - out_stage) / stage_bytes);
-    if (stages < 2 && !k.k3 && k.n_tile > 128 && k.n_tile % 16 == 0) {
+    if (stages < 2 && k.n_tile > 128 && k.n_tile % 16 == 0) {
         // a 256-row weight tile leaves room for one stage only: the packed matrix is row-contiguous, so the same rows
         // are addressed as twice as many tiles of half the width
         TcSetup h = s;
@@ -600,11 +502,10 @@ int tc_prepare(TcLayer& L, const TcSetup& s) {
         // small maps: the box spans `ipt` whole images (rows of the A tile = (n, y, x))
         const cuuint32_t box_h = (cuuint32_t)(k.ipt > 1 ? Ho : k.bh);
         cuuint32_t box[4] = {TC_BK, (cuuint32_t)(k.bw * stride), box_h * (cuuint32_t)stride, (cuuint32_t)k.ipt};
-        if (k.k3) { box[0] = 32; box[1] = 64; box[2] = K3_ROWS; box[3] = 1; }     // 6 halo rows x 64 pixels x 32 channels
         cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
         void* base = (void*)((__half*)s.in_base + (plane ? s.in_plane : 0) + s.in_coff);
         CUresult r = enc(plane ? &L.a_lo : &L.a_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, k.k3 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         SKPS_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(A) failed: %d", (int)r);
     }
@@ -613,11 +514,11 @@ int tc_prepare(TcLayer& L, const TcSetup& s) {
     for (int plane = 0; plane < 2; ++plane) {
         cuuint64_t dims[2] = {(cuuint64_t)K_pad, (cuuint64_t)(k.n_tiles * k.n_tile)};
         cuuint64_t strides[1] = {(cuuint64_t)K_pad * 2};
-        cuuint32_t box[2] = {(cuuint32_t)(k.k3 ? 32 : TC_BK), (cuuint32_t)k.n_tile};
+        cuuint32_t box[2] = {(cuuint32_t)TC_BK, (cuuint32_t)k.n_tile};
         cuuint32_t estr[2] = {1, 1};
         void* base = (void*)(plane ? s.w_lo : s.w_hi);
         CUresult r = enc(plane ? &L.b_lo : &L.b_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, base, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, k.k3 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         SKPS_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
     }
@@ -670,11 +571,10 @@ static int tc_launch_t(const TcLayer& L, const TcK& k, int grid, cudaStream_t st
     return 0;
 }
 
-int tc_launch(const TcLayer& L, int batch, int img0, int num_sms, cudaStream_t stream) {
+int tc_launch(const TcLayer& L, int batch, int num_sms, cudaStream_t stream) {
     TcK k = L.k;
     k.m_tiles = k.ipt > 1 ? (batch + k.ipt - 1) / k.ipt : batch * k.tiles_per_img;
-    k.img0 = img0;
-    k.img_end = img0 + batch;
+    k.img_end = batch;
     int total = ((k.m_tiles + k.mt - 1) / k.mt) * k.n_tiles;
     int grid = total < num_sms ? total : num_sms;
     const bool sp = k.out_fmt == DT_SPLIT16;
@@ -777,13 +677,13 @@ extern "C" SKPS_API int skps_debug_conv_tc2(const float* x, int N, int H, int W,
         }
         TctLayer T;
         if (tct_prepare(T, s)) return 1;
-        if (tct_launch(T, N, 0, sms, 0)) return 1;
+        if (tct_launch(T, N, sms, 0)) return 1;
         SKPS_CUDA(cudaDeviceSynchronize());
         if (d_zero) cudaFree(d_zero);
     } else {
     TcLayer L;
     if (tc_prepare(L, s)) return 1;
-    if (tc_launch(L, N, 0, sms, 0)) return 1;
+    if (tc_launch(L, N, sms, 0)) return 1;
     }
     SKPS_CUDA(cudaDeviceSynchronize());
     if (out_split) {

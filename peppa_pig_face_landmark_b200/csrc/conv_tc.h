@@ -8,12 +8,11 @@ namespace skps {
 
 struct TcK {                     // kernel parameters
     int H, W, bw, bh, tiles_per_img, m_tiles, n_tiles, n_tile;
-    int img0;                    // first sample of this launch (sub-batch execution)
+    int img0;                    // first sample of this launch (always 0: a launch covers the whole batch)
     int img_end;                 // img0 + batch: rows of a multi-image tile past it are not stored
     int ipt;                     // images per 128-pixel tile (> 1 when Ho*Wo < 128, e.g. 8x8 maps)
     int stride;                  // conv stride (1 or 2): the A box walks the input with TMA element strides
     int mt;                      // pixel tiles per weight-tile load (1 or 2)
-    int k3;                      // 3x3 halo-row mode: one stage = 6 input rows x 32 channels (+ the 3 ky weight tiles), see conv_tc.cu
     int tma_store;               // epilogue stages 32-channel chunks in smem and stores them with TMA
     int out_bufs;                // staging buffers per epilogue warp group (1 or 2)
     int taps, kw, dil, pad, cchunks;
@@ -39,8 +38,6 @@ struct TcSetup {
     int kh, kw, dil, pad, stride;                 // H, W above are INPUT dims; output dims = ceil(H/stride) x ceil(W/stride)
     int Cout, act, n_tile, n_tiles;
     float out_scale;
-    int mt_hint;                 // 1 forces single-tile mode
-    int tma_store_hint;          // 1 disables the TMA-store epilogue
     const void* w_hi; const void* w_lo;           // device, (n_tiles*n_tile, K_pad) fp16
     const float* bias;
     void* out; int out_fmt; long long out_plane; int out_ld, out_coff, out_cstride;
@@ -51,6 +48,6 @@ struct TcSetup {
 
 bool tc_shape_ok(int Ho, int Wo, int Cin, int in_ld, int in_coff);
 int tc_prepare(TcLayer& L, const TcSetup& s);
-int tc_launch(const TcLayer& L, int batch, int img0, int num_sms, cudaStream_t stream);
+int tc_launch(const TcLayer& L, int batch, int num_sms, cudaStream_t stream);
 
 }  // namespace skps

@@ -13,15 +13,9 @@
 // bias / activation / fp16 hi-lo split, then the 32 x 32 block is written TRANSPOSED into the
 // warp's 4 KB staging slice (one 64-byte pixel row per store instruction, lane = channel) and leaves as one TMA store per
 // plane, so the NHWC layout of the output is unchanged.
-//
-// Halo-row stages (k3, 3x3 / dilation 1 / W in {32, 64}): as in conv_tc's opt-in mode a stage is (kx, 32-channel half): ONE
-// (bh+2)-row activation box (64-byte swizzled rows) serves the three ky taps - the B operand of tap ky is the 256 box rows that
-// start ky image rows in, a descriptor offset of ky * W * 64 bytes - next to the three ky weight tiles.  L2->SM bytes per tile
-// drop by a third (1728 -> 1152 KB at Cin = 128).  Opt-in (SKPS_TCT_K3=1), see tct_prepare.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <math.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include "../../include/skps_b200.h"
@@ -74,26 +68,6 @@ conv_tct_kernel(const __grid_constant__ CUtensorMap tmX_hi, const __grid_constan
             for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
                 const int img_l = tile / p.tiles_per_img, t = tile - img_l * p.tiles_per_img;
                 const int y0 = t * p.bh;
-                if (p.k3) {
-                    const int halves = p.Cin >> 5, K_row = p.cchunks * 64;
-                    const uint32_t stage_bytes = 6u * 8192u + 2u * (uint32_t)p.xb;
-                    for (int kb = 0; kb < 3 * halves; ++kb) {
-                        const int kx = kb / halves, h = kb - kx * halves;
-                        mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1u);
-                        const uint32_t fb = smem_u32(&full_bar[stage]);
-                        mbar_expect_tx(fb, stage_bytes);
-                        const uint32_t ss = base + (uint32_t)stage * TCT_STAGE;
-                        for (int ky = 0; ky < 3; ++ky) {
-                            const int kcol = (ky * 3 + kx) * K_row + h * 32;
-                            tma_load_2d(ss + (uint32_t)(2 * ky) * 8192u, &tmW_hi, fb, kcol, 0);
-                            tma_load_2d(ss + (uint32_t)(2 * ky + 1) * 8192u, &tmW_lo, fb, kcol, 0);
-                        }
-                        tma_load_4d(ss + 49152u, &tmX_hi, fb, h * 32, kx - 1, y0 - 1, img_l + p.img0);
-                        tma_load_4d(ss + 49152u + (uint32_t)p.xb, &tmX_lo, fb, h * 32, kx - 1, y0 - 1, img_l + p.img0);
-                        if (++stage == TCT_STAGES) { stage = 0; phase ^= 1u; }
-                    }
-                    continue;
-                }
                 for (int kb = 0; kb < kblocks; ++kb) {
                     const int tap = kb / p.cchunks, cc = kb - tap * p.cchunks;
                     const int ky = tap / p.kw, kx = tap - ky * p.kw;
@@ -125,34 +99,6 @@ conv_tct_kernel(const __grid_constant__ CUtensorMap tmX_hi, const __grid_constan
         for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
             const int img_l = tile / p.tiles_per_img, t = tile - img_l * p.tiles_per_img;
             float accv[4][32];                         // 32-pixel chunk ci of this warpgroup's 128 columns
-            if (p.k3) {
-                const int nkb = 3 * (p.Cin >> 5);
-                for (int kb = 0; kb < nkb; ++kb) {
-                    mbar_wait(smem_u32(&full_bar[stage]), phase);
-                    const uint32_t ss = base + (uint32_t)stage * TCT_STAGE;
-                    wg_fence();
-                    for (int ky = 0; ky < 3; ++ky) {
-                        const uint64_t w_hi = make_smem_desc_sw64(ss + (uint32_t)(2 * ky) * 8192u);
-                        const uint64_t w_lo = make_smem_desc_sw64(ss + (uint32_t)(2 * ky + 1) * 8192u);
-                        // tap row ky: the 256 box rows that start ky image rows in
-                        const uint32_t xo = ss + 49152u + (uint32_t)(ky * p.W * 64) + (uint32_t)(half_id * 128 * 64);
-#pragma unroll
-                        for (int ci = 0; ci < 4; ++ci) {
-                            const uint64_t x_hi = make_smem_desc_sw64(xo + (uint32_t)(ci * 32 * 64));
-                            const uint64_t x_lo = make_smem_desc_sw64(xo + (uint32_t)(ci * 32 * 64) + (uint32_t)p.xb);
-                            for (int k = 0; k < 2; ++k) {
-                                const uint64_t koff = (uint64_t)(k * 2);
-                                wg_mma3_128x32(accv[ci], w_hi + koff, w_lo + koff, 64u * 64u, x_hi + koff, x_lo + koff,
-                                               (kb | ky | k) != 0);
-                            }
-                        }
-                    }
-                    wg_commit();
-                    wg_wait0();
-                    if (lane == 0) mbar_arrive(smem_u32(&empty_bar[stage]));
-                    if (++stage == TCT_STAGES) { stage = 0; phase ^= 1u; }
-                }
-            } else
             for (int kb = 0; kb < kblocks; ++kb) {
                 mbar_wait(smem_u32(&full_bar[stage]), phase);
                 const uint32_t ss = base + (uint32_t)stage * TCT_STAGE;
@@ -209,42 +155,21 @@ conv_tct_kernel(const __grid_constant__ CUtensorMap tmX_hi, const __grid_constan
 }
 
 // ------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn tct_encode() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    }
-    return fn;
-}
-
 // The layers this kernel is for: tensor-bound k x k convs whose Cout fills the 128 accumulator rows (else the rows idle and
 // the pixels-as-rows kernel wins), whole 256-pixel row blocks, split-fp16 contiguous output, no residual.
 bool tct_applicable(const TcSetup& s) {
-    static int on = -1;
-    if (on < 0) { const char* e = getenv("SKPS_TCT"); on = (e && e[0] == '0') ? 0 : 1; }
-    if (!on) return false;
     const int stride = s.stride > 0 ? s.stride : 1;
     if (stride != 1 || s.kh != s.kw || s.kh < 3 || s.pad != s.dil * (s.kh - 1) / 2) return false;
-    // Cout threshold: below 96 the idle accumulator rows cost more than the operand reuse buys (SKPS_TCT_MINC overrides it)
-    static int min_c = -1;
-    if (min_c < 0) { const char* e = getenv("SKPS_TCT_MINC"); min_c = e ? atoi(e) : 96; }
     if (s.W < 16 || s.W > TCT_N || TCT_N % s.W || s.H % (TCT_N / s.W)) return false;
     if (s.Cin < 64 || (s.Cin % 8) || (s.in_ld % 8) || (s.in_coff % 8)) return false;
-    if (s.Cout < min_c || s.Cout > TCT_M || (s.Cout % 8) || s.n_tiles != 1) return false;
+    // Cout from 96: below it the idle accumulator rows cost more than the operand reuse buys
+    if (s.Cout < 96 || s.Cout > TCT_M || (s.Cout % 8) || s.n_tiles != 1) return false;
     if (s.res || s.hm_val || s.out_fmt != DT_SPLIT16 || s.out_cstride != 1 || (s.out_ld % 8) || (s.out_coff % 8)) return false;
     return true;
 }
 
 int tct_prepare(TctLayer& L, const TcSetup& s) {
-    EncodeTiledFn enc = tct_encode();
+    EncodeTiledFn enc = tensor_map_encoder();
     SKPS_CHECK(enc, "cuTensorMapEncodeTiled entry point not available");
     SKPS_CHECK(tct_applicable(s), "conv_tct: layer not applicable");
     TctK& k = L.k;
@@ -255,24 +180,14 @@ int tct_prepare(TctLayer& L, const TcSetup& s) {
     SKPS_CHECK(s.bias, "conv_tct: bias required");
     k.bias = s.bias;
     L.smem_bytes = TCT_STAGES * TCT_STAGE + 8 * 4096 + 1024;
-    {
-        // opt-in, as in conv_tc: the 64-byte-row operand layout costs what the third fewer L2->SM bytes save.  Kept (and
-        // unit-tested with SKPS_TCT_K3=1) as the starting point for a 128-byte-row variant.
-        const char* e = getenv("SKPS_TCT_K3");
-        const int k3_on = (e && e[0] == '1') ? 1 : 0;
-        k.xb = (k.bh + 2) * s.W * 64;
-        k.k3 = (k3_on && s.kh == 3 && s.dil == 1 && (s.W == 32 || s.W == 64) && s.Cin % 32 == 0 &&
-                6 * 8192 + 2 * k.xb <= TCT_STAGE) ? 1 : 0;
-    }
     for (int plane = 0; plane < 2; ++plane) {
         cuuint64_t dims[4] = {(cuuint64_t)s.Cin, (cuuint64_t)s.W, (cuuint64_t)s.H, (cuuint64_t)s.max_batch};
         cuuint64_t strides[3] = {(cuuint64_t)s.in_ld * 2, (cuuint64_t)s.W * s.in_ld * 2, (cuuint64_t)s.H * s.W * s.in_ld * 2};
         cuuint32_t box[4] = {64, (cuuint32_t)s.W, (cuuint32_t)k.bh, 1};
-        if (k.k3) { box[0] = 32; box[2] = (cuuint32_t)(k.bh + 2); }
         cuuint32_t estr[4] = {1, 1, 1, 1};
         void* base = (void*)((__half*)s.in_base + (plane ? s.in_plane : 0) + s.in_coff);
         CUresult r = enc(plane ? &L.x_lo : &L.x_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, k.k3 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         SKPS_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(tct X) failed: %d", (int)r);
     }
@@ -280,11 +195,11 @@ int tct_prepare(TctLayer& L, const TcSetup& s) {
     for (int plane = 0; plane < 2; ++plane) {
         cuuint64_t dims[2] = {(cuuint64_t)K_pad, (cuuint64_t)s.n_tile};        // rows beyond n_tile: OOB zero fill
         cuuint64_t strides[1] = {(cuuint64_t)K_pad * 2};
-        cuuint32_t box[2] = {(cuuint32_t)(k.k3 ? 32 : 64), (cuuint32_t)TCT_M};
+        cuuint32_t box[2] = {64, (cuuint32_t)TCT_M};
         cuuint32_t estr[2] = {1, 1};
         void* base = (void*)(plane ? s.w_lo : s.w_hi);
         CUresult r = enc(plane ? &L.w_lo : &L.w_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, base, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, k.k3 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         SKPS_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(tct W) failed: %d", (int)r);
     }
@@ -305,7 +220,7 @@ int tct_prepare(TctLayer& L, const TcSetup& s) {
     return 0;
 }
 
-int tct_launch(const TctLayer& L, int batch, int img0, int num_sms, cudaStream_t stream) {
+int tct_launch(const TctLayer& L, int batch, int num_sms, cudaStream_t stream) {
     static int attr_bytes = 0;
     if (L.smem_bytes > attr_bytes) {
         SKPS_CUDA(cudaFuncSetAttribute(conv_tct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
@@ -313,7 +228,6 @@ int tct_launch(const TctLayer& L, int batch, int img0, int num_sms, cudaStream_t
     }
     TctK k = L.k;
     k.m_tiles = batch * k.tiles_per_img;
-    k.img0 = img0;
     const int grid = k.m_tiles < num_sms ? k.m_tiles : num_sms;
     conv_tct_kernel<<<grid, TCT_THREADS, L.smem_bytes, stream>>>(L.x_hi, L.x_lo, L.w_hi, L.w_lo, L.o_hi, L.o_lo, k);
     SKPS_CUDA(cudaGetLastError());

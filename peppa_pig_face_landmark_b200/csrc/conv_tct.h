@@ -11,8 +11,6 @@ namespace skps {
 struct TctK {                    // kernel parameters
     int W, bh, tiles_per_img, m_tiles, img0;    // tile = bh whole rows = 256 pixels
     int taps, kw, dil, pad, cchunks, Cin, Cout, act;
-    int k3;                      // halo-row stages: (kx, 32-channel half) = one (bh+2)-row box + the three ky weight tiles
-    int xb;                      // k3: bytes of one plane of the activation box
     float out_scale;             // exact power of two undoing the weight pre-scale
     const float* bias;
 };
@@ -26,6 +24,6 @@ struct TctLayer {
 
 bool tct_applicable(const TcSetup& s);          // s.H, s.W: the (stride-1) map; split-fp16 contiguous output, no residual
 int tct_prepare(TctLayer& L, const TcSetup& s);
-int tct_launch(const TctLayer& L, int batch, int img0, int num_sms, cudaStream_t stream);
+int tct_launch(const TctLayer& L, int batch, int num_sms, cudaStream_t stream);
 
 }  // namespace skps

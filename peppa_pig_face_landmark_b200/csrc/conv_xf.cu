@@ -633,21 +633,6 @@ conv_xf_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
 }
 
 // ------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn xf_get_encode() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    }
-    return fn;
-}
-
 static const float* xf_zero_bias() {
     static float* z = nullptr;
     if (!z) {
@@ -696,7 +681,7 @@ static int encode4(EncodeTiledFn enc, CUtensorMap* m, const TView& v, int plane,
 }
 
 int xf_prepare(XfLayer& L, const XfSetup& s) {
-    EncodeTiledFn enc = xf_get_encode();
+    EncodeTiledFn enc = tensor_map_encoder();
     SKPS_CHECK(enc, "cuTensorMapEncodeTiled entry point not available");
     SKPS_CHECK(xf_supported(s), "conv_xf: unsupported layer");
     memset(&L.k, 0, sizeof(L.k));
@@ -850,11 +835,10 @@ static int xf_launch_m(const XfLayer& L, const XfK& k, int grid, cudaStream_t st
     return 1;
 }
 
-int xf_launch(const XfLayer& L, int batch, int img0, int num_sms, cudaStream_t stream) {
+int xf_launch(const XfLayer& L, int batch, int num_sms, cudaStream_t stream) {
     XfK k = L.k;
     k.m_tiles = batch * k.tiles_per_img;
-    k.img0 = img0;
-    k.img_end = img0 + batch;
+    k.img_end = batch;
     const int grid = k.m_tiles < num_sms ? k.m_tiles : num_sms;
     return L.mode == XF_SCALE ? xf_launch_m<XF_SCALE>(L, k, grid, stream) : xf_launch_m<XF_DW>(L, k, grid, stream);
 }
@@ -938,7 +922,7 @@ extern "C" SKPS_API int skps_debug_conv_xf(int mode, const float* x, int N, int 
     XfLayer L;
     if (xf_prepare(L, s)) return 1;
     const int sms = sm_count();
-    if (xf_launch(L, N, 0, sms, 0)) return 1;
+    if (xf_launch(L, N, sms, 0)) return 1;
     SKPS_CUDA(cudaDeviceSynchronize());
     if (out_split) {
         __half* tmp = (__half*)malloc(nout * 4);

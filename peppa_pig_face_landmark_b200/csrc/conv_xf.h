@@ -64,6 +64,6 @@ struct XfSetup {
 
 bool xf_supported(const XfSetup& s);
 int xf_prepare(XfLayer& L, const XfSetup& s);
-int xf_launch(const XfLayer& L, int batch, int img0, int num_sms, cudaStream_t stream);
+int xf_launch(const XfLayer& L, int batch, int num_sms, cudaStream_t stream);
 
 }  // namespace skps

@@ -11,7 +11,6 @@
 // dwconv_kernel: bias first, then taps in (ky,kx) order with fmaf.
 #include <cuda.h>
 #include <cuda_fp16.h>
-#include <stdlib.h>
 
 #include "common.h"
 #include "dw_tma.h"
@@ -315,122 +314,10 @@ upcat_tma_kernel(const __grid_constant__ CUtensorMap tm_low, const DwTmaK p, con
     }
 }
 
-// Same op without the interpolation pass: depthwise3x3(bilinear_x2(low)) is a 3x3 stencil on the LOW-res tile whose
-// weights depend only on the output row/column class (first / even / odd / last): 9 FMAs per output straight from
-// the TMA-staged tile (plan.upcat_effective_weights builds the [4][4][3][3][C] table).  The interpolating kernel
-// above is instruction-issue bound (tens of thread-instructions per output element, DRAM far from its peak).
-__global__ void __launch_bounds__(DW_THREADS, 4)
-upcat_eff_kernel(const __grid_constant__ CUtensorMap tm_low, const DwTmaK p, const int Hl, const int Wl,
-                 const float* __restrict__ weff) {
-    constexpr int CB = 32, CG = CB / 4;
-    constexpr int LOW_BYTES = LH * LW * 128;
-    extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ __align__(8) uint64_t bar;
-    const int tid = threadIdx.x;
-    const int tiles_x = (p.Wo + TW - 1) / TW;
-    const int ty = blockIdx.x / tiles_x, tx = blockIdx.x - ty * tiles_x;
-    const int chunk = blockIdx.y;
-    const int n = blockIdx.z + p.img0;
-    const int oy0 = ty * TH, ox0 = tx * TW;
-    const int ly0 = oy0 / 2 - 1, lx0 = ox0 / 2 - 1;          // low-res origin of the tile (may be -1)
-    const uint32_t sbase = (dsmem_u32(smem) + 127u) & ~127u;
-    const uint32_t bar_a = dsmem_u32(&bar);
-    if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"((uint32_t)LOW_BYTES) : "memory");
-        asm volatile(
-            "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-            ::"r"(sbase), "l"(&tm_low), "r"(bar_a), "r"(chunk * CB), "r"(lx0), "r"(ly0), "r"(n) : "memory");
-    }
-    const int cg = tid % CG, pg = tid / CG;
-    const int c = chunk * CB + cg * 4;
-    constexpr int PX = 4, SEGS = TW / PX;
-    const int row = pg / SEGS, xs = (pg % SEGS) * PX;
-    const int oy = oy0 + row, x0 = ox0 + xs;
-    const bool live = c < p.C && oy < p.Ho && x0 < p.Wo;
-    // row/column classes and the (edge-clamped) low-res rows/columns this thread reads, relative to the tile
-    const int cy = oy == 0 ? 0 : (oy == p.Ho - 1 ? 3 : 1 + (oy & 1));
-    int r[3], cc[4];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) r[a] = min(max((oy >> 1) + a - 1, 0), Hl - 1) - ly0;
-#pragma unroll
-    for (int t = 0; t < 4; ++t) cc[t] = min(max((x0 >> 1) - 1 + t, 0), Wl - 1) - lx0;
-    float4 bias = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (live) bias = *reinterpret_cast<const float4*>(p.bias + c);
-    __syncthreads();
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "UPE_WAIT:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], 0;\n\t"
-        "@p bra UPE_DONE;\n\t"
-        "bra UPE_WAIT;\n\t"
-        "UPE_DONE:\n\t"
-        "}\n" ::"r"(bar_a) : "memory");
-    if (!live) return;
-    const uint8_t* low = smem + (sbase - dsmem_u32(smem));
-    // per output pixel q: weight rows of its column class; accumulate low-res row by low-res row (keeps 4 + 4 float4 live)
-    int wq[PX];                      // element offsets into weff (32-bit: the table is 144*C floats)
-    float4 acc[PX];
-#pragma unroll
-    for (int q = 0; q < PX; ++q) {
-        const int ox = x0 + q;
-        const int cx = ox == 0 ? 0 : (ox == p.Wo - 1 ? 3 : 1 + (ox & 1));
-        wq[q] = ((cy * 4 + cx) * 9) * p.C + c;
-        acc[q] = bias;
-    }
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-        float4 in[4];
-#pragma unroll
-        for (int t = 0; t < 4; ++t) in[t] = *reinterpret_cast<const float4*>(low + (r[a] * LW + cc[t]) * 128 + cg * 16);
-#pragma unroll
-        for (int q = 0; q < PX; ++q)
-#pragma unroll
-            for (int b = 0; b < 3; ++b) {
-                const float4 w = __ldg(reinterpret_cast<const float4*>(weff + wq[q] + (a * 3 + b) * p.C));
-                const float4 v = in[(q >> 1) + b];
-                acc[q].x = fmaf(v.x, w.x, acc[q].x); acc[q].y = fmaf(v.y, w.y, acc[q].y);
-                acc[q].z = fmaf(v.z, w.z, acc[q].z); acc[q].w = fmaf(v.w, w.w, acc[q].w);
-            }
-    }
-#pragma unroll
-    for (int q = 0; q < PX; ++q) {
-        const int ox = x0 + q;
-        if (ox >= p.Wo) break;
-        float4 o = acc[q];
-        o.x = apply_act(o.x, p.act); o.y = apply_act(o.y, p.act); o.z = apply_act(o.z, p.act); o.w = apply_act(o.w, p.act);
-        st4(p.out, p.out_fmt, p.out_plane, (((long long)n * p.Ho + oy) * p.Wo + ox) * p.out_ld + p.out_coff + c, o);
-    }
-}
-
 // ------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn dw_get_encode() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    }
-    return fn;
-}
-
-// Output rows per tile: 16 for the 5x5 stride-1 layers (two output rows per thread), else 8.  SKPS_DW_ROWS2=0 keeps 8
-// everywhere; plan.dw_tile_rows mirrors this (rows of the per-tile channel-sum buffer).
-int dw_tile_rows(int k, int s) {
-    static int rows2 = -1;
-    if (rows2 < 0) {
-        const char* e = getenv("SKPS_DW_ROWS2");
-        rows2 = (e && e[0] == '0') ? 0 : 1;
-    }
-    return (rows2 && k == 5 && s == 1) ? 2 * TH : TH;
-}
+// Output rows per tile: 16 for the 5x5 stride-1 layers (two output rows per thread), else 8.  plan.dw_tile_rows mirrors
+// this (rows of the per-tile channel-sum buffer).
+int dw_tile_rows(int k, int s) { return (k == 5 && s == 1) ? 2 * TH : TH; }
 
 static bool variant_ok(int k, int s, int d) {
     return (k == 3 && s == 1 && d == 1) || (k == 3 && s == 2 && d == 1) || (k == 5 && s == 1 && d == 1) ||
@@ -447,7 +334,7 @@ bool dw_tma_supported(const TView& in, const TView& out, int k, int s, int d, in
 
 int dw_tma_prepare(DwTmaLayer& L, const TView& in, const TView& out, const float* w, const float* bias, int k, int s,
                    int d, int pad, int act, int max_batch, const TView* part) {
-    EncodeTiledFn enc = dw_get_encode();
+    EncodeTiledFn enc = tensor_map_encoder();
     SKPS_CHECK(enc, "cuTensorMapEncodeTiled entry point not available");
     SKPS_CHECK(dw_tma_supported(in, out, k, s, d, pad), "dw_tma: unsupported layer");
     const bool split = in.fmt == DT_SPLIT16;
@@ -483,8 +370,9 @@ int dw_tma_prepare(DwTmaLayer& L, const TView& in, const TView& out, const float
     return 0;
 }
 
-template <int K, int S, int D, bool SPLIT, int RY>
-static int launch_variant_r(const DwTmaLayer& L, const DwTmaK& k, dim3 grid, cudaStream_t stream) {
+template <int K, int S, int D, bool SPLIT>
+static int launch_variant(const DwTmaLayer& L, const DwTmaK& k, dim3 grid, cudaStream_t stream) {
+    constexpr int RY = (K == 5 && S == 1) ? 2 : 1;      // dw_tile_rows(K, S) / TH
     static bool attr_set = false;
     if (!attr_set) {
         SKPS_CUDA(cudaFuncSetAttribute(dw_tma_kernel<K, S, D, SPLIT, RY>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
@@ -495,15 +383,8 @@ static int launch_variant_r(const DwTmaLayer& L, const DwTmaK& k, dim3 grid, cud
     return 0;
 }
 
-template <int K, int S, int D, bool SPLIT>
-static int launch_variant(const DwTmaLayer& L, const DwTmaK& k, dim3 grid, cudaStream_t stream) {
-    if (K == 5 && S == 1 && dw_tile_rows(K, S) == 2 * TH) return launch_variant_r<K, S, D, SPLIT, (K == 5 && S == 1) ? 2 : 1>(L, k, grid, stream);
-    return launch_variant_r<K, S, D, SPLIT, 1>(L, k, grid, stream);
-}
-
-int dw_tma_launch(const DwTmaLayer& L, int batch, int img0, cudaStream_t stream) {
+int dw_tma_launch(const DwTmaLayer& L, int batch, cudaStream_t stream) {
     DwTmaK k = L.k;
-    k.img0 = img0;
     k.chunks = L.chunks;
     k.batch = batch;
     const int tht = dw_tile_rows(L.k_size, L.stride);
@@ -529,8 +410,8 @@ bool upcat_tma_supported(const TView& low, const TView& skip, const TView& out) 
 }
 
 int upcat_tma_prepare(UpcatTmaLayer& L, const TView& low, const TView& skip, const TView& out, const float* w,
-                      const float* bias, const float* weff, int act, int max_batch) {
-    EncodeTiledFn enc = dw_get_encode();
+                      const float* bias, int act, int max_batch) {
+    EncodeTiledFn enc = tensor_map_encoder();
     SKPS_CHECK(enc, "cuTensorMapEncodeTiled entry point not available");
     SKPS_CHECK(upcat_tma_supported(low, skip, out), "upcat_tma: unsupported layer");
     cuuint64_t dims[4] = {(cuuint64_t)low.C, (cuuint64_t)low.W, (cuuint64_t)low.H, (cuuint64_t)max_batch};
@@ -547,7 +428,6 @@ int upcat_tma_prepare(UpcatTmaLayer& L, const TView& low, const TView& skip, con
     k.w = w; k.bias = bias;
     k.out = out.base; k.out_fmt = out.fmt; k.out_plane = out.plane; k.out_ld = out.ld; k.out_coff = out.c_off;
     L.Hl = low.H; L.Wl = low.W;
-    L.weff = weff;
     L.chunks = (low.C + 31) / 32;
     L.smem_bytes = LH * LW * 128 + (TH + 2) * (TW + 2) * 32 * 4 + 128;     // low tile + staged up-sampled window
     // skip channels: an ordinary depthwise layer over the channel slice [Cu, Ctot)
@@ -558,14 +438,12 @@ int upcat_tma_prepare(UpcatTmaLayer& L, const TView& low, const TView& skip, con
     return 0;
 }
 
-int upcat_tma_launch(const UpcatTmaLayer& L, int batch, int img0, cudaStream_t stream) {
-    DwTmaK k = L.k;
-    k.img0 = img0;
+int upcat_tma_launch(const UpcatTmaLayer& L, int batch, cudaStream_t stream) {
+    const DwTmaK& k = L.k;
     dim3 grid(((k.Ho + TH - 1) / TH) * ((k.Wo + TW - 1) / TW), L.chunks, batch);
-    if (L.weff) upcat_eff_kernel<<<grid, DW_THREADS, LH * LW * 128 + 128, stream>>>(L.low, k, L.Hl, L.Wl, L.weff);
-    else upcat_tma_kernel<<<grid, DW_THREADS, L.smem_bytes, stream>>>(L.low, k, L.Hl, L.Wl);
+    upcat_tma_kernel<<<grid, DW_THREADS, L.smem_bytes, stream>>>(L.low, k, L.Hl, L.Wl);
     SKPS_CUDA(cudaGetLastError());
-    return dw_tma_launch(L.skip, batch, img0, stream);
+    return dw_tma_launch(L.skip, batch, stream);
 }
 
 }  // namespace skps

@@ -27,7 +27,7 @@ bool dw_tma_supported(const TView& in, const TView& out, int k, int s, int d, in
 int dw_tma_prepare(DwTmaLayer& L, const TView& in, const TView& out, const float* w, const float* bias, int k, int s,
                    int d, int pad, int act, int max_batch, const TView* part = nullptr);
 int dw_tile_rows(int k, int s);                  // output rows per tile (8, or 16 for 5x5 stride-1 layers); tiles are 16 columns wide
-int dw_tma_launch(const DwTmaLayer& L, int batch, int img0, cudaStream_t stream);
+int dw_tma_launch(const DwTmaLayer& L, int batch, cudaStream_t stream);
 
 // depthwise3x3(concat(bilinear_x2(low), skip)): TMA-staged low-res tiles for the up-sampled channels plus a
 // plain TMA depthwise pass over the skip channels (kps_student.onnx nodes 176-178, 193-195)
@@ -35,13 +35,12 @@ struct UpcatTmaLayer {
     CUtensorMap low;
     DwTmaK k;            // C = channels taken from `low`
     int Hl, Wl, chunks, smem_bytes;
-    const float* weff;   // [4][4][3][3][C] low-res stencil weights (plan.upcat_effective_weights); null = interpolate in smem
     DwTmaLayer skip;
     bool valid = false;
 };
 bool upcat_tma_supported(const TView& low, const TView& skip, const TView& out);
 int upcat_tma_prepare(UpcatTmaLayer& L, const TView& low, const TView& skip, const TView& out, const float* w,
-                      const float* bias, const float* weff, int act, int max_batch);
-int upcat_tma_launch(const UpcatTmaLayer& L, int batch, int img0, cudaStream_t stream);
+                      const float* bias, int act, int max_batch);
+int upcat_tma_launch(const UpcatTmaLayer& L, int batch, cudaStream_t stream);
 
 }  // namespace skps

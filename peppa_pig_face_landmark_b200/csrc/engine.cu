@@ -59,13 +59,10 @@ struct skps_engine {
     std::vector<XfLayer> xf;              // per op; fused producer -> pointwise conv layers (OP_DWPW, OP_CONV with FLAG_XF)
     std::vector<DwTmaLayer> dwt;          // per op; TMA-staged depthwise layers (valid flag)
     std::vector<UpcatTmaLayer> upt;       // per op; TMA-staged fused upsample+concat+depthwise
-    bool use_dw_tma = true;
     // streaming host round trip (skps_engine_submit_host_u8): 2 slots, H2D on its own stream
     cudaStream_t s_copy = nullptr, s_compute = nullptr;
     void* d_slot_in[2] = {nullptr, nullptr};
     cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
-    struct Segment { int first, end, chunk; };
-    std::vector<Segment> segments;        // ops [first,end) run `chunk` samples at a time (L2 residency)
 };
 
 static size_t buf_elems(const BufDesc& b) { return (size_t)b.C * b.H * b.W; }
@@ -81,16 +78,12 @@ static float half_bits_to_float(uint16_t h) {
     float f; memcpy(&f, &bits, 4); return f;
 }
 
-static TView resolve(const skps_engine* e, const View& v, int b0 = 0) {
+static TView resolve(const skps_engine* e, const View& v) {
     TView t;
     memset(&t, 0, sizeof(t));
     if (v.buf < 0) return t;
     const BufDesc& b = e->bufs[v.buf];
-    const bool f32in = (v.buf == e->input_buf && e->f32_mode);
-    t.base = f32in ? (void*)e->d_in_f32 : e->dbuf[v.buf];
-    // sub-batch offset: samples b0.. (SPLIT16 planes are 2 bytes per element each)
-    const size_t esz = f32in ? 4 : (b.dtype == DT_U8 ? 1 : (b.dtype == DT_SPLIT16 ? 2 : 4));
-    t.base = (char*)t.base + (size_t)b0 * b.C * b.H * b.W * esz;
+    t.base = (v.buf == e->input_buf && e->f32_mode) ? (void*)e->d_in_f32 : e->dbuf[v.buf];
     t.ld = b.C;
     t.c_off = v.c_off; t.c_stride = v.c_stride; t.C = v.C; t.H = b.H; t.W = b.W;
     t.sample = (long long)b.C * b.H * b.W;
@@ -99,36 +92,36 @@ static TView resolve(const skps_engine* e, const View& v, int b0 = 0) {
     return t;
 }
 
-// Enqueue ops [first,last) for samples [b0, b0+batch).
-static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int last = -1, int b0 = 0) {
+// Enqueue ops [first,last) for samples [0, batch).
+static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int last = -1) {
     const size_t end = last < 0 ? e->ops.size() : (size_t)last;
     for (size_t i = (size_t)first; i < end; ++i) {
         const OpDesc& op = e->ops[i];
-        TView in0 = resolve(e, op.in[0], b0), in1 = resolve(e, op.in[1], b0), in2 = resolve(e, op.in[2], b0);
-        TView out0 = resolve(e, op.out[0], b0), out1 = resolve(e, op.out[1], b0);
+        TView in0 = resolve(e, op.in[0]), in1 = resolve(e, op.in[1]), in2 = resolve(e, op.in[2]);
+        TView out0 = resolve(e, op.out[0]), out1 = resolve(e, op.out[1]);
         const float* w = op.w_off >= 0 ? e->d_weights + op.w_off : nullptr;
         const float* b = op.b_off >= 0 ? e->d_weights + op.b_off : nullptr;
         int rc = 0;
         switch (op.type) {
             case OP_CONV: {
                 if (op.flags & FLAG_MMA) {
-                    rc = conv_mma_launch(e->mma[i], batch, b0, s);
+                    rc = conv_mma_launch(e->mma[i], batch, s);
                     break;
                 }
                 if (op.flags & FLAG_XF) {
-                    rc = xf_launch(e->xf[i], batch, b0, e->num_sms, s);
+                    rc = xf_launch(e->xf[i], batch, e->num_sms, s);
                     break;
                 }
                 if (op.flags & FLAG_TC) {
                     if (e->hm[i].valid) {
-                        rc = hm_launch(e->hm[i], batch, b0, e->num_sms, s);
+                        rc = hm_launch(e->hm[i], batch, e->num_sms, s);
                         break;
                     }
                     if (e->tct[i].valid) {
-                        rc = tct_launch(e->tct[i], batch, b0, e->num_sms, s);
+                        rc = tct_launch(e->tct[i], batch, e->num_sms, s);
                         break;
                     }
-                    rc = tc_launch(e->tc[i], batch, b0, e->num_sms, s);
+                    rc = tc_launch(e->tc[i], batch, e->num_sms, s);
                     break;
                 }
                 ConvArgs a;
@@ -144,7 +137,7 @@ static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int
             }
             case OP_DWCONV: {
                 if (e->dwt[i].valid) {
-                    rc = dw_tma_launch(e->dwt[i], batch, b0, s);
+                    rc = dw_tma_launch(e->dwt[i], batch, s);
                     break;
                 }
                 DwArgs a;
@@ -154,7 +147,7 @@ static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int
                 rc = launch_dwconv(a, s);
                 break;
             }
-            case OP_DWPW: rc = xf_launch(e->xf[i], batch, b0, e->num_sms, s); break;
+            case OP_DWPW: rc = xf_launch(e->xf[i], batch, e->num_sms, s); break;
             case OP_STEM_BLOCK: {
                 // w = StemBlockW as packed by lowering (dense weights -> kernel-parameter bank); i[0] -> [9][E]+[E] depthwise table
                 StemBlockW W;
@@ -191,14 +184,14 @@ static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int
                                   batch, s);
                 break;
             case OP_ADDN: {
-                TView ins[4] = {in0, in1, in2, resolve(e, op.in3, b0)};
+                TView ins[4] = {in0, in1, in2, resolve(e, op.in3)};
                 int n_in = 0;
                 while (n_in < 4 && ins[n_in].base) ++n_in;
                 rc = launch_addn(ins, n_in, out0, op.act, batch, s);
                 break;
             }
             case OP_UPCAT_DW:
-                rc = e->upt[i].valid ? upcat_tma_launch(e->upt[i], batch, b0, s)
+                rc = e->upt[i].valid ? upcat_tma_launch(e->upt[i], batch, s)
                                      : launch_upcat_dw(in0, in1, out0, w, b, op.act, batch, s);
                 break;
             case OP_DET_DECODE: {
@@ -223,17 +216,6 @@ static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int
     return 0;
 }
 
-// Whole forward: every segment sweeps the batch in L2-sized chunks.
-static int run_forward(skps_engine* e, int batch, cudaStream_t s) {
-    for (const auto& sg : e->segments) {
-        for (int b0 = 0; b0 < batch; b0 += sg.chunk) {
-            int nb = batch - b0 < sg.chunk ? batch - b0 : sg.chunk;
-            if (run_ops(e, nb, s, sg.first, sg.end, b0)) return 1;
-        }
-    }
-    return 0;
-}
-
 extern "C" SKPS_API const char* skps_last_error(void) { return get_error(); }
 extern "C" SKPS_API int skps_version(void) { return 1; }
 
@@ -243,7 +225,7 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
     SKPS_CHECK(words[0] == PLAN_MAGIC && words[1] == 1, "engine_create: bad plan header");
     int n_bufs = words[2], n_ops = words[3];
     const size_t body = (size_t)8 + 4 * (size_t)n_bufs + OP_WORDS * (size_t)n_ops;
-    SKPS_CHECK(n_words > body && n_words == body + 1 + 3 * (size_t)words[body], "engine_create: plan size mismatch");
+    SKPS_CHECK(n_words == body, "engine_create: plan size mismatch");
     SKPS_CUDA(cudaSetDevice(device));
     skps_engine* e = new skps_engine();
     e->device = device;
@@ -254,10 +236,6 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
     for (int i = 0; i < n_bufs; ++i, p += 4) e->bufs.push_back(BufDesc{p[0], p[1], p[2], p[3]});
     e->ops.resize(n_ops);
     memcpy(e->ops.data(), p, sizeof(OpDesc) * n_ops);
-    {
-        const int32_t* t = words + body;
-        for (int i = 0; i < t[0]; ++i) e->segments.push_back({t[1 + 3 * i], t[2 + 3 * i], t[3 + 3 * i]});
-    }
     e->h_weights.assign(weights, weights + n_floats);
     e->n_weights = n_floats;
     e->launches = n_ops;
@@ -267,6 +245,12 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
         set_error("engine_create: %s: %s", what, tmp);
         skps_engine_destroy(e);
         return 1;
+    };
+    auto fail_op = [&](int i, const char* what) {
+        char tmp[900];
+        snprintf(tmp, sizeof(tmp), "%s", get_error());
+        set_error("op %d: %s", i, tmp);
+        return fail(what);
     };
     if (cudaMalloc(&e->d_weights, n_floats * sizeof(float)) != cudaSuccess) { set_error("cudaMalloc weights"); return fail("alloc"); }
     if (cudaMemcpy(e->d_weights, weights, n_floats * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
@@ -296,12 +280,8 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
         TView in0 = resolve(e, op.in[0]), res = resolve(e, op.in[1]), out0 = resolve(e, op.out[0]);
         if (!conv_mma_supported(in0.C, out0.C, op.kh, op.kw, op.sh, op.dh, op.ph) ||
             conv_mma_prepare(e->mma[i], in0, out0, res, (op.flags & FLAG_RES_FIRST) ? 1 : 0, e->d_weights + op.w_off,
-                             op.b_off >= 0 ? e->d_weights + op.b_off : nullptr, op.f[0], op.act, max_batch)) {
-            char tmp[900];
-            snprintf(tmp, sizeof(tmp), "%s", get_error());
-            set_error("op %d: conv_mma: %s", i, tmp);
-            return fail("mma");
-        }
+                             op.b_off >= 0 ? e->d_weights + op.b_off : nullptr, op.f[0], op.act, max_batch))
+            return fail_op(i, "mma");
     }
     e->tc.resize(n_ops);
     e->hm.resize(n_ops);
@@ -315,8 +295,6 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
             return fail("tc");
         }
         TcSetup s = {};
-        { const char* env = getenv("SKPS_TC_MT"); s.mt_hint = (env && env[0] == '1') ? 1 : 0; }
-        { const char* env = getenv("SKPS_TC_TMA_STORE"); s.tma_store_hint = (env && env[0] == '0') ? 1 : 0; }
         s.H = in0.H; s.W = in0.W; s.Cin = in0.C; s.in_ld = in0.ld; s.in_coff = in0.c_off; s.max_batch = max_batch;
         s.in_base = in0.base; s.in_plane = in0.plane;
         s.kh = op.kh; s.kw = op.kw; s.dil = op.dh; s.pad = op.ph; s.stride = op.sh;
@@ -334,30 +312,15 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
             // the lowering sizes the partial buffer for 128-pixel tiles (conv_tc epilogue) or 256-pixel tiles (conv_hm.cu)
             const int tile_px = part.H * part.W > 0 ? out0.H * out0.W / (part.H * part.W) : 0;
             if (tile_px == HM_TILE_PIXELS) {
-                if (hm_prepare(e->hm[i], s)) {
-                    char tmp[900];
-                    snprintf(tmp, sizeof(tmp), "%s", get_error());
-                    set_error("op %d: %s", i, tmp);
-                    return fail("hm");
-                }
+                if (hm_prepare(e->hm[i], s)) return fail_op(i, "hm");
                 continue;
             }
         }
         if (op.dh == op.dw && op.ph == op.pw && tct_applicable(s)) {
-            if (tct_prepare(e->tct[i], s)) {
-                char tmp[900];
-                snprintf(tmp, sizeof(tmp), "%s", get_error());
-                set_error("op %d: %s", i, tmp);
-                return fail("tct");
-            }
+            if (tct_prepare(e->tct[i], s)) return fail_op(i, "tct");
             continue;
         }
-        if (op.dh != op.dw || op.ph != op.pw || tc_prepare(e->tc[i], s)) {
-            char tmp[900];
-            snprintf(tmp, sizeof(tmp), "%s", get_error());
-            set_error("op %d: %s", i, tmp);
-            return fail("tc");
-        }
+        if (op.dh != op.dw || op.ph != op.pw || tc_prepare(e->tc[i], s)) return fail_op(i, "tc");
     }
     // fused producer -> pointwise conv layers (conv_xf.cu): depthwise / up-sample+concat+depthwise / squeeze-excite scale
     e->xf.resize(n_ops);
@@ -384,35 +347,19 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
         s.w_hi = e->d_weights + op.w_off; s.w_lo = e->d_weights + op.i[2];
         s.bias = op.b_off >= 0 ? e->d_weights + op.b_off : nullptr;
         s.res_first = (op.flags & FLAG_RES_FIRST) ? 1 : 0;
-        if (xf_prepare(e->xf[i], s)) {
-            char tmp[900];
-            snprintf(tmp, sizeof(tmp), "%s", get_error());
-            set_error("op %d: %s", i, tmp);
-            return fail("xf");
-        }
+        if (xf_prepare(e->xf[i], s)) return fail_op(i, "xf");
     }
     // depthwise layers: TMA descriptors over the input views
     e->dwt.resize(n_ops);
-    {
-        const char* env = getenv("SKPS_DW_TMA");
-        e->use_dw_tma = !(env && env[0] == '0');
-    }
     e->upt.resize(n_ops);
-    for (int i = 0; i < n_ops && e->use_dw_tma; ++i) {
+    for (int i = 0; i < n_ops; ++i) {
         const OpDesc& op = e->ops[i];
         if (op.type == OP_UPCAT_DW) {
             TView low = resolve(e, op.in[0]), skip = resolve(e, op.in[1]), out0 = resolve(e, op.out[0]);
             if (!upcat_tma_supported(low, skip, out0)) continue;
-            const char* eff = getenv("SKPS_UPCAT_EFF");
-            // the low-res stencil kernel issues 36 weight loads per thread: opt-in until its weights are staged in shared memory
-            const float* weff = (op.i[0] > 0 && eff && eff[0] == '1') ? e->d_weights + op.i[0] : nullptr;
-            if (upcat_tma_prepare(e->upt[i], low, skip, out0, e->d_weights + op.w_off, e->d_weights + op.b_off, weff, op.act,
-                                  max_batch)) {
-                char tmp[900];
-                snprintf(tmp, sizeof(tmp), "%s", get_error());
-                set_error("op %d: %s", i, tmp);
-                return fail("upcat_tma");
-            }
+            if (upcat_tma_prepare(e->upt[i], low, skip, out0, e->d_weights + op.w_off, e->d_weights + op.b_off, op.act,
+                                  max_batch))
+                return fail_op(i, "upcat_tma");
             e->upt[i].valid = true;
             continue;
         }
@@ -421,17 +368,13 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
         if (!dw_tma_supported(in0, out0, op.kh, op.sh, op.dh, op.ph)) continue;
         TView part = resolve(e, op.out[1]);          // FLAG_GAP_PARTIAL: per-tile channel sums for the squeeze-excite gate
         if (dw_tma_prepare(e->dwt[i], in0, out0, e->d_weights + op.w_off, e->d_weights + op.b_off, op.kh, op.sh, op.dh,
-                           op.ph, op.act, max_batch, (op.flags & FLAG_GAP_PARTIAL) ? &part : nullptr)) {
-            char tmp[900];
-            snprintf(tmp, sizeof(tmp), "%s", get_error());
-            set_error("op %d: %s", i, tmp);
-            return fail("dw_tma");
-        }
+                           op.ph, op.act, max_batch, (op.flags & FLAG_GAP_PARTIAL) ? &part : nullptr))
+            return fail_op(i, "dw_tma");
         e->dwt[i].valid = true;
     }
     for (int i = 0; i < n_ops; ++i) {
         if (e->ops[i].type == OP_DWCONV && (e->ops[i].flags & FLAG_GAP_PARTIAL) && !e->dwt[i].valid) {
-            set_error("op %d: per-tile channel sums need the TMA depthwise kernel (SKPS_DW_TMA=0 or unsupported layer)", i);
+            set_error("op %d: per-tile channel sums need the TMA depthwise kernel (unsupported layer)", i);
             return fail("dw_tma");
         }
     }
@@ -506,15 +449,11 @@ extern "C" SKPS_API int skps_engine_read_buffer(skps_engine* e, int buf, int bat
 }
 extern "C" SKPS_API int skps_engine_launches_per_forward(const skps_engine* e) { return e ? e->launches : 0; }
 extern "C" SKPS_API int skps_engine_launches_for_batch(const skps_engine* e, int batch) {
-    if (!e) return 0;
-    long long n = 0;
-    for (const auto& sg : e->segments) {
-        long long per_sweep = 0;
-        for (int i = sg.first; i < sg.end; ++i)      // the TMA fused-upsample op is two kernels (up-sampled part + skip part)
-            per_sweep += (e->ops[i].type == OP_UPCAT_DW && e->upt[i].valid) ? 2 : 1;
-        n += per_sweep * ((batch + sg.chunk - 1) / sg.chunk);
-    }
-    return (int)n;
+    if (!e || batch <= 0) return 0;
+    int n = 0;
+    for (size_t i = 0; i < e->ops.size(); ++i)      // the TMA fused-upsample op is two kernels (up-sampled part + skip part)
+        n += (e->ops[i].type == OP_UPCAT_DW && e->upt[i].valid) ? 2 : 1;
+    return n;
 }
 
 extern "C" SKPS_API int skps_engine_run_op(skps_engine* e, int op_index, int batch, void* stream) {
@@ -526,16 +465,16 @@ extern "C" SKPS_API int skps_engine_run_op(skps_engine* e, int op_index, int bat
 
 // Enqueue the op sequence (through a cached CUDA graph when possible).
 static int enqueue(skps_engine* e, int batch, cudaStream_t s) {
-    if (!e->use_graph || s == nullptr) return run_forward(e, batch, s);   // the legacy default stream cannot be captured
+    if (!e->use_graph || s == nullptr) return run_ops(e, batch, s);   // the legacy default stream cannot be captured
     const int key = batch * 2 + (e->f32_mode ? 1 : 0);
     auto it = e->graphs.find(key);
     if (it == e->graphs.end()) {
         cudaStreamCaptureStatus st;
         SKPS_CUDA(cudaStreamIsCapturing(s, &st));
-        if (st != cudaStreamCaptureStatusNone) return run_forward(e, batch, s);   // already inside a capture
+        if (st != cudaStreamCaptureStatusNone) return run_ops(e, batch, s);   // already inside a capture
         cudaGraph_t g = nullptr;
         SKPS_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-        int rc = run_forward(e, batch, s);
+        int rc = run_ops(e, batch, s);
         cudaError_t ce = cudaStreamEndCapture(s, &g);
         if (rc) { if (g) cudaGraphDestroy(g); return rc; }
         SKPS_CUDA(ce);

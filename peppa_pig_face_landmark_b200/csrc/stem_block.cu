@@ -11,12 +11,10 @@
 // tensor, everything in between lives in shared memory.  The work is ~1.2 M FMAs per tile on tensors with 3 / 16 input
 // channels.  The stem, the block-0 depthwise and its 16->16 pointwise run on the FP32 pipes with every dense weight taken from
 // the kernel-parameter (constant) bank (FFMA with a constant operand, each activation read from shared memory once per 16
-// outputs); the 16->E expansion - half of the FMAs - is a single wgmma K-step per 128 window pixels (TC variant below,
-// the default; SKPS_STEM_TC=0 keeps it on the FP32 pipes); the next tile's input window is prefetched into registers.
+// outputs); the 16->E expansion - half of the FMAs - is a single wgmma K-step per 128 window pixels; the next tile's input
+// window is prefetched into registers.
 #include <cuda_fp16.h>
 #include <string.h>
-
-#include <stdlib.h>
 
 #include "common.h"
 #include "stem_block.h"
@@ -33,16 +31,14 @@ constexpr int SB_PS = 20;                                  // floats per pixel i
 constexpr int SB_NE = SB_EH * SB_EW, SB_NS = SB_SH * SB_SW, SB_NI = SB_IH * SB_IW;
 constexpr int SB_A_FLOATS = (SB_NI * 4 > SB_NE * SB_PS) ? SB_NI * 4 : SB_NE * SB_PS;    // input window, later block-0 depthwise output
 constexpr int SB_B_FLOATS = SB_NS * SB_PS;                 // stem output, later one 16-channel chunk of the expanded tensor
-constexpr int SB_C_FLOATS = SB_NE * SB_PS;                 // block-0 output
-constexpr int SB_SMEM = (SB_A_FLOATS + SB_B_FLOATS + SB_C_FLOATS + 10 * SB_MAX_E + 256) * 4;
-// Tensor-core variant (TC = true): the 16 -> E expansion (half of the block's FMAs) is ONE wgmma K-step.  S3 writes the
-// block-0 output as float16 hi/lo rows (64-byte swizzled rows of which only the first 32 bytes = 16 channels are used) instead
-// of float32, five 128-row MMA tiles cover the 561 window pixels, per 16-channel chunk the accumulators live in registers and S4
-// shrinks to wgmma -> bias/ReLU/mask -> shared memory.  Same fp16 hi/lo three-product scheme as conv_tc.cu.
+// The 16 -> E expansion (half of the block's FMAs) is ONE wgmma K-step.  S3 writes the block-0 output as float16 hi/lo rows
+// (64-byte swizzled rows of which only the first 32 bytes = 16 channels are used), five 128-row MMA tiles cover the 561
+// window pixels, per 16-channel chunk the accumulators live in registers and S4 is wgmma -> bias/ReLU/mask -> shared
+// memory.  Same fp16 hi/lo three-product scheme as conv_tc.cu.
 constexpr int SB_T_TILES = (SB_NE + 127) / 128;            // 5
 constexpr int SB_T_PLANE = SB_T_TILES * 128 * 64;          // one plane of the A operand: 640 rows x 64 B
 constexpr int SB_WB_PLANE = SB_MAX_E * 64;                 // one plane of the B operand: E rows x 64 B
-constexpr int SB_SMEM_TC = (SB_A_FLOATS + SB_B_FLOATS + 10 * SB_MAX_E + 256) * 4 + 1024 + 2 * SB_T_PLANE + 2 * SB_WB_PLANE;
+constexpr int SB_SMEM = (SB_A_FLOATS + SB_B_FLOATS + 10 * SB_MAX_E + 256) * 4 + 1024 + 2 * SB_T_PLANE + 2 * SB_WB_PLANE;
 
 // 8 floats -> 16 bytes of float16 hi and 16 bytes of float16 lo (v = hi + lo)
 __device__ __forceinline__ void split8(const float* v, uint4& hi, uint4& lo) {
@@ -112,17 +108,16 @@ __device__ __forceinline__ void pw16in(const float* __restrict__ x, const float*
         for (int j = 0; j < 16; ++j) acc[j] = fmaf(in[ci], w[ci * CO + OFF + j], acc[j]);
 }
 
-template <int E, bool TC>
+template <int E>
 __global__ void __launch_bounds__(SB_THREADS, 1)
 stem_block_kernel(const StemBlockK p, const __grid_constant__ StemBlockW Wt) {
     extern __shared__ __align__(16) float sm[];
     __shared__ float s_wmax[SB_THREADS / 32];
     float* sA = sm;                                    // input window (float4 per pixel: b, g, r, 0), later s2
     float* sB = sA + SB_A_FLOATS;                      // stem output s1, later the expanded chunk
-    float* sC = sB + SB_B_FLOATS;                      // block-0 output s3 (float32 variant only)
-    float* sW = TC ? sC : sC + SB_C_FLOATS;            // stride-2 depthwise weights [9][E] + bias [E]
+    float* sW = sB + SB_B_FLOATS;                      // stride-2 depthwise weights [9][E] + bias [E]
     float* lut = sW + 10 * SB_MAX_E;                   // i / 255
-    // TC: A operand (block-0 output as fp16 hi/lo rows), then the B operand (expand weights), 1024-byte aligned
+    // A operand (block-0 output as fp16 hi/lo rows), then the B operand (expand weights), 1024-byte aligned
     const uint32_t sT = (smem_u32(lut + 256) + 1023u) & ~1023u;
     const uint32_t sWB = sT + 2u * SB_T_PLANE;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -130,35 +125,32 @@ stem_block_kernel(const StemBlockK p, const __grid_constant__ StemBlockW Wt) {
     for (int i = tid; i < 10 * E; i += SB_THREADS) sW[i] = p.dw1[i];
     const int tiles_x = p.Wq / SB_TW, tiles_per_img = tiles_x * (p.Hq / SB_TH);
     const int Hh = p.H / 2, Wh = p.W / 2;              // half-resolution map
-    float w_inv = 1.f;
-    if (TC) {
-        // expand weights -> fp16 hi/lo B operand [E rows][16 K], pre-multiplied by an exact power of two (undone after the
-        // MMA) so that the lo parts stay in float16's normal range, as plan.pack_tc_weights does for the other layers
-        float wm = 0.f;
-        for (int i = tid; i < 16 * E; i += SB_THREADS) wm = fmaxf(wm, fabsf(Wt.pw1_w[i]));
+    // expand weights -> fp16 hi/lo B operand [E rows][16 K], pre-multiplied by an exact power of two (undone after the
+    // MMA) so that the lo parts stay in float16's normal range, as plan.pack_tc_weights does for the other layers
+    float wm = 0.f;
+    for (int i = tid; i < 16 * E; i += SB_THREADS) wm = fmaxf(wm, fabsf(Wt.pw1_w[i]));
 #pragma unroll
-        for (int o = 16; o; o >>= 1) wm = fmaxf(wm, __shfl_xor_sync(0xffffffffu, wm, o));
-        if (lane == 0) s_wmax[warp] = wm;
-        __syncthreads();
-        wm = 0.f;
+    for (int o = 16; o; o >>= 1) wm = fmaxf(wm, __shfl_xor_sync(0xffffffffu, wm, o));
+    if (lane == 0) s_wmax[warp] = wm;
+    __syncthreads();
+    wm = 0.f;
 #pragma unroll
-        for (int i = 0; i < SB_THREADS / 32; ++i) wm = fmaxf(wm, s_wmax[i]);
-        const int s_exp = wm > 0.f ? ilogbf(8192.f / wm) : 0;
-        const float w_scale = ldexpf(1.f, s_exp);
-        w_inv = ldexpf(1.f, -s_exp);
-        if (tid < 2 * E) {
-            const int co = tid >> 1, c = tid & 1;
-            float v[8];
+    for (int i = 0; i < SB_THREADS / 32; ++i) wm = fmaxf(wm, s_wmax[i]);
+    const int s_exp = wm > 0.f ? ilogbf(8192.f / wm) : 0;
+    const float w_scale = ldexpf(1.f, s_exp);
+    const float w_inv = ldexpf(1.f, -s_exp);
+    if (tid < 2 * E) {
+        const int co = tid >> 1, c = tid & 1;
+        float v[8];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = Wt.pw1_w[(8 * c + j) * E + co] * w_scale;
-            uint4 hi, lo;
-            split8(v, hi, lo);
-            const uint32_t a = sWB + (uint32_t)co * 64u + (uint32_t)((c ^ ((co >> 1) & 3)) << 4);
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(hi.x), "r"(hi.y), "r"(hi.z), "r"(hi.w) : "memory");
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a + (uint32_t)SB_WB_PLANE), "r"(lo.x), "r"(lo.y), "r"(lo.z), "r"(lo.w) : "memory");
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        for (int j = 0; j < 8; ++j) v[j] = Wt.pw1_w[(8 * c + j) * E + co] * w_scale;
+        uint4 hi, lo;
+        split8(v, hi, lo);
+        const uint32_t a = sWB + (uint32_t)co * 64u + (uint32_t)((c ^ ((co >> 1) & 3)) << 4);
+        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(hi.x), "r"(hi.y), "r"(hi.z), "r"(hi.w) : "memory");
+        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a + (uint32_t)SB_WB_PLANE), "r"(lo.x), "r"(lo.y), "r"(lo.z), "r"(lo.w) : "memory");
     }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
 
     // uint8 input: the 39 x 71 window of the NEXT tile is fetched into registers (packed b | g << 8 | r << 16 | valid << 24,
@@ -283,84 +275,64 @@ stem_block_kernel(const StemBlockK p, const __grid_constant__ StemBlockW Wt) {
             for (int g = 0; g < 4; ++g) {
                 const float4 rv = *reinterpret_cast<const float4*>(res + 4 * g);
                 acc[4 * g] += rv.x; acc[4 * g + 1] += rv.y; acc[4 * g + 2] += rv.z; acc[4 * g + 3] += rv.w;
-                if (!TC) *reinterpret_cast<float4*>(sC + px * SB_PS + 4 * g) = make_float4(acc[4 * g], acc[4 * g + 1], acc[4 * g + 2], acc[4 * g + 3]);
             }
-            if (TC) {
-                // row px of the A operand: logical 16-byte chunk c (8 channels) sits at chunk c ^ ((px / 2) % 4) of the 64-byte row
+            // row px of the A operand: logical 16-byte chunk c (8 channels) sits at chunk c ^ ((px / 2) % 4) of the 64-byte row
 #pragma unroll
-                for (int c2 = 0; c2 < 2; ++c2) {
-                    uint4 hi, lo;
-                    split8(acc + 8 * c2, hi, lo);
-                    const uint32_t a = sT + (uint32_t)px * 64u + (uint32_t)((c2 ^ ((px >> 1) & 3)) << 4);
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(hi.x), "r"(hi.y), "r"(hi.z), "r"(hi.w) : "memory");
-                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a + (uint32_t)SB_T_PLANE), "r"(lo.x), "r"(lo.y), "r"(lo.z), "r"(lo.w) : "memory");
-                }
+            for (int c2 = 0; c2 < 2; ++c2) {
+                uint4 hi, lo;
+                split8(acc + 8 * c2, hi, lo);
+                const uint32_t a = sT + (uint32_t)px * 64u + (uint32_t)((c2 ^ ((px >> 1) & 3)) << 4);
+                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(hi.x), "r"(hi.y), "r"(hi.z), "r"(hi.w) : "memory");
+                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a + (uint32_t)SB_T_PLANE), "r"(lo.x), "r"(lo.y), "r"(lo.z), "r"(lo.w) : "memory");
             }
         }
-        if (TC) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
         // ---- S4/S5 per 16-channel chunk of the expanded tensor: 1x1 16->E + ReLU into sB, then depthwise 3x3 s2 + ReLU
         if (!p.in_f32 && tile + (int)gridDim.x < p.n_tiles) prefetch(tile + gridDim.x);     // in flight during S4 / S5
         const int y_ok0 = max(0, -ey0), y_ok1 = min(SB_EH, Hh - ey0), x_ok0 = max(0, -ex0), x_ok1 = min(SB_EW, Wh - ex0);
 #pragma unroll
         for (int ch = 0; ch < E / 16; ++ch) {
-            if (TC) {
-                // warpgroup g < 4 multiplies MMA tile g (window pixels 128g ..) by the 16 expand weights of chunk ch, warpgroup 0
-                // also tile 4; each thread then writes its accumulator fragment (rows 64h + 16w + lane/4 (+8), columns
-                // 8i + 2(lane%4) (+1)) through bias / ReLU / mask straight into sB
-                const int wg = warp >> 2, w = warp & 3;
-                if (wg < 4) {
-                    const uint64_t b_hi = make_smem_desc_sw64(sWB + (uint32_t)(ch * 16 * 64));
-                    const uint64_t b_lo = make_smem_desc_sw64(sWB + (uint32_t)SB_WB_PLANE + (uint32_t)(ch * 16 * 64));
-                    float acc[2][16];
-                    wg_fence();
+            // warpgroup g < 4 multiplies MMA tile g (window pixels 128g ..) by the 16 expand weights of chunk ch, warpgroup 0
+            // also tile 4; each thread then writes its accumulator fragment (rows 64h + 16w + lane/4 (+8), columns
+            // 8i + 2(lane%4) (+1)) through bias / ReLU / mask straight into sB
+            const int wg = warp >> 2, w = warp & 3;
+            if (wg < 4) {
+                const uint64_t b_hi = make_smem_desc_sw64(sWB + (uint32_t)(ch * 16 * 64));
+                const uint64_t b_lo = make_smem_desc_sw64(sWB + (uint32_t)SB_WB_PLANE + (uint32_t)(ch * 16 * 64));
+                float acc[2][16];
+                wg_fence();
 #pragma unroll
-                    for (int t = 0; t < 2; ++t) {
-                        const int m = t ? 4 : wg;
-                        if (t && wg) break;
+                for (int t = 0; t < 2; ++t) {
+                    const int m = t ? 4 : wg;
+                    if (t && wg) break;
 #pragma unroll
-                        for (int h = 0; h < 2; ++h) {
-                            const uint32_t ao = sT + (uint32_t)m * 8192u + (uint32_t)h * 4096u;
-                            const uint64_t a_hi = make_smem_desc_sw64(ao), a_lo = make_smem_desc_sw64(ao + (uint32_t)SB_T_PLANE);
-                            wgmma_n16(acc[t] + 8 * h, a_lo, b_hi, 0u);
-                            wgmma_n16(acc[t] + 8 * h, a_hi, b_lo, 1u);
-                            wgmma_n16(acc[t] + 8 * h, a_hi, b_hi, 1u);
-                        }
+                    for (int h = 0; h < 2; ++h) {
+                        const uint32_t ao = sT + (uint32_t)m * 8192u + (uint32_t)h * 4096u;
+                        const uint64_t a_hi = make_smem_desc_sw64(ao), a_lo = make_smem_desc_sw64(ao + (uint32_t)SB_T_PLANE);
+                        wgmma_n16(acc[t] + 8 * h, a_lo, b_hi, 0u);
+                        wgmma_n16(acc[t] + 8 * h, a_hi, b_lo, 1u);
+                        wgmma_n16(acc[t] + 8 * h, a_hi, b_hi, 1u);
                     }
-                    wg_commit();
-                    wg_wait0();
+                }
+                wg_commit();
+                wg_wait0();
 #pragma unroll
-                    for (int t = 0; t < 2; ++t) {
-                        const int m = t ? 4 : wg;
-                        if (t && wg) break;
+                for (int t = 0; t < 2; ++t) {
+                    const int m = t ? 4 : wg;
+                    if (t && wg) break;
 #pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            const int h = j >> 3, i = (j >> 2) & 1, e = j & 3;
-                            const int px = 128 * m + 64 * h + 16 * w + (lane >> 2) + 8 * (e >> 1);
-                            const int co = 8 * i + 2 * (lane & 3) + (e & 1);
-                            if (px < SB_NE) {
-                                const int r = px / SB_EW, c = px - r * SB_EW;
-                                const bool inside = r >= y_ok0 && r < y_ok1 && c >= x_ok0 && c < x_ok1;
-                                sB[px * SB_PS + co] = inside ? fmaxf(fmaf(acc[t][j], w_inv, Wt.pw1_b[ch * 16 + co]), 0.f) : 0.f;
-                            }
+                    for (int j = 0; j < 16; ++j) {
+                        const int h = j >> 3, i = (j >> 2) & 1, e = j & 3;
+                        const int px = 128 * m + 64 * h + 16 * w + (lane >> 2) + 8 * (e >> 1);
+                        const int co = 8 * i + 2 * (lane & 3) + (e & 1);
+                        if (px < SB_NE) {
+                            const int r = px / SB_EW, c = px - r * SB_EW;
+                            const bool inside = r >= y_ok0 && r < y_ok1 && c >= x_ok0 && c < x_ok1;
+                            sB[px * SB_PS + co] = inside ? fmaxf(fmaf(acc[t][j], w_inv, Wt.pw1_b[ch * 16 + co]), 0.f) : 0.f;
                         }
                     }
                 }
-            } else
-            for (int px = tid; px < SB_NE; px += SB_THREADS) {
-                const int r = px / SB_EW, c = px - r * SB_EW;
-                float acc[16];
-                if (ch == 0) pw16in<E, 0>(sC + px * SB_PS, Wt.pw1_w, Wt.pw1_b, acc);
-                else if (ch == 1) pw16in<E, 16>(sC + px * SB_PS, Wt.pw1_w, Wt.pw1_b, acc);
-                else if (ch == 2) pw16in<E, 32>(sC + px * SB_PS, Wt.pw1_w, Wt.pw1_b, acc);
-                else pw16in<E, 48>(sC + px * SB_PS, Wt.pw1_w, Wt.pw1_b, acc);
-                // zero outside the half-resolution map: the stride-2 depthwise's padding
-                const bool inside = r >= y_ok0 && r < y_ok1 && c >= x_ok0 && c < x_ok1;
-#pragma unroll
-                for (int g = 0; g < 4; ++g)
-                    *reinterpret_cast<float4*>(sB + px * SB_PS + 4 * g) = inside
-                        ? make_float4(fmaxf(acc[4 * g], 0.f), fmaxf(acc[4 * g + 1], 0.f), fmaxf(acc[4 * g + 2], 0.f), fmaxf(acc[4 * g + 3], 0.f))
-                        : make_float4(0.f, 0.f, 0.f, 0.f);
             }
             __syncthreads();
             // depthwise 3x3 stride 2: item = (output pixel, 4-channel group) = 128 x 4 = 512 items
@@ -393,16 +365,13 @@ bool stem_block_supported(int H, int W, int E, const TView& out) {
 }
 
 int stem_block_launch(const StemBlockK& k, const StemBlockW& w, int num_sms, cudaStream_t s) {
-    static int use_tc = -1;
-    if (use_tc < 0) {
-        const char* e = getenv("SKPS_STEM_TC");
-        use_tc = (e && e[0] == '0') ? 0 : 1;
-        SKPS_CUDA(cudaFuncSetAttribute(stem_block_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SB_SMEM));
-        SKPS_CUDA(cudaFuncSetAttribute(stem_block_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SB_SMEM_TC));
+    static bool attr_set = false;
+    if (!attr_set) {
+        SKPS_CUDA(cudaFuncSetAttribute(stem_block_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SB_SMEM));
+        attr_set = true;
     }
     const int grid = k.n_tiles < num_sms ? k.n_tiles : num_sms;
-    if (use_tc) stem_block_kernel<64, true><<<grid, SB_THREADS, SB_SMEM_TC, s>>>(k, w);
-    else stem_block_kernel<64, false><<<grid, SB_THREADS, SB_SMEM, s>>>(k, w);
+    stem_block_kernel<64><<<grid, SB_THREADS, SB_SMEM, s>>>(k, w);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }

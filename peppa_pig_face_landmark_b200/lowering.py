@@ -17,7 +17,7 @@ plan.py.  Patterns handled:
   yolov5-face Detect tail (face_detector graph nodes 502-820)                       -> OP_DET_DECODE
   heat-map arg-max tail (kps graph nodes 201-410; model.py:511-554)                 -> OP_HM_DECODE
 
-Post passes over the plan (each one a function below, each switchable by an environment variable for A/B runs):
+Post passes over the plan (each one a function below):
   _fuse_upsample_concat_dw   Resize(linear x2) -> Concat -> depthwise 3x3            -> OP_UPCAT_DW (no up-sampled tensor)
   _fold_affine_into_producers BatchNorm(+ReLU) over a Concat of conv outputs (ASPP)  -> folded into the producing convs
   _fuse_se_chain             depthwise -> GAP -> FC -> FC (squeeze-excite)           -> per-tile sums in the depthwise + OP_SE_FC
@@ -28,8 +28,6 @@ Post passes over the plan (each one a function below, each switchable by an envi
 Kernel selection for a dense conv happens in the engine (csrc/engine.cu): transposed wgmma kernel (conv_tct.cu) when
 Cout fills the 128 accumulator rows, transposed arg-max head (conv_hm.cu), pixels-as-rows kernel (conv_tc.cu) otherwise.
 """
-import os
-
 import numpy as np
 
 from . import plan as P
@@ -193,9 +191,6 @@ _ACT_AFTER = {"Relu": P.ACT_RELU}
 class _Lowerer:
     def __init__(self, graph, name, in_hw, input_u8=True, use_tc=True):
         self.use_tc = use_tc
-        # stride-2 convs ride on TMA element strides (csrc/conv_tc.cu); SKPS_TC_STRIDE2=0 sends them back to the CUDA-core kernel
-        self.pw_small = os.environ.get("SKPS_PW_SMALL", "1") != "0"
-        self.tc_strides = (1,) if os.environ.get("SKPS_TC_STRIDE2", "1") == "0" else (1, 2)
         self.g = graph
         self.plan = P.Plan(name)
         self.nodes = graph.nodes
@@ -541,7 +536,7 @@ class _Lowerer:
 
     def _mma_eligible(self, xin, out_v, k, s, p, d, flags, gate):
         """csrc/conv_mma.cu: 3x3 stride-1 'same' convs with Cin == Cout in {24, 40} reading a SPLIT16-able view."""
-        if not self.use_tc or os.environ.get("SKPS_CONV_MMA", "1") == "0" or (flags & P.FLAG_IN_U8) or gate is not None:
+        if not self.use_tc or (flags & P.FLAG_IN_U8) or gate is not None:
             return False
         if list(k) != [3, 3] or list(s) != [1, 1] or list(d) != [1, 1] or list(p[:2]) != [1, 1]:
             return False
@@ -559,10 +554,11 @@ class _Lowerer:
         (16-byte rows of float16)."""
         if not self.use_tc or (flags & P.FLAG_IN_U8) or xin.buf.dtype == P.DT_U8:
             return False
-        if self.pw_small and list(k) == [1, 1] and list(s) == [1, 1] and cout == 16 and xin.C <= 32 \
+        if list(k) == [1, 1] and list(s) == [1, 1] and cout == 16 and xin.C <= 32 \
                 and xin.H * xin.W >= 1024 and gate is None:
             return False          # HBM-bound thin pointwise layer: csrc/ops_misc.cu pw_small_kernel (CUDA cores)
-        if s[0] != s[1] or s[0] not in self.tc_strides or k[0] != k[1] or d[0] != d[1] or p[0] != p[1] \
+        # stride-2 convs ride on TMA element strides
+        if s[0] != s[1] or s[0] not in (1, 2) or k[0] != k[1] or d[0] != d[1] or p[0] != p[1] \
                 or p[0] != d[0] * (k[0] - 1) // 2:
             return False
         if xin.c_stride != 1 or xin.C % 8 or xin.c_off % 8 or xin.buf.C % 8:
@@ -572,17 +568,15 @@ class _Lowerer:
         H, W = xin.H // s[0], xin.W // s[0]              # output map: 128-pixel tiles = row blocks, or whole images
         if W < 8:
             return False
-        if H * W < 128:                                  # several whole images per tile (SKPS_TC_SMALL=0: CUDA-core kernel)
-            return 128 % W == 0 and 128 % (H * W) == 0 and os.environ.get("SKPS_TC_SMALL", "1") != "0"
+        if H * W < 128:                                  # several whole images per tile
+            return 128 % W == 0 and 128 % (H * W) == 0
         if (W % 128 == 0) if W >= 128 else (128 % W == 0 and H % (128 // W) == 0):
             return True
-        # any other map: ragged bw x 128/bw tiles (mirrors csrc/conv_tc.cu tc_pick_bw); SKPS_TC_ANY_W=0 turns them off
-        return os.environ.get("SKPS_TC_ANY_W", "1") != "0" and any(bw <= W + 7 and 128 // bw <= H + 7 for bw in (64, 32, 16, 8))
+        # any other map: ragged bw x 128/bw tiles (mirrors csrc/conv_tc.cu tc_pick_bw)
+        return any(bw <= W + 7 and 128 // bw <= H + 7 for bw in (64, 32, 16, 8))
 
     def _xf_scale_ok(self, xin, gate, out_v, k, s, cout):
         """Mirror of csrc/conv_xf.cu xf_supported() for XF_SCALE: 1x1 stride-1 conv, one N tile, 16x8 pixel tiles."""
-        if os.environ.get("SKPS_XF", "1") == "0" or os.environ.get("SKPS_XF_SCALE", "1") == "0":
-            return False
         if list(k) != [1, 1] or list(s) != [1, 1] or P.tc_tiling(cout)[1] != 1:
             return False
         if gate.c_stride != 1 or (gate.buf.C | gate.c_off) % 4 or gate.buf.dtype != P.DT_F32:
@@ -614,7 +608,7 @@ class _Lowerer:
             out_t = self.t[f["out"]]
             hm_split = None
             if groups == 1 and list(k) == [1, 1] and self._is_hm_head(f["out"]) and gate is None \
-                    and os.environ.get("SKPS_HM_SPLIT", "1") != "0" and w.shape[0] % 3 == 0 and b is not None:
+                    and w.shape[0] % 3 == 0 and b is not None:
                 # heat-map head (model.py:511-554 postp): only the score maps are needed densely; the x/y offset maps are
                 # read at ONE pixel per landmark (the arg-max), so the conv computes the first third of its channels and the
                 # decode kernel evaluates the two offset dot products at that pixel from the conv's input
@@ -853,7 +847,6 @@ def _fuse_upsample_concat_dw(pl):
         d.type = P.OP_UPCAT_DW
         x.buf.name += ":skip-only"         # the first `cu` channels of this buffer are never written any more
         d.ins = [low, P.View(x.buf, cu, 1, x.C - cu)]
-        d.extra = P.upcat_effective_weights(d.w[:, :cu])      # low-res stencil weights per output row/column class
         pl.ops.remove(u)
 
 
@@ -925,9 +918,6 @@ def _fuse_dw_pw(pl):
     output has no other reader: transform warps of csrc/conv_xf.cu build the conv's A tiles in shared memory, the
     depthwise output never reaches HBM.  MobileNetV3 blocks without squeeze-excite (kps_student.onnx blocks.0.0, 1.1,
     3.1-3.3: conv_dw -> conv_pw[l]) and both DecoderBlock heads (model.py:133-196)."""
-    if os.environ.get("SKPS_XF", "1") == "0" or os.environ.get("SKPS_XF_DW", "1") == "0":
-        return
-
     def same(a, b):
         return a is not None and b is not None and a.buf is b.buf and (a.c_off, a.c_stride, a.C) == (b.c_off, b.c_stride, b.C)
 
@@ -989,7 +979,7 @@ def _fuse_stem_block(pl):
     depthwise 3x3 s2 + ReLU: the whole full-resolution head of the mobilenetv3 encoder (kps_student.onnx conv_stem,
     blocks.0.0, blocks.1.0/conv_pw + conv_dw) becomes ONE CUDA-core kernel (csrc/stem_block.cu); the 16- and 64-channel
     full-resolution tensors never reach HBM."""
-    if os.environ.get("SKPS_STEM_BLOCK", "1") == "0" or len(pl.ops) < 4:
+    if len(pl.ops) < 4:
         return
     c0, b0, c1, d1 = pl.ops[0], pl.ops[1], pl.ops[2], pl.ops[3]
 
@@ -1038,8 +1028,6 @@ def _fuse_hm_partial(pl):
     """Heat-map head: the decode (model.py:511-554 postp) needs only the maximum and first arg-max of every score map, so the
     head conv's epilogue reduces each 128-pixel tile to (max, pixel index) per channel and the map itself is never stored
     (436 MB per 256-face batch written and read back otherwise).  Split-head plans only (scores separate from offsets)."""
-    if os.environ.get("SKPS_HM_PART", "1") == "0":
-        return
     for dec in pl.ops:
         if dec.type != P.OP_HM_DECODE or len(dec.ins) < 2 or dec.ins[1] is None:
             continue
@@ -1057,7 +1045,7 @@ def _fuse_hm_partial(pl):
         # 256-pixel row-block tiles run on the transposed head kernel (csrc/conv_hm.cu: channels as accumulator rows, the
         # arg-max is a per-thread scan); other shapes keep conv_tc's 128-pixel tiles and its reduce-scatter epilogue
         cin = hm.ins[0].C
-        wide = (os.environ.get("SKPS_HM_T", "1") != "0" and 8 <= W <= 256 and 256 % W == 0 and (H * W) % 256 == 0
+        wide = (8 <= W <= 256 and 256 % W == 0 and (H * W) % 256 == 0
                 and cin % 8 == 0 and cin <= 128 and hm.ints[1] == 1)
         pb = pl.new_buf(2 * ldp, (H * W) // (256 if wide else 128), 1, P.DT_F32, hm.name + ":tile_max")
         pv = P.View(pb, 0, 1, 2 * ldp)
@@ -1071,9 +1059,6 @@ def _fuse_gap_sse(pl):
     """scSE attention (model.py:117-130; DecoderBlock attention2): cSE = sigmoid(FC(relu(FC(mean(x))))) and sSE = sigmoid(conv1x1(x))
     both start with a full pass over x.  One kernel (OP_GAP_SSE) reads x once and writes per-tile channel sums and the sSE map;
     the cSE MLP becomes the squeeze-excite FC kernel on those sums (OP_SE_FC).  Replaces GlobalAveragePool + 3 convs."""
-    if os.environ.get("SKPS_GAP_SSE", "1") == "0":
-        return
-
     def same(a, b):
         return a is not None and b is not None and a.buf is b.buf and (a.c_off, a.c_stride, a.C) == (b.c_off, b.c_stride, b.C)
 
@@ -1135,8 +1120,6 @@ def _fold_affine_into_producers(pl):
     (rows of W and the bias scaled, the ReLU becomes the conv's activation) and the pass over the 256-channel tensor
     disappears.  A nearest-resize producer (the broadcast pooled branch, itself conv+ReLU) gets the affine on its 1x1 source
     tensor instead."""
-    if os.environ.get("SKPS_FOLD_AFFINE", "1") == "0":
-        return
     for a in list(pl.ops):
         if a.type != P.OP_AFFINE_ACT or a.act not in (P.ACT_NONE, P.ACT_RELU):
             continue
@@ -1203,17 +1186,13 @@ def lower(onnx_path, in_hw, name=None, input_u8=True, use_tc=True):
     lw.emit()
     _fuse_upsample_concat_dw(lw.plan)
     _fold_affine_into_producers(lw.plan)
-    if os.environ.get("SKPS_SE_FUSE", "1") != "0":
-        _fuse_se_chain(lw.plan)
+    _fuse_se_chain(lw.plan)
     if use_tc:
         _fuse_dw_pw(lw.plan)
         if input_u8:
             _fuse_stem_block(lw.plan)
         _fuse_hm_partial(lw.plan)
         _fuse_gap_sse(lw.plan)
-    chunk_env = os.environ.get("SKPS_L2_CHUNK_MB", "0")   # sub-batch sweeps, off by default
-    if chunk_env not in ("0", ""):
-        lw.plan.plan_segments(l2_budget=int(chunk_env) << 20)
     if not lw.plan.outputs:
         raise LoweringError("no outputs produced for %s" % onnx_path)
     return lw.plan

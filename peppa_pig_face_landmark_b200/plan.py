@@ -115,8 +115,7 @@ DW_TILE_W = 16
 
 def dw_tile_rows(k, s):
     """Output rows per tile of csrc/dw_tma.cu (rows of the per-tile channel-sum buffer): 16 for 5x5 stride-1 layers, else 8."""
-    import os
-    return 16 if (k == 5 and s == 1 and os.environ.get("SKPS_DW_ROWS2", "1") != "0") else 8
+    return 16 if (k == 5 and s == 1) else 8
 
 
 class Plan:
@@ -127,7 +126,6 @@ class Plan:
         self.input = None        # View of the network input (uint8 NHWC)
         self.outputs = []        # Views of the outputs
         self.macs = 0            # conv MACs per sample (algorithmic work)
-        self.segments = []       # [(first_op, end_op, chunk)]: ops first..end-1 run chunk samples at a time (L2 residency)
 
     def new_buf(self, C, H, W, dtype=DT_F32, name=""):
         b = Buf(len(self.bufs), C, H, W, dtype, name)
@@ -203,56 +201,16 @@ class Plan:
         header = np.array([0x534B5053, 1, len(self.bufs), len(self.ops),
                            self.input.buf.idx, len(self.outputs)] +
                           [v.buf.idx for v in self.outputs] + [0] * (2 - len(self.outputs)), np.int32)
-        segs = self.segments or [(0, len(self.ops), 1 << 20)]
-        assert segs[0][0] == 0 and segs[-1][1] == len(self.ops) and all(a[1] == b[0] for a, b in zip(segs, segs[1:]))
-        tail = [len(segs)] + [int(v) for sg in segs for v in sg]
-        words = np.concatenate([header, np.array(bw, np.int32), np.array(ow, np.int32), np.array(tail, np.int32)])
+        words = np.concatenate([header, np.array(bw, np.int32), np.array(ow, np.int32)])
         return words, blob
 
     def bytes_per_sample(self, op):
-        """Activation bytes one sample moves through `op` (inputs + outputs), for chunk sizing."""
+        """Activation bytes one sample moves through `op` (inputs + outputs), for traffic estimates."""
         tot = 0
         for v in list(op.ins) + list(op.outs):
             if v is not None:
                 tot += v.C * v.buf.H * v.buf.W * (1 if v.buf.dtype == DT_U8 else 4)
         return tot
-
-    def plan_segments(self, l2_budget=96 << 20, full=256):
-        """Group consecutive ops into segments that run `chunk` samples at a time so that what one op writes is
-        still in L2 (50 MB on H100) when the next op reads it.  Per op: chunk = power of two with
-        chunk * (bytes the op moves per sample) <= l2_budget, but never so small that a launch has fewer than
-        ~2 CTAs per SM (128-pixel tiles); ops moving < 256 KB per sample (SE vectors, FCs) adopt their
-        neighbours' chunk."""
-        def pow2floor(v):
-            return 1 << (max(1, int(v)).bit_length() - 1)
-
-        want, low = [], []
-        for op in self.ops:
-            ws = self.bytes_per_sample(op)
-            o = op.outs[0]
-            if ws < (256 << 10) or o.buf.H * o.buf.W == 1:
-                want.append(full)        # chunk-neutral: runs inside whatever sweep its neighbours use
-                low.append(1)
-                continue
-            tiles = max(1, o.buf.H * o.buf.W // 128)
-            lo = 1
-            while lo * tiles < 296 and lo < full:
-                lo *= 2
-            low.append(lo)
-            want.append(min(full, max(lo, pow2floor(l2_budget // ws))))
-        # a segment sweeps the whole batch before the next one starts, so residency only exists inside a segment:
-        # grow each segment while one chunk size satisfies every member (small enough for L2, large enough for the SMs)
-        merged, first, cur, cur_lo = [], 0, want[0], low[0]
-        for i in range(1, len(self.ops)):
-            c, l = min(cur, want[i]), max(cur_lo, low[i])
-            if c >= l:
-                cur, cur_lo = c, l
-            else:
-                merged.append((first, i, cur))
-                first, cur, cur_lo = i, want[i], low[i]
-        merged.append((first, len(self.ops), cur))
-        self.segments = merged
-        return merged
 
 
 # ---- tensor-core (wgmma) convolution support ---------------------------------------------------
@@ -300,7 +258,7 @@ def upcat_effective_weights(w9c):
     low[clamp(y//2 + a - 1)][clamp(x//2 + b - 1)].  Classes: 0 = first row/col (the conv's zero padding removes
     tap 0), 1 = even, 2 = odd, 3 = last row/col (tap 2 removed).  Per dimension U[2m] = .25 L[m-1] + .75 L[m],
     U[2m+1] = .75 L[m] + .25 L[m+1] with edge-clamped indices (model.py:176 F.interpolate(scale_factor=2,
-    mode='bilinear'); csrc/dw_tma.cu upcat_eff_kernel)."""
+    mode='bilinear'))."""
     E = np.array([[.75, .25, 0], [.25, .75, 0], [0, .75, .25]])
     O = np.array([[.25, .75, 0], [0, .75, .25], [0, .25, .75]])
     E0, O1 = E.copy(), O.copy()

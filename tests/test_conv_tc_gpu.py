@@ -58,42 +58,27 @@ def _run(N, H, W, Cin, Cout, k, dil, act, with_bias=True, with_res=False, out_sp
     (2, 64, 64, 24, 72, 1, 1, 1),
     (2, 32, 32, 40, 120, 1, 1, 1),
     (5, 32, 32, 120, 40, 1, 1, 0),
+    # 3x3 on 64-wide maps with a residual and split-fp16 output (the residual keeps them off the transposed kernel)
+    (3, 8, 64, 32, 24, 3, 1, 0, dict(with_res=True, out_split=True)),      # 32 channels, ragged Cout
+    (1, 64, 64, 96, 128, 3, 1, 1, dict(with_res=True, out_split=True)),
+    (2, 12, 64, 64, 64, 3, 1, 1, dict(with_res=True, out_split=True)),     # H = 12
+    (2, 64, 64, 128, 128, 3, 1, 2, dict(with_res=True, out_split=True)),
 ])
 def test_conv_tc_matches_fp32(cfg):
-    err = _run(*cfg)
+    err = _run(*cfg[:8], **(cfg[8] if len(cfg) > 8 else {}))
     assert err < 1e-5, (cfg, err)       # hi/lo split ~2^-22 per product + the tensor core's fp32 accumulate over K/16*3 steps
 
 
 @pytest.mark.parametrize("cfg", [
-    # halo-row mode of conv_tc (3x3, 64-wide maps, Cin % 32 == 0): the three ky taps address one staged 6-row box in place
-    (3, 8, 64, 32, 24, 3, 1, 0),         # two 4-row groups per image, one 32-channel half-chunk, ragged Cout
-    (1, 64, 64, 96, 128, 3, 1, 1),       # three half-chunks
-    (2, 12, 64, 64, 64, 3, 1, 1),        # H = 12: three groups, image borders inside the batch
-    (2, 64, 64, 128, 128, 3, 1, 2),
-])
-def test_conv_tc_halo_row_mode(cfg, monkeypatch):
-    monkeypatch.setenv("SKPS_TC_K3", "1")              # opt-in mode (read by tc_prepare at every layer setup)
-    err = _run(*cfg, with_res=True, out_split=True)
-    assert err < 1e-5, (cfg, err)
-
-
-@pytest.mark.parametrize("cfg", [
     # transposed kernel (csrc/conv_tct.cu): channels as accumulator rows, 256 pixels as N; split-fp16 output, no residual
-    (2, 64, 64, 128, 128, 3, 1, 1),      # decoder conv2 (halo-row stages: 6-row boxes)
-    (2, 32, 32, 96, 128, 3, 1, 1),       # halo-row stages with 10-row boxes, three 32-channel halves
+    (2, 64, 64, 128, 128, 3, 1, 1),      # decoder conv2
+    (2, 32, 32, 96, 128, 3, 1, 1),       # 8-row tiles, K tail (96 channels)
     (1, 32, 32, 64, 96, 3, 2, 0),        # dilated, 8-row tiles, Cout < 128 (the last 32-channel quarter is clipped by the store)
     (3, 8, 128, 72, 104, 3, 1, 2),       # two-row tiles, K tail (72 channels), ragged Cout
     (2, 16, 256, 64, 128, 5, 1, 1),      # 5x5, one row per tile
     (3, 16, 16, 160, 128, 3, 2, 1),      # 16-wide map: a tile is a whole image, store boxes of 2 rows x 16 pixels
 ])
 def test_conv_tct_transposed_kernel(cfg):
-    err = _run(*cfg, out_split=True)
-    assert err < 1e-5, (cfg, err)
-
-
-@pytest.mark.parametrize("cfg", [(2, 64, 64, 128, 128, 3, 1, 1), (2, 32, 32, 96, 128, 3, 1, 1)])
-def test_conv_tct_halo_row_stages(cfg, monkeypatch):
-    monkeypatch.setenv("SKPS_TCT_K3", "1")             # opt-in stage layout (read by tct_prepare at every layer setup)
     err = _run(*cfg, out_split=True)
     assert err < 1e-5, (cfg, err)
 

@@ -21,7 +21,7 @@ TOL_PX, TOL_SCORE = 1e-2, 5e-3            # fp32 execution (plan interpreter, CU
 # on the CPU with every tensor-core conv's operands rounded to the stored fp16 hi/lo planes and exact accumulation and lands
 # at 1.6e-3 px (fp32 execution: 3.6e-3 px) - but the tensor core's fp32 accumulation: each 16-term product block is added
 # into the accumulator with its own rounding, and the three-product scheme makes 3*K/16 adds per output (216 at K = 1152,
-# bounded per conv by test_conv_tc_matches_fp32); 100 layers of random weights amplify that to a few 1e-2 px.  The legacy mma.sync kernel is not the cause (SKPS_CONV_MMA=0: same numbers).
+# bounded per conv by test_conv_tc_matches_fp32); 100 layers of random weights amplify that to a few 1e-2 px.  The legacy mma.sync kernel is not the cause (its layers on the other kernels: same numbers).
 TOL_PX_TC, TOL_SCORE_TC = 6e-2, 2e-2
 
 

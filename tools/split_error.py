@@ -4,7 +4,6 @@ fp64, and compared with the fp64 oracle and with plain fp32 execution:  python t
 import os, sys
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
-os.environ["SKPS_XF"] = "0"               # plain conv ops (the interpreter's emulation hook sits on OP_CONV)
 import numpy as np
 import torch
 from peppa_pig_face_landmark_b200 import lowering
