@@ -108,28 +108,32 @@ conv_hm_kernel(const __grid_constant__ CUtensorMap tmX_hi, const __grid_constant
         int xb = 0;
         for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
             const int img_l = tile / p.tiles_per_img, t = tile - img_l * p.tiles_per_img;
-            float accv[4][32];
+            float acc[128];                            // acc[64 m + 4 i + e]: rows 64m + 16q + lane/4 + 8(e/2), column 8i + ...
+            int prev = 0;
             for (int kc = 0; kc < p.cchunks; ++kc) {
                 mbar_wait(smem_u32(&full_bar[stage]), phase);
                 const uint32_t sx = x_off + (uint32_t)stage * 2u * HM_X_TILE + (uint32_t)(half_id * 128 * 128);
                 const uint64_t w_hi = make_smem_desc(w_off + (uint32_t)(kc * 2) * HM_W_TILE);
                 const uint64_t w_lo = make_smem_desc(w_off + (uint32_t)(kc * 2 + 1) * HM_W_TILE);
-                const int ksteps = min(4, (p.Cin - kc * 64 + 15) / 16);
-                wg_fence();
-#pragma unroll
-                for (int ci = 0; ci < 4; ++ci) {
-                    const uint64_t x_hi = make_smem_desc(sx + (uint32_t)(ci * 32 * 128));
-                    const uint64_t x_lo = make_smem_desc(sx + (uint32_t)(ci * 32 * 128) + HM_X_TILE);
-                    for (int k = 0; k < ksteps; ++k) {
-                        const uint64_t koff = (uint64_t)(k * 32 >> 4);
-                        wg_mma3_128x32(accv[ci], w_hi + koff, w_lo + koff, 64u * 128u, x_hi + koff, x_lo + koff, (kc | k) != 0);
-                    }
+                const uint64_t x_hi = make_smem_desc(sx), x_lo = make_smem_desc(sx + HM_X_TILE);
+                const uint32_t accumulate = kc != 0;
+                wg_fence_acc(acc);
+                switch (min(4, (p.Cin - kc * 64 + 15) / 16)) {   // 16-channel steps that hold real channels; uniform
+                    case 4: wg_fence(); wg_mma3_128x128<4>(acc, w_hi, w_lo, x_hi, x_lo, accumulate); wg_commit(); break;
+                    case 3: wg_fence(); wg_mma3_128x128<3>(acc, w_hi, w_lo, x_hi, x_lo, accumulate); wg_commit(); break;
+                    case 2: wg_fence(); wg_mma3_128x128<2>(acc, w_hi, w_lo, x_hi, x_lo, accumulate); wg_commit(); break;
+                    default: wg_fence(); wg_mma3_128x128<1>(acc, w_hi, w_lo, x_hi, x_lo, accumulate); wg_commit(); break;
                 }
-                wg_commit();
-                wg_wait0();
-                if (lane == 0) mbar_arrive(smem_u32(&empty_bar[stage]));
+                wg_fence_acc(acc);
+                wg_wait<1>();                          // the previous chunk's group has finished reading its stage
+                wg_fence_acc(acc);
+                if (kc > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+                prev = stage;
                 if (++stage == HM_STAGES) { stage = 0; phase ^= 1u; }
             }
+            wg_wait<0>();
+            wg_fence_acc(acc);
+            if (lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
             // running (max, first arg-max) per channel row over this thread's columns, in increasing column order
             float best[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
             int bi[4] = {0x7fffffff, 0x7fffffff, 0x7fffffff, 0x7fffffff};
@@ -142,7 +146,7 @@ conv_hm_kernel(const __grid_constant__ CUtensorMap tmX_hi, const __grid_constant
 #pragma unroll
                         for (int m = 0; m < 2; ++m) {
                             const int r = 2 * m + (e >> 1);
-                            const float sc = fmaf(accv[ci][16 * m + 4 * i + e], p.out_scale, bias[r]);  // as conv_tc forms it
+                            const float sc = fmaf(acc[64 * m + 16 * ci + 4 * i + e], p.out_scale, bias[r]);  // as conv_tc forms it
                             const bool take = sc > best[r];                 // strict: ties keep the earlier pixel
                             best[r] = take ? sc : best[r];
                             bi[r] = take ? half_id * 128 + ci * 32 + 8 * i + 2 * (lane & 3) + (e & 1) : bi[r];

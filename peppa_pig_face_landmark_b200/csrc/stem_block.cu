@@ -301,22 +301,27 @@ stem_block_kernel(const StemBlockK p, const __grid_constant__ StemBlockW Wt) {
                 const uint64_t b_hi = make_smem_desc_sw64(sWB + (uint32_t)(ch * 16 * 64));
                 const uint64_t b_lo = make_smem_desc_sw64(sWB + (uint32_t)SB_WB_PLANE + (uint32_t)(ch * 16 * 64));
                 float acc[2][16];
-                wg_fence();
-#pragma unroll
-                for (int t = 0; t < 2; ++t) {
-                    const int m = t ? 4 : wg;
-                    if (t && wg) break;
+                // straight-line issue per warpgroup role (a branch inside the group would serialise the wgmma)
+                auto mma_tile = [&](float* d, int m) {
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         const uint32_t ao = sT + (uint32_t)m * 8192u + (uint32_t)h * 4096u;
-                        const uint64_t a_hi = make_smem_desc_sw64(ao), a_lo = make_smem_desc_sw64(ao + (uint32_t)SB_T_PLANE);
-                        wgmma_n16(acc[t] + 8 * h, a_lo, b_hi, 0u);
-                        wgmma_n16(acc[t] + 8 * h, a_hi, b_lo, 1u);
-                        wgmma_n16(acc[t] + 8 * h, a_hi, b_hi, 1u);
+                        wg_mma3<16>(d + 8 * h, make_smem_desc_sw64(ao), make_smem_desc_sw64(ao + (uint32_t)SB_T_PLANE), b_hi,
+                                    b_lo, 0u);
                     }
+                };
+                if (wg == 0) {
+                    wg_fence();
+                    mma_tile(acc[0], 0);
+                    mma_tile(acc[1], 4);
+                    wg_commit();
+                    wg_wait0();
+                } else {
+                    wg_fence();
+                    mma_tile(acc[0], wg);
+                    wg_commit();
+                    wg_wait0();
                 }
-                wg_commit();
-                wg_wait0();
 #pragma unroll
                 for (int t = 0; t < 2; ++t) {
                     const int m = t ? 4 : wg;

@@ -2,9 +2,11 @@
 // TMA, wgmma and its shared-memory matrix descriptors.  sm_90a.
 //
 // The accumulator of a 128-row tile lives in the registers of the warpgroup that issues the wgmma instructions: one
-// m64nNk16 per 64-row half, so a warp holds rows 16w..16w+15 of each half.  The epilogues want one row per thread
-// (row 32q + lane of warp q, 32 consecutive columns); wg_rows32 moves a 128 x 32 block into that layout through 16 KB
-// of shared memory.
+// m64nNk16 per 64-row half, so a warp holds rows 16w..16w+15 of each half.
+// conv_tct, conv_hm and stem_block issue wgmma_f16<N> / wg_mma3<N> from straight-line code, keep a group in flight with
+// wg_wait<1> where they pipeline, and read the accumulator fragment directly in their epilogues.
+// conv_tc and conv_xf still issue wg_mma3_128x32 per 32-column chunk and hand each chunk to a one-row-per-thread epilogue
+// layout (row 32q + lane of warp q, 32 consecutive columns) with wg_rows32, through 16 KB of shared memory.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -103,6 +105,82 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw64(uint32_t addr) {
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Waits until at most N committed wgmma groups of this warpgroup are still in flight.
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Pins the accumulator registers in place around asynchronous wgmma: without it the compiler may move or copy them while a
+// group that writes them is still in flight.
+template <int R>
+__device__ __forceinline__ void wg_fence_acc(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, fp16 inputs from shared memory (both K-major), fp32 accumulate in registers:
+// d[4 i + e] = element (16 w + lane/4 + 8 (e/2), 8 i + 2 (lane%4) + e%2) for warp w of the warpgroup.
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wgmma_f16<16>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7"
+        "}, %8, %9, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void wgmma_f16<128>(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, %64, %65, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+
+// One K-step of the hi/lo three-product scheme on a 64 x N accumulator: lo*hi, hi*lo, then hi*hi (small terms first).
+template <int N>
+__device__ __forceinline__ void wg_mma3(float* acc, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo,
+                                        uint32_t accumulate) {
+    wgmma_f16<N>(acc, a_lo, b_hi, accumulate);
+    wgmma_f16<N>(acc, a_hi, b_lo, 1u);
+    wgmma_f16<N>(acc, a_hi, b_hi, 1u);
+}
+
+// KS K-steps of 16 of the three-product scheme on a 128 x 128 accumulator held by one warpgroup: acc[0..63] = A rows 0-63,
+// acc[64..127] = A rows 64-127 (128-byte-swizzled K-major A, row 64 at +8 KB).  Straight-line, so the wgmma stay asynchronous.
+template <int KS>
+__device__ __forceinline__ void wg_mma3_128x128(float* acc, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo,
+                                                uint32_t accumulate) {
+    constexpr uint64_t A_HALF = 64 * 128 >> 4;
+#pragma unroll
+    for (int k = 0; k < KS; ++k) {
+        const uint64_t koff = (uint64_t)(k * 32 >> 4);     // 16 fp16 = 32 bytes along K
+#pragma unroll
+        for (int m = 0; m < 2; ++m)
+            wg_mma3<128>(acc + 64 * m, a_hi + m * A_HALF + koff, a_lo + m * A_HALF + koff, b_hi + koff, b_lo + koff,
+                         k ? 1u : accumulate);
+    }
+}
 
 // D[64 x 32] (+)= A[64 x 16] * B[32 x 16]^T, fp16 inputs from shared memory (both K-major), fp32 accumulate in registers.
 __device__ __forceinline__ void wgmma_n32(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
@@ -117,19 +195,6 @@ __device__ __forceinline__ void wgmma_n32(float* d, uint64_t adesc, uint64_t bde
           "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
         : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// D[64 x 16] (+)= A[64 x 16] * B[16 x 16]^T
-__device__ __forceinline__ void wgmma_n16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %10, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t"
-        "}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-        : "l"(adesc), "l"(bdesc), "r"(accumulate));
-}
-
 // One K-step of the hi/lo three-product scheme on a 128 x 32 block: acc[0..15] = rows 0-63, acc[16..31] = rows 64-127.
 // a_* address the 128-row A tile, a_half the byte distance between its row 0 and row 64.  Small terms first, then hi*hi.
 __device__ __forceinline__ void wg_mma3_128x32(float* acc, uint64_t a_hi, uint64_t a_lo, uint32_t a_half, uint64_t b_hi,
