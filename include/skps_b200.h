@@ -297,6 +297,26 @@ SKPS_API int skps_mpipe_set_align(skps_mpipe* p, int size);
  * M [host] (n, top_k, 2, 3) float64, n = that submit's stream count; entries i >= n_faces[s] are undefined. */
 SKPS_API int skps_mpipe_align_results(skps_mpipe* p, int slot, uint8_t* chips, double* M);
 
+/* ---- Head pose of every face (csrc/headpose.cu; additive) ---------------------------------------------------------------
+ * get_head_pose of the training tree (TRAIN/face_landmark/lib/dataset/headpose.py:48-78) on the 98 WFLW landmarks: the 10
+ * landmarks [33, 37, 42, 46, 60, 64, 68, 72, 55, 59], rounded to float32, paired with the model points of pose.py, the
+ * camera [[W,0,W//2],[0,W,H//2],[0,0,1]] of the face's frame; the same solver as skps_head_pose, one warp per face.
+ * Outputs float64: rvec, tvec, euler (degrees, in the order cv2.decomposeProjectionMatrix returns) (3,) and the 8
+ * re-projected cube corners (8,2) per face. */
+/* FaceAna, whose landmarks are smoothed on the host: kps [host] (n,n_points,2) float64, H x W the frame they belong to;
+ * rvec, tvec, euler [host] (n,3), reproject [host] (n,8,2).  n <= top_k.  Buffers are allocated on the first call; the work
+ * is ordered on `stream`, and the call returns once that stream has reached it.  Synchronous. */
+SKPS_API int skps_pipeline_pose(skps_pipeline* p, const double* kps, int n, int H, int W, double* rvec, double* tvec,
+                                double* euler, double* reproject, void* stream);
+/* FaceAnaStreams: on != 0 makes every following skps_mpipe_submit solve the pose of every returned face from the smoothed
+ * float64 landmarks, with each stream's own frame size, on the compute stream without a host synchronisation; the results
+ * are copied back with the slot's other results.  on = 0 switches it off and frees the buffers (n_streams x top_k x 200
+ * bytes on the device and twice that pinned on the host).  No batch may be in flight. */
+SKPS_API int skps_mpipe_set_pose(skps_mpipe* p, int on);
+/* After skps_mpipe_wait(slot), for a slot submitted with pose on: rvec, tvec, euler [host] (n, top_k, 3) and reproject
+ * [host] (n, top_k, 8, 2) float64, n = that submit's stream count; entries i >= n_faces[s] are undefined. */
+SKPS_API int skps_mpipe_pose_results(skps_mpipe* p, int slot, double* rvec, double* tvec, double* euler, double* reproject);
+
 #ifdef __cplusplus
 }
 #endif

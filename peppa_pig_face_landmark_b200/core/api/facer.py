@@ -29,11 +29,15 @@ def get_cfg():
 
 
 class FaceAna():
-    def __init__(self, verbose=False, top_k=None, max_frame_hw=(2160, 3840), align=None):
+    def __init__(self, verbose=False, top_k=None, max_frame_hw=(2160, 3840), align=None, pose=False):
         """align: None, or a chip side in 16..512: every result dict then also carries 'chip' ((align, align, 3) uint8
         BGR, the face warped to the ArcFace five-point template) and 'M' ((2, 3) float64, the frame -> chip matrix for
-        cv2.warpAffine), computed on the GPU from the returned 'kps' and the frame already in HBM (core/api/align.py)."""
+        cv2.warpAffine), computed on the GPU from the returned 'kps' and the frame already in HBM (core/api/align.py).
+        pose: every result dict then also carries 'pose': {'euler': (3,), 'rvec': (3,), 'tvec': (3,), 'reproject': (8, 2)},
+        float64, Euler angles in degrees - head_poses(kps[None], frame.shape[:2], points=POSE_POINTS_98) of the returned
+        'kps', solved on the GPU."""
         self.align = None if align is None else check_size(align)
+        self.pose = bool(pose)
         if verbose:
             logger.setLevel(logging.DEBUG)
         cfg = get_cfg()
@@ -127,7 +131,21 @@ class FaceAna():
         res = self.to_dict(self.track_box, landmarks, states)
         if self.align is not None and res:
             self._add_chips(res)
+        if self.pose and res:
+            self._add_pose(res, H, W)
         return res
+
+    def _add_pose(self, res, H, W):
+        """'pose' for every face, from its returned 'kps' promoted to float64 (skps_pipeline_pose)."""
+        n = len(res)
+        kps = np.ascontiguousarray(np.stack([np.asarray(r['kps'], np.float64) for r in res]))
+        out = {k: np.empty((n, 3), np.float64) for k in ('rvec', 'tvec', 'euler')}
+        out['reproject'] = np.empty((n, 8, 2), np.float64)
+        rt.check(self.lib.skps_pipeline_pose(self._pipe, kps.ctypes.data, n, H, W, out['rvec'].ctypes.data,
+                                             out['tvec'].ctypes.data, out['euler'].ctypes.data,
+                                             out['reproject'].ctypes.data, self._stream.cuda_stream))
+        for i, r in enumerate(res):
+            r['pose'] = {k: v[i] for k, v in out.items()}
 
     def _add_chips(self, res):
         """'chip' and 'M' for every face, from its returned 'kps' promoted to float64 (skps_pipeline_align)."""

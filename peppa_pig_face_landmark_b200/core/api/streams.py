@@ -8,6 +8,7 @@ device (csrc/mpipe.cu, csrc/temporal.cu) and two batches can be in flight so tha
     fa = FaceAnaStreams(n_streams=16, top_k=4)
     results = fa.run(frames)            # list of S lists of {'box','kps','scores'} - what S FaceAna.run calls return
     # FaceAnaStreams(..., align=112): each dict also has 'chip' (112x112x3 uint8, aligned) and 'M' (2x3 float64)
+    # FaceAnaStreams(..., pose=True): each dict also has 'pose' {'euler', 'rvec', 'tvec', 'reproject'} as FaceAna returns it
     # or, overlapped:
     fa.submit(frames_t0); fa.submit(frames_t1); r0 = fa.collect(); fa.submit(frames_t2); r1 = fa.collect(); ...
 """
@@ -24,10 +25,13 @@ from .onnx_model_base import ONNXEngine
 
 
 class FaceAnaStreams:
-    def __init__(self, n_streams, top_k=None, max_frame_hw=(2160, 3840), device="cuda", align=None):
+    def __init__(self, n_streams, top_k=None, max_frame_hw=(2160, 3840), device="cuda", align=None, pose=False):
         """align: None, or a chip side in 16..512: every result dict then also carries 'chip' and 'M' as FaceAna(align=...)
-        returns them, warped inside the same submit on the device from the smoothed landmarks and the frame in the ring."""
+        returns them, warped inside the same submit on the device from the smoothed landmarks and the frame in the ring.
+        pose: every result dict then also carries 'pose' as FaceAna(pose=True) returns it, solved inside the same submit
+        from the smoothed landmarks, with each stream's own frame size for the camera."""
         self.align = None if align is None else check_size(align)
+        self.pose = bool(pose)
         cfg = get_cfg()['Skps']
         det_cfg, kps_cfg, tr_cfg = cfg['Detect'], cfg['Keypoints'], cfg['Trace']
         self.n_streams = int(n_streams)
@@ -54,6 +58,11 @@ class FaceAnaStreams:
             for o in self._out:
                 o["chips"] = np.zeros((S, K, self.align, self.align, 3), np.uint8)
                 o["M"] = np.zeros((S, K, 2, 3), np.float64)
+        if self.pose:
+            rt.check(self.lib.skps_mpipe_set_pose(h, 1))
+            for o in self._out:
+                o["pose"] = {k: np.zeros((S, K, 3), np.float64) for k in ("rvec", "tvec", "euler")}
+                o["pose"]["reproject"] = np.zeros((S, K, 8, 2), np.float64)
         self._pending = []              # [(slot, n, keep-alive frames)]
         self._next = 0
         self.last_ran_detector = None
@@ -102,6 +111,10 @@ class FaceAnaStreams:
         self.last_ran_detector = o["det"][:n].astype(bool)
         if self.align is not None:
             rt.check(self.lib.skps_mpipe_align_results(self._h, slot, o["chips"].ctypes.data, o["M"].ctypes.data))
+        if self.pose:
+            q = o["pose"]
+            rt.check(self.lib.skps_mpipe_pose_results(self._h, slot, q["rvec"].ctypes.data, q["tvec"].ctypes.data,
+                                                      q["euler"].ctypes.data, q["reproject"].ctypes.data))
         res = []
         for s in range(n):
             k = int(o["n"][s])
@@ -111,6 +124,9 @@ class FaceAnaStreams:
                 for i, r in enumerate(res[-1]):
                     r['chip'] = o["chips"][s, i].copy()
                     r['M'] = o["M"][s, i].copy()
+            if self.pose:
+                for i, r in enumerate(res[-1]):
+                    r['pose'] = {k: v[s, i].copy() for k, v in o["pose"].items()}
         return res
 
     def run(self, frames):

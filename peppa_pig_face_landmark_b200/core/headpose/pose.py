@@ -6,7 +6,8 @@
 its size is used: camera matrix [[w,0,w//2],[0,w,h//2],[0,0,1]], no distortion).  The reference calls cv2.solvePnP,
 cv2.projectPoints, cv2.Rodrigues and cv2.decomposeProjectionMatrix per face; here the whole batch is solved by one CUDA
 kernel (csrc/headpose.cu: DLT start + Levenberg-Marquardt in float64, OpenCV's RQ-based Euler angles).  Additive:
-`head_poses(shapes, (h, w))` for many faces at once, returning rotation/translation vectors too."""
+`head_poses(shapes, (h, w))` for many faces at once, returning rotation/translation vectors too, and
+`head_poses(shapes98, (h, w), points=POSE_POINTS_98)` for the 98-point landmarks the shipped model returns."""
 import numpy as np
 
 from ... import runtime as rt
@@ -34,17 +35,25 @@ line_pairs = [[0, 1], [1, 2], [2, 3], [3, 0],
               [4, 5], [5, 6], [6, 7], [7, 4],
               [0, 4], [1, 5], [2, 6], [3, 7]]
 POSE_POINTS = [17, 21, 22, 26, 36, 39, 42, 45, 31, 35]
+# The same ten points in the 98-point WFLW convention of the shipped landmark model: the reference's training tree solves
+# the head pose on these (TRAIN/face_landmark/lib/dataset/headpose.py:64-65), and its Euler angles are the pose targets the
+# network was trained with.  FaceAna(pose=True) and FaceAnaStreams(pose=True) use them.
+POSE_POINTS_98 = [33, 37, 42, 46, 60, 64, 68, 72, 55, 59]
 
 
-def head_poses(shapes, img_hw):
-    """shapes: (N, >=46, 2) landmark sets (68-point convention) -> dict of float64 arrays
+def head_poses(shapes, img_hw, points=POSE_POINTS):
+    """shapes: (N, P, 2) landmark sets; `points` are the 10 landmarks paired with object_pts (POSE_POINTS for 68-point
+    shapes, POSE_POINTS_98 for 98-point ones) -> dict of float64 arrays
     rvec (N,3), tvec (N,3), euler (N,3) in degrees [pitch, yaw, roll as cv2 orders them], reproject (N,8,2)."""
     rt.require_cuda()
     lib = rt.load_library()
     shapes = np.asarray(shapes)
-    if shapes.ndim != 3 or shapes.shape[1] <= max(POSE_POINTS) or shapes.shape[2] != 2:
-        raise ValueError("expected (N, 68, 2) landmark sets, got %s" % (shapes.shape,))
-    pts = np.ascontiguousarray(shapes[:, POSE_POINTS, :], dtype=np.float32)
+    points = [int(i) for i in points]
+    if len(points) != len(object_pts) or min(points) < 0:
+        raise ValueError("expected %d non-negative landmark indices, got %s" % (len(object_pts), points))
+    if shapes.ndim != 3 or shapes.shape[1] <= max(points) or shapes.shape[2] != 2:
+        raise ValueError("expected (N, >%d, 2) landmark sets, got %s" % (max(points), shapes.shape))
+    pts = np.ascontiguousarray(shapes[:, points, :], dtype=np.float32)
     n = pts.shape[0]
     h, w = int(img_hw[0]), int(img_hw[1])
     out = {"rvec": np.zeros((n, 3)), "tvec": np.zeros((n, 3)), "euler": np.zeros((n, 3)), "reproject": np.zeros((n, 8, 2))}

@@ -3,14 +3,18 @@
 //   cv2.solvePnP(object_pts, image_pts, K, 0)  -> (rvec, tvec)     [SOLVEPNP_ITERATIVE: DLT start + Levenberg-Marquardt]
 //   cv2.projectPoints(reprojectsrc, ...)       -> 8 cube corners
 //   cv2.Rodrigues + cv2.decomposeProjectionMatrix -> Euler angles in degrees
-// One thread per face, float64.  The start value follows OpenCV's (direct linear transform on normalised image points,
+// One warp per face, float64.  The start value follows OpenCV's (direct linear transform on normalised image points,
 // rotation = orthogonal polar factor), the refinement minimises the pixel reprojection error over (rvec, tvec) with
 // Levenberg-Marquardt until the step is below 1e-12 - i.e. the same local minimum OpenCV's 20-iteration solver approaches;
 // agreement with cv2 is checked in tests/test_headpose_gpu.py (tolerance stated there).
+// The lanes share the parallel parts: the 12x12 normal matrix, the row / column updates of every Jacobi rotation, the 12
+// residual evaluations of the numeric Jacobian, J^T J / J^T e and the 6x6 elimination.  Every sum runs in a fixed order
+// (the one-thread solver's, except the Jacobi stopping test), so a face's pose does not depend on the other faces of a launch.
 #include <math.h>
 
 #include "../../include/skps_b200.h"
 #include "common.h"
+#include "mpipe_kernels.h"
 
 namespace skps {
 
@@ -59,57 +63,11 @@ __device__ void inv3T(const double* M, double* O) {        // O = (M^-1)^T
     O[6] = (M[1] * M[5] - M[2] * M[4]) * d; O[7] = (M[2] * M[3] - M[0] * M[5]) * d; O[8] = (M[0] * M[4] - M[1] * M[3]) * d;
 }
 
-// smallest eigenvector of a symmetric 12x12 matrix (cyclic Jacobi); A is destroyed
-__device__ void smallest_eigvec12(double* A, double* V, double* out) {
-    for (int i = 0; i < 144; ++i) V[i] = (i % 13 == 0) ? 1.0 : 0.0;
-    for (int sweep = 0; sweep < 30; ++sweep) {
-        double off = 0;
-        for (int p = 0; p < 12; ++p) for (int q = p + 1; q < 12; ++q) off += A[p * 12 + q] * A[p * 12 + q];
-        if (off < 1e-30) break;
-        for (int p = 0; p < 12; ++p)
-            for (int q = p + 1; q < 12; ++q) {
-                const double apq = A[p * 12 + q];
-                if (fabs(apq) < 1e-300) continue;
-                const double th = (A[q * 12 + q] - A[p * 12 + p]) / (2 * apq);
-                const double t = (th >= 0 ? 1.0 : -1.0) / (fabs(th) + sqrt(th * th + 1));
-                const double c = 1 / sqrt(t * t + 1), s = t * c;
-                for (int k = 0; k < 12; ++k) {
-                    const double akp = A[k * 12 + p], akq = A[k * 12 + q];
-                    A[k * 12 + p] = c * akp - s * akq; A[k * 12 + q] = s * akp + c * akq;
-                }
-                for (int k = 0; k < 12; ++k) {
-                    const double apk = A[p * 12 + k], aqk = A[q * 12 + k];
-                    A[p * 12 + k] = c * apk - s * aqk; A[q * 12 + k] = s * apk + c * aqk;
-                }
-                for (int k = 0; k < 12; ++k) {
-                    const double vkp = V[k * 12 + p], vkq = V[k * 12 + q];
-                    V[k * 12 + p] = c * vkp - s * vkq; V[k * 12 + q] = s * vkp + c * vkq;
-                }
-            }
-    }
-    int m = 0;
-    for (int i = 1; i < 12; ++i) if (A[i * 12 + i] < A[m * 12 + m]) m = i;
-    for (int k = 0; k < 12; ++k) out[k] = V[k * 12 + m];
-}
-
 __device__ void project(const double* R, const double* t, const float* X, double f, double cx, double cy, double* uv) {
     const double x = R[0] * X[0] + R[1] * X[1] + R[2] * X[2] + t[0];
     const double y = R[3] * X[0] + R[4] * X[1] + R[5] * X[2] + t[1];
     const double z = R[6] * X[0] + R[7] * X[1] + R[8] * X[2] + t[2];
     uv[0] = f * x / z + cx; uv[1] = f * y / z + cy;
-}
-
-__device__ double residual(const double* p, const float* obj, const double* img, double f, double cx, double cy, double* e) {
-    double R[9];
-    rodrigues(p, R);
-    double s = 0;
-    for (int i = 0; i < HP_PTS; ++i) {
-        double uv[2];
-        project(R, p + 3, obj + 3 * i, f, cx, cy, uv);
-        e[2 * i] = uv[0] - img[2 * i]; e[2 * i + 1] = uv[1] - img[2 * i + 1];
-        s += e[2 * i] * e[2 * i] + e[2 * i + 1] * e[2 * i + 1];
-    }
-    return s;
 }
 
 // cv::RQDecomp3x3 on a rotation matrix -> Euler angles in degrees (what cv2.decomposeProjectionMatrix returns for [R|t])
@@ -151,37 +109,120 @@ __device__ void euler_rq(const double* Rin, double* eul) {
     eul[2] = ac(Qz[0]) * (Qz[1] >= 0 ? 1 : -1) * deg;
 }
 
-struct HeadPoseK {
-    const float* pts;       // [N][10][2] image points (pixels)
-    const float* obj;       // [10][3] model points
-    const float* cube;      // [8][3] reprojection source
-    int N;
-    float f, cx, cy;        // camera: fx = fy = f (pose.py:50: [w,0,w//2; 0,w,h//2; 0,0,1])
-    double* rvec; double* tvec; double* euler; double* reproj;   // [N][3], [N][3], [N][3], [N][8][2]
-    double* scratch;        // [N][2*144]
+
+constexpr int HP_WARPS = 4;             // faces (warps) per block
+
+// one warp's scratch
+struct PoseSmem {
+    float obj[3 * HP_PTS], cube[24];
+    double img[2 * HP_PTS];             // image points (float32 values)
+    double rows[2][HP_PTS][12];         // the two DLT rows of every point
+    double A[144], V[144];              // normal matrix (diagonalised in place) and its eigenvectors
+    double ep[12][2 * HP_PTS];          // residuals at p + h_j e_j (row 2j) and p - h_j e_j (row 2j+1)
+    double h[6];
+    double J[2 * HP_PTS][6];
+    double JtJ[36], Jte[6];
+    double Mx[6][7];                    // damped normal equations | right-hand side
+    double e[2][2 * HP_PTS];            // residuals at the current and at the trial parameters
 };
 
-__global__ void head_pose_kernel(const HeadPoseK k) {
-    const int n = blockIdx.x * blockDim.x + threadIdx.x;
-    if (n >= k.N) return;
-    const double f = k.f, cx = k.cx, cy = k.cy;
-    double img[2 * HP_PTS];
-    for (int i = 0; i < 2 * HP_PTS; ++i) img[i] = (double)k.pts[(long long)n * 2 * HP_PTS + i];
-    // ---- start value: DLT on normalised image points (OpenCV's non-planar branch), rotation = polar factor
-    double* A = k.scratch + (long long)n * 288;
-    double* V = A + 144;
-    for (int i = 0; i < 144; ++i) A[i] = 0;
-    for (int i = 0; i < HP_PTS; ++i) {
-        const double X = k.obj[3 * i], Y = k.obj[3 * i + 1], Z = k.obj[3 * i + 2];
-        const double x = -(img[2 * i] - cx) / f, y = -(img[2 * i + 1] - cy) / f;
-        const double r0[12] = {X, Y, Z, 1, 0, 0, 0, 0, x * X, x * Y, x * Z, x};
-        const double r1[12] = {0, 0, 0, 0, X, Y, Z, 1, y * X, y * Y, y * Z, y};
-        for (int a = 0; a < 12; ++a) for (int b = 0; b < 12; ++b) A[a * 12 + b] += r0[a] * r0[b] + r1[a] * r1[b];
+// Butterfly sum: the two lanes of a pair add the same two values, so every lane ends with the same bits.
+__device__ __forceinline__ double warp_sum(double v) {
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+// Squared reprojection error at p; lanes 0..9 write the residuals of point `lane` to e, every lane returns the sum.
+__device__ double warp_residual(const PoseSmem& S, const double* p, double f, double cx, double cy, double* e, int lane) {
+    double R[9];
+    rodrigues(p, R);
+    if (lane < HP_PTS) {
+        double uv[2];
+        project(R, p + 3, S.obj + 3 * lane, f, cx, cy, uv);
+        e[2 * lane] = uv[0] - S.img[2 * lane]; e[2 * lane + 1] = uv[1] - S.img[2 * lane + 1];
     }
-    double P[12];
-    smallest_eigvec12(A, V, P);
-    double RR[9] = {P[0], P[1], P[2], P[4], P[5], P[6], P[8], P[9], P[10]};
-    double tt[3] = {P[3], P[7], P[11]};
+    __syncwarp();
+    double s = 0;
+    for (int i = 0; i < HP_PTS; ++i) s += e[2 * i] * e[2 * i] + e[2 * i + 1] * e[2 * i + 1];
+    return s;
+}
+
+__global__ void __launch_bounds__(HP_WARPS * 32) head_pose_warp_kernel(const PoseArgs a) {
+    __shared__ PoseSmem smem[HP_WARPS];
+    const int lane = threadIdx.x & 31;
+    const int face = blockIdx.x * HP_WARPS + (threadIdx.x >> 5);
+    if (face >= a.G * a.K) return;                  // whole warps leave together
+    const int g = face / a.K;
+    if (a.count && face - g * a.K >= a.count[g]) return;
+    PoseSmem& S = smem[threadIdx.x >> 5];
+    const int H = a.hw ? a.hw[2 * g] : a.H, W = a.hw ? a.hw[2 * g + 1] : a.W;
+    const double f = (float)W, cx = (float)(W / 2), cy = (float)(H / 2);
+    // ---- inputs: the 10 image points rounded to float32 (np.float32(shape[...]) in pose.py), the model
+    if (lane < 2 * HP_PTS) {
+        int id = a.idx[0];
+#pragma unroll
+        for (int q = 1; q < HP_PTS; ++q) if ((lane >> 1) == q) id = a.idx[q];
+        const size_t at = ((size_t)face * a.P + id) * 2 + (lane & 1);
+        S.img[lane] = a.pts64 ? (double)(float)a.pts64[at] : (double)a.pts32[at];
+    }
+    if (lane == 0) {
+#pragma unroll
+        for (int q = 0; q < 3 * HP_PTS; ++q) S.obj[q] = a.obj[q];
+#pragma unroll
+        for (int q = 0; q < 24; ++q) S.cube[q] = a.cube[q];
+    }
+    __syncwarp();
+    // ---- start value: DLT on normalised image points (OpenCV's non-planar branch), rotation = polar factor
+    for (int t = lane; t < HP_PTS * 12; t += 32) {  // row 0: X Y Z 1 0 0 0 0 xX xY xZ x, row 1: 0 0 0 0 X Y Z 1 yX yY yZ y
+        const int i = t / 12, c = t - 12 * i, k = c & 3;
+        const double v = k == 3 ? 1.0 : (double)S.obj[3 * i + k];
+        const double x = -(S.img[2 * i] - cx) / f, y = -(S.img[2 * i + 1] - cy) / f;
+        S.rows[0][i][c] = c < 4 ? v : (c < 8 ? 0.0 : x * v);
+        S.rows[1][i][c] = c < 4 ? 0.0 : (c < 8 ? v : y * v);
+    }
+    __syncwarp();
+    for (int t = lane; t < 144; t += 32) {
+        const int r = t / 12, c = t - 12 * r;
+        double s = 0;
+        for (int i = 0; i < HP_PTS; ++i) s += S.rows[0][i][r] * S.rows[0][i][c] + S.rows[1][i][r] * S.rows[1][i][c];
+        S.A[t] = s;
+        S.V[t] = (t % 13 == 0) ? 1.0 : 0.0;
+    }
+    __syncwarp();
+    // smallest eigenvector of A: cyclic Jacobi, lanes 0..11 rotate rows / columns of A, lanes 12..23 columns of V
+    for (int sweep = 0; sweep < 30; ++sweep) {
+        double off = 0;
+        for (int t = lane; t < 144; t += 32) if (t % 12 > t / 12) off += S.A[t] * S.A[t];
+        if (warp_sum(off) < 1e-30) break;
+        for (int p = 0; p < 12; ++p)
+            for (int q = p + 1; q < 12; ++q) {
+                const double apq = S.A[p * 12 + q];
+                if (fabs(apq) < 1e-300) continue;
+                const double th = (S.A[q * 12 + q] - S.A[p * 12 + p]) / (2 * apq);
+                const double t = (th >= 0 ? 1.0 : -1.0) / (fabs(th) + sqrt(th * th + 1));
+                const double c = 1 / sqrt(t * t + 1), s = t * c;
+                __syncwarp();
+                if (lane < 12) {
+                    const double akp = S.A[lane * 12 + p], akq = S.A[lane * 12 + q];
+                    S.A[lane * 12 + p] = c * akp - s * akq; S.A[lane * 12 + q] = s * akp + c * akq;
+                } else if (lane < 24) {
+                    const int k = lane - 12;
+                    const double vkp = S.V[k * 12 + p], vkq = S.V[k * 12 + q];
+                    S.V[k * 12 + p] = c * vkp - s * vkq; S.V[k * 12 + q] = s * vkp + c * vkq;
+                }
+                __syncwarp();
+                if (lane < 12) {
+                    const double apk = S.A[p * 12 + lane], aqk = S.A[q * 12 + lane];
+                    S.A[p * 12 + lane] = c * apk - s * aqk; S.A[q * 12 + lane] = s * apk + c * aqk;
+                }
+                __syncwarp();
+            }
+    }
+    int m = 0;
+    for (int i = 1; i < 12; ++i) if (S.A[i * 13] < S.A[m * 13]) m = i;
+    double RR[9] = {S.V[m], S.V[12 + m], S.V[24 + m], S.V[48 + m], S.V[60 + m], S.V[72 + m], S.V[96 + m], S.V[108 + m],
+                    S.V[120 + m]};
+    double tt[3] = {S.V[36 + m], S.V[84 + m], S.V[132 + m]};
     if (det3(RR) < 0) { for (int i = 0; i < 9; ++i) RR[i] = -RR[i]; for (int i = 0; i < 3; ++i) tt[i] = -tt[i]; }
     double sc = 0;
     for (int i = 0; i < 9; ++i) sc += RR[i] * RR[i];
@@ -199,62 +240,103 @@ __global__ void head_pose_kernel(const HeadPoseK k) {
     rodrigues_inv(R, p);
     for (int i = 0; i < 3; ++i) p[3 + i] = tt[i] * (sqrt(3.0) / sc);
     // ---- Levenberg-Marquardt on the pixel reprojection error (numeric Jacobian, float64)
-    double e[2 * HP_PTS], e2[2 * HP_PTS], J[2 * HP_PTS][6];
-    double cost = residual(p, k.obj, img, f, cx, cy, e);
+    int cur = 0;                                           // S.e[cur] holds the residuals at p
+    double cost = warp_residual(S, p, f, cx, cy, S.e[0], lane);
     double lambda = 1e-3;
     for (int it = 0; it < 100; ++it) {
-        for (int j = 0; j < 6; ++j) {
-            const double h = 1e-6 * fmax(1.0, fabs(p[j]));
-            double pp[6], pm[6], ep[2 * HP_PTS], em[2 * HP_PTS];
-            for (int q = 0; q < 6; ++q) { pp[q] = p[q]; pm[q] = p[q]; }
-            pp[j] += h; pm[j] -= h;
-            residual(pp, k.obj, img, f, cx, cy, ep);
-            residual(pm, k.obj, img, f, cx, cy, em);
-            for (int i = 0; i < 2 * HP_PTS; ++i) J[i][j] = (ep[i] - em[i]) / (2 * h);
+        if (lane < 12) {                                   // lane 2j / 2j+1: residuals at p + h_j e_j / p - h_j e_j
+            const int j = lane >> 1;
+            double pj = p[0];
+#pragma unroll
+            for (int q = 1; q < 6; ++q) if (q == j) pj = p[q];
+            const double h = 1e-6 * fmax(1.0, fabs(pj));
+            double pp[6];
+#pragma unroll
+            for (int q = 0; q < 6; ++q) pp[q] = q == j ? ((lane & 1) ? p[q] - h : p[q] + h) : p[q];
+            double Rj[9];
+            rodrigues(pp, Rj);
+#pragma unroll
+            for (int i = 0; i < HP_PTS; ++i) {
+                double uv[2];
+                project(Rj, pp + 3, S.obj + 3 * i, f, cx, cy, uv);
+                S.ep[lane][2 * i] = uv[0] - S.img[2 * i]; S.ep[lane][2 * i + 1] = uv[1] - S.img[2 * i + 1];
+            }
+            if (!(lane & 1)) S.h[j] = h;
         }
-        double JtJ[36], Jte[6];
-        for (int a = 0; a < 6; ++a) {
-            Jte[a] = 0;
-            for (int i = 0; i < 2 * HP_PTS; ++i) Jte[a] += J[i][a] * e[i];
-            for (int b = 0; b < 6; ++b) {
-                double s = 0;
-                for (int i = 0; i < 2 * HP_PTS; ++i) s += J[i][a] * J[i][b];
-                JtJ[a * 6 + b] = s;
+        __syncwarp();
+        for (int t = lane; t < 2 * HP_PTS * 6; t += 32) {
+            const int i = t / 6, j = t - 6 * i;
+            S.J[i][j] = (S.ep[2 * j][i] - S.ep[2 * j + 1][i]) / (2 * S.h[j]);
+        }
+        __syncwarp();
+        for (int t = lane; t < 42; t += 32) {              // J^T J (36 lanes' worth) and J^T e (6)
+            double s = 0;
+            if (t < 36) {
+                const int r = t / 6, c = t - 6 * r;
+                for (int i = 0; i < 2 * HP_PTS; ++i) s += S.J[i][r] * S.J[i][c];
+                S.JtJ[t] = s;
+            } else {
+                for (int i = 0; i < 2 * HP_PTS; ++i) s += S.J[i][t - 36] * S.e[cur][i];
+                S.Jte[t - 36] = s;
             }
         }
+        __syncwarp();
         bool improved = false;
         double step = 0;
         for (int tries = 0; tries < 12 && !improved; ++tries) {
-            double Mx[36], rhs[6];
-            for (int i = 0; i < 36; ++i) Mx[i] = JtJ[i];
-            for (int a = 0; a < 6; ++a) { Mx[a * 6 + a] += lambda * fmax(JtJ[a * 6 + a], 1e-12); rhs[a] = -Jte[a]; }
+            for (int t = lane; t < 42; t += 32) {
+                const int r = t / 7, c = t - 7 * r;
+                double v;
+                if (c == 6) {
+                    v = -S.Jte[r];
+                } else {
+                    v = S.JtJ[r * 6 + c];
+                    if (r == c) v += lambda * fmax(v, 1e-12);
+                }
+                S.Mx[r][c] = v;
+            }
+            __syncwarp();
             for (int c = 0; c < 6; ++c) {                  // Gaussian elimination with partial pivoting
                 int piv = c;
-                for (int r = c + 1; r < 6; ++r) if (fabs(Mx[r * 6 + c]) > fabs(Mx[piv * 6 + c])) piv = r;
+                for (int r = c + 1; r < 6; ++r) if (fabs(S.Mx[r][c]) > fabs(S.Mx[piv][c])) piv = r;
+                __syncwarp();
                 if (piv != c) {
-                    for (int q = 0; q < 6; ++q) { const double t = Mx[c * 6 + q]; Mx[c * 6 + q] = Mx[piv * 6 + q]; Mx[piv * 6 + q] = t; }
-                    const double t = rhs[c]; rhs[c] = rhs[piv]; rhs[piv] = t;
+                    if (lane < 7) { const double t = S.Mx[c][lane]; S.Mx[c][lane] = S.Mx[piv][lane]; S.Mx[piv][lane] = t; }
+                    __syncwarp();
                 }
-                const double d = Mx[c * 6 + c];
-                for (int r = c + 1; r < 6; ++r) {
-                    const double m = Mx[r * 6 + c] / d;
-                    for (int q = c; q < 6; ++q) Mx[r * 6 + q] -= m * Mx[c * 6 + q];
-                    rhs[r] -= m * rhs[c];
+                // element (r, q) of the rows below c is t = 7 (r - c - 1) + q: up to 35 of them, so two per lane
+                double v[2];
+#pragma unroll
+                for (int u = 0; u < 2; ++u) {
+                    const int t = lane + 32 * u, r = c + 1 + t / 7, q = t % 7;
+                    if (r < 6 && q >= c) {
+                        const double mr = S.Mx[r][c] / S.Mx[c][c];
+                        v[u] = S.Mx[r][q] - mr * S.Mx[c][q];
+                    }
                 }
+                __syncwarp();
+#pragma unroll
+                for (int u = 0; u < 2; ++u) {
+                    const int t = lane + 32 * u, r = c + 1 + t / 7, q = t % 7;
+                    if (r < 6 && q >= c) S.Mx[r][q] = v[u];
+                }
+                __syncwarp();
             }
             double dx[6];
+#pragma unroll
             for (int r = 5; r >= 0; --r) {
-                double s = rhs[r];
-                for (int q = r + 1; q < 6; ++q) s -= Mx[r * 6 + q] * dx[q];
-                dx[r] = s / Mx[r * 6 + r];
+                double s = S.Mx[r][6];
+#pragma unroll
+                for (int q = r + 1; q < 6; ++q) s -= S.Mx[r][q] * dx[q];
+                dx[r] = s / S.Mx[r][r];
             }
             double pn[6];
             for (int q = 0; q < 6; ++q) pn[q] = p[q] + dx[q];
-            const double c2 = residual(pn, k.obj, img, f, cx, cy, e2);
+            const double c2 = warp_residual(S, pn, f, cx, cy, S.e[cur ^ 1], lane);
             if (c2 <= cost) {
                 step = 0;
                 for (int q = 0; q < 6; ++q) { step += dx[q] * dx[q]; p[q] = pn[q]; }
-                for (int i = 0; i < 2 * HP_PTS; ++i) e[i] = e2[i];
+                cur ^= 1;
                 cost = c2; lambda = fmax(lambda * 0.1, 1e-15); improved = true;
             } else {
                 lambda *= 10;
@@ -265,9 +347,34 @@ __global__ void head_pose_kernel(const HeadPoseK k) {
     // keep the rotation vector in [0, pi] like cv2.Rodrigues(cv2.Rodrigues(r)) would
     rodrigues(p, R);
     rodrigues_inv(R, p);
-    for (int i = 0; i < 3; ++i) { k.rvec[(long long)n * 3 + i] = p[i]; k.tvec[(long long)n * 3 + i] = p[3 + i]; }
-    euler_rq(R, k.euler + (long long)n * 3);
-    for (int i = 0; i < 8; ++i) project(R, p + 3, k.cube + 3 * i, f, cx, cy, k.reproj + ((long long)n * 8 + i) * 2);
+    if (lane == 0) {
+        for (int i = 0; i < 3; ++i) { a.rvec[(size_t)face * 3 + i] = p[i]; a.tvec[(size_t)face * 3 + i] = p[3 + i]; }
+        euler_rq(R, a.euler + (size_t)face * 3);
+    }
+    if (lane < 8) project(R, p + 3, S.cube + 3 * lane, f, cx, cy, a.reproj + ((size_t)face * 8 + lane) * 2);
+}
+
+void pose_model_98(PoseArgs& a) {
+    static const int idx[HP_PTS] = {33, 37, 42, 46, 60, 64, 68, 72, 55, 59};        // headpose.py:64-65
+    // the model points and the cube of Skps/core/headpose/pose.py:22-39
+    static const float obj[3 * HP_PTS] = {6.825897f, 6.760612f, 4.402142f, 1.330353f, 7.122144f, 6.903745f,
+                                          -1.330353f, 7.122144f, 6.903745f, -6.825897f, 6.760612f, 4.402142f,
+                                          5.311432f, 5.485328f, 3.987654f, 1.789930f, 5.393625f, 4.413414f,
+                                          -1.789930f, 5.393625f, 4.413414f, -5.311432f, 5.485328f, 3.987654f,
+                                          2.005628f, 1.409845f, 6.165652f, -2.005628f, 1.409845f, 6.165652f};
+    static const float cube[24] = {10, 10, 10, 10, 10, -10, 10, -10, -10, 10, -10, 10,
+                                   -10, 10, 10, -10, 10, -10, -10, -10, -10, -10, -10, 10};
+    memcpy(a.idx, idx, sizeof(idx));
+    memcpy(a.obj, obj, sizeof(obj));
+    memcpy(a.cube, cube, sizeof(cube));
+}
+
+int launch_head_pose(const PoseArgs& a, cudaStream_t s) {
+    const long long faces = (long long)a.G * a.K;
+    if (faces <= 0) return 0;
+    head_pose_warp_kernel<<<(unsigned)((faces + HP_WARPS - 1) / HP_WARPS), HP_WARPS * 32, 0, s>>>(a);
+    SKPS_CUDA(cudaGetLastError());
+    return 0;
 }
 
 }  // namespace skps
@@ -280,28 +387,28 @@ using namespace skps;
 extern "C" SKPS_API int skps_head_pose(const float* pts, int N, int img_w, int img_h, const float* object_pts,
                                        const float* cube_pts, double* rvec, double* tvec, double* euler, double* reproject) {
     SKPS_CHECK(pts && object_pts && cube_pts && rvec && tvec && euler && reproject && N > 0, "head_pose: bad arguments");
-    float *d_pts = nullptr, *d_obj = nullptr, *d_cube = nullptr;
+    float* d_pts = nullptr;
     double* d_out = nullptr;
-    const size_t outn = (size_t)N * (3 + 3 + 3 + 16 + 288);
-    SKPS_CUDA(cudaMalloc(&d_pts, (size_t)N * 20 * 4));
-    SKPS_CUDA(cudaMalloc(&d_obj, 30 * 4));
-    SKPS_CUDA(cudaMalloc(&d_cube, 24 * 4));
-    SKPS_CUDA(cudaMalloc(&d_out, outn * 8));
-    SKPS_CUDA(cudaMemcpy(d_pts, pts, (size_t)N * 20 * 4, cudaMemcpyHostToDevice));
-    SKPS_CUDA(cudaMemcpy(d_obj, object_pts, 30 * 4, cudaMemcpyHostToDevice));
-    SKPS_CUDA(cudaMemcpy(d_cube, cube_pts, 24 * 4, cudaMemcpyHostToDevice));
-    HeadPoseK k;
-    k.pts = d_pts; k.obj = d_obj; k.cube = d_cube; k.N = N;
-    k.f = (float)img_w; k.cx = (float)(img_w / 2); k.cy = (float)(img_h / 2);
-    k.rvec = d_out; k.tvec = d_out + (size_t)N * 3; k.euler = d_out + (size_t)N * 6; k.reproj = d_out + (size_t)N * 9;
-    k.scratch = d_out + (size_t)N * 25;
-    head_pose_kernel<<<(N + 31) / 32, 32>>>(k);
-    SKPS_CUDA(cudaGetLastError());
-    SKPS_CUDA(cudaDeviceSynchronize());
-    SKPS_CUDA(cudaMemcpy(rvec, k.rvec, (size_t)N * 24, cudaMemcpyDeviceToHost));
-    SKPS_CUDA(cudaMemcpy(tvec, k.tvec, (size_t)N * 24, cudaMemcpyDeviceToHost));
-    SKPS_CUDA(cudaMemcpy(euler, k.euler, (size_t)N * 24, cudaMemcpyDeviceToHost));
-    SKPS_CUDA(cudaMemcpy(reproject, k.reproj, (size_t)N * 128, cudaMemcpyDeviceToHost));
-    cudaFree(d_pts); cudaFree(d_obj); cudaFree(d_cube); cudaFree(d_out);
+    SKPS_CUDA(cudaMalloc(&d_pts, (size_t)N * 2 * HP_PTS * 4));
+    if (cudaMalloc(&d_out, (size_t)N * 25 * 8) != cudaSuccess) {
+        cudaFree(d_pts);
+        SKPS_CHECK(false, "head_pose: cannot allocate the outputs of %d faces", N);
+    }
+    PoseArgs a = {};
+    a.pts32 = d_pts; a.G = 1; a.K = N; a.P = HP_PTS;
+    for (int i = 0; i < HP_PTS; ++i) a.idx[i] = i;
+    a.H = img_h; a.W = img_w;
+    memcpy(a.obj, object_pts, sizeof(a.obj));
+    memcpy(a.cube, cube_pts, sizeof(a.cube));
+    a.rvec = d_out; a.tvec = d_out + (size_t)N * 3; a.euler = d_out + (size_t)N * 6; a.reproj = d_out + (size_t)N * 9;
+    int rc = cudaMemcpy(d_pts, pts, (size_t)N * 2 * HP_PTS * 4, cudaMemcpyHostToDevice) != cudaSuccess ||
+             launch_head_pose(a, 0) ||
+             cudaMemcpy(rvec, a.rvec, (size_t)N * 24, cudaMemcpyDeviceToHost) != cudaSuccess ||
+             cudaMemcpy(tvec, a.tvec, (size_t)N * 24, cudaMemcpyDeviceToHost) != cudaSuccess ||
+             cudaMemcpy(euler, a.euler, (size_t)N * 24, cudaMemcpyDeviceToHost) != cudaSuccess ||
+             cudaMemcpy(reproject, a.reproj, (size_t)N * 128, cudaMemcpyDeviceToHost) != cudaSuccess;
+    const cudaError_t err = cudaGetLastError();
+    cudaFree(d_pts); cudaFree(d_out);
+    SKPS_CHECK(!rc, "head_pose: %s", err == cudaSuccess ? get_error() : cudaGetErrorString(err));
     return 0;
 }

@@ -40,14 +40,19 @@ struct skps_mpipe {
         int32_t* h_count = nullptr; int32_t* h_flag = nullptr; int32_t* h_det_count = nullptr;
         double* h_box = nullptr; double* h_kps = nullptr; float* h_scores = nullptr;
         uint8_t* h_chips = nullptr; double* h_M = nullptr;     // pinned, only while alignment is on
+        double* h_pose = nullptr;             // pinned, only while pose is on: rvec, tvec, euler [n][K][3], reproject [n][K][8][2]
         cudaEvent_t ev_in = nullptr, ev_done = nullptr;
         int n = 0;
         int align = 0;                        // chip size this slot's batch was submitted with (0 = none)
+        bool pose = false;                    // this slot's batch was submitted with pose on
         bool busy = false;
     } slot[2];
     // aligned chips (skps_mpipe_set_align): [S][K][size][size][3] / [S][K][2][3], allocated only while align_size > 0
     int align_size = 0;
     uint8_t* d_chips = nullptr; double* d_align_M = nullptr;
+    // head pose (skps_mpipe_set_pose): [S][K][25] doubles, allocated only while pose_on
+    bool pose_on = false;
+    double* d_pose = nullptr;
     // device scratch (one set: batches are serialised on s_compute)
     int32_t *d_hw = nullptr, *d_have_prev = nullptr, *d_flag = nullptr, *d_det_count = nullptr, *d_det_idx = nullptr;
     int32_t *d_count = nullptr, *d_detail = nullptr;
@@ -77,14 +82,14 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
     for (uint8_t* f : p->d_frame) if (f) cudaFree(f);
     for (auto& sl : p->slot) {
         void* host[] = {sl.h_desc, sl.h_stage, sl.h_hw, sl.h_have_prev, sl.h_geom, sl.h_count, sl.h_flag, sl.h_det_count, sl.h_box,
-                        sl.h_kps, sl.h_scores, sl.h_chips, sl.h_M};
+                        sl.h_kps, sl.h_scores, sl.h_chips, sl.h_M, sl.h_pose};
         for (void* q : host) if (q) cudaFreeHost(q);
         if (sl.ev_in) cudaEventDestroy(sl.ev_in);
         if (sl.ev_done) cudaEventDestroy(sl.ev_done);
     }
     void* dev[] = {p->d_desc, p->d_hw, p->d_have_prev, p->d_flag, p->d_det_count, p->d_det_idx, p->d_count, p->d_detail, p->d_diff,
                    p->d_det_rows, p->d_boxes, p->d_kps_now, p->d_prev_lm, p->d_prev_dx, p->d_track, p->d_out_kps,
-                   p->d_track_f32, p->d_n_prev, p->d_prev_f32, p->d_state_idx, p->d_n_track, p->d_chips, p->d_align_M};
+                   p->d_track_f32, p->d_n_prev, p->d_prev_f32, p->d_state_idx, p->d_n_track, p->d_chips, p->d_align_M, p->d_pose};
     for (void* q : dev) if (q) cudaFree(q);
     if (p->s_copy) cudaStreamDestroy(p->s_copy);
     if (p->s_compute) cudaStreamDestroy(p->s_compute);
@@ -264,6 +269,18 @@ extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8
         SKPS_CUDA(cudaMemcpyAsync(sl.h_chips, p->d_chips, chip_bytes * K * n, cudaMemcpyDeviceToHost, sx));
         SKPS_CUDA(cudaMemcpyAsync(sl.h_M, p->d_align_M, 8 * 6 * (size_t)K * n, cudaMemcpyDeviceToHost, sx));
     }
+    sl.pose = p->pose_on;
+    if (sl.pose) {
+        // head pose from the smoothed landmarks, camera per stream from this call's frame size
+        PoseArgs pa = {};
+        pose_model_98(pa);
+        pa.pts64 = p->d_out_kps; pa.G = n; pa.K = K; pa.P = P;
+        pa.count = p->d_count; pa.hw = p->d_hw;
+        const size_t faces = (size_t)n * K;
+        pa.rvec = p->d_pose; pa.tvec = p->d_pose + 3 * faces; pa.euler = p->d_pose + 6 * faces; pa.reproj = p->d_pose + 9 * faces;
+        if (launch_head_pose(pa, sx)) return 1;
+        SKPS_CUDA(cudaMemcpyAsync(sl.h_pose, p->d_pose, 8 * 25 * faces, cudaMemcpyDeviceToHost, sx));
+    }
     SKPS_CUDA(cudaMemcpyAsync(sl.h_count, p->d_count, 4 * n, cudaMemcpyDeviceToHost, sx));
     SKPS_CUDA(cudaMemcpyAsync(sl.h_flag, p->d_flag, 4 * n, cudaMemcpyDeviceToHost, sx));
     SKPS_CUDA(cudaMemcpyAsync(sl.h_det_count, p->d_det_count, 4 * n, cudaMemcpyDeviceToHost, sx));
@@ -347,6 +364,51 @@ extern "C" SKPS_API int skps_mpipe_align_results(skps_mpipe* p, int slot_i, uint
     const size_t faces = (size_t)sl.n * p->K;
     memcpy(chips, sl.h_chips, faces * sl.align * sl.align * 3);
     memcpy(M, sl.h_M, faces * 6 * sizeof(double));
+    return 0;
+}
+
+static void free_pose(skps_mpipe* p) {
+    if (p->d_pose) cudaFree(p->d_pose);
+    p->d_pose = nullptr;
+    for (auto& sl : p->slot) {
+        if (sl.h_pose) cudaFreeHost(sl.h_pose);
+        sl.h_pose = nullptr; sl.pose = false;
+    }
+    p->pose_on = false;
+}
+
+extern "C" SKPS_API int skps_mpipe_set_pose(skps_mpipe* p, int on) {
+    SKPS_CHECK(p, "mpipe_set_pose: null");
+    SKPS_CHECK(!p->slot[0].busy && !p->slot[1].busy, "mpipe_set_pose: a batch is in flight (call skps_mpipe_wait first)");
+    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_CUDA(cudaStreamSynchronize(p->s_compute));
+    if ((on != 0) == p->pose_on) return 0;
+    free_pose(p);
+    if (!on) return 0;
+    SKPS_CHECK(p->P >= 98, "mpipe_set_pose: %d landmarks per face, expected 98", p->P);
+    const size_t bytes = 8 * 25 * (size_t)p->S * p->K;
+    bool ok = cudaMalloc((void**)&p->d_pose, bytes) == cudaSuccess;
+    for (auto& sl : p->slot) ok = ok && cudaMallocHost((void**)&sl.h_pose, bytes) == cudaSuccess;
+    if (!ok) {
+        cudaGetLastError();
+        free_pose(p);
+        SKPS_CHECK(false, "mpipe_set_pose: cannot allocate %zu bytes per buffer", bytes);
+    }
+    p->pose_on = true;
+    return 0;
+}
+
+extern "C" SKPS_API int skps_mpipe_pose_results(skps_mpipe* p, int slot_i, double* rvec, double* tvec, double* euler,
+                                                double* reproject) {
+    SKPS_CHECK(p && (slot_i == 0 || slot_i == 1) && rvec && tvec && euler && reproject, "mpipe_pose_results: bad arguments");
+    const skps_mpipe::Slot& sl = p->slot[slot_i];
+    SKPS_CHECK(!sl.busy, "mpipe_pose_results: slot %d is in flight (call skps_mpipe_wait first)", slot_i);
+    SKPS_CHECK(sl.pose && sl.n > 0, "mpipe_pose_results: slot %d was not submitted with pose on", slot_i);
+    const size_t faces = (size_t)sl.n * p->K;
+    memcpy(rvec, sl.h_pose, faces * 3 * sizeof(double));
+    memcpy(tvec, sl.h_pose + 3 * faces, faces * 3 * sizeof(double));
+    memcpy(euler, sl.h_pose + 6 * faces, faces * 3 * sizeof(double));
+    memcpy(reproject, sl.h_pose + 9 * faces, faces * 16 * sizeof(double));
     return 0;
 }
 

@@ -55,4 +55,21 @@ int launch_mp_temporal(const MpTemporalArgs& a, int n_streams, cudaStream_t s);
 int launch_mp_align(const MpStreamDesc* d, const double* kps, const int* count, int K, int P, int size, uint8_t* chips,
                     double* M, int n, cudaStream_t s);
 
+// Head pose (headpose.cu): get_head_pose for every face i < count[g] of every group g < G, one warp per face.  The 10 image
+// points of a face are pts[g][i][idx[0..9]], rounded to float32; the camera of group g is [[W,0,W//2],[0,W,H//2],[0,0,1]].
+struct PoseArgs {
+    const double* pts64;         // [G][K][P][2] landmarks, float64 ...
+    const float* pts32;          // ... or float32 (exactly one of the two is set)
+    int G, K, P;
+    int idx[10];                 // the landmarks paired with obj[0..9]
+    const int* count;            // [G] faces per group, or null (all K); outputs of faces i >= count[g] are not written
+    const int* hw;               // [G][2] frame H, W per group [dev], or null: H, W below for every group
+    int H, W;
+    float obj[30], cube[24];     // 3-D model points and the re-projected cube (pose.py)
+    double *rvec, *tvec, *euler, *reproj;     // [G][K][3] x3, [G][K][8][2]
+};
+// idx, obj and cube of get_head_pose on 98-point WFLW landmarks (TRAIN/face_landmark/lib/dataset/headpose.py:48-78)
+void pose_model_98(PoseArgs& a);
+int launch_head_pose(const PoseArgs& a, cudaStream_t s);
+
 }  // namespace skps

@@ -10,6 +10,7 @@
 
 #include "../../include/skps_b200.h"
 #include "common.h"
+#include "mpipe_kernels.h"
 
 using namespace skps;
 
@@ -40,6 +41,8 @@ struct skps_pipeline {
     // aligned chips (skps_pipeline_align): allocated on first use, for top_k faces at align_size
     int align_size = 0;
     double* d_align_kps = nullptr; double* d_align_M = nullptr; uint8_t* d_chips = nullptr;
+    // head pose (skps_pipeline_pose): allocated on first use, for top_k faces
+    double* d_pose_kps = nullptr; double* d_pose = nullptr;
 };
 
 extern "C" SKPS_API void skps_pipeline_destroy(skps_pipeline* p) {
@@ -48,7 +51,8 @@ extern "C" SKPS_API void skps_pipeline_destroy(skps_pipeline* p) {
     for (int i = 0; i < 2; ++i) if (p->d_frame[i]) cudaFree(p->d_frame[i]);
     if (p->h_frame) cudaFreeHost(p->h_frame);
     void* dev[] = {p->d_det_rows, p->d_det_idx, p->d_det_count, p->d_track, p->d_boxes, p->d_count, p->d_detail,
-                   p->d_kps, p->d_diff, p->d_align_kps, p->d_align_M, p->d_chips};
+                   p->d_kps, p->d_diff, p->d_align_kps, p->d_align_M, p->d_chips,
+                   p->d_pose_kps, p->d_pose};
     for (void* q : dev) if (q) cudaFree(q);
     void* host[] = {p->h_res, p->h_boxes, p->h_kps, p->h_scores, p->h_det_idx, p->h_det_rows, p->h_track};
     for (void* q : host) if (q) cudaFreeHost(q);
@@ -262,6 +266,35 @@ extern "C" SKPS_API int skps_pipeline_align(skps_pipeline* p, const double* kps,
         return 1;
     SKPS_CUDA(cudaMemcpyAsync(chips, p->d_chips, chip_bytes * n, cudaMemcpyDeviceToHost, s));
     SKPS_CUDA(cudaMemcpyAsync(M, p->d_align_M, sizeof(double) * 6 * n, cudaMemcpyDeviceToHost, s));
+    SKPS_CUDA(cudaStreamSynchronize(s));
+    return 0;
+}
+
+// Head pose of n faces whose landmarks were smoothed on the host: kps [host] (n, n_points, 2) float64, frame H x W for the
+// camera.  The 98-point get_head_pose of the training tree on the GPU, ordered on `stream`.
+extern "C" SKPS_API int skps_pipeline_pose(skps_pipeline* p, const double* kps, int n, int H, int W, double* rvec, double* tvec,
+                                           double* euler, double* reproject, void* stream) {
+    SKPS_CHECK(p && kps && rvec && tvec && euler && reproject, "pipeline_pose: null argument");
+    SKPS_CHECK(n > 0 && n <= p->cfg.top_k, "pipeline_pose: %d faces, expected 1..%d", n, p->cfg.top_k);
+    SKPS_CHECK(H > 0 && W > 0, "pipeline_pose: bad frame size %dx%d", H, W);
+    SKPS_CHECK(p->n_points >= 98, "pipeline_pose: %d landmarks per face, expected 98", p->n_points);
+    cudaStream_t s = (cudaStream_t)stream;
+    SKPS_CUDA(cudaSetDevice(p->device));
+    const int K = p->cfg.top_k, P = p->n_points;
+    if (!p->d_pose) {
+        SKPS_CUDA(cudaMalloc((void**)&p->d_pose_kps, sizeof(double) * 2 * P * K));
+        SKPS_CUDA(cudaMalloc((void**)&p->d_pose, sizeof(double) * 25 * K));
+    }
+    SKPS_CUDA(cudaMemcpyAsync(p->d_pose_kps, kps, sizeof(double) * 2 * P * n, cudaMemcpyHostToDevice, s));
+    PoseArgs a = {};
+    pose_model_98(a);
+    a.pts64 = p->d_pose_kps; a.G = 1; a.K = n; a.P = P; a.H = H; a.W = W;
+    a.rvec = p->d_pose; a.tvec = p->d_pose + 3 * n; a.euler = p->d_pose + 6 * n; a.reproj = p->d_pose + 9 * n;
+    if (launch_head_pose(a, s)) return 1;
+    SKPS_CUDA(cudaMemcpyAsync(rvec, a.rvec, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, s));
+    SKPS_CUDA(cudaMemcpyAsync(tvec, a.tvec, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, s));
+    SKPS_CUDA(cudaMemcpyAsync(euler, a.euler, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, s));
+    SKPS_CUDA(cudaMemcpyAsync(reproject, a.reproj, sizeof(double) * 16 * n, cudaMemcpyDeviceToHost, s));
     SKPS_CUDA(cudaStreamSynchronize(s));
     return 0;
 }

@@ -93,6 +93,9 @@ SIGNATURES = {
     "skps_pipeline_align": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp]),
     "skps_mpipe_set_align": (C.c_int, [c_vp, C.c_int]),
     "skps_mpipe_align_results": (C.c_int, [c_vp, C.c_int, c_vp, c_vp]),
+    "skps_pipeline_pose": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "skps_mpipe_set_pose": (C.c_int, [c_vp, C.c_int]),
+    "skps_mpipe_pose_results": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp]),
 }
 
 _lib = None

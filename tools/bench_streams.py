@@ -5,11 +5,17 @@ host results out: every H2D / D2H is inside the timed region.
 
     python tools/bench_streams.py [--streams 16] [--batches 12] [--configs 1080p_4faces,4k_16faces] [--gather]
     python tools/bench_streams.py --align 112 [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
+    python tools/bench_streams.py --pose [--parent-headpose OLD_headpose.cu --out DIR] [--rounds 5] [--configs ...]
 
 --align SIZE times every config with and without aligned face chips (FaceAnaStreams(align=SIZE)) in the same process,
 alternating the two over --rounds rounds, and reports the median ms_per_call of both.  At 4k_16faces it also times the
 alignment kernel alone with CUDA events (skps_align_faces on one 4K frame in HBM, the landmarks of every face of the last
 call) and reports the bytes it writes per second.  The GPU name and power limit are read in the same run.
+
+--pose does the same with and without head pose (FaceAnaStreams(pose=True)), then times the pose solver alone
+(head_pose_warp_kernel, torch.profiler kernel times) at 16, 256 and 1024 faces.  --parent-headpose compiles an earlier
+csrc/headpose.cu into a side library under --out (not part of the package), times its kernel at the same sizes in the same
+run and reports the largest difference of its skps_head_pose results from this build's on tests/test_headpose_gpu.py's inputs.
 
 Under torchrun every rank drives its own S streams on its own GPU (streams shard across GPUs, no collective on the data
 path); time = max over ranks.  --gather adds one NCCL all_gather of the packed (box, landmarks, scores) rows per call."""
@@ -157,16 +163,18 @@ def time_align_kernel(torch, frame, kps, size, iters=200):
             "timing": "CUDA events around %d back-to-back launches" % iters}
 
 
-def run_align_pair(name, size, n_streams=16, batches=12, warmup=3, rounds=5, length=6):
-    """The same config with and without alignment, alternating; median ms_per_call of each."""
+def run_align_pair(name, size, n_streams=16, batches=12, warmup=3, rounds=5, length=6, feature="align"):
+    """The same config with and without alignment (feature="align", chip side `size`) or head pose (feature="pose"),
+    alternating; median ms_per_call of each."""
     import torch
     import frames
     from Skps import FaceAnaStreams
     maker, topk = getattr(frames, CONFIGS[name][0]), CONFIGS[name][1]
     seqs = make_streams(torch, frames, maker, n_streams, length=length)
     H, W = seqs[0][0].shape[:2]
+    on = {"align": size} if feature == "align" else {"pose": True}
     fas = {"off": FaceAnaStreams(n_streams=n_streams, top_k=topk, max_frame_hw=(H, W)),
-           "on": FaceAnaStreams(n_streams=n_streams, top_k=topk, max_frame_hw=(H, W), align=size)}
+           "on": FaceAnaStreams(n_streams=n_streams, top_k=topk, max_frame_hw=(H, W), **on)}
     L = len(seqs[0])
 
     def batch(t):
@@ -194,6 +202,16 @@ def run_align_pair(name, size, n_streams=16, batches=12, warmup=3, rounds=5, len
             if key == "on":
                 last = res
     per_face = 32 + 98 * 2 * 8 + 98 * 4
+    if feature == "pose":
+        del fas
+        return {"config": name, "streams_per_gpu": n_streams, "calls": batches, "rounds": rounds,
+                "ms_per_call": 1e3 * float(np.median(times["off"])) / batches,
+                "ms_per_call_pose": 1e3 * float(np.median(times["on"])) / batches,
+                "ms_per_call_rounds": [1e3 * v / batches for v in times["off"]],
+                "ms_per_call_pose_rounds": [1e3 * v / batches for v in times["on"]],
+                "faces_per_frame": faces["on"] / (n_streams * batches),
+                "d2h_bytes_per_frame": int(topk * per_face), "d2h_bytes_per_frame_pose": int(topk * (per_face + 25 * 8)),
+                "api": "FaceAnaStreams.submit/collect, pinned host frames, 2 calls in flight; pose: solved in submit"}
     out = {"config": name, "streams_per_gpu": n_streams, "calls": batches, "rounds": rounds, "align_size": size,
            "ms_per_call": 1e3 * float(np.median(times["off"])) / batches,
            "ms_per_call_align": 1e3 * float(np.median(times["on"])) / batches,
@@ -210,6 +228,89 @@ def run_align_pair(name, size, n_streams=16, batches=12, warmup=3, rounds=5, len
     return out
 
 
+def build_parent_headpose(src, out_dir):
+    """An earlier csrc/headpose.cu as a library of its own (skps_head_pose only) under out_dir."""
+    import shutil
+    import subprocess
+    from peppa_pig_face_landmark_b200 import build
+    os.makedirs(out_dir, exist_ok=True)
+    cu = os.path.join(out_dir, "parent_headpose.cu")
+    shutil.copyfile(src, cu)
+    stub = os.path.join(out_dir, "parent_error_stub.cu")
+    with open(stub, "w") as f:       # the error-string helpers live in engine.cu, which the side library leaves out
+        f.write("namespace skps { void set_error(const char*, ...) {} const char* get_error() { return \"\"; } }\n")
+    lib = os.path.join(out_dir, "libparent_headpose.so")
+    subprocess.check_call([build._nvcc()] + build.ARCH + build.COMMON + build.SOURCES["headpose.cu"] +
+                          ["-I", build.CSRC, "-shared", "-o", lib, cu, stub])
+    return lib
+
+
+def _bind_head_pose(path):
+    import ctypes as C
+    lib = C.CDLL(path)
+    fn = lib.skps_head_pose
+    fn.restype = C.c_int
+    fn.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 6
+    return fn
+
+
+def _head_pose(fn, pts, hw):
+    from peppa_pig_face_landmark_b200.core.headpose.pose import object_pts, reprojectsrc
+    n = pts.shape[0]
+    out = {"rvec": np.zeros((n, 3)), "tvec": np.zeros((n, 3)), "euler": np.zeros((n, 3)), "reproject": np.zeros((n, 8, 2))}
+    rc = fn(pts.ctypes.data, n, hw[1], hw[0], object_pts.ctypes.data, reprojectsrc.ctypes.data, out["rvec"].ctypes.data,
+            out["tvec"].ctypes.data, out["euler"].ctypes.data, out["reproject"].ctypes.data)
+    assert rc == 0, "skps_head_pose failed"
+    return out
+
+
+def time_pose_kernels(torch, parent_lib=None, sizes=(16, 256, 1024), iters=30):
+    """Kernel time of the pose solver (and of the parent's, if given) per launch, from torch.profiler kernel records."""
+    from torch.autograd import DeviceType
+    from torch.profiler import ProfilerActivity, profile
+    from peppa_pig_face_landmark_b200 import runtime as rt
+    from peppa_pig_face_landmark_b200.core.headpose.pose import POSE_POINTS
+    from test_headpose_gpu import _synthetic_shapes
+    impls = {"head_pose_warp_kernel": _bind_head_pose(rt.LIB_PATH)}
+    if parent_lib:
+        impls["parent_head_pose_kernel"] = _bind_head_pose(parent_lib)
+    hw = (1080, 1920)
+    out = []
+    for n in sizes:
+        pts = np.ascontiguousarray(_synthetic_shapes(n, hw, seed=n)[:, POSE_POINTS], np.float32)
+        row = {"faces": n}
+        for name, fn in impls.items():
+            for _ in range(3):
+                _head_pose(fn, pts, hw)
+            torch.cuda.synchronize()
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                for _ in range(iters):
+                    _head_pose(fn, pts, hw)
+                torch.cuda.synchronize()
+            us = [e.time_range.elapsed_us() for e in prof.events()
+                  if e.device_type == DeviceType.CUDA and "head_pose" in e.name]
+            assert len(us) == iters, (name, len(us))
+            row[name + "_us"] = float(np.median(us))
+            row[name + "_name"] = [e.name for e in prof.events() if "head_pose" in e.name][0]
+        out.append(row)
+    return {"pose_kernel": out, "timing": "torch.profiler CUDA kernel records, median of %d launches" % iters}
+
+
+def parent_pose_diff(parent_lib):
+    """Largest difference of this build's skps_head_pose from the parent's on test_headpose_gpu's inputs."""
+    from peppa_pig_face_landmark_b200 import runtime as rt
+    from peppa_pig_face_landmark_b200.core.headpose.pose import POSE_POINTS
+    from test_headpose_gpu import _synthetic_shapes
+    new, old = _bind_head_pose(rt.LIB_PATH), _bind_head_pose(parent_lib)
+    d = {k: 0.0 for k in ("rvec", "tvec", "euler", "reproject")}
+    for hw in [(480, 640), (1080, 1920)]:
+        pts = np.ascontiguousarray(_synthetic_shapes(64, hw, seed=hw[0])[:, POSE_POINTS], np.float32)
+        a, b = _head_pose(new, pts, hw), _head_pose(old, pts, hw)
+        for k in d:
+            d[k] = max(d[k], float(np.abs(a[k] - b[k]).max()))
+    return {"max_abs_diff_from_parent": d, "inputs": "test_headpose_gpu._synthetic_shapes(64, hw, seed=hw[0]), 480x640 and 1080x1920"}
+
+
 def main():
     import torch
     a = sys.argv[1:]
@@ -224,6 +325,19 @@ def main():
     if world > 1:
         import torch.distributed as dist
         dist.init_process_group("nccl", device_id=torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0"))))
+    if "--pose" in a:
+        rounds = int(opt("--rounds", 5))
+        print(json.dumps(gpu_info(torch)))
+        parent = None
+        if "--parent-headpose" in a:
+            parent = build_parent_headpose(opt("--parent-headpose", None), opt("--out", "bench_out"))
+            print(json.dumps(parent_pose_diff(parent)))
+        print(json.dumps(time_pose_kernels(torch, parent)))
+        sys.stdout.flush()
+        for name in names:
+            print(json.dumps(run_align_pair(name, 0, n_streams, batches, rounds=rounds, feature="pose")))
+            sys.stdout.flush()
+        return
     if "--align" in a:
         size, rounds = int(opt("--align", 112)), int(opt("--rounds", 5))
         print(json.dumps(gpu_info(torch)))
