@@ -11,6 +11,7 @@ import time
 import numpy as np
 
 from ... import runtime as rt
+from ...graph_tools import detector_onnx_for
 from ...logger.logger import logger
 from .onnx_model_base import ONNXEngine
 
@@ -33,10 +34,13 @@ class FaceDetector:
     MAX_DET = 256
 
     def __init__(self, cfg):
+        """cfg: Skps.yml's Detect section.  The engine is built for cfg['input_shape'] ([h, w, 3]): from the export itself
+        when that is its input size, else from the export retargeted to (h, w) (graph_tools.detector_onnx_for; h and w
+        multiples of 32 in 128..2176 x 128..3840), so the letterbox and the network always agree on the size."""
         root_path = pathlib.Path(__file__).resolve().parents[2]
         model_path = os.path.join(root_path, cfg['model_path'])
-        self.model = ONNXEngine(model_path, max_batch=1)
         self.input_size = cfg['input_shape']
+        self.model = ONNXEngine(detector_onnx_for(model_path, self.input_size[:2]), max_batch=1)
         self.score_thrs = cfg['score_thrs']
         self.iou_thrs = cfg['iou_thrs']
         self.lib = rt.load_library()

@@ -14,6 +14,7 @@ import numpy as np
 import yaml
 
 from ... import runtime as rt
+from ...graph_tools import check_detector_input
 from ...logger.logger import logger
 from ..smoother.lk import EmaFilter, GroupTrack
 from .face_detector import FaceDetector, letterbox_geometry
@@ -29,18 +30,26 @@ def get_cfg():
 
 
 class FaceAna():
-    def __init__(self, verbose=False, top_k=None, max_frame_hw=(2160, 3840), align=None, pose=False):
+    def __init__(self, verbose=False, top_k=None, max_frame_hw=(2160, 3840), align=None, pose=False, det_input=None):
         """align: None, or a chip side in 16..512: every result dict then also carries 'chip' ((align, align, 3) uint8
         BGR, the face warped to the ArcFace five-point template) and 'M' ((2, 3) float64, the frame -> chip matrix for
         cv2.warpAffine), computed on the GPU from the returned 'kps' and the frame already in HBM (core/api/align.py).
         pose: every result dict then also carries 'pose': {'euler': (3,), 'rvec': (3,), 'tvec': (3,), 'reproject': (8, 2)},
         float64, Euler angles in degrees - head_poses(kps[None], frame.shape[:2], points=POSE_POINTS_98) of the returned
-        'kps', solved on the GPU."""
+        'kps', solved on the GPU.
+        det_input: None (Skps.yml's Detect.input_shape, 384x640), or the detector input size (h, w): multiples of 32 in
+        128..2176 x 128..3840.  Every frame is letterboxed to that size, so a larger one finds smaller faces: at 1152x1920
+        a 3840x2160 frame is scaled by 1/2 instead of 1/6.  The detector's work and activation memory grow with h*w
+        (3.97 GMAC and 0.35 GB at 1152x1920, 0.44 GMAC and 0.04 GB at 384x640)."""
+        if det_input is not None:
+            det_input = check_detector_input(det_input)
         self.align = None if align is None else check_size(align)
         self.pose = bool(pose)
         if verbose:
             logger.setLevel(logging.DEBUG)
         cfg = get_cfg()
+        if det_input is not None:
+            cfg['Skps']['Detect']['input_shape'] = [det_input[0], det_input[1], 3]
         self.top_k = int(top_k if top_k is not None else cfg['Skps']['Detect']['topk'])
         self.face_detector = FaceDetector(cfg['Skps']['Detect'])
         self.face_landmark = FaceLandmark(cfg['Skps']['Keypoints'], max_faces=self.top_k)

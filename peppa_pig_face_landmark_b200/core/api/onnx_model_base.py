@@ -126,6 +126,6 @@ class ONNXEngine:
         return out
 
     def _shape(self, outs, n):
-        if self.n_out == 1:                       # detector: (N, 15120, 16)
+        if self.n_out == 1:                       # detector: (N, rows, 16), 15120 rows at 384x640
             return [outs[0].reshape(n, -1, 16)]
         return outs                               # landmark net: (N,196), (N,98)

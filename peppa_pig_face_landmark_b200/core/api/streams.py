@@ -19,17 +19,22 @@ import pathlib
 import numpy as np
 
 from ... import runtime as rt
+from ...graph_tools import check_detector_input, detector_onnx_for
 from .align import check_size
 from .facer import get_cfg
 from .onnx_model_base import ONNXEngine
 
 
 class FaceAnaStreams:
-    def __init__(self, n_streams, top_k=None, max_frame_hw=(2160, 3840), device="cuda", align=None, pose=False):
+    def __init__(self, n_streams, top_k=None, max_frame_hw=(2160, 3840), device="cuda", align=None, pose=False,
+                 det_input=None):
         """align: None, or a chip side in 16..512: every result dict then also carries 'chip' and 'M' as FaceAna(align=...)
         returns them, warped inside the same submit on the device from the smoothed landmarks and the frame in the ring.
         pose: every result dict then also carries 'pose' as FaceAna(pose=True) returns it, solved inside the same submit
-        from the smoothed landmarks, with each stream's own frame size for the camera."""
+        from the smoothed landmarks, with each stream's own frame size for the camera.
+        det_input: None (Skps.yml's 384x640) or the detector input size (h, w), as FaceAna(det_input=...) takes it.  The
+        detector runs on all n_streams frames at once, so its activations take n_streams times FaceAna's memory (about
+        0.35 GB per stream at 1152x1920)."""
         self.align = None if align is None else check_size(align)
         self.pose = bool(pose)
         cfg = get_cfg()['Skps']
@@ -37,7 +42,9 @@ class FaceAnaStreams:
         self.n_streams = int(n_streams)
         self.top_k = int(top_k if top_k is not None else det_cfg['topk'])
         root = pathlib.Path(__file__).resolve().parents[2]
-        self.det = ONNXEngine(os.path.join(root, det_cfg['model_path']), device=device, max_batch=self.n_streams)
+        det_hw = det_cfg['input_shape'][:2] if det_input is None else check_detector_input(det_input)
+        self.det = ONNXEngine(detector_onnx_for(os.path.join(root, det_cfg['model_path']), det_hw), device=device,
+                              max_batch=self.n_streams)
         self.kps = ONNXEngine(os.path.join(root, kps_cfg['model_path']), device=device,
                               max_batch=self.n_streams * self.top_k)
         self.n_points = int(kps_cfg['num_points'])

@@ -256,6 +256,15 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
     if (cudaMemcpy(e->d_weights, weights, n_floats * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
         set_error("cudaMemcpy weights"); return fail("copy");
     }
+    // the elementwise kernels and the detector decode number their threads with 32-bit ints (ops_misc.cu): a batch of a
+    // large input size (a re-targeted detector) must keep every activation tensor below 2^31 elements
+    for (int i = 0; i < n_bufs; ++i) {
+        if (buf_elems(e->bufs[i]) * (size_t)max_batch >= ((size_t)1 << 31)) {
+            set_error("buffer %d (%dx%dx%d) has 2^31 or more elements at batch %d", i, e->bufs[i].H, e->bufs[i].W,
+                      e->bufs[i].C, max_batch);
+            return fail("size");
+        }
+    }
     e->dbuf.assign(n_bufs, nullptr);
     for (int i = 0; i < n_bufs; ++i) {
         size_t bytes = buf_bytes(e->bufs[i]) * (size_t)max_batch;

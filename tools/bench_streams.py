@@ -6,6 +6,7 @@ host results out: every H2D / D2H is inside the timed region.
     python tools/bench_streams.py [--streams 16] [--batches 12] [--configs 1080p_4faces,4k_16faces] [--gather]
     python tools/bench_streams.py --align 112 [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
     python tools/bench_streams.py --pose [--parent-headpose OLD_headpose.cu --out DIR] [--rounds 5] [--configs ...]
+    python tools/bench_streams.py --det-input H W [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
 
 --align SIZE times every config with and without aligned face chips (FaceAnaStreams(align=SIZE)) in the same process,
 alternating the two over --rounds rounds, and reports the median ms_per_call of both.  At 4k_16faces it also times the
@@ -16,6 +17,8 @@ call) and reports the bytes it writes per second.  The GPU name and power limit 
 (head_pose_warp_kernel, torch.profiler kernel times) at 16, 256 and 1024 faces.  --parent-headpose compiles an earlier
 csrc/headpose.cu into a side library under --out (not part of the package), times its kernel at the same sizes in the same
 run and reports the largest difference of its skps_head_pose results from this build's on tests/test_headpose_gpu.py's inputs.
+
+--det-input H W does the same with the detector at Skps.yml's 384x640 and at H x W (FaceAnaStreams(det_input=(H, W))).
 
 Under torchrun every rank drives its own S streams on its own GPU (streams shard across GPUs, no collective on the data
 path); time = max over ranks.  --gather adds one NCCL all_gather of the packed (box, landmarks, scores) rows per call."""
@@ -164,15 +167,15 @@ def time_align_kernel(torch, frame, kps, size, iters=200):
 
 
 def run_align_pair(name, size, n_streams=16, batches=12, warmup=3, rounds=5, length=6, feature="align"):
-    """The same config with and without alignment (feature="align", chip side `size`) or head pose (feature="pose"),
-    alternating; median ms_per_call of each."""
+    """The same config with and without alignment (feature="align", chip side `size`), head pose (feature="pose") or the
+    detector at input size `size` = (h, w) (feature="det_input"), alternating; median ms_per_call of each."""
     import torch
     import frames
     from Skps import FaceAnaStreams
     maker, topk = getattr(frames, CONFIGS[name][0]), CONFIGS[name][1]
     seqs = make_streams(torch, frames, maker, n_streams, length=length)
     H, W = seqs[0][0].shape[:2]
-    on = {"align": size} if feature == "align" else {"pose": True}
+    on = {"align": {"align": size}, "pose": {"pose": True}, "det_input": {"det_input": size}}[feature]
     fas = {"off": FaceAnaStreams(n_streams=n_streams, top_k=topk, max_frame_hw=(H, W)),
            "on": FaceAnaStreams(n_streams=n_streams, top_k=topk, max_frame_hw=(H, W), **on)}
     L = len(seqs[0])
@@ -202,6 +205,17 @@ def run_align_pair(name, size, n_streams=16, batches=12, warmup=3, rounds=5, len
             if key == "on":
                 last = res
     per_face = 32 + 98 * 2 * 8 + 98 * 4
+    if feature == "det_input":
+        del fas
+        ms = {k: 1e3 * float(np.median(v)) / batches for k, v in times.items()}
+        return {"config": name, "streams_per_gpu": n_streams, "calls": batches, "rounds": rounds, "det_input": list(size),
+                "ms_per_call_384x640": ms["off"], "ms_per_call_det_input": ms["on"],
+                "frames_per_s_384x640": 1e3 * n_streams / ms["off"], "frames_per_s_det_input": 1e3 * n_streams / ms["on"],
+                "ms_per_call_384x640_rounds": [1e3 * v / batches for v in times["off"]],
+                "ms_per_call_det_input_rounds": [1e3 * v / batches for v in times["on"]],
+                "faces_per_frame_384x640": faces["off"] / (n_streams * batches),
+                "faces_per_frame_det_input": faces["on"] / (n_streams * batches),
+                "api": "FaceAnaStreams.submit/collect, pinned host frames, 2 calls in flight"}
     if feature == "pose":
         del fas
         return {"config": name, "streams_per_gpu": n_streams, "calls": batches, "rounds": rounds,
@@ -336,6 +350,14 @@ def main():
         sys.stdout.flush()
         for name in names:
             print(json.dumps(run_align_pair(name, 0, n_streams, batches, rounds=rounds, feature="pose")))
+            sys.stdout.flush()
+        return
+    if "--det-input" in a:
+        i = a.index("--det-input")
+        hw, rounds = (int(a[i + 1]), int(a[i + 2])), int(opt("--rounds", 5))
+        print(json.dumps(gpu_info(torch)))
+        for name in names:
+            print(json.dumps(run_align_pair(name, hw, n_streams, batches, rounds=rounds, feature="det_input")))
             sys.stdout.flush()
         return
     if "--align" in a:

@@ -1,6 +1,7 @@
 """Layer-by-layer parity report (GPU box): runs a network through the CUDA engine and through
 the oracle executor on the same input and prints, per plan buffer, the max abs / rel error
-against the ONNX tensor of the same name.  Usage: python tools/layer_report.py [student|detector]"""
+against the ONNX tensor of the same name.  Usage: python tools/layer_report.py [student|detector [H W]]
+(H W: the detector retargeted to that input size, graph_tools.retarget_detector_input)"""
 import os
 import sys
 
@@ -11,7 +12,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
-def report(which="student", batch=2, out=sys.stdout):
+def report(which="student", batch=2, out=sys.stdout, det_input=None):
     import frames
     from oracle import host_ref as H
     from oracle.onnx_exec import Session
@@ -22,7 +23,11 @@ def report(which="student", batch=2, out=sys.stdout):
         x_u8 = frames.crop_variants(batch)
     else:
         path = os.path.join(pre, "yolov5n-0.5.onnx")
-        x, _ = H.letterbox(frames.load_test1())
+        hw = (384, 640)
+        if det_input is not None:
+            from peppa_pig_face_landmark_b200.graph_tools import ensure_detector_onnx
+            path, hw = ensure_detector_onnx(path, det_input), tuple(det_input)
+        x, _ = H.letterbox(frames.load_test1() if det_input is None else frames.frame_4k(), *hw)
         x_u8 = np.round(x.transpose(0, 2, 3, 1) * 255).astype(np.uint8)
         batch = 1
     eng = ONNXEngine(path, max_batch=batch)
@@ -74,7 +79,8 @@ def report(which="student", batch=2, out=sys.stdout):
 
 if __name__ == "__main__":
     which = sys.argv[1] if len(sys.argv) > 1 else "student"
+    det_input = (int(sys.argv[2]), int(sys.argv[3])) if len(sys.argv) > 3 else None
     os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
     with open(os.path.join(ROOT, "gpurun_out", "layer_report_%s.txt" % which), "w") as f:
-        report(which, out=f)
+        report(which, out=f, det_input=det_input)
     print(open(os.path.join(ROOT, "gpurun_out", "layer_report_%s.txt" % which)).read()[-3000:])
