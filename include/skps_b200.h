@@ -152,16 +152,31 @@ SKPS_API int skps_letterbox(const uint8_t* frame, int H, int W, int pitch,
                    int rw, int rh, int top, int left, void* stream);
 
 /* xywh2xyxy + py_nms + scale_coords (face_detector.py:73-136) on the raw (rows,16) output.
- * Writes up to max_det kept rows (16 floats each, cols 0-3 mapped back to frame pixels),
- * their row indices into the raw output, and the count.  All [dev]. */
+ * Writes up to max_det (<= 256) kept rows (16 floats each, cols 0-3 mapped back to frame pixels),
+ * their row indices into the raw output, and the count.  All [dev].  This entry keeps its limit:
+ * with more than 1024 rows over the score threshold it writes count = -candidates and nothing
+ * else.  skps_detect_post_batch below has no limit. */
 SKPS_API int skps_detect_post(const float* raw, int rows, float score_thres, float iou_thres,
                      float scale, float pad_x, float pad_y,
                      float* kept_rows, int32_t* kept_idx, int32_t* count, int max_det,
                      void* stream);
 
+/* The same post-processing for any number of candidates (up to every row), for `batch` frames at
+ * once: raw [dev] (batch,rows,16); recover [dev] (batch,3) float32 = scale, pad_x, pad_y of each
+ * frame's letterbox.  Frame f gets its kept rows in kept_rows [dev] (batch,capacity,16), their row
+ * indices in kept_idx [dev] (batch,capacity) and their number, min(kept, capacity), in count[f]
+ * [dev]; capacity >= rows keeps every box.  Candidates are ranked by (score, row index) descending
+ * and suppressed exactly as py_nms does.  `workspace` [dev] holds at least
+ * skps_detect_post_workspace_size(rows, batch) bytes (about 40 bytes per row and frame); the call
+ * allocates nothing.  Asynchronous on `stream`. */
+SKPS_API size_t skps_detect_post_workspace_size(int rows, int batch);
+SKPS_API int skps_detect_post_batch(const float* raw, int rows, int batch, float score_thres, float iou_thres,
+                                    const float* recover, float* kept_rows, int32_t* kept_idx, int32_t* count,
+                                    int capacity, void* workspace, size_t workspace_bytes, void* stream);
+
 /* FaceAna.judge_boxs + sort_and_filter (facer.py:120-189): IoU-match detections against the
- * previous track boxes (EMA alpha), drop area<=min_face, keep top_k by area.  `track` [dev]
- * (n_track,4) may be NULL.  Writes (count,4) boxes. */
+ * previous track boxes (EMA alpha), drop area<=min_face, keep top_k (<= 64) by area.  Any number
+ * of detections.  `track` [dev] (n_track,4) may be NULL.  Writes (count,4) boxes. */
 SKPS_API int skps_select_faces(const float* det_rows, const int32_t* det_count, int det_stride,
                       const float* track, int n_track,
                       float iou_thres, float alpha, float one_minus_alpha,
@@ -210,12 +225,21 @@ SKPS_API int skps_pipeline_reset(skps_pipeline* p);
  * NULL.  If run_detector==0 the `track` boxes are used as the face boxes (facer.py:61).
  * Results [host]: n_faces, boxes (top_k,4) — the boxes handed to the landmark stage
  * (facer.py:66 boxes_return), kps (top_k,n_points,2), scores (top_k,n_points),
- * det_idx (top_k... max_det) kept detector row indices (parity checks).  Synchronous. */
+ * n_det = the number of boxes the detector kept (every one of them goes through judge_boxs and
+ * sort_and_filter); det_idx (256) and det_rows (256,16), may be NULL: the first min(n_det, 256)
+ * kept row indices and rows (parity checks; skps_pipeline_det_results returns all of them).
+ * Memory: room for every detector row as a kept box plus the NMS workspace, about 108 bytes per
+ * detector row (1.6 MB at 384x640, 15 MB at 1152x1920).  Synchronous. */
 SKPS_API int skps_pipeline_run(skps_pipeline* p, const uint8_t* frame, int H, int W, int frame_on_device,
                       int run_detector, int rw, int rh, int top, int left, float scale,
                       const float* track, int n_track,
                       int32_t* n_faces, float* boxes4, float* kps, float* scores,
                       int32_t* n_det, int32_t* det_idx, float* det_rows, void* stream);
+
+/* Every kept row of the last skps_pipeline_run that ran the detector: det_idx [host] (n_det) and
+ * det_rows [host] (n_det,16), either may be NULL; fails if capacity < n_det.  Copies only n_det
+ * rows from the device.  Synchronous. */
+SKPS_API int skps_pipeline_det_results(skps_pipeline* p, int capacity, int32_t* det_idx, float* det_rows);
 
 /* Mean absolute frame difference vs the previously submitted frame (facer.py:111-113);
  * returns -1.0 in *mean_diff when there is no previous frame of the same size. */
@@ -245,7 +269,9 @@ SKPS_API int skps_head_pose(const float* pts, int N, int img_w, int img_h, const
  * What one FaceAna instance per stream does on the host in the reference (facer.py:52-85 with GroupTrack / OneEuroFilter /
  * EmaFilter of Skps/core/smoother/lk.py:6-162) happens here for up to n_streams streams per call with all per-stream state
  * on the device: one detector forward and one landmark forward per call, batched over the streams.
- * det needs max_batch >= n_streams, kps needs max_batch >= n_streams * cfg->top_k.  Not thread-safe per handle. */
+ * det needs max_batch >= n_streams, kps needs max_batch >= n_streams * cfg->top_k.  Every stream may keep any number of
+ * detector boxes; the NMS output and workspace take about 108 bytes per detector row and stream.  Not thread-safe per
+ * handle. */
 typedef struct skps_mpipe skps_mpipe;
 SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, const skps_pipeline_cfg* cfg, int n_streams,
                                skps_mpipe** out);

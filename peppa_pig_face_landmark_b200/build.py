@@ -28,6 +28,7 @@ SOURCES = {
     "ops_misc.cu": [],
     "debug_ops.cu": [],
     "image_ops.cu": ["-fmad=false"],     # float32/double expressions must round like numpy's
+    "nms.cu": ["-fmad=false"],           # the NMS IoU and scale_coords must round like numpy's
     "align.cu": ["-fmad=false"],         # double source coordinates must round like OpenCV's warpAffine
 }
 

@@ -31,7 +31,7 @@ def letterbox_geometry(h, w, in_h, in_w):
 
 
 class FaceDetector:
-    MAX_DET = 256
+    MAX_DET = 256           # kept rows skps_pipeline_run returns (FaceAna fetches the rest when there are more)
 
     def __init__(self, cfg):
         """cfg: Skps.yml's Detect section.  The engine is built for cfg['input_shape'] ([h, w, 3]): from the export itself
@@ -47,9 +47,13 @@ class FaceDetector:
         torch = rt.require_cuda()
         dev = self.model.device
         self._rows = self.model.out_elems[0] // 16
-        self._kept = torch.zeros((self.MAX_DET, 16), dtype=torch.float32, device=dev)
-        self._idx = torch.zeros((self.MAX_DET,), dtype=torch.int32, device=dev)
+        # every detector row can be a kept box: output and NMS workspace for all of them, sized once here
+        self._kept = torch.zeros((self._rows, 16), dtype=torch.float32, device=dev)
+        self._idx = torch.zeros((self._rows,), dtype=torch.int32, device=dev)
         self._count = torch.zeros((1,), dtype=torch.int32, device=dev)
+        self._recover = torch.zeros((3,), dtype=torch.float32, device=dev)
+        self._ws_bytes = self.lib.skps_detect_post_workspace_size(self._rows, 1)
+        self._ws = torch.empty((self._ws_bytes,), dtype=torch.uint8, device=dev)
         self.last_keep_idx = None
 
     # ------------------------------------------------------------------
@@ -93,14 +97,14 @@ class FaceDetector:
         s.wait_stream(torch.cuda.current_stream(self.model.device))
         scale, left, top = self._letterbox_device(frame, h, w)
         rt.check(self.lib.skps_engine_forward(self.model.handle, self.model.input_ptr(), 1, None, s.cuda_stream))
-        rt.check(self.lib.skps_detect_post(self.model.output_ptr(0), self._rows, self.score_thrs, self.iou_thrs,
-                                           scale, float(left), float(top), self._kept.data_ptr(),
-                                           self._idx.data_ptr(), self._count.data_ptr(), self.MAX_DET,
-                                           s.cuda_stream))
+        with torch.cuda.stream(s):
+            self._recover.copy_(torch.tensor([scale, float(left), float(top)], dtype=torch.float32), non_blocking=False)
+        rt.check(self.lib.skps_detect_post_batch(self.model.output_ptr(0), self._rows, 1, self.score_thrs, self.iou_thrs,
+                                                 self._recover.data_ptr(), self._kept.data_ptr(), self._idx.data_ptr(),
+                                                 self._count.data_ptr(), self._rows, self._ws.data_ptr(), self._ws_bytes,
+                                                 s.cuda_stream))
         s.synchronize()
         n = int(self._count.item())
-        if n < 0:
-            raise RuntimeError("FaceDetector: %d candidates over the score threshold (the NMS kernel ranks at most 1024)" % -n)
         bboxes = self._kept[:n].cpu().numpy()
         self.last_keep_idx = self._idx[:n].cpu().numpy().astype(np.int64)
         logger.info('detect done, time consume: %.5f' % (time.time() - t0))

@@ -124,8 +124,14 @@ class FaceAna():
             landmarks = self._kps[:n].copy() if n else np.array([])
             states = self._scores[:n].copy() if n else np.array([])
             if run_det:
-                self.last_det_idx = self._det_idx[:self._ndet.value].astype(np.int64)
-                self.last_det_rows = self._det_rows[:self._ndet.value].copy()
+                nd = self._ndet.value
+                idx, rows = self._det_idx, self._det_rows
+                if nd > len(idx):
+                    # a crowd: skps_pipeline_run returned the first 256 kept rows, the device holds all of them
+                    idx, rows = np.empty((nd,), np.int32), np.empty((nd, 16), np.float32)
+                    rt.check(self.lib.skps_pipeline_det_results(self._pipe, nd, idx.ctypes.data, rows.ctypes.data))
+                self.last_det_idx = idx[:nd].astype(np.int64)
+                self.last_det_rows = rows[:nd].copy()
         if run_det:
             self.trace.previous_landmarks_set = None
 

@@ -1,6 +1,5 @@
 // Image-side kernels of the FaceAna path (sm_90a): letterbox, per-face crop+resize (both bit-exact
-// with cv2.resize INTER_LINEAR on uint8), detector post-processing (score filter, greedy NMS,
-// un-letterbox), face selection (IoU track match + EMA, area filter, top-k), landmark
+// with cv2.resize INTER_LINEAR on uint8), face selection (IoU track match + EMA, area filter, top-k), landmark
 // de-normalisation and the frame-difference gate.  All HBM-bound byte/index work; compiled with
 // -fmad=false so float32 expressions round exactly like the numpy expressions they restate.
 #include "../../include/skps_b200.h"
@@ -204,123 +203,8 @@ __global__ void nme_kernel(const float* __restrict__ target, const float* __rest
 }
 
 // ------------------------------------------------------------------------------------------
-// Detector post-processing (face_detector.py:31-37, 73-136).  One block.
-//   1. rows with obj > score_thres -> xyxy candidates (more than MAXC: count = -candidates, nothing else written)
-//   2. order = (score desc, row index desc)  [np.argsort(score)[::-1]; ties measure-zero]
-//   3. greedy NMS: survivors are those with iou < iou_thres against every kept box
-//   4. kept rows copied out with cols 0-3 mapped back: (v - pad) / scale
-// ------------------------------------------------------------------------------------------
-constexpr int MAXC = 1024;
-
-__device__ __forceinline__ float iou_nms(const float4 a, const float4 b) {
-    // face_detector.py:117-130, float32 throughout
-    float area = (a.z - a.x) * (a.w - a.y);
-    float xx1 = fmaxf(a.x, b.x), yy1 = fmaxf(a.y, b.y);
-    float xx2 = fminf(a.z, b.z), yy2 = fminf(a.w, b.w);
-    float inter = fmaxf(0.f, yy2 - yy1) * fmaxf(0.f, xx2 - xx1);
-    float other = (b.w - b.y) * (b.z - b.x);
-    return inter / (area + other - inter);
-}
-
-__device__ __forceinline__ void detect_post_body(const float* __restrict__ raw, int rows,
-                                                           float score_thres, float iou_thres,
-                                                           float scale, float pad_x, float pad_y,
-                                                           float* __restrict__ kept_rows, int* __restrict__ kept_idx,
-                                                           int* __restrict__ count, int max_det) {
-    __shared__ int s_n;
-    __shared__ int s_cand[MAXC];         // row index of candidate
-    __shared__ float s_score[MAXC];
-    __shared__ int s_order[MAXC];        // candidate slot by rank
-    __shared__ float4 s_box[MAXC];       // xyxy by rank
-    __shared__ unsigned char s_dead[MAXC];
-    __shared__ int s_keep[256];
-    __shared__ int s_nkeep;
-    const int tid = threadIdx.x, nt = blockDim.x;
-    if (tid == 0) { s_n = 0; s_nkeep = 0; }
-    __syncthreads();
-    for (int r = tid; r < rows; r += nt) {
-        float sc = raw[(long long)r * 16 + 4];
-        if (sc > score_thres) {
-            int slot = atomicAdd(&s_n, 1);
-            if (slot < MAXC) { s_cand[slot] = r; s_score[slot] = sc; }
-        }
-    }
-    __syncthreads();
-    if (s_n > MAXC) {
-        // more candidates than the kernel can rank: refuse (count = -candidates) rather than drop an order-dependent subset;
-        // the host raises.  The reference has no cap (face_detector.py:95-136); 1024 rows over obj 0.5 is a noise frame.
-        if (tid == 0) *count = -s_n;
-        return;
-    }
-    const int n = s_n;
-    // rank sort: key (score desc, row desc) is a total order, so the result is deterministic
-    for (int i = tid; i < n; i += nt) {
-        float si = s_score[i];
-        int ri = s_cand[i];
-        int rank = 0;
-        for (int j = 0; j < n; ++j) {
-            float sj = s_score[j];
-            rank += (sj > si) || (sj == si && s_cand[j] > ri);
-        }
-        s_order[rank] = i;
-    }
-    __syncthreads();
-    for (int k = tid; k < n; k += nt) {
-        const float* r = raw + (long long)s_cand[s_order[k]] * 16;
-        float hw = r[2] / 2.f, hh = r[3] / 2.f;                      // xywh2xyxy, face_detector.py:76-79
-        s_box[k] = make_float4(r[0] - hw, r[1] - hh, r[0] + hw, r[1] + hh);
-        s_dead[k] = 0;
-    }
-    __syncthreads();
-    for (int i = 0; i < n; ++i) {
-        if (s_dead[i]) continue;                 // uniform: shared value, read after barrier
-        if (tid == 0 && s_nkeep < max_det) s_keep[s_nkeep++] = i;
-        const float4 cur = s_box[i];
-        for (int j = i + 1 + tid; j < n; j += nt) {
-            if (!s_dead[j]) {
-                float iou = iou_nms(cur, s_box[j]);
-                if (!(iou < iou_thres)) s_dead[j] = 1;
-            }
-        }
-        __syncthreads();
-    }
-    __syncthreads();
-    const int nk = s_nkeep;
-    if (tid == 0) *count = nk;
-    for (int e = tid; e < nk * 16; e += nt) {
-        int k = e / 16, c = e % 16;
-        int rank = s_keep[k];
-        int row = s_cand[s_order[rank]];
-        float v;
-        if (c < 4) {
-            float4 b = s_box[rank];
-            float bv = c == 0 ? b.x : (c == 1 ? b.y : (c == 2 ? b.z : b.w));
-            v = (bv - ((c & 1) ? pad_y : pad_x)) / scale;           // scale_coords, face_detector.py:86-91
-        } else {
-            v = raw[(long long)row * 16 + c];
-        }
-        kept_rows[k * 16 + c] = v;
-        if (c == 0) kept_idx[k] = row;
-    }
-}
-__global__ void __launch_bounds__(1024) detect_post_kernel(const float* __restrict__ raw, int rows, float score_thres,
-                                                           float iou_thres, float scale, float pad_x, float pad_y,
-                                                           float* __restrict__ kept_rows, int* __restrict__ kept_idx,
-                                                           int* __restrict__ count, int max_det) {
-    detect_post_body(raw, rows, score_thres, iou_thres, scale, pad_x, pad_y, kept_rows, kept_idx, count, max_det);
-}
-__global__ void __launch_bounds__(1024) mp_detect_post_kernel(const MpStreamDesc* __restrict__ d, const float* __restrict__ raw,
-                                                              int rows, float score_thres, float iou_thres,
-                                                              float* __restrict__ kept_rows, int* __restrict__ kept_idx,
-                                                              int* __restrict__ count, int max_det) {
-    const int st = blockIdx.x;
-    const MpStreamDesc D = d[st];
-    detect_post_body(raw + (size_t)rows * 16 * st, rows, score_thres, iou_thres, D.scale, (float)D.left, (float)D.top,
-                     kept_rows + (size_t)16 * max_det * st, kept_idx + (size_t)max_det * st, count + st, max_det);
-}
-
-// ------------------------------------------------------------------------------------------
-// judge_boxs + sort_and_filter (facer.py:120-189).  One warp; K <= 256 detections.
+// judge_boxs + sort_and_filter (facer.py:120-189).  One block of 256 threads per frame, any number of detections.
+// (Detector post-processing, face_detector.py:31-37 and 73-136, is in nms.cu.)
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ float iou_track(const float* r1, const float* r2) {
     float s1 = (r1[2] - r1[0]) * (r1[3] - r1[1]);
@@ -332,58 +216,109 @@ __device__ __forceinline__ float iou_track(const float* r1, const float* r2) {
     return inter / (sum - inter);
 }
 
+constexpr int SEL_THREADS = 256;
+constexpr int SEL_CACHE = 4096;       // selection keys kept in shared memory; later detections recompute theirs
+
+// judge_boxs for one detection: the box after the EMA with the first track box it matches (facer.py:176-181, lk.py:95-96)
+__device__ __forceinline__ void judged_box(const float* now, const float* __restrict__ track, int n_track, float iou_thres,
+                                           float alpha, float oma, float b[4]) {
+    b[0] = now[0]; b[1] = now[1]; b[2] = now[2]; b[3] = now[3];
+    for (int j = 0; j < n_track; ++j) {
+        const float* prev = track + j * 4;
+        if (iou_track(now, prev) > iou_thres) {
+            for (int c = 0; c < 4; ++c) b[c] = alpha * now[c] + oma * prev[c];
+            break;
+        }
+    }
+}
+
+// Selection key of detection i: 0 when its area fails the filter, else (area, i) as one integer with the order of
+// "larger area first, ties by later index first" (facer.py:138 area.argsort()[-k:][::-1], a stable ascending sort read
+// backwards).  +0.f turns an area of -0 into +0, which compares equal to it in float.
+__device__ __forceinline__ unsigned long long select_key(const float* __restrict__ det, int det_stride, int i,
+                                                         const float* __restrict__ track, int n_track, float iou_thres,
+                                                         float alpha, float oma, float min_face) {
+    float b[4];
+    judged_box(det + (long long)i * det_stride, track, n_track, iou_thres, alpha, oma, b);
+    const float area = (b[2] - b[0]) * (b[3] - b[1]);
+    if (!(area > min_face)) return 0ull;
+    const unsigned u = __float_as_uint(area + 0.f);
+    const unsigned ord = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+    return ((unsigned long long)ord << 32) | (unsigned)i;     // ord >= 0x007fffff: a passing key is never 0
+}
+
 __device__ __forceinline__ void select_faces_body(const float* __restrict__ det, int n_det, int det_stride,
                                                   const float* __restrict__ track, int n_track, float iou_thres, float alpha,
                                                   float oma, float min_face, int top_k, float* __restrict__ boxes4,
                                                   int* __restrict__ count) {
-    __shared__ float s_box[256][4];
-    __shared__ float s_area[256];
-    __shared__ int s_sel[256];
+    __shared__ unsigned long long s_key[SEL_CACHE];
+    __shared__ unsigned long long s_best[2][SEL_THREADS / 32];
+    __shared__ int s_wcount[SEL_THREADS / 32];
+    __shared__ int s_sel[64];
     __shared__ int s_m;
-    const int tid = threadIdx.x;
-    const int n = min(n_det, 256);
-    if (tid < n) {
-        const float* now = det + (long long)tid * det_stride;
-        float b[4] = {now[0], now[1], now[2], now[3]};
-        for (int j = 0; j < n_track; ++j) {                           // facer.py:176-181: first match wins
-            const float* prev = track + j * 4;
-            if (iou_track(now, prev) > iou_thres) {
-                for (int c = 0; c < 4; ++c) b[c] = alpha * now[c] + oma * prev[c];   // lk.py:95-96
-                break;
-            }
-        }
-        for (int c = 0; c < 4; ++c) s_box[tid][c] = b[c];
-        s_area[tid] = (b[2] - b[0]) * (b[3] - b[1]);
-    }
+    const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5, nw = nt >> 5;
+    const int n = max(n_det, 0);
+    auto key_of = [&](int i) {
+        return i < SEL_CACHE ? s_key[i] : select_key(det, det_stride, i, track, n_track, iou_thres, alpha, oma, min_face);
+    };
+    if (tid == 0) s_m = 0;
     __syncthreads();
-    if (tid == 0) {
-        // area filter keeps detector order (facer.py:132-136)
-        int m = 0;
-        for (int i = 0; i < n; ++i)
-            if (s_area[i] > min_face) s_sel[m++] = i;
-        if (m > top_k) {
-            // top_k largest areas, descending (facer.py:138: area.argsort()[-k:][::-1]); ties by later index
-            // first, matching a stable ascending sort read backwards.
-            int picked[64];
-            for (int k = 0; k < top_k; ++k) {
-                int best = -1;
-                for (int q = 0; q < m; ++q) {
-                    int i = s_sel[q];
-                    if (i < 0) continue;
-                    if (best < 0 || s_area[i] >= s_area[s_sel[best]]) best = q;
-                }
-                picked[k] = s_sel[best];
-                s_sel[best] = -1;
-            }
-            for (int k = 0; k < top_k; ++k) s_sel[k] = picked[k];
-            m = top_k;
-        }
-        s_m = m;
-        *count = m;
+    int my_m = 0;
+    for (int i = tid; i < n; i += nt) {
+        const unsigned long long k = select_key(det, det_stride, i, track, n_track, iou_thres, alpha, oma, min_face);
+        if (i < SEL_CACHE) s_key[i] = k;
+        my_m += k != 0ull;
     }
+    if (my_m) atomicAdd(&s_m, my_m);
     __syncthreads();
-    const int m = s_m;
-    if (tid < m * 4) boxes4[tid] = s_box[s_sel[tid / 4]][tid % 4];
+    const int m_all = s_m;
+    const int m = min(m_all, top_k);
+    if (m_all <= top_k) {
+        // every face passing the area filter, in detector order (facer.py:132-136)
+        int off = 0;
+        for (int base = 0; base < n; base += nt) {
+            const int i = base + tid;
+            const bool pass = i < n && key_of(i) != 0ull;
+            const unsigned bal = __ballot_sync(0xffffffffu, pass);
+            if (lane == 0) s_wcount[warp] = __popc(bal);
+            __syncthreads();
+            int before = off, total = off;
+            for (int q = 0; q < nw; ++q) {
+                if (q < warp) before += s_wcount[q];
+                total += s_wcount[q];
+            }
+            if (pass) s_sel[before + __popc(bal & ((1u << lane) - 1))] = i;
+            off = total;
+            __syncthreads();
+        }
+    } else {
+        // top_k rounds of a block-wide maximum over the keys below the previous pick
+        unsigned long long prev = ~0ull;
+        for (int k = 0; k < top_k; ++k) {
+            unsigned long long best = 0ull;
+            for (int i = tid; i < n; i += nt) {
+                const unsigned long long q = key_of(i);
+                if (q < prev && q > best) best = q;
+            }
+            for (int o = 16; o > 0; o >>= 1) {
+                const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o);
+                best = other > best ? other : best;
+            }
+            if (lane == 0) s_best[k & 1][warp] = best;
+            __syncthreads();
+            best = 0ull;
+            for (int q = 0; q < nw; ++q) best = s_best[k & 1][q] > best ? s_best[k & 1][q] : best;
+            if (tid == 0) s_sel[k] = (int)(unsigned)(best & 0xffffffffu);
+            prev = best;
+        }
+        __syncthreads();
+    }
+    if (tid == 0) *count = m;
+    if (tid < m * 4) {
+        float b[4];
+        judged_box(det + (long long)s_sel[tid / 4] * det_stride, track, n_track, iou_thres, alpha, oma, b);
+        boxes4[tid] = b[tid % 4];
+    }
 }
 
 __global__ void __launch_bounds__(256) select_faces_kernel(const float* __restrict__ det, const int* __restrict__ det_count,
@@ -396,14 +331,14 @@ __global__ void __launch_bounds__(256) select_faces_kernel(const float* __restri
 // Multi-stream variant (mpipe.cu): block = stream.  flag[s] != 0: this frame ran the detector -> judge_boxs(track, det rows)
 // (facer.py:58); else boxes = the stream's track boxes (facer.py:61).  Track boxes and their count live on the device.
 __global__ void __launch_bounds__(256) mp_select_kernel(const float* __restrict__ det_rows, const int* __restrict__ det_count,
-                                                        int max_det, const int* __restrict__ flag,
+                                                        int det_cap, const int* __restrict__ flag,
                                                         const float* __restrict__ track, const int* __restrict__ n_track,
                                                         float iou_thres, float alpha, float oma, float min_face, int top_k,
                                                         float* __restrict__ boxes4, int* __restrict__ count) {
     const int s = blockIdx.x;
     const float* trk = track + (long long)s * top_k * 4;
     if (flag[s])
-        select_faces_body(det_rows + (long long)s * max_det * 16, det_count[s], 16, trk, n_track[s], iou_thres, alpha, oma,
+        select_faces_body(det_rows + (long long)s * det_cap * 16, det_count[s], 16, trk, n_track[s], iou_thres, alpha, oma,
                           min_face, top_k, boxes4 + (long long)s * top_k * 4, count + s);
     else
         select_faces_body(trk, n_track[s], 4, nullptr, 0, iou_thres, alpha, oma, min_face, top_k,
@@ -526,12 +461,6 @@ int launch_mp_letterbox(const MpStreamDesc* d, uint8_t* out, size_t out_stride, 
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }
-int launch_mp_detect_post(const MpStreamDesc* d, const float* raw, int rows, float score_thres, float iou_thres, float* kept_rows,
-                          int* kept_idx, int* count, int max_det, int n, cudaStream_t s) {
-    mp_detect_post_kernel<<<n, 1024, 0, s>>>(d, raw, rows, score_thres, iou_thres, kept_rows, kept_idx, count, max_det);
-    SKPS_CUDA(cudaGetLastError());
-    return 0;
-}
 int launch_mp_crop(const MpStreamDesc* d, const float* boxes, const int* count, int K, float face_scale, float min_face,
                    uint8_t* crops, int S, int* detail, int n, cudaStream_t s) {
     mp_crop_kernel<<<dim3((S + 255) / 256, S, K * n), 256, 0, s>>>(d, boxes, count, K, face_scale, min_face, crops, S, detail);
@@ -545,10 +474,10 @@ int launch_mp_landmark_post(const float* xy, const int* detail, const int* count
     return 0;
 }
 
-int launch_mp_select(const float* det_rows, const int* det_count, int max_det, const int* flag, const float* track,
+int launch_mp_select(const float* det_rows, const int* det_count, int det_cap, const int* flag, const float* track,
                      const int* n_track, float iou_thres, float alpha, float oma, float min_face, int top_k, float* boxes4,
                      int* count, int n_streams, cudaStream_t s) {
-    mp_select_kernel<<<n_streams, 256, 0, s>>>(det_rows, det_count, max_det, flag, track, n_track, iou_thres, alpha, oma,
+    mp_select_kernel<<<n_streams, SEL_THREADS, 0, s>>>(det_rows, det_count, det_cap, flag, track, n_track, iou_thres, alpha, oma,
                                                 min_face, top_k, boxes4, count);
     SKPS_CUDA(cudaGetLastError());
     return 0;
@@ -570,21 +499,11 @@ extern "C" SKPS_API int skps_letterbox(const uint8_t* frame, int H, int W, int p
     return 0;
 }
 
-extern "C" SKPS_API int skps_detect_post(const float* raw, int rows, float score_thres, float iou_thres, float scale,
-                                float pad_x, float pad_y, float* kept_rows, int32_t* kept_idx, int32_t* count,
-                                int max_det, void* stream) {
-    SKPS_CHECK(raw && kept_rows && kept_idx && count && max_det > 0 && max_det <= 256, "detect_post: bad arguments");
-    detect_post_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(raw, rows, score_thres, iou_thres, scale, pad_x, pad_y,
-                                                            kept_rows, kept_idx, count, max_det);
-    SKPS_CUDA(cudaGetLastError());
-    return 0;
-}
-
 extern "C" SKPS_API int skps_select_faces(const float* det_rows, const int32_t* det_count, int det_stride, const float* track,
                                  int n_track, float iou_thres, float alpha, float one_minus_alpha, float min_face,
                                  int top_k, float* boxes4, int32_t* count, void* stream) {
     SKPS_CHECK(det_rows && det_count && boxes4 && count && top_k > 0 && top_k <= 64, "select_faces: bad arguments");
-    select_faces_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(det_rows, det_count, det_stride, track,
+    select_faces_kernel<<<1, SEL_THREADS, 0, (cudaStream_t)stream>>>(det_rows, det_count, det_stride, track,
                                                             track ? n_track : 0, iou_thres, alpha, one_minus_alpha,
                                                             min_face, top_k, boxes4, count);
     SKPS_CUDA(cudaGetLastError());

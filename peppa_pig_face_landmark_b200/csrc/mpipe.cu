@@ -25,7 +25,7 @@ struct skps_mpipe {
     skps_engine* kps = nullptr;
     skps_pipeline_cfg cfg;
     int device = 0, S = 0, K = 0, P = 0;
-    int det_h = 0, det_w = 0, kps_hw = 0, det_rows = 0, max_det = 256;
+    int det_h = 0, det_w = 0, kps_hw = 0, det_rows = 0;     // every detector row can be a kept box: room for det_rows
     size_t frame_bytes = 0;
     cudaStream_t s_copy = nullptr, s_compute = nullptr;
     // per stream: ring of 3 frames (previous / current / next batch's upload)
@@ -37,7 +37,7 @@ struct skps_mpipe {
         uint8_t* h_stage = nullptr;           // pinned staging for pageable frames [S][frame_bytes]
         int32_t* h_hw = nullptr; int32_t* h_have_prev = nullptr; int32_t* h_geom = nullptr;     // pinned, uploaded per batch
         MpStreamDesc* h_desc = nullptr;       // pinned: per-stream frame pointers + letterbox geometry of this batch
-        int32_t* h_count = nullptr; int32_t* h_flag = nullptr; int32_t* h_det_count = nullptr;
+        int32_t* h_count = nullptr; int32_t* h_flag = nullptr;
         double* h_box = nullptr; double* h_kps = nullptr; float* h_scores = nullptr;
         uint8_t* h_chips = nullptr; double* h_M = nullptr;     // pinned, only while alignment is on
         double* h_pose = nullptr;             // pinned, only while pose is on: rvec, tvec, euler [n][K][3], reproject [n][K][8][2]
@@ -58,6 +58,7 @@ struct skps_mpipe {
     int32_t *d_count = nullptr, *d_detail = nullptr;
     unsigned long long* d_diff = nullptr;
     MpStreamDesc* d_desc = nullptr;           // this batch's descriptors (uploaded on the compute stream, in order)
+    void* d_nms_ws = nullptr;                 // NMS workspace, det_rows candidates per stream
     float *d_det_rows = nullptr, *d_boxes = nullptr, *d_kps_now = nullptr;
     // temporal state
     double *d_prev_lm = nullptr, *d_prev_dx = nullptr, *d_track = nullptr, *d_out_kps = nullptr;
@@ -81,7 +82,7 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
     if (p->s_copy) cudaStreamSynchronize(p->s_copy);
     for (uint8_t* f : p->d_frame) if (f) cudaFree(f);
     for (auto& sl : p->slot) {
-        void* host[] = {sl.h_desc, sl.h_stage, sl.h_hw, sl.h_have_prev, sl.h_geom, sl.h_count, sl.h_flag, sl.h_det_count, sl.h_box,
+        void* host[] = {sl.h_desc, sl.h_stage, sl.h_hw, sl.h_have_prev, sl.h_geom, sl.h_count, sl.h_flag, sl.h_box,
                         sl.h_kps, sl.h_scores, sl.h_chips, sl.h_M, sl.h_pose};
         for (void* q : host) if (q) cudaFreeHost(q);
         if (sl.ev_in) cudaEventDestroy(sl.ev_in);
@@ -89,7 +90,8 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
     }
     void* dev[] = {p->d_desc, p->d_hw, p->d_have_prev, p->d_flag, p->d_det_count, p->d_det_idx, p->d_count, p->d_detail, p->d_diff,
                    p->d_det_rows, p->d_boxes, p->d_kps_now, p->d_prev_lm, p->d_prev_dx, p->d_track, p->d_out_kps,
-                   p->d_track_f32, p->d_n_prev, p->d_prev_f32, p->d_state_idx, p->d_n_track, p->d_chips, p->d_align_M, p->d_pose};
+                   p->d_track_f32, p->d_n_prev, p->d_prev_f32, p->d_state_idx, p->d_n_track, p->d_chips, p->d_align_M, p->d_pose,
+                   p->d_nms_ws};
     for (void* q : dev) if (q) cudaFree(q);
     if (p->s_copy) cudaStreamDestroy(p->s_copy);
     if (p->s_compute) cudaStreamDestroy(p->s_compute);
@@ -148,15 +150,16 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
         MP_HOST(sl.h_hw, sizeof(int32_t) * 2 * S); MP_HOST(sl.h_have_prev, sizeof(int32_t) * S);
         MP_HOST(sl.h_geom, sizeof(int32_t) * 8 * S);
         MP_HOST(sl.h_desc, sizeof(MpStreamDesc) * S);
-        MP_HOST(sl.h_count, sizeof(int32_t) * S); MP_HOST(sl.h_flag, sizeof(int32_t) * S); MP_HOST(sl.h_det_count, sizeof(int32_t) * S);
+        MP_HOST(sl.h_count, sizeof(int32_t) * S); MP_HOST(sl.h_flag, sizeof(int32_t) * S);
         MP_HOST(sl.h_box, sizeof(double) * 4 * K * S); MP_HOST(sl.h_kps, sizeof(double) * 2 * P * K * S);
         MP_HOST(sl.h_scores, sizeof(float) * P * K * S);
         if (cudaEventCreateWithFlags(&sl.ev_in, cudaEventDisableTiming) != cudaSuccess ||
             cudaEventCreateWithFlags(&sl.ev_done, cudaEventDisableTiming) != cudaSuccess) { set_error("cudaEventCreate"); return fail("event"); }
     }
     MP_DEV(p->d_desc, sizeof(MpStreamDesc) * S); MP_DEV(p->d_hw, 8 * S); MP_DEV(p->d_have_prev, 4 * S); MP_DEV(p->d_flag, 4 * S); MP_DEV(p->d_det_count, 4 * S);
-    MP_DEV(p->d_det_idx, 4 * (size_t)p->max_det * S); MP_DEV(p->d_count, 4 * S); MP_DEV(p->d_detail, 4 * 5 * (size_t)K * S);
-    MP_DEV(p->d_diff, 8 * S); MP_DEV(p->d_det_rows, 4 * 16 * (size_t)p->max_det * S); MP_DEV(p->d_boxes, 4 * 4 * (size_t)K * S);
+    MP_DEV(p->d_det_idx, 4 * (size_t)p->det_rows * S); MP_DEV(p->d_count, 4 * S); MP_DEV(p->d_detail, 4 * 5 * (size_t)K * S);
+    MP_DEV(p->d_diff, 8 * S); MP_DEV(p->d_det_rows, 4 * 16 * (size_t)p->det_rows * S);
+    MP_DEV(p->d_nms_ws, nms_workspace_bytes(p->det_rows, S)); MP_DEV(p->d_boxes, 4 * 4 * (size_t)K * S);
     MP_DEV(p->d_kps_now, 4 * 2 * (size_t)P * K * S);
     MP_DEV(p->d_prev_lm, 8 * 2 * 2 * (size_t)P * K * S); MP_DEV(p->d_prev_dx, 8 * 2 * 2 * (size_t)P * K * S);
     MP_DEV(p->d_track, 8 * 4 * (size_t)K * S); MP_DEV(p->d_out_kps, 8 * 2 * (size_t)P * K * S);
@@ -235,10 +238,13 @@ extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8
     // the detector runs for every stream of the batch (one launch sequence); the gate only chooses whose rows are used
     if (skps_engine_forward(p->det, det_in, n, nullptr, sx)) return 1;
     const float* det_out = skps_engine_output_ptr(p->det, 0);
-    if (launch_mp_detect_post(p->d_desc, det_out, p->det_rows, c.score_thres, c.iou_thres, p->d_det_rows, p->d_det_idx,
-                              p->d_det_count, p->max_det, n, sx))
-        return 1;
-    if (launch_mp_select(p->d_det_rows, p->d_det_count, p->max_det, p->d_flag, p->d_track_f32, p->d_n_track, c.track_iou,
+    NmsArgs na = {};
+    na.raw = det_out; na.rows = p->det_rows; na.batch = n; na.score_thres = c.score_thres; na.iou_thres = c.iou_thres;
+    na.desc = p->d_desc; na.limit = p->det_rows; na.capacity = p->det_rows;
+    na.kept_rows = p->d_det_rows; na.kept_idx = p->d_det_idx; na.count = p->d_det_count;
+    na.ws = p->d_nms_ws; na.ws_cap = p->det_rows;
+    if (launch_nms(na, sx)) return 1;
+    if (launch_mp_select(p->d_det_rows, p->d_det_count, p->det_rows, p->d_flag, p->d_track_f32, p->d_n_track, c.track_iou,
                          c.alpha, (float)(1.0 - (double)c.alpha), c.min_face, K, p->d_boxes, p->d_count, n, sx))
         return 1;
     uint8_t* kps_in = (uint8_t*)skps_engine_input_ptr(p->kps);
@@ -283,7 +289,6 @@ extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8
     }
     SKPS_CUDA(cudaMemcpyAsync(sl.h_count, p->d_count, 4 * n, cudaMemcpyDeviceToHost, sx));
     SKPS_CUDA(cudaMemcpyAsync(sl.h_flag, p->d_flag, 4 * n, cudaMemcpyDeviceToHost, sx));
-    SKPS_CUDA(cudaMemcpyAsync(sl.h_det_count, p->d_det_count, 4 * n, cudaMemcpyDeviceToHost, sx));
     SKPS_CUDA(cudaMemcpyAsync(sl.h_box, p->d_track, 8 * 4 * (size_t)K * n, cudaMemcpyDeviceToHost, sx));
     SKPS_CUDA(cudaMemcpyAsync(sl.h_kps, p->d_out_kps, 8 * 2 * (size_t)P * K * n, cudaMemcpyDeviceToHost, sx));
     SKPS_CUDA(cudaMemcpyAsync(sl.h_scores, skps_engine_output_ptr(p->kps, 1), 4 * (size_t)P * K * n, cudaMemcpyDeviceToHost, sx));
@@ -309,8 +314,6 @@ extern "C" SKPS_API int skps_mpipe_wait(skps_mpipe* p, int slot_i, int32_t* n_fa
     sl.busy = false;
     const int K = p->K, P = p->P, n = sl.n;
     for (int s = 0; s < n; ++s) {
-        SKPS_CHECK(!(sl.h_flag[s] && sl.h_det_count[s] < 0), "stream %d: detector produced %d candidates over the score threshold (limit 1024)",
-                   s, -sl.h_det_count[s]);
         n_faces[s] = sl.h_count[s];
         if (ran_detector) ran_detector[s] = sl.h_flag[s];
     }

@@ -35,17 +35,37 @@ struct MpStreamDesc {
     float scale;                 // letterbox geometry (face_detector.py:49-62)
     int rw, rh, top, left;
 };
-// Batched over the streams of a call (grid z / x = stream): what S x {skps_frame_absdiff_sum, skps_letterbox, skps_detect_post,
-// skps_crop_resize, skps_landmark_post} launches did, in five launches.  Same device code per element, bit for bit.
+// Batched over the streams of a call (grid z / x = stream): what S x {skps_frame_absdiff_sum, skps_letterbox,
+// skps_crop_resize, skps_landmark_post} launches did, in four launches.  Same device code per element, bit for bit.
 int launch_mp_absdiff(const MpStreamDesc* d, unsigned long long* diff, int n, size_t max_bytes, cudaStream_t s);
 int launch_mp_letterbox(const MpStreamDesc* d, uint8_t* out, size_t out_stride, int in_h, int in_w, int n, cudaStream_t s);
-int launch_mp_detect_post(const MpStreamDesc* d, const float* raw, int rows, float score_thres, float iou_thres, float* kept_rows,
-                          int* kept_idx, int* count, int max_det, int n, cudaStream_t s);
+
+// Detector post-processing (nms.cu): score filter, sort, greedy NMS and scale_coords of `batch` frames of `rows` raw rows each
+// (raw [batch][rows][16]), for any number of candidates.  Frame f keeps its boxes in kept_rows [f][capacity][16] /
+// kept_idx [f][capacity] and their number, at most capacity, in count[f]; a frame with more than `limit` candidates gets
+// count[f] = -candidates and nothing else.
+struct NmsArgs {
+    const float* raw;
+    int rows, batch;
+    float score_thres, iou_thres;
+    const MpStreamDesc* desc;    // letterbox of frame f: desc[f].scale / left / top, or
+    const float* recover;        // [batch][3] scale, pad_x, pad_y [dev], or (both null) the three scalars below
+    float scale, pad_x, pad_y;
+    int limit, capacity;
+    float* kept_rows;
+    int* kept_idx;
+    int* count;
+    void* ws;                    // nms_workspace_bytes(ws_cap, batch) bytes [dev]
+    int ws_cap;                  // candidates the workspace holds per frame, >= min(rows, limit)
+};
+size_t nms_workspace_bytes(int cap, int batch);
+int launch_nms(const NmsArgs& a, cudaStream_t s);
+
 int launch_mp_crop(const MpStreamDesc* d, const float* boxes, const int* count, int K, float face_scale, float min_face,
                    uint8_t* crops, int S, int* detail, int n, cudaStream_t s);
 int launch_mp_landmark_post(const float* xy, const int* detail, const int* count, int K, int P, float* kps, int n, cudaStream_t s);
 
-int launch_mp_select(const float* det_rows, const int* det_count, int max_det, const int* flag, const float* track,
+int launch_mp_select(const float* det_rows, const int* det_count, int det_cap, const int* flag, const float* track,
                      const int* n_track, float iou_thres, float alpha, float oma, float min_face, int top_k, float* boxes4,
                      int* count, int n_streams, cudaStream_t s);
 int launch_mp_decide(const unsigned long long* diff, const int* hw, const int* have_prev, int* flag, int n, cudaStream_t s);

@@ -20,7 +20,9 @@ struct skps_pipeline {
     skps_pipeline_cfg cfg;
     int device = 0;
     int det_h = 0, det_w = 0, kps_hw = 0, n_points = 0, det_rows = 0;
-    int max_det = 256;
+    static constexpr int RUN_DET = 256;           // kept rows skps_pipeline_run returns; skps_pipeline_det_results has all
+    int last_n_det = 0;                           // kept boxes of the last detector run
+    void* d_nms_ws = nullptr;                     // NMS workspace for det_rows candidates
     uint8_t* d_frame[2] = {nullptr, nullptr};     // current / previous frame
     int cur = 0;
     int prev_h = 0, prev_w = 0;                   // size of the frame in d_frame[cur^1] (0 = none)
@@ -50,7 +52,7 @@ extern "C" SKPS_API void skps_pipeline_destroy(skps_pipeline* p) {
     cudaSetDevice(p->device);
     for (int i = 0; i < 2; ++i) if (p->d_frame[i]) cudaFree(p->d_frame[i]);
     if (p->h_frame) cudaFreeHost(p->h_frame);
-    void* dev[] = {p->d_det_rows, p->d_det_idx, p->d_det_count, p->d_track, p->d_boxes, p->d_count, p->d_detail,
+    void* dev[] = {p->d_det_rows, p->d_det_idx, p->d_det_count, p->d_nms_ws, p->d_track, p->d_boxes, p->d_count, p->d_detail,
                    p->d_kps, p->d_diff, p->d_align_kps, p->d_align_M, p->d_chips,
                    p->d_pose_kps, p->d_pose};
     for (void* q : dev) if (q) cudaFree(q);
@@ -82,9 +84,11 @@ extern "C" SKPS_API int skps_pipeline_create(skps_engine* det, skps_engine* kps,
 #define HALLOC(ptr, bytes) SKPS_CUDA(cudaMallocHost((void**)&(ptr), (bytes)))
     PALLOC(p->d_frame[0], fbytes); PALLOC(p->d_frame[1], fbytes);
     HALLOC(p->h_frame, fbytes);
-    PALLOC(p->d_det_rows, sizeof(float) * 16 * p->max_det);
-    PALLOC(p->d_det_idx, sizeof(int32_t) * p->max_det);
+    // every row of the detector can be a kept box: room for all of them, sized once here
+    PALLOC(p->d_det_rows, sizeof(float) * 16 * p->det_rows);
+    PALLOC(p->d_det_idx, sizeof(int32_t) * p->det_rows);
     PALLOC(p->d_det_count, sizeof(int32_t));
+    PALLOC(p->d_nms_ws, nms_workspace_bytes(p->det_rows, 1));
     PALLOC(p->d_track, sizeof(float) * 4 * 256);
     PALLOC(p->d_boxes, sizeof(float) * 4 * K);
     PALLOC(p->d_count, sizeof(int32_t));
@@ -95,8 +99,8 @@ extern "C" SKPS_API int skps_pipeline_create(skps_engine* det, skps_engine* kps,
     HALLOC(p->h_boxes, sizeof(float) * 4 * K);
     HALLOC(p->h_kps, sizeof(float) * 2 * P * K);
     HALLOC(p->h_scores, sizeof(float) * P * K);
-    HALLOC(p->h_det_idx, sizeof(int32_t) * p->max_det);
-    HALLOC(p->h_det_rows, sizeof(float) * 16 * p->max_det);
+    HALLOC(p->h_det_idx, sizeof(int32_t) * skps_pipeline::RUN_DET);
+    HALLOC(p->h_det_rows, sizeof(float) * 16 * skps_pipeline::RUN_DET);
     HALLOC(p->h_track, sizeof(float) * 4 * 256);
     SKPS_CUDA(cudaMemset(p->d_det_count, 0, sizeof(int32_t)));
     *out = p;
@@ -186,9 +190,14 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, const uint8_t* frame
         uint8_t* det_in = (uint8_t*)skps_engine_input_ptr(p->det);
         if (skps_letterbox(d_frame, H, W, W * 3, det_in, p->det_h, p->det_w, rw, rh, top, left, s)) return 1;
         if (skps_engine_forward(p->det, det_in, 1, nullptr, s)) return 1;
-        if (skps_detect_post(skps_engine_output_ptr(p->det, 0), p->det_rows, c.score_thres, c.iou_thres, scale,
-                             (float)left, (float)top, p->d_det_rows, p->d_det_idx, p->d_det_count, p->max_det, s))
-            return 1;
+        NmsArgs na = {};
+        na.raw = skps_engine_output_ptr(p->det, 0); na.rows = p->det_rows; na.batch = 1;
+        na.score_thres = c.score_thres; na.iou_thres = c.iou_thres;
+        na.scale = scale; na.pad_x = (float)left; na.pad_y = (float)top;
+        na.limit = p->det_rows; na.capacity = p->det_rows;
+        na.kept_rows = p->d_det_rows; na.kept_idx = p->d_det_idx; na.count = p->d_det_count;
+        na.ws = p->d_nms_ws; na.ws_cap = p->det_rows;
+        if (launch_nms(na, s)) return 1;
         // facer.py:58 judge_boxs(track_box, boxes) then :64 sort_and_filter
         if (skps_select_faces(p->d_det_rows, p->d_det_count, 16, n_track > 0 ? p->d_track : nullptr, n_track,
                               c.track_iou, c.alpha, (float)(1.0 - (double)c.alpha), c.min_face, K, p->d_boxes,
@@ -216,12 +225,14 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, const uint8_t* frame
                               cudaMemcpyDeviceToHost, s));
     if (run_detector) SKPS_CUDA(cudaMemcpyAsync(&p->h_res->n_det, p->d_det_count, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     if (run_detector && n_det) {
-        SKPS_CUDA(cudaMemcpyAsync(p->h_det_idx, p->d_det_idx, sizeof(int32_t) * p->max_det, cudaMemcpyDeviceToHost, s));
-        SKPS_CUDA(cudaMemcpyAsync(p->h_det_rows, p->d_det_rows, sizeof(float) * 16 * p->max_det, cudaMemcpyDeviceToHost, s));
+        // the first RUN_DET kept rows (what callers of this function size their buffers for); the rest stay on the device
+        // for skps_pipeline_det_results
+        const int R = skps_pipeline::RUN_DET < p->det_rows ? skps_pipeline::RUN_DET : p->det_rows;
+        SKPS_CUDA(cudaMemcpyAsync(p->h_det_idx, p->d_det_idx, sizeof(int32_t) * R, cudaMemcpyDeviceToHost, s));
+        SKPS_CUDA(cudaMemcpyAsync(p->h_det_rows, p->d_det_rows, sizeof(float) * 16 * R, cudaMemcpyDeviceToHost, s));
     }
     SKPS_CUDA(cudaStreamSynchronize(s));
-    SKPS_CHECK(!run_detector || p->h_res->n_det >= 0, "detector produced %d candidates over the score threshold (limit 1024)",
-               -p->h_res->n_det);
+    if (run_detector) p->last_n_det = p->h_res->n_det;
     const int nf = p->h_res->n_faces;
     *n_faces = nf;
     memcpy(boxes4, p->h_boxes, sizeof(float) * 4 * nf);
@@ -229,12 +240,26 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, const uint8_t* frame
     memcpy(scores, p->h_scores, sizeof(float) * P * nf);
     if (n_det) {
         *n_det = run_detector ? p->h_res->n_det : 0;
-        if (run_detector && det_idx) memcpy(det_idx, p->h_det_idx, sizeof(int32_t) * (*n_det));
-        if (run_detector && det_rows) memcpy(det_rows, p->h_det_rows, sizeof(float) * 16 * (*n_det));
+        const int nr = *n_det < skps_pipeline::RUN_DET ? *n_det : skps_pipeline::RUN_DET;
+        if (run_detector && det_idx) memcpy(det_idx, p->h_det_idx, sizeof(int32_t) * nr);
+        if (run_detector && det_rows) memcpy(det_rows, p->h_det_rows, sizeof(float) * 16 * nr);
     }
     // the frame just processed becomes "previous" for the next frame_diff (facer.py:57,62)
     p->prev_h = H; p->prev_w = W;
     p->cur ^= 1;
+    return 0;
+}
+
+// Every kept row of the last detector run, copied from the device on request: a crowd can keep thousands of boxes, and
+// skps_pipeline_run returns only the first 256 so that no frame pays for copying them all.
+extern "C" SKPS_API int skps_pipeline_det_results(skps_pipeline* p, int capacity, int32_t* det_idx, float* det_rows) {
+    SKPS_CHECK(p, "pipeline_det_results: null");
+    const int n = p->last_n_det;
+    SKPS_CHECK(capacity >= n, "pipeline_det_results: the last detector run kept %d boxes, capacity is %d", n, capacity);
+    if (n == 0) return 0;
+    SKPS_CUDA(cudaSetDevice(p->device));
+    if (det_idx) SKPS_CUDA(cudaMemcpy(det_idx, p->d_det_idx, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
+    if (det_rows) SKPS_CUDA(cudaMemcpy(det_rows, p->d_det_rows, sizeof(float) * 16 * n, cudaMemcpyDeviceToHost));
     return 0;
 }
 

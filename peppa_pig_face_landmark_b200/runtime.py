@@ -64,6 +64,9 @@ SIGNATURES = {
                                  C.c_int, C.c_int, C.c_int, C.c_int, c_vp]),
     "skps_detect_post": (C.c_int, [c_vp, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
                                    c_vp, c_vp, c_vp, C.c_int, c_vp]),
+    "skps_detect_post_workspace_size": (C.c_size_t, [C.c_int, C.c_int]),
+    "skps_detect_post_batch": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_float, C.c_float, c_vp, c_vp, c_vp, c_vp, C.c_int,
+                                         c_vp, C.c_size_t, c_vp]),
     "skps_select_faces": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, C.c_int, C.c_float, C.c_float, C.c_float,
                                     C.c_float, C.c_int, c_vp, c_vp, c_vp]),
     "skps_crop_resize": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, C.c_int, C.c_float, C.c_float,
@@ -76,6 +79,7 @@ SIGNATURES = {
     "skps_pipeline_run": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_int, C.c_float, c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
                                     c_vp]),
+    "skps_pipeline_det_results": (C.c_int, [c_vp, C.c_int, c_vp, c_vp]),
     "skps_crop_rect": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, C.c_int, c_vp]),
     "skps_nme": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
     "skps_head_pose": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
