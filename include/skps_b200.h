@@ -94,6 +94,16 @@ SKPS_API int skps_engine_launches_for_batch(const skps_engine* e, int batch);
 /* Profiling: enqueue only op `op_index` of the plan on the buffers left by the last forward
  * (bench.py times the dominant kernel with CUDA events around this call). */
 SKPS_API int skps_engine_run_op(skps_engine* e, int op_index, int batch, void* stream);
+/* Which kernel op `op_index` runs and the geometry it picked (for tests that must know which branch they exercised).
+ * Returns a SKPS_KERNEL_* id, or -1 on a bad index.  info[0..3] (zero where unused):
+ *   TC: bw, bh (output pixels of a 128-pixel tile), ipt (images per tile), mt (pixel tiles per weight tile);
+ *   TCT: bh (output rows per 256-pixel tile);  DW_TMA: output rows per tile (tiles are 16 columns wide). */
+enum {
+    SKPS_KERNEL_MISC = 0, SKPS_KERNEL_TC = 1, SKPS_KERNEL_TCT = 2, SKPS_KERNEL_HM = 3, SKPS_KERNEL_MMA = 4,
+    SKPS_KERNEL_XF = 5, SKPS_KERNEL_SIMT_CONV = 6, SKPS_KERNEL_DW_TMA = 7, SKPS_KERNEL_DW = 8,
+    SKPS_KERNEL_UPCAT_TMA = 9, SKPS_KERNEL_UPCAT = 10, SKPS_KERNEL_STEM_BLOCK = 11
+};
+SKPS_API int skps_engine_op_kernel(const skps_engine* e, int op_index, int32_t info[4]);
 
 /* Unit-test entry for the wgmma convolution kernel (csrc/conv_tc.cu): one 'same' conv on host
  * data.  x float32 NHWC, w_hi/w_lo float16 (n_tiles*n_tile, K_pad) as packed by

@@ -472,6 +472,42 @@ extern "C" SKPS_API int skps_engine_run_op(skps_engine* e, int op_index, int bat
     return run_ops(e, batch, (cudaStream_t)stream, op_index, op_index + 1);
 }
 
+// The branch run_ops() takes for one op, and the tiling its kernel was prepared with.
+extern "C" SKPS_API int skps_engine_op_kernel(const skps_engine* e, int op_index, int32_t info[4]) {
+    if (!e || op_index < 0 || op_index >= (int)e->ops.size()) return -1;
+    int32_t tmp[4];
+    int32_t* inf = info ? info : tmp;
+    inf[0] = inf[1] = inf[2] = inf[3] = 0;
+    const size_t i = (size_t)op_index;
+    const OpDesc& op = e->ops[i];
+    switch (op.type) {
+        case OP_CONV:
+            if (op.flags & FLAG_MMA) return SKPS_KERNEL_MMA;
+            if (op.flags & FLAG_XF) return SKPS_KERNEL_XF;
+            if (op.flags & FLAG_TC) {
+                if (e->hm[i].valid) return SKPS_KERNEL_HM;
+                if (e->tct[i].valid) {
+                    inf[0] = e->tct[i].k.bh;
+                    return SKPS_KERNEL_TCT;
+                }
+                const TcK& k = e->tc[i].k;
+                inf[0] = k.bw; inf[1] = k.bh; inf[2] = k.ipt; inf[3] = k.mt;
+                return SKPS_KERNEL_TC;
+            }
+            return SKPS_KERNEL_SIMT_CONV;
+        case OP_DWCONV:
+            if (e->dwt[i].valid) {
+                inf[0] = dw_tile_rows(e->dwt[i].k_size, e->dwt[i].stride);
+                return SKPS_KERNEL_DW_TMA;
+            }
+            return SKPS_KERNEL_DW;
+        case OP_DWPW: return SKPS_KERNEL_XF;
+        case OP_UPCAT_DW: return e->upt[i].valid ? SKPS_KERNEL_UPCAT_TMA : SKPS_KERNEL_UPCAT;
+        case OP_STEM_BLOCK: return SKPS_KERNEL_STEM_BLOCK;
+        default: return SKPS_KERNEL_MISC;
+    }
+}
+
 // Enqueue the op sequence (through a cached CUDA graph when possible).
 static int enqueue(skps_engine* e, int batch, cudaStream_t s) {
     if (!e->use_graph || s == nullptr) return run_ops(e, batch, s);   // the legacy default stream cannot be captured
