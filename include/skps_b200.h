@@ -97,11 +97,12 @@ SKPS_API int skps_engine_run_op(skps_engine* e, int op_index, int batch, void* s
 /* Which kernel op `op_index` runs and the geometry it picked (for tests that must know which branch they exercised).
  * Returns a SKPS_KERNEL_* id, or -1 on a bad index.  info[0..3] (zero where unused):
  *   TC: bw, bh (output pixels of a 128-pixel tile), ipt (images per tile), mt (pixel tiles per weight tile);
- *   TCT: bh (output rows per 256-pixel tile);  DW_TMA: output rows per tile (tiles are 16 columns wide). */
+ *   TCT: bh (output rows per 256-pixel tile);  DW_TMA: output rows per tile (tiles are 16 columns wide);
+ *   PW: output channels per work unit, work units per 128-pixel tile. */
 enum {
     SKPS_KERNEL_MISC = 0, SKPS_KERNEL_TC = 1, SKPS_KERNEL_TCT = 2, SKPS_KERNEL_HM = 3, SKPS_KERNEL_MMA = 4,
     SKPS_KERNEL_XF = 5, SKPS_KERNEL_SIMT_CONV = 6, SKPS_KERNEL_DW_TMA = 7, SKPS_KERNEL_DW = 8,
-    SKPS_KERNEL_UPCAT_TMA = 9, SKPS_KERNEL_UPCAT = 10, SKPS_KERNEL_STEM_BLOCK = 11
+    SKPS_KERNEL_UPCAT_TMA = 9, SKPS_KERNEL_UPCAT = 10, SKPS_KERNEL_STEM_BLOCK = 11, SKPS_KERNEL_PW = 12
 };
 SKPS_API int skps_engine_op_kernel(const skps_engine* e, int op_index, int32_t info[4]);
 
@@ -119,6 +120,16 @@ SKPS_API int skps_debug_conv_tc2(const float* x, int N, int H, int W, int Cin, c
                                  const float* bias, int Cout, int ksize, int dil, int act, int n_tile, int n_tiles,
                                  float out_scale, const float* residual, int out_split, float* out, int stride,
                                  int res_first, int max_batch);
+
+/* Unit-test entry of the pointwise kernel (csrc/conv_pw.cu): one 1x1 stride-1 conv of the first `batch` images of
+ * host buffers holding max_batch.  x float32 (max_batch, H, W, in_ld), read at channels [in_coff, in_coff + Cin); w_hi/w_lo
+ * float16 (n_tiles*n_tile, K_pad) as packed by plan.pack_tc_weights; act none, ReLU or h-swish; out float32
+ * (max_batch, H, W, out_ld), in and out: the conv writes channels [out_coff, out_coff + Cout) of the first batch*H*W
+ * pixels (through split-fp16 planes when out_split != 0) and leaves the rest as it came in.  Fails for a layer the
+ * kernel does not take (unaligned views, Cout not a multiple of 8). */
+SKPS_API int skps_debug_conv_pw(const float* x, int batch, int max_batch, int H, int W, int Cin, int in_ld, int in_coff,
+                                const void* w_hi, const void* w_lo, const float* bias, int Cout, int act, int n_tile,
+                                int n_tiles, float out_scale, int out_split, int out_ld, int out_coff, float* out);
 
 /* Unit-test entry of the transposed heat-map head kernel (csrc/conv_hm.cu; kps graph /student/hm/Conv + the arg-max half of
  * postp, TRAIN/face_landmark/lib/core/base_trainer/model.py:511-554): x float32 NHWC, w_hi/w_lo (n_tile, K_pad) float16 as

@@ -22,6 +22,7 @@ SOURCES = {
     "conv_xf.cu": [],
     "conv_hm.cu": [],
     "conv_tct.cu": [],
+    "conv_pw.cu": [],
     "stem_block.cu": [],
     "conv_mma.cu": [],
     "dw_tma.cu": [],

@@ -16,6 +16,9 @@
 //   32-column chunks of the tile (the chunks alternate between them) and run the epilogue on them
 //   (registers -> bias/act/residual -> global).  Persistent CTAs, one per SM; the producer fills the next
 //   stages while the epilogue of a tile runs.
+// * Which layers run here: the engine gives the heat-map head to conv_hm.cu, k x k convs with Cout 96-128 to conv_tct.cu and
+//   1x1 stride-1 layers without residual or SiLU to conv_pw.cu, in that order; conv_tc takes the rest (the dilated ASPP
+//   convs, stride-2, residual and SiLU layers, channel-shuffled outputs).  skps_debug_conv_tc2 still runs 1x1 layers here.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <stdlib.h>

@@ -14,6 +14,7 @@
 #include "common.h"
 #include "conv_mma.h"
 #include "conv_hm.h"
+#include "conv_pw.h"
 #include "conv_tc.h"
 #include "conv_tct.h"
 #include "conv_xf.h"
@@ -54,6 +55,7 @@ struct skps_engine {
     int num_sms = 132;
     std::vector<TcLayer> tc;              // per op; valid where ops[i].flags & FLAG_TC
     std::vector<TctLayer> tct;            // per op; valid where the transposed kernel (conv_tct.cu) takes the layer
+    std::vector<PwLayer> pw;              // per op; valid where the pointwise kernel (conv_pw.cu) takes the layer
     std::vector<HmLayer> hm;              // per op; valid for the heat-map head when its partial rows are 256-pixel tiles
     std::vector<ConvMmaLayer> mma;        // per op; valid where ops[i].flags & FLAG_MMA
     std::vector<XfLayer> xf;              // per op; fused producer -> pointwise conv layers (OP_DWPW, OP_CONV with FLAG_XF)
@@ -119,6 +121,10 @@ static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int
                     }
                     if (e->tct[i].valid) {
                         rc = tct_launch(e->tct[i], batch, e->num_sms, s);
+                        break;
+                    }
+                    if (e->pw[i].valid) {
+                        rc = pw_launch(e->pw[i], batch, e->num_sms, s);
                         break;
                     }
                     rc = tc_launch(e->tc[i], batch, e->num_sms, s);
@@ -295,6 +301,7 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
     e->tc.resize(n_ops);
     e->hm.resize(n_ops);
     e->tct.resize(n_ops);
+    e->pw.resize(n_ops);
     for (int i = 0; i < n_ops; ++i) {
         const OpDesc& op = e->ops[i];
         if (op.type != OP_CONV || !(op.flags & FLAG_TC) || (op.flags & FLAG_XF)) continue;
@@ -327,6 +334,10 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
         }
         if (op.dh == op.dw && op.ph == op.pw && tct_applicable(s)) {
             if (tct_prepare(e->tct[i], s)) return fail_op(i, "tct");
+            continue;
+        }
+        if (op.ph == op.pw && pw_applicable(s)) {
+            if (pw_prepare(e->pw[i], s)) return fail_op(i, "pw");
             continue;
         }
         if (op.dh != op.dw || op.ph != op.pw || tc_prepare(e->tc[i], s)) return fail_op(i, "tc");
@@ -489,6 +500,10 @@ extern "C" SKPS_API int skps_engine_op_kernel(const skps_engine* e, int op_index
                 if (e->tct[i].valid) {
                     inf[0] = e->tct[i].k.bh;
                     return SKPS_KERNEL_TCT;
+                }
+                if (e->pw[i].valid) {
+                    inf[0] = e->pw[i].nc; inf[1] = e->pw[i].k.n_chunks;
+                    return SKPS_KERNEL_PW;
                 }
                 const TcK& k = e->tc[i].k;
                 inf[0] = k.bw; inf[1] = k.bh; inf[2] = k.ipt; inf[3] = k.mt;

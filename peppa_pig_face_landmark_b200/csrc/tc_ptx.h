@@ -1,12 +1,14 @@
-// PTX wrappers shared by the tensor-core kernels (conv_tc.cu, conv_tct.cu, conv_hm.cu, conv_xf.cu, stem_block.cu): mbarrier,
-// TMA, wgmma and its shared-memory matrix descriptors.  sm_90a.
+// PTX wrappers shared by the tensor-core kernels (conv_tc.cu, conv_tct.cu, conv_pw.cu, conv_hm.cu, conv_xf.cu, stem_block.cu):
+// mbarrier, TMA, wgmma and its shared-memory matrix descriptors.  sm_90a.
 //
 // The accumulator of a 128-row tile lives in the registers of the warpgroup that issues the wgmma instructions: one
 // m64nNk16 per 64-row half, so a warp holds rows 16w..16w+15 of each half.
-// conv_tct, conv_hm and stem_block issue wgmma_f16<N> / wg_mma3<N> from straight-line code, keep a group in flight with
-// wg_wait<1> where they pipeline, and read the accumulator fragment directly in their epilogues.
-// conv_tc and conv_xf still issue wg_mma3_128x32 per 32-column chunk and hand each chunk to a one-row-per-thread epilogue
-// layout (row 32q + lane of warp q, 32 consecutive columns) with wg_rows32, through 16 KB of shared memory.
+// conv_tct (k x k convs with Cout 96-128), conv_pw (1x1 stride-1 convs without residual or SiLU), conv_hm and stem_block
+// issue wgmma_f16<N> / wg_mma3<N> from straight-line code, keep a group in flight with wg_wait<1> where they pipeline, and
+// read the accumulator fragment directly in their epilogues.
+// conv_tc (the layers left: dilated ASPP, stride-2, residual and SiLU convs, channel-shuffled outputs) and conv_xf still
+// issue wg_mma3_128x32 per 32-column chunk and hand each chunk to a one-row-per-thread epilogue layout (row 32q + lane of
+// warp q, 32 consecutive columns) with wg_rows32, through 16 KB of shared memory.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>

@@ -24,9 +24,10 @@ from peppa_pig_face_landmark_b200 import plan as P  # noqa: E402
 from oracle.plan_interp import PlanInterp, rd, split16_round, _act  # noqa: E402
 
 KERNELS = {0: "misc", 1: "tc", 2: "tct", 3: "hm", 4: "mma", 5: "xf", 6: "simt", 7: "dw_tma", 8: "dw", 9: "upcat_tma",
-           10: "upcat", 11: "stem_block"}
-K_MISC, K_TC, K_TCT, K_HM, K_MMA, K_XF, K_SIMT, K_DW_TMA, K_DW, K_UPCAT_TMA, K_UPCAT, K_STEM = range(12)
-TENSOR_CORE = (K_TC, K_TCT, K_HM, K_MMA, K_XF)
+           10: "upcat", 11: "stem_block", 12: "pw"}
+K_MISC, K_TC, K_TCT, K_HM, K_MMA, K_XF, K_SIMT, K_DW_TMA, K_DW, K_UPCAT_TMA, K_UPCAT, K_STEM, K_PW = range(13)
+TENSOR_CORE = (K_TC, K_TCT, K_HM, K_MMA, K_XF, K_PW)
+PW_BM = 128                    # pixels per conv_pw tile: the tiles run over the flat (n, y, x) index of the batch
 
 U = 2.0 ** -24                 # unit roundoff of float32 (round to nearest)
 
@@ -438,8 +439,14 @@ def _stored(op):
     return list(op.outs)
 
 
-def edge_tile(kernel, info, H, W, y, x):
-    """Whether output pixel (y, x) of an H x W map lies in a tile that hangs over the map's border."""
+def edge_tile(kernel, info, H, W, y, x, n=None, batch=None):
+    """Whether output pixel (y, x) of an H x W map lies in a tile that hangs over the map's border; for conv_pw, whether
+    pixel (n, y, x) lies in the last, partial tile of a batch of `batch` maps."""
+    if kernel == K_PW:
+        if n is None or batch is None:
+            return None
+        rows = batch * H * W
+        return bool(rows % PW_BM and (n * H + y) * W + x >= rows // PW_BM * PW_BM)
     if kernel == K_TC and info[2] == 1:
         bw, bh = info[0], info[1]
     elif kernel == K_DW_TMA:
@@ -627,7 +634,7 @@ def check_ops(ex, x_u8, log=None, keep=None):
         res.ratio, res.where, rows = evaluate(op, kernel, info, interp, ins, got, batch)
         if res.where is not None and res.where[2] >= 0:
             o = op.outs[0]
-            res.edge = edge_tile(kernel, info, o.H, o.W, res.where[1], res.where[2])
+            res.edge = edge_tile(kernel, info, o.H, o.W, res.where[1], res.where[2], res.where[0], batch)
         if keep is not None and keep(res):
             detail[i] = (got, rows)
         results.append(res)
@@ -668,7 +675,8 @@ def tc_geometry(r):
 
 BRANCHES = ["tc bw=%d ragged %s" % (bw, side) for bw in (64, 32, 16, 8) for side in ("right", "bottom")] + [
     "tc ipt>1", "tc mt=2 odd tile count", "tc stride 2 ragged", "tct", "simt conv W<8",
-    "dw_tma s1 W<16", "dw_tma s1 W>=16", "dw_tma s2 W<16", "dw_tma s2 W>=16", "upcat_tma", "dwpw H%8!=0", "stem block"]
+    "dw_tma s1 W<16", "dw_tma s1 W>=16", "dw_tma s2 W<16", "dw_tma s2 W>=16", "upcat_tma", "dwpw H%8!=0", "stem block",
+    "pw partial last tile", "pw N chunks > 1"]
 
 
 def coverage(tagged):
@@ -691,6 +699,11 @@ def coverage(tagged):
                 hit.append("tc stride 2 ragged")
         elif r.kernel == K_TCT:
             hit.append("tct")
+        elif r.kernel == K_PW:
+            if (r.batch * o.H * o.W) % PW_BM:
+                hit.append("pw partial last tile")
+            if r.info[1] > 1:
+                hit.append("pw N chunks > 1")
         elif r.kernel == K_SIMT and o.W < 8:
             hit.append("simt conv W<8")
         elif r.kernel == K_DW_TMA:
