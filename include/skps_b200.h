@@ -98,11 +98,13 @@ SKPS_API int skps_engine_run_op(skps_engine* e, int op_index, int batch, void* s
  * Returns a SKPS_KERNEL_* id, or -1 on a bad index.  info[0..3] (zero where unused):
  *   TC: bw, bh (output pixels of a 128-pixel tile), ipt (images per tile), mt (pixel tiles per weight tile);
  *   TCT: bh (output rows per 256-pixel tile);  DW_TMA: output rows per tile (tiles are 16 columns wide);
- *   PW: output channels per work unit, work units per 128-pixel tile. */
+ *   PW: output channels per work unit, work units per 128-pixel tile;
+ *   FPW: pixels per tile (128, 16 x 8), output channels per work unit, work units per tile, mode (0 scale, 1 depthwise). */
 enum {
     SKPS_KERNEL_MISC = 0, SKPS_KERNEL_TC = 1, SKPS_KERNEL_TCT = 2, SKPS_KERNEL_HM = 3, SKPS_KERNEL_MMA = 4,
     SKPS_KERNEL_XF = 5, SKPS_KERNEL_SIMT_CONV = 6, SKPS_KERNEL_DW_TMA = 7, SKPS_KERNEL_DW = 8,
-    SKPS_KERNEL_UPCAT_TMA = 9, SKPS_KERNEL_UPCAT = 10, SKPS_KERNEL_STEM_BLOCK = 11, SKPS_KERNEL_PW = 12
+    SKPS_KERNEL_UPCAT_TMA = 9, SKPS_KERNEL_UPCAT = 10, SKPS_KERNEL_STEM_BLOCK = 11, SKPS_KERNEL_PW = 12,
+    SKPS_KERNEL_FPW = 13
 };
 SKPS_API int skps_engine_op_kernel(const skps_engine* e, int op_index, int32_t info[4]);
 
@@ -146,6 +148,13 @@ SKPS_API int skps_debug_conv_xf(int mode, const float* x, int N, int H, int W, i
                                 const float* gate, const float* dww, int dw_act, const void* w_hi, const void* w_lo,
                                 const float* bias, int Cout, int act, int n_tile, float out_scale, const float* residual,
                                 int res_first, int out_split, float* out, const float* weff);
+/* The same layer through the register-accumulator kernel (csrc/conv_fpw.cu), for images [0, batch) of N: `out` is read
+ * as well as written, and images past the batch must come back as they went in.  Fails for a layer conv_fpw does not take
+ * (maps not made of whole 16 x 8 tiles, widths it does not instantiate). */
+SKPS_API int skps_debug_conv_fpw(int mode, const float* x, int N, int H, int W, int Cx, int x_split, const float* low, int Cl,
+                                 const float* gate, const float* dww, int dw_act, const void* w_hi, const void* w_lo,
+                                 const float* bias, int Cout, int act, int n_tile, float out_scale, const float* residual,
+                                 int res_first, int out_split, float* out, const float* weff, int batch);
 
 /* Unit-test entries for two fused kernels that otherwise only run inside a whole network (csrc/debug_ops.cu):
  * the squeeze-excite gate (mean of per-tile channel sums -> FC -> act -> FC -> act; kps_student.onnx .../se/ nodes) and the

@@ -23,6 +23,7 @@ SOURCES = {
     "conv_hm.cu": [],
     "conv_tct.cu": [],
     "conv_pw.cu": [],
+    "conv_fpw.cu": [],
     "stem_block.cu": [],
     "conv_mma.cu": [],
     "dw_tma.cu": [],

@@ -17,6 +17,7 @@
 #include "conv_pw.h"
 #include "conv_tc.h"
 #include "conv_tct.h"
+#include "conv_fpw.h"
 #include "conv_xf.h"
 #include "dw_tma.h"
 #include "stem_block.h"
@@ -59,6 +60,7 @@ struct skps_engine {
     std::vector<HmLayer> hm;              // per op; valid for the heat-map head when its partial rows are 256-pixel tiles
     std::vector<ConvMmaLayer> mma;        // per op; valid where ops[i].flags & FLAG_MMA
     std::vector<XfLayer> xf;              // per op; fused producer -> pointwise conv layers (OP_DWPW, OP_CONV with FLAG_XF)
+    std::vector<FpwLayer> fpw;            // per op; valid where the register-accumulator kernel (conv_fpw.cu) takes such a layer
     std::vector<DwTmaLayer> dwt;          // per op; TMA-staged depthwise layers (valid flag)
     std::vector<UpcatTmaLayer> upt;       // per op; TMA-staged fused upsample+concat+depthwise
     // streaming host round trip (skps_engine_submit_host_u8): 2 slots, H2D on its own stream
@@ -111,7 +113,7 @@ static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int
                     break;
                 }
                 if (op.flags & FLAG_XF) {
-                    rc = xf_launch(e->xf[i], batch, e->num_sms, s);
+                    rc = e->fpw[i].valid ? fpw_launch(e->fpw[i], batch, e->num_sms, s) : xf_launch(e->xf[i], batch, e->num_sms, s);
                     break;
                 }
                 if (op.flags & FLAG_TC) {
@@ -153,7 +155,9 @@ static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int
                 rc = launch_dwconv(a, s);
                 break;
             }
-            case OP_DWPW: rc = xf_launch(e->xf[i], batch, e->num_sms, s); break;
+            case OP_DWPW:
+                rc = e->fpw[i].valid ? fpw_launch(e->fpw[i], batch, e->num_sms, s) : xf_launch(e->xf[i], batch, e->num_sms, s);
+                break;
             case OP_STEM_BLOCK: {
                 // w = StemBlockW as packed by lowering (dense weights -> kernel-parameter bank); i[0] -> [9][E]+[E] depthwise table
                 StemBlockW W;
@@ -342,8 +346,10 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
         }
         if (op.dh != op.dw || op.ph != op.pw || tc_prepare(e->tc[i], s)) return fail_op(i, "tc");
     }
-    // fused producer -> pointwise conv layers (conv_xf.cu): depthwise / up-sample+concat+depthwise / squeeze-excite scale
+    // fused producer -> pointwise conv layers: depthwise / up-sample+concat+depthwise / squeeze-excite scale, on conv_fpw.cu
+    // where it takes the layer (whole 16 x 8 tiles, unit-stride aligned output, instantiated width), else on conv_xf.cu
     e->xf.resize(n_ops);
+    e->fpw.resize(n_ops);
     for (int i = 0; i < n_ops; ++i) {
         const OpDesc& op = e->ops[i];
         const bool dwpw = op.type == OP_DWPW, scale = op.type == OP_CONV && (op.flags & FLAG_XF);
@@ -367,6 +373,10 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
         s.w_hi = e->d_weights + op.w_off; s.w_lo = e->d_weights + op.i[2];
         s.bias = op.b_off >= 0 ? e->d_weights + op.b_off : nullptr;
         s.res_first = (op.flags & FLAG_RES_FIRST) ? 1 : 0;
+        if (fpw_supported(s)) {
+            if (fpw_prepare(e->fpw[i], s)) return fail_op(i, "fpw");
+            continue;
+        }
         if (xf_prepare(e->xf[i], s)) return fail_op(i, "xf");
     }
     // depthwise layers: TMA descriptors over the input views
@@ -494,7 +504,11 @@ extern "C" SKPS_API int skps_engine_op_kernel(const skps_engine* e, int op_index
     switch (op.type) {
         case OP_CONV:
             if (op.flags & FLAG_MMA) return SKPS_KERNEL_MMA;
-            if (op.flags & FLAG_XF) return SKPS_KERNEL_XF;
+            if (op.flags & FLAG_XF) {
+                if (!e->fpw[i].valid) return SKPS_KERNEL_XF;
+                inf[0] = 128; inf[1] = e->fpw[i].n; inf[2] = e->fpw[i].k.nsplit; inf[3] = e->fpw[i].mode;
+                return SKPS_KERNEL_FPW;
+            }
             if (op.flags & FLAG_TC) {
                 if (e->hm[i].valid) return SKPS_KERNEL_HM;
                 if (e->tct[i].valid) {
@@ -516,7 +530,10 @@ extern "C" SKPS_API int skps_engine_op_kernel(const skps_engine* e, int op_index
                 return SKPS_KERNEL_DW_TMA;
             }
             return SKPS_KERNEL_DW;
-        case OP_DWPW: return SKPS_KERNEL_XF;
+        case OP_DWPW:
+            if (!e->fpw[i].valid) return SKPS_KERNEL_XF;
+            inf[0] = 128; inf[1] = e->fpw[i].n; inf[2] = e->fpw[i].k.nsplit; inf[3] = e->fpw[i].mode;
+            return SKPS_KERNEL_FPW;
         case OP_UPCAT_DW: return e->upt[i].valid ? SKPS_KERNEL_UPCAT_TMA : SKPS_KERNEL_UPCAT;
         case OP_STEM_BLOCK: return SKPS_KERNEL_STEM_BLOCK;
         default: return SKPS_KERNEL_MISC;

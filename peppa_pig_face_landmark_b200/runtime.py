@@ -57,6 +57,9 @@ SIGNATURES = {
                                      C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, C.c_int, c_vp]),
     "skps_debug_conv_xf": (C.c_int, [C.c_int, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, C.c_int, c_vp, c_vp,
                                      C.c_int, c_vp, c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_float, c_vp, C.c_int, C.c_int, c_vp, c_vp]),
+    "skps_debug_conv_fpw": (C.c_int, [C.c_int, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, C.c_int, c_vp, c_vp,
+                                      C.c_int, c_vp, c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_float, c_vp, C.c_int, C.c_int, c_vp,
+                                      c_vp, C.c_int]),
     "skps_debug_conv_hm": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, C.c_int, C.c_int, C.c_float,
                                     c_vp, c_vp]),
     "skps_debug_se_fc": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_vp]),

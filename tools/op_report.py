@@ -24,9 +24,10 @@ from peppa_pig_face_landmark_b200 import plan as P  # noqa: E402
 from oracle.plan_interp import PlanInterp, rd, split16_round, _act  # noqa: E402
 
 KERNELS = {0: "misc", 1: "tc", 2: "tct", 3: "hm", 4: "mma", 5: "xf", 6: "simt", 7: "dw_tma", 8: "dw", 9: "upcat_tma",
-           10: "upcat", 11: "stem_block", 12: "pw"}
-K_MISC, K_TC, K_TCT, K_HM, K_MMA, K_XF, K_SIMT, K_DW_TMA, K_DW, K_UPCAT_TMA, K_UPCAT, K_STEM, K_PW = range(13)
-TENSOR_CORE = (K_TC, K_TCT, K_HM, K_MMA, K_XF, K_PW)
+           10: "upcat", 11: "stem_block", 12: "pw", 13: "fpw"}
+K_MISC, K_TC, K_TCT, K_HM, K_MMA, K_XF, K_SIMT, K_DW_TMA, K_DW, K_UPCAT_TMA, K_UPCAT, K_STEM, K_PW, K_FPW = range(14)
+# conv_fpw runs conv_xf's layers with conv_xf's operands and epilogue: the same tensor-core bound applies
+TENSOR_CORE = (K_TC, K_TCT, K_HM, K_MMA, K_XF, K_PW, K_FPW)
 PW_BM = 128                    # pixels per conv_pw tile: the tiles run over the flat (n, y, x) index of the batch
 
 U = 2.0 ** -24                 # unit roundoff of float32 (round to nearest)
@@ -120,6 +121,8 @@ def kernel_class(op, kernel):
         return "det_decode"
     if t == P.OP_HM_DECODE or (t == P.OP_CONV and op.flags & P.FLAG_HM_PART):
         return "hm"
+    if kernel == K_FPW:
+        return KERNELS[K_XF]            # conv_xf's layers, operands and epilogue: reported in conv_xf's class
     if kernel in TENSOR_CORE:
         return KERNELS[kernel]
     return KERNELS[kernel] if kernel != K_MISC else "fp32:" + P.OP_NAMES[t][3:].lower()
@@ -441,7 +444,10 @@ def _stored(op):
 
 def edge_tile(kernel, info, H, W, y, x, n=None, batch=None):
     """Whether output pixel (y, x) of an H x W map lies in a tile that hangs over the map's border; for conv_pw, whether
-    pixel (n, y, x) lies in the last, partial tile of a batch of `batch` maps."""
+    pixel (n, y, x) lies in the last, partial tile of a batch of `batch` maps.  conv_fpw only takes maps made of whole 16 x 8
+    tiles, so none of its pixels is in an edge tile."""
+    if kernel == K_FPW:
+        return False
     if kernel == K_PW:
         if n is None or batch is None:
             return None
