@@ -143,7 +143,8 @@ SKPS_API int skps_debug_conv_hm(const float* x, int N, int H, int W, int Cin, co
 /* Debug/unit-test entry of the fused producer -> 1x1 conv kernels (csrc/conv_xf.cu): mode 0 = squeeze-excite scale
  * (x * gate[n,c]) ahead of the conv, mode 1 = depthwise 3x3 [over concat(bilinear_x2(low), x)] ahead of the conv.
  * Replaces, for one layer, what onnxruntime runs for the reference's ONNX nodes Mul->Conv / Resize->Concat->Conv(dw)->Conv
- * (Skps/core/api/onnx_model_base.py:23).  Host float32 NHWC in/out; w_hi/w_lo as packed by plan.pack_tc_weights. */
+ * (Skps/core/api/onnx_model_base.py:23).  Host float32 NHWC in/out; w_hi/w_lo as packed by plan.pack_tc_weights.  `out` is
+ * read as well as written, so elements the kernel leaves unwritten come back as they went in. */
 SKPS_API int skps_debug_conv_xf(int mode, const float* x, int N, int H, int W, int Cx, int x_split, const float* low, int Cl,
                                 const float* gate, const float* dww, int dw_act, const void* w_hi, const void* w_lo,
                                 const float* bias, int Cout, int act, int n_tile, float out_scale, const float* residual,

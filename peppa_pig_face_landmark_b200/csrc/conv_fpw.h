@@ -1,31 +1,20 @@
 // Fused "producer -> pointwise conv" layers on a wgmma kernel whose accumulators stay in registers (conv_fpw.cu): the
-// student's depthwise -> 1x1 and squeeze-excite -> 1x1 layers.  Same layers and setup as conv_xf.cu (XfSetup); the engine
+// student's depthwise -> 1x1 and squeeze-excite -> 1x1 layers.  The A producer is conv_xf's (xf_producer.h); the engine
 // routes a layer here when fpw_supported() holds and leaves the rest (ragged maps, channel-shuffled outputs) on conv_xf.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "conv_xf.h"
+#include "xf_producer.h"
 
 namespace skps {
 
 struct FpwK {
-    int H, W, tiles_x, tiles_per_img;               // output map, 16 x 8 pixel tiles (no edge tiles: H % 8 == W % 16 == 0)
+    XfProducer a;                                   // the A producer (no edge tiles: H % 8 == W % 16 == 0)
     int units;                                      // work units of the launch: batch * tiles_per_img * nsplit
     int nsplit;                                     // work units per tile: ceil(N tile / unit width)
-    int cchunks, Cin;                               // K chunks of 64 channels
-    int rs, as, bs, out_bufs;                       // ring depths: raw tiles, A tiles, B tiles, epilogue staging buffers
-    int dw_act;                                     // activation between the depthwise stage and the pointwise conv
-    int Hl, Wl;                                     // low-res map of the up-sampled channels (XS_UP_F32)
-    int halves;                                     // transform mapping: 1 = two halves x 2-row patches (layers with up-sampled channels)
-    int wcx;                                        // column classes per staged weight block: 3, or 4 when the map is one tile wide
-    uint8_t sub_mode[2 * XF_MAX_CHUNKS];            // per 32-channel sub-chunk
-    int16_t sub_c[2 * XF_MAX_CHUNKS];               // channel coordinate of the sub-chunk in its source tensor
-    uint8_t chunk_subs[XF_MAX_CHUNKS];              // sub-chunks that hold real channels (1 or 2)
-    uint8_t chunk_ksteps[XF_MAX_CHUNKS];            // 16-channel MMA steps that hold real channels (1..4)
-    const float* dww;                               // [9][Kpad] depthwise weights then [Kpad] bias, zero padded
-    const float* gate; int gate_ld, gate_coff;      // XF_SCALE: squeeze-excite gate (N,1,1,C) float32
+    int bs, out_bufs;                               // ring depths: B tiles, epilogue staging buffers
     // epilogue: act(fmaf(acc, out_scale, bias) [+ res]) as in conv_xf
     int Cout;
     float out_scale;

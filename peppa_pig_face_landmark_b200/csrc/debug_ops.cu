@@ -1,9 +1,14 @@
-// Unit-test entry points for the small fused kernels that otherwise only run inside a whole network:
-// the squeeze-excite gate (se_fc_kernel) and the heat-map decode (hm_decode_kernel).  Host float32 in/out.
+// Unit-test entry points for the fused kernels that otherwise only run inside a whole network: the squeeze-excite gate
+// (se_fc_kernel), the heat-map decode (hm_decode_kernel) and the fused producer -> 1x1 conv layers (conv_xf.cu,
+// conv_fpw.cu).  Host float32 in/out.
+#include <cuda_fp16.h>
+#include <stdlib.h>
 #include <string.h>
 
 #include "../../include/skps_b200.h"
 #include "common.h"
+#include "conv_fpw.h"
+#include "conv_xf.h"
 
 using namespace skps;
 
@@ -17,12 +22,83 @@ struct DBuf {
         return 0;
     }
 };
-TView mk(void* base, int C, int H, int W, int ld = 0) {
+TView mk(void* base, int C, int H, int W, int ld = 0, int fmt = DT_F32, long long plane = 0) {
     TView t;
     memset(&t, 0, sizeof(t));
     t.base = base; t.ld = ld ? ld : C; t.c_off = 0; t.c_stride = 1; t.C = C; t.H = H; t.W = W;
-    t.sample = (long long)t.ld * H * W; t.fmt = DT_F32; t.plane = 0;
+    t.sample = (long long)t.ld * H * W; t.fmt = fmt; t.plane = plane;
     return t;
+}
+__global__ void f32_to_split(const float* __restrict__ src, __half* __restrict__ hi, __half* __restrict__ lo, long long n) {
+    long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float v = src[i];
+    const __half h = __float2half_rn(v);
+    hi[i] = h;
+    lo[i] = __float2half_rn(v - __half2float(h));
+}
+
+// One fused layer on host data through conv_fpw (fpw) or conv_xf, on images [0, batch) of buffers sized for N.  `out` comes
+// in as well as out (through the split-fp16 planes when out_split != 0), so that what the kernel leaves unwritten comes
+// back as it went in.
+int debug_conv_fused(bool fpw, int mode, const float* x, int N, int H, int W, int Cx, int x_split, const float* low, int Cl,
+                     const float* gate, const float* dww, int dw_act, const void* w_hi, const void* w_lo, const float* bias,
+                     int Cout, int act, int n_tile, float out_scale, const float* residual, int res_first, int out_split,
+                     float* out, const float* weff, int batch) {
+    SKPS_CHECK(x && w_hi && w_lo && out && N > 0 && batch > 0 && batch <= N, "debug_conv_fused: bad argument");
+    SKPS_CHECK(!low || (weff && Cl % 32 == 0), "debug_conv_fused: class weights");
+    const int K = Cx + (low ? Cl : 0), Kpad = (K + 63) / 64 * 64;
+    const long long nx = (long long)N * H * W * Cx, nl = low ? (long long)N * (H / 2) * (W / 2) * Cl : 0;
+    const long long nout = (long long)N * H * W * Cout;
+    const bool xs = x_split || mode == XF_SCALE;
+    DBuf dx, dxs, dl, dg, dw, dwh, dwl, db, dr, dout, dwe;
+    SKPS_CHECK(!dx.put(x, nx * 4) && !dxs.put(nullptr, nx * 4) && !dl.put(low, nl * 4) && !dg.put(gate, (size_t)N * Cx * 4) &&
+               !dw.put(dww, (size_t)10 * Kpad * 4) && !dwh.put(w_hi, (size_t)n_tile * Kpad * 2) &&
+               !dwl.put(w_lo, (size_t)n_tile * Kpad * 2) && !db.put(bias, (size_t)Cout * 4) && !dr.put(residual, nout * 4) &&
+               !dout.put(nullptr, nout * 4 * (out_split ? 2 : 1)) && !dwe.put(weff, low ? (size_t)Cl * 144 * 4 : 0),
+               "debug_conv_fused: cudaMalloc/copy failed");
+    SKPS_CUDA(cudaMemcpy(dout.p, out, nout * 4, cudaMemcpyHostToDevice));
+    if (xs) {
+        f32_to_split<<<(unsigned)((nx + 255) / 256), 256>>>((const float*)dx.p, (__half*)dxs.p, (__half*)dxs.p + nx, nx);
+        SKPS_CUDA(cudaGetLastError());
+    }
+    // the output's initial contents: float32, or split into the hi/lo planes
+    void* obase = dout.p;
+    if (out_split) {
+        obase = (float*)dout.p + nout;
+        f32_to_split<<<(unsigned)((nout + 255) / 256), 256>>>((const float*)dout.p, (__half*)obase, (__half*)obase + nout, nout);
+        SKPS_CUDA(cudaGetLastError());
+    }
+    XfSetup s;
+    memset(&s, 0, sizeof(s));
+    s.mode = mode; s.max_batch = N;
+    s.x = xs ? mk(dxs.p, Cx, H, W, 0, DT_SPLIT16, nx) : mk(dx.p, Cx, H, W);
+    if (low) s.low = mk(dl.p, Cl, H / 2, W / 2);
+    if (gate) s.gate = mk(dg.p, Cx, 1, 1);
+    s.dww = (const float*)dw.p; s.dw_act = dw_act; s.weff = low ? (const float*)dwe.p : nullptr;
+    s.Cout = Cout; s.act = act; s.n_tile = n_tile; s.n_tiles = 1; s.out_scale = out_scale;
+    s.w_hi = dwh.p; s.w_lo = dwl.p; s.bias = bias ? (const float*)db.p : nullptr;
+    s.out = mk(obase, Cout, H, W, 0, out_split ? DT_SPLIT16 : DT_F32, nout);
+    if (residual) s.res = mk(dr.p, Cout, H, W);
+    s.res_first = res_first;
+    if (fpw) {
+        FpwLayer L;
+        if (fpw_prepare(L, s) || fpw_launch(L, batch, sm_count(), 0)) return 1;
+    } else {
+        XfLayer L;
+        if (xf_prepare(L, s) || xf_launch(L, batch, sm_count(), 0)) return 1;
+    }
+    SKPS_CUDA(cudaDeviceSynchronize());
+    if (out_split) {
+        __half* tmp = (__half*)malloc(nout * 4);
+        SKPS_CHECK(tmp, "debug_conv_fused: host allocation failed");
+        SKPS_CUDA(cudaMemcpy(tmp, obase, nout * 4, cudaMemcpyDeviceToHost));
+        for (long long i = 0; i < nout; ++i) out[i] = __half2float(tmp[i]) + __half2float(tmp[nout + i]);
+        free(tmp);
+    } else {
+        SKPS_CUDA(cudaMemcpy(out, dout.p, nout * 4, cudaMemcpyDeviceToHost));
+    }
+    return 0;
 }
 }  // namespace
 
@@ -69,4 +145,33 @@ extern "C" SKPS_API int skps_debug_hm_decode(const float* hm, int N, int H, int 
     SKPS_CUDA(cudaMemcpy(xy, dx.p, (size_t)N * 2 * npts * 4, cudaMemcpyDeviceToHost));
     SKPS_CUDA(cudaMemcpy(score, ds.p, (size_t)N * npts * 4, cudaMemcpyDeviceToHost));
     return 0;
+}
+
+// One fused layer through conv_xf on host data (tests/test_conv_xf_gpu.py).
+//   mode 0 (XF_SCALE): out = act(conv1x1(x * gate[n,c]) ...)            x (N,H,W,Cx) float32, gate (N,Cx)
+//   mode 1 (XF_DW)   : out = act(conv1x1(dw_act(dw3x3(concat(up2(low), x)))))   low (N,H/2,W/2,Cl) or null
+//   x_split: the kernel reads x as fp16 hi/lo planes (else float32; XF_SCALE always splits)
+//   dww: [9][Kpad] depthwise weights then [Kpad] bias, Kpad = ceil((Cl+Cx)/64)*64 (XF_DW)
+//   w_hi/w_lo: (n_tile, Kpad) float16 as packed by plan.pack_tc_weights; residual (N,H,W,Cout) float32 or null
+//   weff: [Cl/32][4][4][9][32] class weights of the up-sampled channels (plan.pack_upcat_class_weights), null without low
+//   out: (N,H,W,Cout); elements the kernel leaves unwritten come back as they went in
+extern "C" SKPS_API int skps_debug_conv_xf(int mode, const float* x, int N, int H, int W, int Cx, int x_split,
+                                           const float* low, int Cl, const float* gate, const float* dww, int dw_act,
+                                           const void* w_hi, const void* w_lo, const float* bias, int Cout, int act,
+                                           int n_tile, float out_scale, const float* residual, int res_first,
+                                           int out_split, float* out, const float* weff) {
+    return debug_conv_fused(false, mode, x, N, H, W, Cx, x_split, low, Cl, gate, dww, dw_act, w_hi, w_lo, bias, Cout, act,
+                            n_tile, out_scale, residual, res_first, out_split, out, weff, N);
+}
+
+// One fused layer through conv_fpw on host data (tests/test_conv_fpw_gpu.py).  The arguments of skps_debug_conv_xf, then
+// `batch` <= N: the kernel runs images [0, batch) of buffers sized for N, so that images past the batch can be checked to
+// come back as they went in.  Fails for a layer conv_fpw does not take.
+extern "C" SKPS_API int skps_debug_conv_fpw(int mode, const float* x, int N, int H, int W, int Cx, int x_split,
+                                            const float* low, int Cl, const float* gate, const float* dww, int dw_act,
+                                            const void* w_hi, const void* w_lo, const float* bias, int Cout, int act,
+                                            int n_tile, float out_scale, const float* residual, int res_first,
+                                            int out_split, float* out, const float* weff, int batch) {
+    return debug_conv_fused(true, mode, x, N, H, W, Cx, x_split, low, Cl, gate, dww, dw_act, w_hi, w_lo, bias, Cout, act,
+                            n_tile, out_scale, residual, res_first, out_split, out, weff, batch);
 }

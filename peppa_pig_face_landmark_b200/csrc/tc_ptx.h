@@ -1,5 +1,5 @@
-// PTX wrappers shared by the tensor-core kernels (conv_tc.cu, conv_tct.cu, conv_pw.cu, conv_fpw.cu, conv_hm.cu, conv_xf.cu,
-// stem_block.cu):
+// PTX wrappers shared by the tensor-core kernels (conv_tc.cu, conv_tct.cu, conv_pw.cu, conv_hm.cu, stem_block.cu, and
+// conv_xf.cu and conv_fpw.cu with the A producer they share, xf_producer.h):
 // mbarrier, TMA, wgmma and its shared-memory matrix descriptors.  sm_90a.
 //
 // The accumulator of a 128-row tile lives in the registers of the warpgroup that issues the wgmma instructions: one

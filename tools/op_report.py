@@ -26,7 +26,7 @@ from oracle.plan_interp import PlanInterp, rd, split16_round, _act  # noqa: E402
 KERNELS = {0: "misc", 1: "tc", 2: "tct", 3: "hm", 4: "mma", 5: "xf", 6: "simt", 7: "dw_tma", 8: "dw", 9: "upcat_tma",
            10: "upcat", 11: "stem_block", 12: "pw", 13: "fpw"}
 K_MISC, K_TC, K_TCT, K_HM, K_MMA, K_XF, K_SIMT, K_DW_TMA, K_DW, K_UPCAT_TMA, K_UPCAT, K_STEM, K_PW, K_FPW = range(14)
-# conv_fpw runs conv_xf's layers with conv_xf's operands and epilogue: the same tensor-core bound applies
+# conv_fpw runs conv_xf's layers on the same A producer (csrc/xf_producer.h) and epilogue: the same tensor-core bound applies
 TENSOR_CORE = (K_TC, K_TCT, K_HM, K_MMA, K_XF, K_PW, K_FPW)
 PW_BM = 128                    # pixels per conv_pw tile: the tiles run over the flat (n, y, x) index of the batch
 
