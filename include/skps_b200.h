@@ -94,6 +94,14 @@ SKPS_API int skps_engine_launches_for_batch(const skps_engine* e, int batch);
 /* Profiling: enqueue only op `op_index` of the plan on the buffers left by the last forward
  * (bench.py times the dominant kernel with CUDA events around this call). */
 SKPS_API int skps_engine_run_op(skps_engine* e, int op_index, int batch, void* stream);
+/* Test hook: size the grids of the persistent kernels (conv_tc, conv_tct, conv_hm, conv_pw, conv_xf, conv_fpw, the stem
+ * block; conv_mma: n x its CTAs per SM) for n SMs instead of the device's, so that every CTA walks more work units.  n = 0
+ * restores the device's count; n < 0 or above it fails.  Drops the engine's captured forwards.  Results must not change:
+ * what a unit computes depends only on its index. */
+SKPS_API int skps_engine_set_num_sms(skps_engine* e, int n);
+/* The launch of op `op_index` at `batch` under the current setting: out = {CTAs, work units} for a persistent kernel,
+ * {0, 0} for any other op. */
+SKPS_API int skps_engine_op_grid(const skps_engine* e, int op_index, int batch, int32_t out[2]);
 /* Which kernel op `op_index` runs and the geometry it picked (for tests that must know which branch they exercised).
  * Returns a SKPS_KERNEL_* id, or -1 on a bad index.  info[0..3] (zero where unused):
  *   TC: bw, bh (output pixels of a 128-pixel tile), ipt (images per tile), mt (pixel tiles per weight tile);

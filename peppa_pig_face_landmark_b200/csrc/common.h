@@ -16,6 +16,15 @@ inline int sm_count() {
     return n;
 }
 
+// Launch of a persistent kernel: `ctas` CTAs walk `units` work units as blockIdx.x, + gridDim.x, ...  Each persistent
+// launcher computes it in one helper (tc_grid, pw_grid, ...) that skps_engine_op_grid reports as well.
+struct Grid {
+    int ctas, units;
+};
+inline Grid persistent_grid(long long units, long long max_ctas) {
+    return Grid{(int)(units < max_ctas ? units : max_ctas), (int)units};
+}
+
 // cuTensorMapEncodeTiled, looked up through the runtime so that the library needs no link against the driver library;
 // null when the driver does not provide it
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,

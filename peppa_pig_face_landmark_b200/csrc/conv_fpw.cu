@@ -351,11 +351,17 @@ static int fpw_launch_n(const FpwLayer& L, const FpwK& k, int grid, cudaStream_t
     return 1;
 }
 
-int fpw_launch(const FpwLayer& L, int batch, int num_sms, cudaStream_t stream) {
-    SKPS_CHECK(L.valid, "conv_fpw: layer not prepared");
+Grid fpw_grid(const FpwLayer& L, int batch, int num_sms, FpwK* kp) {
     FpwK k = L.k;
     k.units = batch * k.a.tiles_per_img * k.nsplit;
-    const int grid = k.units < num_sms ? k.units : num_sms;
+    if (kp) *kp = k;
+    return persistent_grid(k.units, num_sms);
+}
+
+int fpw_launch(const FpwLayer& L, int batch, int num_sms, cudaStream_t stream) {
+    SKPS_CHECK(L.valid, "conv_fpw: layer not prepared");
+    FpwK k;
+    const int grid = fpw_grid(L, batch, num_sms, &k).ctas;
     if (L.mode == XF_DW) {
         switch (L.n) {
             case 32: return fpw_launch_n<XF_DW, 32>(L, k, grid, stream);

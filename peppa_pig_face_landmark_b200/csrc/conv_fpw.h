@@ -32,6 +32,7 @@ struct FpwLayer {
 
 bool fpw_supported(const XfSetup& s);
 int fpw_prepare(FpwLayer& L, const XfSetup& s);
+Grid fpw_grid(const FpwLayer& L, int batch, int num_sms, FpwK* k = nullptr);   // as tc_grid
 int fpw_launch(const FpwLayer& L, int batch, int num_sms, cudaStream_t stream);
 
 }  // namespace skps

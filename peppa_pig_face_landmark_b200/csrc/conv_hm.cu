@@ -235,15 +235,21 @@ int hm_prepare(HmLayer& L, const TcSetup& s) {
     return 0;
 }
 
+Grid hm_grid(const HmLayer& L, int batch, int num_sms, HmK* kp) {
+    HmK k = L.k;
+    k.m_tiles = batch * k.tiles_per_img;
+    if (kp) *kp = k;
+    return persistent_grid(k.m_tiles, num_sms);
+}
+
 int hm_launch(const HmLayer& L, int batch, int num_sms, cudaStream_t stream) {
     static int attr_bytes = 0;
     if (L.smem_bytes > attr_bytes) {
         SKPS_CUDA(cudaFuncSetAttribute(conv_hm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
         attr_bytes = L.smem_bytes;
     }
-    HmK k = L.k;
-    k.m_tiles = batch * k.tiles_per_img;
-    const int grid = k.m_tiles < num_sms ? k.m_tiles : num_sms;
+    HmK k;
+    const int grid = hm_grid(L, batch, num_sms, &k).ctas;
     conv_hm_kernel<<<grid, HM_THREADS, L.smem_bytes, stream>>>(L.x_hi, L.x_lo, L.w_hi, L.w_lo, k);
     SKPS_CUDA(cudaGetLastError());
     return 0;

@@ -27,6 +27,7 @@ constexpr int HM_TILE_PIXELS = 256;
 
 bool hm_shape_ok(int H, int W, int Cin, int Cout, int in_ld, int in_coff);
 int hm_prepare(HmLayer& L, const TcSetup& s);                 // s.hm_val / hm_idx / hm_ld set, 1x1, linear
+Grid hm_grid(const HmLayer& L, int batch, int num_sms, HmK* k = nullptr);   // as tc_grid
 int hm_launch(const HmLayer& L, int batch, int num_sms, cudaStream_t stream);
 
 }  // namespace skps

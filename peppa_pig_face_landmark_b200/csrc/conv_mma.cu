@@ -235,6 +235,22 @@ conv_mma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant
 }
 
 // ------------------------------------------------------------------------------------------ host side
+// Shared-memory limit of the instantiation and its resident CTAs per SM
+template <int CIN, int COUT>
+static int mma_setup_t(int* ctas_per_sm) {
+    static bool attr_set = false;
+    static int ctas = 1;
+    constexpr int smem = MmaCfg<CIN, COUT>::SMEM;
+    if (!attr_set) {
+        SKPS_CUDA(cudaFuncSetAttribute(conv_mma_kernel<CIN, COUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        SKPS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, conv_mma_kernel<CIN, COUT>, MMA_THREADS, smem));
+        if (ctas < 1) ctas = 1;
+        attr_set = true;
+    }
+    *ctas_per_sm = ctas;
+    return 0;
+}
+
 bool conv_mma_supported(int cin, int cout, int kh, int kw, int stride, int dil, int pad) {
     return kh == 3 && kw == 3 && stride == 1 && dil == 1 && pad == 1 && cin == cout && (cin == 24 || cin == 40);
 }
@@ -269,36 +285,28 @@ int conv_mma_prepare(ConvMmaLayer& L, const TView& in, const TView& out, const T
     k.res = res.base; k.res_fmt = res.fmt; k.res_plane = res.plane; k.res_ld = res.ld; k.res_coff = res.c_off;
     k.res_first = res.base ? res_first : 0;
     L.cin = in.C; L.cout = out.C;
+    if ((in.C == 24 ? mma_setup_t<24, 24>(&L.ctas_per_sm) : mma_setup_t<40, 40>(&L.ctas_per_sm))) return 1;
     L.valid = true;
     return 0;
 }
 
 template <int CIN, int COUT>
-static int mma_launch_t(const ConvMmaLayer& L, const ConvMmaK& k, cudaStream_t stream) {
-    static bool attr_set = false;
-    static int ctas_per_sm = 1, sms = 132;
-    constexpr int smem = MmaCfg<CIN, COUT>::SMEM;
-    if (!attr_set) {
-        SKPS_CUDA(cudaFuncSetAttribute(conv_mma_kernel<CIN, COUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        SKPS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, conv_mma_kernel<CIN, COUT>, MMA_THREADS, smem));
-        if (ctas_per_sm < 1) ctas_per_sm = 1;
-        attr_set = true;
-    }
-    const long long total = (long long)k.tiles_img * k.batch;
-    const int grid = (int)(total < (long long)sms * ctas_per_sm ? total : (long long)sms * ctas_per_sm);
-    conv_mma_kernel<CIN, COUT><<<grid, MMA_THREADS, smem, stream>>>(L.a_hi, L.a_lo, k);
+static int mma_launch_t(const ConvMmaLayer& L, const ConvMmaK& k, int grid, cudaStream_t stream) {
+    conv_mma_kernel<CIN, COUT><<<grid, MMA_THREADS, MmaCfg<CIN, COUT>::SMEM, stream>>>(L.a_hi, L.a_lo, k);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }
 
-int conv_mma_launch(const ConvMmaLayer& L, int batch, cudaStream_t stream) {
+Grid conv_mma_grid(const ConvMmaLayer& L, int batch, int num_sms) {
+    return persistent_grid((long long)L.k.tiles_img * batch, (long long)num_sms * L.ctas_per_sm);
+}
+
+int conv_mma_launch(const ConvMmaLayer& L, int batch, int num_sms, cudaStream_t stream) {
     ConvMmaK k = L.k;
     k.batch = batch;
-    if (L.cin == 24) return mma_launch_t<24, 24>(L, k, stream);
-    if (L.cin == 40) return mma_launch_t<40, 40>(L, k, stream);
+    const int grid = conv_mma_grid(L, batch, num_sms).ctas;
+    if (L.cin == 24) return mma_launch_t<24, 24>(L, k, grid, stream);
+    if (L.cin == 40) return mma_launch_t<40, 40>(L, k, grid, stream);
     set_error("conv_mma: %d channels not instantiated", L.cin);
     return 1;
 }
@@ -350,7 +358,7 @@ extern "C" SKPS_API int skps_debug_conv_mma(const float* x, int N, int H, int W,
     if (d_res) { r = in; r.base = d_res; r.fmt = DT_F32; r.plane = 0; }
     ConvMmaLayer L;
     if (conv_mma_prepare(L, in, o, r, res_first, d_w, d_bias, out_scale, act, N)) return 1;
-    if (conv_mma_launch(L, N, 0)) return 1;
+    if (conv_mma_launch(L, N, sm_count(), 0)) return 1;
     SKPS_CUDA(cudaDeviceSynchronize());
     if (out_split) {
         __half* tmp = (__half*)malloc(n * 4);

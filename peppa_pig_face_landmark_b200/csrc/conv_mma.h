@@ -22,12 +22,14 @@ struct ConvMmaLayer {
     CUtensorMap a_hi, a_lo;      // (Cin, W, H, N) fp16 planes of the input view, box (Cin, 18, 10, 1)
     ConvMmaK k;
     int cin, cout;
+    int ctas_per_sm = 1;         // resident CTAs of the kernel per SM (occupancy): the grid is num_sms x ctas_per_sm at most
     bool valid = false;
 };
 
 bool conv_mma_supported(int cin, int cout, int kh, int kw, int stride, int dil, int pad);
 int conv_mma_prepare(ConvMmaLayer& L, const TView& in, const TView& out, const TView& res, int res_first, const void* w_packed,
                      const float* bias, float out_scale, int act, int max_batch);
-int conv_mma_launch(const ConvMmaLayer& L, int batch, cudaStream_t stream);
+Grid conv_mma_grid(const ConvMmaLayer& L, int batch, int num_sms);   // as tc_grid
+int conv_mma_launch(const ConvMmaLayer& L, int batch, int num_sms, cudaStream_t stream);
 
 }  // namespace skps

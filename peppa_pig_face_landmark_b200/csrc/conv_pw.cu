@@ -332,13 +332,20 @@ static int pw_launch_nc(const PwLayer& L, const PwK& k, const CUtensorMap& o_hi,
     return 1;
 }
 
+Grid pw_grid(const PwLayer& L, int batch, int num_sms, PwK* kp) {
+    PwK k = L.k;
+    k.m_tiles = (int)((L.hw * batch + PW_BM - 1) / PW_BM);
+    if (kp) *kp = k;
+    return persistent_grid((long long)k.m_tiles * k.n_chunks, num_sms);
+}
+
 int pw_launch(const PwLayer& L, int batch, int num_sms, cudaStream_t stream) {
     SKPS_CHECK(L.valid, "conv_pw: layer not prepared");
     EncodeTiledFn enc = tensor_map_encoder();
     SKPS_CHECK(enc, "cuTensorMapEncodeTiled entry point not available");
     const long long rows = L.hw * batch;
-    PwK k = L.k;
-    k.m_tiles = (int)((rows + PW_BM - 1) / PW_BM);
+    PwK k;
+    const int grid = pw_grid(L, batch, num_sms, &k).ctas;
     // output: {Cout, batch*H*W} per plane, one box = 32 channels x 128 pixels in the staging layout the epilogue writes
     const bool split = L.out_fmt == DT_SPLIT16;
     const int oes = split ? 2 : 4;
@@ -356,8 +363,6 @@ int pw_launch(const PwLayer& L, int batch, int num_sms, cudaStream_t stream) {
         SKPS_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(pw out) failed: %d", (int)r);
     }
     if (!split) o[1] = o[0];
-    const int units = k.m_tiles * k.n_chunks;
-    const int grid = units < num_sms ? units : num_sms;
     return split ? pw_launch_nc<true>(L, k, o[0], o[1], grid, stream) : pw_launch_nc<false>(L, k, o[0], o[1], grid, stream);
 }
 

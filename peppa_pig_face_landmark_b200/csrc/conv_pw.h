@@ -32,6 +32,7 @@ struct PwLayer {                 // prepared once per conv op at engine creation
 
 bool pw_applicable(const TcSetup& s);
 int pw_prepare(PwLayer& L, const TcSetup& s);
+Grid pw_grid(const PwLayer& L, int batch, int num_sms, PwK* k = nullptr);   // as tc_grid
 int pw_launch(const PwLayer& L, int batch, int num_sms, cudaStream_t stream);
 
 }  // namespace skps

@@ -574,12 +574,17 @@ static int tc_launch_t(const TcLayer& L, const TcK& k, int grid, cudaStream_t st
     return 0;
 }
 
-int tc_launch(const TcLayer& L, int batch, int num_sms, cudaStream_t stream) {
+Grid tc_grid(const TcLayer& L, int batch, int num_sms, TcK* kp) {
     TcK k = L.k;
     k.m_tiles = k.ipt > 1 ? (batch + k.ipt - 1) / k.ipt : batch * k.tiles_per_img;
     k.img_end = batch;
-    int total = ((k.m_tiles + k.mt - 1) / k.mt) * k.n_tiles;
-    int grid = total < num_sms ? total : num_sms;
+    if (kp) *kp = k;
+    return persistent_grid((long long)((k.m_tiles + k.mt - 1) / k.mt) * k.n_tiles, num_sms);
+}
+
+int tc_launch(const TcLayer& L, int batch, int num_sms, cudaStream_t stream) {
+    TcK k;
+    const int grid = tc_grid(L, batch, num_sms, &k).ctas;
     const bool sp = k.out_fmt == DT_SPLIT16;
     switch (k.act) {
         case ACT_NONE: return sp ? tc_launch_t<ACT_NONE, true>(L, k, grid, stream) : tc_launch_t<ACT_NONE, false>(L, k, grid, stream);

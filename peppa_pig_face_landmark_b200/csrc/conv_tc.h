@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "common.h"
+
 namespace skps {
 
 struct TcK {                     // kernel parameters
@@ -48,6 +50,8 @@ struct TcSetup {
 
 bool tc_shape_ok(int Ho, int Wo, int Cin, int in_ld, int in_coff);
 int tc_prepare(TcLayer& L, const TcSetup& s);
+// The launch at `batch` on num_sms SMs; fills the batch's kernel parameters into *k when k is not null
+Grid tc_grid(const TcLayer& L, int batch, int num_sms, TcK* k = nullptr);
 int tc_launch(const TcLayer& L, int batch, int num_sms, cudaStream_t stream);
 
 }  // namespace skps

@@ -264,10 +264,16 @@ static int tct_launch_t(const TctLayer& L, const TctK& k, int grid, cudaStream_t
     return 0;
 }
 
-int tct_launch(const TctLayer& L, int batch, int num_sms, cudaStream_t stream) {
+Grid tct_grid(const TctLayer& L, int batch, int num_sms, TctK* kp) {
     TctK k = L.k;
     k.m_tiles = batch * k.tiles_per_img;
-    const int grid = k.m_tiles < num_sms ? k.m_tiles : num_sms;
+    if (kp) *kp = k;
+    return persistent_grid(k.m_tiles, num_sms);
+}
+
+int tct_launch(const TctLayer& L, int batch, int num_sms, cudaStream_t stream) {
+    TctK k;
+    const int grid = tct_grid(L, batch, num_sms, &k).ctas;
     switch (k.act) {
         case ACT_NONE: return tct_launch_t<ACT_NONE>(L, k, grid, stream);
         case ACT_RELU: return tct_launch_t<ACT_RELU>(L, k, grid, stream);

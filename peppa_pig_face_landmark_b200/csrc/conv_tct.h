@@ -24,6 +24,7 @@ struct TctLayer {
 
 bool tct_applicable(const TcSetup& s);          // s.H, s.W: the (stride-1) map; split-fp16 contiguous output, no residual
 int tct_prepare(TctLayer& L, const TcSetup& s);
+Grid tct_grid(const TctLayer& L, int batch, int num_sms, TctK* k = nullptr);   // as tc_grid
 int tct_launch(const TctLayer& L, int batch, int num_sms, cudaStream_t stream);
 
 }  // namespace skps

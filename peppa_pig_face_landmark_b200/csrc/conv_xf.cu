@@ -473,10 +473,16 @@ static int xf_launch_m(const XfLayer& L, const XfK& k, int grid, cudaStream_t st
     return 1;
 }
 
-int xf_launch(const XfLayer& L, int batch, int num_sms, cudaStream_t stream) {
+Grid xf_grid(const XfLayer& L, int batch, int num_sms, XfK* kp) {
     XfK k = L.k;
     k.m_tiles = batch * k.a.tiles_per_img;
-    const int grid = k.m_tiles < num_sms ? k.m_tiles : num_sms;
+    if (kp) *kp = k;
+    return persistent_grid(k.m_tiles, num_sms);
+}
+
+int xf_launch(const XfLayer& L, int batch, int num_sms, cudaStream_t stream) {
+    XfK k;
+    const int grid = xf_grid(L, batch, num_sms, &k).ctas;
     return L.mode == XF_SCALE ? xf_launch_m<XF_SCALE>(L, k, grid, stream) : xf_launch_m<XF_DW>(L, k, grid, stream);
 }
 

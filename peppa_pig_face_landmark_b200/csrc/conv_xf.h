@@ -30,6 +30,7 @@ struct XfLayer {
 };
 
 int xf_prepare(XfLayer& L, const XfSetup& s);
+Grid xf_grid(const XfLayer& L, int batch, int num_sms, XfK* k = nullptr);   // as tc_grid
 int xf_launch(const XfLayer& L, int batch, int num_sms, cudaStream_t stream);
 
 }  // namespace skps

@@ -53,7 +53,8 @@ struct skps_engine {
     std::map<int, cudaGraphExec_t> graphs;   // batch -> captured forward
     int launches = 0;
     bool use_graph = true;
-    int num_sms = 132;
+    int device_sms = 132;                 // the device's SM count
+    int num_sms = 132;                    // SMs the persistent kernels' grids are sized for (skps_engine_set_num_sms)
     std::vector<TcLayer> tc;              // per op; valid where ops[i].flags & FLAG_TC
     std::vector<TctLayer> tct;            // per op; valid where the transposed kernel (conv_tct.cu) takes the layer
     std::vector<PwLayer> pw;              // per op; valid where the pointwise kernel (conv_pw.cu) takes the layer
@@ -96,6 +97,19 @@ static TView resolve(const skps_engine* e, const View& v) {
     return t;
 }
 
+// Kernel parameters of a stem block op for samples [0, batch).
+static StemBlockK stem_params(const skps_engine* e, const OpDesc& op, int batch) {
+    const TView in0 = resolve(e, op.in[0]), out0 = resolve(e, op.out[0]);
+    StemBlockK k;
+    k.in = e->f32_mode ? nullptr : (const uint8_t*)in0.base;
+    k.in_f32 = e->f32_mode ? (const float*)in0.base : nullptr;      // resolve() points at d_in_f32 in this mode
+    k.H = in0.H; k.W = in0.W; k.Hq = out0.H; k.Wq = out0.W;
+    k.img0 = 0; k.n_tiles = batch * (out0.H / 8) * (out0.W / 16);
+    k.dw1 = e->d_weights + op.i[0];
+    k.out = out0.base; k.out_fmt = out0.fmt; k.out_plane = out0.plane; k.out_ld = out0.ld; k.out_coff = out0.c_off;
+    return k;
+}
+
 // Enqueue ops [first,last) for samples [0, batch).
 static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int last = -1) {
     const size_t end = last < 0 ? e->ops.size() : (size_t)last;
@@ -109,7 +123,7 @@ static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int
         switch (op.type) {
             case OP_CONV: {
                 if (op.flags & FLAG_MMA) {
-                    rc = conv_mma_launch(e->mma[i], batch, s);
+                    rc = conv_mma_launch(e->mma[i], batch, e->num_sms, s);
                     break;
                 }
                 if (op.flags & FLAG_XF) {
@@ -162,13 +176,7 @@ static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int
                 // w = StemBlockW as packed by lowering (dense weights -> kernel-parameter bank); i[0] -> [9][E]+[E] depthwise table
                 StemBlockW W;
                 memcpy(&W, e->h_weights.data() + op.w_off, sizeof(W));
-                StemBlockK k;
-                k.in = e->f32_mode ? nullptr : (const uint8_t*)in0.base;
-                k.in_f32 = e->f32_mode ? (const float*)in0.base : nullptr;      // resolve() points at d_in_f32 in this mode
-                k.H = in0.H; k.W = in0.W; k.Hq = out0.H; k.Wq = out0.W;
-                k.img0 = 0; k.n_tiles = batch * (out0.H / 8) * (out0.W / 16);
-                k.dw1 = e->d_weights + op.i[0];
-                k.out = out0.base; k.out_fmt = out0.fmt; k.out_plane = out0.plane; k.out_ld = out0.ld; k.out_coff = out0.c_off;
+                const StemBlockK k = stem_params(e, op, batch);
                 if (in0.fmt != DT_U8 || !stem_block_supported(in0.H, in0.W, out0.C, out0)) {
                     set_error("stem block: unsupported shape");
                     rc = 1;
@@ -290,7 +298,8 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
         set_error("cudaMalloc staging");
         return fail("alloc");
     }
-    cudaDeviceGetAttribute(&e->num_sms, cudaDevAttrMultiProcessorCount, device);
+    cudaDeviceGetAttribute(&e->device_sms, cudaDevAttrMultiProcessorCount, device);
+    e->num_sms = e->device_sms;
     // tensor-core conv layers: TMA descriptors over the (fixed) activation buffers and weight matrices
     e->mma.resize(n_ops);
     for (int i = 0; i < n_ops; ++i) {
@@ -538,6 +547,42 @@ extern "C" SKPS_API int skps_engine_op_kernel(const skps_engine* e, int op_index
         case OP_STEM_BLOCK: return SKPS_KERNEL_STEM_BLOCK;
         default: return SKPS_KERNEL_MISC;
     }
+}
+
+extern "C" SKPS_API int skps_engine_set_num_sms(skps_engine* e, int n) {
+    SKPS_CHECK(e, "set_num_sms: null engine");
+    SKPS_CHECK(n >= 0 && n <= e->device_sms, "set_num_sms: %d outside 0..%d", n, e->device_sms);
+    SKPS_CUDA(cudaSetDevice(e->device));
+    // a captured forward keeps the grids it was captured with
+    for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);
+    e->graphs.clear();
+    e->num_sms = n ? n : e->device_sms;
+    return 0;
+}
+
+// The grid run_ops() launches for a persistent op, from the same helpers the launchers size it with.
+extern "C" SKPS_API int skps_engine_op_grid(const skps_engine* e, int op_index, int batch, int32_t out[2]) {
+    SKPS_CHECK(e && out && op_index >= 0 && op_index < (int)e->ops.size(), "op_grid: bad arguments");
+    SKPS_CHECK(batch > 0 && batch <= e->max_batch, "op_grid: batch %d outside 1..%d", batch, e->max_batch);
+    const size_t i = (size_t)op_index;
+    const OpDesc& op = e->ops[i];
+    const int sms = e->num_sms;
+    Grid g = {0, 0};
+    if (op.type == OP_CONV && (op.flags & FLAG_MMA)) {
+        g = conv_mma_grid(e->mma[i], batch, sms);
+    } else if (op.type == OP_DWPW || (op.type == OP_CONV && (op.flags & FLAG_XF))) {
+        g = e->fpw[i].valid ? fpw_grid(e->fpw[i], batch, sms) : xf_grid(e->xf[i], batch, sms);
+    } else if (op.type == OP_CONV && (op.flags & FLAG_TC)) {
+        g = e->hm[i].valid ? hm_grid(e->hm[i], batch, sms)
+            : e->tct[i].valid ? tct_grid(e->tct[i], batch, sms)
+            : e->pw[i].valid ? pw_grid(e->pw[i], batch, sms)
+            : tc_grid(e->tc[i], batch, sms);
+    } else if (op.type == OP_STEM_BLOCK) {
+        g = stem_block_grid(stem_params(e, op, batch), sms);
+    }
+    out[0] = g.ctas;
+    out[1] = g.units;
+    return 0;
 }
 
 // Enqueue the op sequence (through a cached CUDA graph when possible).

@@ -32,6 +32,7 @@ struct StemBlockK {
 };
 
 bool stem_block_supported(int H, int W, int E, const TView& out);
+Grid stem_block_grid(const StemBlockK& k, int num_sms);      // k.n_tiles set
 int stem_block_launch(const StemBlockK& k, const StemBlockW& w, int num_sms, cudaStream_t s);
 
 }  // namespace skps

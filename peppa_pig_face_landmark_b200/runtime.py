@@ -48,6 +48,8 @@ SIGNATURES = {
     "skps_engine_launches_for_batch": (C.c_int, [c_vp, C.c_int]),
     "skps_engine_run_op": (C.c_int, [c_vp, C.c_int, C.c_int, c_vp]),
     "skps_engine_op_kernel": (C.c_int, [c_vp, C.c_int, c_i32p]),
+    "skps_engine_set_num_sms": (C.c_int, [c_vp, C.c_int]),
+    "skps_engine_op_grid": (C.c_int, [c_vp, C.c_int, C.c_int, c_i32p]),
     "skps_debug_conv_tc": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, C.c_int, C.c_int,
                                      C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, c_vp, C.c_int, c_vp]),
     "skps_debug_conv_tc2": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, C.c_int, C.c_int,

@@ -41,6 +41,11 @@ CASES = [
     (2, 3, 12, 20, 40, 120, HSWISH, False, (64, 16), (136, 8)),
     (2, 2, 16, 16, 80, 184, RELU, True, (96, 8), (200, 16)),
     (3, 4, 5, 7, 160, 960, NONE, True, (176, 16), (1000, 24)),
+    # more units than SMs: every CTA walks several units, so both consumer warpgroups take work and every ring wraps
+    (150, 150, 16, 16, 80, 184, HSWISH, False, None, None),         # 300 tiles x 2 chunks
+    # ... with the partial last tile (188 tiles, the last one 64 pixels) on a CTA's second unit, that is on warpgroup 1
+    # on 132 SMs, and channel windows on both sides
+    (100, 101, 12, 20, 40, 120, HSWISH, True, (64, 16), (136, 8)),
 ]
 
 

@@ -63,6 +63,8 @@ def _run(N, H, W, Cin, Cout, k, dil, act, with_bias=True, with_res=False, out_sp
     (1, 64, 64, 96, 128, 3, 1, 1, dict(with_res=True, out_split=True)),
     (2, 12, 64, 64, 64, 3, 1, 1, dict(with_res=True, out_split=True)),     # H = 12
     (2, 64, 64, 128, 128, 3, 1, 2, dict(with_res=True, out_split=True)),
+    # more pixel tiles than SMs (640): the persistent loop wraps every ring and reuses the epilogue staging buffers
+    (20, 64, 64, 64, 64, 3, 1, 1),
 ])
 def test_conv_tc_matches_fp32(cfg):
     err = _run(*cfg[:8], **(cfg[8] if len(cfg) > 8 else {}))
@@ -77,6 +79,7 @@ def test_conv_tc_matches_fp32(cfg):
     (3, 8, 128, 72, 104, 3, 1, 2),       # two-row tiles, K tail (72 channels), ragged Cout
     (2, 16, 256, 64, 128, 5, 1, 1),      # 5x5, one row per tile
     (3, 16, 16, 160, 128, 3, 2, 1),      # 16-wide map: a tile is a whole image, store boxes of 2 rows x 16 pixels
+    (12, 64, 64, 128, 128, 3, 1, 1),     # more tiles than SMs (192): the persistent loop wraps
 ])
 def test_conv_tct_transposed_kernel(cfg):
     err = _run(*cfg, out_split=True)
@@ -104,6 +107,7 @@ def test_conv_tc_residual_before_activation():
     (2, 32, 32, 40, 72, 3, 1, 0),
     (4, 16, 16, 72, 144, 3, 1, 0),       # output 8x8: two images per tile
     (3, 16, 16, 72, 144, 3, 1, 1),       # ... with a partial last tile
+    (160, 32, 32, 40, 72, 3, 1, 0),      # more tiles than SMs (320)
 ])
 def test_conv_tc_stride2(cfg):
     err = _run(*cfg, stride=2)
@@ -155,6 +159,8 @@ def test_conv_mma_small_channel_3x3():
     assert _run_mma(3, 32, 32, 40, 1, with_res=True, res_first=True, out_split=False) < 1e-5
     assert _run_mma(2, 32, 32, 40, 0, with_res=True, res_first=False) < 1e-5
     assert _run_mma(1, 24, 40, 24, 0) < 1e-5                                             # partial tiles in both directions
+    # more tiles (2048) than the grid's SMs x CTAs per SM: every CTA walks its double buffer through several tiles
+    assert _run_mma(64, 64, 64, 24, 1, with_res=True, res_first=True) < 1e-5
 
 
 @pytest.mark.parametrize("x_scale", [1e-3, 1.0, 1e3])
@@ -193,7 +199,8 @@ def test_conv_tc_elementwise_error_bound_small_and_large_inputs(x_scale):
     assert worst <= 1.0
 
 
-@pytest.mark.parametrize("shape", [(3, 64, 64, 128, 104), (2, 32, 32, 128, 98), (5, 16, 16, 64, 24), (1, 8, 32, 72, 128)])
+@pytest.mark.parametrize("shape", [(3, 64, 64, 128, 104), (2, 32, 32, 128, 98), (5, 16, 16, 64, 24), (1, 8, 32, 72, 128),
+                                   (12, 64, 64, 128, 98)])        # more tiles than SMs (192)
 def test_conv_hm_transposed_head_matches_fp64_argmax(shape):
     """csrc/conv_hm.cu: score maps as accumulator rows, per-tile (max, first arg-max) from a per-thread scan.  Against an fp64
     conv: the per-tile maximum within fp32 noise, and the reported pixel must BE a maximum of its tile (its fp64 score within

@@ -104,6 +104,7 @@ def test_xf_depthwise_pointwise_matches_fp32(cfg):
     (3, 32, 32, 40, 256, 256),          # decoder/upsampler1 head (N = 256: two halves of 128)
     (1, 16, 32, 8, 64, 16),             # smallest legal map, one skip sub-chunk
     (2, 16, 16, 40, 64, 32),            # map one tile wide: first and last columns in the same tile (Student@128)
+    (150, 16, 16, 40, 64, 32),          # more tiles than SMs (300): the persistent loop wraps the rings
 ])
 def test_xf_upsample_concat_depthwise_pointwise_matches_fp32(cfg):
     N, H, W, Cs, Cl, Cout = cfg

@@ -391,6 +391,17 @@ class EngineOps:
         self.rt.check(self.lib.skps_engine_run_op(self.eng.handle, i, self.batch, self.eng.stream.cuda_stream))
         self.eng.stream.synchronize()
 
+    def op_grid(self, i):
+        """(CTAs, work units) of op i's launch if it runs a persistent kernel, else (0, 0)."""
+        import ctypes as C
+        g = (C.c_int32 * 2)()
+        self.rt.check(self.lib.skps_engine_op_grid(self.eng.handle, i, self.batch, g))
+        return g[0], g[1]
+
+    def set_num_sms(self, n):
+        """Size the persistent kernels' grids for n SMs (0: the device's)."""
+        self.rt.check(self.lib.skps_engine_set_num_sms(self.eng.handle, n))
+
 
 class InterpOps:
     """The float32 PlanInterp standing in for the engine (the checker's own test, without a GPU).  Kernel ids are the
@@ -723,6 +734,38 @@ def coverage(tagged):
         for h in hit:
             if h in cov:
                 cov[h].append("%s:%d" % (tag, r.index))
+    return cov
+
+
+# The persistent kernels launch min(units, SMs) CTAs (conv_mma: SMs x its CTAs per SM), and each CTA walks units
+# blockIdx.x, + gridDim.x, ...: the ring phases, conv_pw's alternating warpgroups, the reuse of the epilogue staging buffers
+# and the stem block's prefetch only act from a CTA's second unit on.  A sweep with the grid capped below the SM count
+# (skps_engine_set_num_sms) must reach these.
+PERSISTENT = {K_TC: "tc", K_TCT: "tct", K_HM: "hm", K_PW: "pw", K_XF: "xf", K_FPW: "fpw", K_STEM: "stem_block",
+              K_MMA: "mma"}
+WALK_BRANCHES = ["%s >= 3 units per CTA" % PERSISTENT[k] for k in sorted(PERSISTENT)] + [
+    "pw every CTA >= 4 units, last unit on each warpgroup"]
+
+
+def units_per_cta(ctas, units):
+    """Units each CTA of a persistent launch walks: CTA b takes units b, b + ctas, ... (ascending in b's order)."""
+    return [len(range(b, units, ctas)) for b in range(ctas)]
+
+
+def walk_coverage(walks):
+    """Branch name -> ["plan:op index@cap", ...] for every name in WALK_BRANCHES, over (label, kernel, ctas, units)
+    tuples, one per persistent launch.  conv_pw gives unit `local` of a CTA to warpgroup local % 2: with at least 4 units
+    on every CTA each warpgroup takes at least 2, and a grid that does not divide the units leaves CTAs with an odd and
+    CTAs with an even count, so the last unit falls on warpgroup 0 on some and on warpgroup 1 on others."""
+    cov = {b: [] for b in WALK_BRANCHES}
+    for label, kernel, ctas, units in walks:
+        if kernel not in PERSISTENT or not ctas:
+            continue
+        per = units_per_cta(ctas, units)
+        if max(per) >= 3:
+            cov["%s >= 3 units per CTA" % PERSISTENT[kernel]].append(label)
+        if kernel == K_PW and min(per) >= 4 and units % ctas:
+            cov["pw every CTA >= 4 units, last unit on each warpgroup"].append(label)
     return cov
 
 
