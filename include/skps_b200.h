@@ -214,8 +214,11 @@ SKPS_API int skps_detect_post_batch(const float* raw, int rows, int batch, float
                                     int capacity, void* workspace, size_t workspace_bytes, void* stream);
 
 /* FaceAna.judge_boxs + sort_and_filter (facer.py:120-189): IoU-match detections against the
- * previous track boxes (EMA alpha), drop area<=min_face, keep top_k (<= 64) by area.  Any number
- * of detections.  `track` [dev] (n_track,4) may be NULL.  Writes (count,4) boxes. */
+ * previous track boxes (EMA alpha), drop area<=min_face, keep top_k (1..SKPS_MAX_TOP_K) by area:
+ * all of them in detector order when at most top_k pass, else the top_k largest, descending,
+ * equal areas later index first.  Any number of detections; one block per call, a radix select
+ * whose passes over the detections do not grow with top_k.  `track` [dev] (n_track,4) may be
+ * NULL.  Writes (count,4) boxes. */
 SKPS_API int skps_select_faces(const float* det_rows, const int32_t* det_count, int det_stride,
                       const float* track, int n_track,
                       float iou_thres, float alpha, float one_minus_alpha,
@@ -240,6 +243,13 @@ SKPS_API int skps_frame_absdiff_sum(const uint8_t* a, const uint8_t* b, size_t n
 
 /* ------------------------------------------------------------------ FaceAna.run (facer.py:52-85) */
 
+/* Largest top_k of skps_select_faces and skps_pipeline_* (the reference's Detect.topk has no cap). */
+#define SKPS_MAX_TOP_K 1024
+/* Faces per landmark forward in skps_pipeline_run: the landmark engine needs max_batch >=
+ * min(top_k, SKPS_LANDMARK_CHUNK).  The Student@256 plan holds about 47 MB of activations per
+ * face of max_batch, so a full chunk takes about 3 GB whatever top_k is. */
+#define SKPS_LANDMARK_CHUNK 64
+
 typedef struct skps_pipeline_cfg {
     float score_thres, iou_thres;       /* Skps.yml Detect.score_thrs / iou_thrs         */
     float min_face;                     /* Detect.min_face (area)                        */
@@ -262,6 +272,12 @@ SKPS_API int skps_pipeline_reset(skps_pipeline* p);
  * letterbox geometry (rw,rh,top,left,scale) is computed by the caller exactly as
  * face_detector.py:51-62 does.  `track` [host] (n_track,4) float32 previous track boxes or
  * NULL.  If run_detector==0 the `track` boxes are used as the face boxes (facer.py:61).
+ * top_k is 1..SKPS_MAX_TOP_K and `track` holds at most max(256, top_k) boxes.
+ * The face count is read back after the selection, then the landmark net runs on exactly the
+ * n_faces crops, in ceil(n_faces / SKPS_LANDMARK_CHUNK) forwards (none for a faceless frame).
+ * The landmark engine captures one CUDA graph per batch size it meets, so up to
+ * SKPS_LANDMARK_CHUNK graphs are captured lazily, each on the first frame with that many faces
+ * in a chunk.  A face's results do not depend on the chunk it runs in.
  * Results [host]: n_faces, boxes (top_k,4) — the boxes handed to the landmark stage
  * (facer.py:66 boxes_return), kps (top_k,n_points,2), scores (top_k,n_points),
  * n_det = the number of boxes the detector kept (every one of them goes through judge_boxs and

@@ -16,10 +16,14 @@ import yaml
 from ... import runtime as rt
 from ...graph_tools import check_detector_input
 from ...logger.logger import logger
-from ..smoother.lk import EmaFilter, GroupTrack
+from ..smoother.lk import EmaFilter, GroupTrack, first_match, rects
 from .face_detector import FaceDetector, letterbox_geometry
 from .face_landmark import FaceLandmark
 from .align import check_size
+
+
+MAX_TOP_K = 1024           # SKPS_MAX_TOP_K of include/skps_b200.h
+LANDMARK_CHUNK = 64        # SKPS_LANDMARK_CHUNK: faces per landmark forward in skps_pipeline_run
 
 
 def get_cfg():
@@ -40,19 +44,23 @@ class FaceAna():
         det_input: None (Skps.yml's Detect.input_shape, 384x640), or the detector input size (h, w): multiples of 32 in
         128..2176 x 128..3840.  Every frame is letterboxed to that size, so a larger one finds smaller faces: at 1152x1920
         a 3840x2160 frame is scaled by 1/2 instead of 1/6.  The detector's work and activation memory grow with h*w
-        (3.97 GMAC and 0.35 GB at 1152x1920, 0.44 GMAC and 0.04 GB at 384x640)."""
+        (3.97 GMAC and 0.35 GB at 1152x1920, 0.44 GMAC and 0.04 GB at 384x640).
+        top_k: None (Skps.yml's Detect.topk, 5), or 1..1024 faces per frame.  The landmark net runs on the faces found,
+        in chunks of at most 64, so its activation memory is that of min(top_k, 64) faces (about 47 MB per face)."""
+        cfg = get_cfg()
+        self.top_k = int(top_k if top_k is not None else cfg['Skps']['Detect']['topk'])
+        if not 1 <= self.top_k <= MAX_TOP_K:
+            raise ValueError("top_k %d outside 1..%d" % (self.top_k, MAX_TOP_K))
         if det_input is not None:
             det_input = check_detector_input(det_input)
         self.align = None if align is None else check_size(align)
         self.pose = bool(pose)
         if verbose:
             logger.setLevel(logging.DEBUG)
-        cfg = get_cfg()
         if det_input is not None:
             cfg['Skps']['Detect']['input_shape'] = [det_input[0], det_input[1], 3]
-        self.top_k = int(top_k if top_k is not None else cfg['Skps']['Detect']['topk'])
         self.face_detector = FaceDetector(cfg['Skps']['Detect'])
-        self.face_landmark = FaceLandmark(cfg['Skps']['Keypoints'], max_faces=self.top_k)
+        self.face_landmark = FaceLandmark(cfg['Skps']['Keypoints'], max_faces=min(self.top_k, LANDMARK_CHUNK))
         self.trace = GroupTrack(cfg['Skps']['Trace'])
         logger.info('model init done!')
         self.track_box = None
@@ -137,11 +145,7 @@ class FaceAna():
 
         landmarks = self.trace.calculate(image, landmarks)
 
-        track = []
-        for i in range(landmarks.shape[0]):
-            track.append([np.min(landmarks[i][:, 0]), np.min(landmarks[i][:, 1]),
-                          np.max(landmarks[i][:, 0]), np.max(landmarks[i][:, 1])])
-        tmp_box = np.array(track)
+        tmp_box = rects(landmarks) if landmarks.shape[0] else np.array([])
         self.track_box = self.judge_boxs(boxes_return, tmp_box)
         res = self.to_dict(self.track_box, landmarks, states)
         if self.align is not None and res:
@@ -204,15 +208,18 @@ class FaceAna():
         """facer.py:144-189."""
         if previuous_bboxs is None:
             return now_bboxs
-        out = []
-        for now in now_bboxs:
-            matched = None
-            for prev in previuous_bboxs:
-                if _iou(now, prev) > self.iou_thres:
-                    matched = prev
-                    break
-            out.append(now[0:4] if matched is None else self.smooth(now, matched))
-        return np.array(out)
+        if len(now_bboxs) == 0:
+            return np.array([])
+        now = now_bboxs[:, :4]
+        prev = previuous_bboxs[:, :4] if len(previuous_bboxs) else np.zeros((0, 4), now.dtype)
+        match = first_match(now, prev, self.iou_thres)
+        hit = match >= 0
+        if not hit.any():
+            return now.copy()
+        ema = self.filter(now[hit], prev[match[hit]])
+        out = now.astype(np.result_type(now, ema))        # np.array of the rows: float64 if any row is
+        out[hit] = ema
+        return out
 
     def smooth(self, now_box, previous_box):
         return self.filter(now_box[:4], previous_box[:4])
@@ -224,11 +231,3 @@ class FaceAna():
         self.previous_box = None
         rt.check(self.lib.skps_pipeline_reset(self._pipe))
 
-
-def _iou(rec1, rec2):
-    s1 = (rec1[2] - rec1[0]) * (rec1[3] - rec1[1])
-    s2 = (rec2[2] - rec2[0]) * (rec2[3] - rec2[1])
-    x1, y1 = max(rec1[0], rec2[0]), max(rec1[1], rec2[1])
-    x2, y2 = min(rec1[2], rec2[2]), min(rec1[3], rec2[3])
-    inter = max(0, x2 - x1) * max(0, y2 - y1)
-    return inter / (s1 + s2 - inter)

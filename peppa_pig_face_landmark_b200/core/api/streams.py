@@ -41,6 +41,11 @@ class FaceAnaStreams:
         det_cfg, kps_cfg, tr_cfg = cfg['Detect'], cfg['Keypoints'], cfg['Trace']
         self.n_streams = int(n_streams)
         self.top_k = int(top_k if top_k is not None else det_cfg['topk'])
+        if not 1 <= self.top_k <= 64:
+            # one landmark forward of n_streams * top_k faces per call, sized on the device with no host read-back, so
+            # top_k bounds its memory (about 47 MB per face); FaceAna takes up to 1024
+            raise ValueError("FaceAnaStreams: top_k %d outside 1..64 (the landmark batch is n_streams * top_k faces; "
+                             "FaceAna takes up to 1024)" % self.top_k)
         root = pathlib.Path(__file__).resolve().parents[2]
         det_hw = det_cfg['input_shape'][:2] if det_input is None else check_detector_input(det_input)
         self.det = ONNXEngine(detector_onnx_for(os.path.join(root, det_cfg['model_path']), det_hw), device=device,

@@ -1,6 +1,7 @@
-"""Temporal smoothing of landmarks and boxes — host-side numpy, O(K*98) per frame, stateful.
+"""Temporal smoothing of landmarks and boxes — host-side numpy, stateful.
 Same classes and call signatures as the reference's Skps/core/smoother/lk.py (GroupTrack :6-91,
-OneEuroFilter :105-149, EmaFilter :155-162)."""
+OneEuroFilter :105-149, EmaFilter :155-162).  The reference matches faces pair by pair in Python; here one
+(n_now, n_prev) IoU matrix and one filter call per frame give bit for bit the same arrays, dtypes included."""
 import math
 
 import numpy as np
@@ -19,6 +20,48 @@ def _bbox_of(points):
     return [np.min(points[:, 0]), np.min(points[:, 1]), np.max(points[:, 0]), np.max(points[:, 1])]
 
 
+def rects(sets):
+    """[min x, min y, max x, max y] of every landmark set (n, P, 2) -> (n, 4), in the sets' dtype."""
+    return np.stack([sets[:, :, 0].min(1), sets[:, :, 1].min(1), sets[:, :, 0].max(1), sets[:, :, 1].max(1)], 1)
+
+
+def first_match(r1, r2, thres):
+    """For every row of r1 (n, 4), the first row of r2 (m, 4) with iou > thres, else -1: what the reference's loop
+    `for prev in r2: if iou(now, prev) > thres: break` finds with _iou on numpy scalars.
+
+    Python's min / max return one of their operands, each with its own dtype, and numpy then computes in float32 only
+    when both operands are float32 (float64 otherwise).  With r1 and r2 of different dtypes that choice is made per
+    element, so each intermediate carries a "float32" flag next to its float64 value."""
+    n, m = r1.shape[0], r2.shape[0]
+    if n == 0 or m == 0:
+        return np.full(n, -1, np.int64)
+    f32, f64 = np.float32, np.float64
+    a32, b32 = r1.dtype == f32, r2.dtype == f32
+    a, b = r1.astype(f64)[:, None, :], r2.astype(f64)[None, :, :]
+
+    def pick(take_b, c):                 # value and float32 flag of `b[c] if take_b else a[c]`
+        return np.where(take_b, b[..., c], a[..., c]), np.where(take_b, b32, a32)
+
+    def sub(x, y):
+        (xv, x32), (yv, y32) = x, y
+        both = x32 & y32
+        return np.where(both, (xv.astype(f32) - yv.astype(f32)).astype(f64), xv - yv), both
+
+    with np.errstate(all="ignore"):      # the float32 branch of np.where is also evaluated on float64 values
+        w = sub(pick(b[..., 2] < a[..., 2], 2), pick(b[..., 0] > a[..., 0], 0))     # min(r1[2], r2[2]) - max(r1[0], r2[0])
+        h = sub(pick(b[..., 3] < a[..., 3], 3), pick(b[..., 1] > a[..., 1], 1))
+        both = w[1] & h[1]
+        inter = np.where(both, (w[0].astype(f32) * h[0].astype(f32)).astype(f64), w[0] * h[0])
+        area1 = (r1[:, 2] - r1[:, 0]) * (r1[:, 3] - r1[:, 1])
+        area2 = (r2[:, 2] - r2[:, 0]) * (r2[:, 3] - r2[:, 1])
+        s = area1[:, None] + area2[None, :]                       # float32 only when both rects are float32
+        inter = inter.astype(s.dtype)
+        iou = inter / (s - inter)
+        # max(0, w) * max(0, h) is 0 (iou 0 or nan) unless both are positive
+        hit = (w[0] > 0) & (h[0] > 0) & (iou > thres)
+    return np.where(hit.any(1), hit.argmax(1), -1)
+
+
 def _iou(r1, r2):
     a1 = (r1[2] - r1[0]) * (r1[3] - r1[1])
     a2 = (r2[2] - r2[0]) * (r2[3] - r2[1])
@@ -35,8 +78,9 @@ class OneEuroFilter:
         self.min_cutoff, self.beta, self.d_cutoff = min_cutoff, beta, d_cutoff
 
     def __call__(self, x, x_prev, dx_prev):
-        speed = np.sqrt(np.sum((x - x_prev) ** 2, axis=1))
-        speed_prev = np.sqrt(np.sum(dx_prev ** 2, axis=1))
+        """x, x_prev, dx_prev: (P, 2) for one face or (n, P, 2) for n faces at once."""
+        speed = np.sqrt(np.sum((x - x_prev) ** 2, axis=-1))
+        speed_prev = np.sqrt(np.sum(dx_prev ** 2, axis=-1))
         speed_hat = _blend(_alpha(self.d_cutoff), speed, speed_prev)
         a = _alpha(self.min_cutoff + self.beta * np.abs(speed_hat))
         a = np.expand_dims(a, -1)
@@ -78,21 +122,22 @@ class GroupTrack:
             self.previous_landmarks_set = now_landmarks_set
             self.previous_dx = np.zeros_like(now_landmarks_set)
             return now_landmarks_set
-        result, deltas = [], []
-        for cur in now_landmarks_set:
-            match = None
-            for j in range(prev.shape[0]):
-                if self.iou(cur, prev[j]) > self.iou_thres:
-                    match = j
-                    break
-            if match is None:
-                result.append(cur)
-                deltas.append(np.zeros_like(cur))
+        now = now_landmarks_set
+        if now.shape[0] == 0:
+            result, deltas = np.array([]), np.array([])
+        else:
+            match = first_match(rects(now), rects(prev), self.iou_thres)
+            hit = match >= 0
+            if not hit.any():
+                result, deltas = now.copy(), np.zeros_like(now)
             else:
-                f = self.smooth(cur / scale, prev[match] / scale, self.previous_dx[match] / scale) * scale
-                result.append(f)
-                deltas.append(prev[match] - f)
-        result = np.array(result)
+                # np.array of float32 and float64 rows is float64: unmatched rows are the landmarks as they came
+                j = match[hit]
+                f = self.smooth(now[hit] / scale, prev[j] / scale, self.previous_dx[j] / scale) * scale
+                result = now.astype(np.float64)
+                result[hit] = f
+                deltas = np.zeros(now.shape, np.float64)
+                deltas[hit] = prev[j] - f
         self.previous_landmarks_set = result
-        self.previous_dx = np.array(deltas)
+        self.previous_dx = deltas
         return result

@@ -217,7 +217,8 @@ __device__ __forceinline__ float iou_track(const float* r1, const float* r2) {
 }
 
 constexpr int SEL_THREADS = 256;
-constexpr int SEL_CACHE = 4096;       // selection keys kept in shared memory; later detections recompute theirs
+constexpr int SEL_CACHE = 8192;       // area orders kept in shared memory (32 KB); later detections recompute theirs
+constexpr int SEL_MAX_K = SKPS_MAX_TOP_K;
 
 // judge_boxs for one detection: the box after the EMA with the first track box it matches (facer.py:176-181, lk.py:95-96)
 __device__ __forceinline__ void judged_box(const float* now, const float* __restrict__ track, int n_track, float iou_thres,
@@ -235,39 +236,48 @@ __device__ __forceinline__ void judged_box(const float* now, const float* __rest
 // Selection key of detection i: 0 when its area fails the filter, else (area, i) as one integer with the order of
 // "larger area first, ties by later index first" (facer.py:138 area.argsort()[-k:][::-1], a stable ascending sort read
 // backwards).  +0.f turns an area of -0 into +0, which compares equal to it in float.
-__device__ __forceinline__ unsigned long long select_key(const float* __restrict__ det, int det_stride, int i,
-                                                         const float* __restrict__ track, int n_track, float iou_thres,
-                                                         float alpha, float oma, float min_face) {
+// The upper half of the key: 0 when the area fails the filter, else the area's bits in an unsigned order that sorts like
+// the float.  ord >= 0x007fffff, so a passing key is never 0.
+__device__ __forceinline__ unsigned select_ord(const float* __restrict__ det, int det_stride, int i,
+                                               const float* __restrict__ track, int n_track, float iou_thres, float alpha,
+                                               float oma, float min_face) {
     float b[4];
     judged_box(det + (long long)i * det_stride, track, n_track, iou_thres, alpha, oma, b);
     const float area = (b[2] - b[0]) * (b[3] - b[1]);
-    if (!(area > min_face)) return 0ull;
+    if (!(area > min_face)) return 0u;
     const unsigned u = __float_as_uint(area + 0.f);
-    const unsigned ord = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-    return ((unsigned long long)ord << 32) | (unsigned)i;     // ord >= 0x007fffff: a passing key is never 0
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ unsigned long long select_key(unsigned ord, int i) {
+    return ord ? ((unsigned long long)ord << 32) | (unsigned)i : 0ull;
 }
 
+// Selection for any top_k <= SEL_MAX_K in a number of passes over the keys that does not grow with top_k: a radix select
+// (8-bit digits, most significant first) finds the top_k-th largest key T, the keys >= T are gathered and bitonic-sorted
+// descending.  Keys past the shared cache are recomputed once per pass.
 __device__ __forceinline__ void select_faces_body(const float* __restrict__ det, int n_det, int det_stride,
                                                   const float* __restrict__ track, int n_track, float iou_thres, float alpha,
                                                   float oma, float min_face, int top_k, float* __restrict__ boxes4,
                                                   int* __restrict__ count) {
-    __shared__ unsigned long long s_key[SEL_CACHE];
-    __shared__ unsigned long long s_best[2][SEL_THREADS / 32];
+    __shared__ unsigned s_ord[SEL_CACHE];
+    __shared__ unsigned long long s_win[SEL_MAX_K];
+    __shared__ int s_sel[SEL_MAX_K];
+    __shared__ int s_hist[256];
     __shared__ int s_wcount[SEL_THREADS / 32];
-    __shared__ int s_sel[64];
-    __shared__ int s_m;
+    __shared__ int s_m, s_bin, s_krem, s_done;
     const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5, nw = nt >> 5;
     const int n = max(n_det, 0);
     auto key_of = [&](int i) {
-        return i < SEL_CACHE ? s_key[i] : select_key(det, det_stride, i, track, n_track, iou_thres, alpha, oma, min_face);
+        return select_key(i < SEL_CACHE ? s_ord[i]
+                                        : select_ord(det, det_stride, i, track, n_track, iou_thres, alpha, oma, min_face), i);
     };
     if (tid == 0) s_m = 0;
     __syncthreads();
     int my_m = 0;
     for (int i = tid; i < n; i += nt) {
-        const unsigned long long k = select_key(det, det_stride, i, track, n_track, iou_thres, alpha, oma, min_face);
-        if (i < SEL_CACHE) s_key[i] = k;
-        my_m += k != 0ull;
+        const unsigned o = select_ord(det, det_stride, i, track, n_track, iou_thres, alpha, oma, min_face);
+        if (i < SEL_CACHE) s_ord[i] = o;
+        my_m += o != 0u;
     }
     if (my_m) atomicAdd(&s_m, my_m);
     __syncthreads();
@@ -292,32 +302,78 @@ __device__ __forceinline__ void select_faces_body(const float* __restrict__ det,
             __syncthreads();
         }
     } else {
-        // top_k rounds of a block-wide maximum over the keys below the previous pick
-        unsigned long long prev = ~0ull;
-        for (int k = 0; k < top_k; ++k) {
-            unsigned long long best = 0ull;
+        // radix select of the top_k-th largest passing key; the passing keys are unique, so exactly top_k are >= it
+        unsigned long long prefix = 0ull, mask = 0ull;
+        int k_rem = top_k;
+        for (int shift = 56; shift >= 0; shift -= 8) {
+            for (int b = tid; b < 256; b += nt) s_hist[b] = 0;
+            __syncthreads();
             for (int i = tid; i < n; i += nt) {
                 const unsigned long long q = key_of(i);
-                if (q < prev && q > best) best = q;
+                if (q != 0ull && (q & mask) == prefix) atomicAdd(&s_hist[(int)(q >> shift) & 255], 1);
             }
-            for (int o = 16; o > 0; o >>= 1) {
-                const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o);
-                best = other > best ? other : best;
-            }
-            if (lane == 0) s_best[k & 1][warp] = best;
             __syncthreads();
-            best = 0ull;
-            for (int q = 0; q < nw; ++q) best = s_best[k & 1][q] > best ? s_best[k & 1][q] : best;
-            if (tid == 0) s_sel[k] = (int)(unsigned)(best & 0xffffffffu);
-            prev = best;
+            if (warp == 0) {
+                // lane l owns digits 255-8l .. 248-8l; `above` = keys with a larger digit than the lane's first
+                int c[8], sum = 0;
+#pragma unroll
+                for (int q = 0; q < 8; ++q) { c[q] = s_hist[255 - (lane * 8 + q)]; sum += c[q]; }
+                int incl = sum;
+                for (int o = 1; o < 32; o <<= 1) {
+                    const int v = __shfl_up_sync(0xffffffffu, incl, o);
+                    if (lane >= o) incl += v;
+                }
+                int above = incl - sum;
+#pragma unroll
+                for (int q = 0; q < 8; ++q) {
+                    if (above < k_rem && above + c[q] >= k_rem) {
+                        s_bin = 255 - (lane * 8 + q);
+                        s_krem = k_rem - above;
+                        s_done = above + c[q] == k_rem;       // every key with this digit is in: T has zero lower digits
+                    }
+                    above += c[q];
+                }
+            }
+            __syncthreads();
+            prefix |= (unsigned long long)s_bin << shift;
+            mask |= 0xffull << shift;
+            k_rem = s_krem;
+            const bool done = s_done;
+            __syncthreads();
+            if (done) break;
         }
+        // gather the top_k keys >= T (in any order), sort them descending
+        if (tid == 0) s_m = 0;
+        __syncthreads();
+        for (int i = tid; i < n; i += nt) {
+            const unsigned long long q = key_of(i);
+            if (q != 0ull && q >= prefix) s_win[atomicAdd(&s_m, 1)] = q;
+        }
+        int np2 = 1;
+        while (np2 < m) np2 <<= 1;
+        __syncthreads();
+        for (int i = m + tid; i < np2; i += nt) s_win[i] = 0ull;
+        __syncthreads();
+        for (int k = 2; k <= np2; k <<= 1) {
+            for (int j = k >> 1; j > 0; j >>= 1) {
+                for (int i = tid; i < np2; i += nt) {
+                    const int ixj = i ^ j;
+                    if (ixj > i) {
+                        const unsigned long long a = s_win[i], b = s_win[ixj];
+                        if (((i & k) == 0) ? (a < b) : (a > b)) { s_win[i] = b; s_win[ixj] = a; }
+                    }
+                }
+                __syncthreads();
+            }
+        }
+        for (int i = tid; i < m; i += nt) s_sel[i] = (int)(unsigned)(s_win[i] & 0xffffffffull);
         __syncthreads();
     }
     if (tid == 0) *count = m;
-    if (tid < m * 4) {
+    for (int f = tid; f < m; f += nt) {
         float b[4];
-        judged_box(det + (long long)s_sel[tid / 4] * det_stride, track, n_track, iou_thres, alpha, oma, b);
-        boxes4[tid] = b[tid % 4];
+        judged_box(det + (long long)s_sel[f] * det_stride, track, n_track, iou_thres, alpha, oma, b);
+        for (int c = 0; c < 4; ++c) boxes4[f * 4 + c] = b[c];
     }
 }
 
@@ -502,7 +558,7 @@ extern "C" SKPS_API int skps_letterbox(const uint8_t* frame, int H, int W, int p
 extern "C" SKPS_API int skps_select_faces(const float* det_rows, const int32_t* det_count, int det_stride, const float* track,
                                  int n_track, float iou_thres, float alpha, float one_minus_alpha, float min_face,
                                  int top_k, float* boxes4, int32_t* count, void* stream) {
-    SKPS_CHECK(det_rows && det_count && boxes4 && count && top_k > 0 && top_k <= 64, "select_faces: bad arguments");
+    SKPS_CHECK(det_rows && det_count && boxes4 && count && top_k > 0 && top_k <= SEL_MAX_K, "select_faces: bad arguments");
     select_faces_kernel<<<1, SEL_THREADS, 0, (cudaStream_t)stream>>>(det_rows, det_count, det_stride, track,
                                                             track ? n_track : 0, iou_thres, alpha, one_minus_alpha,
                                                             min_face, top_k, boxes4, count);

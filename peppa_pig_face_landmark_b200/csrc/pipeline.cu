@@ -1,9 +1,11 @@
 // skps_pipeline: the device-side chain of FaceAna.run (Skps/core/api/facer.py:52-85):
 //   frame -> letterbox -> detector -> NMS/un-letterbox -> judge_boxs(track) -> sort_and_filter
 //         -> per-face crop+resize -> landmark net -> de-normalise
-// One H2D copy of the frame in, one D2H copy of the packed results out, nothing in between
-// touches the host.  The temporal smoothing that follows (GroupTrack, facer.py:71-82) is O(K*98)
-// host math on the returned landmarks.
+// One H2D copy of the frame in, the face count read back after the selection, one D2H copy of the
+// packed results out.  The landmark net runs on exactly the selected faces, in chunks of at most
+// SKPS_LANDMARK_CHUNK, so its activations stay those of one chunk whatever top_k is (up to 1024).
+// The temporal smoothing that follows (GroupTrack, facer.py:71-82) is host math on the returned
+// landmarks.
 #include <string.h>
 
 #include <vector>
@@ -30,7 +32,9 @@ struct skps_pipeline {
     float* d_det_rows = nullptr; int32_t* d_det_idx = nullptr; int32_t* d_det_count = nullptr;
     float* d_track = nullptr;
     float* d_boxes = nullptr; int32_t* d_count = nullptr; int32_t* d_detail = nullptr;
-    float* d_kps = nullptr;
+    float* d_kps = nullptr; float* d_scores = nullptr;
+    int32_t* d_counts = nullptr;                  // d_counts[c] = c for c in 0..SKPS_LANDMARK_CHUNK: per-chunk face counts
+    int track_cap = 0;                            // track boxes accepted: max(256, top_k)
     unsigned long long* d_diff = nullptr;
     // packed host result block (pinned)
     struct Host {
@@ -53,7 +57,7 @@ extern "C" SKPS_API void skps_pipeline_destroy(skps_pipeline* p) {
     for (int i = 0; i < 2; ++i) if (p->d_frame[i]) cudaFree(p->d_frame[i]);
     if (p->h_frame) cudaFreeHost(p->h_frame);
     void* dev[] = {p->d_det_rows, p->d_det_idx, p->d_det_count, p->d_nms_ws, p->d_track, p->d_boxes, p->d_count, p->d_detail,
-                   p->d_kps, p->d_diff, p->d_align_kps, p->d_align_M, p->d_chips,
+                   p->d_kps, p->d_scores, p->d_counts, p->d_diff, p->d_align_kps, p->d_align_M, p->d_chips,
                    p->d_pose_kps, p->d_pose};
     for (void* q : dev) if (q) cudaFree(q);
     void* host[] = {p->h_res, p->h_boxes, p->h_kps, p->h_scores, p->h_det_idx, p->h_det_rows, p->h_track};
@@ -64,7 +68,8 @@ extern "C" SKPS_API void skps_pipeline_destroy(skps_pipeline* p) {
 extern "C" SKPS_API int skps_pipeline_create(skps_engine* det, skps_engine* kps, const skps_pipeline_cfg* cfg,
                                     skps_pipeline** out) {
     SKPS_CHECK(det && kps && cfg && out, "pipeline_create: null argument");
-    SKPS_CHECK(cfg->top_k > 0 && cfg->top_k <= 64, "pipeline_create: top_k %d outside 1..64", cfg->top_k);
+    SKPS_CHECK(cfg->top_k > 0 && cfg->top_k <= SKPS_MAX_TOP_K, "pipeline_create: top_k %d outside 1..%d", cfg->top_k,
+               SKPS_MAX_TOP_K);
     skps_pipeline* p = new skps_pipeline();
     p->det = det; p->kps = kps; p->cfg = *cfg;
     int c = 0;
@@ -89,11 +94,14 @@ extern "C" SKPS_API int skps_pipeline_create(skps_engine* det, skps_engine* kps,
     PALLOC(p->d_det_idx, sizeof(int32_t) * p->det_rows);
     PALLOC(p->d_det_count, sizeof(int32_t));
     PALLOC(p->d_nms_ws, nms_workspace_bytes(p->det_rows, 1));
-    PALLOC(p->d_track, sizeof(float) * 4 * 256);
+    p->track_cap = K > 256 ? K : 256;
+    PALLOC(p->d_track, sizeof(float) * 4 * p->track_cap);
     PALLOC(p->d_boxes, sizeof(float) * 4 * K);
     PALLOC(p->d_count, sizeof(int32_t));
     PALLOC(p->d_detail, sizeof(int32_t) * 5 * K);
     PALLOC(p->d_kps, sizeof(float) * 2 * P * K);
+    PALLOC(p->d_scores, sizeof(float) * P * K);
+    PALLOC(p->d_counts, sizeof(int32_t) * (SKPS_LANDMARK_CHUNK + 1));
     PALLOC(p->d_diff, sizeof(unsigned long long));
     HALLOC(p->h_res, sizeof(skps_pipeline::Host));
     HALLOC(p->h_boxes, sizeof(float) * 4 * K);
@@ -101,8 +109,11 @@ extern "C" SKPS_API int skps_pipeline_create(skps_engine* det, skps_engine* kps,
     HALLOC(p->h_scores, sizeof(float) * P * K);
     HALLOC(p->h_det_idx, sizeof(int32_t) * skps_pipeline::RUN_DET);
     HALLOC(p->h_det_rows, sizeof(float) * 16 * skps_pipeline::RUN_DET);
-    HALLOC(p->h_track, sizeof(float) * 4 * 256);
+    HALLOC(p->h_track, sizeof(float) * 4 * p->track_cap);
     SKPS_CUDA(cudaMemset(p->d_det_count, 0, sizeof(int32_t)));
+    int32_t counts[SKPS_LANDMARK_CHUNK + 1];
+    for (int i = 0; i <= SKPS_LANDMARK_CHUNK; ++i) counts[i] = i;
+    SKPS_CUDA(cudaMemcpy(p->d_counts, counts, sizeof(counts), cudaMemcpyHostToDevice));
     *out = p;
     return 0;
 }
@@ -170,7 +181,7 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, const uint8_t* frame
                                  const float* track, int n_track, int32_t* n_faces, float* boxes4, float* kps,
                                  float* scores, int32_t* n_det, int32_t* det_idx, float* det_rows, void* stream) {
     SKPS_CHECK(p && n_faces && boxes4 && kps && scores, "pipeline_run: null argument");
-    SKPS_CHECK(n_track >= 0 && n_track <= 256, "pipeline_run: n_track %d", n_track);
+    SKPS_CHECK(n_track >= 0 && n_track <= p->track_cap, "pipeline_run: n_track %d outside 0..%d", n_track, p->track_cap);
     cudaStream_t s = (cudaStream_t)stream;
     SKPS_CUDA(cudaSetDevice(p->device));
     const skps_pipeline_cfg& c = p->cfg;
@@ -212,17 +223,30 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, const uint8_t* frame
                               (float)(1.0 - (double)c.alpha), c.min_face, K, p->d_boxes, p->d_count, s))
             return 1;
     }
-    uint8_t* kps_in = (uint8_t*)skps_engine_input_ptr(p->kps);
-    if (skps_crop_resize(d_frame, H, W, W * 3, p->d_boxes, p->d_count, K, c.face_scale, c.kps_min_face, kps_in,
-                         p->kps_hw, p->d_detail, s))
-        return 1;
-    if (skps_engine_forward(p->kps, kps_in, K, nullptr, s)) return 1;
-    if (skps_landmark_post(skps_engine_output_ptr(p->kps, 0), p->d_detail, p->d_count, K, P, p->d_kps, s)) return 1;
+    // the face count decides how many crops the landmark net sees
     SKPS_CUDA(cudaMemcpyAsync(&p->h_res->n_faces, p->d_count, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    SKPS_CUDA(cudaMemcpyAsync(p->h_boxes, p->d_boxes, sizeof(float) * 4 * K, cudaMemcpyDeviceToHost, s));
-    SKPS_CUDA(cudaMemcpyAsync(p->h_kps, p->d_kps, sizeof(float) * 2 * P * K, cudaMemcpyDeviceToHost, s));
-    SKPS_CUDA(cudaMemcpyAsync(p->h_scores, skps_engine_output_ptr(p->kps, 1), sizeof(float) * P * K,
-                              cudaMemcpyDeviceToHost, s));
+    SKPS_CUDA(cudaStreamSynchronize(s));
+    const int nf = p->h_res->n_faces;
+    // chunks of exactly the selected faces: the crops go straight into the engine's input, the landmarks and scores of
+    // each chunk to their offsets in d_kps / d_scores (the next chunk overwrites the engine's outputs)
+    uint8_t* kps_in = (uint8_t*)skps_engine_input_ptr(p->kps);
+    for (int f0 = 0; f0 < nf; f0 += SKPS_LANDMARK_CHUNK) {
+        const int nc = nf - f0 < SKPS_LANDMARK_CHUNK ? nf - f0 : SKPS_LANDMARK_CHUNK;
+        const int32_t* d_nc = p->d_counts + nc;
+        if (skps_crop_resize(d_frame, H, W, W * 3, p->d_boxes + 4 * f0, d_nc, nc, c.face_scale, c.kps_min_face, kps_in,
+                             p->kps_hw, p->d_detail + 5 * f0, s))
+            return 1;
+        float* outs[2] = {nullptr, p->d_scores + (size_t)P * f0};
+        if (skps_engine_forward(p->kps, kps_in, nc, outs, s)) return 1;
+        if (skps_landmark_post(skps_engine_output_ptr(p->kps, 0), p->d_detail + 5 * f0, d_nc, nc, P,
+                               p->d_kps + (size_t)2 * P * f0, s))
+            return 1;
+    }
+    if (nf > 0) {
+        SKPS_CUDA(cudaMemcpyAsync(p->h_boxes, p->d_boxes, sizeof(float) * 4 * nf, cudaMemcpyDeviceToHost, s));
+        SKPS_CUDA(cudaMemcpyAsync(p->h_kps, p->d_kps, sizeof(float) * 2 * P * nf, cudaMemcpyDeviceToHost, s));
+        SKPS_CUDA(cudaMemcpyAsync(p->h_scores, p->d_scores, sizeof(float) * P * nf, cudaMemcpyDeviceToHost, s));
+    }
     if (run_detector) SKPS_CUDA(cudaMemcpyAsync(&p->h_res->n_det, p->d_det_count, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     if (run_detector && n_det) {
         // the first RUN_DET kept rows (what callers of this function size their buffers for); the rest stay on the device
@@ -233,7 +257,6 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, const uint8_t* frame
     }
     SKPS_CUDA(cudaStreamSynchronize(s));
     if (run_detector) p->last_n_det = p->h_res->n_det;
-    const int nf = p->h_res->n_faces;
     *n_faces = nf;
     memcpy(boxes4, p->h_boxes, sizeof(float) * 4 * nf);
     memcpy(kps, p->h_kps, sizeof(float) * 2 * P * nf);

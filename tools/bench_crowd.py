@@ -10,9 +10,13 @@
    where it accepts them.
 2. Whole pipeline at det_input=(1152, 1920): FaceAna.run and FaceAnaStreams.run (4 streams) per call on the 384-face crowd,
    the detector running on every call.
-3. With --parent DIR (a built checkout of an earlier commit): tools/bench_streams.py at 1080p_4faces and 4k_16faces and
-   tools/bench_detector.py, alternating this tree and DIR over --rounds rounds, and whether FaceAna / FaceAnaStreams return
-   bit-identical results at the default 384x640 input on the golden frames in both trees.
+   FaceAna.run on the 384-face crowd at top_k 16, 64 and 512, split into the frame-difference gate, the device chain
+   (detector + selection + landmark chunks; skps_pipeline_run), the landmark forwards alone (CUDA events on the landmark
+   engine at the chunk sizes that many faces take) and the host temporal layer (the rest of the call).
+3. With --parent DIR (a built checkout of an earlier commit): tools/bench_streams.py at 1080p_4faces and 4k_16faces,
+   tools/bench_detector.py and FaceAna.run at the default config on the golden frames, alternating this tree and DIR over
+   --rounds rounds, and whether FaceAna / FaceAnaStreams return bit-identical results at the default 384x640 input on the
+   golden frames in both trees.
 The GPU name and power limit are read in the same run.  Nothing is written outside --out."""
 import argparse
 import ctypes as C
@@ -143,6 +147,101 @@ def time_pipeline(torch, iters):
     return res
 
 
+class _TimedLib:
+    """The library with host-clock timers around the two synchronous pipeline calls of FaceAna.run."""
+
+    def __init__(self, lib):
+        self._lib, self.ms = lib, {}
+
+    def __getattr__(self, name):
+        f = getattr(self._lib, name)
+        if name not in ("skps_pipeline_run", "skps_pipeline_frame_diff"):
+            return f
+
+        def timed(*a):
+            import time
+            t = time.perf_counter()
+            rc = f(*a)
+            self.ms[name] = self.ms.get(name, 0.0) + (time.perf_counter() - t) * 1e3
+            return rc
+        return timed
+
+
+def time_crowd_top_k(torch, iters):
+    """FaceAna.run on the 384-face crowd (detector on every call) at several top_k, split by stage."""
+    import time
+    import frames
+    from Skps import FaceAna
+    from peppa_pig_face_landmark_b200 import runtime as rt
+    lib = rt.load_library()
+    fr = frames.multi_face_frame(2160, 3840, (16, 24), 150)
+    out = []
+    for top_k in (16, 64, 512):
+        facer = FaceAna(top_k=top_k, det_input=(1152, 1920))
+        timed = _TimedLib(facer.lib)
+        facer.lib = timed
+        for _ in range(3):
+            facer.reset()
+            n = len(facer.run(fr))
+        reps = max(5, iters // 5)
+        totals = []
+        timed.ms = {}
+        for _ in range(reps):
+            facer.reset()
+            torch.cuda.synchronize()
+            t = time.perf_counter()
+            facer.run(fr)
+            totals.append((time.perf_counter() - t) * 1e3)
+        ms = {k: v / reps for k, v in timed.ms.items()}
+        # the landmark forwards alone: chunks of 64 and the remainder, on the engine FaceAna built
+        eng = facer.face_landmark.model
+        chunk = eng.max_batch
+        sizes = [chunk] * (n // chunk) + ([n % chunk] if n % chunk else [])
+
+        def fwd(s):
+            for b in sizes:
+                rt.check(lib.skps_engine_forward(eng.handle, eng.input_ptr(), b, None, s.cuda_stream))
+        lm = _events(torch, fwd, max(5, iters // 5))
+        totals.sort()
+        out.append({"case": "faceana_crowd384_top_k", "top_k": top_k, "faces": n, "landmark_chunks": len(sizes),
+                    "ms_per_call_median": round(totals[len(totals) // 2], 3),
+                    "ms_per_call_mean": round(sum(totals) / reps, 3),
+                    "ms_frame_diff": round(ms.get("skps_pipeline_frame_diff", 0.0), 3),
+                    "ms_pipeline_run": round(ms.get("skps_pipeline_run", 0.0), 3),
+                    "ms_landmark_forwards": round(lm, 3),
+                    "ms_detector_selection_crops": round(ms.get("skps_pipeline_run", 0.0) - lm, 3),
+                    "ms_host_temporal_and_rest": round(sum(totals) / reps - sum(ms.values()), 3)})
+        del facer
+    return out
+
+
+def time_default(iters):
+    """FaceAna.run per call at the default config (top_k 5, 384x640) on the golden frames: test1.jpg with the detector on
+    every call, and the golden video sequence (detector or tracker path as the frame difference decides)."""
+    import time
+    import torch
+    import frames
+    from golden.make_golden_frames import video_frames
+    from Skps import FaceAna
+    f = FaceAna()
+    t1, v = frames.load_test1(), video_frames()
+    res = {}
+    for what, call, per in (("faceana_default_test1_ms", lambda: (f.reset(), f.run(t1)), 1),
+                            ("faceana_default_video_ms", lambda: [f.run(x) for x in v], len(v))):
+        for _ in range(3):
+            call()
+        ts = []
+        for _ in range(max(10, iters)):
+            torch.cuda.synchronize()
+            t = time.perf_counter()
+            call()
+            torch.cuda.synchronize()
+            ts.append((time.perf_counter() - t) * 1e3 / per)
+        ts.sort()
+        res[what] = round(ts[len(ts) // 2], 4)
+    return res
+
+
 def dump_default(path):
     """FaceAna / FaceAnaStreams at the default detector input on the golden frames, every returned array, into one npz."""
     import numpy as np
@@ -185,14 +284,18 @@ def compare_with_parent(parent, rounds, out_dir):
     import numpy as np
     trees = {"this": ROOT, "parent": os.path.abspath(parent)}
     py = sys.executable
-    res = {k: {"streams": [], "detector": []} for k in trees}
+    res = {k: {"streams": [], "detector": [], "default": []} for k in trees}
     for _ in range(rounds):
         for k, root in trees.items():
             res[k]["streams"] += _run_json([py, "tools/bench_streams.py", "--configs", "1080p_4faces,4k_16faces"], root)
             res[k]["detector"] += _run_json([py, "tools/bench_detector.py"], root)
+            res[k]["default"] += _run_json([py, os.path.abspath(__file__), "--time-default", "--root", root], root)
     summary = {}
     for k in trees:
         by = {}
+        for r in res[k]["default"]:
+            for name, v in r.items():
+                by.setdefault(name, []).append(v)
         for r in res[k]["streams"]:
             if "config" in r and "ms_per_call" in r:
                 by.setdefault(r["config"], []).append(r["ms_per_call"])
@@ -222,10 +325,14 @@ def main():
     ap.add_argument("--out", default=None)
     ap.add_argument("--dump", default=None)
     ap.add_argument("--root", default=ROOT)
+    ap.add_argument("--time-default", action="store_true")
     args = ap.parse_args()
     _paths(args.root)
     if args.dump:
         dump_default(args.dump)
+        return
+    if args.time_default:
+        print(json.dumps(time_default(args.iters)), flush=True)
         return
     import torch
     if not torch.cuda.is_available():
@@ -240,6 +347,8 @@ def main():
     for r in time_nms(torch, args.iters, parent_lib):
         print(json.dumps(r), flush=True)
     print(json.dumps(time_pipeline(torch, args.iters)), flush=True)
+    for r in time_crowd_top_k(torch, args.iters):
+        print(json.dumps(r), flush=True)
     if args.parent:
         out_dir = os.path.abspath(args.out or tempfile.mkdtemp(prefix="bench_crowd_"))
         os.makedirs(out_dir, exist_ok=True)
