@@ -325,7 +325,6 @@ int fpw_prepare(FpwLayer& L, const XfSetup& s) {
     SKPS_CHECK(k.bias, "conv_fpw: zero-bias allocation failed");
     k.res = s.res.base; k.res_fmt = s.res.fmt; k.res_plane = s.res.plane; k.res_ld = s.res.ld; k.res_coff = s.res.c_off;
     k.res_first = s.res.base ? s.res_first : 0;
-    L.valid = true;
     return 0;
 }
 
@@ -359,7 +358,6 @@ Grid fpw_grid(const FpwLayer& L, int batch, int num_sms, FpwK* kp) {
 }
 
 int fpw_launch(const FpwLayer& L, int batch, int num_sms, cudaStream_t stream) {
-    SKPS_CHECK(L.valid, "conv_fpw: layer not prepared");
     FpwK k;
     const int grid = fpw_grid(L, batch, num_sms, &k).ctas;
     if (L.mode == XF_DW) {

@@ -27,7 +27,6 @@ struct FpwLayer {
     FpwK k;
     int mode = 0, n = 0, act = 0, out_fmt = 0;      // n: output channels per work unit (the kernel's N)
     int smem_bytes = 0;
-    bool valid = false;
 };
 
 bool fpw_supported(const XfSetup& s);

@@ -231,7 +231,6 @@ int hm_prepare(HmLayer& L, const TcSetup& s) {
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         SKPS_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(hm W) failed: %d", (int)r);
     }
-    L.valid = true;
     return 0;
 }
 

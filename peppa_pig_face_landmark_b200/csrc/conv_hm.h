@@ -20,7 +20,6 @@ struct HmLayer {
     CUtensorMap x_hi, x_lo, w_hi, w_lo;
     HmK k;
     int smem_bytes = 0;
-    bool valid = false;
 };
 
 constexpr int HM_TILE_PIXELS = 256;

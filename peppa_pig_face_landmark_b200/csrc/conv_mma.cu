@@ -286,7 +286,6 @@ int conv_mma_prepare(ConvMmaLayer& L, const TView& in, const TView& out, const T
     k.res_first = res.base ? res_first : 0;
     L.cin = in.C; L.cout = out.C;
     if ((in.C == 24 ? mma_setup_t<24, 24>(&L.ctas_per_sm) : mma_setup_t<40, 40>(&L.ctas_per_sm))) return 1;
-    L.valid = true;
     return 0;
 }
 

@@ -23,7 +23,6 @@ struct ConvMmaLayer {
     ConvMmaK k;
     int cin, cout;
     int ctas_per_sm = 1;         // resident CTAs of the kernel per SM (occupancy): the grid is num_sms x ctas_per_sm at most
-    bool valid = false;
 };
 
 bool conv_mma_supported(int cin, int cout, int kh, int kw, int stride, int dil, int pad);

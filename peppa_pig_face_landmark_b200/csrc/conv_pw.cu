@@ -287,7 +287,6 @@ int pw_prepare(PwLayer& L, const TcSetup& s) {
                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         SKPS_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(pw B) failed: %d", (int)r);
     }
-    L.valid = true;
     return 0;
 }
 
@@ -340,7 +339,6 @@ Grid pw_grid(const PwLayer& L, int batch, int num_sms, PwK* kp) {
 }
 
 int pw_launch(const PwLayer& L, int batch, int num_sms, cudaStream_t stream) {
-    SKPS_CHECK(L.valid, "conv_pw: layer not prepared");
     EncodeTiledFn enc = tensor_map_encoder();
     SKPS_CHECK(enc, "cuTensorMapEncodeTiled entry point not available");
     const long long rows = L.hw * batch;

@@ -27,7 +27,6 @@ struct PwLayer {                 // prepared once per conv op at engine creation
     void* out = nullptr; long long out_plane = 0; int out_ld = 0, out_coff = 0;
     long long hw = 0;            // pixels per image
     int smem_bytes = 0;
-    bool valid = false;
 };
 
 bool pw_applicable(const TcSetup& s);

@@ -248,7 +248,6 @@ int tct_prepare(TctLayer& L, const TcSetup& s) {
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         SKPS_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(tct out) failed: %d", (int)r);
     }
-    L.valid = true;
     return 0;
 }
 

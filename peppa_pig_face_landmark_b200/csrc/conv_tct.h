@@ -19,7 +19,6 @@ struct TctLayer {
     CUtensorMap x_hi, x_lo, w_hi, w_lo, o_hi, o_lo;
     TctK k;
     int smem_bytes = 0;
-    bool valid = false;
 };
 
 bool tct_applicable(const TcSetup& s);          // s.H, s.W: the (stride-1) map; split-fp16 contiguous output, no residual

@@ -445,7 +445,6 @@ int xf_prepare(XfLayer& L, const XfSetup& s) {
     k.out_cstride = out.c_stride;
     k.res = s.res.base; k.res_fmt = s.res.fmt; k.res_plane = s.res.plane; k.res_ld = s.res.ld; k.res_coff = s.res.c_off;
     k.res_first = s.res.base ? s.res_first : 0;
-    L.valid = true;
     return 0;
 }
 

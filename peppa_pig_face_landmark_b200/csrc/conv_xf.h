@@ -26,7 +26,6 @@ struct XfLayer {
     CUtensorMap src0, src1_hi, src1_lo, b_hi, b_lo, o_hi, o_lo, w_eff;
     XfK k;
     int mode, smem_bytes;
-    bool valid = false;
 };
 
 int xf_prepare(XfLayer& L, const XfSetup& s);

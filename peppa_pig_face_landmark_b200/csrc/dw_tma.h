@@ -20,7 +20,6 @@ struct DwTmaLayer {
     CUtensorMap hi, lo;
     DwTmaK k;
     int k_size, stride, dil, split, chunks, smem_bytes;
-    bool valid = false;
 };
 
 bool dw_tma_supported(const TView& in, const TView& out, int k, int s, int d, int pad);
@@ -36,7 +35,6 @@ struct UpcatTmaLayer {
     DwTmaK k;            // C = channels taken from `low`
     int Hl, Wl, chunks, smem_bytes;
     DwTmaLayer skip;
-    bool valid = false;
 };
 bool upcat_tma_supported(const TView& low, const TView& skip, const TView& out);
 int upcat_tma_prepare(UpcatTmaLayer& L, const TView& low, const TView& skip, const TView& out, const float* w,

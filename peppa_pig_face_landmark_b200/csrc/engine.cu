@@ -8,6 +8,7 @@
 #include <string.h>
 
 #include <map>
+#include <variant>
 #include <vector>
 
 #include "../../include/skps_b200.h"
@@ -37,6 +38,16 @@ const char* get_error() { return g_err; }
 
 using namespace skps;
 
+// The kernel one plan op runs, chosen once at engine creation (prepare_op), and the layer prepared for it.  run_ops,
+// skps_engine_op_kernel, skps_engine_op_grid and skps_engine_launches_for_batch all read this record.  MISC, SIMT_CONV,
+// DW and UPCAT hold no layer: their arguments are built from the OpDesc at every launch, because f32 mode
+// (skps_engine_forward_host_f32) redirects the input buffer then.  STEM_BLOCK holds its dense weights.
+struct OpKernel {
+    int kind = SKPS_KERNEL_MISC;          // SKPS_KERNEL_*
+    std::variant<std::monostate, ConvMmaLayer, TcLayer, TctLayer, PwLayer, HmLayer, XfLayer, FpwLayer, DwTmaLayer,
+                 UpcatTmaLayer, StemBlockW> layer;
+};
+
 struct skps_engine {
     int device = 0, max_batch = 0;
     std::vector<BufDesc> bufs;
@@ -55,15 +66,7 @@ struct skps_engine {
     bool use_graph = true;
     int device_sms = 132;                 // the device's SM count
     int num_sms = 132;                    // SMs the persistent kernels' grids are sized for (skps_engine_set_num_sms)
-    std::vector<TcLayer> tc;              // per op; valid where ops[i].flags & FLAG_TC
-    std::vector<TctLayer> tct;            // per op; valid where the transposed kernel (conv_tct.cu) takes the layer
-    std::vector<PwLayer> pw;              // per op; valid where the pointwise kernel (conv_pw.cu) takes the layer
-    std::vector<HmLayer> hm;              // per op; valid for the heat-map head when its partial rows are 256-pixel tiles
-    std::vector<ConvMmaLayer> mma;        // per op; valid where ops[i].flags & FLAG_MMA
-    std::vector<XfLayer> xf;              // per op; fused producer -> pointwise conv layers (OP_DWPW, OP_CONV with FLAG_XF)
-    std::vector<FpwLayer> fpw;            // per op; valid where the register-accumulator kernel (conv_fpw.cu) takes such a layer
-    std::vector<DwTmaLayer> dwt;          // per op; TMA-staged depthwise layers (valid flag)
-    std::vector<UpcatTmaLayer> upt;       // per op; TMA-staged fused upsample+concat+depthwise
+    std::vector<OpKernel> kern;           // per op
     // streaming host round trip (skps_engine_submit_host_u8): 2 slots, H2D on its own stream
     cudaStream_t s_copy = nullptr, s_compute = nullptr;
     void* d_slot_in[2] = {nullptr, nullptr};
@@ -113,39 +116,27 @@ static StemBlockK stem_params(const skps_engine* e, const OpDesc& op, int batch)
 // Enqueue ops [first,last) for samples [0, batch).
 static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int last = -1) {
     const size_t end = last < 0 ? e->ops.size() : (size_t)last;
+    const int sms = e->num_sms;
     for (size_t i = (size_t)first; i < end; ++i) {
         const OpDesc& op = e->ops[i];
+        const auto& L = e->kern[i].layer;
         TView in0 = resolve(e, op.in[0]), in1 = resolve(e, op.in[1]), in2 = resolve(e, op.in[2]);
         TView out0 = resolve(e, op.out[0]), out1 = resolve(e, op.out[1]);
         const float* w = op.w_off >= 0 ? e->d_weights + op.w_off : nullptr;
         const float* b = op.b_off >= 0 ? e->d_weights + op.b_off : nullptr;
         int rc = 0;
-        switch (op.type) {
-            case OP_CONV: {
-                if (op.flags & FLAG_MMA) {
-                    rc = conv_mma_launch(e->mma[i], batch, e->num_sms, s);
-                    break;
-                }
-                if (op.flags & FLAG_XF) {
-                    rc = e->fpw[i].valid ? fpw_launch(e->fpw[i], batch, e->num_sms, s) : xf_launch(e->xf[i], batch, e->num_sms, s);
-                    break;
-                }
-                if (op.flags & FLAG_TC) {
-                    if (e->hm[i].valid) {
-                        rc = hm_launch(e->hm[i], batch, e->num_sms, s);
-                        break;
-                    }
-                    if (e->tct[i].valid) {
-                        rc = tct_launch(e->tct[i], batch, e->num_sms, s);
-                        break;
-                    }
-                    if (e->pw[i].valid) {
-                        rc = pw_launch(e->pw[i], batch, e->num_sms, s);
-                        break;
-                    }
-                    rc = tc_launch(e->tc[i], batch, e->num_sms, s);
-                    break;
-                }
+        switch (e->kern[i].kind) {
+            case SKPS_KERNEL_MMA: rc = conv_mma_launch(std::get<ConvMmaLayer>(L), batch, sms, s); break;
+            case SKPS_KERNEL_TC: rc = tc_launch(std::get<TcLayer>(L), batch, sms, s); break;
+            case SKPS_KERNEL_TCT: rc = tct_launch(std::get<TctLayer>(L), batch, sms, s); break;
+            case SKPS_KERNEL_PW: rc = pw_launch(std::get<PwLayer>(L), batch, sms, s); break;
+            case SKPS_KERNEL_HM: rc = hm_launch(std::get<HmLayer>(L), batch, sms, s); break;
+            case SKPS_KERNEL_XF: rc = xf_launch(std::get<XfLayer>(L), batch, sms, s); break;
+            case SKPS_KERNEL_FPW: rc = fpw_launch(std::get<FpwLayer>(L), batch, sms, s); break;
+            case SKPS_KERNEL_DW_TMA: rc = dw_tma_launch(std::get<DwTmaLayer>(L), batch, s); break;
+            case SKPS_KERNEL_UPCAT_TMA: rc = upcat_tma_launch(std::get<UpcatTmaLayer>(L), batch, s); break;
+            case SKPS_KERNEL_STEM_BLOCK: rc = stem_block_launch(stem_params(e, op, batch), std::get<StemBlockW>(L), sms, s); break;
+            case SKPS_KERNEL_SIMT_CONV: {
                 ConvArgs a;
                 a.in = in0; a.res = in1; a.gate = in2; a.out = out0; a.w = w; a.bias = b;
                 a.kh = op.kh; a.kw = op.kw; a.sh = op.sh; a.sw = op.sw; a.ph = op.ph; a.pw = op.pw;
@@ -157,11 +148,7 @@ static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int
                 rc = launch_conv(a, s);
                 break;
             }
-            case OP_DWCONV: {
-                if (e->dwt[i].valid) {
-                    rc = dw_tma_launch(e->dwt[i], batch, s);
-                    break;
-                }
+            case SKPS_KERNEL_DW: {
                 DwArgs a;
                 a.in = in0; a.out = out0; a.w = w; a.bias = b;
                 a.kh = op.kh; a.kw = op.kw; a.sh = op.sh; a.sw = op.sw; a.ph = op.ph; a.pw = op.pw;
@@ -169,60 +156,45 @@ static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int
                 rc = launch_dwconv(a, s);
                 break;
             }
-            case OP_DWPW:
-                rc = e->fpw[i].valid ? fpw_launch(e->fpw[i], batch, e->num_sms, s) : xf_launch(e->xf[i], batch, e->num_sms, s);
-                break;
-            case OP_STEM_BLOCK: {
-                // w = StemBlockW as packed by lowering (dense weights -> kernel-parameter bank); i[0] -> [9][E]+[E] depthwise table
-                StemBlockW W;
-                memcpy(&W, e->h_weights.data() + op.w_off, sizeof(W));
-                const StemBlockK k = stem_params(e, op, batch);
-                if (in0.fmt != DT_U8 || !stem_block_supported(in0.H, in0.W, out0.C, out0)) {
-                    set_error("stem block: unsupported shape");
-                    rc = 1;
-                    break;
+            case SKPS_KERNEL_UPCAT: rc = launch_upcat_dw(in0, in1, out0, w, b, op.act, batch, s); break;
+            default:                                   // SKPS_KERNEL_MISC
+                switch (op.type) {
+                    case OP_MAXPOOL2: rc = launch_maxpool2(in0, out0, batch, s); break;
+                    case OP_RESIZE_NEAREST: rc = launch_resize_nearest(in0, out0, batch, s); break;
+                    case OP_UPSAMPLE_BILINEAR2X: rc = launch_bilinear2x(in0, out0, batch, s); break;
+                    case OP_COPY: rc = launch_copy(in0, out0, batch, s); break;
+                    case OP_GAP: rc = launch_gap(in0, out0, batch, s); break;
+                    case OP_AFFINE_ACT: rc = launch_affine_act(in0, out0, w, b, op.act, batch, s); break;
+                    case OP_SCSE: rc = launch_scse(in0, in1, in2, out0, batch, s); break;
+                    case OP_SCALE_CH: rc = launch_scale_ch(in0, in1, out0, batch, s); break;
+                    case OP_GAP_SSE:
+                        rc = launch_gap_sse(in0, out0, out1, w, op.b_off >= 0 ? e->h_weights[op.b_off] : 0.f, op.act, batch, s);
+                        break;
+                    case OP_SE_FC:
+                        // in0 = per-tile channel sums [n][tiles][C]; w = W1^T [C][Cr], i[0] -> W2^T [Cr][C]; b = [b1 (Cr) | b2 (C)]
+                        rc = launch_se_fc(in0, out0, w, b, e->d_weights + op.i[0], b + op.i[1], op.i[1], op.act, op.i[2],
+                                          op.i[3], batch, s);
+                        break;
+                    case OP_ADDN: {
+                        TView ins[4] = {in0, in1, in2, resolve(e, op.in3)};
+                        int n_in = 0;
+                        while (n_in < 4 && ins[n_in].base) ++n_in;
+                        rc = launch_addn(ins, n_in, out0, op.act, batch, s);
+                        break;
+                    }
+                    case OP_DET_DECODE: {
+                        TView heads[3] = {in0, in1, in2};
+                        rc = launch_det_decode(heads, e->h_weights.data() + op.w_off, out0, op.i[0], batch, s);
+                        break;
+                    }
+                    case OP_HM_DECODE: {
+                        TView part = in2;                  // FLAG_HM_PART: per-tile (max, arg-max) rows from the head conv
+                        rc = launch_hm_decode(in0, in1, w, b, out0, out1, op.i[0], batch, s,
+                                              (op.flags & FLAG_HM_PART) ? &part : nullptr);
+                        break;
+                    }
+                    default: set_error("engine: unknown op type %d (op %zu)", op.type, i); return 1;
                 }
-                rc = stem_block_launch(k, W, e->num_sms, s);
-                break;
-            }
-            case OP_MAXPOOL2: rc = launch_maxpool2(in0, out0, batch, s); break;
-            case OP_RESIZE_NEAREST: rc = launch_resize_nearest(in0, out0, batch, s); break;
-            case OP_UPSAMPLE_BILINEAR2X: rc = launch_bilinear2x(in0, out0, batch, s); break;
-            case OP_COPY: rc = launch_copy(in0, out0, batch, s); break;
-            case OP_GAP: rc = launch_gap(in0, out0, batch, s); break;
-            case OP_AFFINE_ACT: rc = launch_affine_act(in0, out0, w, b, op.act, batch, s); break;
-            case OP_SCSE: rc = launch_scse(in0, in1, in2, out0, batch, s); break;
-            case OP_SCALE_CH: rc = launch_scale_ch(in0, in1, out0, batch, s); break;
-            case OP_GAP_SSE:
-                rc = launch_gap_sse(in0, out0, out1, w, op.b_off >= 0 ? e->h_weights[op.b_off] : 0.f, op.act, batch, s);
-                break;
-            case OP_SE_FC:
-                // in0 = per-tile channel sums [n][tiles][C]; w = W1^T [C][Cr], i[0] -> W2^T [Cr][C]; b = [b1 (Cr) | b2 (C)]
-                rc = launch_se_fc(in0, out0, w, b, e->d_weights + op.i[0], b + op.i[1], op.i[1], op.act, op.i[2], op.i[3],
-                                  batch, s);
-                break;
-            case OP_ADDN: {
-                TView ins[4] = {in0, in1, in2, resolve(e, op.in3)};
-                int n_in = 0;
-                while (n_in < 4 && ins[n_in].base) ++n_in;
-                rc = launch_addn(ins, n_in, out0, op.act, batch, s);
-                break;
-            }
-            case OP_UPCAT_DW:
-                rc = e->upt[i].valid ? upcat_tma_launch(e->upt[i], batch, s)
-                                     : launch_upcat_dw(in0, in1, out0, w, b, op.act, batch, s);
-                break;
-            case OP_DET_DECODE: {
-                TView heads[3] = {in0, in1, in2};
-                rc = launch_det_decode(heads, e->h_weights.data() + op.w_off, out0, op.i[0], batch, s);
-                break;
-            }
-            case OP_HM_DECODE: {
-                TView part = in2;                          // FLAG_HM_PART: per-tile (max, arg-max) rows from the head conv
-                rc = launch_hm_decode(in0, in1, w, b, out0, out1, op.i[0], batch, s, (op.flags & FLAG_HM_PART) ? &part : nullptr);
-                break;
-            }
-            default: set_error("engine: unknown op type %d (op %zu)", op.type, i); return 1;
         }
         if (rc) {
             char tmp[900];
@@ -236,6 +208,151 @@ static int run_ops(skps_engine* e, int batch, cudaStream_t s, int first = 0, int
 
 extern "C" SKPS_API const char* skps_last_error(void) { return get_error(); }
 extern "C" SKPS_API int skps_version(void) { return 1; }
+
+// A tensor-core conv op as conv_tc, conv_tct, conv_pw and conv_hm prepare it.
+static TcSetup tc_setup(const skps_engine* e, const OpDesc& op) {
+    const TView in0 = resolve(e, op.in[0]), res = resolve(e, op.in[1]), out0 = resolve(e, op.out[0]);
+    TcSetup s = {};
+    s.H = in0.H; s.W = in0.W; s.Cin = in0.C; s.in_ld = in0.ld; s.in_coff = in0.c_off; s.max_batch = e->max_batch;
+    s.in_base = in0.base; s.in_plane = in0.plane;
+    s.kh = op.kh; s.kw = op.kw; s.dil = op.dh; s.pad = op.ph; s.stride = op.sh;
+    s.Cout = out0.C; s.act = op.act; s.n_tile = op.i[0]; s.n_tiles = op.i[1]; s.out_scale = op.f[0];
+    s.w_hi = e->d_weights + op.w_off; s.w_lo = e->d_weights + op.i[2];
+    s.bias = op.b_off >= 0 ? e->d_weights + op.b_off : nullptr;
+    s.out = out0.base; s.out_fmt = out0.fmt; s.out_plane = out0.plane; s.out_ld = out0.ld; s.out_coff = out0.c_off;
+    s.out_cstride = out0.c_stride;
+    s.res = res.base; s.res_fmt = res.fmt; s.res_plane = res.plane; s.res_ld = res.ld; s.res_coff = res.c_off;
+    s.res_first = (op.flags & FLAG_RES_FIRST) ? 1 : 0;
+    if (op.flags & FLAG_HM_PART) {
+        // out[1] = [tiles][2 * ld] per sample: ld maxima then ld arg-max indices; the map itself is not stored
+        TView part = resolve(e, op.out[1]);
+        s.hm_val = (float*)part.base; s.hm_idx = (int*)part.base + part.ld / 2; s.hm_ld = part.ld;
+    }
+    return s;
+}
+
+// A fused producer -> pointwise conv op (OP_DWPW: depthwise / up-sample+concat+depthwise; OP_CONV: squeeze-excite
+// scale) as conv_fpw and conv_xf prepare it.
+static XfSetup xf_setup(const skps_engine* e, const OpDesc& op) {
+    const bool dwpw = op.type == OP_DWPW;
+    XfSetup s;
+    memset(&s, 0, sizeof(s));
+    s.mode = dwpw ? XF_DW : XF_SCALE;
+    s.max_batch = e->max_batch;
+    s.x = resolve(e, op.in[0]);
+    s.res = resolve(e, op.in[1]);
+    if (dwpw) {
+        s.low = resolve(e, op.in[2]);
+        s.dww = e->d_weights + op.i[3];
+        s.dw_act = (int)op.f[1];
+        s.weff = s.low.base ? e->d_weights + op.i2[0] : nullptr;
+    } else {
+        s.gate = resolve(e, op.in[2]);
+    }
+    s.out = resolve(e, op.out[0]);
+    s.Cout = s.out.C; s.act = op.act; s.n_tile = op.i[0]; s.n_tiles = op.i[1]; s.out_scale = op.f[0];
+    s.w_hi = e->d_weights + op.w_off; s.w_lo = e->d_weights + op.i[2];
+    s.bias = op.b_off >= 0 ? e->d_weights + op.b_off : nullptr;
+    s.res_first = (op.flags & FLAG_RES_FIRST) ? 1 : 0;
+    return s;
+}
+
+// Chooses the kernel op i runs and prepares its layer (TMA descriptors over the fixed activation buffers and weights).
+// Returns null, or the name of the kernel whose preparation failed with the error naming the op.
+static const char* prepare_op(skps_engine* e, int i) {
+    const OpDesc& op = e->ops[i];
+    OpKernel& k = e->kern[i];
+    auto failed = [&](const char* what) {
+        char tmp[900];
+        snprintf(tmp, sizeof(tmp), "%s", get_error());
+        set_error("op %d: %s", i, tmp);
+        return what;
+    };
+    const TView in0 = resolve(e, op.in[0]), in1 = resolve(e, op.in[1]);
+    const TView out0 = resolve(e, op.out[0]), out1 = resolve(e, op.out[1]);
+    if (op.type == OP_CONV && (op.flags & FLAG_MMA)) {
+        k.kind = SKPS_KERNEL_MMA;
+        if (!conv_mma_supported(in0.C, out0.C, op.kh, op.kw, op.sh, op.dh, op.ph) ||
+            conv_mma_prepare(k.layer.emplace<ConvMmaLayer>(), in0, out0, in1, (op.flags & FLAG_RES_FIRST) ? 1 : 0,
+                             e->d_weights + op.w_off, op.b_off >= 0 ? e->d_weights + op.b_off : nullptr, op.f[0],
+                             op.act, e->max_batch))
+            return failed("mma");
+        return nullptr;
+    }
+    // conv_fpw where it takes the layer (whole 16 x 8 tiles, unit-stride aligned output, instantiated width), else conv_xf
+    if (op.type == OP_DWPW || (op.type == OP_CONV && (op.flags & FLAG_XF))) {
+        const XfSetup s = xf_setup(e, op);
+        if (fpw_supported(s)) {
+            k.kind = SKPS_KERNEL_FPW;
+            return fpw_prepare(k.layer.emplace<FpwLayer>(), s) ? failed("fpw") : nullptr;
+        }
+        k.kind = SKPS_KERNEL_XF;
+        return xf_prepare(k.layer.emplace<XfLayer>(), s) ? failed("xf") : nullptr;
+    }
+    if (op.type == OP_CONV && (op.flags & FLAG_TC)) {
+        if (in0.fmt != DT_SPLIT16 || in0.c_stride != 1 || op.in[2].buf >= 0 || op.sh != op.sw) {
+            set_error("op %d: tensor-core conv needs a SPLIT16 unit-stride input and no gate", i);
+            return "tc";
+        }
+        const TcSetup s = tc_setup(e, op);
+        // the lowering sizes the partial buffer for 128-pixel tiles (conv_tc epilogue) or 256-pixel tiles (conv_hm.cu)
+        if ((op.flags & FLAG_HM_PART) && out1.H * out1.W > 0 && out0.H * out0.W / (out1.H * out1.W) == HM_TILE_PIXELS) {
+            k.kind = SKPS_KERNEL_HM;
+            return hm_prepare(k.layer.emplace<HmLayer>(), s) ? failed("hm") : nullptr;
+        }
+        if (op.dh == op.dw && op.ph == op.pw && tct_applicable(s)) {
+            k.kind = SKPS_KERNEL_TCT;
+            return tct_prepare(k.layer.emplace<TctLayer>(), s) ? failed("tct") : nullptr;
+        }
+        if (op.ph == op.pw && pw_applicable(s)) {
+            k.kind = SKPS_KERNEL_PW;
+            return pw_prepare(k.layer.emplace<PwLayer>(), s) ? failed("pw") : nullptr;
+        }
+        k.kind = SKPS_KERNEL_TC;
+        return op.dh != op.dw || op.ph != op.pw || tc_prepare(k.layer.emplace<TcLayer>(), s) ? failed("tc") : nullptr;
+    }
+    if (op.type == OP_CONV) {
+        k.kind = SKPS_KERNEL_SIMT_CONV;
+        return nullptr;
+    }
+    if (op.type == OP_DWCONV) {
+        if (op.kh == op.kw && op.sh == op.sw && op.dh == op.dw && op.ph == op.pw &&
+            dw_tma_supported(in0, out0, op.kh, op.sh, op.dh, op.ph)) {
+            k.kind = SKPS_KERNEL_DW_TMA;
+            // FLAG_GAP_PARTIAL: out[1] = per-tile channel sums for the squeeze-excite gate
+            return dw_tma_prepare(k.layer.emplace<DwTmaLayer>(), in0, out0, e->d_weights + op.w_off,
+                                  e->d_weights + op.b_off, op.kh, op.sh, op.dh, op.ph, op.act, e->max_batch,
+                                  (op.flags & FLAG_GAP_PARTIAL) ? &out1 : nullptr) ? failed("dw_tma") : nullptr;
+        }
+        if (op.flags & FLAG_GAP_PARTIAL) {
+            set_error("op %d: per-tile channel sums need the TMA depthwise kernel (unsupported layer)", i);
+            return "dw_tma";
+        }
+        k.kind = SKPS_KERNEL_DW;
+        return nullptr;
+    }
+    if (op.type == OP_UPCAT_DW) {              // in[0] = the low-resolution map, in[1] = the skip connection
+        if (!upcat_tma_supported(in0, in1, out0)) {
+            k.kind = SKPS_KERNEL_UPCAT;
+            return nullptr;
+        }
+        k.kind = SKPS_KERNEL_UPCAT_TMA;
+        return upcat_tma_prepare(k.layer.emplace<UpcatTmaLayer>(), in0, in1, out0, e->d_weights + op.w_off,
+                                 e->d_weights + op.b_off, op.act, e->max_batch) ? failed("upcat_tma") : nullptr;
+    }
+    if (op.type == OP_STEM_BLOCK) {
+        if (in0.fmt != DT_U8 || !stem_block_supported(in0.H, in0.W, out0.C, out0)) {
+            set_error("op %d: stem block: unsupported shape", i);
+            return "stem_block";
+        }
+        k.kind = SKPS_KERNEL_STEM_BLOCK;
+        // w = StemBlockW as packed by lowering (dense weights -> kernel-parameter bank); i[0] -> [9][E]+[E] depthwise table
+        memcpy(&k.layer.emplace<StemBlockW>(), e->h_weights.data() + op.w_off, sizeof(StemBlockW));
+        return nullptr;
+    }
+    k.kind = SKPS_KERNEL_MISC;
+    return nullptr;
+}
 
 extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words, const float* weights, size_t n_floats,
                                   int max_batch, int device, skps_engine** out) {
@@ -263,12 +380,6 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
         set_error("engine_create: %s: %s", what, tmp);
         skps_engine_destroy(e);
         return 1;
-    };
-    auto fail_op = [&](int i, const char* what) {
-        char tmp[900];
-        snprintf(tmp, sizeof(tmp), "%s", get_error());
-        set_error("op %d: %s", i, tmp);
-        return fail(what);
     };
     if (cudaMalloc(&e->d_weights, n_floats * sizeof(float)) != cudaSuccess) { set_error("cudaMalloc weights"); return fail("alloc"); }
     if (cudaMemcpy(e->d_weights, weights, n_floats * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
@@ -300,123 +411,9 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
     }
     cudaDeviceGetAttribute(&e->device_sms, cudaDevAttrMultiProcessorCount, device);
     e->num_sms = e->device_sms;
-    // tensor-core conv layers: TMA descriptors over the (fixed) activation buffers and weight matrices
-    e->mma.resize(n_ops);
-    for (int i = 0; i < n_ops; ++i) {
-        const OpDesc& op = e->ops[i];
-        if (op.type != OP_CONV || !(op.flags & FLAG_MMA)) continue;
-        TView in0 = resolve(e, op.in[0]), res = resolve(e, op.in[1]), out0 = resolve(e, op.out[0]);
-        if (!conv_mma_supported(in0.C, out0.C, op.kh, op.kw, op.sh, op.dh, op.ph) ||
-            conv_mma_prepare(e->mma[i], in0, out0, res, (op.flags & FLAG_RES_FIRST) ? 1 : 0, e->d_weights + op.w_off,
-                             op.b_off >= 0 ? e->d_weights + op.b_off : nullptr, op.f[0], op.act, max_batch))
-            return fail_op(i, "mma");
-    }
-    e->tc.resize(n_ops);
-    e->hm.resize(n_ops);
-    e->tct.resize(n_ops);
-    e->pw.resize(n_ops);
-    for (int i = 0; i < n_ops; ++i) {
-        const OpDesc& op = e->ops[i];
-        if (op.type != OP_CONV || !(op.flags & FLAG_TC) || (op.flags & FLAG_XF)) continue;
-        TView in0 = resolve(e, op.in[0]), res = resolve(e, op.in[1]), out0 = resolve(e, op.out[0]);
-        if (in0.fmt != DT_SPLIT16 || in0.c_stride != 1 || op.in[2].buf >= 0 || op.sh != op.sw) {
-            set_error("op %d: tensor-core conv needs a SPLIT16 unit-stride input and no gate", i);
-            return fail("tc");
-        }
-        TcSetup s = {};
-        s.H = in0.H; s.W = in0.W; s.Cin = in0.C; s.in_ld = in0.ld; s.in_coff = in0.c_off; s.max_batch = max_batch;
-        s.in_base = in0.base; s.in_plane = in0.plane;
-        s.kh = op.kh; s.kw = op.kw; s.dil = op.dh; s.pad = op.ph; s.stride = op.sh;
-        s.Cout = out0.C; s.act = op.act; s.n_tile = op.i[0]; s.n_tiles = op.i[1]; s.out_scale = op.f[0];
-        s.w_hi = e->d_weights + op.w_off; s.w_lo = e->d_weights + op.i[2];
-        s.bias = op.b_off >= 0 ? e->d_weights + op.b_off : nullptr;
-        s.out = out0.base; s.out_fmt = out0.fmt; s.out_plane = out0.plane; s.out_ld = out0.ld; s.out_coff = out0.c_off;
-        s.out_cstride = out0.c_stride;
-        s.res = res.base; s.res_fmt = res.fmt; s.res_plane = res.plane; s.res_ld = res.ld; s.res_coff = res.c_off;
-        s.res_first = (op.flags & FLAG_RES_FIRST) ? 1 : 0;
-        if (op.flags & FLAG_HM_PART) {
-            // out[1] = [tiles][2 * ld] per sample: ld maxima then ld arg-max indices; the map itself is not stored
-            TView part = resolve(e, op.out[1]);
-            s.hm_val = (float*)part.base; s.hm_idx = (int*)part.base + part.ld / 2; s.hm_ld = part.ld;
-            // the lowering sizes the partial buffer for 128-pixel tiles (conv_tc epilogue) or 256-pixel tiles (conv_hm.cu)
-            const int tile_px = part.H * part.W > 0 ? out0.H * out0.W / (part.H * part.W) : 0;
-            if (tile_px == HM_TILE_PIXELS) {
-                if (hm_prepare(e->hm[i], s)) return fail_op(i, "hm");
-                continue;
-            }
-        }
-        if (op.dh == op.dw && op.ph == op.pw && tct_applicable(s)) {
-            if (tct_prepare(e->tct[i], s)) return fail_op(i, "tct");
-            continue;
-        }
-        if (op.ph == op.pw && pw_applicable(s)) {
-            if (pw_prepare(e->pw[i], s)) return fail_op(i, "pw");
-            continue;
-        }
-        if (op.dh != op.dw || op.ph != op.pw || tc_prepare(e->tc[i], s)) return fail_op(i, "tc");
-    }
-    // fused producer -> pointwise conv layers: depthwise / up-sample+concat+depthwise / squeeze-excite scale, on conv_fpw.cu
-    // where it takes the layer (whole 16 x 8 tiles, unit-stride aligned output, instantiated width), else on conv_xf.cu
-    e->xf.resize(n_ops);
-    e->fpw.resize(n_ops);
-    for (int i = 0; i < n_ops; ++i) {
-        const OpDesc& op = e->ops[i];
-        const bool dwpw = op.type == OP_DWPW, scale = op.type == OP_CONV && (op.flags & FLAG_XF);
-        if (!dwpw && !scale) continue;
-        XfSetup s;
-        memset(&s, 0, sizeof(s));
-        s.mode = dwpw ? XF_DW : XF_SCALE;
-        s.max_batch = max_batch;
-        s.x = resolve(e, op.in[0]);
-        s.res = resolve(e, op.in[1]);
-        if (dwpw) {
-            s.low = resolve(e, op.in[2]);
-            s.dww = e->d_weights + op.i[3];
-            s.dw_act = (int)op.f[1];
-            s.weff = s.low.base ? e->d_weights + op.i2[0] : nullptr;
-        } else {
-            s.gate = resolve(e, op.in[2]);
-        }
-        s.out = resolve(e, op.out[0]);
-        s.Cout = s.out.C; s.act = op.act; s.n_tile = op.i[0]; s.n_tiles = op.i[1]; s.out_scale = op.f[0];
-        s.w_hi = e->d_weights + op.w_off; s.w_lo = e->d_weights + op.i[2];
-        s.bias = op.b_off >= 0 ? e->d_weights + op.b_off : nullptr;
-        s.res_first = (op.flags & FLAG_RES_FIRST) ? 1 : 0;
-        if (fpw_supported(s)) {
-            if (fpw_prepare(e->fpw[i], s)) return fail_op(i, "fpw");
-            continue;
-        }
-        if (xf_prepare(e->xf[i], s)) return fail_op(i, "xf");
-    }
-    // depthwise layers: TMA descriptors over the input views
-    e->dwt.resize(n_ops);
-    e->upt.resize(n_ops);
-    for (int i = 0; i < n_ops; ++i) {
-        const OpDesc& op = e->ops[i];
-        if (op.type == OP_UPCAT_DW) {
-            TView low = resolve(e, op.in[0]), skip = resolve(e, op.in[1]), out0 = resolve(e, op.out[0]);
-            if (!upcat_tma_supported(low, skip, out0)) continue;
-            if (upcat_tma_prepare(e->upt[i], low, skip, out0, e->d_weights + op.w_off, e->d_weights + op.b_off, op.act,
-                                  max_batch))
-                return fail_op(i, "upcat_tma");
-            e->upt[i].valid = true;
-            continue;
-        }
-        if (op.type != OP_DWCONV || op.kh != op.kw || op.sh != op.sw || op.dh != op.dw || op.ph != op.pw) continue;
-        TView in0 = resolve(e, op.in[0]), out0 = resolve(e, op.out[0]);
-        if (!dw_tma_supported(in0, out0, op.kh, op.sh, op.dh, op.ph)) continue;
-        TView part = resolve(e, op.out[1]);          // FLAG_GAP_PARTIAL: per-tile channel sums for the squeeze-excite gate
-        if (dw_tma_prepare(e->dwt[i], in0, out0, e->d_weights + op.w_off, e->d_weights + op.b_off, op.kh, op.sh, op.dh,
-                           op.ph, op.act, max_batch, (op.flags & FLAG_GAP_PARTIAL) ? &part : nullptr))
-            return fail_op(i, "dw_tma");
-        e->dwt[i].valid = true;
-    }
-    for (int i = 0; i < n_ops; ++i) {
-        if (e->ops[i].type == OP_DWCONV && (e->ops[i].flags & FLAG_GAP_PARTIAL) && !e->dwt[i].valid) {
-            set_error("op %d: per-tile channel sums need the TMA depthwise kernel (unsupported layer)", i);
-            return fail("dw_tma");
-        }
-    }
+    e->kern.resize(n_ops);
+    for (int i = 0; i < n_ops; ++i)
+        if (const char* what = prepare_op(e, i)) return fail(what);
     *out = e;
     return 0;
 }
@@ -490,8 +487,8 @@ extern "C" SKPS_API int skps_engine_launches_per_forward(const skps_engine* e) {
 extern "C" SKPS_API int skps_engine_launches_for_batch(const skps_engine* e, int batch) {
     if (!e || batch <= 0) return 0;
     int n = 0;
-    for (size_t i = 0; i < e->ops.size(); ++i)      // the TMA fused-upsample op is two kernels (up-sampled part + skip part)
-        n += (e->ops[i].type == OP_UPCAT_DW && e->upt[i].valid) ? 2 : 1;
+    for (const OpKernel& k : e->kern)      // the TMA fused-upsample op is two kernels (up-sampled part + skip part)
+        n += k.kind == SKPS_KERNEL_UPCAT_TMA ? 2 : 1;
     return n;
 }
 
@@ -508,45 +505,31 @@ extern "C" SKPS_API int skps_engine_op_kernel(const skps_engine* e, int op_index
     int32_t tmp[4];
     int32_t* inf = info ? info : tmp;
     inf[0] = inf[1] = inf[2] = inf[3] = 0;
-    const size_t i = (size_t)op_index;
-    const OpDesc& op = e->ops[i];
-    switch (op.type) {
-        case OP_CONV:
-            if (op.flags & FLAG_MMA) return SKPS_KERNEL_MMA;
-            if (op.flags & FLAG_XF) {
-                if (!e->fpw[i].valid) return SKPS_KERNEL_XF;
-                inf[0] = 128; inf[1] = e->fpw[i].n; inf[2] = e->fpw[i].k.nsplit; inf[3] = e->fpw[i].mode;
-                return SKPS_KERNEL_FPW;
-            }
-            if (op.flags & FLAG_TC) {
-                if (e->hm[i].valid) return SKPS_KERNEL_HM;
-                if (e->tct[i].valid) {
-                    inf[0] = e->tct[i].k.bh;
-                    return SKPS_KERNEL_TCT;
-                }
-                if (e->pw[i].valid) {
-                    inf[0] = e->pw[i].nc; inf[1] = e->pw[i].k.n_chunks;
-                    return SKPS_KERNEL_PW;
-                }
-                const TcK& k = e->tc[i].k;
-                inf[0] = k.bw; inf[1] = k.bh; inf[2] = k.ipt; inf[3] = k.mt;
-                return SKPS_KERNEL_TC;
-            }
-            return SKPS_KERNEL_SIMT_CONV;
-        case OP_DWCONV:
-            if (e->dwt[i].valid) {
-                inf[0] = dw_tile_rows(e->dwt[i].k_size, e->dwt[i].stride);
-                return SKPS_KERNEL_DW_TMA;
-            }
-            return SKPS_KERNEL_DW;
-        case OP_DWPW:
-            if (!e->fpw[i].valid) return SKPS_KERNEL_XF;
-            inf[0] = 128; inf[1] = e->fpw[i].n; inf[2] = e->fpw[i].k.nsplit; inf[3] = e->fpw[i].mode;
-            return SKPS_KERNEL_FPW;
-        case OP_UPCAT_DW: return e->upt[i].valid ? SKPS_KERNEL_UPCAT_TMA : SKPS_KERNEL_UPCAT;
-        case OP_STEM_BLOCK: return SKPS_KERNEL_STEM_BLOCK;
-        default: return SKPS_KERNEL_MISC;
+    const OpKernel& k = e->kern[op_index];
+    switch (k.kind) {
+        case SKPS_KERNEL_TC: {
+            const TcK& t = std::get<TcLayer>(k.layer).k;
+            inf[0] = t.bw; inf[1] = t.bh; inf[2] = t.ipt; inf[3] = t.mt;
+            break;
+        }
+        case SKPS_KERNEL_TCT: inf[0] = std::get<TctLayer>(k.layer).k.bh; break;
+        case SKPS_KERNEL_PW: {
+            const PwLayer& L = std::get<PwLayer>(k.layer);
+            inf[0] = L.nc; inf[1] = L.k.n_chunks;
+            break;
+        }
+        case SKPS_KERNEL_FPW: {
+            const FpwLayer& L = std::get<FpwLayer>(k.layer);
+            inf[0] = 128; inf[1] = L.n; inf[2] = L.k.nsplit; inf[3] = L.mode;
+            break;
+        }
+        case SKPS_KERNEL_DW_TMA: {
+            const DwTmaLayer& L = std::get<DwTmaLayer>(k.layer);
+            inf[0] = dw_tile_rows(L.k_size, L.stride);
+            break;
+        }
     }
+    return k.kind;
 }
 
 extern "C" SKPS_API int skps_engine_set_num_sms(skps_engine* e, int n) {
@@ -564,21 +547,18 @@ extern "C" SKPS_API int skps_engine_set_num_sms(skps_engine* e, int n) {
 extern "C" SKPS_API int skps_engine_op_grid(const skps_engine* e, int op_index, int batch, int32_t out[2]) {
     SKPS_CHECK(e && out && op_index >= 0 && op_index < (int)e->ops.size(), "op_grid: bad arguments");
     SKPS_CHECK(batch > 0 && batch <= e->max_batch, "op_grid: batch %d outside 1..%d", batch, e->max_batch);
-    const size_t i = (size_t)op_index;
-    const OpDesc& op = e->ops[i];
+    const OpKernel& k = e->kern[op_index];
     const int sms = e->num_sms;
     Grid g = {0, 0};
-    if (op.type == OP_CONV && (op.flags & FLAG_MMA)) {
-        g = conv_mma_grid(e->mma[i], batch, sms);
-    } else if (op.type == OP_DWPW || (op.type == OP_CONV && (op.flags & FLAG_XF))) {
-        g = e->fpw[i].valid ? fpw_grid(e->fpw[i], batch, sms) : xf_grid(e->xf[i], batch, sms);
-    } else if (op.type == OP_CONV && (op.flags & FLAG_TC)) {
-        g = e->hm[i].valid ? hm_grid(e->hm[i], batch, sms)
-            : e->tct[i].valid ? tct_grid(e->tct[i], batch, sms)
-            : e->pw[i].valid ? pw_grid(e->pw[i], batch, sms)
-            : tc_grid(e->tc[i], batch, sms);
-    } else if (op.type == OP_STEM_BLOCK) {
-        g = stem_block_grid(stem_params(e, op, batch), sms);
+    switch (k.kind) {
+        case SKPS_KERNEL_MMA: g = conv_mma_grid(std::get<ConvMmaLayer>(k.layer), batch, sms); break;
+        case SKPS_KERNEL_TC: g = tc_grid(std::get<TcLayer>(k.layer), batch, sms); break;
+        case SKPS_KERNEL_TCT: g = tct_grid(std::get<TctLayer>(k.layer), batch, sms); break;
+        case SKPS_KERNEL_PW: g = pw_grid(std::get<PwLayer>(k.layer), batch, sms); break;
+        case SKPS_KERNEL_HM: g = hm_grid(std::get<HmLayer>(k.layer), batch, sms); break;
+        case SKPS_KERNEL_XF: g = xf_grid(std::get<XfLayer>(k.layer), batch, sms); break;
+        case SKPS_KERNEL_FPW: g = fpw_grid(std::get<FpwLayer>(k.layer), batch, sms); break;
+        case SKPS_KERNEL_STEM_BLOCK: g = stem_block_grid(stem_params(e, e->ops[op_index], batch), sms); break;
     }
     out[0] = g.ctas;
     out[1] = g.units;
