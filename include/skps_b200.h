@@ -240,6 +240,13 @@ SKPS_API int skps_landmark_post(const float* xy_norm, const int32_t* detail, con
 /* FaceAna.diff_frames (facer.py:98-118): sum |a-b| over n bytes into *sum [dev] (uint64). */
 SKPS_API int skps_frame_absdiff_sum(const uint8_t* a, const uint8_t* b, size_t n,
                            unsigned long long* sum, void* stream);
+/* Frame ingest, the device-frame step of skps_pipeline_* and skps_mpipe_*: gathers an HxWx3 uint8 [dev] frame whose
+ * rows start `pitch` bytes apart (pitch >= 3W; frame and pitch of any alignment, e.g. a decoder surface or an ROI view)
+ * into `packed` [dev] (H*W*3 bytes, 16-byte aligned), and in the same pass sets *sum [dev] (uint64) to sum |frame - prev|
+ * over all bytes, exactly what skps_frame_absdiff_sum(prev, packed) returns; prev [dev] (packed, 16-byte aligned) may be
+ * NULL (copy only, *sum = 0).  Asynchronous on `stream`. */
+SKPS_API int skps_frame_ingest(const uint8_t* frame, int H, int W, int pitch, uint8_t* packed, const uint8_t* prev,
+                               unsigned long long* sum, void* stream);
 
 /* ------------------------------------------------------------------ FaceAna.run (facer.py:52-85) */
 
@@ -300,6 +307,13 @@ SKPS_API int skps_pipeline_det_results(skps_pipeline* p, int capacity, int32_t* 
  * returns -1.0 in *mean_diff when there is no previous frame of the same size. */
 SKPS_API int skps_pipeline_frame_diff(skps_pipeline* p, const uint8_t* frame, int H, int W,
                              int frame_on_device, double* mean_diff, void* stream);
+/* skps_pipeline_frame_diff for a frame already on the pipeline's device, HxWx3 uint8 BGR with rows `pitch` bytes apart
+ * (pitch >= 3W, any alignment): one skps_frame_ingest pass stages it and sums the difference.  The frame is read after all
+ * work queued on `producer_stream` before this call (the stream that wrote it; 0 is the legacy default stream), and work
+ * queued on producer_stream after this call returns runs after the read, so the producer may overwrite the frame at once.
+ * skps_pipeline_run(frame = NULL, ...) then runs on the staged copy. */
+SKPS_API int skps_pipeline_frame_diff_device(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch,
+                                             void* producer_stream, double* mean_diff, void* stream);
 /* Adopt the frame staged by skps_pipeline_frame_diff as the previous frame without running the chain: the skip path of
  * FaceAna.run (facer.py:57-62 replaces previous_image on every call, also when nothing is detected or tracked). */
 SKPS_API int skps_pipeline_commit_frame(skps_pipeline* p, int H, int W);
@@ -344,6 +358,31 @@ SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot, const uint8_t* const* fr
  * scores (n, top_k, n_points) float32; ran_detector[s] (may be NULL) = the frame-difference gate's decision. */
 SKPS_API int skps_mpipe_wait(skps_mpipe* p, int slot, int32_t* n_faces, double* boxes, double* kps, float* scores,
                              int32_t* ran_detector);
+/* Caller-owned [dev] result buffers of one batch, on the pipeline's device, laid out as skps_mpipe_wait /
+ * skps_mpipe_align_results / skps_mpipe_pose_results fill their host buffers (n = the submit's stream count; entries
+ * i >= n_faces[s] are unspecified).  chips and M are needed while alignment is on, rvec..reproject while pose is on. */
+typedef struct skps_mpipe_outputs {
+    int32_t* n_faces;                   /* (n)                             */
+    int32_t* ran_detector;              /* (n)                             */
+    double* boxes;                      /* (n, top_k, 4)                   */
+    double* kps;                        /* (n, top_k, n_points, 2)         */
+    float* scores;                      /* (n, top_k, n_points)            */
+    uint8_t* chips;                     /* (n, top_k, size, size, 3)       */
+    double* M;                          /* (n, top_k, 2, 3)                */
+    double *rvec, *tvec, *euler;        /* (n, top_k, 3) each              */
+    double* reproject;                  /* (n, top_k, 8, 2)                */
+} skps_mpipe_outputs;
+/* skps_mpipe_submit for frames already on the pipeline's device: frame i HxWx3 uint8 BGR with rows pitches[i] bytes apart
+ * (>= 3W, any alignment), gathered into the stream's ring and diffed against its previous frame in one launch for the
+ * batch.  The frames are read after all work queued on `producer_stream` before this call, and work queued on it after this
+ * call returns runs after they have been read.  out = NULL: results come back to host memory through skps_mpipe_wait as
+ * for skps_mpipe_submit.  out != NULL: the batch's results are copied into *out on the device instead, and the slot is
+ * completed by skps_mpipe_wait_stream.  Asynchronous. */
+SKPS_API int skps_mpipe_submit_device(skps_mpipe* p, int slot, const uint8_t* const* frames, const int32_t* pitches,
+                                      const int32_t* hw, int n, const skps_mpipe_outputs* out, void* producer_stream);
+/* Completes a slot submitted with device outputs without blocking the host: work queued on `consumer_stream` after this
+ * call runs after the batch's results are in the caller's buffers.  The slot can then be submitted again. */
+SKPS_API int skps_mpipe_wait_stream(skps_mpipe* p, int slot, void* consumer_stream);
 
 /* ---- Aligned face chips (csrc/align.cu; additive) -----------------------------------------------------------------------
  * What a caller does with the 98 landmarks before a recognition / attribute model: estimate the least-squares similarity

@@ -20,6 +20,7 @@ from ..smoother.lk import EmaFilter, GroupTrack, first_match, rects
 from .face_detector import FaceDetector, letterbox_geometry
 from .face_landmark import FaceLandmark
 from .align import check_size
+from .device_frames import check_cuda_frame, is_cuda_tensor
 
 
 MAX_TOP_K = 1024           # SKPS_MAX_TOP_K of include/skps_b200.h
@@ -82,6 +83,8 @@ class FaceAna():
         rt.check(self.lib.skps_pipeline_create(det.model.handle, kps.model.handle, C.byref(pc), C.byref(h)))
         self._pipe = h
         self._stream = det.model.stream
+        self._device = det.model.device
+        self._max_hw = (int(max_frame_hw[0]), int(max_frame_hw[1]))
         K, P = self.top_k, kps.keypoints_num
         self._n = C.c_int32(0)
         self._ndet = C.c_int32(0)
@@ -102,10 +105,19 @@ class FaceAna():
 
     # ------------------------------------------------------------------ facer.py:52-85
     def run(self, image):
-        image = np.ascontiguousarray(image)
-        if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
-            raise ValueError("expected an HxWx3 uint8 BGR image, got %s %s" % (image.dtype, image.shape))
-        H, W = image.shape[:2]
+        """image: an HxWx3 uint8 BGR numpy array, or a torch.uint8 CUDA tensor (H, W, 3) in BGR order on this object's
+        device with stride(2) == 1, stride(1) == 3 and any row pitch stride(0) >= 3W (a packed tensor, a pitched decoder
+        surface, big[y0:y1, x0:x1]).  A CUDA frame is copied once on the GPU, never through the host, and the results are
+        those of image.cpu().numpy() bit for bit.  Ordering on torch.cuda.current_stream(): the frame is read after all
+        work already queued on it, and work queued on it after run() returns runs after the frame has been read, so a
+        decoder may overwrite the surface at once."""
+        if is_cuda_tensor(image):
+            H, W, _ = check_cuda_frame(image, self._device, self._max_hw)
+        else:
+            image = np.ascontiguousarray(image)
+            if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
+                raise ValueError("expected an HxWx3 uint8 BGR image, got %s %s" % (image.dtype, image.shape))
+            H, W = image.shape[:2]
         run_det = self.diff_frames(self.previous_image, image)     # stages the frame on the device
         self.previous_image = image
         det = self.face_detector
@@ -184,10 +196,17 @@ class FaceAna():
     def diff_frames(self, previous_frame, image):
         """facer.py:98-118: mean |prev - cur| > 5 -> run the detector.  The sum is taken on the GPU
         against the previous frame kept in HBM; the frame uploaded here is reused by run()."""
-        H, W = image.shape[:2]
         d = C.c_double(0.0)
-        rt.check(self.lib.skps_pipeline_frame_diff(self._pipe, image.ctypes.data, H, W, 0, C.byref(d),
-                                                   self._stream.cuda_stream))
+        if is_cuda_tensor(image):
+            import torch
+            H, W, pitch = check_cuda_frame(image, self._device, self._max_hw)
+            rt.check(self.lib.skps_pipeline_frame_diff_device(self._pipe, image.data_ptr(), H, W, pitch,
+                                                              torch.cuda.current_stream(self._device).cuda_stream,
+                                                              C.byref(d), self._stream.cuda_stream))
+        else:
+            H, W = image.shape[:2]
+            rt.check(self.lib.skps_pipeline_frame_diff(self._pipe, image.ctypes.data, H, W, 0, C.byref(d),
+                                                       self._stream.cuda_stream))
         if previous_frame is None or d.value < 0:
             return True
         return bool(d.value > self.diff_thres)

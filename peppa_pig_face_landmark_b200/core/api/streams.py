@@ -11,6 +11,9 @@ device (csrc/mpipe.cu, csrc/temporal.cu) and two batches can be in flight so tha
     # FaceAnaStreams(..., pose=True): each dict also has 'pose' {'euler', 'rvec', 'tvec', 'reproject'} as FaceAna returns it
     # or, overlapped:
     fa.submit(frames_t0); fa.submit(frames_t1); r0 = fa.collect(); fa.submit(frames_t2); r1 = fa.collect(); ...
+    # frames already on the GPU (torch.uint8 CUDA tensors (H, W, 3), any row pitch), results left on the GPU:
+    res = [fa.new_results(), fa.new_results()]
+    fa.submit(cuda_frames_t0, out=res[0]); fa.submit(cuda_frames_t1, out=res[1]); r0 = fa.collect(); ...
 """
 import ctypes as C
 import os
@@ -21,6 +24,7 @@ import numpy as np
 from ... import runtime as rt
 from ...graph_tools import check_detector_input, detector_onnx_for
 from .align import check_size
+from .device_frames import check_cuda_frame, is_cuda_tensor
 from .facer import get_cfg
 from .onnx_model_base import ONNXEngine
 
@@ -53,6 +57,8 @@ class FaceAnaStreams:
         self.kps = ONNXEngine(os.path.join(root, kps_cfg['model_path']), device=device,
                               max_batch=self.n_streams * self.top_k)
         self.n_points = int(kps_cfg['num_points'])
+        self.device = self.det.device
+        self.max_frame_hw = (int(max_frame_hw[0]), int(max_frame_hw[1]))
         self.lib = rt.load_library()
         pc = rt.PipelineCfg(score_thres=det_cfg['score_thrs'], iou_thres=det_cfg['iou_thrs'],
                             min_face=float(det_cfg['min_face']), top_k=self.top_k, track_iou=float(tr_cfg['iou_thres']),
@@ -75,7 +81,7 @@ class FaceAnaStreams:
             for o in self._out:
                 o["pose"] = {k: np.zeros((S, K, 3), np.float64) for k in ("rvec", "tvec", "euler")}
                 o["pose"]["reproject"] = np.zeros((S, K, 8, 2), np.float64)
-        self._pending = []              # [(slot, n, keep-alive frames)]
+        self._pending = []              # [(slot, n, keep-alive frames, device results or None)]
         self._next = 0
         self.last_ran_detector = None
 
@@ -91,14 +97,33 @@ class FaceAnaStreams:
             self.collect()
         rt.check(self.lib.skps_mpipe_reset(self._h, -1 if stream is None else int(stream)))
 
-    def submit(self, frames):
-        """Enqueue one HxWx3 uint8 BGR frame per stream (frames[i] -> stream i, len(frames) <= n_streams).  At most two
-        batches may be pending; results come back from collect() in submission order."""
+    def submit(self, frames, out=None):
+        """Enqueue one frame per stream (frames[i] -> stream i, len(frames) <= n_streams).  At most two batches may be
+        pending; results come back from collect() in submission order.
+
+        frames: all HxWx3 uint8 BGR numpy arrays, or all torch.uint8 CUDA tensors (H, W, 3) in BGR order on this object's
+        device with stride(2) == 1, stride(1) == 3 and any row pitch stride(0) >= 3W (packed tensors, pitched decoder
+        surfaces, big[y0:y1, x0:x1] views); a mix raises ValueError.  CUDA frames never cross PCIe: one kernel for the
+        batch gathers them into the pipeline's frame ring.  Ordering on torch.cuda.current_stream(): they are read after all
+        work already queued on it, and work queued on it after submit() returns runs after they have been read, so a
+        decoder may reuse its surfaces at once.
+
+        out: None (collect() returns host results), or, with CUDA frames, a dict from new_results() not used by a batch
+        still in flight: the batch's results are written into it on the GPU and nothing is copied to the host."""
         if len(self._pending) == 2:
             raise RuntimeError("FaceAnaStreams: two batches already in flight; call collect() first")
         n = len(frames)
         if not 0 < n <= self.n_streams:
             raise ValueError("expected 1..%d frames, got %d" % (self.n_streams, n))
+        on_device = [is_cuda_tensor(f) for f in frames]
+        if any(on_device):
+            if not all(on_device):
+                raise ValueError("one batch takes either host frames or CUDA frames, got both (streams %s are CUDA)"
+                                 % [i for i, d in enumerate(on_device) if d])
+            self._submit_device(frames, out)
+            return
+        if out is not None:
+            raise ValueError("out= keeps results on the GPU and takes CUDA frames; these are host frames")
         keep = []
         for f in frames:
             f = np.ascontiguousarray(f)
@@ -109,14 +134,84 @@ class FaceAnaStreams:
         hw = np.array([[f.shape[0], f.shape[1]] for f in keep], np.int32)
         slot = self._next
         rt.check(self.lib.skps_mpipe_submit(self._h, slot, ptrs, hw.ctypes.data, n, 0))
-        self._pending.append((slot, n, keep))
+        self._pending.append((slot, n, keep, None))
         self._next ^= 1
 
+    def _submit_device(self, frames, out):
+        import torch
+        n = len(frames)
+        layout = [check_cuda_frame(f, self.device, self.max_frame_hw) for f in frames]
+        outs = None
+        if out is not None:
+            self._check_out(out)
+            outs = rt.MpipeOutputs(n_faces=out["n"].data_ptr(), ran_detector=out["ran_detector"].data_ptr(),
+                                   boxes=out["box"].data_ptr(), kps=out["kps"].data_ptr(), scores=out["scores"].data_ptr())
+            for k, field in (("chip", "chips"), ("M", "M"), ("rvec", "rvec"), ("tvec", "tvec"), ("euler", "euler"),
+                             ("reproject", "reproject")):
+                if k in out:
+                    setattr(outs, field, out[k].data_ptr())
+        ptrs = (C.c_void_p * n)(*[f.data_ptr() for f in frames])
+        pitches = np.array([p for _, _, p in layout], np.int32)
+        hw = np.array([[h, w] for h, w, _ in layout], np.int32)
+        slot = self._next
+        rt.check(self.lib.skps_mpipe_submit_device(self._h, slot, ptrs, pitches.ctypes.data, hw.ctypes.data, n,
+                                                   None if outs is None else C.byref(outs),
+                                                   torch.cuda.current_stream(self.device).cuda_stream))
+        self._pending.append((slot, n, list(frames), out))
+        self._next ^= 1
+
+    def _result_layout(self):
+        import torch
+        S, K, P = self.n_streams, self.top_k, self.n_points
+        f64 = torch.float64
+        r = {"n": ((S,), torch.int32), "ran_detector": ((S,), torch.int32), "box": ((S, K, 4), f64),
+             "kps": ((S, K, P, 2), f64), "scores": ((S, K, P), torch.float32)}
+        if self.align is not None:
+            r["chip"] = ((S, K, self.align, self.align, 3), torch.uint8)
+            r["M"] = ((S, K, 2, 3), f64)
+        if self.pose:
+            r.update(rvec=((S, K, 3), f64), tvec=((S, K, 3), f64), euler=((S, K, 3), f64), reproject=((S, K, 8, 2), f64))
+        return r
+
+    def new_results(self):
+        """Device result buffers for submit(cuda_frames, out=...): a dict of CUDA tensors on this object's device,
+        n (S,) int32 faces per stream; ran_detector (S,) int32, the frame-difference gate's decision; box (S,K,4) and kps
+        (S,K,P,2) float64; scores (S,K,P) float32; with align, chip (S,K,size,size,3) uint8 and M (S,K,2,3) float64; with
+        pose, rvec, tvec, euler (S,K,3) and reproject (S,K,8,2) float64.  Per stream s, face rows i >= n[s] (and streams
+        past the batch's length) are unspecified."""
+        import torch
+        return {k: torch.empty(shape, dtype=dt, device=self.device) for k, (shape, dt) in self._result_layout().items()}
+
+    def _check_out(self, out):
+        import torch
+        want = self._result_layout()
+        if not isinstance(out, dict) or set(out) != set(want):
+            raise ValueError("out: expected a dict with keys %s (see new_results())" % sorted(want))
+        for k, (shape, dt) in want.items():
+            t = out[k]
+            if (not isinstance(t, torch.Tensor) or tuple(t.shape) != shape or t.dtype != dt or t.device != self.device
+                    or not t.is_contiguous()):
+                got = ("%s %s on %s" % (t.dtype, tuple(t.shape), t.device)) if isinstance(t, torch.Tensor) \
+                    else type(t).__name__
+                raise ValueError("out[%r]: expected a contiguous %s tensor %s on %s, got %s" % (k, dt, shape, self.device,
+                                                                                               got))
+        busy = {t.data_ptr() for _, _, _, o in self._pending if o is not None for t in o.values()}
+        if any(t.data_ptr() in busy for t in out.values()):
+            raise ValueError("out: these buffers belong to a batch still in flight; collect() it first")
+
     def collect(self):
-        """Results of the oldest pending batch: a list (one entry per stream) of lists of {'box','kps','scores'}."""
+        """Results of the oldest pending batch: a list (one entry per stream) of lists of {'box','kps','scores'}; for a
+        batch submitted with out=, that dict, with no host synchronisation: torch.cuda.current_stream() is made to wait
+        for the batch, so work queued on it afterwards sees the results (last_ran_detector is then None; the gate's
+        decisions are out['ran_detector'])."""
         if not self._pending:
             raise RuntimeError("FaceAnaStreams: nothing submitted")
-        slot, n, _keep = self._pending.pop(0)
+        slot, n, _keep, out = self._pending.pop(0)
+        if out is not None:
+            import torch
+            rt.check(self.lib.skps_mpipe_wait_stream(self._h, slot, torch.cuda.current_stream(self.device).cuda_stream))
+            self.last_ran_detector = None
+            return out
         o = self._out[slot]
         rt.check(self.lib.skps_mpipe_wait(self._h, slot, o["n"].ctypes.data, o["box"].ctypes.data, o["kps"].ctypes.data,
                                           o["sc"].ctypes.data, o["det"].ctypes.data))

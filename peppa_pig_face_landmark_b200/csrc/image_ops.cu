@@ -473,24 +473,85 @@ __global__ void mp_landmark_post_kernel(const float* __restrict__ xy, const int*
     kps[(size_t)2 * per * st + i * 2 + 1] = oy;
 }
 
-__global__ void __launch_bounds__(256) mp_absdiff_kernel(const MpStreamDesc* __restrict__ d, unsigned long long* __restrict__ sum) {
-    // per stream exactly absdiff_sum_kernel (integer sums: the order of the atomic adds does not matter)
-    const MpStreamDesc D = d[blockIdx.y];
-    if (!D.have_prev) return;
-    const uint8_t* a = D.prev;
-    const uint8_t* b = D.cur;
-    const size_t n = (size_t)D.H * D.W * 3, nv = n / 16;
-    unsigned long long local = 0;
-    const uint4* a4 = reinterpret_cast<const uint4*>(a);
-    const uint4* b4 = reinterpret_cast<const uint4*>(b);
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += (size_t)gridDim.x * blockDim.x) {
-        uint4 x = a4[i], y = b4[i];
-        local += __vsadu4(x.x, y.x) + __vsadu4(x.y, y.y) + __vsadu4(x.z, y.z) + __vsadu4(x.w, y.w);
+// 16 bytes from an address of any alignment: the one or two aligned 16-byte blocks that hold them, shifted into place.
+// Every block loaded holds a byte of the range, so no load leaves the allocation.
+__device__ __forceinline__ uint4 load16_any(const uint8_t* p) {
+    const unsigned off = (unsigned)((uintptr_t)p & 15);
+    const uint4* a = reinterpret_cast<const uint4*>(p - off);
+    const uint4 lo = __ldg(a);
+    if (off == 0) return lo;
+    const uint4 hi = __ldg(a + 1);
+    unsigned w0, w1, w2, w3, w4;
+    switch (off >> 2) {
+        case 0: w0 = lo.x; w1 = lo.y; w2 = lo.z; w3 = lo.w; w4 = hi.x; break;
+        case 1: w0 = lo.y; w1 = lo.z; w2 = lo.w; w3 = hi.x; w4 = hi.y; break;
+        case 2: w0 = lo.z; w1 = lo.w; w2 = hi.x; w3 = hi.y; w4 = hi.z; break;
+        default: w0 = lo.w; w1 = hi.x; w2 = hi.y; w3 = hi.z; w4 = hi.w; break;
     }
-    if (blockIdx.x == 0) {
-        for (size_t i = nv * 16 + threadIdx.x; i < n; i += blockDim.x) {
-            int dd = (int)a[i] - (int)b[i];
-            local += (unsigned)(dd < 0 ? -dd : dd);
+    const unsigned sh = (off & 3) * 8;
+    return make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh),
+                      __funnelshift_r(w3, w4, sh));
+}
+
+// Ingest of one frame: the packed frame cur is cut into 16-byte units; unit u takes bytes [16u, 16u + 16) of the frame
+// from row y = 16u / (3W) of the pitched source.  A unit inside one row is one 16-byte store from load16_any; a unit that
+// crosses a row end, and the partial last unit, go byte by byte.  Returns this thread's part of sum |cur - prev|.
+__device__ __forceinline__ unsigned long long ingest_units(const MpStreamDesc& D) {
+    const unsigned row = (unsigned)D.W * 3u, n = row * (unsigned)D.H, units = (n + 15) / 16;
+    const uint8_t* __restrict__ src = D.src;
+    uint8_t* __restrict__ cur = D.cur;
+    const uint8_t* __restrict__ prev = D.have_prev ? D.prev : nullptr;
+    unsigned long long local = 0;
+    for (unsigned u = blockIdx.x * blockDim.x + threadIdx.x; u < units; u += gridDim.x * blockDim.x) {
+        const unsigned o = u * 16, y = o / row, x = o - y * row;
+        if (x + 16 <= row) {
+            const uint4 v = load16_any(src + (size_t)y * D.src_pitch + x);
+            *reinterpret_cast<uint4*>(cur + o) = v;
+            if (prev) {
+                const uint4 q = *reinterpret_cast<const uint4*>(prev + o);
+                local += __vsadu4(v.x, q.x) + __vsadu4(v.y, q.y) + __vsadu4(v.z, q.z) + __vsadu4(v.w, q.w);
+            }
+        } else {
+            unsigned yy = y, xx = x;
+            const unsigned end = o + 16 < n ? o + 16 : n;
+            for (unsigned i = o; i < end; ++i) {
+                const uint8_t v = src[(size_t)yy * D.src_pitch + xx];
+                cur[i] = v;
+                if (prev) {
+                    const int dd = (int)v - (int)prev[i];
+                    local += (unsigned)(dd < 0 ? -dd : dd);
+                }
+                if (++xx == row) { xx = 0; ++yy; }
+            }
+        }
+    }
+    return local;
+}
+
+__global__ void __launch_bounds__(256) mp_absdiff_kernel(const MpStreamDesc* __restrict__ d, MpStreamDesc one,
+                                                         unsigned long long* __restrict__ sum) {
+    // per stream exactly absdiff_sum_kernel (integer sums: the order of the atomic adds does not matter); a stream with a
+    // source frame is gathered into its packed frame in the same pass
+    const MpStreamDesc D = d ? d[blockIdx.y] : one;
+    if (!D.have_prev && !D.src) return;
+    unsigned long long local = 0;
+    if (D.src) {
+        local = ingest_units(D);
+    } else {
+        const uint8_t* a = D.prev;
+        const uint8_t* b = D.cur;
+        const size_t n = (size_t)D.H * D.W * 3, nv = n / 16;
+        const uint4* a4 = reinterpret_cast<const uint4*>(a);
+        const uint4* b4 = reinterpret_cast<const uint4*>(b);
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += (size_t)gridDim.x * blockDim.x) {
+            uint4 x = a4[i], y = b4[i];
+            local += __vsadu4(x.x, y.x) + __vsadu4(x.y, y.y) + __vsadu4(x.z, y.z) + __vsadu4(x.w, y.w);
+        }
+        if (blockIdx.x == 0) {
+            for (size_t i = nv * 16 + threadIdx.x; i < n; i += blockDim.x) {
+                int dd = (int)a[i] - (int)b[i];
+                local += (unsigned)(dd < 0 ? -dd : dd);
+            }
         }
     }
     for (int o = 16; o > 0; o >>= 1) local += __shfl_down_sync(0xffffffffu, local, o);
@@ -504,11 +565,22 @@ __global__ void __launch_bounds__(256) mp_absdiff_kernel(const MpStreamDesc* __r
     }
 }
 
-int launch_mp_absdiff(const MpStreamDesc* d, unsigned long long* diff, int n, size_t max_bytes, cudaStream_t s) {
+static int absdiff_grid(size_t max_bytes) {
     size_t blocks = (max_bytes / 16 + 255) / 256;
     if (blocks > 592) blocks = 592;
     if (blocks < 1) blocks = 1;
-    mp_absdiff_kernel<<<dim3((unsigned)blocks, n), 256, 0, s>>>(d, diff);
+    return (int)blocks;
+}
+int launch_mp_absdiff(const MpStreamDesc* d, unsigned long long* diff, int n, size_t max_bytes, cudaStream_t s) {
+    SKPS_CHECK(max_bytes < (1ull << 32) - 16, "absdiff: a %zu-byte frame is larger than 4 GB", max_bytes);
+    mp_absdiff_kernel<<<dim3(absdiff_grid(max_bytes), n), 256, 0, s>>>(d, MpStreamDesc{}, diff);
+    SKPS_CUDA(cudaGetLastError());
+    return 0;
+}
+int launch_frame_ingest(const MpStreamDesc& one, unsigned long long* diff, cudaStream_t s) {
+    const size_t bytes = (size_t)one.H * one.W * 3;
+    SKPS_CHECK(bytes < (1ull << 32) - 16, "ingest: a %zu-byte frame is larger than 4 GB", bytes);
+    mp_absdiff_kernel<<<dim3(absdiff_grid(bytes), 1), 256, 0, s>>>(nullptr, one, diff);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }
@@ -614,4 +686,15 @@ extern "C" SKPS_API int skps_frame_absdiff_sum(const uint8_t* a, const uint8_t* 
     absdiff_sum_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a, b, n, sum);
     SKPS_CUDA(cudaGetLastError());
     return 0;
+}
+
+extern "C" SKPS_API int skps_frame_ingest(const uint8_t* frame, int H, int W, int pitch, uint8_t* packed, const uint8_t* prev,
+                                          unsigned long long* sum, void* stream) {
+    SKPS_CHECK(frame && packed && sum && H > 0 && W > 0 && (H == 1 || pitch >= 3 * W), "ingest: bad arguments");
+    SKPS_CHECK(((uintptr_t)packed % 16 == 0) && ((uintptr_t)prev % 16 == 0), "ingest: packed and prev must be 16-byte aligned");
+    SKPS_CUDA(cudaMemsetAsync(sum, 0, sizeof(unsigned long long), (cudaStream_t)stream));
+    MpStreamDesc D = {};
+    D.cur = packed; D.prev = prev; D.have_prev = prev != nullptr; D.H = H; D.W = W;
+    D.src = frame; D.src_pitch = pitch;
+    return launch_frame_ingest(D, sum, (cudaStream_t)stream);
 }

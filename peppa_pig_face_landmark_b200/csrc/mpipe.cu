@@ -2,7 +2,8 @@
 //
 // One call takes one frame from each of up to S streams and runs, batched across the streams and with every piece of
 // per-stream state resident in HBM:
-//   H2D (copy stream, overlapped with the previous batch's compute) -> |prev - cur| gate -> letterbox x S ->
+//   H2D (copy stream, overlapped with the previous batch's compute) -> |prev - cur| gate (which gathers frames already on
+//   the device into the ring in the same pass) -> letterbox x S ->
 //   ONE detector forward (batch S) -> NMS x S -> judge_boxs/sort_and_filter x S (detector rows or track boxes, chosen on
 //   the device by the gate) -> crops x S -> ONE landmark forward (batch S * top_k) -> de-normalise -> GroupTrack / One-Euro /
 //   track-box EMA x S (temporal.cu, float64 with numpy's promotion rules) -> D2H of the packed results.
@@ -42,11 +43,15 @@ struct skps_mpipe {
         uint8_t* h_chips = nullptr; double* h_M = nullptr;     // pinned, only while alignment is on
         double* h_pose = nullptr;             // pinned, only while pose is on: rvec, tvec, euler [n][K][3], reproject [n][K][8][2]
         cudaEvent_t ev_in = nullptr, ev_done = nullptr;
+        cudaEvent_t ev_staged = nullptr;      // the batch's uploads from the pinned h_hw / h_have_prev / h_desc are done
         int n = 0;
         int align = 0;                        // chip size this slot's batch was submitted with (0 = none)
         bool pose = false;                    // this slot's batch was submitted with pose on
         bool busy = false;
+        bool device_out = false;              // the batch's results go to caller buffers (skps_mpipe_wait_stream)
     } slot[2];
+    // device frames: the producer's stream is ordered before the ingest (ev_ready) and the ingest before its later work (ev_read)
+    cudaEvent_t ev_ready = nullptr, ev_read = nullptr;
     // aligned chips (skps_mpipe_set_align): [S][K][size][size][3] / [S][K][2][3], allocated only while align_size > 0
     int align_size = 0;
     uint8_t* d_chips = nullptr; double* d_align_M = nullptr;
@@ -87,7 +92,10 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
         for (void* q : host) if (q) cudaFreeHost(q);
         if (sl.ev_in) cudaEventDestroy(sl.ev_in);
         if (sl.ev_done) cudaEventDestroy(sl.ev_done);
+        if (sl.ev_staged) cudaEventDestroy(sl.ev_staged);
     }
+    if (p->ev_ready) cudaEventDestroy(p->ev_ready);
+    if (p->ev_read) cudaEventDestroy(p->ev_read);
     void* dev[] = {p->d_desc, p->d_hw, p->d_have_prev, p->d_flag, p->d_det_count, p->d_det_idx, p->d_count, p->d_detail, p->d_diff,
                    p->d_det_rows, p->d_boxes, p->d_kps_now, p->d_prev_lm, p->d_prev_dx, p->d_track, p->d_out_kps,
                    p->d_track_f32, p->d_n_prev, p->d_prev_f32, p->d_state_idx, p->d_n_track, p->d_chips, p->d_align_M, p->d_pose,
@@ -154,8 +162,11 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
         MP_HOST(sl.h_box, sizeof(double) * 4 * K * S); MP_HOST(sl.h_kps, sizeof(double) * 2 * P * K * S);
         MP_HOST(sl.h_scores, sizeof(float) * P * K * S);
         if (cudaEventCreateWithFlags(&sl.ev_in, cudaEventDisableTiming) != cudaSuccess ||
-            cudaEventCreateWithFlags(&sl.ev_done, cudaEventDisableTiming) != cudaSuccess) { set_error("cudaEventCreate"); return fail("event"); }
+            cudaEventCreateWithFlags(&sl.ev_done, cudaEventDisableTiming) != cudaSuccess ||
+            cudaEventCreateWithFlags(&sl.ev_staged, cudaEventDisableTiming) != cudaSuccess) { set_error("cudaEventCreate"); return fail("event"); }
     }
+    if (cudaEventCreateWithFlags(&p->ev_ready, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&p->ev_read, cudaEventDisableTiming) != cudaSuccess) { set_error("cudaEventCreate"); return fail("event"); }
     MP_DEV(p->d_desc, sizeof(MpStreamDesc) * S); MP_DEV(p->d_hw, 8 * S); MP_DEV(p->d_have_prev, 4 * S); MP_DEV(p->d_flag, 4 * S); MP_DEV(p->d_det_count, 4 * S);
     MP_DEV(p->d_det_idx, 4 * (size_t)p->det_rows * S); MP_DEV(p->d_count, 4 * S); MP_DEV(p->d_detail, 4 * 5 * (size_t)K * S);
     MP_DEV(p->d_diff, 8 * S); MP_DEV(p->d_det_rows, 4 * 16 * (size_t)p->det_rows * S);
@@ -177,26 +188,39 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
     return 0;
 }
 
-extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* hw, int n,
-                                          int frames_on_device) {
+// One batch.  Host frames are uploaded on the copy stream into the next ring position; device frames (rows pitches[i]
+// bytes apart, or 3W when pitches is null) are gathered there by the mp_absdiff launch on the compute stream, after the
+// work queued on *producer (when given).  out: results into caller buffers on the device instead of the slot's pinned ones.
+static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* pitches, const int32_t* hw,
+                        int n, bool on_device, const skps_mpipe_outputs* out, const cudaStream_t* producer) {
     SKPS_CHECK(p && frames && hw && (slot_i == 0 || slot_i == 1) && n > 0 && n <= p->S, "mpipe_submit: bad arguments");
     skps_mpipe::Slot& sl = p->slot[slot_i];
     SKPS_CHECK(!sl.busy, "mpipe_submit: slot %d still holds results (call skps_mpipe_wait first)", slot_i);
+    SKPS_CHECK(!out || (out->n_faces && out->ran_detector && out->boxes && out->kps && out->scores),
+               "mpipe_submit: device outputs need n_faces, ran_detector, boxes, kps and scores");
+    SKPS_CHECK(!out || !p->align_size || (out->chips && out->M), "mpipe_submit: alignment is on; device outputs need chips and M");
+    SKPS_CHECK(!out || !p->pose_on || (out->rvec && out->tvec && out->euler && out->reproject),
+               "mpipe_submit: pose is on; device outputs need rvec, tvec, euler and reproject");
     SKPS_CUDA(cudaSetDevice(p->device));
     const skps_pipeline_cfg& c = p->cfg;
     const int S = p->S, K = p->K, P = p->P;
     cudaStream_t sc = p->s_copy, sx = p->s_compute;
+    // a slot completed by skps_mpipe_wait_stream was not waited for on the host: its last batch may still be reading the
+    // pinned per-batch buffers rewritten below
+    SKPS_CUDA(cudaEventSynchronize(sl.ev_staged));
+    // and it may still read the ring position that host frames are about to be uploaded into
+    if (!on_device && sl.device_out) SKPS_CUDA(cudaStreamWaitEvent(sc, sl.ev_done, 0));
     // ---- uploads on the copy stream: frame i of stream i into the next ring position
     for (int s = 0; s < n; ++s) {
         const int H = hw[2 * s], W = hw[2 * s + 1];
         SKPS_CHECK(frames[s] && H > 0 && W > 0 && (size_t)H * W * 3 <= p->frame_bytes,
                    "mpipe_submit: frame %d is %dx%d, larger than the pipeline maximum %dx%d", s, H, W, c.max_h, c.max_w);
+        SKPS_CHECK(!pitches || H == 1 || pitches[s] >= 3 * W, "mpipe_submit: frame %d has row pitch %d, less than 3 x width %d",
+                   s, pitches ? pitches[s] : 0, W);
         const size_t bytes = (size_t)H * W * 3;
         const int pos = (p->ring_pos[s] + 1) % 3;
         uint8_t* dst = p->d_frame[(size_t)s * 3 + pos];
-        if (frames_on_device) {
-            SKPS_CUDA(cudaMemcpyAsync(dst, frames[s], bytes, cudaMemcpyDeviceToDevice, sc));
-        } else {
+        if (!on_device) {
             cudaPointerAttributes attr;
             const bool pinned = cudaPointerGetAttributes(&attr, frames[s]) == cudaSuccess && attr.type == cudaMemoryTypeHost;
             const uint8_t* src = frames[s];
@@ -210,9 +234,14 @@ extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8
         sl.h_hw[2 * s] = H; sl.h_hw[2 * s + 1] = W;
         sl.h_have_prev[s] = (p->prev_h[s] == H && p->prev_w[s] == W) ? 1 : 0;
     }
-    SKPS_CUDA(cudaEventRecord(sl.ev_in, sc));
+    if (!on_device) {
+        SKPS_CUDA(cudaEventRecord(sl.ev_in, sc));
+        SKPS_CUDA(cudaStreamWaitEvent(sx, sl.ev_in, 0));
+    } else if (producer) {
+        SKPS_CUDA(cudaEventRecord(p->ev_ready, *producer));
+        SKPS_CUDA(cudaStreamWaitEvent(sx, p->ev_ready, 0));
+    }
     // ---- compute
-    SKPS_CUDA(cudaStreamWaitEvent(sx, sl.ev_in, 0));
     SKPS_CUDA(cudaMemcpyAsync(p->d_hw, sl.h_hw, 8 * n, cudaMemcpyHostToDevice, sx));
     SKPS_CUDA(cudaMemcpyAsync(p->d_have_prev, sl.h_have_prev, 4 * n, cudaMemcpyHostToDevice, sx));
     SKPS_CUDA(cudaMemsetAsync(p->d_diff, 0, 8 * n, sx));
@@ -227,12 +256,22 @@ extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8
         D.cur = p->d_frame[(size_t)s * 3 + (p->ring_pos[s] + 1) % 3];
         D.prev = sl.h_have_prev[s] ? p->d_frame[(size_t)s * 3 + p->ring_pos[s]] : nullptr;
         D.H = H; D.W = W; D.have_prev = sl.h_have_prev[s];
+        D.src = on_device ? frames[s] : nullptr;
+        D.src_pitch = pitches ? pitches[s] : W * 3;
         letterbox_geometry(H, W, p->det_h, p->det_w, &D.scale, &D.rw, &D.rh, &D.top, &D.left);
         memcpy(&sl.h_geom[8 * s], &D.scale, 4); sl.h_geom[8 * s + 1] = D.top; sl.h_geom[8 * s + 2] = D.left;
         if ((size_t)H * W * 3 > max_bytes) max_bytes = (size_t)H * W * 3;
     }
     SKPS_CUDA(cudaMemcpyAsync(p->d_desc, sl.h_desc, sizeof(MpStreamDesc) * n, cudaMemcpyHostToDevice, sx));
+    SKPS_CUDA(cudaEventRecord(sl.ev_staged, sx));
     if (launch_mp_absdiff(p->d_desc, p->d_diff, n, max_bytes, sx)) return 1;
+    if (on_device && producer) {
+        SKPS_CUDA(cudaEventRecord(p->ev_read, sx));
+        SKPS_CUDA(cudaStreamWaitEvent(*producer, p->ev_read, 0));
+    }
+    // results: D2H into the slot's pinned buffers, or D2D into the caller's; either way before the next batch on sx can
+    // overwrite d_out_kps, the engine's score output or the chips
+    const cudaMemcpyKind result_kind = out ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     if (launch_mp_letterbox(p->d_desc, det_in, det_in_bytes, p->det_h, p->det_w, n, sx)) return 1;
     if (launch_mp_decide(p->d_diff, p->d_hw, p->d_have_prev, p->d_flag, n, sx)) return 1;
     // the detector runs for every stream of the batch (one launch sequence); the gate only chooses whose rows are used
@@ -272,8 +311,8 @@ extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8
         // chips from the smoothed landmarks, on the frames still in the ring
         const size_t chip_bytes = (size_t)sl.align * sl.align * 3;
         if (launch_mp_align(p->d_desc, p->d_out_kps, p->d_count, K, P, sl.align, p->d_chips, p->d_align_M, n, sx)) return 1;
-        SKPS_CUDA(cudaMemcpyAsync(sl.h_chips, p->d_chips, chip_bytes * K * n, cudaMemcpyDeviceToHost, sx));
-        SKPS_CUDA(cudaMemcpyAsync(sl.h_M, p->d_align_M, 8 * 6 * (size_t)K * n, cudaMemcpyDeviceToHost, sx));
+        SKPS_CUDA(cudaMemcpyAsync(out ? out->chips : sl.h_chips, p->d_chips, chip_bytes * K * n, result_kind, sx));
+        SKPS_CUDA(cudaMemcpyAsync(out ? out->M : sl.h_M, p->d_align_M, 8 * 6 * (size_t)K * n, result_kind, sx));
     }
     sl.pose = p->pose_on;
     if (sl.pose) {
@@ -285,13 +324,21 @@ extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8
         const size_t faces = (size_t)n * K;
         pa.rvec = p->d_pose; pa.tvec = p->d_pose + 3 * faces; pa.euler = p->d_pose + 6 * faces; pa.reproj = p->d_pose + 9 * faces;
         if (launch_head_pose(pa, sx)) return 1;
-        SKPS_CUDA(cudaMemcpyAsync(sl.h_pose, p->d_pose, 8 * 25 * faces, cudaMemcpyDeviceToHost, sx));
+        if (out) {
+            SKPS_CUDA(cudaMemcpyAsync(out->rvec, pa.rvec, 8 * 3 * faces, result_kind, sx));
+            SKPS_CUDA(cudaMemcpyAsync(out->tvec, pa.tvec, 8 * 3 * faces, result_kind, sx));
+            SKPS_CUDA(cudaMemcpyAsync(out->euler, pa.euler, 8 * 3 * faces, result_kind, sx));
+            SKPS_CUDA(cudaMemcpyAsync(out->reproject, pa.reproj, 8 * 16 * faces, result_kind, sx));
+        } else {
+            SKPS_CUDA(cudaMemcpyAsync(sl.h_pose, p->d_pose, 8 * 25 * faces, result_kind, sx));
+        }
     }
-    SKPS_CUDA(cudaMemcpyAsync(sl.h_count, p->d_count, 4 * n, cudaMemcpyDeviceToHost, sx));
-    SKPS_CUDA(cudaMemcpyAsync(sl.h_flag, p->d_flag, 4 * n, cudaMemcpyDeviceToHost, sx));
-    SKPS_CUDA(cudaMemcpyAsync(sl.h_box, p->d_track, 8 * 4 * (size_t)K * n, cudaMemcpyDeviceToHost, sx));
-    SKPS_CUDA(cudaMemcpyAsync(sl.h_kps, p->d_out_kps, 8 * 2 * (size_t)P * K * n, cudaMemcpyDeviceToHost, sx));
-    SKPS_CUDA(cudaMemcpyAsync(sl.h_scores, skps_engine_output_ptr(p->kps, 1), 4 * (size_t)P * K * n, cudaMemcpyDeviceToHost, sx));
+    SKPS_CUDA(cudaMemcpyAsync(out ? out->n_faces : sl.h_count, p->d_count, 4 * n, result_kind, sx));
+    SKPS_CUDA(cudaMemcpyAsync(out ? out->ran_detector : sl.h_flag, p->d_flag, 4 * n, result_kind, sx));
+    SKPS_CUDA(cudaMemcpyAsync(out ? out->boxes : sl.h_box, p->d_track, 8 * 4 * (size_t)K * n, result_kind, sx));
+    SKPS_CUDA(cudaMemcpyAsync(out ? out->kps : sl.h_kps, p->d_out_kps, 8 * 2 * (size_t)P * K * n, result_kind, sx));
+    SKPS_CUDA(cudaMemcpyAsync(out ? out->scores : sl.h_scores, skps_engine_output_ptr(p->kps, 1), 4 * (size_t)P * K * n,
+                              result_kind, sx));
     SKPS_CUDA(cudaEventRecord(sl.ev_done, sx));
     // ring discipline: this batch read positions r (previous) and r+1 (current); the next batch uploads into r+2 (free), the
     // one after into r again - and that one reuses this slot, so the caller has passed skps_mpipe_wait(slot) by then
@@ -301,6 +348,37 @@ extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8
     }
     sl.n = n;
     sl.busy = true;
+    sl.device_out = out != nullptr;
+    return 0;
+}
+
+extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* hw, int n,
+                                          int frames_on_device) {
+    return submit_batch(p, slot_i, frames, nullptr, hw, n, frames_on_device != 0, nullptr, nullptr);
+}
+
+extern "C" SKPS_API int skps_mpipe_submit_device(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* pitches,
+                                                 const int32_t* hw, int n, const skps_mpipe_outputs* out, void* producer_stream) {
+    SKPS_CHECK(p && frames && pitches && hw && n > 0 && n <= p->S, "mpipe_submit_device: bad arguments");
+    SKPS_CUDA(cudaSetDevice(p->device));
+    for (int s = 0; s < n; ++s) {
+        cudaPointerAttributes attr;
+        SKPS_CUDA(cudaPointerGetAttributes(&attr, frames[s]));
+        SKPS_CHECK((attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) && attr.device == p->device,
+                   "mpipe_submit_device: frame %d is not in memory of device %d", s, p->device);
+    }
+    const cudaStream_t producer = (cudaStream_t)producer_stream;
+    return submit_batch(p, slot_i, frames, pitches, hw, n, true, out, &producer);
+}
+
+extern "C" SKPS_API int skps_mpipe_wait_stream(skps_mpipe* p, int slot_i, void* consumer_stream) {
+    SKPS_CHECK(p && (slot_i == 0 || slot_i == 1), "mpipe_wait_stream: bad arguments");
+    skps_mpipe::Slot& sl = p->slot[slot_i];
+    SKPS_CHECK(sl.busy, "mpipe_wait_stream: nothing submitted on slot %d", slot_i);
+    SKPS_CHECK(sl.device_out, "mpipe_wait_stream: slot %d has host results (call skps_mpipe_wait)", slot_i);
+    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_CUDA(cudaStreamWaitEvent((cudaStream_t)consumer_stream, sl.ev_done, 0));
+    sl.busy = false;
     return 0;
 }
 
@@ -309,6 +387,7 @@ extern "C" SKPS_API int skps_mpipe_wait(skps_mpipe* p, int slot_i, int32_t* n_fa
     SKPS_CHECK(p && (slot_i == 0 || slot_i == 1) && n_faces && boxes && kps && scores, "mpipe_wait: bad arguments");
     skps_mpipe::Slot& sl = p->slot[slot_i];
     SKPS_CHECK(sl.busy, "mpipe_wait: nothing submitted on slot %d", slot_i);
+    SKPS_CHECK(!sl.device_out, "mpipe_wait: slot %d has device results (call skps_mpipe_wait_stream)", slot_i);
     SKPS_CUDA(cudaSetDevice(p->device));
     SKPS_CUDA(cudaEventSynchronize(sl.ev_done));
     sl.busy = false;
@@ -363,7 +442,8 @@ extern "C" SKPS_API int skps_mpipe_align_results(skps_mpipe* p, int slot_i, uint
     SKPS_CHECK(p && (slot_i == 0 || slot_i == 1) && chips && M, "mpipe_align_results: bad arguments");
     const skps_mpipe::Slot& sl = p->slot[slot_i];
     SKPS_CHECK(!sl.busy, "mpipe_align_results: slot %d is in flight (call skps_mpipe_wait first)", slot_i);
-    SKPS_CHECK(sl.align > 0 && sl.n > 0, "mpipe_align_results: slot %d was not submitted with alignment on", slot_i);
+    SKPS_CHECK(sl.align > 0 && sl.n > 0 && !sl.device_out, "mpipe_align_results: slot %d was not submitted with alignment on "
+               "and host results", slot_i);
     const size_t faces = (size_t)sl.n * p->K;
     memcpy(chips, sl.h_chips, faces * sl.align * sl.align * 3);
     memcpy(M, sl.h_M, faces * 6 * sizeof(double));
@@ -406,7 +486,8 @@ extern "C" SKPS_API int skps_mpipe_pose_results(skps_mpipe* p, int slot_i, doubl
     SKPS_CHECK(p && (slot_i == 0 || slot_i == 1) && rvec && tvec && euler && reproject, "mpipe_pose_results: bad arguments");
     const skps_mpipe::Slot& sl = p->slot[slot_i];
     SKPS_CHECK(!sl.busy, "mpipe_pose_results: slot %d is in flight (call skps_mpipe_wait first)", slot_i);
-    SKPS_CHECK(sl.pose && sl.n > 0, "mpipe_pose_results: slot %d was not submitted with pose on", slot_i);
+    SKPS_CHECK(sl.pose && sl.n > 0 && !sl.device_out, "mpipe_pose_results: slot %d was not submitted with pose on and host "
+               "results", slot_i);
     const size_t faces = (size_t)sl.n * p->K;
     memcpy(rvec, sl.h_pose, faces * 3 * sizeof(double));
     memcpy(tvec, sl.h_pose + 3 * faces, faces * 3 * sizeof(double));

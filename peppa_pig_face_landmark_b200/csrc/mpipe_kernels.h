@@ -29,15 +29,21 @@ struct MpTemporalArgs {
 
 // One frame of one stream as the batched pre/post-processing kernels see it (filled on the host per call, one upload).
 struct MpStreamDesc {
-    const uint8_t* cur;          // this call's frame (HxWx3 uint8 BGR, device)
-    const uint8_t* prev;         // the previous frame of the stream, or null
+    uint8_t* cur;                // this call's frame (packed HxWx3 uint8 BGR, device, 16-byte aligned)
+    const uint8_t* prev;         // the previous frame of the stream (packed, 16-byte aligned), or null
     int H, W, have_prev;
     float scale;                 // letterbox geometry (face_detector.py:49-62)
     int rw, rh, top, left;
+    const uint8_t* src;          // the caller's device frame, gathered into cur by launch_mp_absdiff, or null (cur holds it)
+    int src_pitch;               // bytes from one row of src to the next, >= 3 W, any alignment
 };
 // Batched over the streams of a call (grid z / x = stream): what S x {skps_frame_absdiff_sum, skps_letterbox,
 // skps_crop_resize, skps_landmark_post} launches did, in four launches.  Same device code per element, bit for bit.
+// launch_mp_absdiff also ingests: a stream with src set gets its frame gathered into cur and, with have_prev, |cur - prev|
+// summed in the same pass (the same integer sum as from a packed cur).  d [dev] holds n descriptors; launch_frame_ingest
+// runs the same kernel on one descriptor passed by value (diff = one counter, zeroed by the caller).
 int launch_mp_absdiff(const MpStreamDesc* d, unsigned long long* diff, int n, size_t max_bytes, cudaStream_t s);
+int launch_frame_ingest(const MpStreamDesc& one, unsigned long long* diff, cudaStream_t s);
 int launch_mp_letterbox(const MpStreamDesc* d, uint8_t* out, size_t out_stride, int in_h, int in_w, int n, cudaStream_t s);
 
 // Detector post-processing (nms.cu): score filter, sort, greedy NMS and scale_coords of `batch` frames of `rows` raw rows each

@@ -49,6 +49,8 @@ struct skps_pipeline {
     double* d_align_kps = nullptr; double* d_align_M = nullptr; uint8_t* d_chips = nullptr;
     // head pose (skps_pipeline_pose): allocated on first use, for top_k faces
     double* d_pose_kps = nullptr; double* d_pose = nullptr;
+    // device frames: the producer's stream is ordered before the ingest (ev_ready) and the ingest before its later work (ev_read)
+    cudaEvent_t ev_ready = nullptr, ev_read = nullptr;
 };
 
 extern "C" SKPS_API void skps_pipeline_destroy(skps_pipeline* p) {
@@ -62,6 +64,8 @@ extern "C" SKPS_API void skps_pipeline_destroy(skps_pipeline* p) {
     for (void* q : dev) if (q) cudaFree(q);
     void* host[] = {p->h_res, p->h_boxes, p->h_kps, p->h_scores, p->h_det_idx, p->h_det_rows, p->h_track};
     for (void* q : host) if (q) cudaFreeHost(q);
+    if (p->ev_ready) cudaEventDestroy(p->ev_ready);
+    if (p->ev_read) cudaEventDestroy(p->ev_read);
     delete p;
 }
 
@@ -114,6 +118,8 @@ extern "C" SKPS_API int skps_pipeline_create(skps_engine* det, skps_engine* kps,
     int32_t counts[SKPS_LANDMARK_CHUNK + 1];
     for (int i = 0; i <= SKPS_LANDMARK_CHUNK; ++i) counts[i] = i;
     SKPS_CUDA(cudaMemcpy(p->d_counts, counts, sizeof(counts), cudaMemcpyHostToDevice));
+    SKPS_CUDA(cudaEventCreateWithFlags(&p->ev_ready, cudaEventDisableTiming));
+    SKPS_CUDA(cudaEventCreateWithFlags(&p->ev_read, cudaEventDisableTiming));
     *out = p;
     return 0;
 }
@@ -124,14 +130,41 @@ extern "C" SKPS_API int skps_pipeline_reset(skps_pipeline* p) {
     return 0;
 }
 
+static int check_frame_size(const skps_pipeline* p, int H, int W) {
+    SKPS_CHECK(H > 0 && W > 0 && (size_t)H * W <= (size_t)p->cfg.max_h * p->cfg.max_w,
+               "frame %dx%d has more pixels than the pipeline maximum %dx%d", H, W, p->cfg.max_h, p->cfg.max_w);
+    return 0;
+}
+
+// Gather a [dev] frame whose rows are `pitch` bytes apart into d_frame[cur] (one skps_frame_ingest pass); with `diff`, sum
+// |frame - previous frame| into d_diff in the same pass.  With a producer stream, the read waits for the work queued on it
+// so far, and its later work waits for the read.
+static int ingest_frame(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch, bool diff, const cudaStream_t* producer,
+                        cudaStream_t s) {
+    if (check_frame_size(p, H, W)) return 1;
+    if (producer) {
+        SKPS_CUDA(cudaEventRecord(p->ev_ready, *producer));
+        SKPS_CUDA(cudaStreamWaitEvent(s, p->ev_ready, 0));
+    }
+    MpStreamDesc D = {};
+    D.cur = p->d_frame[p->cur]; D.prev = diff ? p->d_frame[p->cur ^ 1] : nullptr; D.have_prev = diff;
+    D.H = H; D.W = W; D.src = frame; D.src_pitch = pitch;
+    if (diff) SKPS_CUDA(cudaMemsetAsync(p->d_diff, 0, sizeof(unsigned long long), s));
+    if (launch_frame_ingest(D, p->d_diff, s)) return 1;
+    if (producer) {
+        SKPS_CUDA(cudaEventRecord(p->ev_read, s));
+        SKPS_CUDA(cudaStreamWaitEvent(*producer, p->ev_read, 0));
+    }
+    return 0;
+}
+
 // Upload (or adopt) the frame into d_frame[cur]; returns the device pointer.
 static int stage_frame(skps_pipeline* p, const uint8_t* frame, int H, int W, int on_device, cudaStream_t s,
                        const uint8_t** dptr) {
-    SKPS_CHECK(H > 0 && W > 0 && (size_t)H * W <= (size_t)p->cfg.max_h * p->cfg.max_w,
-               "frame %dx%d has more pixels than the pipeline maximum %dx%d", H, W, p->cfg.max_h, p->cfg.max_w);
+    if (check_frame_size(p, H, W)) return 1;
     size_t bytes = (size_t)H * W * 3;
     if (on_device) {
-        SKPS_CUDA(cudaMemcpyAsync(p->d_frame[p->cur], frame, bytes, cudaMemcpyDeviceToDevice, s));
+        if (ingest_frame(p, frame, H, W, W * 3, false, nullptr, s)) return 1;
     } else {
         // frames already in pinned (page-locked) memory go straight to the GPU; pageable frames are first copied
         // into the pipeline's pinned staging buffer so the H2D copy stays asynchronous and at full PCIe rate
@@ -147,24 +180,54 @@ static int stage_frame(skps_pipeline* p, const uint8_t* frame, int H, int W, int
     return 0;
 }
 
+// facer.py:113: np.sum(diff)/H/W/3, from the sum in d_diff.
+static int read_mean_diff(skps_pipeline* p, int H, int W, double* mean_diff, cudaStream_t s) {
+    SKPS_CUDA(cudaMemcpyAsync(&p->h_res->diff, p->d_diff, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
+    SKPS_CUDA(cudaStreamSynchronize(s));
+    *mean_diff = (double)p->h_res->diff / (double)H / (double)W / 3.0;
+    return 0;
+}
+
+// Stage and diff a [dev] frame in one ingest pass (see ingest_frame for `producer`).
+static int frame_diff_device(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch, const cudaStream_t* producer,
+                             double* mean_diff, cudaStream_t s) {
+    const bool diff = p->prev_h == H && p->prev_w == W;
+    if (ingest_frame(p, frame, H, W, pitch, diff, producer, s)) return 1;
+    if (!diff) {
+        *mean_diff = -1.0;
+        return 0;
+    }
+    return read_mean_diff(p, H, W, mean_diff, s);
+}
+
 extern "C" SKPS_API int skps_pipeline_frame_diff(skps_pipeline* p, const uint8_t* frame, int H, int W, int on_device,
                                         double* mean_diff, void* stream) {
     SKPS_CHECK(p && frame && mean_diff, "frame_diff: null argument");
     cudaStream_t s = (cudaStream_t)stream;
     SKPS_CUDA(cudaSetDevice(p->device));
+    if (on_device) return frame_diff_device(p, frame, H, W, W * 3, nullptr, mean_diff, s);
     const uint8_t* d = nullptr;
-    if (stage_frame(p, frame, H, W, on_device, s, &d)) return 1;
+    if (stage_frame(p, frame, H, W, 0, s, &d)) return 1;
     if (p->prev_h != H || p->prev_w != W) {
         *mean_diff = -1.0;
         return 0;
     }
     size_t n = (size_t)H * W * 3;
     if (skps_frame_absdiff_sum(p->d_frame[p->cur ^ 1], d, n, p->d_diff, s)) return 1;
-    SKPS_CUDA(cudaMemcpyAsync(&p->h_res->diff, p->d_diff, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-    SKPS_CUDA(cudaStreamSynchronize(s));
-    // facer.py:113: np.sum(diff)/H/W/3.
-    *mean_diff = (double)p->h_res->diff / (double)H / (double)W / 3.0;
-    return 0;
+    return read_mean_diff(p, H, W, mean_diff, s);
+}
+
+extern "C" SKPS_API int skps_pipeline_frame_diff_device(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch,
+                                                        void* producer_stream, double* mean_diff, void* stream) {
+    SKPS_CHECK(p && frame && mean_diff, "frame_diff_device: null argument");
+    SKPS_CHECK(H == 1 || pitch >= 3 * W, "frame_diff_device: row pitch %d is less than 3 x width %d", pitch, W);
+    SKPS_CUDA(cudaSetDevice(p->device));
+    cudaPointerAttributes attr;
+    SKPS_CUDA(cudaPointerGetAttributes(&attr, frame));
+    SKPS_CHECK((attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) && attr.device == p->device,
+               "frame_diff_device: the frame is not in memory of device %d", p->device);
+    const cudaStream_t producer = (cudaStream_t)producer_stream;
+    return frame_diff_device(p, frame, H, W, pitch, &producer, mean_diff, (cudaStream_t)stream);
 }
 
 // The frame staged by skps_pipeline_frame_diff becomes the "previous" frame without running the chain (FaceAna.run on

@@ -25,6 +25,12 @@ class PipelineCfg(C.Structure):
                 ("max_h", C.c_int), ("max_w", C.c_int)]
 
 
+class MpipeOutputs(C.Structure):
+    """skps_mpipe_outputs: device addresses of one batch's result buffers."""
+    _fields_ = [(name, c_vp) for name in ("n_faces", "ran_detector", "boxes", "kps", "scores", "chips", "M", "rvec", "tvec",
+                                          "euler", "reproject")]
+
+
 # name -> (restype, argtypes); every symbol include/skps_b200.h declares
 SIGNATURES = {
     "skps_last_error": (C.c_char_p, []),
@@ -81,6 +87,7 @@ SIGNATURES = {
                                    c_vp, C.c_int, c_vp, c_vp]),
     "skps_landmark_post": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_int, c_vp, c_vp]),
     "skps_frame_absdiff_sum": (C.c_int, [c_vp, c_vp, C.c_size_t, c_vp, c_vp]),
+    "skps_frame_ingest": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp]),
     "skps_pipeline_create": (C.c_int, [c_vp, c_vp, C.POINTER(PipelineCfg), C.POINTER(c_vp)]),
     "skps_pipeline_destroy": (None, [c_vp]),
     "skps_pipeline_reset": (C.c_int, [c_vp]),
@@ -97,8 +104,11 @@ SIGNATURES = {
     "skps_mpipe_dims": (C.c_int, [c_vp, c_i32p, c_i32p, c_i32p]),
     "skps_mpipe_submit": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, C.c_int, C.c_int]),
     "skps_mpipe_wait": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "skps_mpipe_submit_device": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int, C.POINTER(MpipeOutputs), c_vp]),
+    "skps_mpipe_wait_stream": (C.c_int, [c_vp, C.c_int, c_vp]),
     "skps_pipeline_commit_frame": (C.c_int, [c_vp, C.c_int, C.c_int]),
     "skps_pipeline_frame_diff": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double), c_vp]),
+    "skps_pipeline_frame_diff_device": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, C.POINTER(C.c_double), c_vp]),
     "skps_warp_affine": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
     "skps_align_faces": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp,
                                    c_vp]),
