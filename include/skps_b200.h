@@ -275,8 +275,10 @@ SKPS_API int skps_pipeline_reset(skps_pipeline* p);
 
 /* One frame, detector path of FaceAna.run (facer.py:56-68): letterbox -> detector -> NMS ->
  * judge_boxs(track) -> sort_and_filter -> crops -> landmark net -> de-normalise, with no host
- * round trip in between.  `frame` [host] (or [dev] when frame_on_device) HxWx3 uint8 BGR;
- * letterbox geometry (rw,rh,top,left,scale) is computed by the caller exactly as
+ * round trip in between.  Runs on the frame staged by skps_pipeline_frame_diff or
+ * skps_pipeline_frame_diff_device, at the size it was staged with; fails when none is staged.
+ * Afterwards that frame is the previous frame and no frame is staged.
+ * Letterbox geometry (rw,rh,top,left,scale) is computed by the caller exactly as
  * face_detector.py:51-62 does.  `track` [host] (n_track,4) float32 previous track boxes or
  * NULL.  If run_detector==0 the `track` boxes are used as the face boxes (facer.py:61).
  * top_k is 1..SKPS_MAX_TOP_K and `track` holds at most max(256, top_k) boxes.
@@ -292,8 +294,7 @@ SKPS_API int skps_pipeline_reset(skps_pipeline* p);
  * kept row indices and rows (parity checks; skps_pipeline_det_results returns all of them).
  * Memory: room for every detector row as a kept box plus the NMS workspace, about 108 bytes per
  * detector row (1.6 MB at 384x640, 15 MB at 1152x1920).  Synchronous. */
-SKPS_API int skps_pipeline_run(skps_pipeline* p, const uint8_t* frame, int H, int W, int frame_on_device,
-                      int run_detector, int rw, int rh, int top, int left, float scale,
+SKPS_API int skps_pipeline_run(skps_pipeline* p, int run_detector, int rw, int rh, int top, int left, float scale,
                       const float* track, int n_track,
                       int32_t* n_faces, float* boxes4, float* kps, float* scores,
                       int32_t* n_det, int32_t* det_idx, float* det_rows, void* stream);
@@ -303,20 +304,20 @@ SKPS_API int skps_pipeline_run(skps_pipeline* p, const uint8_t* frame, int H, in
  * rows from the device.  Synchronous. */
 SKPS_API int skps_pipeline_det_results(skps_pipeline* p, int capacity, int32_t* det_idx, float* det_rows);
 
-/* Mean absolute frame difference vs the previously submitted frame (facer.py:111-113);
- * returns -1.0 in *mean_diff when there is no previous frame of the same size. */
-SKPS_API int skps_pipeline_frame_diff(skps_pipeline* p, const uint8_t* frame, int H, int W,
-                             int frame_on_device, double* mean_diff, void* stream);
+/* Stage a frame for skps_pipeline_run / skps_pipeline_commit_frame and return its mean absolute
+ * difference to the previous frame (facer.py:111-113), or -1.0 in *mean_diff when there is no
+ * previous frame of the same size.  `frame` [host] HxWx3 uint8 BGR, pinned or pageable. */
+SKPS_API int skps_pipeline_frame_diff(skps_pipeline* p, const uint8_t* frame, int H, int W, double* mean_diff,
+                                      void* stream);
 /* skps_pipeline_frame_diff for a frame already on the pipeline's device, HxWx3 uint8 BGR with rows `pitch` bytes apart
  * (pitch >= 3W, any alignment): one skps_frame_ingest pass stages it and sums the difference.  The frame is read after all
  * work queued on `producer_stream` before this call (the stream that wrote it; 0 is the legacy default stream), and work
- * queued on producer_stream after this call returns runs after the read, so the producer may overwrite the frame at once.
- * skps_pipeline_run(frame = NULL, ...) then runs on the staged copy. */
+ * queued on producer_stream after this call returns runs after the read, so the producer may overwrite the frame at once. */
 SKPS_API int skps_pipeline_frame_diff_device(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch,
                                              void* producer_stream, double* mean_diff, void* stream);
-/* Adopt the frame staged by skps_pipeline_frame_diff as the previous frame without running the chain: the skip path of
- * FaceAna.run (facer.py:57-62 replaces previous_image on every call, also when nothing is detected or tracked). */
-SKPS_API int skps_pipeline_commit_frame(skps_pipeline* p, int H, int W);
+/* Adopt the staged frame as the previous frame without running the chain: the skip path of FaceAna.run (facer.py:57-62
+ * replaces previous_image on every call, also when nothing is detected or tracked).  Fails when no frame is staged. */
+SKPS_API int skps_pipeline_commit_frame(skps_pipeline* p);
 
 /* WFLW evaluation helpers (TRAIN/face_landmark/tools/eval_WFLW.py).  skps_crop_rect: zero-bordered rectangular crop of a
  * [dev] BGR frame resized to out_hw x out_hw, bit-exact with copyMakeBorder + slicing + cv2.resize (:38-80, :113-124).
@@ -348,11 +349,11 @@ SKPS_API void skps_mpipe_destroy(skps_mpipe* p);
 /* FaceAna.reset() for one stream (or all: stream = -1): forget the previous frame, the track boxes, the landmark history. */
 SKPS_API int skps_mpipe_reset(skps_mpipe* p, int stream);
 SKPS_API int skps_mpipe_dims(const skps_mpipe* p, int* n_streams, int* top_k, int* n_points);
-/* Enqueue frame i (HxWx3 uint8 BGR, [host] pinned or pageable, or [dev]) of stream i for i < n; hw = {H0,W0,H1,W1,...}.
+/* Enqueue frame i (HxWx3 uint8 BGR, [host] pinned or pageable) of stream i for i < n; hw = {H0,W0,H1,W1,...}.
  * slot in {0,1}: submit(0) submit(1) wait(0) submit(0) ... keeps two batches in flight (uploads overlap compute).
- * Pinned frames must stay valid until skps_mpipe_wait(slot).  Asynchronous. */
-SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot, const uint8_t* const* frames, const int32_t* hw, int n,
-                               int frames_on_device);
+ * Pinned frames must stay valid until skps_mpipe_wait(slot).  Frames on the device go through skps_mpipe_submit_device.
+ * Asynchronous. */
+SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot, const uint8_t* const* frames, const int32_t* hw, int n);
 /* Block until the slot's results are in host memory.  Per stream s < n: n_faces[s]; boxes (n, top_k, 4) float64 = the
  * refreshed track boxes (the 'box' entries of FaceAna.run); kps (n, top_k, n_points, 2) float64 smoothed landmarks;
  * scores (n, top_k, n_points) float32; ran_detector[s] (may be NULL) = the frame-difference gate's decision. */

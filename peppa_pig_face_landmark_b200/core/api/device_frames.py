@@ -1,7 +1,18 @@
-"""Frames already in GPU memory (a decoder surface, a tensor from NVDEC / DALI / torchvision, an ROI view of either): the
-layout FaceAna.run and FaceAnaStreams.submit accept, checked before anything is enqueued.  Pixels stay HxWx3 uint8 BGR as
-the reference's run(image) takes them; only where the frame lives and its row pitch differ from a numpy frame."""
+"""The frames FaceAna.run and FaceAnaStreams.submit accept, checked before anything is enqueued: numpy arrays, and frames
+already in GPU memory (a decoder surface, a tensor from NVDEC / DALI / torchvision, an ROI view of either).  Pixels stay
+HxWx3 uint8 BGR as the reference's run(image) takes them; only where the frame lives and its row pitch differ between the
+two."""
 import sys
+
+import numpy as np
+
+
+def check_host_frame(frame):
+    """`frame` as a C-contiguous numpy array; ValueError unless it is an HxWx3 uint8 image."""
+    frame = np.ascontiguousarray(frame)
+    if frame.dtype != np.uint8 or frame.ndim != 3 or frame.shape[2] != 3:
+        raise ValueError("expected an HxWx3 uint8 BGR image, got %s %s" % (frame.dtype, frame.shape))
+    return frame
 
 
 def is_cuda_tensor(x):

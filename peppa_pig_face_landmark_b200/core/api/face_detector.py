@@ -13,6 +13,7 @@ import numpy as np
 from ... import runtime as rt
 from ...graph_tools import detector_onnx_for
 from ...logger.logger import logger
+from .device_frames import check_host_frame
 from .onnx_model_base import ONNXEngine
 
 
@@ -59,10 +60,7 @@ class FaceDetector:
     # ------------------------------------------------------------------
     def _upload(self, image):
         torch = rt.require_cuda()
-        image = np.ascontiguousarray(image)
-        if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
-            raise ValueError("expected an HxWx3 uint8 BGR image, got %s %s" % (image.dtype, image.shape))
-        return torch.from_numpy(image).to(self.model.device, non_blocking=False)
+        return torch.from_numpy(check_host_frame(image)).to(self.model.device, non_blocking=False)
 
     def _letterbox_device(self, frame_dev, h, w):
         in_h, in_w = self.input_size[0], self.input_size[1]

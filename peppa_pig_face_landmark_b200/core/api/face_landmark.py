@@ -14,6 +14,14 @@ from ... import runtime as rt
 from ...logger.logger import logger
 from .onnx_model_base import ONNXEngine
 
+MIN_FACE = 20              # face_landmark.py:26,76: boxes with a side of at most this many pixels get no landmarks
+
+
+def face_scale(cfg):
+    """Crop side over box side, float32(1 + 2 * base_extend_range[0]) (face_landmark.py:83 in float32); cfg: Skps.yml's
+    Keypoints section."""
+    return float(np.float32(1 + 2 * cfg['base_extend_range'][0]))
+
 
 class FaceLandmark:
     def __init__(self, cfg, max_faces=16):
@@ -21,11 +29,11 @@ class FaceLandmark:
         model_path = os.path.join(root_path, cfg['model_path'])
         self.max_faces = int(max_faces)
         self.model = ONNXEngine(model_path, max_batch=self.max_faces)
-        self.min_face = 20
+        self.min_face = MIN_FACE
         self.keypoints_num = cfg['num_points']
         self.input_size = cfg['input_shape']
         self.extend = cfg['base_extend_range']
-        self.face_scale = float(np.float32(1 + 2 * self.extend[0]))      # face_landmark.py:83 in float32
+        self.face_scale = face_scale(cfg)
         self.lib = rt.load_library()
         torch = rt.require_cuda()
         dev = self.model.device

@@ -18,9 +18,9 @@ from ...graph_tools import check_detector_input
 from ...logger.logger import logger
 from ..smoother.lk import EmaFilter, GroupTrack, first_match, rects
 from .face_detector import FaceDetector, letterbox_geometry
-from .face_landmark import FaceLandmark
+from .face_landmark import MIN_FACE, FaceLandmark, face_scale
 from .align import check_size
-from .device_frames import check_cuda_frame, is_cuda_tensor
+from .device_frames import check_cuda_frame, check_host_frame, is_cuda_tensor
 
 
 MAX_TOP_K = 1024           # SKPS_MAX_TOP_K of include/skps_b200.h
@@ -32,6 +32,15 @@ def get_cfg():
     cfg_path = os.path.join(root_path, 'config', 'Skps.yml')
     with open(cfg_path, encoding="UTF-8") as f:
         return yaml.load(f, Loader=yaml.FullLoader)
+
+
+def pipeline_cfg(cfg, top_k, max_frame_hw):
+    """The skps_pipeline_cfg of FaceAna and FaceAnaStreams from Skps.yml's Skps section."""
+    det, trace = cfg['Detect'], cfg['Trace']
+    return rt.PipelineCfg(score_thres=det['score_thrs'], iou_thres=det['iou_thrs'], min_face=float(det['min_face']),
+                          top_k=int(top_k), track_iou=float(trace['iou_thres']), alpha=float(trace['smooth_box']),
+                          face_scale=face_scale(cfg['Keypoints']), kps_min_face=float(MIN_FACE),
+                          max_h=int(max_frame_hw[0]), max_w=int(max_frame_hw[1]))
 
 
 class FaceAna():
@@ -52,6 +61,7 @@ class FaceAna():
         self.top_k = int(top_k if top_k is not None else cfg['Skps']['Detect']['topk'])
         if not 1 <= self.top_k <= MAX_TOP_K:
             raise ValueError("top_k %d outside 1..%d" % (self.top_k, MAX_TOP_K))
+        pc = pipeline_cfg(cfg['Skps'], self.top_k, max_frame_hw)
         if det_input is not None:
             det_input = check_detector_input(det_input)
         self.align = None if align is None else check_size(align)
@@ -75,10 +85,6 @@ class FaceAna():
 
         self.lib = rt.load_library()
         det, kps = self.face_detector, self.face_landmark
-        pc = rt.PipelineCfg(score_thres=det.score_thrs, iou_thres=det.iou_thrs, min_face=float(self.min_face),
-                            top_k=self.top_k, track_iou=float(self.iou_thres), alpha=float(self.alpha),
-                            face_scale=kps.face_scale, kps_min_face=float(kps.min_face),
-                            max_h=int(max_frame_hw[0]), max_w=int(max_frame_hw[1]))
         h = C.c_void_p()
         rt.check(self.lib.skps_pipeline_create(det.model.handle, kps.model.handle, C.byref(pc), C.byref(h)))
         self._pipe = h
@@ -111,14 +117,9 @@ class FaceAna():
         those of image.cpu().numpy() bit for bit.  Ordering on torch.cuda.current_stream(): the frame is read after all
         work already queued on it, and work queued on it after run() returns runs after the frame has been read, so a
         decoder may overwrite the surface at once."""
-        if is_cuda_tensor(image):
-            H, W, _ = check_cuda_frame(image, self._device, self._max_hw)
-        else:
-            image = np.ascontiguousarray(image)
-            if image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] != 3:
-                raise ValueError("expected an HxWx3 uint8 BGR image, got %s %s" % (image.dtype, image.shape))
-            H, W = image.shape[:2]
-        run_det = self.diff_frames(self.previous_image, image)     # stages the frame on the device
+        image = image if is_cuda_tensor(image) else check_host_frame(image)
+        run_det = self.diff_frames(self.previous_image, image)     # checks a CUDA frame, stages the frame on the device
+        H, W = image.shape[:2]
         self.previous_image = image
         det = self.face_detector
         in_h, in_w = det.input_size[0], det.input_size[1]
@@ -132,13 +133,12 @@ class FaceAna():
             # facer.py:61 with an empty/None track: nothing to do (the reference would fail on None)
             boxes_return = np.zeros((0, 4), np.float32)
             landmarks, states = np.array([]), np.array([])
-            rt.check(self.lib.skps_pipeline_commit_frame(self._pipe, H, W))     # the staged frame is the new "previous"
+            rt.check(self.lib.skps_pipeline_commit_frame(self._pipe))     # the staged frame is the new "previous"
         else:
             rt.check(self.lib.skps_pipeline_run(
-                self._pipe, None, H, W, 0, 1 if run_det else 0, rw, rh, top, left, float(scale),
-                rt.ptr(track32), n_track, C.byref(self._n), self._boxes.ctypes.data, self._kps.ctypes.data,
-                self._scores.ctypes.data, C.byref(self._ndet), self._det_idx.ctypes.data,
-                self._det_rows.ctypes.data, self._stream.cuda_stream))
+                self._pipe, 1 if run_det else 0, rw, rh, top, left, float(scale), rt.ptr(track32), n_track, C.byref(self._n),
+                self._boxes.ctypes.data, self._kps.ctypes.data, self._scores.ctypes.data, C.byref(self._ndet),
+                self._det_idx.ctypes.data, self._det_rows.ctypes.data, self._stream.cuda_stream))
             n = self._n.value
             boxes_return = self._boxes[:n].copy()
             landmarks = self._kps[:n].copy() if n else np.array([])
@@ -204,8 +204,7 @@ class FaceAna():
                                                               torch.cuda.current_stream(self._device).cuda_stream,
                                                               C.byref(d), self._stream.cuda_stream))
         else:
-            H, W = image.shape[:2]
-            rt.check(self.lib.skps_pipeline_frame_diff(self._pipe, image.ctypes.data, H, W, 0, C.byref(d),
+            rt.check(self.lib.skps_pipeline_frame_diff(self._pipe, image.ctypes.data, *image.shape[:2], C.byref(d),
                                                        self._stream.cuda_stream))
         if previous_frame is None or d.value < 0:
             return True

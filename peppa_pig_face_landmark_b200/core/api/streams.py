@@ -24,8 +24,8 @@ import numpy as np
 from ... import runtime as rt
 from ...graph_tools import check_detector_input, detector_onnx_for
 from .align import check_size
-from .device_frames import check_cuda_frame, is_cuda_tensor
-from .facer import get_cfg
+from .device_frames import check_cuda_frame, check_host_frame, is_cuda_tensor
+from .facer import get_cfg, pipeline_cfg
 from .onnx_model_base import ONNXEngine
 
 
@@ -42,7 +42,7 @@ class FaceAnaStreams:
         self.align = None if align is None else check_size(align)
         self.pose = bool(pose)
         cfg = get_cfg()['Skps']
-        det_cfg, kps_cfg, tr_cfg = cfg['Detect'], cfg['Keypoints'], cfg['Trace']
+        det_cfg, kps_cfg = cfg['Detect'], cfg['Keypoints']
         self.n_streams = int(n_streams)
         self.top_k = int(top_k if top_k is not None else det_cfg['topk'])
         if not 1 <= self.top_k <= 64:
@@ -50,6 +50,7 @@ class FaceAnaStreams:
             # top_k bounds its memory (about 47 MB per face); FaceAna takes up to 1024
             raise ValueError("FaceAnaStreams: top_k %d outside 1..64 (the landmark batch is n_streams * top_k faces; "
                              "FaceAna takes up to 1024)" % self.top_k)
+        pc = pipeline_cfg(cfg, self.top_k, max_frame_hw)
         root = pathlib.Path(__file__).resolve().parents[2]
         det_hw = det_cfg['input_shape'][:2] if det_input is None else check_detector_input(det_input)
         self.det = ONNXEngine(detector_onnx_for(os.path.join(root, det_cfg['model_path']), det_hw), device=device,
@@ -60,11 +61,6 @@ class FaceAnaStreams:
         self.device = self.det.device
         self.max_frame_hw = (int(max_frame_hw[0]), int(max_frame_hw[1]))
         self.lib = rt.load_library()
-        pc = rt.PipelineCfg(score_thres=det_cfg['score_thrs'], iou_thres=det_cfg['iou_thrs'],
-                            min_face=float(det_cfg['min_face']), top_k=self.top_k, track_iou=float(tr_cfg['iou_thres']),
-                            alpha=float(tr_cfg['smooth_box']),
-                            face_scale=float(np.float32(1 + 2 * kps_cfg['base_extend_range'][0])), kps_min_face=20.0,
-                            max_h=int(max_frame_hw[0]), max_w=int(max_frame_hw[1]))
         h = C.c_void_p()
         rt.check(self.lib.skps_mpipe_create(self.det.handle, self.kps.handle, C.byref(pc), self.n_streams, C.byref(h)))
         self._h = h
@@ -124,16 +120,11 @@ class FaceAnaStreams:
             return
         if out is not None:
             raise ValueError("out= keeps results on the GPU and takes CUDA frames; these are host frames")
-        keep = []
-        for f in frames:
-            f = np.ascontiguousarray(f)
-            if f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3:
-                raise ValueError("expected HxWx3 uint8 BGR images, got %s %s" % (f.dtype, f.shape))
-            keep.append(f)
+        keep = [check_host_frame(f) for f in frames]
         ptrs = (C.c_void_p * n)(*[f.ctypes.data for f in keep])
         hw = np.array([[f.shape[0], f.shape[1]] for f in keep], np.int32)
         slot = self._next
-        rt.check(self.lib.skps_mpipe_submit(self._h, slot, ptrs, hw.ctypes.data, n, 0))
+        rt.check(self.lib.skps_mpipe_submit(self._h, slot, ptrs, hw.ctypes.data, n))
         self._pending.append((slot, n, keep, None))
         self._next ^= 1
 

@@ -102,6 +102,30 @@ const char* get_error();
         }                                     \
     } while (0)
 
+// The fail-and-destroy lambdas of the *_create functions report a failed step as "<fn>: <what>: <error set by the step>".
+inline void prefix_error(const char* fn, const char* what) {
+    char tmp[900];
+    snprintf(tmp, sizeof(tmp), "%s", get_error());
+    set_error("%s: %s: %s", fn, what, tmp);
+}
+
+// Allocations of a *_create function that owns a fail-and-destroy lambda `fail(what)`: on failure the size is recorded and
+// fail("alloc") frees everything allocated so far.
+#define SKPS_DEV_ALLOC(ptr, bytes)                                                                                  \
+    do {                                                                                                            \
+        if (cudaMalloc((void**)&(ptr), (bytes)) != cudaSuccess) {                                                   \
+            skps::set_error("cudaMalloc %zu bytes", (size_t)(bytes));                                               \
+            return fail("alloc");                                                                                   \
+        }                                                                                                           \
+    } while (0)
+#define SKPS_HOST_ALLOC(ptr, bytes)                                                                                 \
+    do {                                                                                                            \
+        if (cudaMallocHost((void**)&(ptr), (bytes)) != cudaSuccess) {                                               \
+            skps::set_error("cudaMallocHost %zu bytes", (size_t)(bytes));                                           \
+            return fail("alloc");                                                                                   \
+        }                                                                                                           \
+    } while (0)
+
 // ---- activation (device) -------------------------------------------------------------------
 // HardSigmoid follows ONNX: max(0, min(1, alpha*x + beta)) with alpha = float32(1/6), beta = 0.5
 // (kps_student.onnx node 2 etc.); alpha*x+beta is evaluated as mul then add (no FMA) to match a

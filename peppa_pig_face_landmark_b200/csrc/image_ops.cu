@@ -2,6 +2,8 @@
 // with cv2.resize INTER_LINEAR on uint8), face selection (IoU track match + EMA, area filter, top-k), landmark
 // de-normalisation and the frame-difference gate.  All HBM-bound byte/index work; compiled with
 // -fmad=false so float32 expressions round exactly like the numpy expressions they restate.
+#include <string.h>
+
 #include "../../include/skps_b200.h"
 #include "common.h"
 #include "mpipe_kernels.h"
@@ -583,6 +585,24 @@ int launch_frame_ingest(const MpStreamDesc& one, unsigned long long* diff, cudaS
     mp_absdiff_kernel<<<dim3(absdiff_grid(bytes), 1), 256, 0, s>>>(nullptr, one, diff);
     SKPS_CUDA(cudaGetLastError());
     return 0;
+}
+int upload_host_frame(const uint8_t* frame, size_t bytes, uint8_t* stage, uint8_t* dst, cudaStream_t s) {
+    cudaPointerAttributes attr;
+    const bool pinned = cudaPointerGetAttributes(&attr, frame) == cudaSuccess && attr.type == cudaMemoryTypeHost;
+    if (!pinned) {
+        cudaGetLastError();          // clear the "invalid value" a pageable pointer may leave behind
+        memcpy(stage, frame, bytes);
+    }
+    SKPS_CUDA(cudaMemcpyAsync(dst, pinned ? frame : stage, bytes, cudaMemcpyHostToDevice, s));
+    return 0;
+}
+int check_device_frame(const void* frame, int device, const char* fn, int index) {
+    cudaPointerAttributes attr;
+    SKPS_CUDA(cudaPointerGetAttributes(&attr, frame));
+    if ((attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) && attr.device == device) return 0;
+    if (index < 0) set_error("%s: the frame is not in memory of device %d", fn, device);
+    else set_error("%s: frame %d is not in memory of device %d", fn, index, device);
+    return 1;
 }
 int launch_mp_letterbox(const MpStreamDesc* d, uint8_t* out, size_t out_stride, int in_h, int in_w, int n, cudaStream_t s) {
     mp_letterbox_kernel<<<dim3((in_w + 255) / 256, in_h, n), 256, 0, s>>>(d, out, out_stride, in_h, in_w);

@@ -136,9 +136,7 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
     p->P = skps_engine_output_elems(kps, 1);
     cudaGetDevice(&p->device);
     auto fail = [&](const char* what) {
-        char tmp[900];
-        snprintf(tmp, sizeof(tmp), "%s", get_error());
-        set_error("mpipe_create: %s: %s", what, tmp);
+        prefix_error("mpipe_create", what);
         skps_mpipe_destroy(p);
         return 1;
     };
@@ -150,34 +148,33 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
     p->frame_bytes = ((size_t)cfg->max_h * cfg->max_w * 3 + 255) & ~(size_t)255;
     p->ring_pos.assign(S, 0); p->prev_h.assign(S, 0); p->prev_w.assign(S, 0);
     p->d_frame.assign((size_t)S * 3, nullptr);
-#define MP_DEV(ptr, bytes) if (cudaMalloc((void**)&(ptr), (bytes)) != cudaSuccess) { set_error("cudaMalloc %zu bytes", (size_t)(bytes)); return fail("alloc"); }
-#define MP_HOST(ptr, bytes) if (cudaMallocHost((void**)&(ptr), (bytes)) != cudaSuccess) { set_error("cudaMallocHost %zu bytes", (size_t)(bytes)); return fail("alloc"); }
-    for (auto& f : p->d_frame) MP_DEV(f, p->frame_bytes);
+    for (auto& f : p->d_frame) SKPS_DEV_ALLOC(f, p->frame_bytes);
     for (auto& sl : p->slot) {
-        MP_HOST(sl.h_stage, p->frame_bytes * S);
-        MP_HOST(sl.h_hw, sizeof(int32_t) * 2 * S); MP_HOST(sl.h_have_prev, sizeof(int32_t) * S);
-        MP_HOST(sl.h_geom, sizeof(int32_t) * 8 * S);
-        MP_HOST(sl.h_desc, sizeof(MpStreamDesc) * S);
-        MP_HOST(sl.h_count, sizeof(int32_t) * S); MP_HOST(sl.h_flag, sizeof(int32_t) * S);
-        MP_HOST(sl.h_box, sizeof(double) * 4 * K * S); MP_HOST(sl.h_kps, sizeof(double) * 2 * P * K * S);
-        MP_HOST(sl.h_scores, sizeof(float) * P * K * S);
+        SKPS_HOST_ALLOC(sl.h_stage, p->frame_bytes * S);
+        SKPS_HOST_ALLOC(sl.h_hw, sizeof(int32_t) * 2 * S); SKPS_HOST_ALLOC(sl.h_have_prev, sizeof(int32_t) * S);
+        SKPS_HOST_ALLOC(sl.h_geom, sizeof(int32_t) * 8 * S);
+        SKPS_HOST_ALLOC(sl.h_desc, sizeof(MpStreamDesc) * S);
+        SKPS_HOST_ALLOC(sl.h_count, sizeof(int32_t) * S); SKPS_HOST_ALLOC(sl.h_flag, sizeof(int32_t) * S);
+        SKPS_HOST_ALLOC(sl.h_box, sizeof(double) * 4 * K * S); SKPS_HOST_ALLOC(sl.h_kps, sizeof(double) * 2 * P * K * S);
+        SKPS_HOST_ALLOC(sl.h_scores, sizeof(float) * P * K * S);
         if (cudaEventCreateWithFlags(&sl.ev_in, cudaEventDisableTiming) != cudaSuccess ||
             cudaEventCreateWithFlags(&sl.ev_done, cudaEventDisableTiming) != cudaSuccess ||
             cudaEventCreateWithFlags(&sl.ev_staged, cudaEventDisableTiming) != cudaSuccess) { set_error("cudaEventCreate"); return fail("event"); }
     }
     if (cudaEventCreateWithFlags(&p->ev_ready, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&p->ev_read, cudaEventDisableTiming) != cudaSuccess) { set_error("cudaEventCreate"); return fail("event"); }
-    MP_DEV(p->d_desc, sizeof(MpStreamDesc) * S); MP_DEV(p->d_hw, 8 * S); MP_DEV(p->d_have_prev, 4 * S); MP_DEV(p->d_flag, 4 * S); MP_DEV(p->d_det_count, 4 * S);
-    MP_DEV(p->d_det_idx, 4 * (size_t)p->det_rows * S); MP_DEV(p->d_count, 4 * S); MP_DEV(p->d_detail, 4 * 5 * (size_t)K * S);
-    MP_DEV(p->d_diff, 8 * S); MP_DEV(p->d_det_rows, 4 * 16 * (size_t)p->det_rows * S);
-    MP_DEV(p->d_nms_ws, nms_workspace_bytes(p->det_rows, S)); MP_DEV(p->d_boxes, 4 * 4 * (size_t)K * S);
-    MP_DEV(p->d_kps_now, 4 * 2 * (size_t)P * K * S);
-    MP_DEV(p->d_prev_lm, 8 * 2 * 2 * (size_t)P * K * S); MP_DEV(p->d_prev_dx, 8 * 2 * 2 * (size_t)P * K * S);
-    MP_DEV(p->d_track, 8 * 4 * (size_t)K * S); MP_DEV(p->d_out_kps, 8 * 2 * (size_t)P * K * S);
-    MP_DEV(p->d_track_f32, 4 * 4 * (size_t)K * S);
-    MP_DEV(p->d_n_prev, 4 * S); MP_DEV(p->d_prev_f32, 4 * S); MP_DEV(p->d_state_idx, 4 * S); MP_DEV(p->d_n_track, 4 * S);
-#undef MP_DEV
-#undef MP_HOST
+    SKPS_DEV_ALLOC(p->d_desc, sizeof(MpStreamDesc) * S); SKPS_DEV_ALLOC(p->d_hw, 8 * S); SKPS_DEV_ALLOC(p->d_have_prev, 4 * S);
+    SKPS_DEV_ALLOC(p->d_flag, 4 * S); SKPS_DEV_ALLOC(p->d_det_count, 4 * S);
+    SKPS_DEV_ALLOC(p->d_det_idx, 4 * (size_t)p->det_rows * S); SKPS_DEV_ALLOC(p->d_count, 4 * S);
+    SKPS_DEV_ALLOC(p->d_detail, 4 * 5 * (size_t)K * S);
+    SKPS_DEV_ALLOC(p->d_diff, 8 * S); SKPS_DEV_ALLOC(p->d_det_rows, 4 * 16 * (size_t)p->det_rows * S);
+    SKPS_DEV_ALLOC(p->d_nms_ws, nms_workspace_bytes(p->det_rows, S)); SKPS_DEV_ALLOC(p->d_boxes, 4 * 4 * (size_t)K * S);
+    SKPS_DEV_ALLOC(p->d_kps_now, 4 * 2 * (size_t)P * K * S);
+    SKPS_DEV_ALLOC(p->d_prev_lm, 8 * 2 * 2 * (size_t)P * K * S); SKPS_DEV_ALLOC(p->d_prev_dx, 8 * 2 * 2 * (size_t)P * K * S);
+    SKPS_DEV_ALLOC(p->d_track, 8 * 4 * (size_t)K * S); SKPS_DEV_ALLOC(p->d_out_kps, 8 * 2 * (size_t)P * K * S);
+    SKPS_DEV_ALLOC(p->d_track_f32, 4 * 4 * (size_t)K * S);
+    SKPS_DEV_ALLOC(p->d_n_prev, 4 * S); SKPS_DEV_ALLOC(p->d_prev_f32, 4 * S); SKPS_DEV_ALLOC(p->d_state_idx, 4 * S);
+    SKPS_DEV_ALLOC(p->d_n_track, 4 * S);
     cudaMemset(p->d_prev_lm, 0, 8 * 2 * 2 * (size_t)P * K * S); cudaMemset(p->d_prev_dx, 0, 8 * 2 * 2 * (size_t)P * K * S);
     cudaMemset(p->d_state_idx, 0, 4 * S); cudaMemset(p->d_track_f32, 0, 4 * 4 * (size_t)K * S);
     cudaMemset(p->d_track, 0, 8 * 4 * (size_t)K * S);
@@ -188,11 +185,13 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
     return 0;
 }
 
-// One batch.  Host frames are uploaded on the copy stream into the next ring position; device frames (rows pitches[i]
-// bytes apart, or 3W when pitches is null) are gathered there by the mp_absdiff launch on the compute stream, after the
-// work queued on *producer (when given).  out: results into caller buffers on the device instead of the slot's pinned ones.
-static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* pitches, const int32_t* hw,
-                        int n, bool on_device, const skps_mpipe_outputs* out, const cudaStream_t* producer) {
+// One batch.  Host frames (pitches null) are uploaded on the copy stream into the next ring position; device frames (rows
+// pitches[i] bytes apart) are gathered there by the mp_absdiff launch on the compute stream, after the work queued on
+// `producer`, whose later work waits for that launch.  out: results into caller buffers on the device instead of the slot's
+// pinned ones.
+static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* hw, int n,
+                        const int32_t* pitches, cudaStream_t producer, const skps_mpipe_outputs* out) {
+    const bool on_device = pitches != nullptr;
     SKPS_CHECK(p && frames && hw && (slot_i == 0 || slot_i == 1) && n > 0 && n <= p->S, "mpipe_submit: bad arguments");
     skps_mpipe::Slot& sl = p->slot[slot_i];
     SKPS_CHECK(!sl.busy, "mpipe_submit: slot %d still holds results (call skps_mpipe_wait first)", slot_i);
@@ -215,31 +214,22 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
         const int H = hw[2 * s], W = hw[2 * s + 1];
         SKPS_CHECK(frames[s] && H > 0 && W > 0 && (size_t)H * W * 3 <= p->frame_bytes,
                    "mpipe_submit: frame %d is %dx%d, larger than the pipeline maximum %dx%d", s, H, W, c.max_h, c.max_w);
-        SKPS_CHECK(!pitches || H == 1 || pitches[s] >= 3 * W, "mpipe_submit: frame %d has row pitch %d, less than 3 x width %d",
-                   s, pitches ? pitches[s] : 0, W);
-        const size_t bytes = (size_t)H * W * 3;
-        const int pos = (p->ring_pos[s] + 1) % 3;
-        uint8_t* dst = p->d_frame[(size_t)s * 3 + pos];
-        if (!on_device) {
-            cudaPointerAttributes attr;
-            const bool pinned = cudaPointerGetAttributes(&attr, frames[s]) == cudaSuccess && attr.type == cudaMemoryTypeHost;
-            const uint8_t* src = frames[s];
-            if (!pinned) {
-                cudaGetLastError();
-                memcpy(sl.h_stage + p->frame_bytes * s, frames[s], bytes);
-                src = sl.h_stage + p->frame_bytes * s;
-            }
-            SKPS_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, sc));
+        if (on_device) {
+            SKPS_CHECK(H == 1 || pitches[s] >= 3 * W, "mpipe_submit: frame %d has row pitch %d, less than 3 x width %d", s,
+                       pitches[s], W);
+        } else if (upload_host_frame(frames[s], (size_t)H * W * 3, sl.h_stage + p->frame_bytes * s,
+                                     p->d_frame[(size_t)s * 3 + (p->ring_pos[s] + 1) % 3], sc)) {
+            return 1;
         }
         sl.h_hw[2 * s] = H; sl.h_hw[2 * s + 1] = W;
         sl.h_have_prev[s] = (p->prev_h[s] == H && p->prev_w[s] == W) ? 1 : 0;
     }
-    if (!on_device) {
+    if (on_device) {
+        SKPS_CUDA(cudaEventRecord(p->ev_ready, producer));
+        SKPS_CUDA(cudaStreamWaitEvent(sx, p->ev_ready, 0));
+    } else {
         SKPS_CUDA(cudaEventRecord(sl.ev_in, sc));
         SKPS_CUDA(cudaStreamWaitEvent(sx, sl.ev_in, 0));
-    } else if (producer) {
-        SKPS_CUDA(cudaEventRecord(p->ev_ready, *producer));
-        SKPS_CUDA(cudaStreamWaitEvent(sx, p->ev_ready, 0));
     }
     // ---- compute
     SKPS_CUDA(cudaMemcpyAsync(p->d_hw, sl.h_hw, 8 * n, cudaMemcpyHostToDevice, sx));
@@ -257,7 +247,7 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
         D.prev = sl.h_have_prev[s] ? p->d_frame[(size_t)s * 3 + p->ring_pos[s]] : nullptr;
         D.H = H; D.W = W; D.have_prev = sl.h_have_prev[s];
         D.src = on_device ? frames[s] : nullptr;
-        D.src_pitch = pitches ? pitches[s] : W * 3;
+        D.src_pitch = on_device ? pitches[s] : W * 3;
         letterbox_geometry(H, W, p->det_h, p->det_w, &D.scale, &D.rw, &D.rh, &D.top, &D.left);
         memcpy(&sl.h_geom[8 * s], &D.scale, 4); sl.h_geom[8 * s + 1] = D.top; sl.h_geom[8 * s + 2] = D.left;
         if ((size_t)H * W * 3 > max_bytes) max_bytes = (size_t)H * W * 3;
@@ -265,9 +255,9 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     SKPS_CUDA(cudaMemcpyAsync(p->d_desc, sl.h_desc, sizeof(MpStreamDesc) * n, cudaMemcpyHostToDevice, sx));
     SKPS_CUDA(cudaEventRecord(sl.ev_staged, sx));
     if (launch_mp_absdiff(p->d_desc, p->d_diff, n, max_bytes, sx)) return 1;
-    if (on_device && producer) {
+    if (on_device) {
         SKPS_CUDA(cudaEventRecord(p->ev_read, sx));
-        SKPS_CUDA(cudaStreamWaitEvent(*producer, p->ev_read, 0));
+        SKPS_CUDA(cudaStreamWaitEvent(producer, p->ev_read, 0));
     }
     // results: D2H into the slot's pinned buffers, or D2D into the caller's; either way before the next batch on sx can
     // overwrite d_out_kps, the engine's score output or the chips
@@ -352,23 +342,17 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     return 0;
 }
 
-extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* hw, int n,
-                                          int frames_on_device) {
-    return submit_batch(p, slot_i, frames, nullptr, hw, n, frames_on_device != 0, nullptr, nullptr);
+extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* hw, int n) {
+    return submit_batch(p, slot_i, frames, hw, n, nullptr, nullptr, nullptr);
 }
 
 extern "C" SKPS_API int skps_mpipe_submit_device(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* pitches,
                                                  const int32_t* hw, int n, const skps_mpipe_outputs* out, void* producer_stream) {
     SKPS_CHECK(p && frames && pitches && hw && n > 0 && n <= p->S, "mpipe_submit_device: bad arguments");
     SKPS_CUDA(cudaSetDevice(p->device));
-    for (int s = 0; s < n; ++s) {
-        cudaPointerAttributes attr;
-        SKPS_CUDA(cudaPointerGetAttributes(&attr, frames[s]));
-        SKPS_CHECK((attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) && attr.device == p->device,
-                   "mpipe_submit_device: frame %d is not in memory of device %d", s, p->device);
-    }
-    const cudaStream_t producer = (cudaStream_t)producer_stream;
-    return submit_batch(p, slot_i, frames, pitches, hw, n, true, out, &producer);
+    for (int s = 0; s < n; ++s)
+        if (check_device_frame(frames[s], p->device, "mpipe_submit_device", s)) return 1;
+    return submit_batch(p, slot_i, frames, hw, n, pitches, (cudaStream_t)producer_stream, out);
 }
 
 extern "C" SKPS_API int skps_mpipe_wait_stream(skps_mpipe* p, int slot_i, void* consumer_stream) {

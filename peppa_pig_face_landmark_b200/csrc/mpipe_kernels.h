@@ -44,6 +44,12 @@ struct MpStreamDesc {
 // runs the same kernel on one descriptor passed by value (diff = one counter, zeroed by the caller).
 int launch_mp_absdiff(const MpStreamDesc* d, unsigned long long* diff, int n, size_t max_bytes, cudaStream_t s);
 int launch_frame_ingest(const MpStreamDesc& one, unsigned long long* diff, cudaStream_t s);
+// Frame staging on the host side, shared by skps_pipeline and skps_mpipe.  upload_host_frame queues the H2D copy of a [host]
+// frame of `bytes` bytes into dst on s: a pinned frame is copied as it is, a pageable one first into `stage` (pinned, at
+// least `bytes`) so that the copy stays asynchronous and at full PCIe rate.  check_device_frame fails unless `frame` is
+// device or managed memory of `device`; the error names the caller `fn` and, for index >= 0, the frame's index.
+int upload_host_frame(const uint8_t* frame, size_t bytes, uint8_t* stage, uint8_t* dst, cudaStream_t s);
+int check_device_frame(const void* frame, int device, const char* fn, int index);
 int launch_mp_letterbox(const MpStreamDesc* d, uint8_t* out, size_t out_stride, int in_h, int in_w, int n, cudaStream_t s);
 
 // Detector post-processing (nms.cu): score filter, sort, greedy NMS and scale_coords of `batch` frames of `rows` raw rows each

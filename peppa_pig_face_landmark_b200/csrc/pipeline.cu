@@ -27,6 +27,7 @@ struct skps_pipeline {
     void* d_nms_ws = nullptr;                     // NMS workspace for det_rows candidates
     uint8_t* d_frame[2] = {nullptr, nullptr};     // current / previous frame
     int cur = 0;
+    int cur_h = 0, cur_w = 0;                     // size of the frame staged in d_frame[cur] by frame_diff* (0 = none)
     int prev_h = 0, prev_w = 0;                   // size of the frame in d_frame[cur^1] (0 = none)
     uint8_t* h_frame = nullptr;                   // pinned staging
     float* d_det_rows = nullptr; int32_t* d_det_idx = nullptr; int32_t* d_det_count = nullptr;
@@ -74,52 +75,56 @@ extern "C" SKPS_API int skps_pipeline_create(skps_engine* det, skps_engine* kps,
     SKPS_CHECK(det && kps && cfg && out, "pipeline_create: null argument");
     SKPS_CHECK(cfg->top_k > 0 && cfg->top_k <= SKPS_MAX_TOP_K, "pipeline_create: top_k %d outside 1..%d", cfg->top_k,
                SKPS_MAX_TOP_K);
-    skps_pipeline* p = new skps_pipeline();
-    p->det = det; p->kps = kps; p->cfg = *cfg;
-    int c = 0;
-    skps_engine_input_dims(det, &p->det_h, &p->det_w, &c);
-    int kh = 0, kw = 0;
+    int c = 0, det_h = 0, det_w = 0, kh = 0, kw = 0;
+    skps_engine_input_dims(det, &det_h, &det_w, &c);
     skps_engine_input_dims(kps, &kh, &kw, &c);
     SKPS_CHECK(kh == kw, "pipeline_create: landmark input must be square");
-    p->kps_hw = kh;
     SKPS_CHECK(skps_engine_num_outputs(det) == 1 && skps_engine_num_outputs(kps) == 2, "pipeline_create: engine outputs");
+    const int P = skps_engine_output_elems(kps, 1), K = cfg->top_k;
+    SKPS_CHECK(skps_engine_output_elems(kps, 0) == 2 * P, "pipeline_create: landmark outputs");
+    skps_pipeline* p = new skps_pipeline();
+    p->det = det; p->kps = kps; p->cfg = *cfg;
+    p->det_h = det_h; p->det_w = det_w; p->kps_hw = kh; p->n_points = P;
     p->det_rows = skps_engine_output_elems(det, 0) / 16;
-    p->n_points = skps_engine_output_elems(kps, 1);
-    SKPS_CHECK(skps_engine_output_elems(kps, 0) == 2 * p->n_points, "pipeline_create: landmark outputs");
     cudaGetDevice(&p->device);
+    auto fail = [&](const char* what) {
+        prefix_error("pipeline_create", what);
+        skps_pipeline_destroy(p);
+        return 1;
+    };
     const size_t fbytes = (size_t)cfg->max_h * cfg->max_w * 3;
-    const int K = cfg->top_k, P = p->n_points;
-#define PALLOC(ptr, bytes) SKPS_CUDA(cudaMalloc((void**)&(ptr), (bytes)))
-#define HALLOC(ptr, bytes) SKPS_CUDA(cudaMallocHost((void**)&(ptr), (bytes)))
-    PALLOC(p->d_frame[0], fbytes); PALLOC(p->d_frame[1], fbytes);
-    HALLOC(p->h_frame, fbytes);
+    SKPS_DEV_ALLOC(p->d_frame[0], fbytes); SKPS_DEV_ALLOC(p->d_frame[1], fbytes);
+    SKPS_HOST_ALLOC(p->h_frame, fbytes);
     // every row of the detector can be a kept box: room for all of them, sized once here
-    PALLOC(p->d_det_rows, sizeof(float) * 16 * p->det_rows);
-    PALLOC(p->d_det_idx, sizeof(int32_t) * p->det_rows);
-    PALLOC(p->d_det_count, sizeof(int32_t));
-    PALLOC(p->d_nms_ws, nms_workspace_bytes(p->det_rows, 1));
+    SKPS_DEV_ALLOC(p->d_det_rows, sizeof(float) * 16 * p->det_rows);
+    SKPS_DEV_ALLOC(p->d_det_idx, sizeof(int32_t) * p->det_rows);
+    SKPS_DEV_ALLOC(p->d_det_count, sizeof(int32_t));
+    SKPS_DEV_ALLOC(p->d_nms_ws, nms_workspace_bytes(p->det_rows, 1));
     p->track_cap = K > 256 ? K : 256;
-    PALLOC(p->d_track, sizeof(float) * 4 * p->track_cap);
-    PALLOC(p->d_boxes, sizeof(float) * 4 * K);
-    PALLOC(p->d_count, sizeof(int32_t));
-    PALLOC(p->d_detail, sizeof(int32_t) * 5 * K);
-    PALLOC(p->d_kps, sizeof(float) * 2 * P * K);
-    PALLOC(p->d_scores, sizeof(float) * P * K);
-    PALLOC(p->d_counts, sizeof(int32_t) * (SKPS_LANDMARK_CHUNK + 1));
-    PALLOC(p->d_diff, sizeof(unsigned long long));
-    HALLOC(p->h_res, sizeof(skps_pipeline::Host));
-    HALLOC(p->h_boxes, sizeof(float) * 4 * K);
-    HALLOC(p->h_kps, sizeof(float) * 2 * P * K);
-    HALLOC(p->h_scores, sizeof(float) * P * K);
-    HALLOC(p->h_det_idx, sizeof(int32_t) * skps_pipeline::RUN_DET);
-    HALLOC(p->h_det_rows, sizeof(float) * 16 * skps_pipeline::RUN_DET);
-    HALLOC(p->h_track, sizeof(float) * 4 * p->track_cap);
-    SKPS_CUDA(cudaMemset(p->d_det_count, 0, sizeof(int32_t)));
+    SKPS_DEV_ALLOC(p->d_track, sizeof(float) * 4 * p->track_cap);
+    SKPS_DEV_ALLOC(p->d_boxes, sizeof(float) * 4 * K);
+    SKPS_DEV_ALLOC(p->d_count, sizeof(int32_t));
+    SKPS_DEV_ALLOC(p->d_detail, sizeof(int32_t) * 5 * K);
+    SKPS_DEV_ALLOC(p->d_kps, sizeof(float) * 2 * P * K);
+    SKPS_DEV_ALLOC(p->d_scores, sizeof(float) * P * K);
+    SKPS_DEV_ALLOC(p->d_counts, sizeof(int32_t) * (SKPS_LANDMARK_CHUNK + 1));
+    SKPS_DEV_ALLOC(p->d_diff, sizeof(unsigned long long));
+    SKPS_HOST_ALLOC(p->h_res, sizeof(skps_pipeline::Host));
+    SKPS_HOST_ALLOC(p->h_boxes, sizeof(float) * 4 * K);
+    SKPS_HOST_ALLOC(p->h_kps, sizeof(float) * 2 * P * K);
+    SKPS_HOST_ALLOC(p->h_scores, sizeof(float) * P * K);
+    SKPS_HOST_ALLOC(p->h_det_idx, sizeof(int32_t) * skps_pipeline::RUN_DET);
+    SKPS_HOST_ALLOC(p->h_det_rows, sizeof(float) * 16 * skps_pipeline::RUN_DET);
+    SKPS_HOST_ALLOC(p->h_track, sizeof(float) * 4 * p->track_cap);
     int32_t counts[SKPS_LANDMARK_CHUNK + 1];
     for (int i = 0; i <= SKPS_LANDMARK_CHUNK; ++i) counts[i] = i;
-    SKPS_CUDA(cudaMemcpy(p->d_counts, counts, sizeof(counts), cudaMemcpyHostToDevice));
-    SKPS_CUDA(cudaEventCreateWithFlags(&p->ev_ready, cudaEventDisableTiming));
-    SKPS_CUDA(cudaEventCreateWithFlags(&p->ev_read, cudaEventDisableTiming));
+    if (cudaMemset(p->d_det_count, 0, sizeof(int32_t)) != cudaSuccess ||
+        cudaMemcpy(p->d_counts, counts, sizeof(counts), cudaMemcpyHostToDevice) != cudaSuccess) {
+        set_error("%s", cudaGetErrorString(cudaGetLastError()));
+        return fail("init");
+    }
+    if (cudaEventCreateWithFlags(&p->ev_ready, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&p->ev_read, cudaEventDisableTiming) != cudaSuccess) { set_error("cudaEventCreate"); return fail("event"); }
     *out = p;
     return 0;
 }
@@ -136,50 +141,6 @@ static int check_frame_size(const skps_pipeline* p, int H, int W) {
     return 0;
 }
 
-// Gather a [dev] frame whose rows are `pitch` bytes apart into d_frame[cur] (one skps_frame_ingest pass); with `diff`, sum
-// |frame - previous frame| into d_diff in the same pass.  With a producer stream, the read waits for the work queued on it
-// so far, and its later work waits for the read.
-static int ingest_frame(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch, bool diff, const cudaStream_t* producer,
-                        cudaStream_t s) {
-    if (check_frame_size(p, H, W)) return 1;
-    if (producer) {
-        SKPS_CUDA(cudaEventRecord(p->ev_ready, *producer));
-        SKPS_CUDA(cudaStreamWaitEvent(s, p->ev_ready, 0));
-    }
-    MpStreamDesc D = {};
-    D.cur = p->d_frame[p->cur]; D.prev = diff ? p->d_frame[p->cur ^ 1] : nullptr; D.have_prev = diff;
-    D.H = H; D.W = W; D.src = frame; D.src_pitch = pitch;
-    if (diff) SKPS_CUDA(cudaMemsetAsync(p->d_diff, 0, sizeof(unsigned long long), s));
-    if (launch_frame_ingest(D, p->d_diff, s)) return 1;
-    if (producer) {
-        SKPS_CUDA(cudaEventRecord(p->ev_read, s));
-        SKPS_CUDA(cudaStreamWaitEvent(*producer, p->ev_read, 0));
-    }
-    return 0;
-}
-
-// Upload (or adopt) the frame into d_frame[cur]; returns the device pointer.
-static int stage_frame(skps_pipeline* p, const uint8_t* frame, int H, int W, int on_device, cudaStream_t s,
-                       const uint8_t** dptr) {
-    if (check_frame_size(p, H, W)) return 1;
-    size_t bytes = (size_t)H * W * 3;
-    if (on_device) {
-        if (ingest_frame(p, frame, H, W, W * 3, false, nullptr, s)) return 1;
-    } else {
-        // frames already in pinned (page-locked) memory go straight to the GPU; pageable frames are first copied
-        // into the pipeline's pinned staging buffer so the H2D copy stays asynchronous and at full PCIe rate
-        cudaPointerAttributes attr;
-        bool pinned = cudaPointerGetAttributes(&attr, frame) == cudaSuccess && attr.type == cudaMemoryTypeHost;
-        if (!pinned) {
-            cudaGetLastError();          // clear the "invalid value" a pageable pointer may leave behind
-            memcpy(p->h_frame, frame, bytes);
-        }
-        SKPS_CUDA(cudaMemcpyAsync(p->d_frame[p->cur], pinned ? frame : p->h_frame, bytes, cudaMemcpyHostToDevice, s));
-    }
-    *dptr = p->d_frame[p->cur];
-    return 0;
-}
-
 // facer.py:113: np.sum(diff)/H/W/3, from the sum in d_diff.
 static int read_mean_diff(skps_pipeline* p, int H, int W, double* mean_diff, cudaStream_t s) {
     SKPS_CUDA(cudaMemcpyAsync(&p->h_res->diff, p->d_diff, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
@@ -188,11 +149,44 @@ static int read_mean_diff(skps_pipeline* p, int H, int W, double* mean_diff, cud
     return 0;
 }
 
-// Stage and diff a [dev] frame in one ingest pass (see ingest_frame for `producer`).
-static int frame_diff_device(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch, const cudaStream_t* producer,
-                             double* mean_diff, cudaStream_t s) {
+extern "C" SKPS_API int skps_pipeline_frame_diff(skps_pipeline* p, const uint8_t* frame, int H, int W, double* mean_diff,
+                                                 void* stream) {
+    SKPS_CHECK(p && frame && mean_diff, "frame_diff: null argument");
+    cudaStream_t s = (cudaStream_t)stream;
+    SKPS_CUDA(cudaSetDevice(p->device));
+    if (check_frame_size(p, H, W)) return 1;
+    const size_t n = (size_t)H * W * 3;
+    if (upload_host_frame(frame, n, p->h_frame, p->d_frame[p->cur], s)) return 1;
+    p->cur_h = H; p->cur_w = W;
+    if (p->prev_h != H || p->prev_w != W) {
+        *mean_diff = -1.0;
+        return 0;
+    }
+    if (skps_frame_absdiff_sum(p->d_frame[p->cur ^ 1], p->d_frame[p->cur], n, p->d_diff, s)) return 1;
+    return read_mean_diff(p, H, W, mean_diff, s);
+}
+
+// One skps_frame_ingest pass gathers the [dev] frame into d_frame[cur] and, against a previous frame of the same size, sums
+// the difference.  The read waits for the work queued on the producer stream so far, and the producer's later work waits
+// for the read.
+extern "C" SKPS_API int skps_pipeline_frame_diff_device(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch,
+                                                        void* producer_stream, double* mean_diff, void* stream) {
+    SKPS_CHECK(p && frame && mean_diff, "frame_diff_device: null argument");
+    SKPS_CHECK(H == 1 || pitch >= 3 * W, "frame_diff_device: row pitch %d is less than 3 x width %d", pitch, W);
+    cudaStream_t s = (cudaStream_t)stream, producer = (cudaStream_t)producer_stream;
+    SKPS_CUDA(cudaSetDevice(p->device));
+    if (check_device_frame(frame, p->device, "frame_diff_device", -1) || check_frame_size(p, H, W)) return 1;
     const bool diff = p->prev_h == H && p->prev_w == W;
-    if (ingest_frame(p, frame, H, W, pitch, diff, producer, s)) return 1;
+    SKPS_CUDA(cudaEventRecord(p->ev_ready, producer));
+    SKPS_CUDA(cudaStreamWaitEvent(s, p->ev_ready, 0));
+    MpStreamDesc D = {};
+    D.cur = p->d_frame[p->cur]; D.prev = diff ? p->d_frame[p->cur ^ 1] : nullptr; D.have_prev = diff;
+    D.H = H; D.W = W; D.src = frame; D.src_pitch = pitch;
+    if (diff) SKPS_CUDA(cudaMemsetAsync(p->d_diff, 0, sizeof(unsigned long long), s));
+    if (launch_frame_ingest(D, p->d_diff, s)) return 1;
+    SKPS_CUDA(cudaEventRecord(p->ev_read, s));
+    SKPS_CUDA(cudaStreamWaitEvent(producer, p->ev_read, 0));
+    p->cur_h = H; p->cur_w = W;
     if (!diff) {
         *mean_diff = -1.0;
         return 0;
@@ -200,61 +194,33 @@ static int frame_diff_device(skps_pipeline* p, const uint8_t* frame, int H, int 
     return read_mean_diff(p, H, W, mean_diff, s);
 }
 
-extern "C" SKPS_API int skps_pipeline_frame_diff(skps_pipeline* p, const uint8_t* frame, int H, int W, int on_device,
-                                        double* mean_diff, void* stream) {
-    SKPS_CHECK(p && frame && mean_diff, "frame_diff: null argument");
-    cudaStream_t s = (cudaStream_t)stream;
-    SKPS_CUDA(cudaSetDevice(p->device));
-    if (on_device) return frame_diff_device(p, frame, H, W, W * 3, nullptr, mean_diff, s);
-    const uint8_t* d = nullptr;
-    if (stage_frame(p, frame, H, W, 0, s, &d)) return 1;
-    if (p->prev_h != H || p->prev_w != W) {
-        *mean_diff = -1.0;
-        return 0;
-    }
-    size_t n = (size_t)H * W * 3;
-    if (skps_frame_absdiff_sum(p->d_frame[p->cur ^ 1], d, n, p->d_diff, s)) return 1;
-    return read_mean_diff(p, H, W, mean_diff, s);
-}
-
-extern "C" SKPS_API int skps_pipeline_frame_diff_device(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch,
-                                                        void* producer_stream, double* mean_diff, void* stream) {
-    SKPS_CHECK(p && frame && mean_diff, "frame_diff_device: null argument");
-    SKPS_CHECK(H == 1 || pitch >= 3 * W, "frame_diff_device: row pitch %d is less than 3 x width %d", pitch, W);
-    SKPS_CUDA(cudaSetDevice(p->device));
-    cudaPointerAttributes attr;
-    SKPS_CUDA(cudaPointerGetAttributes(&attr, frame));
-    SKPS_CHECK((attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) && attr.device == p->device,
-               "frame_diff_device: the frame is not in memory of device %d", p->device);
-    const cudaStream_t producer = (cudaStream_t)producer_stream;
-    return frame_diff_device(p, frame, H, W, pitch, &producer, mean_diff, (cudaStream_t)stream);
-}
-
-// The frame staged by skps_pipeline_frame_diff becomes the "previous" frame without running the chain (FaceAna.run on
-// a static frame with nothing to track, facer.py:57-62: previous_image is replaced every frame).
-extern "C" SKPS_API int skps_pipeline_commit_frame(skps_pipeline* p, int H, int W) {
-    SKPS_CHECK(p && H > 0 && W > 0, "commit_frame: bad arguments");
-    p->prev_h = H; p->prev_w = W;
+// The staged frame becomes the "previous" frame (facer.py:57,62: previous_image is replaced every frame).
+static void advance_frame(skps_pipeline* p) {
+    p->prev_h = p->cur_h; p->prev_w = p->cur_w;
+    p->cur_h = p->cur_w = 0;
     p->cur ^= 1;
+}
+
+// The frame staged by skps_pipeline_frame_diff* becomes the "previous" frame without running the chain (FaceAna.run on
+// a static frame with nothing to track, facer.py:57-62).
+extern "C" SKPS_API int skps_pipeline_commit_frame(skps_pipeline* p) {
+    SKPS_CHECK(p, "commit_frame: null");
+    SKPS_CHECK(p->cur_h > 0, "commit_frame: no frame staged (call skps_pipeline_frame_diff or _frame_diff_device first)");
+    advance_frame(p);
     return 0;
 }
 
-extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, const uint8_t* frame, int H, int W, int frame_on_device,
-                                 int run_detector, int rw, int rh, int top, int left, float scale,
-                                 const float* track, int n_track, int32_t* n_faces, float* boxes4, float* kps,
-                                 float* scores, int32_t* n_det, int32_t* det_idx, float* det_rows, void* stream) {
+extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, int run_detector, int rw, int rh, int top, int left, float scale,
+                                          const float* track, int n_track, int32_t* n_faces, float* boxes4, float* kps,
+                                          float* scores, int32_t* n_det, int32_t* det_idx, float* det_rows, void* stream) {
     SKPS_CHECK(p && n_faces && boxes4 && kps && scores, "pipeline_run: null argument");
+    SKPS_CHECK(p->cur_h > 0, "pipeline_run: no frame staged (call skps_pipeline_frame_diff or _frame_diff_device first)");
     SKPS_CHECK(n_track >= 0 && n_track <= p->track_cap, "pipeline_run: n_track %d outside 0..%d", n_track, p->track_cap);
     cudaStream_t s = (cudaStream_t)stream;
     SKPS_CUDA(cudaSetDevice(p->device));
     const skps_pipeline_cfg& c = p->cfg;
-    const int K = c.top_k, P = p->n_points;
-    const uint8_t* d_frame = nullptr;
-    if (frame) {
-        if (stage_frame(p, frame, H, W, frame_on_device, s, &d_frame)) return 1;
-    } else {
-        d_frame = p->d_frame[p->cur];          // already staged by skps_pipeline_frame_diff
-    }
+    const int K = c.top_k, P = p->n_points, H = p->cur_h, W = p->cur_w;
+    const uint8_t* d_frame = p->d_frame[p->cur];
     if (n_track > 0) {
         SKPS_CHECK(track, "pipeline_run: track is null");
         memcpy(p->h_track, track, sizeof(float) * 4 * n_track);
@@ -330,9 +296,7 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, const uint8_t* frame
         if (run_detector && det_idx) memcpy(det_idx, p->h_det_idx, sizeof(int32_t) * nr);
         if (run_detector && det_rows) memcpy(det_rows, p->h_det_rows, sizeof(float) * 16 * nr);
     }
-    // the frame just processed becomes "previous" for the next frame_diff (facer.py:57,62)
-    p->prev_h = H; p->prev_w = W;
-    p->cur ^= 1;
+    advance_frame(p);
     return 0;
 }
 

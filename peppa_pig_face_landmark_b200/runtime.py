@@ -91,9 +91,8 @@ SIGNATURES = {
     "skps_pipeline_create": (C.c_int, [c_vp, c_vp, C.POINTER(PipelineCfg), C.POINTER(c_vp)]),
     "skps_pipeline_destroy": (None, [c_vp]),
     "skps_pipeline_reset": (C.c_int, [c_vp]),
-    "skps_pipeline_run": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
-                                    C.c_int, C.c_float, c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
-                                    c_vp]),
+    "skps_pipeline_run": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, c_vp, C.c_int,
+                                    c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "skps_pipeline_det_results": (C.c_int, [c_vp, C.c_int, c_vp, c_vp]),
     "skps_crop_rect": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, C.c_int, c_vp]),
     "skps_nme": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
@@ -102,12 +101,12 @@ SIGNATURES = {
     "skps_mpipe_destroy": (None, [c_vp]),
     "skps_mpipe_reset": (C.c_int, [c_vp, C.c_int]),
     "skps_mpipe_dims": (C.c_int, [c_vp, c_i32p, c_i32p, c_i32p]),
-    "skps_mpipe_submit": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, C.c_int, C.c_int]),
+    "skps_mpipe_submit": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, C.c_int]),
     "skps_mpipe_wait": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "skps_mpipe_submit_device": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int, C.POINTER(MpipeOutputs), c_vp]),
     "skps_mpipe_wait_stream": (C.c_int, [c_vp, C.c_int, c_vp]),
-    "skps_pipeline_commit_frame": (C.c_int, [c_vp, C.c_int, C.c_int]),
-    "skps_pipeline_frame_diff": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double), c_vp]),
+    "skps_pipeline_commit_frame": (C.c_int, [c_vp]),
+    "skps_pipeline_frame_diff": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.POINTER(C.c_double), c_vp]),
     "skps_pipeline_frame_diff_device": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, C.POINTER(C.c_double), c_vp]),
     "skps_warp_affine": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
     "skps_align_faces": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp,
