@@ -7,9 +7,19 @@
 // operand and 256 pixels as N, a tile reuses each weight slice for twice the pixels.  Same fp16 hi/lo three-product scheme,
 // same 4-D TMA activation boxes (padding / dilation = OOB fill) and K-padded weight matrix as conv_tc.
 //
-// Tile = 256 pixels = bh whole rows of one image (W | 256).  Stage = one (tap, 64-channel chunk): weights 2 x 16 KB +
-// activations 2 x 32 KB; two stages.  Warpgroups 1 and 2 each accumulate 128 channels x 128 pixels (pixel columns [0,128) and
-// [128,256)) in registers with m64n128k16 wgmma, one k-block's group kept in flight while the next is issued, and run the
+// Tile = 256 pixels = bh whole rows of one image (W | 256).  K runs in the order (kx, 32-channel half-chunk, ky, 16-channel
+// step), and the kh vertical taps of one (kx, half-chunk) read ONE activation load:
+//   halo slot   = the bh + dil (kh - 1) input rows y0 - pad ... y0 + bh - 1 + pad at column shift kx dil - pad, W pixels x 64 B
+//                 each (64-byte swizzle), hi and lo plane, one 4-D TMA box per plane (padding = OOB fill).  Tap ky's B operand
+//                 is the slot from row ky dil on: a byte offset of ky dil W 64, a whole number of 512-byte swizzle atoms for
+//                 every admitted W, and a warpgroup's 128 pixels are contiguous in it because whole rows are.
+//   weight slot = the 128 x 32 slice of the packed matrix for one (tap, half-chunk), hi and lo: 16 KB.
+// The two have their own mbarrier rings: three weight slots, and as many halo slots (at most three, at least two) as fit
+// beside them and the epilogue staging; the MMA warps free a weight slot per tap and the halo slot after the last ky.  A
+// tile so fetches each input row once per column shift kx, not once per tap.  Layers whose halo slot does not fit twice run
+// on conv_tc.
+// Warpgroups 1 and 2 each accumulate 128 channels x 128 pixels (pixel columns [0,128) and [128,256)) in registers with
+// m64n128k16 wgmma, one tap's group kept in flight while the next is issued, and run the
 // epilogue on them straight from the accumulator fragment: bias / activation / fp16 hi-lo split, written TRANSPOSED
 // (pixel rows of 32 channels) into the warpgroup's 16 KB staging buffer, 32 pixels at a time, which leaves as one TMA store
 // per 32-channel quarter and plane, so the NHWC layout of the output is unchanged.
@@ -17,6 +27,8 @@
 #include <cuda_fp16.h>
 #include <math.h>
 #include <string.h>
+
+#include <algorithm>
 
 #include "../../include/skps_b200.h"
 #include "common.h"
@@ -27,10 +39,13 @@ namespace skps {
 
 constexpr int TCT_THREADS = 288;         // warps 0-7 MMA + epilogue (two warpgroups), warp 8 TMA
 constexpr int TCT_M = 128, TCT_N = 256;
-constexpr int TCT_W_TILE = TCT_M * 128;  // weights of one k-block, one plane: 128 rows x 128 B
-constexpr int TCT_X_TILE = TCT_N * 128;  // activations of one k-block, one plane: 256 pixel rows x 128 B
-constexpr int TCT_STAGE = 2 * TCT_W_TILE + 2 * TCT_X_TILE;      // 96 KB
-constexpr int TCT_STAGES = 2;
+constexpr int TCT_KC = 32;               // channels per slot: one 64-byte swizzled row, two K-steps of 16
+constexpr int TCT_W_PLANE = TCT_M * 2 * TCT_KC;      // weights of one (tap, half-chunk), one plane: 128 rows x 64 B
+constexpr int TCT_W_SLOT = 2 * TCT_W_PLANE;          // 16 KB
+constexpr int TCT_W_SLOTS = 3;
+constexpr int TCT_MAX_X_SLOTS = 3;
+constexpr int TCT_OUT_BYTES = 2 * 16384;             // epilogue staging of the two warpgroups
+constexpr int TCT_SMEM_LIMIT = 227 * 1024 - 256;     // dynamic shared memory a CTA may ask for beside the barriers
 
 template <int ACT>
 __global__ void __launch_bounds__(TCT_THREADS, 1)
@@ -38,13 +53,18 @@ conv_tct_kernel(const __grid_constant__ CUtensorMap tmX_hi, const __grid_constan
                 const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo,
                 const __grid_constant__ CUtensorMap tmO_hi, const __grid_constant__ CUtensorMap tmO_lo, const TctK p) {
     extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t full_bar[TCT_STAGES], empty_bar[TCT_STAGES];
+    __shared__ __align__(8) uint64_t full_w[TCT_W_SLOTS], empty_w[TCT_W_SLOTS], full_x[TCT_MAX_X_SLOTS],
+        empty_x[TCT_MAX_X_SLOTS];
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t out_off = base + (uint32_t)TCT_STAGES * TCT_STAGE;       // 2 epilogue warpgroups x 16 KB
+    const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;            // the weight ring
+    const uint32_t x_base = base + (uint32_t)TCT_W_SLOTS * TCT_W_SLOT;      // the halo ring
+    const uint32_t x_slot = 2u * (uint32_t)p.x_plane;
+    const uint32_t out_off = x_base + (uint32_t)p.x_slots * x_slot;         // 2 epilogue warpgroups x 16 KB
     const int tiles = p.m_tiles;
-    const int kblocks = p.taps * p.cchunks;
+    const int kh = p.taps / p.kw;
+    const int halves = (p.Cin + TCT_KC - 1) / TCT_KC;
+    const int groups = p.kw * halves;                  // (kx, half-chunk) pairs of a tile, kx outer
 
     if (warp == 8 && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmX_hi) : "memory");
@@ -53,9 +73,13 @@ conv_tct_kernel(const __grid_constant__ CUtensorMap tmX_hi, const __grid_constan
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW_lo) : "memory");
     }
     if (warp == 1 && lane == 0) {
-        for (int s = 0; s < TCT_STAGES; ++s) {
-            mbar_init(smem_u32(&full_bar[s]), 1);
-            mbar_init(smem_u32(&empty_bar[s]), 8);            // one arrival per MMA warp
+        for (int s = 0; s < TCT_W_SLOTS; ++s) {
+            mbar_init(smem_u32(&full_w[s]), 1);
+            mbar_init(smem_u32(&empty_w[s]), 8);              // one arrival per MMA warp
+        }
+        for (int s = 0; s < p.x_slots; ++s) {
+            mbar_init(smem_u32(&full_x[s]), 1);
+            mbar_init(smem_u32(&empty_x[s]), 8);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -63,26 +87,42 @@ conv_tct_kernel(const __grid_constant__ CUtensorMap tmX_hi, const __grid_constan
 
     if (warp == 8) {
         // ================================================================== TMA producer
-        if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        // The CTA's groups are numbered across its tiles, so the rings run ahead over tile boundaries.  Halo slot n + 1 is
+        // requested after the first weight slice of group n: the MMA warps free a halo slot when the first tap of the next
+        // group has been issued, so with two halo slots that slice must already be on its way.
+        if (lane == 0 && (int)blockIdx.x < tiles) {
+            const int total = ((tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x) * groups;
+            int xs = 0, ws = 0;
+            uint32_t xphase = 0, wphase = 0;
+            auto load_halo = [&](int n) {
+                const int i = n / groups, g = n - i * groups;
+                const int kx = g / halves, hc = g - kx * halves;
+                const int tile = (int)blockIdx.x + i * (int)gridDim.x;
                 const int img_l = tile / p.tiles_per_img, t = tile - img_l * p.tiles_per_img;
-                const int y0 = t * p.bh;
-                for (int kb = 0; kb < kblocks; ++kb) {
-                    const int tap = kb / p.cchunks, cc = kb - tap * p.cchunks;
-                    const int ky = tap / p.kw, kx = tap - ky * p.kw;
-                    mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1u);
-                    const uint32_t fb = smem_u32(&full_bar[stage]);
-                    mbar_expect_tx(fb, (uint32_t)TCT_STAGE);
-                    const uint32_t ss = base + (uint32_t)stage * TCT_STAGE;
-                    tma_load_2d(ss, &tmW_hi, fb, kb * 64, 0);
-                    tma_load_2d(ss + TCT_W_TILE, &tmW_lo, fb, kb * 64, 0);
-                    const int cx = kx * p.dil - p.pad, cy = y0 + ky * p.dil - p.pad;
-                    tma_load_4d(ss + 2 * TCT_W_TILE, &tmX_hi, fb, cc * 64, cx, cy, img_l + p.img0);
-                    tma_load_4d(ss + 2 * TCT_W_TILE + TCT_X_TILE, &tmX_lo, fb, cc * 64, cx, cy, img_l + p.img0);
-                    if (++stage == TCT_STAGES) { stage = 0; phase ^= 1u; }
+                mbar_wait(smem_u32(&empty_x[xs]), xphase ^ 1u);
+                const uint32_t fb = smem_u32(&full_x[xs]);
+                mbar_expect_tx(fb, x_slot);
+                const uint32_t sx = x_base + (uint32_t)xs * x_slot;
+                const int cx = kx * p.dil - p.pad, cy = t * p.bh - p.pad;
+                tma_load_4d(sx, &tmX_hi, fb, hc * TCT_KC, cx, cy, img_l + p.img0);
+                tma_load_4d(sx + (uint32_t)p.x_plane, &tmX_lo, fb, hc * TCT_KC, cx, cy, img_l + p.img0);
+                if (++xs == p.x_slots) { xs = 0; xphase ^= 1u; }
+            };
+            load_halo(0);
+            for (int n = 0, g = 0; n < total; ++n) {
+                const int kx = g / halves, hc = g - kx * halves;
+                for (int ky = 0; ky < kh; ++ky) {
+                    mbar_wait(smem_u32(&empty_w[ws]), wphase ^ 1u);
+                    const uint32_t fb = smem_u32(&full_w[ws]);
+                    mbar_expect_tx(fb, (uint32_t)TCT_W_SLOT);
+                    const uint32_t sw = base + (uint32_t)ws * TCT_W_SLOT;
+                    const int col = (ky * p.kw + kx) * p.cchunks * 64 + hc * TCT_KC;
+                    tma_load_2d(sw, &tmW_hi, fb, col, 0);
+                    tma_load_2d(sw + TCT_W_PLANE, &tmW_lo, fb, col, 0);
+                    if (++ws == TCT_W_SLOTS) { ws = 0; wphase ^= 1u; }
+                    if (ky == 0 && n + 1 < total) load_halo(n + 1);
                 }
+                if (++g == groups) g = 0;
             }
         }
     } else {
@@ -111,40 +151,54 @@ conv_tct_kernel(const __grid_constant__ CUtensorMap tmX_hi, const __grid_constan
             row_addr[r] = sbuf + (uint32_t)(2 * (r >> 1) + (q >> 1)) * 4096u + (uint32_t)(2 * (lane & 3)) * 64u +
                           (uint32_t)((((cq >> 3) ^ (lane & 3)) & 3) << 4) + (uint32_t)(cq & 7) * 2u;
         }
-        // 16-channel steps of the last 64-channel chunk that hold real channels (TMA zero-fills the rest)
-        const int ks_last = min(4, (p.Cin - (p.cchunks - 1) * 64 + 15) / 16);
-        int stage = 0;
-        uint32_t phase = 0;
+        // 16-channel steps of the last half-chunk that hold real channels (TMA zero-fills the rest)
+        const int ks_last = (p.Cin - (halves - 1) * TCT_KC + 15) / 16;
+        const uint32_t tap_step = (uint32_t)(p.dil * p.W * 2 * TCT_KC);     // bytes between the rows of taps ky and ky + 1
+        int xs = 0, ws = 0;
+        uint32_t xphase = 0, wphase = 0;
         for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
             const int img_l = tile / p.tiles_per_img, t = tile - img_l * p.tiles_per_img;
             float acc[128];
-            int prev = 0;
-            for (int kb = 0; kb < kblocks; ++kb) {
-                mbar_wait(smem_u32(&full_bar[stage]), phase);
-                const uint32_t ss = base + (uint32_t)stage * TCT_STAGE;
-                const uint64_t w_hi = make_smem_desc(ss), w_lo = make_smem_desc(ss + TCT_W_TILE);
-                const uint32_t xo = ss + 2 * TCT_W_TILE + (uint32_t)(half_id * 128 * 128);
-                const uint64_t x_hi = make_smem_desc(xo), x_lo = make_smem_desc(xo + TCT_X_TILE);
-                const int ks = kb % p.cchunks == p.cchunks - 1 ? ks_last : 4;
-                const uint32_t accumulate = kb != 0;
-                wg_fence_acc(acc);
-                switch (ks) {                          // uniform over the CTA
-                    case 4: wg_fence(); wg_mma3_128x128<4>(acc, w_hi, w_lo, x_hi, x_lo, accumulate); wg_commit(); break;
-                    case 3: wg_fence(); wg_mma3_128x128<3>(acc, w_hi, w_lo, x_hi, x_lo, accumulate); wg_commit(); break;
-                    case 2: wg_fence(); wg_mma3_128x128<2>(acc, w_hi, w_lo, x_hi, x_lo, accumulate); wg_commit(); break;
-                    default: wg_fence(); wg_mma3_128x128<1>(acc, w_hi, w_lo, x_hi, x_lo, accumulate); wg_commit(); break;
+            int prev_w = -1, prev_x = -1;          // slots the group in flight reads; prev_x only behind a group's last tap
+            for (int g = 0, hc = 0; g < groups; ++g) {
+                mbar_wait(smem_u32(&full_x[xs]), xphase);
+                // the warpgroup's 128 pixels of tap ky: whole rows, ky dil rows below the slot's first
+                const uint32_t xo = x_base + (uint32_t)xs * x_slot + (uint32_t)(half_id * 128 * 2 * TCT_KC);
+                const bool two = hc != halves - 1 || ks_last == 2;
+                for (int ky = 0; ky < kh; ++ky) {
+                    mbar_wait(smem_u32(&full_w[ws]), wphase);
+                    const uint32_t sw = base + (uint32_t)ws * TCT_W_SLOT;
+                    const uint64_t w_hi = make_smem_desc_sw64(sw), w_lo = make_smem_desc_sw64(sw + TCT_W_PLANE);
+                    const uint32_t xk = xo + (uint32_t)ky * tap_step;
+                    const uint64_t x_hi = make_smem_desc_sw64(xk), x_lo = make_smem_desc_sw64(xk + (uint32_t)p.x_plane);
+                    const uint32_t accumulate = (g | ky) != 0;
+                    wg_fence_acc(acc);
+                    if (two) {                         // uniform over the CTA
+                        wg_fence(); wg_mma3_128x128<2, 64>(acc, w_hi, w_lo, x_hi, x_lo, accumulate); wg_commit();
+                    } else {
+                        wg_fence(); wg_mma3_128x128<1, 64>(acc, w_hi, w_lo, x_hi, x_lo, accumulate); wg_commit();
+                    }
+                    wg_fence_acc(acc);
+                    // keep this tap's group in flight; the previous one has finished reading its slots
+                    wg_wait<1>();
+                    wg_fence_acc(acc);
+                    if (lane == 0) {
+                        if (prev_w >= 0) mbar_arrive(smem_u32(&empty_w[prev_w]));
+                        if (prev_x >= 0) mbar_arrive(smem_u32(&empty_x[prev_x]));
+                    }
+                    prev_w = ws;
+                    prev_x = ky == kh - 1 ? xs : -1;
+                    if (++ws == TCT_W_SLOTS) { ws = 0; wphase ^= 1u; }
                 }
-                wg_fence_acc(acc);
-                // keep this k-block's group in flight; the previous one has finished reading its stage
-                wg_wait<1>();
-                wg_fence_acc(acc);
-                if (kb > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
-                prev = stage;
-                if (++stage == TCT_STAGES) { stage = 0; phase ^= 1u; }
+                if (++xs == p.x_slots) { xs = 0; xphase ^= 1u; }
+                if (++hc == halves) hc = 0;
             }
             wg_wait<0>();
             wg_fence_acc(acc);
-            if (lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+            if (lane == 0) {
+                mbar_arrive(smem_u32(&empty_w[prev_w]));
+                mbar_arrive(smem_u32(&empty_x[prev_x]));
+            }
 #pragma unroll
             for (int ci = 0; ci < 4; ++ci) {
                 if (leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the buffer's last store has drained
@@ -186,6 +240,14 @@ conv_tct_kernel(const __grid_constant__ CUtensorMap tmX_hi, const __grid_constan
 // ------------------------------------------------------------------------------------------ host side
 // The layers this kernel is for: tensor-bound k x k convs whose Cout fills the 128 accumulator rows (else the rows idle and
 // the pixels-as-rows kernel wins), whole 256-pixel row blocks, split-fp16 contiguous output, no residual.
+// Bytes of one plane of a halo slot: the tile's rows and the dil (k - 1) rows around them, W pixels of 32 channels each.
+static int tct_x_plane(const TcSetup& s) { return (TCT_N / s.W + s.dil * (s.kh - 1)) * s.W * 2 * TCT_KC; }
+// Halo slots that fit beside the weight ring and the epilogue staging.
+static int tct_x_slots(const TcSetup& s) {
+    const int room = TCT_SMEM_LIMIT - 1024 - TCT_W_SLOTS * TCT_W_SLOT - TCT_OUT_BYTES;
+    return std::min(TCT_MAX_X_SLOTS, room / (2 * tct_x_plane(s)));
+}
+
 bool tct_applicable(const TcSetup& s) {
     const int stride = s.stride > 0 ? s.stride : 1;
     if (stride != 1 || s.kh != s.kw || s.kh < 3 || s.pad != s.dil * (s.kh - 1) / 2) return false;
@@ -197,7 +259,8 @@ bool tct_applicable(const TcSetup& s) {
     // SiLU's correctly rounded division is a subroutine call that does not fit beside the 128 accumulator registers without
     // spilling; conv_tc runs such layers
     if (s.act == ACT_SILU) return false;
-    return true;
+    // the halo ring needs two slots to overlap a fill with the MMAs; wider halos (5x5 on 256-wide maps) run on conv_tc
+    return tct_x_slots(s) >= 2;
 }
 
 int tct_prepare(TctLayer& L, const TcSetup& s) {
@@ -211,15 +274,16 @@ int tct_prepare(TctLayer& L, const TcSetup& s) {
     k.cchunks = (s.Cin + 63) / 64; k.Cin = s.Cin; k.Cout = s.Cout; k.act = s.act; k.out_scale = s.out_scale;
     SKPS_CHECK(s.bias, "conv_tct: bias required");
     k.bias = s.bias;
-    L.smem_bytes = TCT_STAGES * TCT_STAGE + 8 * 4096 + 1024;
+    k.x_plane = tct_x_plane(s); k.x_slots = tct_x_slots(s);
+    L.smem_bytes = 1024 + TCT_W_SLOTS * TCT_W_SLOT + k.x_slots * 2 * k.x_plane + TCT_OUT_BYTES;
     for (int plane = 0; plane < 2; ++plane) {
         cuuint64_t dims[4] = {(cuuint64_t)s.Cin, (cuuint64_t)s.W, (cuuint64_t)s.H, (cuuint64_t)s.max_batch};
         cuuint64_t strides[3] = {(cuuint64_t)s.in_ld * 2, (cuuint64_t)s.W * s.in_ld * 2, (cuuint64_t)s.H * s.W * s.in_ld * 2};
-        cuuint32_t box[4] = {64, (cuuint32_t)s.W, (cuuint32_t)k.bh, 1};
+        cuuint32_t box[4] = {TCT_KC, (cuuint32_t)s.W, (cuuint32_t)(k.bh + s.dil * (s.kh - 1)), 1};   // one halo slot plane
         cuuint32_t estr[4] = {1, 1, 1, 1};
         void* base = (void*)((__half*)s.in_base + (plane ? s.in_plane : 0) + s.in_coff);
         CUresult r = enc(plane ? &L.x_lo : &L.x_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         SKPS_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(tct X) failed: %d", (int)r);
     }
@@ -227,11 +291,11 @@ int tct_prepare(TctLayer& L, const TcSetup& s) {
     for (int plane = 0; plane < 2; ++plane) {
         cuuint64_t dims[2] = {(cuuint64_t)K_pad, (cuuint64_t)s.n_tile};        // rows beyond n_tile: OOB zero fill
         cuuint64_t strides[1] = {(cuuint64_t)K_pad * 2};
-        cuuint32_t box[2] = {64, (cuuint32_t)TCT_M};
+        cuuint32_t box[2] = {TCT_KC, (cuuint32_t)TCT_M};
         cuuint32_t estr[2] = {1, 1};
         void* base = (void*)(plane ? s.w_lo : s.w_hi);
         CUresult r = enc(plane ? &L.w_lo : &L.w_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, base, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         SKPS_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(tct W) failed: %d", (int)r);
     }

@@ -11,6 +11,7 @@ namespace skps {
 struct TctK {                    // kernel parameters
     int W, bh, tiles_per_img, m_tiles, img0;    // tile = bh whole rows = 256 pixels
     int taps, kw, dil, pad, cchunks, Cin, Cout, act;
+    int x_plane, x_slots;        // bytes of one plane of a halo slot (bh + dil (kh - 1) rows x W pixels x 64 B); slots in the ring
     float out_scale;             // exact power of two undoing the weight pre-scale
     const float* bias;
 };

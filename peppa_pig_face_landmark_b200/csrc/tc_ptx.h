@@ -243,11 +243,13 @@ __device__ __forceinline__ void wg_mma3(float* acc, uint64_t a_hi, uint64_t a_lo
 }
 
 // KS K-steps of 16 of the three-product scheme on a 128 x 128 accumulator held by one warpgroup: acc[0..63] = A rows 0-63,
-// acc[64..127] = A rows 64-127 (128-byte-swizzled K-major A, row 64 at +8 KB).  Straight-line, so the wgmma stay asynchronous.
-template <int KS>
+// acc[64..127] = A rows 64-127 (swizzled K-major A with rows of ROW_BYTES = 128 or 64, row 64 at +64 rows).  Straight-line, so
+// the wgmma stay asynchronous.
+template <int KS, int ROW_BYTES = 128>
 __device__ __forceinline__ void wg_mma3_128x128(float* acc, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo,
                                                 uint32_t accumulate) {
-    constexpr uint64_t A_HALF = 64 * 128 >> 4;
+    static_assert(KS * 32 <= ROW_BYTES, "K-steps past the swizzled row");
+    constexpr uint64_t A_HALF = 64 * ROW_BYTES >> 4;
 #pragma unroll
     for (int k = 0; k < KS; ++k) {
         const uint64_t koff = (uint64_t)(k * 32 >> 4);     // 16 fp16 = 32 bytes along K
