@@ -304,6 +304,12 @@ SKPS_API int skps_pipeline_run(skps_pipeline* p, int run_detector, int rw, int r
  * rows from the device.  Synchronous. */
 SKPS_API int skps_pipeline_det_results(skps_pipeline* p, int capacity, int32_t* det_idx, float* det_rows);
 
+/* Track-id sources of the faces the last skps_pipeline_run returned: src [host] (n) int32, n <= that run's n_faces.
+ * Face i's source is, on a detector frame, the index of the first `track` box its detection matched (IoU > track_iou),
+ * -1 for none; with run_detector == 0 the index of the `track` box it is.  Copied back with the run's other results:
+ * no device work, no synchronisation. */
+SKPS_API int skps_pipeline_face_sources(skps_pipeline* p, int n, int32_t* src);
+
 /* Stage a frame for skps_pipeline_run / skps_pipeline_commit_frame and return its mean absolute
  * difference to the previous frame (facer.py:111-113), or -1.0 in *mean_diff when there is no
  * previous frame of the same size.  `frame` [host] HxWx3 uint8 BGR, pinned or pageable. */
@@ -346,7 +352,8 @@ typedef struct skps_mpipe skps_mpipe;
 SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, const skps_pipeline_cfg* cfg, int n_streams,
                                skps_mpipe** out);
 SKPS_API void skps_mpipe_destroy(skps_mpipe* p);
-/* FaceAna.reset() for one stream (or all: stream = -1): forget the previous frame, the track boxes, the landmark history. */
+/* FaceAna.reset() for one stream (or all: stream = -1): forget the previous frame, the track boxes, the landmark history;
+ * the stream's track ids start from 0 again. */
 SKPS_API int skps_mpipe_reset(skps_mpipe* p, int stream);
 SKPS_API int skps_mpipe_dims(const skps_mpipe* p, int* n_streams, int* top_k, int* n_points);
 /* Enqueue frame i (HxWx3 uint8 BGR, [host] pinned or pageable) of stream i for i < n; hw = {H0,W0,H1,W1,...}.
@@ -372,6 +379,7 @@ typedef struct skps_mpipe_outputs {
     double* M;                          /* (n, top_k, 2, 3)                */
     double *rvec, *tvec, *euler;        /* (n, top_k, 3) each              */
     double* reproject;                  /* (n, top_k, 8, 2)                */
+    int64_t* ids;                       /* (n, top_k) track ids, or NULL   */
 } skps_mpipe_outputs;
 /* skps_mpipe_submit for frames already on the pipeline's device: frame i HxWx3 uint8 BGR with rows pitches[i] bytes apart
  * (>= 3W, any alignment), gathered into the stream's ring and diffed against its previous frame in one launch for the
@@ -384,6 +392,12 @@ SKPS_API int skps_mpipe_submit_device(skps_mpipe* p, int slot, const uint8_t* co
 /* Completes a slot submitted with device outputs without blocking the host: work queued on `consumer_stream` after this
  * call runs after the batch's results are in the caller's buffers.  The slot can then be submitted again. */
 SKPS_API int skps_mpipe_wait_stream(skps_mpipe* p, int slot, void* consumer_stream);
+/* Track ids (additive): every stream keeps an id per track box on the device.  Per call, in output order, a face whose
+ * source (the track box its detection matched, or on a gate-skipped frame the track box it is) is a track box whose id no
+ * earlier face of the call took inherits that id; every other face gets the stream's next number, starting at 0 after
+ * skps_mpipe_reset.  After skps_mpipe_wait(slot): ids [host] (n, top_k) int64, n = that submit's stream count; entries
+ * i >= n_faces[s] are undefined.  Device results get them through skps_mpipe_outputs.ids. */
+SKPS_API int skps_mpipe_track_ids(skps_mpipe* p, int slot, int64_t* ids);
 
 /* ---- Aligned face chips (csrc/align.cu; additive) -----------------------------------------------------------------------
  * What a caller does with the 98 landmarks before a recognition / attribute model: estimate the least-squares similarity

@@ -16,7 +16,7 @@ import yaml
 from ... import runtime as rt
 from ...graph_tools import check_detector_input
 from ...logger.logger import logger
-from ..smoother.lk import EmaFilter, GroupTrack, first_match, rects
+from ..smoother.lk import EmaFilter, GroupTrack, assign_track_ids, first_match, rects
 from .face_detector import FaceDetector, letterbox_geometry
 from .face_landmark import MIN_FACE, FaceLandmark, face_scale
 from .align import check_size
@@ -44,7 +44,8 @@ def pipeline_cfg(cfg, top_k, max_frame_hw):
 
 
 class FaceAna():
-    def __init__(self, verbose=False, top_k=None, max_frame_hw=(2160, 3840), align=None, pose=False, det_input=None):
+    def __init__(self, verbose=False, top_k=None, max_frame_hw=(2160, 3840), align=None, pose=False, det_input=None,
+                 track_ids=False):
         """align: None, or a chip side in 16..512: every result dict then also carries 'chip' ((align, align, 3) uint8
         BGR, the face warped to the ArcFace five-point template) and 'M' ((2, 3) float64, the frame -> chip matrix for
         cv2.warpAffine), computed on the GPU from the returned 'kps' and the frame already in HBM (core/api/align.py).
@@ -56,7 +57,14 @@ class FaceAna():
         a 3840x2160 frame is scaled by 1/2 instead of 1/6.  The detector's work and activation memory grow with h*w
         (3.97 GMAC and 0.35 GB at 1152x1920, 0.44 GMAC and 0.04 GB at 384x640).
         top_k: None (Skps.yml's Detect.topk, 5), or 1..1024 faces per frame.  The landmark net runs on the faces found,
-        in chunks of at most 64, so its activation memory is that of min(top_k, 64) faces (about 47 MB per face)."""
+        in chunks of at most 64, so its activation memory is that of min(top_k, 64) faces (about 47 MB per face).
+        track_ids: every result dict then also carries 'id', an int that follows the face from call to call.  Ids are
+        numbered per FaceAna from 0, and reset() starts again from 0.  Each returned face has a source: on a frame that ran
+        the detector, the first of the previous call's faces whose box its detection overlaps with IoU > Trace.iou_thres
+        (the match judge_boxs smooths the box with), or none; on a frame the difference gate skipped, the previous face
+        it is.  In the order of the returned list, a face inherits its source's id unless an earlier face of the same
+        call already took it, and every other face gets the next unused number.  A face the tracker loses for one frame
+        comes back with a new id: there is no re-identification."""
         cfg = get_cfg()
         self.top_k = int(top_k if top_k is not None else cfg['Skps']['Detect']['topk'])
         if not 1 <= self.top_k <= MAX_TOP_K:
@@ -66,6 +74,7 @@ class FaceAna():
             det_input = check_detector_input(det_input)
         self.align = None if align is None else check_size(align)
         self.pose = bool(pose)
+        self.track_ids = bool(track_ids)
         if verbose:
             logger.setLevel(logging.DEBUG)
         if det_input is not None:
@@ -100,6 +109,7 @@ class FaceAna():
         self._det_idx = np.zeros((FaceDetector.MAX_DET,), np.int32)
         self._det_rows = np.zeros((FaceDetector.MAX_DET, 16), np.float32)
         self._have_prev = False
+        self._ids, self._next_id = [], 0     # ids of the track boxes (index-aligned with track_box), next unused id
         self.last_det_idx = None       # kept detector rows of the last detector run (parity checks)
         self.last_det_rows = None
 
@@ -129,6 +139,7 @@ class FaceAna():
         track32 = None
         if n_track:
             track32 = np.ascontiguousarray(np.asarray(track)[:, :4], dtype=np.float32)
+        ids = []
         if not run_det and n_track == 0:
             # facer.py:61 with an empty/None track: nothing to do (the reference would fail on None)
             boxes_return = np.zeros((0, 4), np.float32)
@@ -143,6 +154,10 @@ class FaceAna():
             boxes_return = self._boxes[:n].copy()
             landmarks = self._kps[:n].copy() if n else np.array([])
             states = self._scores[:n].copy() if n else np.array([])
+            if self.track_ids and n:
+                src = np.empty((n,), np.int32)
+                rt.check(self.lib.skps_pipeline_face_sources(self._pipe, n, src.ctypes.data))
+                ids, self._next_id = assign_track_ids(src, self._ids, self._next_id)
             if run_det:
                 nd = self._ndet.value
                 idx, rows = self._det_idx, self._det_rows
@@ -160,6 +175,10 @@ class FaceAna():
         tmp_box = rects(landmarks) if landmarks.shape[0] else np.array([])
         self.track_box = self.judge_boxs(boxes_return, tmp_box)
         res = self.to_dict(self.track_box, landmarks, states)
+        if self.track_ids:
+            self._ids = ids
+            for r, i in zip(res, ids):
+                r['id'] = i
         if self.align is not None and res:
             self._add_chips(res)
         if self.pose and res:
@@ -247,5 +266,6 @@ class FaceAna():
         self.track_box = None
         self.previous_image = None
         self.previous_box = None
+        self._ids, self._next_id = [], 0
         rt.check(self.lib.skps_pipeline_reset(self._pipe))
 

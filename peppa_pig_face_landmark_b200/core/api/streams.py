@@ -9,6 +9,7 @@ device (csrc/mpipe.cu, csrc/temporal.cu) and two batches can be in flight so tha
     results = fa.run(frames)            # list of S lists of {'box','kps','scores'} - what S FaceAna.run calls return
     # FaceAnaStreams(..., align=112): each dict also has 'chip' (112x112x3 uint8, aligned) and 'M' (2x3 float64)
     # FaceAnaStreams(..., pose=True): each dict also has 'pose' {'euler', 'rvec', 'tvec', 'reproject'} as FaceAna returns it
+    # FaceAnaStreams(..., track_ids=True): each dict also has 'id', the track id FaceAna(track_ids=True) gives the face
     # or, overlapped:
     fa.submit(frames_t0); fa.submit(frames_t1); r0 = fa.collect(); fa.submit(frames_t2); r1 = fa.collect(); ...
     # frames already on the GPU (torch.uint8 CUDA tensors (H, W, 3), any row pitch), results left on the GPU:
@@ -31,16 +32,20 @@ from .onnx_model_base import ONNXEngine
 
 class FaceAnaStreams:
     def __init__(self, n_streams, top_k=None, max_frame_hw=(2160, 3840), device="cuda", align=None, pose=False,
-                 det_input=None):
+                 det_input=None, track_ids=False):
         """align: None, or a chip side in 16..512: every result dict then also carries 'chip' and 'M' as FaceAna(align=...)
         returns them, warped inside the same submit on the device from the smoothed landmarks and the frame in the ring.
         pose: every result dict then also carries 'pose' as FaceAna(pose=True) returns it, solved inside the same submit
         from the smoothed landmarks, with each stream's own frame size for the camera.
         det_input: None (Skps.yml's 384x640) or the detector input size (h, w), as FaceAna(det_input=...) takes it.  The
         detector runs on all n_streams frames at once, so its activations take n_streams times FaceAna's memory (about
-        0.35 GB per stream at 1152x1920)."""
+        0.35 GB per stream at 1152x1920).
+        track_ids: every result dict then also carries 'id', the int FaceAna(track_ids=True) returns for the face: ids
+        are numbered per stream from 0, reset(stream) starts that stream again from 0, and the rule that assigns them is
+        FaceAna's.  The ids are kept on the device next to the track boxes, whether or not they are returned."""
         self.align = None if align is None else check_size(align)
         self.pose = bool(pose)
+        self.track_ids = bool(track_ids)
         cfg = get_cfg()['Skps']
         det_cfg, kps_cfg = cfg['Detect'], cfg['Keypoints']
         self.n_streams = int(n_streams)
@@ -66,7 +71,8 @@ class FaceAnaStreams:
         self._h = h
         S, K, P = self.n_streams, self.top_k, self.n_points
         self._out = [dict(n=np.zeros(S, np.int32), box=np.zeros((S, K, 4), np.float64), kps=np.zeros((S, K, P, 2), np.float64),
-                          sc=np.zeros((S, K, P), np.float32), det=np.zeros(S, np.int32)) for _ in range(2)]
+                          sc=np.zeros((S, K, P), np.float32), det=np.zeros(S, np.int32), ids=np.zeros((S, K), np.int64))
+                     for _ in range(2)]
         if self.align is not None:
             rt.check(self.lib.skps_mpipe_set_align(h, self.align))
             for o in self._out:
@@ -138,7 +144,7 @@ class FaceAnaStreams:
             outs = rt.MpipeOutputs(n_faces=out["n"].data_ptr(), ran_detector=out["ran_detector"].data_ptr(),
                                    boxes=out["box"].data_ptr(), kps=out["kps"].data_ptr(), scores=out["scores"].data_ptr())
             for k, field in (("chip", "chips"), ("M", "M"), ("rvec", "rvec"), ("tvec", "tvec"), ("euler", "euler"),
-                             ("reproject", "reproject")):
+                             ("reproject", "reproject"), ("id", "ids")):
                 if k in out:
                     setattr(outs, field, out[k].data_ptr())
         ptrs = (C.c_void_p * n)(*[f.data_ptr() for f in frames])
@@ -162,14 +168,16 @@ class FaceAnaStreams:
             r["M"] = ((S, K, 2, 3), f64)
         if self.pose:
             r.update(rvec=((S, K, 3), f64), tvec=((S, K, 3), f64), euler=((S, K, 3), f64), reproject=((S, K, 8, 2), f64))
+        if self.track_ids:
+            r["id"] = ((S, K), torch.int64)
         return r
 
     def new_results(self):
         """Device result buffers for submit(cuda_frames, out=...): a dict of CUDA tensors on this object's device,
         n (S,) int32 faces per stream; ran_detector (S,) int32, the frame-difference gate's decision; box (S,K,4) and kps
         (S,K,P,2) float64; scores (S,K,P) float32; with align, chip (S,K,size,size,3) uint8 and M (S,K,2,3) float64; with
-        pose, rvec, tvec, euler (S,K,3) and reproject (S,K,8,2) float64.  Per stream s, face rows i >= n[s] (and streams
-        past the batch's length) are unspecified."""
+        pose, rvec, tvec, euler (S,K,3) and reproject (S,K,8,2) float64; with track_ids, id (S,K) int64.  Per stream s,
+        face rows i >= n[s] (and streams past the batch's length) are unspecified."""
         import torch
         return {k: torch.empty(shape, dtype=dt, device=self.device) for k, (shape, dt) in self._result_layout().items()}
 
@@ -213,6 +221,8 @@ class FaceAnaStreams:
             q = o["pose"]
             rt.check(self.lib.skps_mpipe_pose_results(self._h, slot, q["rvec"].ctypes.data, q["tvec"].ctypes.data,
                                                       q["euler"].ctypes.data, q["reproject"].ctypes.data))
+        if self.track_ids:
+            rt.check(self.lib.skps_mpipe_track_ids(self._h, slot, o["ids"].ctypes.data))
         res = []
         for s in range(n):
             k = int(o["n"][s])
@@ -225,6 +235,9 @@ class FaceAnaStreams:
             if self.pose:
                 for i, r in enumerate(res[-1]):
                     r['pose'] = {k: v[s, i].copy() for k, v in o["pose"].items()}
+            if self.track_ids:
+                for i, r in enumerate(res[-1]):
+                    r['id'] = int(o["ids"][s, i])
         return res
 
     def run(self, frames):

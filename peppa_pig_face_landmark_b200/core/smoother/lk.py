@@ -62,6 +62,22 @@ def first_match(r1, r2, thres):
     return np.where(hit.any(1), hit.argmax(1), -1)
 
 
+def assign_track_ids(sources, prev_ids, next_id):
+    """Track ids of one call's faces, in output order.  sources[i] is the index into prev_ids (the ids of the previous
+    call's faces) of the track box face i continues, or -1.  A face inherits that id unless an earlier face of the call
+    already took it; every other face gets the next unused number.  Returns (ids as a list of ints, the new next_id)."""
+    ids, taken = [], set()
+    for s in sources:
+        s = int(s)
+        if s >= 0 and prev_ids[s] not in taken:
+            ids.append(prev_ids[s])
+        else:
+            ids.append(next_id)
+            next_id += 1
+        taken.add(ids[-1])
+    return ids, next_id
+
+
 def _iou(r1, r2):
     a1 = (r1[2] - r1[0]) * (r1[3] - r1[1])
     a2 = (r2[2] - r2[0]) * (r2[3] - r2[1])

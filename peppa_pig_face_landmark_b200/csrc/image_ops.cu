@@ -222,17 +222,19 @@ constexpr int SEL_THREADS = 256;
 constexpr int SEL_CACHE = 8192;       // area orders kept in shared memory (32 KB); later detections recompute theirs
 constexpr int SEL_MAX_K = SKPS_MAX_TOP_K;
 
-// judge_boxs for one detection: the box after the EMA with the first track box it matches (facer.py:176-181, lk.py:95-96)
-__device__ __forceinline__ void judged_box(const float* now, const float* __restrict__ track, int n_track, float iou_thres,
-                                           float alpha, float oma, float b[4]) {
+// judge_boxs for one detection: the box after the EMA with the first track box it matches (facer.py:176-181, lk.py:95-96).
+// Returns the index of that track box, -1 when none matches.
+__device__ __forceinline__ int judged_box(const float* now, const float* __restrict__ track, int n_track, float iou_thres,
+                                          float alpha, float oma, float b[4]) {
     b[0] = now[0]; b[1] = now[1]; b[2] = now[2]; b[3] = now[3];
     for (int j = 0; j < n_track; ++j) {
         const float* prev = track + j * 4;
         if (iou_track(now, prev) > iou_thres) {
             for (int c = 0; c < 4; ++c) b[c] = alpha * now[c] + oma * prev[c];
-            break;
+            return j;
         }
     }
+    return -1;
 }
 
 // Selection key of detection i: 0 when its area fails the filter, else (area, i) as one integer with the order of
@@ -257,10 +259,13 @@ __device__ __forceinline__ unsigned long long select_key(unsigned ord, int i) {
 // Selection for any top_k <= SEL_MAX_K in a number of passes over the keys that does not grow with top_k: a radix select
 // (8-bit digits, most significant first) finds the top_k-th largest key T, the keys >= T are gathered and bitonic-sorted
 // descending.  Keys past the shared cache are recomputed once per pass.
+// src, when not null, gets each selected face's source for the track ids: the row it was selected from when the rows are
+// the previous track boxes (src_is_row, the gate-skipped frame of facer.py:61), else the track box its detection matched
+// (-1 for none).
 __device__ __forceinline__ void select_faces_body(const float* __restrict__ det, int n_det, int det_stride,
                                                   const float* __restrict__ track, int n_track, float iou_thres, float alpha,
                                                   float oma, float min_face, int top_k, float* __restrict__ boxes4,
-                                                  int* __restrict__ count) {
+                                                  int* __restrict__ count, int* __restrict__ src, bool src_is_row) {
     __shared__ unsigned s_ord[SEL_CACHE];
     __shared__ unsigned long long s_win[SEL_MAX_K];
     __shared__ int s_sel[SEL_MAX_K];
@@ -374,16 +379,19 @@ __device__ __forceinline__ void select_faces_body(const float* __restrict__ det,
     if (tid == 0) *count = m;
     for (int f = tid; f < m; f += nt) {
         float b[4];
-        judged_box(det + (long long)s_sel[f] * det_stride, track, n_track, iou_thres, alpha, oma, b);
+        const int j = judged_box(det + (long long)s_sel[f] * det_stride, track, n_track, iou_thres, alpha, oma, b);
         for (int c = 0; c < 4; ++c) boxes4[f * 4 + c] = b[c];
+        if (src) src[f] = src_is_row ? s_sel[f] : j;
     }
 }
 
 __global__ void __launch_bounds__(256) select_faces_kernel(const float* __restrict__ det, const int* __restrict__ det_count,
                                                            int det_stride, const float* __restrict__ track, int n_track,
                                                            float iou_thres, float alpha, float oma, float min_face,
-                                                           int top_k, float* __restrict__ boxes4, int* __restrict__ count) {
-    select_faces_body(det, *det_count, det_stride, track, n_track, iou_thres, alpha, oma, min_face, top_k, boxes4, count);
+                                                           int top_k, float* __restrict__ boxes4, int* __restrict__ count,
+                                                           int* __restrict__ src, int src_is_row) {
+    select_faces_body(det, *det_count, det_stride, track, n_track, iou_thres, alpha, oma, min_face, top_k, boxes4, count,
+                      src, src_is_row != 0);
 }
 
 // Multi-stream variant (mpipe.cu): block = stream.  flag[s] != 0: this frame ran the detector -> judge_boxs(track, det rows)
@@ -392,15 +400,16 @@ __global__ void __launch_bounds__(256) mp_select_kernel(const float* __restrict_
                                                         int det_cap, const int* __restrict__ flag,
                                                         const float* __restrict__ track, const int* __restrict__ n_track,
                                                         float iou_thres, float alpha, float oma, float min_face, int top_k,
-                                                        float* __restrict__ boxes4, int* __restrict__ count) {
+                                                        float* __restrict__ boxes4, int* __restrict__ count,
+                                                        int* __restrict__ src) {
     const int s = blockIdx.x;
     const float* trk = track + (long long)s * top_k * 4;
     if (flag[s])
         select_faces_body(det_rows + (long long)s * det_cap * 16, det_count[s], 16, trk, n_track[s], iou_thres, alpha, oma,
-                          min_face, top_k, boxes4 + (long long)s * top_k * 4, count + s);
+                          min_face, top_k, boxes4 + (long long)s * top_k * 4, count + s, src + (long long)s * top_k, false);
     else
         select_faces_body(trk, n_track[s], 4, nullptr, 0, iou_thres, alpha, oma, min_face, top_k,
-                          boxes4 + (long long)s * top_k * 4, count + s);
+                          boxes4 + (long long)s * top_k * 4, count + s, src + (long long)s * top_k, true);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -624,9 +633,19 @@ int launch_mp_landmark_post(const float* xy, const int* detail, const int* count
 
 int launch_mp_select(const float* det_rows, const int* det_count, int det_cap, const int* flag, const float* track,
                      const int* n_track, float iou_thres, float alpha, float oma, float min_face, int top_k, float* boxes4,
-                     int* count, int n_streams, cudaStream_t s) {
+                     int* count, int* src, int n_streams, cudaStream_t s) {
     mp_select_kernel<<<n_streams, SEL_THREADS, 0, s>>>(det_rows, det_count, det_cap, flag, track, n_track, iou_thres, alpha, oma,
-                                                min_face, top_k, boxes4, count);
+                                                min_face, top_k, boxes4, count, src);
+    SKPS_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int launch_select_faces(const float* det_rows, const int32_t* det_count, int det_stride, const float* track, int n_track,
+                        float iou_thres, float alpha, float one_minus_alpha, float min_face, int top_k, float* boxes4,
+                        int32_t* count, int32_t* src, bool src_is_row, cudaStream_t s) {
+    SKPS_CHECK(det_rows && det_count && boxes4 && count && top_k > 0 && top_k <= SEL_MAX_K, "select_faces: bad arguments");
+    select_faces_kernel<<<1, SEL_THREADS, 0, s>>>(det_rows, det_count, det_stride, track, track ? n_track : 0, iou_thres, alpha,
+                                                  one_minus_alpha, min_face, top_k, boxes4, count, src, src_is_row ? 1 : 0);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }
@@ -650,12 +669,8 @@ extern "C" SKPS_API int skps_letterbox(const uint8_t* frame, int H, int W, int p
 extern "C" SKPS_API int skps_select_faces(const float* det_rows, const int32_t* det_count, int det_stride, const float* track,
                                  int n_track, float iou_thres, float alpha, float one_minus_alpha, float min_face,
                                  int top_k, float* boxes4, int32_t* count, void* stream) {
-    SKPS_CHECK(det_rows && det_count && boxes4 && count && top_k > 0 && top_k <= SEL_MAX_K, "select_faces: bad arguments");
-    select_faces_kernel<<<1, SEL_THREADS, 0, (cudaStream_t)stream>>>(det_rows, det_count, det_stride, track,
-                                                            track ? n_track : 0, iou_thres, alpha, one_minus_alpha,
-                                                            min_face, top_k, boxes4, count);
-    SKPS_CUDA(cudaGetLastError());
-    return 0;
+    return launch_select_faces(det_rows, det_count, det_stride, track, n_track, iou_thres, alpha, one_minus_alpha, min_face,
+                               top_k, boxes4, count, nullptr, false, (cudaStream_t)stream);
 }
 
 extern "C" SKPS_API int skps_crop_resize(const uint8_t* frame, int H, int W, int pitch, const float* boxes4,

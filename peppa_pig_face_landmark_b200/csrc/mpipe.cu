@@ -42,6 +42,7 @@ struct skps_mpipe {
         double* h_box = nullptr; double* h_kps = nullptr; float* h_scores = nullptr;
         uint8_t* h_chips = nullptr; double* h_M = nullptr;     // pinned, only while alignment is on
         double* h_pose = nullptr;             // pinned, only while pose is on: rvec, tvec, euler [n][K][3], reproject [n][K][8][2]
+        int64_t* h_ids = nullptr;             // pinned [S][K] track ids
         cudaEvent_t ev_in = nullptr, ev_done = nullptr;
         cudaEvent_t ev_staged = nullptr;      // the batch's uploads from the pinned h_hw / h_have_prev / h_desc are done
         int n = 0;
@@ -69,6 +70,10 @@ struct skps_mpipe {
     double *d_prev_lm = nullptr, *d_prev_dx = nullptr, *d_track = nullptr, *d_out_kps = nullptr;
     float* d_track_f32 = nullptr;
     int32_t *d_n_prev = nullptr, *d_prev_f32 = nullptr, *d_state_idx = nullptr, *d_n_track = nullptr;
+    // track ids: the source of each selected face, the id of each track box, the next unused id per stream
+    int32_t* d_src = nullptr;                 // [S][K]
+    int64_t* d_ids = nullptr;                 // [S][K]
+    int64_t* d_next_id = nullptr;             // [S]
 };
 
 static void letterbox_geometry(int H, int W, int in_h, int in_w, float* scale, int* rw, int* rh, int* top, int* left) {
@@ -88,7 +93,7 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
     for (uint8_t* f : p->d_frame) if (f) cudaFree(f);
     for (auto& sl : p->slot) {
         void* host[] = {sl.h_desc, sl.h_stage, sl.h_hw, sl.h_have_prev, sl.h_geom, sl.h_count, sl.h_flag, sl.h_box,
-                        sl.h_kps, sl.h_scores, sl.h_chips, sl.h_M, sl.h_pose};
+                        sl.h_kps, sl.h_scores, sl.h_chips, sl.h_M, sl.h_pose, sl.h_ids};
         for (void* q : host) if (q) cudaFreeHost(q);
         if (sl.ev_in) cudaEventDestroy(sl.ev_in);
         if (sl.ev_done) cudaEventDestroy(sl.ev_done);
@@ -99,7 +104,7 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
     void* dev[] = {p->d_desc, p->d_hw, p->d_have_prev, p->d_flag, p->d_det_count, p->d_det_idx, p->d_count, p->d_detail, p->d_diff,
                    p->d_det_rows, p->d_boxes, p->d_kps_now, p->d_prev_lm, p->d_prev_dx, p->d_track, p->d_out_kps,
                    p->d_track_f32, p->d_n_prev, p->d_prev_f32, p->d_state_idx, p->d_n_track, p->d_chips, p->d_align_M, p->d_pose,
-                   p->d_nms_ws};
+                   p->d_nms_ws, p->d_src, p->d_ids, p->d_next_id};
     for (void* q : dev) if (q) cudaFree(q);
     if (p->s_copy) cudaStreamDestroy(p->s_copy);
     if (p->s_compute) cudaStreamDestroy(p->s_compute);
@@ -112,10 +117,13 @@ extern "C" SKPS_API int skps_mpipe_reset(skps_mpipe* p, int stream) {
     SKPS_CUDA(cudaStreamSynchronize(p->s_compute));
     const int a = stream < 0 ? 0 : stream, b = stream < 0 ? p->S : stream + 1;
     for (int s = a; s < b; ++s) {
-        // FaceAna.reset (facer.py:200-208) + a fresh GroupTrack: no previous frame, no track boxes, no landmark history
+        // FaceAna.reset (facer.py:200-208) + a fresh GroupTrack: no previous frame, no track boxes, no landmark history;
+        // track ids number from 0 again
         p->prev_h[s] = p->prev_w[s] = 0;
         const int32_t zero = 0, none = -1, one = 1;
         SKPS_CUDA(cudaMemcpy(p->d_n_track + s, &zero, 4, cudaMemcpyHostToDevice));
+        SKPS_CUDA(cudaMemsetAsync(p->d_next_id + s, 0, 8, p->s_compute));
+        SKPS_CUDA(cudaMemsetAsync(p->d_ids + (size_t)s * p->K, 0xff, 8 * (size_t)p->K, p->s_compute));
         SKPS_CUDA(cudaMemcpy(p->d_n_prev + s, &none, 4, cudaMemcpyHostToDevice));
         SKPS_CUDA(cudaMemcpy(p->d_prev_f32 + s, &one, 4, cudaMemcpyHostToDevice));
     }
@@ -157,6 +165,7 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
         SKPS_HOST_ALLOC(sl.h_count, sizeof(int32_t) * S); SKPS_HOST_ALLOC(sl.h_flag, sizeof(int32_t) * S);
         SKPS_HOST_ALLOC(sl.h_box, sizeof(double) * 4 * K * S); SKPS_HOST_ALLOC(sl.h_kps, sizeof(double) * 2 * P * K * S);
         SKPS_HOST_ALLOC(sl.h_scores, sizeof(float) * P * K * S);
+        SKPS_HOST_ALLOC(sl.h_ids, sizeof(int64_t) * K * S);
         if (cudaEventCreateWithFlags(&sl.ev_in, cudaEventDisableTiming) != cudaSuccess ||
             cudaEventCreateWithFlags(&sl.ev_done, cudaEventDisableTiming) != cudaSuccess ||
             cudaEventCreateWithFlags(&sl.ev_staged, cudaEventDisableTiming) != cudaSuccess) { set_error("cudaEventCreate"); return fail("event"); }
@@ -175,6 +184,7 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
     SKPS_DEV_ALLOC(p->d_track_f32, 4 * 4 * (size_t)K * S);
     SKPS_DEV_ALLOC(p->d_n_prev, 4 * S); SKPS_DEV_ALLOC(p->d_prev_f32, 4 * S); SKPS_DEV_ALLOC(p->d_state_idx, 4 * S);
     SKPS_DEV_ALLOC(p->d_n_track, 4 * S);
+    SKPS_DEV_ALLOC(p->d_src, 4 * (size_t)K * S); SKPS_DEV_ALLOC(p->d_ids, 8 * (size_t)K * S); SKPS_DEV_ALLOC(p->d_next_id, 8 * S);
     cudaMemset(p->d_prev_lm, 0, 8 * 2 * 2 * (size_t)P * K * S); cudaMemset(p->d_prev_dx, 0, 8 * 2 * 2 * (size_t)P * K * S);
     cudaMemset(p->d_state_idx, 0, 4 * S); cudaMemset(p->d_track_f32, 0, 4 * 4 * (size_t)K * S);
     cudaMemset(p->d_track, 0, 8 * 4 * (size_t)K * S);
@@ -274,7 +284,7 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     na.ws = p->d_nms_ws; na.ws_cap = p->det_rows;
     if (launch_nms(na, sx)) return 1;
     if (launch_mp_select(p->d_det_rows, p->d_det_count, p->det_rows, p->d_flag, p->d_track_f32, p->d_n_track, c.track_iou,
-                         c.alpha, (float)(1.0 - (double)c.alpha), c.min_face, K, p->d_boxes, p->d_count, n, sx))
+                         c.alpha, (float)(1.0 - (double)c.alpha), c.min_face, K, p->d_boxes, p->d_count, p->d_src, n, sx))
         return 1;
     uint8_t* kps_in = (uint8_t*)skps_engine_input_ptr(p->kps);
     if (launch_mp_crop(p->d_desc, p->d_boxes, p->d_count, K, c.face_scale, c.kps_min_face, kps_in, p->kps_hw, p->d_detail, n, sx))
@@ -286,6 +296,7 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     a.kps_now = p->d_kps_now; a.count = p->d_count; a.flag = p->d_flag; a.hw = p->d_hw; a.boxes4 = p->d_boxes;
     a.prev_lm = p->d_prev_lm; a.prev_dx = p->d_prev_dx; a.n_prev = p->d_n_prev; a.prev_f32 = p->d_prev_f32;
     a.state_idx = p->d_state_idx; a.track_box = p->d_track; a.track_f32 = p->d_track_f32; a.n_track = p->d_n_track;
+    a.src = p->d_src; a.ids = p->d_ids; a.next_id = p->d_next_id;
     a.out_kps = p->d_out_kps;
     // the python floats of lk.py / facer.py, evaluated in the same order
     // (the cfg carries them as float32; Skps.yml's 0.5 / 0.3 come back exactly by rounding to 6 decimals in double)
@@ -329,6 +340,7 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     SKPS_CUDA(cudaMemcpyAsync(out ? out->kps : sl.h_kps, p->d_out_kps, 8 * 2 * (size_t)P * K * n, result_kind, sx));
     SKPS_CUDA(cudaMemcpyAsync(out ? out->scores : sl.h_scores, skps_engine_output_ptr(p->kps, 1), 4 * (size_t)P * K * n,
                               result_kind, sx));
+    if (!out || out->ids) SKPS_CUDA(cudaMemcpyAsync(out ? out->ids : sl.h_ids, p->d_ids, 8 * (size_t)K * n, result_kind, sx));
     SKPS_CUDA(cudaEventRecord(sl.ev_done, sx));
     // ring discipline: this batch read positions r (previous) and r+1 (current); the next batch uploads into r+2 (free), the
     // one after into r again - and that one reuses this slot, so the caller has passed skps_mpipe_wait(slot) by then
@@ -477,6 +489,15 @@ extern "C" SKPS_API int skps_mpipe_pose_results(skps_mpipe* p, int slot_i, doubl
     memcpy(tvec, sl.h_pose + 3 * faces, faces * 3 * sizeof(double));
     memcpy(euler, sl.h_pose + 6 * faces, faces * 3 * sizeof(double));
     memcpy(reproject, sl.h_pose + 9 * faces, faces * 16 * sizeof(double));
+    return 0;
+}
+
+extern "C" SKPS_API int skps_mpipe_track_ids(skps_mpipe* p, int slot_i, int64_t* ids) {
+    SKPS_CHECK(p && (slot_i == 0 || slot_i == 1) && ids, "mpipe_track_ids: bad arguments");
+    const skps_mpipe::Slot& sl = p->slot[slot_i];
+    SKPS_CHECK(!sl.busy, "mpipe_track_ids: slot %d is in flight (call skps_mpipe_wait first)", slot_i);
+    SKPS_CHECK(sl.n > 0 && !sl.device_out, "mpipe_track_ids: slot %d was not submitted with host results", slot_i);
+    memcpy(ids, sl.h_ids, sizeof(int64_t) * sl.n * p->K);
     return 0;
 }
 

@@ -21,6 +21,9 @@ struct MpTemporalArgs {
     double* track_box;           // [S][K][4] float64 track boxes (returned as 'box')
     float* track_f32;            // [S][K][4] the same, as float32 (next frame's judge_boxs / crop input)
     int* n_track;                // [S]
+    const int* src;              // [S][K] source of each face this frame (launch_mp_select), an index into the old track
+    int64_t* ids;                // [S][K] track id of each track box
+    int64_t* next_id;            // [S] the next unused id of the stream
     // outputs
     double* out_kps;             // [S][K][P][2]
     // constants (python floats computed on the host exactly as lk.py does)
@@ -77,9 +80,16 @@ int launch_mp_crop(const MpStreamDesc* d, const float* boxes, const int* count, 
                    uint8_t* crops, int S, int* detail, int n, cudaStream_t s);
 int launch_mp_landmark_post(const float* xy, const int* detail, const int* count, int K, int P, float* kps, int n, cudaStream_t s);
 
+// judge_boxs + sort_and_filter (image_ops.cu).  src [dev] (top_k) or null: each selected face's source for the track ids,
+// the row it came from when src_is_row (the rows are the previous track boxes), else the index of the track box its
+// detection matched, -1 for none.  skps_select_faces is this with src null.
+int launch_select_faces(const float* det_rows, const int32_t* det_count, int det_stride, const float* track, int n_track,
+                        float iou_thres, float alpha, float one_minus_alpha, float min_face, int top_k, float* boxes4,
+                        int32_t* count, int32_t* src, bool src_is_row, cudaStream_t s);
+// The same per stream of a batch; src [dev] [S][K] as above, the rows being the track boxes where flag[s] == 0.
 int launch_mp_select(const float* det_rows, const int* det_count, int det_cap, const int* flag, const float* track,
                      const int* n_track, float iou_thres, float alpha, float oma, float min_face, int top_k, float* boxes4,
-                     int* count, int n_streams, cudaStream_t s);
+                     int* count, int* src, int n_streams, cudaStream_t s);
 int launch_mp_decide(const unsigned long long* diff, const int* hw, const int* have_prev, int* flag, int n, cudaStream_t s);
 int launch_mp_temporal(const MpTemporalArgs& a, int n_streams, cudaStream_t s);
 // Aligned face chips (align.cu): per face of stream g < n with i < count[g], M = similarity of kps[g][i] (P x 2 float64) to the

@@ -32,7 +32,9 @@ struct skps_pipeline {
     uint8_t* h_frame = nullptr;                   // pinned staging
     float* d_det_rows = nullptr; int32_t* d_det_idx = nullptr; int32_t* d_det_count = nullptr;
     float* d_track = nullptr;
+    // d_boxes / h_boxes: top_k boxes, then the top_k int32 sources of the track ids (one D2H copy for both)
     float* d_boxes = nullptr; int32_t* d_count = nullptr; int32_t* d_detail = nullptr;
+    int last_n_faces = 0;                         // faces of the last skps_pipeline_run
     float* d_kps = nullptr; float* d_scores = nullptr;
     int32_t* d_counts = nullptr;                  // d_counts[c] = c for c in 0..SKPS_LANDMARK_CHUNK: per-chunk face counts
     int track_cap = 0;                            // track boxes accepted: max(256, top_k)
@@ -70,6 +72,8 @@ extern "C" SKPS_API void skps_pipeline_destroy(skps_pipeline* p) {
     delete p;
 }
 
+static size_t boxes_block_bytes(int K) { return (sizeof(float) * 4 + sizeof(int32_t)) * (size_t)K; }
+
 extern "C" SKPS_API int skps_pipeline_create(skps_engine* det, skps_engine* kps, const skps_pipeline_cfg* cfg,
                                     skps_pipeline** out) {
     SKPS_CHECK(det && kps && cfg && out, "pipeline_create: null argument");
@@ -102,7 +106,7 @@ extern "C" SKPS_API int skps_pipeline_create(skps_engine* det, skps_engine* kps,
     SKPS_DEV_ALLOC(p->d_nms_ws, nms_workspace_bytes(p->det_rows, 1));
     p->track_cap = K > 256 ? K : 256;
     SKPS_DEV_ALLOC(p->d_track, sizeof(float) * 4 * p->track_cap);
-    SKPS_DEV_ALLOC(p->d_boxes, sizeof(float) * 4 * K);
+    SKPS_DEV_ALLOC(p->d_boxes, boxes_block_bytes(K));
     SKPS_DEV_ALLOC(p->d_count, sizeof(int32_t));
     SKPS_DEV_ALLOC(p->d_detail, sizeof(int32_t) * 5 * K);
     SKPS_DEV_ALLOC(p->d_kps, sizeof(float) * 2 * P * K);
@@ -110,7 +114,7 @@ extern "C" SKPS_API int skps_pipeline_create(skps_engine* det, skps_engine* kps,
     SKPS_DEV_ALLOC(p->d_counts, sizeof(int32_t) * (SKPS_LANDMARK_CHUNK + 1));
     SKPS_DEV_ALLOC(p->d_diff, sizeof(unsigned long long));
     SKPS_HOST_ALLOC(p->h_res, sizeof(skps_pipeline::Host));
-    SKPS_HOST_ALLOC(p->h_boxes, sizeof(float) * 4 * K);
+    SKPS_HOST_ALLOC(p->h_boxes, boxes_block_bytes(K));
     SKPS_HOST_ALLOC(p->h_kps, sizeof(float) * 2 * P * K);
     SKPS_HOST_ALLOC(p->h_scores, sizeof(float) * P * K);
     SKPS_HOST_ALLOC(p->h_det_idx, sizeof(int32_t) * skps_pipeline::RUN_DET);
@@ -132,6 +136,7 @@ extern "C" SKPS_API int skps_pipeline_create(skps_engine* det, skps_engine* kps,
 extern "C" SKPS_API int skps_pipeline_reset(skps_pipeline* p) {
     SKPS_CHECK(p, "pipeline_reset: null");
     p->prev_h = p->prev_w = 0;            // FaceAna.reset (facer.py:200-208): previous_image = None
+    p->last_n_faces = 0;
     return 0;
 }
 
@@ -207,6 +212,7 @@ extern "C" SKPS_API int skps_pipeline_commit_frame(skps_pipeline* p) {
     SKPS_CHECK(p, "commit_frame: null");
     SKPS_CHECK(p->cur_h > 0, "commit_frame: no frame staged (call skps_pipeline_frame_diff or _frame_diff_device first)");
     advance_frame(p);
+    p->last_n_faces = 0;
     return 0;
 }
 
@@ -221,6 +227,7 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, int run_detector, in
     const skps_pipeline_cfg& c = p->cfg;
     const int K = c.top_k, P = p->n_points, H = p->cur_h, W = p->cur_w;
     const uint8_t* d_frame = p->d_frame[p->cur];
+    int32_t* d_src = (int32_t*)(p->d_boxes + 4 * K);
     if (n_track > 0) {
         SKPS_CHECK(track, "pipeline_run: track is null");
         memcpy(p->h_track, track, sizeof(float) * 4 * n_track);
@@ -239,17 +246,17 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, int run_detector, in
         na.ws = p->d_nms_ws; na.ws_cap = p->det_rows;
         if (launch_nms(na, s)) return 1;
         // facer.py:58 judge_boxs(track_box, boxes) then :64 sort_and_filter
-        if (skps_select_faces(p->d_det_rows, p->d_det_count, 16, n_track > 0 ? p->d_track : nullptr, n_track,
-                              c.track_iou, c.alpha, (float)(1.0 - (double)c.alpha), c.min_face, K, p->d_boxes,
-                              p->d_count, s))
+        if (launch_select_faces(p->d_det_rows, p->d_det_count, 16, n_track > 0 ? p->d_track : nullptr, n_track,
+                                c.track_iou, c.alpha, (float)(1.0 - (double)c.alpha), c.min_face, K, p->d_boxes,
+                                p->d_count, d_src, false, s))
             return 1;
     } else {
         // facer.py:61: boxes = track_box, then sort_and_filter
         int32_t nt = n_track;
         p->h_res->n_det = nt;
         SKPS_CUDA(cudaMemcpyAsync(p->d_det_count, &p->h_res->n_det, sizeof(int32_t), cudaMemcpyHostToDevice, s));
-        if (skps_select_faces(p->d_track, p->d_det_count, 4, nullptr, 0, c.track_iou, c.alpha,
-                              (float)(1.0 - (double)c.alpha), c.min_face, K, p->d_boxes, p->d_count, s))
+        if (launch_select_faces(p->d_track, p->d_det_count, 4, nullptr, 0, c.track_iou, c.alpha,
+                                (float)(1.0 - (double)c.alpha), c.min_face, K, p->d_boxes, p->d_count, d_src, true, s))
             return 1;
     }
     // the face count decides how many crops the landmark net sees
@@ -272,7 +279,7 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, int run_detector, in
             return 1;
     }
     if (nf > 0) {
-        SKPS_CUDA(cudaMemcpyAsync(p->h_boxes, p->d_boxes, sizeof(float) * 4 * nf, cudaMemcpyDeviceToHost, s));
+        SKPS_CUDA(cudaMemcpyAsync(p->h_boxes, p->d_boxes, boxes_block_bytes(K), cudaMemcpyDeviceToHost, s));
         SKPS_CUDA(cudaMemcpyAsync(p->h_kps, p->d_kps, sizeof(float) * 2 * P * nf, cudaMemcpyDeviceToHost, s));
         SKPS_CUDA(cudaMemcpyAsync(p->h_scores, p->d_scores, sizeof(float) * P * nf, cudaMemcpyDeviceToHost, s));
     }
@@ -286,6 +293,7 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, int run_detector, in
     }
     SKPS_CUDA(cudaStreamSynchronize(s));
     if (run_detector) p->last_n_det = p->h_res->n_det;
+    p->last_n_faces = nf;
     *n_faces = nf;
     memcpy(boxes4, p->h_boxes, sizeof(float) * 4 * nf);
     memcpy(kps, p->h_kps, sizeof(float) * 2 * P * nf);
@@ -297,6 +305,15 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, int run_detector, in
         if (run_detector && det_rows) memcpy(det_rows, p->h_det_rows, sizeof(float) * 16 * nr);
     }
     advance_frame(p);
+    return 0;
+}
+
+// The sources skps_pipeline_run's selection found, kept in host memory by its D2H copy: no device work, no synchronisation.
+extern "C" SKPS_API int skps_pipeline_face_sources(skps_pipeline* p, int n, int32_t* src) {
+    SKPS_CHECK(p && src, "pipeline_face_sources: null argument");
+    SKPS_CHECK(n >= 0 && n <= p->last_n_faces, "pipeline_face_sources: the last run returned %d faces, asked for %d",
+               p->last_n_faces, n);
+    memcpy(src, (const int32_t*)(p->h_boxes + 4 * p->cfg.top_k), sizeof(int32_t) * n);
     return 0;
 }
 

@@ -90,6 +90,7 @@ __global__ void __launch_bounds__(128) mp_temporal_kernel(const MpTemporalArgs a
     __shared__ double red[16];
     __shared__ double rect_now[4], rect_prev[4];
     __shared__ int s_match;
+    __shared__ int64_t s_ids[64];                                     // the old track ids (skps_mpipe_create: top_k <= 64)
     const int n = a.count[s];
     const float* now = a.kps_now + (long long)s * K * set;            // float32 (n, P, 2)
     const int cur = a.state_idx[s], nxt = cur ^ 1;
@@ -185,6 +186,23 @@ __global__ void __launch_bounds__(128) mp_temporal_kernel(const MpTemporalArgs a
         __syncthreads();
     }
     if (tid == 0) {
+        // track ids, in output order: a face inherits the id of its source track box unless an earlier face of this frame
+        // took it; every other face gets the stream's next number.  The new ids are index-aligned with the new track boxes.
+        int64_t* ids = a.ids + (long long)s * K;
+        const int n_old = a.n_track[s];
+        for (int j = 0; j < n_old; ++j) s_ids[j] = ids[j];
+        unsigned long long taken = 0ull;                              // bit j: track box j's id is given out (K <= 64)
+        int64_t next = a.next_id[s];
+        for (int i = 0; i < n; ++i) {
+            const int j = a.src[(long long)s * K + i];
+            if (j >= 0 && j < n_old && !((taken >> j) & 1ull)) {
+                taken |= 1ull << j;
+                ids[i] = s_ids[j];
+            } else {
+                ids[i] = next++;
+            }
+        }
+        a.next_id[s] = next;
         a.n_prev[s] = n;
         a.prev_f32[s] = all_f32 ? 1 : 0;
         a.n_track[s] = n;

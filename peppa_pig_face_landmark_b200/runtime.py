@@ -28,7 +28,7 @@ class PipelineCfg(C.Structure):
 class MpipeOutputs(C.Structure):
     """skps_mpipe_outputs: device addresses of one batch's result buffers."""
     _fields_ = [(name, c_vp) for name in ("n_faces", "ran_detector", "boxes", "kps", "scores", "chips", "M", "rvec", "tvec",
-                                          "euler", "reproject")]
+                                          "euler", "reproject", "ids")]
 
 
 # name -> (restype, argtypes); every symbol include/skps_b200.h declares
@@ -94,6 +94,7 @@ SIGNATURES = {
     "skps_pipeline_run": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, c_vp, C.c_int,
                                     c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "skps_pipeline_det_results": (C.c_int, [c_vp, C.c_int, c_vp, c_vp]),
+    "skps_pipeline_face_sources": (C.c_int, [c_vp, C.c_int, c_vp]),
     "skps_crop_rect": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, C.c_int, c_vp]),
     "skps_nme": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
     "skps_head_pose": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
@@ -105,6 +106,7 @@ SIGNATURES = {
     "skps_mpipe_wait": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "skps_mpipe_submit_device": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int, C.POINTER(MpipeOutputs), c_vp]),
     "skps_mpipe_wait_stream": (C.c_int, [c_vp, C.c_int, c_vp]),
+    "skps_mpipe_track_ids": (C.c_int, [c_vp, C.c_int, c_vp]),
     "skps_pipeline_commit_frame": (C.c_int, [c_vp]),
     "skps_pipeline_frame_diff": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.POINTER(C.c_double), c_vp]),
     "skps_pipeline_frame_diff_device": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, C.POINTER(C.c_double), c_vp]),

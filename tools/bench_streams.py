@@ -7,6 +7,7 @@ host results out: every H2D / D2H is inside the timed region.
     python tools/bench_streams.py --align 112 [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
     python tools/bench_streams.py --pose [--parent-headpose OLD_headpose.cu --out DIR] [--rounds 5] [--configs ...]
     python tools/bench_streams.py --det-input H W [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
+    python tools/bench_streams.py --track-ids [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
 
 --align SIZE times every config with and without aligned face chips (FaceAnaStreams(align=SIZE)) in the same process,
 alternating the two over --rounds rounds, and reports the median ms_per_call of both.  At 4k_16faces it also times the
@@ -19,6 +20,8 @@ csrc/headpose.cu into a side library under --out (not part of the package), time
 run and reports the largest difference of its skps_head_pose results from this build's on tests/test_headpose_gpu.py's inputs.
 
 --det-input H W does the same with the detector at Skps.yml's 384x640 and at H x W (FaceAnaStreams(det_input=(H, W))).
+
+--track-ids does the same without and with track ids in the results (FaceAnaStreams(track_ids=True)).
 
 Under torchrun every rank drives its own S streams on its own GPU (streams shard across GPUs, no collective on the data
 path); time = max over ranks.  --gather adds one NCCL all_gather of the packed (box, landmarks, scores) rows per call."""
@@ -167,15 +170,17 @@ def time_align_kernel(torch, frame, kps, size, iters=200):
 
 
 def run_align_pair(name, size, n_streams=16, batches=12, warmup=3, rounds=5, length=6, feature="align"):
-    """The same config with and without alignment (feature="align", chip side `size`), head pose (feature="pose") or the
-    detector at input size `size` = (h, w) (feature="det_input"), alternating; median ms_per_call of each."""
+    """The same config with and without alignment (feature="align", chip side `size`), head pose (feature="pose"), track
+    ids (feature="track_ids") or the detector at input size `size` = (h, w) (feature="det_input"), alternating; median
+    ms_per_call of each."""
     import torch
     import frames
     from Skps import FaceAnaStreams
     maker, topk = getattr(frames, CONFIGS[name][0]), CONFIGS[name][1]
     seqs = make_streams(torch, frames, maker, n_streams, length=length)
     H, W = seqs[0][0].shape[:2]
-    on = {"align": {"align": size}, "pose": {"pose": True}, "det_input": {"det_input": size}}[feature]
+    on = {"align": {"align": size}, "pose": {"pose": True}, "det_input": {"det_input": size},
+          "track_ids": {"track_ids": True}}[feature]
     fas = {"off": FaceAnaStreams(n_streams=n_streams, top_k=topk, max_frame_hw=(H, W)),
            "on": FaceAnaStreams(n_streams=n_streams, top_k=topk, max_frame_hw=(H, W), **on)}
     L = len(seqs[0])
@@ -216,6 +221,16 @@ def run_align_pair(name, size, n_streams=16, batches=12, warmup=3, rounds=5, len
                 "faces_per_frame_384x640": faces["off"] / (n_streams * batches),
                 "faces_per_frame_det_input": faces["on"] / (n_streams * batches),
                 "api": "FaceAnaStreams.submit/collect, pinned host frames, 2 calls in flight"}
+    if feature == "track_ids":
+        del fas
+        ms = {k: 1e3 * float(np.median(v)) / batches for k, v in times.items()}
+        return {"config": name, "streams_per_gpu": n_streams, "calls": batches, "rounds": rounds,
+                "ms_per_call": ms["off"], "ms_per_call_track_ids": ms["on"],
+                "frames_per_s": 1e3 * n_streams / ms["off"], "frames_per_s_track_ids": 1e3 * n_streams / ms["on"],
+                "ms_per_call_rounds": [1e3 * v / batches for v in times["off"]],
+                "ms_per_call_track_ids_rounds": [1e3 * v / batches for v in times["on"]],
+                "faces_per_frame": faces["on"] / (n_streams * batches),
+                "api": "FaceAnaStreams.submit/collect, pinned host frames, 2 calls in flight; ids kept on the device"}
     if feature == "pose":
         del fas
         return {"config": name, "streams_per_gpu": n_streams, "calls": batches, "rounds": rounds,
@@ -358,6 +373,13 @@ def main():
         print(json.dumps(gpu_info(torch)))
         for name in names:
             print(json.dumps(run_align_pair(name, hw, n_streams, batches, rounds=rounds, feature="det_input")))
+            sys.stdout.flush()
+        return
+    if "--track-ids" in a:
+        rounds = int(opt("--rounds", 5))
+        print(json.dumps(gpu_info(torch)))
+        for name in names:
+            print(json.dumps(run_align_pair(name, 0, n_streams, batches, rounds=rounds, feature="track_ids")))
             sys.stdout.flush()
         return
     if "--align" in a:
