@@ -398,6 +398,24 @@ SKPS_API int skps_mpipe_wait_stream(skps_mpipe* p, int slot, void* consumer_stre
  * skps_mpipe_reset.  After skps_mpipe_wait(slot): ids [host] (n, top_k) int64, n = that submit's stream count; entries
  * i >= n_faces[s] are undefined.  Device results get them through skps_mpipe_outputs.ids. */
 SKPS_API int skps_mpipe_track_ids(skps_mpipe* p, int slot, int64_t* ids);
+/* Debug/unit-test entry of the temporal step of skps_mpipe_submit (csrc/temporal.cu): GroupTrack.calculate, the track-box
+ * EMA of judge_boxs and the track ids, for streams 0..n_streams-1 in one launch, with the constants skps_mpipe_submit derives
+ * from cfg (its track_iou and alpha; top_k is the argument).  All other pointers [dev], laid out as skps_mpipe keeps them
+ * (S >= n_streams, K = top_k in 1..64, P = n_points):
+ *   inputs  kps_now (S,K,P,2) float32, count (S), flag (S) detector ran, hw (S,2) frame H, W, boxes4 (S,K,4) float32 boxes of
+ *           the landmark stage, src (S,K) each face's source track box or -1; count[s] <= K;
+ *   state   updated in place: prev_lm, prev_dx (S,2,K,P,2) float64, n_prev (S) (-1: none), prev_f32 (S), state_idx (S)
+ *           (which half of prev_lm / prev_dx is current), track_box (S,K,4) float64, track_f32 (S,K,4), n_track (S) <= K,
+ *           ids (S,K) int64, next_id (S) int64; skps_mpipe_create / skps_mpipe_reset start a stream at n_prev = -1,
+ *           prev_f32 = 1, n_track = 0, ids -1, next_id = 0, state_idx 0 and every buffer zero;
+ *   output  out_kps (S,K,P,2) float64 smoothed landmarks.
+ * Streams >= n_streams are not touched.  Asynchronous on `stream`. */
+SKPS_API int skps_debug_mp_temporal(const skps_pipeline_cfg* cfg, int n_streams, int top_k, int n_points,
+                                    const float* kps_now, const int32_t* count, const int32_t* flag, const int32_t* hw,
+                                    const float* boxes4, const int32_t* src, double* prev_lm, double* prev_dx,
+                                    int32_t* n_prev, int32_t* prev_f32, int32_t* state_idx, double* track_box,
+                                    float* track_f32, int32_t* n_track, int64_t* ids, int64_t* next_id, double* out_kps,
+                                    void* stream);
 
 /* ---- Aligned face chips (csrc/align.cu; additive) -----------------------------------------------------------------------
  * What a caller does with the 98 landmarks before a recognition / attribute model: estimate the least-squares similarity

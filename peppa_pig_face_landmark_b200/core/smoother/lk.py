@@ -65,11 +65,12 @@ def first_match(r1, r2, thres):
 def assign_track_ids(sources, prev_ids, next_id):
     """Track ids of one call's faces, in output order.  sources[i] is the index into prev_ids (the ids of the previous
     call's faces) of the track box face i continues, or -1.  A face inherits that id unless an earlier face of the call
-    already took it; every other face gets the next unused number.  Returns (ids as a list of ints, the new next_id)."""
+    already took it; every other face, including one whose source is past the previous call's faces, gets the next unused
+    number, as on the device.  Returns (ids as a list of ints, the new next_id)."""
     ids, taken = [], set()
     for s in sources:
         s = int(s)
-        if s >= 0 and prev_ids[s] not in taken:
+        if 0 <= s < len(prev_ids) and prev_ids[s] not in taken:
             ids.append(prev_ids[s])
         else:
             ids.append(next_id)

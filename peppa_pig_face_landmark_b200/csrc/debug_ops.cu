@@ -1,6 +1,7 @@
 // Unit-test entry points for the fused kernels that otherwise only run inside a whole network: the squeeze-excite gate
 // (se_fc_kernel), the heat-map decode (hm_decode_kernel) and the fused producer -> 1x1 conv layers (conv_xf.cu,
-// conv_fpw.cu).  Host float32 in/out.
+// conv_fpw.cu), host float32 in/out; and for the temporal step of the multi-stream pipeline (temporal.cu) on device
+// buffers the caller owns.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 #include <string.h>
@@ -9,6 +10,7 @@
 #include "common.h"
 #include "conv_fpw.h"
 #include "conv_xf.h"
+#include "mpipe_kernels.h"
 
 using namespace skps;
 
@@ -162,6 +164,28 @@ extern "C" SKPS_API int skps_debug_conv_xf(int mode, const float* x, int N, int 
                                            int out_split, float* out, const float* weff) {
     return debug_conv_fused(false, mode, x, N, H, W, Cx, x_split, low, Cl, gate, dww, dw_act, w_hi, w_lo, bias, Cout, act,
                             n_tile, out_scale, residual, res_first, out_split, out, weff, N);
+}
+
+// One launch of the temporal step of skps_mpipe_submit (mp_temporal_kernel) for streams [0, n_streams), with the constants
+// skps_mpipe_submit derives from the cfg and the state in the caller's device buffers (MpTemporalArgs layouts).
+extern "C" SKPS_API int skps_debug_mp_temporal(const skps_pipeline_cfg* cfg, int n_streams, int top_k, int n_points,
+                                               const float* kps_now, const int32_t* count, const int32_t* flag,
+                                               const int32_t* hw, const float* boxes4, const int32_t* src, double* prev_lm,
+                                               double* prev_dx, int32_t* n_prev, int32_t* prev_f32, int32_t* state_idx,
+                                               double* track_box, float* track_f32, int32_t* n_track, int64_t* ids,
+                                               int64_t* next_id, double* out_kps, void* stream) {
+    SKPS_CHECK(cfg && kps_now && count && flag && hw && boxes4 && src && prev_lm && prev_dx && n_prev && prev_f32 &&
+               state_idx && track_box && track_f32 && n_track && ids && next_id && out_kps, "debug_mp_temporal: null argument");
+    SKPS_CHECK(top_k > 0 && top_k <= 64, "debug_mp_temporal: top_k %d outside 1..64", top_k);
+    SKPS_CHECK(n_streams > 0 && n_points > 0, "debug_mp_temporal: %d streams of %d points", n_streams, n_points);
+    MpTemporalArgs a;
+    a.top_k = top_k; a.n_points = n_points;
+    a.kps_now = kps_now; a.count = count; a.flag = flag; a.hw = hw; a.boxes4 = boxes4;
+    a.prev_lm = prev_lm; a.prev_dx = prev_dx; a.n_prev = n_prev; a.prev_f32 = prev_f32; a.state_idx = state_idx;
+    a.track_box = track_box; a.track_f32 = track_f32; a.n_track = n_track; a.src = src; a.ids = ids; a.next_id = next_id;
+    a.out_kps = out_kps;
+    mp_temporal_constants(*cfg, a);
+    return launch_mp_temporal(a, n_streams, (cudaStream_t)stream);
 }
 
 // One fused layer through conv_fpw on host data (tests/test_conv_fpw_gpu.py).  The arguments of skps_debug_conv_xf, then

@@ -85,6 +85,17 @@ static void letterbox_geometry(int H, int W, int in_h, int in_w, float* scale, i
     *scale = (float)s;
 }
 
+void skps::mp_temporal_constants(const skps_pipeline_cfg& c, MpTemporalArgs& a) {
+    // the python floats of lk.py / facer.py, evaluated in the same order
+    // (the cfg carries them as float32; Skps.yml's 0.5 / 0.3 come back exactly by rounding to 6 decimals in double)
+    a.iou_thres = nearbyint((double)c.track_iou * 1e6) / 1e6;
+    a.alpha = nearbyint((double)c.alpha * 1e6) / 1e6;
+    a.one_minus_alpha = 1.0 - a.alpha;
+    a.two_pi = 2 * 3.141592653589793;
+    { const double r = a.two_pi * 1.0 * 1.0; a.a_d = r / (r + 1); a.one_minus_a_d = 1 - a.a_d; }
+    a.min_cutoff = 0.15; a.beta = 0.8;
+}
+
 extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
     if (!p) return;
     cudaSetDevice(p->device);
@@ -298,14 +309,7 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     a.state_idx = p->d_state_idx; a.track_box = p->d_track; a.track_f32 = p->d_track_f32; a.n_track = p->d_n_track;
     a.src = p->d_src; a.ids = p->d_ids; a.next_id = p->d_next_id;
     a.out_kps = p->d_out_kps;
-    // the python floats of lk.py / facer.py, evaluated in the same order
-    // (the cfg carries them as float32; Skps.yml's 0.5 / 0.3 come back exactly by rounding to 6 decimals in double)
-    a.iou_thres = nearbyint((double)c.track_iou * 1e6) / 1e6;
-    a.alpha = nearbyint((double)c.alpha * 1e6) / 1e6;
-    a.one_minus_alpha = 1.0 - a.alpha;
-    a.two_pi = 2 * 3.141592653589793;
-    { const double r = a.two_pi * 1.0 * 1.0; a.a_d = r / (r + 1); a.one_minus_a_d = 1 - a.a_d; }
-    a.min_cutoff = 0.15; a.beta = 0.8;
+    mp_temporal_constants(c, a);
     if (launch_mp_temporal(a, n, sx)) return 1;
     sl.align = p->align_size;
     if (sl.align) {

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+struct skps_pipeline_cfg;
+
 namespace skps {
 
 struct MpTemporalArgs {
@@ -29,6 +31,8 @@ struct MpTemporalArgs {
     // constants (python floats computed on the host exactly as lk.py does)
     double iou_thres, alpha, one_minus_alpha, a_d, one_minus_a_d, min_cutoff, beta, two_pi;
 };
+// Sets the constants of `a` from the pipeline's cfg (mpipe.cu): what skps_mpipe_submit and skps_debug_mp_temporal launch with.
+void mp_temporal_constants(const skps_pipeline_cfg& c, MpTemporalArgs& a);
 
 // One frame of one stream as the batched pre/post-processing kernels see it (filled on the host per call, one upload).
 struct MpStreamDesc {

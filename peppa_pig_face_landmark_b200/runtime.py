@@ -107,6 +107,7 @@ SIGNATURES = {
     "skps_mpipe_submit_device": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int, C.POINTER(MpipeOutputs), c_vp]),
     "skps_mpipe_wait_stream": (C.c_int, [c_vp, C.c_int, c_vp]),
     "skps_mpipe_track_ids": (C.c_int, [c_vp, C.c_int, c_vp]),
+    "skps_debug_mp_temporal": (C.c_int, [C.POINTER(PipelineCfg), C.c_int, C.c_int, C.c_int] + [c_vp] * 18),
     "skps_pipeline_commit_frame": (C.c_int, [c_vp]),
     "skps_pipeline_frame_diff": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.POINTER(C.c_double), c_vp]),
     "skps_pipeline_frame_diff_device": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, C.POINTER(C.c_double), c_vp]),

@@ -66,6 +66,13 @@ def test_numbering_after_reset():
     assert t.call([-1, -1]) == [0, 1]
 
 
+def test_a_source_past_the_previous_faces_gets_a_fresh_number():
+    t = _Track()
+    t.call([-1, -1])                            # ids 0, 1
+    assert t.call([2, 1, 5, 0]) == [2, 1, 3, 0]
+    assert t.next_id == 4
+
+
 def test_ids_are_python_ints():
     ids, nxt = assign_track_ids(np.array([-1, 0], np.int32), [7], 8)
     assert ids == [8, 7] and nxt == 9
