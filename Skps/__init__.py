@@ -2,5 +2,6 @@
 from peppa_pig_face_landmark_b200.core.api.facer import FaceAna
 
 from peppa_pig_face_landmark_b200.core.api.streams import FaceAnaStreams   # additive: many streams per GPU
+from peppa_pig_face_landmark_b200.core.api.face_landmark import FaceLandmark   # additive: landmarks on the caller's boxes
 
-__all__ = ['FaceAna', 'FaceAnaStreams']
+__all__ = ['FaceAna', 'FaceAnaStreams', 'FaceLandmark']

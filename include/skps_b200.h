@@ -233,6 +233,26 @@ SKPS_API int skps_crop_resize(const uint8_t* frame, int H, int W, int pitch,
                      float face_scale /* float32(1+2*extend) */, float min_face,
                      uint8_t* crops, int out_hw, int32_t* detail, void* stream);
 
+/* Where one face's pixels are, for skps_crop_faces: `base` [dev] holds the rectangle of an H x W
+ * frame that starts at column ox, row oy and is rw x rh pixels, rows `pitch` bytes apart.  A face
+ * in a whole frame has ox = oy = 0, rw = W, rh = H; a face may also point at just the rectangle its
+ * crop can read (FaceLandmark's host frames upload only that). */
+typedef struct skps_face_src {
+    const uint8_t* base;
+    int32_t pitch;
+    int32_t H, W;                       /* the whole frame                               */
+    int32_t ox, oy, rw, rh;             /* the rectangle base holds                      */
+    int32_t _pad;
+} skps_face_src;
+
+/* skps_crop_resize for n faces (0..65535) that may each come from a different frame, in one launch:
+ * face i is cropped from src[i] [dev] with box boxes4[i] [dev] (n,4).  Geometry, zero border and
+ * bilinear are skps_crop_resize's, so crops [dev] (n,out_hw,out_hw,3) and detail [dev] (n,5) are
+ * the bytes it writes for the same box on the whole frame.  The rectangle of src[i] must hold
+ * every pixel of the frame the crop reads. */
+SKPS_API int skps_crop_faces(const skps_face_src* src, const float* boxes4, int n, float face_scale,
+                             float min_face, uint8_t* crops, int out_hw, int32_t* detail, void* stream);
+
 /* FaceLandmark.postprocess (face_landmark.py:106-115): x*w + x1 - add, y*h + y1 - add. */
 SKPS_API int skps_landmark_post(const float* xy_norm, const int32_t* detail, const int32_t* count,
                        int max_faces, int n_points, float* kps, void* stream);

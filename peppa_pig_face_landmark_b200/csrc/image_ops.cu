@@ -106,6 +106,37 @@ __device__ __forceinline__ CropGeo crop_geometry(const float* b, int H, int W, f
     return g;
 }
 
+// Output pixel (x, y) of the crop of one face with box b into o, and at (0, 0) its detail d = [h, w, y1, x1, add].  The
+// frame is H x W; `base` holds only its rectangle starting at column ox, row oy, rows `pitch` bytes apart.  Whether a tap
+// is in the frame or in the zero border is decided against the whole frame, so a caller that holds only the rectangle
+// the taps can reach gets the same bytes as one that holds the whole frame (ox = oy = 0).
+__device__ __forceinline__ void crop_face_px(const uint8_t* __restrict__ base, int H, int W, int pitch, int ox, int oy,
+                                             const float* __restrict__ b, float face_scale, float min_face,
+                                             uint8_t* __restrict__ o, int S, int* __restrict__ d, int x, int y) {
+    CropGeo g = crop_geometry(b, H, W, face_scale, min_face);
+    if (x == 0 && y == 0) {
+        d[0] = g.h; d[1] = g.w; d[2] = g.y1; d[3] = g.x1; d[4] = g.add;
+    }
+    if (!g.ok) { o[0] = 0; o[1] = 0; o[2] = 0; return; }
+    Tap tx = linear_tap(x, S, g.w, true);
+    Tap ty = linear_tap(y, S, g.h, false);
+    // crop coordinates -> frame coordinates (outside the frame = the zero border)
+    int fx0 = g.x1 + tx.i0 - g.add, fx1 = g.x1 + tx.i1 - g.add;
+    int fy0 = g.y1 + ty.i0 - g.add, fy1 = g.y1 + ty.i1 - g.add;
+    bool vx0 = fx0 >= 0 && fx0 < W, vx1 = fx1 >= 0 && fx1 < W;
+    bool vy0 = fy0 >= 0 && fy0 < H, vy1 = fy1 >= 0 && fy1 < H;
+    const uint8_t* r0 = base + (long long)((vy0 ? fy0 : oy) - oy) * pitch;
+    const uint8_t* r1 = base + (long long)((vy1 ? fy1 : oy) - oy) * pitch;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        int p00 = (vy0 && vx0) ? r0[(fx0 - ox) * 3 + c] : 0, p01 = (vy0 && vx1) ? r0[(fx1 - ox) * 3 + c] : 0;
+        int p10 = (vy1 && vx0) ? r1[(fx0 - ox) * 3 + c] : 0, p11 = (vy1 && vx1) ? r1[(fx1 - ox) * 3 + c] : 0;
+        int h0 = p00 * tx.w0 + p01 * tx.w1;
+        int h1 = p10 * tx.w0 + p11 * tx.w1;
+        o[c] = (uint8_t)vblend(h0, h1, ty.w0, ty.w1);          // stays BGR (face_landmark.py:44)
+    }
+}
+
 __device__ __forceinline__ void crop_px(const uint8_t* __restrict__ frame, int H, int W, int pitch,
                                         const float* __restrict__ boxes, const int* __restrict__ count, float face_scale,
                                         float min_face, uint8_t* __restrict__ crops, int S, int* __restrict__ detail,
@@ -118,29 +149,7 @@ __device__ __forceinline__ void crop_px(const uint8_t* __restrict__ frame, int H
         if (x == 0 && y == 0) { for (int k = 0; k < 5; ++k) detail[face * 5 + k] = 0; }
         return;
     }
-    CropGeo g = crop_geometry(boxes + face * 4, H, W, face_scale, min_face);
-    if (x == 0 && y == 0) {
-        detail[face * 5 + 0] = g.h; detail[face * 5 + 1] = g.w;
-        detail[face * 5 + 2] = g.y1; detail[face * 5 + 3] = g.x1; detail[face * 5 + 4] = g.add;
-    }
-    if (!g.ok) { o[0] = 0; o[1] = 0; o[2] = 0; return; }
-    Tap tx = linear_tap(x, S, g.w, true);
-    Tap ty = linear_tap(y, S, g.h, false);
-    // crop coordinates -> frame coordinates (outside the frame = the zero border)
-    int fx0 = g.x1 + tx.i0 - g.add, fx1 = g.x1 + tx.i1 - g.add;
-    int fy0 = g.y1 + ty.i0 - g.add, fy1 = g.y1 + ty.i1 - g.add;
-    bool vx0 = fx0 >= 0 && fx0 < W, vx1 = fx1 >= 0 && fx1 < W;
-    bool vy0 = fy0 >= 0 && fy0 < H, vy1 = fy1 >= 0 && fy1 < H;
-    const uint8_t* r0 = frame + (long long)(vy0 ? fy0 : 0) * pitch;
-    const uint8_t* r1 = frame + (long long)(vy1 ? fy1 : 0) * pitch;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        int p00 = (vy0 && vx0) ? r0[fx0 * 3 + c] : 0, p01 = (vy0 && vx1) ? r0[fx1 * 3 + c] : 0;
-        int p10 = (vy1 && vx0) ? r1[fx0 * 3 + c] : 0, p11 = (vy1 && vx1) ? r1[fx1 * 3 + c] : 0;
-        int h0 = p00 * tx.w0 + p01 * tx.w1;
-        int h1 = p10 * tx.w0 + p11 * tx.w1;
-        o[c] = (uint8_t)vblend(h0, h1, ty.w0, ty.w1);          // stays BGR (face_landmark.py:44)
-    }
+    crop_face_px(frame, H, W, pitch, 0, 0, boxes + face * 4, face_scale, min_face, o, S, detail + face * 5, x, y);
 }
 __global__ void __launch_bounds__(256) crop_resize_kernel(const uint8_t* __restrict__ frame, int H, int W, int pitch,
                                                           const float* __restrict__ boxes, const int* __restrict__ count,
@@ -156,6 +165,16 @@ __global__ void __launch_bounds__(256) mp_crop_kernel(const MpStreamDesc* __rest
     const MpStreamDesc D = d[st];
     crop_px(D.cur, D.H, D.W, D.W * 3, boxes + (size_t)4 * K * st, count + st, face_scale, min_face,
             crops + (size_t)S * S * 3 * K * st, S, detail + (size_t)5 * K * st, face, blockIdx.x * blockDim.x + threadIdx.x, blockIdx.y);
+}
+// Face table variant (FaceLandmark.submit): block z = face, each face with its own frame or frame rectangle.
+__global__ void __launch_bounds__(256) crop_faces_kernel(const skps_face_src* __restrict__ src, const float* __restrict__ boxes,
+                                                         float face_scale, float min_face, uint8_t* __restrict__ crops, int S,
+                                                         int* __restrict__ detail) {
+    const int face = blockIdx.z, x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+    if (x >= S) return;
+    const skps_face_src F = src[face];
+    crop_face_px(F.base, F.H, F.W, F.pitch, F.ox, F.oy, boxes + face * 4, face_scale, min_face,
+                 crops + (((long long)face * S + y) * S + x) * 3, S, detail + face * 5, x, y);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -680,6 +699,17 @@ extern "C" SKPS_API int skps_crop_resize(const uint8_t* frame, int H, int W, int
     dim3 grid((out_hw + 255) / 256, out_hw, max_faces);
     crop_resize_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(frame, H, W, pitch, boxes4, count, face_scale,
                                                                min_face, crops, out_hw, detail);
+    SKPS_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" SKPS_API int skps_crop_faces(const skps_face_src* src, const float* boxes4, int n, float face_scale, float min_face,
+                                        uint8_t* crops, int out_hw, int32_t* detail, void* stream) {
+    SKPS_CHECK(n >= 0 && n <= 65535 && out_hw > 0, "crop_faces: n %d outside 0..65535 or out_hw %d", n, out_hw);
+    if (n == 0) return 0;
+    SKPS_CHECK(src && boxes4 && crops && detail, "crop_faces: bad arguments");
+    dim3 grid((out_hw + 255) / 256, out_hw, n);
+    crop_faces_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src, boxes4, face_scale, min_face, crops, out_hw, detail);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }

@@ -85,6 +85,7 @@ SIGNATURES = {
                                     C.c_float, C.c_int, c_vp, c_vp, c_vp]),
     "skps_crop_resize": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, C.c_int, C.c_float, C.c_float,
                                    c_vp, C.c_int, c_vp, c_vp]),
+    "skps_crop_faces": (C.c_int, [c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, C.c_int, c_vp, c_vp]),
     "skps_landmark_post": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_int, c_vp, c_vp]),
     "skps_frame_absdiff_sum": (C.c_int, [c_vp, c_vp, C.c_size_t, c_vp, c_vp]),
     "skps_frame_ingest": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp]),
