@@ -356,10 +356,21 @@ SKPS_API int skps_nme(const float* target, const float* preds, int n, int n_poin
 /* Batched head pose (csrc/headpose.cu), the GPU counterpart of Skps/core/headpose/pose.py:48-77 get_head_pose():
  * solvePnP (iterative) on 10 landmark/model point pairs with the camera matrix [[w,0,w//2],[0,w,h//2],[0,0,1]], projection
  * of the 8 cube corners, Euler angles as cv2.decomposeProjectionMatrix reports them.  pts [host] (N,10,2) float32 in the
- * order of pose.py:60-61; object_pts (10,3), cube_pts (8,3) float32.  Outputs [host] float64: rvec, tvec, euler (N,3),
- * reproject (N,8,2). */
+ * order of pose.py:60-61; object_pts (10,3), cube_pts (8,3) float32.  Outputs [host] float64: rvec (|rvec| <= pi), tvec,
+ * euler (N,3), reproject (N,8,2).  The Euler triple is the classic RQDecomp3x3's; where the decomposition is ambiguous it
+ * can differ from OpenCV's while composing to the same R = Rz(roll) Ry(yaw) Rx(pitch): at a pitch of exactly 180 degrees
+ * with nonzero yaw (Ry(pi - 0.1): (180, 5.73, 180) here, (0, 174.27, 0) from OpenCV 4.13), at exact 180-degree rotations
+ * about some axes, and within |cos yaw| < 1e-3 of gimbal lock, where the first Givens rotation is normalised exactly. */
 SKPS_API int skps_head_pose(const float* pts, int N, int img_w, int img_h, const float* object_pts, const float* cube_pts,
                             double* rvec, double* tvec, double* euler, double* reproject);
+
+/* The head-pose solver's rotation helpers on their own, run in device code (test entry): R_out[i] = rotation matrix of the
+ * rotation vector r_in[i] (cv2.Rodrigues), r_out[i] = rotation vector of R_in[i] (cv2.Rodrigues of a matrix), euler_out[i]
+ * = Euler angles of R_in[i] in degrees (cv2.RQDecomp3x3; at exact 180-degree rotations about some axes and within about 1e-5
+ * of yaw = +-90 degrees the triple may differ from OpenCV's but composes to the same R).  r_in (n,3), R_in (n,3,3)
+ * row-major; all [host] float64. */
+SKPS_API int skps_debug_rotation(const double* r_in, const double* R_in, int n, double* R_out, double* r_out,
+                                 double* euler_out);
 
 /* ---- FaceAna.run for many concurrent video streams (csrc/mpipe.cu; SURVEY 8f-1, 8f-2) ---------------------------------
  * What one FaceAna instance per stream does on the host in the reference (facer.py:52-85 with GroupTrack / OneEuroFilter /
@@ -475,7 +486,7 @@ SKPS_API int skps_mpipe_align_results(skps_mpipe* p, int slot, uint8_t* chips, d
  * landmarks [33, 37, 42, 46, 60, 64, 68, 72, 55, 59], rounded to float32, paired with the model points of pose.py, the
  * camera [[W,0,W//2],[0,W,H//2],[0,0,1]] of the face's frame; the same solver as skps_head_pose, one warp per face.
  * Outputs float64: rvec, tvec, euler (degrees, in the order cv2.decomposeProjectionMatrix returns) (3,) and the 8
- * re-projected cube corners (8,2) per face. */
+ * re-projected cube corners (8,2) per face; Euler angles as described at skps_head_pose. */
 /* FaceAna, whose landmarks are smoothed on the host: kps [host] (n,n_points,2) float64, H x W the frame they belong to;
  * rvec, tvec, euler [host] (n,3), reproject [host] (n,8,2).  n <= top_k.  Buffers are allocated on the first call; the work
  * is ordered on `stream`, and the call returns once that stream has reached it.  Synchronous. */

@@ -6,7 +6,10 @@
 // One warp per face, float64.  The start value follows OpenCV's (direct linear transform on normalised image points,
 // rotation = orthogonal polar factor), the refinement minimises the pixel reprojection error over (rvec, tvec) with
 // Levenberg-Marquardt until the step is below 1e-12 - i.e. the same local minimum OpenCV's 20-iteration solver approaches;
-// agreement with cv2 is checked in tests/test_headpose_gpu.py (tolerance stated there).
+// agreement with cv2 is checked in tests/test_headpose_gpu.py (tolerance stated there), stationarity and agreement over
+// the pose space in tests/test_headpose_edges_gpu.py.  The damping grows until a step improves (up to lambda = 1e16), so
+// the solver ends no worse than cv2 on small noisy faces too; a few of those (about 1 in 100 below 50 px) lie in a long
+// flat valley that it has not crossed after 100 iterations, where cv2's 20 have not either.
 // The lanes share the parallel parts: the 12x12 normal matrix, the row / column updates of every Jacobi rotation, the 12
 // residual evaluations of the numeric Jacobian, J^T J / J^T e and the 6x6 elimination.  Every sum runs in a fixed order
 // (the one-thread solver's, except the Jacobi stopping test), so a face's pose does not depend on the other faces of a launch.
@@ -70,23 +73,39 @@ __device__ void project(const double* R, const double* t, const float* X, double
     uv[0] = f * x / z + cx; uv[1] = f * y / z + cy;
 }
 
-// cv::RQDecomp3x3 on a rotation matrix -> Euler angles in degrees (what cv2.decomposeProjectionMatrix returns for [R|t])
+// Normalise a Givens pair (c, s) the way cv::RQDecomp3x3 does, 1 / sqrt(c^2 + s^2 + DBL_EPSILON), while that is a rotation
+// to within sqrt(DBL_EPSILON / (c^2 + s^2)) <= 1.5e-5 in the angle.  Below |(c, s)| = 1e-3 (only the first pair, at
+// |cos yaw| < 1e-3) the epsilon would dominate and leave Qx far from a rotation - the Euler triple would then not compose
+// back to R (off by up to 2 within 1e-8 of yaw = +-90 degrees) - so there the pair is normalised exactly, and an all-zero
+// pair (yaw exactly +-90) is taken as (1, 0), i.e. pitch 0 and the whole rotation about z in the roll.
+__device__ __forceinline__ void givens_unit(double& c, double& s) {
+    const double n2 = c * c + s * s, z = 1.0 / sqrt(n2 + (n2 >= 1e-6 ? 2.220446049250313e-16 : 0.0));
+    c = n2 > 0 ? c * z : 1.0;
+    s = n2 > 0 ? s * z : 0.0;
+}
+
+// cv::RQDecomp3x3 on a rotation matrix -> Euler angles in degrees (what cv2.decomposeProjectionMatrix returns for [R|t]).
+// This is the classic Givens-rotation RQDecomp3x3.  Where the decomposition is not unique it may pick a different triple
+// than a given OpenCV build: at an exact 180-degree pitch (R[2][1] = 0 and R[2][2] < 0, e.g. Ry(pi - 0.1): (180, 5.73, 180)
+// here, (0, 174.27, 0) from OpenCV 4.13; also the exact 180-degree rotations about some axes) and near yaw = +-90 degrees
+// (gimbal lock, where only pitch - roll or pitch + roll is defined).  The triple always composes back to the same
+// R = Rz(roll) Ry(yaw) Rx(pitch); tests/test_headpose_edges_gpu.py pins that.
 __device__ void euler_rq(const double* Rin, double* eul) {
     double M[9];
     for (int i = 0; i < 9; ++i) M[i] = Rin[i];
     auto mul = [](const double* A, const double* B, double* C) {
         for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) C[i * 3 + j] = A[i * 3] * B[j] + A[i * 3 + 1] * B[3 + j] + A[i * 3 + 2] * B[6 + j];
     };
-    double s = M[7], c = M[8], z = 1.0 / sqrt(c * c + s * s + 2.220446049250313e-16);
-    c *= z; s *= z;
+    double s = M[7], c = M[8];
+    givens_unit(c, s);
     double Qx[9] = {1, 0, 0, 0, c, s, 0, -s, c}, R[9];
     mul(M, Qx, R);
-    s = -R[6]; c = R[8]; z = 1.0 / sqrt(c * c + s * s + 2.220446049250313e-16);
-    c *= z; s *= z;
+    s = -R[6]; c = R[8];
+    givens_unit(c, s);
     double Qy[9] = {c, 0, -s, 0, 1, 0, s, 0, c};
     mul(R, Qy, M);
-    s = M[3]; c = M[4]; z = 1.0 / sqrt(c * c + s * s + 2.220446049250313e-16);
-    c *= z; s *= z;
+    s = M[3]; c = M[4];
+    givens_unit(c, s);
     double Qz[9] = {c, s, 0, -s, c, 0, 0, 0, 1};
     mul(M, Qz, R);
     // decomposition ambiguity: diagonal entries of R (except the last) positive; rotate by 180 degrees where needed
@@ -283,7 +302,9 @@ __global__ void __launch_bounds__(HP_WARPS * 32) head_pose_warp_kernel(const Pos
         __syncwarp();
         bool improved = false;
         double step = 0;
-        for (int tries = 0; tries < 12 && !improved; ++tries) {
+        // Raise the damping until a step improves, up to lambda = 1e16 (a gradient step of relative size 1e-16): a fixed
+        // number of tries ended small noisy faces at points that were neither stationary nor as good as cv2's.
+        while (!improved && lambda <= 1e16) {
             for (int t = lane; t < 42; t += 32) {
                 const int r = t / 7, c = t - 7 * r;
                 double v;
@@ -344,11 +365,17 @@ __global__ void __launch_bounds__(HP_WARPS * 32) head_pose_warp_kernel(const Pos
         }
         if (!improved || step < 1e-24) break;
     }
-    // keep the rotation vector in [0, pi] like cv2.Rodrigues(cv2.Rodrigues(r)) would
+    // Report the rotation vector with |r| <= pi: shorten the angle by the nearest multiple of 2 pi on the same axis (the
+    // iterations may leave it several turns long on small noisy faces).  A round trip through the matrix would do the same
+    // but loses up to 2e-5 near theta = pi, where rodrigues_inv rebuilds the axis from the diagonal only (the frontal
+    // face [pi, 0, 0] is right there).  r waits in S.h (free once the iterations end) so that it does not stay in
+    // registers across rodrigues.
+    if (lane == 0) for (int i = 0; i < 3; ++i) S.h[i] = p[i];
     rodrigues(p, R);
-    rodrigues_inv(R, p);
     if (lane == 0) {
-        for (int i = 0; i < 3; ++i) { a.rvec[(size_t)face * 3 + i] = p[i]; a.tvec[(size_t)face * 3 + i] = p[3 + i]; }
+        const double th = sqrt(S.h[0] * S.h[0] + S.h[1] * S.h[1] + S.h[2] * S.h[2]);
+        const double k = th > M_PI ? (th - 2 * M_PI * rint(th / (2 * M_PI))) / th : 1.0;
+        for (int i = 0; i < 3; ++i) { a.rvec[(size_t)face * 3 + i] = S.h[i] * k; a.tvec[(size_t)face * 3 + i] = p[3 + i]; }
         euler_rq(R, a.euler + (size_t)face * 3);
     }
     if (lane < 8) project(R, p + 3, S.cube + 3 * lane, f, cx, cy, a.reproj + ((size_t)face * 8 + lane) * 2);
@@ -367,6 +394,15 @@ void pose_model_98(PoseArgs& a) {
     memcpy(a.idx, idx, sizeof(idx));
     memcpy(a.obj, obj, sizeof(obj));
     memcpy(a.cube, cube, sizeof(cube));
+}
+
+__global__ void debug_rotation_kernel(const double* r_in, const double* R_in, int n, double* R_out, double* r_out,
+                                      double* euler_out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    rodrigues(r_in + 3 * (size_t)i, R_out + 9 * (size_t)i);
+    rodrigues_inv(R_in + 9 * (size_t)i, r_out + 3 * (size_t)i);
+    euler_rq(R_in + 9 * (size_t)i, euler_out + 3 * (size_t)i);
 }
 
 int launch_head_pose(const PoseArgs& a, cudaStream_t s) {
@@ -410,5 +446,28 @@ extern "C" SKPS_API int skps_head_pose(const float* pts, int N, int img_w, int i
     const cudaError_t err = cudaGetLastError();
     cudaFree(d_pts); cudaFree(d_out);
     SKPS_CHECK(!rc, "head_pose: %s", err == cudaSuccess ? get_error() : cudaGetErrorString(err));
+    return 0;
+}
+
+// The solver's rotation helpers on their own, in device code: R_out[i] = rodrigues(r_in[i]); r_out[i] = rodrigues_inv(R_in[i]);
+// euler_out[i] = euler_rq(R_in[i]).  r_in (n,3), R_in (n,3,3) row-major, all [host] float64.
+extern "C" SKPS_API int skps_debug_rotation(const double* r_in, const double* R_in, int n, double* R_out, double* r_out,
+                                            double* euler_out) {
+    SKPS_CHECK(r_in && R_in && R_out && r_out && euler_out && n > 0, "debug_rotation: bad arguments");
+    double* d = nullptr;
+    SKPS_CUDA(cudaMalloc(&d, (size_t)n * 30 * 8));
+    double *dr = d, *dR = d + (size_t)n * 3, *dRo = d + (size_t)n * 12, *dro = d + (size_t)n * 21, *de = d + (size_t)n * 24;
+    int rc = cudaMemcpy(dr, r_in, (size_t)n * 24, cudaMemcpyHostToDevice) != cudaSuccess ||
+             cudaMemcpy(dR, R_in, (size_t)n * 72, cudaMemcpyHostToDevice) != cudaSuccess;
+    cudaError_t err = cudaSuccess;
+    if (!rc) {
+        debug_rotation_kernel<<<(n + 127) / 128, 128>>>(dr, dR, n, dRo, dro, de);
+        err = cudaGetLastError();
+        if (err == cudaSuccess) err = cudaMemcpy(R_out, dRo, (size_t)n * 72, cudaMemcpyDeviceToHost);
+        if (err == cudaSuccess) err = cudaMemcpy(r_out, dro, (size_t)n * 24, cudaMemcpyDeviceToHost);
+        if (err == cudaSuccess) err = cudaMemcpy(euler_out, de, (size_t)n * 24, cudaMemcpyDeviceToHost);
+    }
+    cudaFree(d);
+    SKPS_CHECK(!rc && err == cudaSuccess, "debug_rotation: %s", rc ? "cannot copy the inputs" : cudaGetErrorString(err));
     return 0;
 }

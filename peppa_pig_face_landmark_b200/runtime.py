@@ -99,6 +99,7 @@ SIGNATURES = {
     "skps_crop_rect": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, C.c_int, c_vp]),
     "skps_nme": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
     "skps_head_pose": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "skps_debug_rotation": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_vp, c_vp]),
     "skps_mpipe_create": (C.c_int, [c_vp, c_vp, C.POINTER(PipelineCfg), C.c_int, C.POINTER(c_vp)]),
     "skps_mpipe_destroy": (None, [c_vp]),
     "skps_mpipe_reset": (C.c_int, [c_vp, C.c_int]),

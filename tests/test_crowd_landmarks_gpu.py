@@ -143,7 +143,10 @@ def test_faceana_crowd_chips_and_pose(crowd384):
     from Skps import FaceAna
     facer = FaceAna(top_k=512, det_input=(1152, 1920), align=112, pose=True)
     plain = FaceAna(top_k=512, det_input=(1152, 1920))
+    from Skps.core.headpose.pose import POSE_POINTS_98
+    from test_headpose_edges_gpu import cost, cv2_solve, is_stationary, not_worse_bound, stationarity
     res, want = facer.run(crowd384), plain.run(crowd384)
+    hw = crowd384.shape[:2]
     assert len(res) == 384
     for r, w in zip(res, want):
         assert np.array_equal(r["kps"], w["kps"]) and np.array_equal(r["box"], w["box"])
@@ -151,6 +154,10 @@ def test_faceana_crowd_chips_and_pose(crowd384):
         assert r["M"].shape == (2, 3) and np.isfinite(r["M"]).all()
         p = r["pose"]
         assert p["euler"].shape == (3,) and np.isfinite(p["euler"]).all() and np.isfinite(p["reproject"]).all()
+        # every face's pose is a stationary point of its reprojection error and no worse than cv2.solvePnP's
+        img = np.asarray(r["kps"], np.float32)[POSE_POINTS_98]
+        assert is_stationary(img, p["rvec"], p["tvec"], hw), stationarity(img, p["rvec"], p["tvec"], hw)
+        assert cost(img, p["rvec"], p["tvec"], hw) <= not_worse_bound(img, *cv2_solve(img, hw), hw)
     # every face of the crowd is the same picture, so every chip is nearly the same
     chips = np.stack([r["chip"] for r in res]).astype(np.int16)
     assert np.median(np.abs(chips - chips[0]).mean(axis=(1, 2, 3))) < 20
