@@ -394,7 +394,8 @@ SKPS_API int skps_mpipe_dims(const skps_mpipe* p, int* n_streams, int* top_k, in
 SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot, const uint8_t* const* frames, const int32_t* hw, int n);
 /* Block until the slot's results are in host memory.  Per stream s < n: n_faces[s]; boxes (n, top_k, 4) float64 = the
  * refreshed track boxes (the 'box' entries of FaceAna.run); kps (n, top_k, n_points, 2) float64 smoothed landmarks;
- * scores (n, top_k, n_points) float32; ran_detector[s] (may be NULL) = the frame-difference gate's decision. */
+ * scores (n, top_k, n_points) float32; ran_detector[s] (may be NULL) = the frame used the detector's rows (the
+ * frame-difference gate's decision on a keyframe; every frame is one unless skps_mpipe_set_detect_every says otherwise). */
 SKPS_API int skps_mpipe_wait(skps_mpipe* p, int slot, int32_t* n_faces, double* boxes, double* kps, float* scores,
                              int32_t* ran_detector);
 /* Caller-owned [dev] result buffers of one batch, on the pipeline's device, laid out as skps_mpipe_wait /
@@ -500,6 +501,17 @@ SKPS_API int skps_mpipe_set_pose(skps_mpipe* p, int on);
 /* After skps_mpipe_wait(slot), for a slot submitted with pose on: rvec, tvec, euler [host] (n, top_k, 3) and reproject
  * [host] (n, top_k, 8, 2) float64, n = that submit's stream count; entries i >= n_faces[s] are undefined. */
 SKPS_API int skps_mpipe_pose_results(skps_mpipe* p, int slot, double* rvec, double* tvec, double* euler, double* reproject);
+
+/* ---- Detection cadence (csrc/mpipe.cu; additive) -----------------------------------------------------------------------
+ * Each stream counts its frames from skps_mpipe_create / skps_mpipe_reset: i = 0, 1, 2, ..., advanced only by submits that
+ * include a frame for it.  With every = N, stream s's frame i is a keyframe when the stream has no previous frame of this
+ * frame's size, or when (i + s % N) % N == 0; only keyframes are letterboxed, run through the detector and NMS (packed, in
+ * stream order, as one batch of m frames), and a keyframe's rows are used when the frame-difference gate fires or there is
+ * no previous frame of its size.  Every other frame takes the tracker path on the track boxes.  every = 1 (the default):
+ * every frame is a keyframe, as without this call.  Takes effect from the next submit; the frame counters keep running. */
+SKPS_API int skps_mpipe_set_detect_every(skps_mpipe* p, int every);
+/* The number of frames the detector ran on in the slot's last submitted batch (0..n; 0 skips the detector). */
+SKPS_API int skps_mpipe_detector_frames(const skps_mpipe* p, int slot, int* m);
 
 #ifdef __cplusplus
 }

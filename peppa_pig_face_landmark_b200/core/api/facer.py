@@ -27,6 +27,36 @@ MAX_TOP_K = 1024           # SKPS_MAX_TOP_K of include/skps_b200.h
 LANDMARK_CHUNK = 64        # SKPS_LANDMARK_CHUNK: faces per landmark forward in skps_pipeline_run
 
 
+def check_detect_every(every, offset=0):
+    """(every, offset) as ints: every >= 1 and offset in 0..every-1, else ValueError."""
+    def is_int(v):
+        return isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_))
+    if not is_int(every) or every < 1:
+        raise ValueError("detect_every must be an int >= 1, got %r" % (every,))
+    if not is_int(offset) or not 0 <= offset < every:
+        raise ValueError("detect_offset must be an int in 0..%d, got %r" % (every - 1, offset))
+    return int(every), int(offset)
+
+
+class DetectCadence:
+    """The detection cadence of one stream: frames are counted from construction or reset(), i = 0, 1, 2, ..., and frame
+    i is a keyframe when it is forced (no previous frame of its size) or (i + offset) % every == 0.  FaceAna keeps one;
+    skps_mpipe keeps the same count per stream in C, with offset s % every."""
+
+    def __init__(self, every=1, offset=0):
+        self.every, self.offset = check_detect_every(every, offset)
+        self.frame = 0
+
+    def step(self, forced):
+        """Whether the next frame is a keyframe; counts it."""
+        key = bool(forced) or (self.frame + self.offset) % self.every == 0
+        self.frame += 1
+        return key
+
+    def reset(self):
+        self.frame = 0
+
+
 def get_cfg():
     root_path = pathlib.Path(__file__).resolve().parents[2]
     cfg_path = os.path.join(root_path, 'config', 'Skps.yml')
@@ -45,7 +75,7 @@ def pipeline_cfg(cfg, top_k, max_frame_hw):
 
 class FaceAna():
     def __init__(self, verbose=False, top_k=None, max_frame_hw=(2160, 3840), align=None, pose=False, det_input=None,
-                 track_ids=False):
+                 track_ids=False, detect_every=1, detect_offset=0):
         """align: None, or a chip side in 16..512: every result dict then also carries 'chip' ((align, align, 3) uint8
         BGR, the face warped to the ArcFace five-point template) and 'M' ((2, 3) float64, the frame -> chip matrix for
         cv2.warpAffine), computed on the GPU from the returned 'kps' and the frame already in HBM (core/api/align.py).
@@ -64,7 +94,16 @@ class FaceAna():
         (the match judge_boxs smooths the box with), or none; on a frame the difference gate skipped, the previous face
         it is.  In the order of the returned list, a face inherits its source's id unless an earlier face of the same
         call already took it, and every other face gets the next unused number.  A face the tracker loses for one frame
-        comes back with a new id: there is no re-identification."""
+        comes back with a new id: there is no re-identification.
+        detect_every, detect_offset: the detection cadence.  Frames are counted from construction or reset(), i = 0, 1,
+        2, ...; frame i runs the detector when there is no previous frame of its size (the first frame, a size change),
+        or when (i + detect_offset) % detect_every == 0 and the frame-difference gate fires.  Every other frame takes the
+        tracker path on the last frame's landmark boxes, One-Euro smoothing included.  So a face that enters the scene is
+        found at the next keyframe, up to detect_every - 1 frames late, and a face that leaves is followed by its
+        landmark box until the next keyframe.  detect_every=1 (the default) is the reference's behaviour.
+        last_ran_detector tells whether the last run() used the detector."""
+        self._cadence = DetectCadence(detect_every, detect_offset)
+        self.detect_every, self.detect_offset = self._cadence.every, self._cadence.offset
         cfg = get_cfg()
         self.top_k = int(top_k if top_k is not None else cfg['Skps']['Detect']['topk'])
         if not 1 <= self.top_k <= MAX_TOP_K:
@@ -111,6 +150,7 @@ class FaceAna():
         self._have_prev = False
         self._ids, self._next_id = [], 0     # ids of the track boxes (index-aligned with track_box), next unused id
         self.last_det_idx = None       # kept detector rows of the last detector run (parity checks)
+        self.last_ran_detector = None
         self.last_det_rows = None
 
     def __del__(self):
@@ -128,7 +168,10 @@ class FaceAna():
         work already queued on it, and work queued on it after run() returns runs after the frame has been read, so a
         decoder may overwrite the surface at once."""
         image = image if is_cuda_tensor(image) else check_host_frame(image)
-        run_det = self.diff_frames(self.previous_image, image)     # checks a CUDA frame, stages the frame on the device
+        d = self._frame_diff(image)     # checks a CUDA frame, stages the frame on the device
+        forced = self.previous_image is None or d < 0       # no previous frame of this size
+        run_det = self._cadence.step(forced) and (forced or d > self.diff_thres)
+        self.last_ran_detector = run_det
         H, W = image.shape[:2]
         self.previous_image = image
         det = self.face_detector
@@ -215,6 +258,14 @@ class FaceAna():
     def diff_frames(self, previous_frame, image):
         """facer.py:98-118: mean |prev - cur| > 5 -> run the detector.  The sum is taken on the GPU
         against the previous frame kept in HBM; the frame uploaded here is reused by run()."""
+        d = self._frame_diff(image)
+        if previous_frame is None or d < 0:
+            return True
+        return bool(d > self.diff_thres)
+
+    def _frame_diff(self, image):
+        """Stages `image` on the device and returns the mean |prev - cur| against the previous staged frame, or a
+        negative number when that frame has another size (or there is none)."""
         d = C.c_double(0.0)
         if is_cuda_tensor(image):
             import torch
@@ -225,9 +276,7 @@ class FaceAna():
         else:
             rt.check(self.lib.skps_pipeline_frame_diff(self._pipe, image.ctypes.data, *image.shape[:2], C.byref(d),
                                                        self._stream.cuda_stream))
-        if previous_frame is None or d.value < 0:
-            return True
-        return bool(d.value > self.diff_thres)
+        return d.value
 
     def sort_and_filter(self, bboxes):
         """facer.py:120-142 (host copy of what skps_select_faces does on the device)."""
@@ -267,5 +316,6 @@ class FaceAna():
         self.previous_image = None
         self.previous_box = None
         self._ids, self._next_id = [], 0
+        self._cadence.reset()
         rt.check(self.lib.skps_pipeline_reset(self._pipe))
 

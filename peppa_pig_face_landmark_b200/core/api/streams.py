@@ -10,6 +10,7 @@ device (csrc/mpipe.cu, csrc/temporal.cu) and two batches can be in flight so tha
     # FaceAnaStreams(..., align=112): each dict also has 'chip' (112x112x3 uint8, aligned) and 'M' (2x3 float64)
     # FaceAnaStreams(..., pose=True): each dict also has 'pose' {'euler', 'rvec', 'tvec', 'reproject'} as FaceAna returns it
     # FaceAnaStreams(..., track_ids=True): each dict also has 'id', the track id FaceAna(track_ids=True) gives the face
+    # FaceAnaStreams(..., detect_every=4): stream s runs the detector on a quarter of its frames, staggered by s % 4
     # or, overlapped:
     fa.submit(frames_t0); fa.submit(frames_t1); r0 = fa.collect(); fa.submit(frames_t2); r1 = fa.collect(); ...
     # frames already on the GPU (torch.uint8 CUDA tensors (H, W, 3), any row pitch), results left on the GPU:
@@ -26,13 +27,13 @@ from ... import runtime as rt
 from ...graph_tools import check_detector_input, detector_onnx_for
 from .align import check_size
 from .device_frames import check_cuda_frame, check_host_frame, is_cuda_tensor
-from .facer import get_cfg, pipeline_cfg
+from .facer import check_detect_every, get_cfg, pipeline_cfg
 from .onnx_model_base import ONNXEngine
 
 
 class FaceAnaStreams:
     def __init__(self, n_streams, top_k=None, max_frame_hw=(2160, 3840), device="cuda", align=None, pose=False,
-                 det_input=None, track_ids=False):
+                 det_input=None, track_ids=False, detect_every=1):
         """align: None, or a chip side in 16..512: every result dict then also carries 'chip' and 'M' as FaceAna(align=...)
         returns them, warped inside the same submit on the device from the smoothed landmarks and the frame in the ring.
         pose: every result dict then also carries 'pose' as FaceAna(pose=True) returns it, solved inside the same submit
@@ -42,7 +43,16 @@ class FaceAnaStreams:
         0.35 GB per stream at 1152x1920).
         track_ids: every result dict then also carries 'id', the int FaceAna(track_ids=True) returns for the face: ids
         are numbered per stream from 0, reset(stream) starts that stream again from 0, and the rule that assigns them is
-        FaceAna's.  The ids are kept on the device next to the track boxes, whether or not they are returned."""
+        FaceAna's.  The ids are kept on the device next to the track boxes, whether or not they are returned.
+        detect_every: the detection cadence of FaceAna(detect_every=N, detect_offset=s % N) for stream s, which it
+        returns bit for bit.  A stream counts its frames from construction or reset(stream), advancing only on calls
+        that include a frame for it; frame i runs the detector when the stream has no previous frame of its size, or
+        when (i + s % N) % N == 0 and the frame-difference gate fires, and otherwise takes the tracker path.  A face that
+        enters is found up to N - 1 frames late; one that leaves is followed by its landmark box until the next keyframe.
+        The staggered offsets spread the keyframes over the calls: the detector runs on about n_streams / N frames per
+        call, packed into one batch, and not at all on a call without keyframes (last_detector_frames).  The detector
+        engine keeps one CUDA graph per batch size it meets; with the stagger those are only a few sizes."""
+        self.detect_every = check_detect_every(detect_every)[0]
         self.align = None if align is None else check_size(align)
         self.pose = bool(pose)
         self.track_ids = bool(track_ids)
@@ -69,6 +79,8 @@ class FaceAnaStreams:
         h = C.c_void_p()
         rt.check(self.lib.skps_mpipe_create(self.det.handle, self.kps.handle, C.byref(pc), self.n_streams, C.byref(h)))
         self._h = h
+        if self.detect_every != 1:
+            rt.check(self.lib.skps_mpipe_set_detect_every(h, self.detect_every))
         S, K, P = self.n_streams, self.top_k, self.n_points
         self._out = [dict(n=np.zeros(S, np.int32), box=np.zeros((S, K, 4), np.float64), kps=np.zeros((S, K, P, 2), np.float64),
                           sc=np.zeros((S, K, P), np.float32), det=np.zeros(S, np.int32), ids=np.zeros((S, K), np.int64))
@@ -86,6 +98,8 @@ class FaceAnaStreams:
         self._pending = []              # [(slot, n, keep-alive frames, device results or None)]
         self._next = 0
         self.last_ran_detector = None
+        self.last_detector_frames = None      # frames the detector ran on in the last collected batch
+        self._m = C.c_int32(0)
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -94,7 +108,8 @@ class FaceAnaStreams:
             self._h = None
 
     def reset(self, stream=None):
-        """FaceAna.reset (facer.py:200-208) for one stream, or for all of them."""
+        """FaceAna.reset (facer.py:200-208) for one stream, or for all of them; the stream's frame count starts again
+        from 0."""
         while self._pending:
             self.collect()
         rt.check(self.lib.skps_mpipe_reset(self._h, -1 if stream is None else int(stream)))
@@ -174,7 +189,8 @@ class FaceAnaStreams:
 
     def new_results(self):
         """Device result buffers for submit(cuda_frames, out=...): a dict of CUDA tensors on this object's device,
-        n (S,) int32 faces per stream; ran_detector (S,) int32, the frame-difference gate's decision; box (S,K,4) and kps
+        n (S,) int32 faces per stream; ran_detector (S,) int32, whether the frame used the detector's rows (a keyframe
+        whose frame-difference gate fired, or with no previous frame of its size); box (S,K,4) and kps
         (S,K,P,2) float64; scores (S,K,P) float32; with align, chip (S,K,size,size,3) uint8 and M (S,K,2,3) float64; with
         pose, rvec, tvec, euler (S,K,3) and reproject (S,K,8,2) float64; with track_ids, id (S,K) int64.  Per stream s,
         face rows i >= n[s] (and streams past the batch's length) are unspecified."""
@@ -206,6 +222,8 @@ class FaceAnaStreams:
         if not self._pending:
             raise RuntimeError("FaceAnaStreams: nothing submitted")
         slot, n, _keep, out = self._pending.pop(0)
+        rt.check(self.lib.skps_mpipe_detector_frames(self._h, slot, C.byref(self._m)))
+        self.last_detector_frames = int(self._m.value)
         if out is not None:
             import torch
             rt.check(self.lib.skps_mpipe_wait_stream(self._h, slot, torch.cuda.current_stream(self.device).cuda_stream))

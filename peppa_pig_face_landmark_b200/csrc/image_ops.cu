@@ -415,20 +415,24 @@ __global__ void __launch_bounds__(256) select_faces_kernel(const float* __restri
 
 // Multi-stream variant (mpipe.cu): block = stream.  flag[s] != 0: this frame ran the detector -> judge_boxs(track, det rows)
 // (facer.py:58); else boxes = the stream's track boxes (facer.py:61).  Track boxes and their count live on the device.
+// The detector rows of stream s are those of detector frame det_slot[s] (det_slot null: frame s).
 __global__ void __launch_bounds__(256) mp_select_kernel(const float* __restrict__ det_rows, const int* __restrict__ det_count,
-                                                        int det_cap, const int* __restrict__ flag,
+                                                        int det_cap, const int* __restrict__ det_slot,
+                                                        const int* __restrict__ flag,
                                                         const float* __restrict__ track, const int* __restrict__ n_track,
                                                         float iou_thres, float alpha, float oma, float min_face, int top_k,
                                                         float* __restrict__ boxes4, int* __restrict__ count,
                                                         int* __restrict__ src) {
     const int s = blockIdx.x;
     const float* trk = track + (long long)s * top_k * 4;
-    if (flag[s])
-        select_faces_body(det_rows + (long long)s * det_cap * 16, det_count[s], 16, trk, n_track[s], iou_thres, alpha, oma,
+    if (flag[s]) {
+        const int f = det_slot ? det_slot[s] : s;
+        select_faces_body(det_rows + (long long)f * det_cap * 16, det_count[f], 16, trk, n_track[s], iou_thres, alpha, oma,
                           min_face, top_k, boxes4 + (long long)s * top_k * 4, count + s, src + (long long)s * top_k, false);
-    else
+    } else {
         select_faces_body(trk, n_track[s], 4, nullptr, 0, iou_thres, alpha, oma, min_face, top_k,
                           boxes4 + (long long)s * top_k * 4, count + s, src + (long long)s * top_k, true);
+    }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -650,11 +654,11 @@ int launch_mp_landmark_post(const float* xy, const int* detail, const int* count
     return 0;
 }
 
-int launch_mp_select(const float* det_rows, const int* det_count, int det_cap, const int* flag, const float* track,
-                     const int* n_track, float iou_thres, float alpha, float oma, float min_face, int top_k, float* boxes4,
-                     int* count, int* src, int n_streams, cudaStream_t s) {
-    mp_select_kernel<<<n_streams, SEL_THREADS, 0, s>>>(det_rows, det_count, det_cap, flag, track, n_track, iou_thres, alpha, oma,
-                                                min_face, top_k, boxes4, count, src);
+int launch_mp_select(const float* det_rows, const int* det_count, int det_cap, const int* det_slot, const int* flag,
+                     const float* track, const int* n_track, float iou_thres, float alpha, float oma, float min_face, int top_k,
+                     float* boxes4, int* count, int* src, int n_streams, cudaStream_t s) {
+    mp_select_kernel<<<n_streams, SEL_THREADS, 0, s>>>(det_rows, det_count, det_cap, det_slot, flag, track, n_track, iou_thres,
+                                                       alpha, oma, min_face, top_k, boxes4, count, src);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }

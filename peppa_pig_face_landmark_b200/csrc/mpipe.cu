@@ -3,9 +3,9 @@
 // One call takes one frame from each of up to S streams and runs, batched across the streams and with every piece of
 // per-stream state resident in HBM:
 //   H2D (copy stream, overlapped with the previous batch's compute) -> |prev - cur| gate (which gathers frames already on
-//   the device into the ring in the same pass) -> letterbox x S ->
-//   ONE detector forward (batch S) -> NMS x S -> judge_boxs/sort_and_filter x S (detector rows or track boxes, chosen on
-//   the device by the gate) -> crops x S -> ONE landmark forward (batch S * top_k) -> de-normalise -> GroupTrack / One-Euro /
+//   the device into the ring in the same pass) -> letterbox x m ->
+//   ONE detector forward (batch m: the keyframes of skps_mpipe_set_detect_every, all S streams by default) -> NMS x m ->
+//   judge_boxs/sort_and_filter x S (detector rows or track boxes, chosen on the device by the gate) -> crops x S -> ONE landmark forward (batch S * top_k) -> de-normalise -> GroupTrack / One-Euro /
 //   track-box EMA x S (temporal.cu, float64 with numpy's promotion rules) -> D2H of the packed results.
 // The host never sees a decision: which streams re-detect, how many faces each has and all smoothing state are device
 // data.  Two result slots let the caller keep two batches in flight (submit(0) submit(1) wait(0) submit(0) ...): the frames
@@ -33,11 +33,16 @@ struct skps_mpipe {
     std::vector<uint8_t*> d_frame;            // [S*3]
     std::vector<int> ring_pos;                // [S] index of the most recent frame in the ring
     std::vector<int> prev_h, prev_w;          // [S] size of the most recent frame (0 = none: FaceAna.reset)
+    // detection cadence (skps_mpipe_set_detect_every): frames of each stream since create / reset
+    int detect_every = 1;
+    std::vector<long long> frame_idx;         // [S]
     // per slot
     struct Slot {
         uint8_t* h_stage = nullptr;           // pinned staging for pageable frames [S][frame_bytes]
         int32_t* h_hw = nullptr; int32_t* h_have_prev = nullptr; int32_t* h_geom = nullptr;     // pinned, uploaded per batch
-        MpStreamDesc* h_desc = nullptr;       // pinned: per-stream frame pointers + letterbox geometry of this batch
+        MpStreamDesc* h_desc = nullptr;       // pinned [2S]: per-stream frame pointers + letterbox geometry of this batch,
+                                              // then those of its keyframes, packed
+        int32_t* h_det_slot = nullptr;        // pinned [S]: detector frame of each stream, -1 for none
         int32_t* h_count = nullptr; int32_t* h_flag = nullptr;
         double* h_box = nullptr; double* h_kps = nullptr; float* h_scores = nullptr;
         uint8_t* h_chips = nullptr; double* h_M = nullptr;     // pinned, only while alignment is on
@@ -46,6 +51,7 @@ struct skps_mpipe {
         cudaEvent_t ev_in = nullptr, ev_done = nullptr;
         cudaEvent_t ev_staged = nullptr;      // the batch's uploads from the pinned h_hw / h_have_prev / h_desc are done
         int n = 0;
+        int m = 0;                            // frames the detector ran on (keyframes of the batch)
         int align = 0;                        // chip size this slot's batch was submitted with (0 = none)
         bool pose = false;                    // this slot's batch was submitted with pose on
         bool busy = false;
@@ -61,9 +67,9 @@ struct skps_mpipe {
     double* d_pose = nullptr;
     // device scratch (one set: batches are serialised on s_compute)
     int32_t *d_hw = nullptr, *d_have_prev = nullptr, *d_flag = nullptr, *d_det_count = nullptr, *d_det_idx = nullptr;
-    int32_t *d_count = nullptr, *d_detail = nullptr;
+    int32_t *d_count = nullptr, *d_detail = nullptr, *d_det_slot = nullptr;
     unsigned long long* d_diff = nullptr;
-    MpStreamDesc* d_desc = nullptr;           // this batch's descriptors (uploaded on the compute stream, in order)
+    MpStreamDesc* d_desc = nullptr;           // this batch's descriptors (uploaded on the compute stream, in order) [2S]
     void* d_nms_ws = nullptr;                 // NMS workspace, det_rows candidates per stream
     float *d_det_rows = nullptr, *d_boxes = nullptr, *d_kps_now = nullptr;
     // temporal state
@@ -103,7 +109,7 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
     if (p->s_copy) cudaStreamSynchronize(p->s_copy);
     for (uint8_t* f : p->d_frame) if (f) cudaFree(f);
     for (auto& sl : p->slot) {
-        void* host[] = {sl.h_desc, sl.h_stage, sl.h_hw, sl.h_have_prev, sl.h_geom, sl.h_count, sl.h_flag, sl.h_box,
+        void* host[] = {sl.h_desc, sl.h_det_slot, sl.h_stage, sl.h_hw, sl.h_have_prev, sl.h_geom, sl.h_count, sl.h_flag, sl.h_box,
                         sl.h_kps, sl.h_scores, sl.h_chips, sl.h_M, sl.h_pose, sl.h_ids};
         for (void* q : host) if (q) cudaFreeHost(q);
         if (sl.ev_in) cudaEventDestroy(sl.ev_in);
@@ -115,7 +121,7 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
     void* dev[] = {p->d_desc, p->d_hw, p->d_have_prev, p->d_flag, p->d_det_count, p->d_det_idx, p->d_count, p->d_detail, p->d_diff,
                    p->d_det_rows, p->d_boxes, p->d_kps_now, p->d_prev_lm, p->d_prev_dx, p->d_track, p->d_out_kps,
                    p->d_track_f32, p->d_n_prev, p->d_prev_f32, p->d_state_idx, p->d_n_track, p->d_chips, p->d_align_M, p->d_pose,
-                   p->d_nms_ws, p->d_src, p->d_ids, p->d_next_id};
+                   p->d_nms_ws, p->d_src, p->d_ids, p->d_next_id, p->d_det_slot};
     for (void* q : dev) if (q) cudaFree(q);
     if (p->s_copy) cudaStreamDestroy(p->s_copy);
     if (p->s_compute) cudaStreamDestroy(p->s_compute);
@@ -131,6 +137,7 @@ extern "C" SKPS_API int skps_mpipe_reset(skps_mpipe* p, int stream) {
         // FaceAna.reset (facer.py:200-208) + a fresh GroupTrack: no previous frame, no track boxes, no landmark history;
         // track ids number from 0 again
         p->prev_h[s] = p->prev_w[s] = 0;
+        p->frame_idx[s] = 0;
         const int32_t zero = 0, none = -1, one = 1;
         SKPS_CUDA(cudaMemcpy(p->d_n_track + s, &zero, 4, cudaMemcpyHostToDevice));
         SKPS_CUDA(cudaMemsetAsync(p->d_next_id + s, 0, 8, p->s_compute));
@@ -165,14 +172,14 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
     }
     const int S = p->S, K = p->K, P = p->P;
     p->frame_bytes = ((size_t)cfg->max_h * cfg->max_w * 3 + 255) & ~(size_t)255;
-    p->ring_pos.assign(S, 0); p->prev_h.assign(S, 0); p->prev_w.assign(S, 0);
+    p->ring_pos.assign(S, 0); p->prev_h.assign(S, 0); p->prev_w.assign(S, 0); p->frame_idx.assign(S, 0);
     p->d_frame.assign((size_t)S * 3, nullptr);
     for (auto& f : p->d_frame) SKPS_DEV_ALLOC(f, p->frame_bytes);
     for (auto& sl : p->slot) {
         SKPS_HOST_ALLOC(sl.h_stage, p->frame_bytes * S);
         SKPS_HOST_ALLOC(sl.h_hw, sizeof(int32_t) * 2 * S); SKPS_HOST_ALLOC(sl.h_have_prev, sizeof(int32_t) * S);
         SKPS_HOST_ALLOC(sl.h_geom, sizeof(int32_t) * 8 * S);
-        SKPS_HOST_ALLOC(sl.h_desc, sizeof(MpStreamDesc) * S);
+        SKPS_HOST_ALLOC(sl.h_desc, sizeof(MpStreamDesc) * 2 * S); SKPS_HOST_ALLOC(sl.h_det_slot, sizeof(int32_t) * S);
         SKPS_HOST_ALLOC(sl.h_count, sizeof(int32_t) * S); SKPS_HOST_ALLOC(sl.h_flag, sizeof(int32_t) * S);
         SKPS_HOST_ALLOC(sl.h_box, sizeof(double) * 4 * K * S); SKPS_HOST_ALLOC(sl.h_kps, sizeof(double) * 2 * P * K * S);
         SKPS_HOST_ALLOC(sl.h_scores, sizeof(float) * P * K * S);
@@ -183,7 +190,7 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
     }
     if (cudaEventCreateWithFlags(&p->ev_ready, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&p->ev_read, cudaEventDisableTiming) != cudaSuccess) { set_error("cudaEventCreate"); return fail("event"); }
-    SKPS_DEV_ALLOC(p->d_desc, sizeof(MpStreamDesc) * S); SKPS_DEV_ALLOC(p->d_hw, 8 * S); SKPS_DEV_ALLOC(p->d_have_prev, 4 * S);
+    SKPS_DEV_ALLOC(p->d_desc, sizeof(MpStreamDesc) * 2 * S); SKPS_DEV_ALLOC(p->d_det_slot, 4 * S); SKPS_DEV_ALLOC(p->d_hw, 8 * S); SKPS_DEV_ALLOC(p->d_have_prev, 4 * S);
     SKPS_DEV_ALLOC(p->d_flag, 4 * S); SKPS_DEV_ALLOC(p->d_det_count, 4 * S);
     SKPS_DEV_ALLOC(p->d_det_idx, 4 * (size_t)p->det_rows * S); SKPS_DEV_ALLOC(p->d_count, 4 * S);
     SKPS_DEV_ALLOC(p->d_detail, 4 * 5 * (size_t)K * S);
@@ -259,21 +266,42 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     uint8_t* det_in = (uint8_t*)skps_engine_input_ptr(p->det);
     const size_t det_in_bytes = (size_t)p->det_h * p->det_w * 3;
     // per-stream frame pointers + letterbox geometry: one small upload, then every pre/post-processing step is ONE launch for
-    // all streams (it was 5 launches per stream and call - ~80 launch gaps of a 5 ms call at 16 streams)
+    // all streams (it was 5 launches per stream and call - ~80 launch gaps of a 5 ms call at 16 streams).
+    // Keyframes (skps_mpipe_set_detect_every): stream s's frame i is one when the stream has no previous frame of this size
+    // or (i + s % N) % N == 0.  Only keyframes go through the letterbox, the detector and NMS, as detector frames 0..m-1 in
+    // stream order; the host knows them now, so the detector batch shrinks with no read-back.
+    const int N = p->detect_every;
+    int m = 0;
     size_t max_bytes = 0;
     for (int s = 0; s < n; ++s) {
         const int H = hw[2 * s], W = hw[2 * s + 1];
+        const bool key = !sl.h_have_prev[s] || (p->frame_idx[s] + s % N) % N == 0;
+        sl.h_det_slot[s] = key ? m++ : -1;
         MpStreamDesc& D = sl.h_desc[s];
         D.cur = p->d_frame[(size_t)s * 3 + (p->ring_pos[s] + 1) % 3];
-        D.prev = sl.h_have_prev[s] ? p->d_frame[(size_t)s * 3 + p->ring_pos[s]] : nullptr;
-        D.H = H; D.W = W; D.have_prev = sl.h_have_prev[s];
+        // the difference sum only decides keyframes: the other streams skip it (a device frame is still gathered into cur)
+        D.have_prev = sl.h_have_prev[s] && key;
+        D.prev = D.have_prev ? p->d_frame[(size_t)s * 3 + p->ring_pos[s]] : nullptr;
+        D.H = H; D.W = W;
         D.src = on_device ? frames[s] : nullptr;
         D.src_pitch = on_device ? pitches[s] : W * 3;
         letterbox_geometry(H, W, p->det_h, p->det_w, &D.scale, &D.rw, &D.rh, &D.top, &D.left);
         memcpy(&sl.h_geom[8 * s], &D.scale, 4); sl.h_geom[8 * s + 1] = D.top; sl.h_geom[8 * s + 2] = D.left;
         if ((size_t)H * W * 3 > max_bytes) max_bytes = (size_t)H * W * 3;
     }
-    SKPS_CUDA(cudaMemcpyAsync(p->d_desc, sl.h_desc, sizeof(MpStreamDesc) * n, cudaMemcpyHostToDevice, sx));
+    // the keyframes' descriptors, packed after the batch's; when every stream is a keyframe the batch is that list, and the
+    // kernels take det_slot = null (frame s is stream s's), exactly as without a cadence
+    const MpStreamDesc* d_key_desc = p->d_desc;
+    const int32_t* det_slot = nullptr;
+    int n_desc = n;
+    if (m < n) {
+        for (int s = 0; s < n; ++s)
+            if (sl.h_det_slot[s] >= 0) sl.h_desc[n + sl.h_det_slot[s]] = sl.h_desc[s];
+        d_key_desc = p->d_desc + n; n_desc = n + m;
+        det_slot = p->d_det_slot;
+        SKPS_CUDA(cudaMemcpyAsync(p->d_det_slot, sl.h_det_slot, 4 * n, cudaMemcpyHostToDevice, sx));
+    }
+    SKPS_CUDA(cudaMemcpyAsync(p->d_desc, sl.h_desc, sizeof(MpStreamDesc) * n_desc, cudaMemcpyHostToDevice, sx));
     SKPS_CUDA(cudaEventRecord(sl.ev_staged, sx));
     if (launch_mp_absdiff(p->d_desc, p->d_diff, n, max_bytes, sx)) return 1;
     if (on_device) {
@@ -283,19 +311,23 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     // results: D2H into the slot's pinned buffers, or D2D into the caller's; either way before the next batch on sx can
     // overwrite d_out_kps, the engine's score output or the chips
     const cudaMemcpyKind result_kind = out ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-    if (launch_mp_letterbox(p->d_desc, det_in, det_in_bytes, p->det_h, p->det_w, n, sx)) return 1;
-    if (launch_mp_decide(p->d_diff, p->d_hw, p->d_have_prev, p->d_flag, n, sx)) return 1;
-    // the detector runs for every stream of the batch (one launch sequence); the gate only chooses whose rows are used
-    if (skps_engine_forward(p->det, det_in, n, nullptr, sx)) return 1;
-    const float* det_out = skps_engine_output_ptr(p->det, 0);
-    NmsArgs na = {};
-    na.raw = det_out; na.rows = p->det_rows; na.batch = n; na.score_thres = c.score_thres; na.iou_thres = c.iou_thres;
-    na.desc = p->d_desc; na.limit = p->det_rows; na.capacity = p->det_rows;
-    na.kept_rows = p->d_det_rows; na.kept_idx = p->d_det_idx; na.count = p->d_det_count;
-    na.ws = p->d_nms_ws; na.ws_cap = p->det_rows;
-    if (launch_nms(na, sx)) return 1;
-    if (launch_mp_select(p->d_det_rows, p->d_det_count, p->det_rows, p->d_flag, p->d_track_f32, p->d_n_track, c.track_iou,
-                         c.alpha, (float)(1.0 - (double)c.alpha), c.min_face, K, p->d_boxes, p->d_count, p->d_src, n, sx))
+    if (m > 0 && launch_mp_letterbox(d_key_desc, det_in, det_in_bytes, p->det_h, p->det_w, m, sx)) return 1;
+    if (launch_mp_decide(p->d_diff, p->d_hw, p->d_have_prev, det_slot, p->d_flag, n, sx)) return 1;
+    // the detector runs for every keyframe of the batch (one launch sequence, batch m); the gate only chooses whose rows are
+    // used.  With no keyframe the detector and NMS are skipped and every stream takes the tracker path.
+    if (m > 0) {
+        if (skps_engine_forward(p->det, det_in, m, nullptr, sx)) return 1;
+        const float* det_out = skps_engine_output_ptr(p->det, 0);
+        NmsArgs na = {};
+        na.raw = det_out; na.rows = p->det_rows; na.batch = m; na.score_thres = c.score_thres; na.iou_thres = c.iou_thres;
+        na.desc = d_key_desc; na.limit = p->det_rows; na.capacity = p->det_rows;
+        na.kept_rows = p->d_det_rows; na.kept_idx = p->d_det_idx; na.count = p->d_det_count;
+        na.ws = p->d_nms_ws; na.ws_cap = p->det_rows;
+        if (launch_nms(na, sx)) return 1;
+    }
+    if (launch_mp_select(p->d_det_rows, p->d_det_count, p->det_rows, det_slot, p->d_flag, p->d_track_f32, p->d_n_track,
+                         c.track_iou, c.alpha, (float)(1.0 - (double)c.alpha), c.min_face, K, p->d_boxes, p->d_count, p->d_src,
+                         n, sx))
         return 1;
     uint8_t* kps_in = (uint8_t*)skps_engine_input_ptr(p->kps);
     if (launch_mp_crop(p->d_desc, p->d_boxes, p->d_count, K, c.face_scale, c.kps_min_face, kps_in, p->kps_hw, p->d_detail, n, sx))
@@ -351,8 +383,10 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     for (int s = 0; s < n; ++s) {
         p->ring_pos[s] = (p->ring_pos[s] + 1) % 3;
         p->prev_h[s] = hw[2 * s]; p->prev_w[s] = hw[2 * s + 1];
+        ++p->frame_idx[s];
     }
     sl.n = n;
+    sl.m = m;
     sl.busy = true;
     sl.device_out = out != nullptr;
     return 0;
@@ -502,6 +536,19 @@ extern "C" SKPS_API int skps_mpipe_track_ids(skps_mpipe* p, int slot_i, int64_t*
     SKPS_CHECK(!sl.busy, "mpipe_track_ids: slot %d is in flight (call skps_mpipe_wait first)", slot_i);
     SKPS_CHECK(sl.n > 0 && !sl.device_out, "mpipe_track_ids: slot %d was not submitted with host results", slot_i);
     memcpy(ids, sl.h_ids, sizeof(int64_t) * sl.n * p->K);
+    return 0;
+}
+
+extern "C" SKPS_API int skps_mpipe_set_detect_every(skps_mpipe* p, int every) {
+    SKPS_CHECK(p && every >= 1, "mpipe_set_detect_every: every %d is not >= 1", every);
+    p->detect_every = every;
+    return 0;
+}
+
+extern "C" SKPS_API int skps_mpipe_detector_frames(const skps_mpipe* p, int slot_i, int* m) {
+    SKPS_CHECK(p && (slot_i == 0 || slot_i == 1) && m, "mpipe_detector_frames: bad arguments");
+    SKPS_CHECK(p->slot[slot_i].n > 0, "mpipe_detector_frames: nothing submitted on slot %d", slot_i);
+    *m = p->slot[slot_i].m;
     return 0;
 }
 

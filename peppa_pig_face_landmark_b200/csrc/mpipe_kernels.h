@@ -90,11 +90,16 @@ int launch_mp_landmark_post(const float* xy, const int* detail, const int* count
 int launch_select_faces(const float* det_rows, const int32_t* det_count, int det_stride, const float* track, int n_track,
                         float iou_thres, float alpha, float one_minus_alpha, float min_face, int top_k, float* boxes4,
                         int32_t* count, int32_t* src, bool src_is_row, cudaStream_t s);
-// The same per stream of a batch; src [dev] [S][K] as above, the rows being the track boxes where flag[s] == 0.
-int launch_mp_select(const float* det_rows, const int* det_count, int det_cap, const int* flag, const float* track,
-                     const int* n_track, float iou_thres, float alpha, float oma, float min_face, int top_k, float* boxes4,
-                     int* count, int* src, int n_streams, cudaStream_t s);
-int launch_mp_decide(const unsigned long long* diff, const int* hw, const int* have_prev, int* flag, int n, cudaStream_t s);
+// The same per stream of a batch; src [dev] [S][K] as above, the rows being the track boxes where flag[s] == 0.  det_slot
+// [dev] [S]: the detector frame (row of det_rows / det_count) of each stream, -1 where the detector did not run on it; null:
+// frame s is stream s's.
+int launch_mp_select(const float* det_rows, const int* det_count, int det_cap, const int* det_slot, const int* flag,
+                     const float* track, const int* n_track, float iou_thres, float alpha, float oma, float min_face, int top_k,
+                     float* boxes4, int* count, int* src, int n_streams, cudaStream_t s);
+// flag[s] = the stream uses its detector rows: det_slot[s] >= 0 (det_slot null: always) and (!have_prev[s] or the mean
+// difference > 5)
+int launch_mp_decide(const unsigned long long* diff, const int* hw, const int* have_prev, const int* det_slot, int* flag, int n,
+                     cudaStream_t s);
 int launch_mp_temporal(const MpTemporalArgs& a, int n_streams, cudaStream_t s);
 // Aligned face chips (align.cu): per face of stream g < n with i < count[g], M = similarity of kps[g][i] (P x 2 float64) to the
 // ArcFace template at `size`, chips[g][i] = cv2.warpAffine(desc[g].cur, M, (size, size)); chips [n][K][size][size][3], M [n][K][2][3].

@@ -73,11 +73,14 @@ __device__ void set_rect(const double* pts, int P, double* r, double* red /*[4][
 }
 
 // Gate of facer.py:55-62: run the detector when there is no previous frame of this size or the mean absolute difference
-// exceeds 5 (np.sum(diff) / H / W / 3. in float64).
+// exceeds 5 (np.sum(diff) / H / W / 3. in float64).  Only keyframes (det_slot[s] >= 0; det_slot null: every stream) run
+// the detector; the host makes every frame without a previous frame of its size a keyframe.
 __global__ void mp_decide_kernel(const unsigned long long* __restrict__ diff, const int* __restrict__ hw,
-                                 const int* __restrict__ have_prev, int* __restrict__ flag, int n) {
+                                 const int* __restrict__ have_prev, const int* __restrict__ det_slot, int* __restrict__ flag,
+                                 int n) {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n) return;
+    if (det_slot && det_slot[s] < 0) { flag[s] = 0; return; }
     if (!have_prev[s]) { flag[s] = 1; return; }
     const double m = (double)diff[s] / (double)hw[2 * s] / (double)hw[2 * s + 1] / 3.0;
     flag[s] = m > 5.0 ? 1 : 0;
@@ -210,8 +213,9 @@ __global__ void __launch_bounds__(128) mp_temporal_kernel(const MpTemporalArgs a
     }
 }
 
-int launch_mp_decide(const unsigned long long* diff, const int* hw, const int* have_prev, int* flag, int n, cudaStream_t s) {
-    mp_decide_kernel<<<(n + 63) / 64, 64, 0, s>>>(diff, hw, have_prev, flag, n);
+int launch_mp_decide(const unsigned long long* diff, const int* hw, const int* have_prev, const int* det_slot, int* flag, int n,
+                     cudaStream_t s) {
+    mp_decide_kernel<<<(n + 63) / 64, 64, 0, s>>>(diff, hw, have_prev, det_slot, flag, n);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }

@@ -122,6 +122,8 @@ SIGNATURES = {
     "skps_pipeline_pose": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "skps_mpipe_set_pose": (C.c_int, [c_vp, C.c_int]),
     "skps_mpipe_pose_results": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp]),
+    "skps_mpipe_set_detect_every": (C.c_int, [c_vp, C.c_int]),
+    "skps_mpipe_detector_frames": (C.c_int, [c_vp, C.c_int, c_i32p]),
 }
 
 _lib = None

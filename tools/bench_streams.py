@@ -8,6 +8,7 @@ host results out: every H2D / D2H is inside the timed region.
     python tools/bench_streams.py --pose [--parent-headpose OLD_headpose.cu --out DIR] [--rounds 5] [--configs ...]
     python tools/bench_streams.py --det-input H W [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
     python tools/bench_streams.py --track-ids [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
+    python tools/bench_streams.py --detect-every N [--det-input H W] [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
 
 --align SIZE times every config with and without aligned face chips (FaceAnaStreams(align=SIZE)) in the same process,
 alternating the two over --rounds rounds, and reports the median ms_per_call of both.  At 4k_16faces it also times the
@@ -22,6 +23,11 @@ run and reports the largest difference of its skps_head_pose results from this b
 --det-input H W does the same with the detector at Skps.yml's 384x640 and at H x W (FaceAnaStreams(det_input=(H, W))).
 
 --track-ids does the same without and with track ids in the results (FaceAnaStreams(track_ids=True)).
+
+--detect-every N does the same with FaceAnaStreams(detect_every=1) and (detect_every=N), at Skps.yml's detector input or,
+with --det-input H W, at H x W, and reports detector_frames_per_call of both (the mean of last_detector_frames).  Every
+detector batch size the staggered cadence meets is warmed up first (the detector engine captures one CUDA graph per batch
+size).  It then times FaceAna.run per call on stream 0's frames at detect_every 1 and N, alternating over the same rounds.
 
 Under torchrun every rank drives its own S streams on its own GPU (streams shard across GPUs, no collective on the data
 path); time = max over ranks.  --gather adds one NCCL all_gather of the packed (box, landmarks, scores) rows per call."""
@@ -340,6 +346,76 @@ def parent_pose_diff(parent_lib):
     return {"max_abs_diff_from_parent": d, "inputs": "test_headpose_gpu._synthetic_shapes(64, hw, seed=hw[0]), 480x640 and 1080x1920"}
 
 
+def run_detect_every_pair(name, every, det_input=None, n_streams=16, batches=12, rounds=5, length=6, single_calls=60):
+    """FaceAnaStreams at detect_every 1 and `every` (alternating rounds, median ms_per_call and the mean detector batch of
+    each), then FaceAna.run on stream 0's frames at both settings."""
+    import torch
+    import frames
+    from Skps import FaceAna, FaceAnaStreams
+    maker, topk = getattr(frames, CONFIGS[name][0]), CONFIGS[name][1]
+    seqs = make_streams(torch, frames, maker, n_streams, length=length)
+    H, W = seqs[0][0].shape[:2]
+    kw = {} if det_input is None else {"det_input": det_input}
+    fas = {1: FaceAnaStreams(n_streams=n_streams, top_k=topk, max_frame_hw=(H, W), detect_every=1, **kw),
+           every: FaceAnaStreams(n_streams=n_streams, top_k=topk, max_frame_hw=(H, W), detect_every=every, **kw)}
+    L = len(seqs[0])
+
+    def batch(t):
+        return [seqs[s][t % L] for s in range(n_streams)]
+    for fa in fas.values():
+        for t in range(every + 2):         # the first call (all streams) and every staggered batch size after it
+            fa.run(batch(t))
+    times = {k: [] for k in fas}
+    det_frames = {k: [] for k in fas}
+    for r in range(rounds):
+        for key in (list(fas) if r % 2 == 0 else list(fas)[::-1]):
+            fa = fas[key]
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            fa.submit(batch(0))
+            for t in range(1, batches):
+                fa.submit(batch(t))
+                fa.collect()
+                det_frames[key].append(fa.last_detector_frames)
+            fa.collect()
+            det_frames[key].append(fa.last_detector_frames)
+            torch.cuda.synchronize()
+            times[key].append(time.perf_counter() - t0)
+    del fas
+    singles = {k: FaceAna(top_k=topk, max_frame_hw=(H, W), detect_every=k, **kw) for k in (1, every)}
+    for f in singles.values():
+        for t in range(2 * every):
+            f.run(seqs[0][t % L])
+    single_times = {k: [] for k in singles}
+    ran = {k: 0 for k in singles}
+    for r in range(rounds):
+        for key in (list(singles) if r % 2 == 0 else list(singles)[::-1]):
+            f = singles[key]
+            t0 = time.perf_counter()
+            for t in range(single_calls):
+                f.run(seqs[0][t % L])
+                ran[key] += f.last_ran_detector
+            single_times[key].append(time.perf_counter() - t0)
+    del singles
+    ms = {k: 1e3 * float(np.median(v)) / batches for k, v in times.items()}
+    ms1 = {k: 1e3 * float(np.median(v)) / single_calls for k, v in single_times.items()}
+    return {"config": name, "streams_per_gpu": n_streams, "calls": batches, "rounds": rounds, "detect_every": every,
+            "det_input": list(det_input) if det_input is not None else [384, 640],
+            "ms_per_call_every_1": ms[1], "ms_per_call_every_n": ms[every],
+            "frames_per_s_every_1": 1e3 * n_streams / ms[1], "frames_per_s_every_n": 1e3 * n_streams / ms[every],
+            "ms_per_call_every_1_rounds": [1e3 * v / batches for v in times[1]],
+            "ms_per_call_every_n_rounds": [1e3 * v / batches for v in times[every]],
+            "detector_frames_per_call_every_1": float(np.mean(det_frames[1])),
+            "detector_frames_per_call_every_n": float(np.mean(det_frames[every])),
+            "faceana_ms_per_run_every_1": ms1[1], "faceana_ms_per_run_every_n": ms1[every],
+            "faceana_ms_per_run_every_1_rounds": [1e3 * v / single_calls for v in single_times[1]],
+            "faceana_ms_per_run_every_n_rounds": [1e3 * v / single_calls for v in single_times[every]],
+            "faceana_detector_share_every_1": ran[1] / (rounds * single_calls),
+            "faceana_detector_share_every_n": ran[every] / (rounds * single_calls),
+            "api": "FaceAnaStreams.submit/collect, pinned host frames, 2 calls in flight; FaceAna.run on stream 0's "
+                   "frames (host results, synchronous)"}
+
+
 def main():
     import torch
     a = sys.argv[1:]
@@ -365,6 +441,17 @@ def main():
         sys.stdout.flush()
         for name in names:
             print(json.dumps(run_align_pair(name, 0, n_streams, batches, rounds=rounds, feature="pose")))
+            sys.stdout.flush()
+        return
+    if "--detect-every" in a:
+        every, rounds = int(opt("--detect-every", 4)), int(opt("--rounds", 5))
+        hw = None
+        if "--det-input" in a:
+            i = a.index("--det-input")
+            hw = (int(a[i + 1]), int(a[i + 2]))
+        print(json.dumps(gpu_info(torch)))
+        for name in names:
+            print(json.dumps(run_detect_every_pair(name, every, hw, n_streams, batches, rounds=rounds)))
             sys.stdout.flush()
         return
     if "--det-input" in a:
