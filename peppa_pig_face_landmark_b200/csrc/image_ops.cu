@@ -66,15 +66,15 @@ __device__ __forceinline__ void letterbox_px(const uint8_t* __restrict__ frame, 
         o[2 - c] = (uint8_t)vblend(h0, h1, ty.w0, ty.w1);      // BGR -> RGB
     }
 }
-__global__ void __launch_bounds__(256) letterbox_kernel(const uint8_t* __restrict__ frame, int H, int W, int pitch,
-                                                        uint8_t* __restrict__ out, int in_h, int in_w,
-                                                        int rw, int rh, int top, int left) {
-    letterbox_px(frame, H, W, pitch, out, in_h, in_w, rw, rh, top, left, blockIdx.x * blockDim.x + threadIdx.x, blockIdx.y);
-}
-__global__ void __launch_bounds__(256) mp_letterbox_kernel(const MpStreamDesc* __restrict__ d, uint8_t* __restrict__ out,
-                                                           size_t out_stride, int in_h, int in_w) {
-    const MpStreamDesc D = d[blockIdx.z];
-    letterbox_px(D.cur, D.H, D.W, D.W * 3, out + out_stride * blockIdx.z, in_h, in_w, D.rw, D.rh, D.top, D.left,
+// block z = frame
+__global__ void __launch_bounds__(256) letterbox_frames_kernel(const LetterboxArgs a) {
+    const uint8_t* frame = a.frame;
+    int H = a.H, W = a.W, pitch = a.pitch, rw = a.rw, rh = a.rh, top = a.top, left = a.left;
+    if (a.desc) {
+        const MpStreamDesc D = a.desc[blockIdx.z];
+        frame = D.cur; H = D.H; W = D.W; pitch = D.W * 3; rw = D.rw; rh = D.rh; top = D.top; left = D.left;
+    }
+    letterbox_px(frame, H, W, pitch, a.out + a.out_stride * blockIdx.z, a.in_h, a.in_w, rw, rh, top, left,
                  blockIdx.x * blockDim.x + threadIdx.x, blockIdx.y);
 }
 
@@ -151,20 +151,18 @@ __device__ __forceinline__ void crop_px(const uint8_t* __restrict__ frame, int H
     }
     crop_face_px(frame, H, W, pitch, 0, 0, boxes + face * 4, face_scale, min_face, o, S, detail + face * 5, x, y);
 }
-__global__ void __launch_bounds__(256) crop_resize_kernel(const uint8_t* __restrict__ frame, int H, int W, int pitch,
-                                                          const float* __restrict__ boxes, const int* __restrict__ count,
-                                                          float face_scale, float min_face,
-                                                          uint8_t* __restrict__ crops, int S, int* __restrict__ detail) {
-    crop_px(frame, H, W, pitch, boxes, count, face_scale, min_face, crops, S, detail, blockIdx.z, blockIdx.x * blockDim.x + threadIdx.x,
-            blockIdx.y);
-}
-__global__ void __launch_bounds__(256) mp_crop_kernel(const MpStreamDesc* __restrict__ d, const float* __restrict__ boxes,
-                                                      const int* __restrict__ count, int K, float face_scale, float min_face,
-                                                      uint8_t* __restrict__ crops, int S, int* __restrict__ detail) {
-    const int st = blockIdx.z / K, face = blockIdx.z - st * K;
-    const MpStreamDesc D = d[st];
-    crop_px(D.cur, D.H, D.W, D.W * 3, boxes + (size_t)4 * K * st, count + st, face_scale, min_face,
-            crops + (size_t)S * S * 3 * K * st, S, detail + (size_t)5 * K * st, face, blockIdx.x * blockDim.x + threadIdx.x, blockIdx.y);
+// block z = face of a frame (K per frame)
+__global__ void __launch_bounds__(256) crop_frames_kernel(const CropArgs a) {
+    const int g = blockIdx.z / a.K, face = blockIdx.z - g * a.K;
+    const uint8_t* frame = a.frame;
+    int H = a.H, W = a.W, pitch = a.pitch;
+    if (a.desc) {
+        const MpStreamDesc D = a.desc[g];
+        frame = D.cur; H = D.H; W = D.W; pitch = D.W * 3;
+    }
+    crop_px(frame, H, W, pitch, a.boxes + (size_t)4 * a.K * g, a.count + g, a.face_scale, a.min_face,
+            a.crops + (size_t)a.S * a.S * 3 * a.K * g, a.S, a.detail + (size_t)5 * a.K * g, face,
+            blockIdx.x * blockDim.x + threadIdx.x, blockIdx.y);
 }
 // Face table variant (FaceLandmark.submit): block z = face, each face with its own frame or frame rectangle.
 __global__ void __launch_bounds__(256) crop_faces_kernel(const skps_face_src* __restrict__ src, const float* __restrict__ boxes,
@@ -404,91 +402,31 @@ __device__ __forceinline__ void select_faces_body(const float* __restrict__ det,
     }
 }
 
-__global__ void __launch_bounds__(256) select_faces_kernel(const float* __restrict__ det, const int* __restrict__ det_count,
-                                                           int det_stride, const float* __restrict__ track, int n_track,
-                                                           float iou_thres, float alpha, float oma, float min_face,
-                                                           int top_k, float* __restrict__ boxes4, int* __restrict__ count,
-                                                           int* __restrict__ src, int src_is_row) {
-    select_faces_body(det, *det_count, det_stride, track, n_track, iou_thres, alpha, oma, min_face, top_k, boxes4, count,
-                      src, src_is_row != 0);
-}
-
-// Multi-stream variant (mpipe.cu): block = stream.  flag[s] != 0: this frame ran the detector -> judge_boxs(track, det rows)
-// (facer.py:58); else boxes = the stream's track boxes (facer.py:61).  Track boxes and their count live on the device.
-// The detector rows of stream s are those of detector frame det_slot[s] (det_slot null: frame s).
-__global__ void __launch_bounds__(256) mp_select_kernel(const float* __restrict__ det_rows, const int* __restrict__ det_count,
-                                                        int det_cap, const int* __restrict__ det_slot,
-                                                        const int* __restrict__ flag,
-                                                        const float* __restrict__ track, const int* __restrict__ n_track,
-                                                        float iou_thres, float alpha, float oma, float min_face, int top_k,
-                                                        float* __restrict__ boxes4, int* __restrict__ count,
-                                                        int* __restrict__ src) {
-    const int s = blockIdx.x;
-    const float* trk = track + (long long)s * top_k * 4;
-    if (flag[s]) {
-        const int f = det_slot ? det_slot[s] : s;
-        select_faces_body(det_rows + (long long)f * det_cap * 16, det_count[f], 16, trk, n_track[s], iou_thres, alpha, oma,
-                          min_face, top_k, boxes4 + (long long)s * top_k * 4, count + s, src + (long long)s * top_k, false);
-    } else {
-        select_faces_body(trk, n_track[s], 4, nullptr, 0, iou_thres, alpha, oma, min_face, top_k,
-                          boxes4 + (long long)s * top_k * 4, count + s, src + (long long)s * top_k, true);
+// block = frame: judge_boxs(track, detector rows) when the frame ran the detector (facer.py:58), else its track boxes
+// (facer.py:61), then sort_and_filter
+__global__ void __launch_bounds__(256) select_frames_kernel(const SelectArgs a) {
+    const int g = blockIdx.x;
+    const float* trk = a.track + (size_t)g * a.top_k * 4;
+    const int n_trk = a.track ? (a.n_track ? a.n_track[g] : a.n_track1) : 0;
+    const bool det = a.flag ? a.flag[g] != 0 : a.flag1 != 0;
+    const float* rows = trk;
+    int n_rows = n_trk, stride = 4;
+    if (det) {
+        const int f = a.det_slot ? a.det_slot[g] : g;
+        rows = a.det_rows + (size_t)f * a.det_cap * a.det_stride; n_rows = a.det_count[f]; stride = a.det_stride;
     }
+    select_faces_body(rows, n_rows, stride, det ? trk : nullptr, det ? n_trk : 0, a.iou_thres, a.alpha, a.one_minus_alpha,
+                      a.min_face, a.top_k, a.boxes4 + (size_t)g * a.top_k * 4, a.count + g,
+                      a.src ? a.src + (size_t)g * a.top_k : nullptr, !det);
 }
 
 // ------------------------------------------------------------------------------------------
 // FaceLandmark.postprocess (face_landmark.py:106-115): float32 product, then + x1 - add in
 // float64, stored as float32 (numpy>=2 promotion of `float32 * int + np.int32 - int`).
 // ------------------------------------------------------------------------------------------
-__global__ void landmark_post_kernel(const float* __restrict__ xy, const int* __restrict__ detail,
-                                     const int* __restrict__ count, int max_faces, int P, float* __restrict__ kps) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= max_faces * P) return;
-    int f = i / P;
-    float ox = 0.f, oy = 0.f;
-    if (f < *count) {
-        const int* d = detail + f * 5;      // [h, w, y1, x1, add]
-        float px = xy[i * 2] * (float)d[1];
-        float py = xy[i * 2 + 1] * (float)d[0];
-        ox = (float)((double)px + (double)d[3] - (double)d[4]);
-        oy = (float)((double)py + (double)d[2] - (double)d[4]);
-    }
-    kps[i * 2] = ox;
-    kps[i * 2 + 1] = oy;
-}
-
-// ------------------------------------------------------------------------------------------
-// Frame difference gate (facer.py:111-113): sum |a-b| over all bytes.  uint4 loads, __vsadu4.
-// ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) absdiff_sum_kernel(const uint8_t* __restrict__ a, const uint8_t* __restrict__ b,
-                                                          size_t n, unsigned long long* __restrict__ sum) {
-    size_t nv = n / 16;
-    unsigned long long local = 0;
-    const uint4* a4 = reinterpret_cast<const uint4*>(a);
-    const uint4* b4 = reinterpret_cast<const uint4*>(b);
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += (size_t)gridDim.x * blockDim.x) {
-        uint4 x = a4[i], y = b4[i];
-        local += __vsadu4(x.x, y.x) + __vsadu4(x.y, y.y) + __vsadu4(x.z, y.z) + __vsadu4(x.w, y.w);
-    }
-    if (blockIdx.x == 0) {
-        for (size_t i = nv * 16 + threadIdx.x; i < n; i += blockDim.x) {
-            int d = (int)a[i] - (int)b[i];
-            local += (unsigned)(d < 0 ? -d : d);
-        }
-    }
-    for (int o = 16; o > 0; o >>= 1) local += __shfl_down_sync(0xffffffffu, local, o);
-    __shared__ unsigned long long warp_sum[8];
-    if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = local;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        unsigned long long t = 0;
-        for (int w = 0; w < 8; ++w) t += warp_sum[w];
-        atomicAdd(sum, t);
-    }
-}
-
-__global__ void mp_landmark_post_kernel(const float* __restrict__ xy, const int* __restrict__ detail, const int* __restrict__ count,
-                                        int K, int P, float* __restrict__ kps, int n) {
-    // per stream exactly landmark_post_kernel: element i of stream st
+__global__ void landmark_post_frames_kernel(const float* __restrict__ xy, const int* __restrict__ detail,
+                                            const int* __restrict__ count, int K, int P, float* __restrict__ kps, int n) {
+    // element i of frame st
     const int per = K * P;
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= per * n) return;
@@ -505,6 +443,29 @@ __global__ void mp_landmark_post_kernel(const float* __restrict__ xy, const int*
     }
     kps[(size_t)2 * per * st + i * 2] = ox;
     kps[(size_t)2 * per * st + i * 2 + 1] = oy;
+}
+
+// ------------------------------------------------------------------------------------------
+// Frame difference gate (facer.py:111-113): sum |a-b| over all bytes.  uint4 loads, __vsadu4.
+// ------------------------------------------------------------------------------------------
+// This thread's part of sum |a - b| over n bytes (a, b 16-byte aligned); block 0 takes the bytes past the last 16.
+__device__ __forceinline__ unsigned long long absdiff_bytes(const uint8_t* __restrict__ a, const uint8_t* __restrict__ b,
+                                                            size_t n) {
+    const size_t nv = n / 16;
+    unsigned long long local = 0;
+    const uint4* a4 = reinterpret_cast<const uint4*>(a);
+    const uint4* b4 = reinterpret_cast<const uint4*>(b);
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += (size_t)gridDim.x * blockDim.x) {
+        uint4 x = a4[i], y = b4[i];
+        local += __vsadu4(x.x, y.x) + __vsadu4(x.y, y.y) + __vsadu4(x.z, y.z) + __vsadu4(x.w, y.w);
+    }
+    if (blockIdx.x == 0) {
+        for (size_t i = nv * 16 + threadIdx.x; i < n; i += blockDim.x) {
+            int d = (int)a[i] - (int)b[i];
+            local += (unsigned)(d < 0 ? -d : d);
+        }
+    }
+    return local;
 }
 
 // 16 bytes from an address of any alignment: the one or two aligned 16-byte blocks that hold them, shifted into place.
@@ -562,32 +523,13 @@ __device__ __forceinline__ unsigned long long ingest_units(const MpStreamDesc& D
     return local;
 }
 
-__global__ void __launch_bounds__(256) mp_absdiff_kernel(const MpStreamDesc* __restrict__ d, MpStreamDesc one,
-                                                         unsigned long long* __restrict__ sum) {
-    // per stream exactly absdiff_sum_kernel (integer sums: the order of the atomic adds does not matter); a stream with a
-    // source frame is gathered into its packed frame in the same pass
+// block y = frame (integer sums: the order of the atomic adds does not matter)
+__global__ void __launch_bounds__(256) diff_frames_kernel(const MpStreamDesc* __restrict__ d, MpStreamDesc one, size_t one_bytes,
+                                                          unsigned long long* __restrict__ sum) {
     const MpStreamDesc D = d ? d[blockIdx.y] : one;
+    const size_t n = d ? (size_t)D.H * D.W * 3 : one_bytes;
     if (!D.have_prev && !D.src) return;
-    unsigned long long local = 0;
-    if (D.src) {
-        local = ingest_units(D);
-    } else {
-        const uint8_t* a = D.prev;
-        const uint8_t* b = D.cur;
-        const size_t n = (size_t)D.H * D.W * 3, nv = n / 16;
-        const uint4* a4 = reinterpret_cast<const uint4*>(a);
-        const uint4* b4 = reinterpret_cast<const uint4*>(b);
-        for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += (size_t)gridDim.x * blockDim.x) {
-            uint4 x = a4[i], y = b4[i];
-            local += __vsadu4(x.x, y.x) + __vsadu4(x.y, y.y) + __vsadu4(x.z, y.z) + __vsadu4(x.w, y.w);
-        }
-        if (blockIdx.x == 0) {
-            for (size_t i = nv * 16 + threadIdx.x; i < n; i += blockDim.x) {
-                int dd = (int)a[i] - (int)b[i];
-                local += (unsigned)(dd < 0 ? -dd : dd);
-            }
-        }
-    }
+    unsigned long long local = D.src ? ingest_units(D) : absdiff_bytes(D.prev, D.cur, n);
     for (int o = 16; o > 0; o >>= 1) local += __shfl_down_sync(0xffffffffu, local, o);
     __shared__ unsigned long long warp_sum[8];
     if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = local;
@@ -599,22 +541,15 @@ __global__ void __launch_bounds__(256) mp_absdiff_kernel(const MpStreamDesc* __r
     }
 }
 
-static int absdiff_grid(size_t max_bytes) {
-    size_t blocks = (max_bytes / 16 + 255) / 256;
-    if (blocks > 592) blocks = 592;
+int launch_frame_diff(const MpStreamDesc* d, int n, const MpStreamDesc& one, size_t bytes, unsigned long long* sum,
+                      cudaStream_t s) {
+    // ingest_units counts the 16-byte units of a frame in 32 bits
+    SKPS_CHECK(bytes < (1ull << 32) - 16 || !(d || one.src), "frame_diff: a %zu-byte frame is larger than 4 GB", bytes);
+    // a 16-byte unit per thread, at most 8 blocks per SM per frame
+    size_t blocks = (bytes / 16 + 255) / 256;
+    if (blocks > (size_t)sm_count() * 8) blocks = (size_t)sm_count() * 8;
     if (blocks < 1) blocks = 1;
-    return (int)blocks;
-}
-int launch_mp_absdiff(const MpStreamDesc* d, unsigned long long* diff, int n, size_t max_bytes, cudaStream_t s) {
-    SKPS_CHECK(max_bytes < (1ull << 32) - 16, "absdiff: a %zu-byte frame is larger than 4 GB", max_bytes);
-    mp_absdiff_kernel<<<dim3(absdiff_grid(max_bytes), n), 256, 0, s>>>(d, MpStreamDesc{}, diff);
-    SKPS_CUDA(cudaGetLastError());
-    return 0;
-}
-int launch_frame_ingest(const MpStreamDesc& one, unsigned long long* diff, cudaStream_t s) {
-    const size_t bytes = (size_t)one.H * one.W * 3;
-    SKPS_CHECK(bytes < (1ull << 32) - 16, "ingest: a %zu-byte frame is larger than 4 GB", bytes);
-    mp_absdiff_kernel<<<dim3(absdiff_grid(bytes), 1), 256, 0, s>>>(nullptr, one, diff);
+    diff_frames_kernel<<<dim3((unsigned)blocks, n), 256, 0, s>>>(d, one, bytes, sum);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }
@@ -636,39 +571,24 @@ int check_device_frame(const void* frame, int device, const char* fn, int index)
     else set_error("%s: frame %d is not in memory of device %d", fn, index, device);
     return 1;
 }
-int launch_mp_letterbox(const MpStreamDesc* d, uint8_t* out, size_t out_stride, int in_h, int in_w, int n, cudaStream_t s) {
-    mp_letterbox_kernel<<<dim3((in_w + 255) / 256, in_h, n), 256, 0, s>>>(d, out, out_stride, in_h, in_w);
+int launch_letterbox(const LetterboxArgs& a, int n, cudaStream_t s) {
+    letterbox_frames_kernel<<<dim3((a.in_w + 255) / 256, a.in_h, n), 256, 0, s>>>(a);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }
-int launch_mp_crop(const MpStreamDesc* d, const float* boxes, const int* count, int K, float face_scale, float min_face,
-                   uint8_t* crops, int S, int* detail, int n, cudaStream_t s) {
-    mp_crop_kernel<<<dim3((S + 255) / 256, S, K * n), 256, 0, s>>>(d, boxes, count, K, face_scale, min_face, crops, S, detail);
+int launch_crop(const CropArgs& a, int n, cudaStream_t s) {
+    crop_frames_kernel<<<dim3((a.S + 255) / 256, a.S, a.K * n), 256, 0, s>>>(a);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }
-int launch_mp_landmark_post(const float* xy, const int* detail, const int* count, int K, int P, float* kps, int n, cudaStream_t s) {
+int launch_landmark_post(const float* xy, const int* detail, const int* count, int K, int P, float* kps, int n, cudaStream_t s) {
     const int total = K * P * n;
-    mp_landmark_post_kernel<<<(total + 255) / 256, 256, 0, s>>>(xy, detail, count, K, P, kps, n);
+    landmark_post_frames_kernel<<<(total + 255) / 256, 256, 0, s>>>(xy, detail, count, K, P, kps, n);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }
-
-int launch_mp_select(const float* det_rows, const int* det_count, int det_cap, const int* det_slot, const int* flag,
-                     const float* track, const int* n_track, float iou_thres, float alpha, float oma, float min_face, int top_k,
-                     float* boxes4, int* count, int* src, int n_streams, cudaStream_t s) {
-    mp_select_kernel<<<n_streams, SEL_THREADS, 0, s>>>(det_rows, det_count, det_cap, det_slot, flag, track, n_track, iou_thres,
-                                                       alpha, oma, min_face, top_k, boxes4, count, src);
-    SKPS_CUDA(cudaGetLastError());
-    return 0;
-}
-
-int launch_select_faces(const float* det_rows, const int32_t* det_count, int det_stride, const float* track, int n_track,
-                        float iou_thres, float alpha, float one_minus_alpha, float min_face, int top_k, float* boxes4,
-                        int32_t* count, int32_t* src, bool src_is_row, cudaStream_t s) {
-    SKPS_CHECK(det_rows && det_count && boxes4 && count && top_k > 0 && top_k <= SEL_MAX_K, "select_faces: bad arguments");
-    select_faces_kernel<<<1, SEL_THREADS, 0, s>>>(det_rows, det_count, det_stride, track, track ? n_track : 0, iou_thres, alpha,
-                                                  one_minus_alpha, min_face, top_k, boxes4, count, src, src_is_row ? 1 : 0);
+int launch_select(const SelectArgs& a, int n, cudaStream_t s) {
+    select_frames_kernel<<<n, SEL_THREADS, 0, s>>>(a);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }
@@ -683,28 +603,32 @@ using namespace skps;
 extern "C" SKPS_API int skps_letterbox(const uint8_t* frame, int H, int W, int pitch, uint8_t* out, int in_h, int in_w,
                               int rw, int rh, int top, int left, void* stream) {
     SKPS_CHECK(frame && out && H > 0 && W > 0 && rw > 0 && rh > 0, "letterbox: bad arguments");
-    dim3 grid((in_w + 255) / 256, in_h);
-    letterbox_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(frame, H, W, pitch, out, in_h, in_w, rw, rh, top, left);
-    SKPS_CUDA(cudaGetLastError());
-    return 0;
+    LetterboxArgs a = {};
+    a.frame = frame; a.H = H; a.W = W; a.pitch = pitch; a.rw = rw; a.rh = rh; a.top = top; a.left = left;
+    a.out = out; a.in_h = in_h; a.in_w = in_w;
+    return launch_letterbox(a, 1, (cudaStream_t)stream);
 }
 
 extern "C" SKPS_API int skps_select_faces(const float* det_rows, const int32_t* det_count, int det_stride, const float* track,
                                  int n_track, float iou_thres, float alpha, float one_minus_alpha, float min_face,
                                  int top_k, float* boxes4, int32_t* count, void* stream) {
-    return launch_select_faces(det_rows, det_count, det_stride, track, n_track, iou_thres, alpha, one_minus_alpha, min_face,
-                               top_k, boxes4, count, nullptr, false, (cudaStream_t)stream);
+    SKPS_CHECK(det_rows && det_count && boxes4 && count && top_k > 0 && top_k <= SEL_MAX_K, "select_faces: bad arguments");
+    SelectArgs a = {};
+    a.det_rows = det_rows; a.det_count = det_count; a.det_stride = det_stride; a.flag1 = 1;
+    a.track = track; a.n_track1 = n_track;
+    a.iou_thres = iou_thres; a.alpha = alpha; a.one_minus_alpha = one_minus_alpha; a.min_face = min_face; a.top_k = top_k;
+    a.boxes4 = boxes4; a.count = count;
+    return launch_select(a, 1, (cudaStream_t)stream);
 }
 
 extern "C" SKPS_API int skps_crop_resize(const uint8_t* frame, int H, int W, int pitch, const float* boxes4,
                                 const int32_t* count, int max_faces, float face_scale, float min_face,
                                 uint8_t* crops, int out_hw, int32_t* detail, void* stream) {
     SKPS_CHECK(frame && boxes4 && count && crops && detail && max_faces > 0, "crop_resize: bad arguments");
-    dim3 grid((out_hw + 255) / 256, out_hw, max_faces);
-    crop_resize_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(frame, H, W, pitch, boxes4, count, face_scale,
-                                                               min_face, crops, out_hw, detail);
-    SKPS_CUDA(cudaGetLastError());
-    return 0;
+    CropArgs a = {};
+    a.frame = frame; a.H = H; a.W = W; a.pitch = pitch; a.boxes = boxes4; a.count = count; a.K = max_faces;
+    a.face_scale = face_scale; a.min_face = min_face; a.crops = crops; a.S = out_hw; a.detail = detail;
+    return launch_crop(a, 1, (cudaStream_t)stream);
 }
 
 extern "C" SKPS_API int skps_crop_faces(const skps_face_src* src, const float* boxes4, int n, float face_scale, float min_face,
@@ -739,11 +663,7 @@ extern "C" SKPS_API int skps_nme(const float* target, const float* preds, int n,
 extern "C" SKPS_API int skps_landmark_post(const float* xy_norm, const int32_t* detail, const int32_t* count, int max_faces,
                                   int n_points, float* kps, void* stream) {
     SKPS_CHECK(xy_norm && detail && count && kps, "landmark_post: bad arguments");
-    int total = max_faces * n_points;
-    landmark_post_kernel<<<(total + 127) / 128, 128, 0, (cudaStream_t)stream>>>(xy_norm, detail, count, max_faces,
-                                                                               n_points, kps);
-    SKPS_CUDA(cudaGetLastError());
-    return 0;
+    return launch_landmark_post(xy_norm, detail, count, max_faces, n_points, kps, 1, (cudaStream_t)stream);
 }
 
 extern "C" SKPS_API int skps_frame_absdiff_sum(const uint8_t* a, const uint8_t* b, size_t n, unsigned long long* sum,
@@ -751,10 +671,9 @@ extern "C" SKPS_API int skps_frame_absdiff_sum(const uint8_t* a, const uint8_t* 
     SKPS_CHECK(a && b && sum, "absdiff: bad arguments");
     SKPS_CHECK(((uintptr_t)a % 16 == 0) && ((uintptr_t)b % 16 == 0), "absdiff: pointers must be 16-byte aligned");
     SKPS_CUDA(cudaMemsetAsync(sum, 0, sizeof(unsigned long long), (cudaStream_t)stream));
-    const int blocks = sm_count() * 8;
-    absdiff_sum_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a, b, n, sum);
-    SKPS_CUDA(cudaGetLastError());
-    return 0;
+    MpStreamDesc D = {};
+    D.prev = a; D.cur = const_cast<uint8_t*>(b); D.have_prev = 1;      // cur is written only when src is set
+    return launch_frame_diff(nullptr, 1, D, n, sum, (cudaStream_t)stream);
 }
 
 extern "C" SKPS_API int skps_frame_ingest(const uint8_t* frame, int H, int W, int pitch, uint8_t* packed, const uint8_t* prev,
@@ -765,5 +684,5 @@ extern "C" SKPS_API int skps_frame_ingest(const uint8_t* frame, int H, int W, in
     MpStreamDesc D = {};
     D.cur = packed; D.prev = prev; D.have_prev = prev != nullptr; D.H = H; D.W = W;
     D.src = frame; D.src_pitch = pitch;
-    return launch_frame_ingest(D, sum, (cudaStream_t)stream);
+    return launch_frame_diff(nullptr, 1, D, (size_t)H * W * 3, sum, (cudaStream_t)stream);
 }

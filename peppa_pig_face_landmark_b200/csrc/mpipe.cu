@@ -214,7 +214,7 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
 }
 
 // One batch.  Host frames (pitches null) are uploaded on the copy stream into the next ring position; device frames (rows
-// pitches[i] bytes apart) are gathered there by the mp_absdiff launch on the compute stream, after the work queued on
+// pitches[i] bytes apart) are gathered there by the frame-difference launch on the compute stream, after the work queued on
 // `producer`, whose later work waits for that launch.  out: results into caller buffers on the device instead of the slot's
 // pinned ones.
 static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* hw, int n,
@@ -303,7 +303,7 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     }
     SKPS_CUDA(cudaMemcpyAsync(p->d_desc, sl.h_desc, sizeof(MpStreamDesc) * n_desc, cudaMemcpyHostToDevice, sx));
     SKPS_CUDA(cudaEventRecord(sl.ev_staged, sx));
-    if (launch_mp_absdiff(p->d_desc, p->d_diff, n, max_bytes, sx)) return 1;
+    if (launch_frame_diff(p->d_desc, n, MpStreamDesc{}, max_bytes, p->d_diff, sx)) return 1;
     if (on_device) {
         SKPS_CUDA(cudaEventRecord(p->ev_read, sx));
         SKPS_CUDA(cudaStreamWaitEvent(producer, p->ev_read, 0));
@@ -311,7 +311,9 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     // results: D2H into the slot's pinned buffers, or D2D into the caller's; either way before the next batch on sx can
     // overwrite d_out_kps, the engine's score output or the chips
     const cudaMemcpyKind result_kind = out ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-    if (m > 0 && launch_mp_letterbox(d_key_desc, det_in, det_in_bytes, p->det_h, p->det_w, m, sx)) return 1;
+    LetterboxArgs la = {};
+    la.desc = d_key_desc; la.out = det_in; la.out_stride = det_in_bytes; la.in_h = p->det_h; la.in_w = p->det_w;
+    if (m > 0 && launch_letterbox(la, m, sx)) return 1;
     if (launch_mp_decide(p->d_diff, p->d_hw, p->d_have_prev, det_slot, p->d_flag, n, sx)) return 1;
     // the detector runs for every keyframe of the batch (one launch sequence, batch m); the gate only chooses whose rows are
     // used.  With no keyframe the detector and NMS are skipped and every stream takes the tracker path.
@@ -325,15 +327,20 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
         na.ws = p->d_nms_ws; na.ws_cap = p->det_rows;
         if (launch_nms(na, sx)) return 1;
     }
-    if (launch_mp_select(p->d_det_rows, p->d_det_count, p->det_rows, det_slot, p->d_flag, p->d_track_f32, p->d_n_track,
-                         c.track_iou, c.alpha, (float)(1.0 - (double)c.alpha), c.min_face, K, p->d_boxes, p->d_count, p->d_src,
-                         n, sx))
-        return 1;
+    SelectArgs sa = {};
+    sa.det_rows = p->d_det_rows; sa.det_count = p->d_det_count; sa.det_stride = 16; sa.det_cap = p->det_rows;
+    sa.det_slot = det_slot; sa.flag = p->d_flag; sa.track = p->d_track_f32; sa.n_track = p->d_n_track;
+    sa.iou_thres = c.track_iou; sa.alpha = c.alpha; sa.one_minus_alpha = (float)(1.0 - (double)c.alpha);
+    sa.min_face = c.min_face; sa.top_k = K;
+    sa.boxes4 = p->d_boxes; sa.count = p->d_count; sa.src = p->d_src;
+    if (launch_select(sa, n, sx)) return 1;
     uint8_t* kps_in = (uint8_t*)skps_engine_input_ptr(p->kps);
-    if (launch_mp_crop(p->d_desc, p->d_boxes, p->d_count, K, c.face_scale, c.kps_min_face, kps_in, p->kps_hw, p->d_detail, n, sx))
-        return 1;
+    CropArgs ca = {};
+    ca.desc = p->d_desc; ca.boxes = p->d_boxes; ca.count = p->d_count; ca.K = K;
+    ca.face_scale = c.face_scale; ca.min_face = c.kps_min_face; ca.crops = kps_in; ca.S = p->kps_hw; ca.detail = p->d_detail;
+    if (launch_crop(ca, n, sx)) return 1;
     if (skps_engine_forward(p->kps, kps_in, n * K, nullptr, sx)) return 1;
-    if (launch_mp_landmark_post(skps_engine_output_ptr(p->kps, 0), p->d_detail, p->d_count, K, P, p->d_kps_now, n, sx)) return 1;
+    if (launch_landmark_post(skps_engine_output_ptr(p->kps, 0), p->d_detail, p->d_count, K, P, p->d_kps_now, n, sx)) return 1;
     MpTemporalArgs a;
     a.top_k = K; a.n_points = P;
     a.kps_now = p->d_kps_now; a.count = p->d_count; a.flag = p->d_flag; a.hw = p->d_hw; a.boxes4 = p->d_boxes;

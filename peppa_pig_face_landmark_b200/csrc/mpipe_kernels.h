@@ -23,7 +23,7 @@ struct MpTemporalArgs {
     double* track_box;           // [S][K][4] float64 track boxes (returned as 'box')
     float* track_f32;            // [S][K][4] the same, as float32 (next frame's judge_boxs / crop input)
     int* n_track;                // [S]
-    const int* src;              // [S][K] source of each face this frame (launch_mp_select), an index into the old track
+    const int* src;              // [S][K] source of each face this frame (launch_select), an index into the old track
     int64_t* ids;                // [S][K] track id of each track box
     int64_t* next_id;            // [S] the next unused id of the stream
     // outputs
@@ -41,23 +41,73 @@ struct MpStreamDesc {
     int H, W, have_prev;
     float scale;                 // letterbox geometry (face_detector.py:49-62)
     int rw, rh, top, left;
-    const uint8_t* src;          // the caller's device frame, gathered into cur by launch_mp_absdiff, or null (cur holds it)
+    const uint8_t* src;          // the caller's device frame, gathered into cur by launch_frame_diff, or null (cur holds it)
     int src_pitch;               // bytes from one row of src to the next, >= 3 W, any alignment
 };
-// Batched over the streams of a call (grid z / x = stream): what S x {skps_frame_absdiff_sum, skps_letterbox,
-// skps_crop_resize, skps_landmark_post} launches did, in four launches.  Same device code per element, bit for bit.
-// launch_mp_absdiff also ingests: a stream with src set gets its frame gathered into cur and, with have_prev, |cur - prev|
-// summed in the same pass (the same integer sum as from a packed cur).  d [dev] holds n descriptors; launch_frame_ingest
-// runs the same kernel on one descriptor passed by value (diff = one counter, zeroed by the caller).
-int launch_mp_absdiff(const MpStreamDesc* d, unsigned long long* diff, int n, size_t max_bytes, cudaStream_t s);
-int launch_frame_ingest(const MpStreamDesc& one, unsigned long long* diff, cudaStream_t s);
+
+// Image ops (image_ops.cu): one kernel per op, launched by skps_pipeline (FaceAna), skps_mpipe (FaceAnaStreams) and the
+// public skps_letterbox, skps_crop_resize, skps_select_faces, skps_landmark_post, skps_frame_absdiff_sum and
+// skps_frame_ingest alike.  A launch covers one frame, given by pointer, size and row pitch with its per-frame counts and
+// flags as scalars, or the n frames of a call, given by their descriptors desc [dev] (cur, H, W, row pitch 3 W) with
+// per-frame device arrays.  Only the addressing at the top of a kernel tells the two apart; the per-element code is one.
+
+// Letterbox (face_detector.py:45-71) of frame g into out + g * out_stride, in_h x in_w x 3 RGB.
+struct LetterboxArgs {
+    const uint8_t* frame; int H, W, pitch;      // the one frame (desc null) ...
+    int rw, rh, top, left;                      // ... and its letterbox geometry
+    const MpStreamDesc* desc;                   // or frame g's: desc[g], geometry included
+    uint8_t* out; size_t out_stride;
+    int in_h, in_w;
+};
+int launch_letterbox(const LetterboxArgs& a, int n, cudaStream_t s);
+
+// Crop + resize (face_landmark.py:66-104) of faces i < count[g] of frame g into crops [g][i] (S x S x 3) and detail [g][i]
+// ([h, w, y1, x1, add]); faces i >= count[g] of the K get zeros.
+struct CropArgs {
+    const uint8_t* frame; int H, W, pitch;      // the one frame (desc null), or
+    const MpStreamDesc* desc;                   // frame g's: desc[g].cur, H, W
+    const float* boxes; const int* count;       // [n][K][4], [n] [dev]
+    int K;
+    float face_scale, min_face;
+    uint8_t* crops; int S; int* detail;         // [n][K][S][S][3], [n][K][5]
+};
+int launch_crop(const CropArgs& a, int n, cudaStream_t s);
+
+// judge_boxs + sort_and_filter (facer.py:58-64), one block per frame.  Frame g selects from the rows of its detector frame
+// f = det_slot[g] (det_slot null: f = g), det_count[f] rows of det_stride floats at det_rows + f * det_cap * det_stride,
+// IoU-matched against its track boxes, when it ran the detector; else from its track boxes themselves (facer.py:61).
+// src [n][top_k] [dev] or null: each selected face's source for the track ids, the row it came from when the rows are the
+// track boxes, else the index of the track box its detection matched, -1 for none.
+struct SelectArgs {
+    const float* det_rows; const int* det_count;    // [dev]
+    int det_stride, det_cap;
+    const int* det_slot;                            // [n] [dev] or null
+    const int* flag;                                // [n] [dev]: frame g ran the detector, or null: flag1
+    const float* track;                             // [n][top_k][4] [dev], or null (no track boxes)
+    const int* n_track;                             // [n] [dev], or null: n_track1
+    int flag1, n_track1;
+    float iou_thres, alpha, one_minus_alpha, min_face;
+    int top_k;                                      // 1..SKPS_MAX_TOP_K
+    float* boxes4; int* count; int* src;            // [n][top_k][4], [n], [n][top_k] [dev]
+};
+int launch_select(const SelectArgs& a, int n, cudaStream_t s);
+
+// FaceLandmark.postprocess (face_landmark.py:106-115): the landmarks xy [n][K][P][2] of the crops described by detail
+// [n][K][5] in frame pixels, kps [n][K][P][2]; zeros for faces i >= count[g].
+int launch_landmark_post(const float* xy, const int* detail, const int* count, int K, int P, float* kps, int n, cudaStream_t s);
+
+// The frame-difference gate (facer.py:111-113): sum[g] += sum |cur - prev| over frame g's bytes when have_prev.  A frame
+// with src set is first gathered into cur in the same pass (the same integer sum as from a packed cur).  Frame g is d[g]
+// [dev], or (d null, n = 1) `one` of `bytes` bytes, any count when one.src is null; with d, bytes is the largest frame's.
+int launch_frame_diff(const MpStreamDesc* d, int n, const MpStreamDesc& one, size_t bytes, unsigned long long* sum,
+                      cudaStream_t s);
+
 // Frame staging on the host side, shared by skps_pipeline and skps_mpipe.  upload_host_frame queues the H2D copy of a [host]
 // frame of `bytes` bytes into dst on s: a pinned frame is copied as it is, a pageable one first into `stage` (pinned, at
 // least `bytes`) so that the copy stays asynchronous and at full PCIe rate.  check_device_frame fails unless `frame` is
 // device or managed memory of `device`; the error names the caller `fn` and, for index >= 0, the frame's index.
 int upload_host_frame(const uint8_t* frame, size_t bytes, uint8_t* stage, uint8_t* dst, cudaStream_t s);
 int check_device_frame(const void* frame, int device, const char* fn, int index);
-int launch_mp_letterbox(const MpStreamDesc* d, uint8_t* out, size_t out_stride, int in_h, int in_w, int n, cudaStream_t s);
 
 // Detector post-processing (nms.cu): score filter, sort, greedy NMS and scale_coords of `batch` frames of `rows` raw rows each
 // (raw [batch][rows][16]), for any number of candidates.  Frame f keeps its boxes in kept_rows [f][capacity][16] /
@@ -80,22 +130,6 @@ struct NmsArgs {
 size_t nms_workspace_bytes(int cap, int batch);
 int launch_nms(const NmsArgs& a, cudaStream_t s);
 
-int launch_mp_crop(const MpStreamDesc* d, const float* boxes, const int* count, int K, float face_scale, float min_face,
-                   uint8_t* crops, int S, int* detail, int n, cudaStream_t s);
-int launch_mp_landmark_post(const float* xy, const int* detail, const int* count, int K, int P, float* kps, int n, cudaStream_t s);
-
-// judge_boxs + sort_and_filter (image_ops.cu).  src [dev] (top_k) or null: each selected face's source for the track ids,
-// the row it came from when src_is_row (the rows are the previous track boxes), else the index of the track box its
-// detection matched, -1 for none.  skps_select_faces is this with src null.
-int launch_select_faces(const float* det_rows, const int32_t* det_count, int det_stride, const float* track, int n_track,
-                        float iou_thres, float alpha, float one_minus_alpha, float min_face, int top_k, float* boxes4,
-                        int32_t* count, int32_t* src, bool src_is_row, cudaStream_t s);
-// The same per stream of a batch; src [dev] [S][K] as above, the rows being the track boxes where flag[s] == 0.  det_slot
-// [dev] [S]: the detector frame (row of det_rows / det_count) of each stream, -1 where the detector did not run on it; null:
-// frame s is stream s's.
-int launch_mp_select(const float* det_rows, const int* det_count, int det_cap, const int* det_slot, const int* flag,
-                     const float* track, const int* n_track, float iou_thres, float alpha, float oma, float min_face, int top_k,
-                     float* boxes4, int* count, int* src, int n_streams, cudaStream_t s);
 // flag[s] = the stream uses its detector rows: det_slot[s] >= 0 (det_slot null: always) and (!have_prev[s] or the mean
 // difference > 5)
 int launch_mp_decide(const unsigned long long* diff, const int* hw, const int* have_prev, const int* det_slot, int* flag, int n,

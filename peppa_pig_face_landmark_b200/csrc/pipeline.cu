@@ -167,11 +167,14 @@ extern "C" SKPS_API int skps_pipeline_frame_diff(skps_pipeline* p, const uint8_t
         *mean_diff = -1.0;
         return 0;
     }
-    if (skps_frame_absdiff_sum(p->d_frame[p->cur ^ 1], p->d_frame[p->cur], n, p->d_diff, s)) return 1;
+    SKPS_CUDA(cudaMemsetAsync(p->d_diff, 0, sizeof(unsigned long long), s));
+    MpStreamDesc D = {};
+    D.cur = p->d_frame[p->cur]; D.prev = p->d_frame[p->cur ^ 1]; D.have_prev = 1; D.H = H; D.W = W;
+    if (launch_frame_diff(nullptr, 1, D, n, p->d_diff, s)) return 1;
     return read_mean_diff(p, H, W, mean_diff, s);
 }
 
-// One skps_frame_ingest pass gathers the [dev] frame into d_frame[cur] and, against a previous frame of the same size, sums
+// One ingest pass gathers the [dev] frame into d_frame[cur] and, against a previous frame of the same size, sums
 // the difference.  The read waits for the work queued on the producer stream so far, and the producer's later work waits
 // for the read.
 extern "C" SKPS_API int skps_pipeline_frame_diff_device(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch,
@@ -188,7 +191,7 @@ extern "C" SKPS_API int skps_pipeline_frame_diff_device(skps_pipeline* p, const 
     D.cur = p->d_frame[p->cur]; D.prev = diff ? p->d_frame[p->cur ^ 1] : nullptr; D.have_prev = diff;
     D.H = H; D.W = W; D.src = frame; D.src_pitch = pitch;
     if (diff) SKPS_CUDA(cudaMemsetAsync(p->d_diff, 0, sizeof(unsigned long long), s));
-    if (launch_frame_ingest(D, p->d_diff, s)) return 1;
+    if (launch_frame_diff(nullptr, 1, D, (size_t)H * W * 3, p->d_diff, s)) return 1;
     SKPS_CUDA(cudaEventRecord(p->ev_read, s));
     SKPS_CUDA(cudaStreamWaitEvent(producer, p->ev_read, 0));
     p->cur_h = H; p->cur_w = W;
@@ -234,8 +237,12 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, int run_detector, in
         SKPS_CUDA(cudaMemcpyAsync(p->d_track, p->h_track, sizeof(float) * 4 * n_track, cudaMemcpyHostToDevice, s));
     }
     if (run_detector) {
+        SKPS_CHECK(rw > 0 && rh > 0, "pipeline_run: letterbox size %dx%d", rw, rh);
         uint8_t* det_in = (uint8_t*)skps_engine_input_ptr(p->det);
-        if (skps_letterbox(d_frame, H, W, W * 3, det_in, p->det_h, p->det_w, rw, rh, top, left, s)) return 1;
+        LetterboxArgs la = {};
+        la.frame = d_frame; la.H = H; la.W = W; la.pitch = W * 3; la.rw = rw; la.rh = rh; la.top = top; la.left = left;
+        la.out = det_in; la.in_h = p->det_h; la.in_w = p->det_w;
+        if (launch_letterbox(la, 1, s)) return 1;
         if (skps_engine_forward(p->det, det_in, 1, nullptr, s)) return 1;
         NmsArgs na = {};
         na.raw = skps_engine_output_ptr(p->det, 0); na.rows = p->det_rows; na.batch = 1;
@@ -245,20 +252,15 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, int run_detector, in
         na.kept_rows = p->d_det_rows; na.kept_idx = p->d_det_idx; na.count = p->d_det_count;
         na.ws = p->d_nms_ws; na.ws_cap = p->det_rows;
         if (launch_nms(na, s)) return 1;
-        // facer.py:58 judge_boxs(track_box, boxes) then :64 sort_and_filter
-        if (launch_select_faces(p->d_det_rows, p->d_det_count, 16, n_track > 0 ? p->d_track : nullptr, n_track,
-                                c.track_iou, c.alpha, (float)(1.0 - (double)c.alpha), c.min_face, K, p->d_boxes,
-                                p->d_count, d_src, false, s))
-            return 1;
-    } else {
-        // facer.py:61: boxes = track_box, then sort_and_filter
-        int32_t nt = n_track;
-        p->h_res->n_det = nt;
-        SKPS_CUDA(cudaMemcpyAsync(p->d_det_count, &p->h_res->n_det, sizeof(int32_t), cudaMemcpyHostToDevice, s));
-        if (launch_select_faces(p->d_track, p->d_det_count, 4, nullptr, 0, c.track_iou, c.alpha,
-                                (float)(1.0 - (double)c.alpha), c.min_face, K, p->d_boxes, p->d_count, d_src, true, s))
-            return 1;
     }
+    // facer.py:58 judge_boxs(track_box, boxes) on the detector's boxes, or :61 boxes = track_box; then :64 sort_and_filter
+    SelectArgs sa = {};
+    sa.det_rows = p->d_det_rows; sa.det_count = p->d_det_count; sa.det_stride = 16; sa.flag1 = run_detector != 0;
+    sa.track = p->d_track; sa.n_track1 = n_track;
+    sa.iou_thres = c.track_iou; sa.alpha = c.alpha; sa.one_minus_alpha = (float)(1.0 - (double)c.alpha);
+    sa.min_face = c.min_face; sa.top_k = K;
+    sa.boxes4 = p->d_boxes; sa.count = p->d_count; sa.src = d_src;
+    if (launch_select(sa, 1, s)) return 1;
     // the face count decides how many crops the landmark net sees
     SKPS_CUDA(cudaMemcpyAsync(&p->h_res->n_faces, p->d_count, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     SKPS_CUDA(cudaStreamSynchronize(s));
@@ -266,16 +268,18 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, int run_detector, in
     // chunks of exactly the selected faces: the crops go straight into the engine's input, the landmarks and scores of
     // each chunk to their offsets in d_kps / d_scores (the next chunk overwrites the engine's outputs)
     uint8_t* kps_in = (uint8_t*)skps_engine_input_ptr(p->kps);
+    CropArgs ca = {};
+    ca.frame = d_frame; ca.H = H; ca.W = W; ca.pitch = W * 3;
+    ca.face_scale = c.face_scale; ca.min_face = c.kps_min_face; ca.crops = kps_in; ca.S = p->kps_hw;
     for (int f0 = 0; f0 < nf; f0 += SKPS_LANDMARK_CHUNK) {
         const int nc = nf - f0 < SKPS_LANDMARK_CHUNK ? nf - f0 : SKPS_LANDMARK_CHUNK;
         const int32_t* d_nc = p->d_counts + nc;
-        if (skps_crop_resize(d_frame, H, W, W * 3, p->d_boxes + 4 * f0, d_nc, nc, c.face_scale, c.kps_min_face, kps_in,
-                             p->kps_hw, p->d_detail + 5 * f0, s))
-            return 1;
+        ca.boxes = p->d_boxes + 4 * f0; ca.count = d_nc; ca.K = nc; ca.detail = p->d_detail + 5 * f0;
+        if (launch_crop(ca, 1, s)) return 1;
         float* outs[2] = {nullptr, p->d_scores + (size_t)P * f0};
         if (skps_engine_forward(p->kps, kps_in, nc, outs, s)) return 1;
-        if (skps_landmark_post(skps_engine_output_ptr(p->kps, 0), p->d_detail + 5 * f0, d_nc, nc, P,
-                               p->d_kps + (size_t)2 * P * f0, s))
+        if (launch_landmark_post(skps_engine_output_ptr(p->kps, 0), p->d_detail + 5 * f0, d_nc, nc, P,
+                                 p->d_kps + (size_t)2 * P * f0, 1, s))
             return 1;
     }
     if (nf > 0) {

@@ -63,7 +63,8 @@ def test_no_row_near_the_score_threshold(oracle_raw, name):
     assert np.abs(raw[:, 4] - 0.5).min() > THRESHOLD_CLEARANCE, name
 
 
-def test_nms_and_selection_kernels_do_not_spill():
+def test_each_nms_and_selection_kernel_does_not_spill():
+    # the four NMS kernels of nms.cu and the one selection kernel FaceAna and FaceAnaStreams share, each by name
     found = []
     for src, names in (("nms.cu", ("nms_",)), ("image_ops.cu", ("select_",))):
         out = _ptxas_report(src)
@@ -72,6 +73,8 @@ def test_nms_and_selection_kernels_do_not_spill():
         mine = [p for p in props if any(k in p[0] for k in names)]
         assert mine, out
         found += mine
-    assert len(found) >= 6
+    for k in ("nms_greedy_kernel", "nms_merge_kernel", "nms_chunk_sort_kernel", "nms_compact_kernel",
+              "select_frames_kernel"):
+        assert any(k in p[0] for p in found), (k, found)
     bad = [p for p in found if p[1:] != ("0", "0", "0")]
     assert not bad, bad

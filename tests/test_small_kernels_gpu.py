@@ -1,5 +1,5 @@
 """Direct kernel-vs-oracle unit tests of the small fused kernels that the whole-network tests only cover implicitly:
-select_faces_kernel (judge_boxs + sort_and_filter, facer.py:120-189), se_fc_kernel (squeeze-excite gate) and
+skps_select_faces (judge_boxs + sort_and_filter, facer.py:120-189), se_fc_kernel (squeeze-excite gate) and
 hm_decode_kernel (arg-max + offsets, model.py:511-554; ties -> first index)."""
 import ctypes as C
 
