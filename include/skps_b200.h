@@ -190,6 +190,26 @@ SKPS_API int skps_letterbox(const uint8_t* frame, int H, int W, int pitch,
                    uint8_t* out, int in_h, int in_w,
                    int rw, int rh, int top, int left, void* stream);
 
+/* Where one frame's pixels are, for skps_letterbox_frames.  With row_pairs = 0, `base` holds the
+ * whole H x W frame, rows `pitch` bytes apart (a CUDA frame read where it is, at any pitch).  With
+ * row_pairs = 1, `base` holds 2*rh rows `pitch` bytes apart: rows 2y and 2y+1 are the frame rows
+ * i0 and i1 of cv2's vertical tap for resized row y (linear_tap(y, rh, H) in image_ops.cu), the
+ * only rows output row top+y reads.  Both rows of a pair are always held, even where the weight of
+ * i1 is 0.  FaceDetector uploads a host frame that way when 2*rh < H, so a 4K frame at 384x640
+ * sends 720 of its 2160 rows. */
+typedef struct skps_det_src {
+    const uint8_t* base;                /* [dev] the rows of the frame this descriptor holds          */
+    int32_t pitch;                      /* bytes from one held row to the next (>= 3W, any alignment) */
+    int32_t H, W;                       /* the whole frame                                            */
+    int32_t rw, rh, top, left;          /* letterbox geometry (face_detector.py:49-62)                */
+    int32_t row_pairs;                  /* 0: base holds rows 0..H-1; 1: base holds 2*rh row pairs    */
+} skps_det_src;
+
+/* skps_letterbox for n frames (0..65535) of any sizes in one launch: frame i, described by src[i]
+ * [dev], is letterboxed into out [dev] + i*in_h*in_w*3.  The bytes of each frame are those
+ * skps_letterbox writes for the whole frame with the same geometry. */
+SKPS_API int skps_letterbox_frames(const skps_det_src* src, int n, uint8_t* out, int in_h, int in_w, void* stream);
+
 /* xywh2xyxy + py_nms + scale_coords (face_detector.py:73-136) on the raw (rows,16) output.
  * Writes up to max_det (<= 256) kept rows (16 floats each, cols 0-3 mapped back to frame pixels),
  * their row indices into the raw output, and the count.  All [dev].  This entry keeps its limit:

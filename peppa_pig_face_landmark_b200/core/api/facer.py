@@ -118,7 +118,7 @@ class FaceAna():
             logger.setLevel(logging.DEBUG)
         if det_input is not None:
             cfg['Skps']['Detect']['input_shape'] = [det_input[0], det_input[1], 3]
-        self.face_detector = FaceDetector(cfg['Skps']['Detect'])
+        self.face_detector = FaceDetector(cfg['Skps']['Detect'], max_frames=1)
         self.face_landmark = FaceLandmark(cfg['Skps']['Keypoints'], max_faces=min(self.top_k, LANDMARK_CHUNK))
         self.trace = GroupTrack(cfg['Skps']['Trace'])
         logger.info('model init done!')

@@ -45,7 +45,8 @@ __device__ __forceinline__ int vblend(int h0, int h1, int b0, int b1) {
 // Letterbox (face_detector.py:45-71): BGR->RGB, resize to (rw,rh), pad 114.  One thread per
 // output pixel (3 channels); output is uint8 RGB NHWC, /255 happens in the first conv.
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void letterbox_px(const uint8_t* __restrict__ frame, int H, int W, int pitch,
+// `frame` holds the whole frame, or with row_pairs only the two rows each resized row reads: rows 2 dy and 2 dy + 1.
+__device__ __forceinline__ void letterbox_px(const uint8_t* __restrict__ frame, int H, int W, int pitch, int row_pairs,
                                              uint8_t* __restrict__ out, int in_h, int in_w, int rw, int rh, int top, int left,
                                              int x, int y) {
     if (x >= in_w) return;
@@ -57,8 +58,8 @@ __device__ __forceinline__ void letterbox_px(const uint8_t* __restrict__ frame, 
     }
     Tap tx = linear_tap(dx, rw, W, true);
     Tap ty = linear_tap(dy, rh, H, false);
-    const uint8_t* r0 = frame + (long long)ty.i0 * pitch;
-    const uint8_t* r1 = frame + (long long)ty.i1 * pitch;
+    const uint8_t* r0 = frame + (long long)(row_pairs ? 2 * dy : ty.i0) * pitch;
+    const uint8_t* r1 = frame + (long long)(row_pairs ? 2 * dy + 1 : ty.i1) * pitch;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
         int h0 = r0[tx.i0 * 3 + c] * tx.w0 + r0[tx.i1 * 3 + c] * tx.w1;
@@ -69,12 +70,16 @@ __device__ __forceinline__ void letterbox_px(const uint8_t* __restrict__ frame, 
 // block z = frame
 __global__ void __launch_bounds__(256) letterbox_frames_kernel(const LetterboxArgs a) {
     const uint8_t* frame = a.frame;
-    int H = a.H, W = a.W, pitch = a.pitch, rw = a.rw, rh = a.rh, top = a.top, left = a.left;
+    int H = a.H, W = a.W, pitch = a.pitch, rw = a.rw, rh = a.rh, top = a.top, left = a.left, row_pairs = 0;
     if (a.desc) {
         const MpStreamDesc D = a.desc[blockIdx.z];
         frame = D.cur; H = D.H; W = D.W; pitch = D.W * 3; rw = D.rw; rh = D.rh; top = D.top; left = D.left;
+    } else if (a.src) {
+        const skps_det_src F = a.src[blockIdx.z];
+        frame = F.base; H = F.H; W = F.W; pitch = F.pitch; rw = F.rw; rh = F.rh; top = F.top; left = F.left;
+        row_pairs = F.row_pairs;
     }
-    letterbox_px(frame, H, W, pitch, a.out + a.out_stride * blockIdx.z, a.in_h, a.in_w, rw, rh, top, left,
+    letterbox_px(frame, H, W, pitch, row_pairs, a.out + a.out_stride * blockIdx.z, a.in_h, a.in_w, rw, rh, top, left,
                  blockIdx.x * blockDim.x + threadIdx.x, blockIdx.y);
 }
 
@@ -607,6 +612,17 @@ extern "C" SKPS_API int skps_letterbox(const uint8_t* frame, int H, int W, int p
     a.frame = frame; a.H = H; a.W = W; a.pitch = pitch; a.rw = rw; a.rh = rh; a.top = top; a.left = left;
     a.out = out; a.in_h = in_h; a.in_w = in_w;
     return launch_letterbox(a, 1, (cudaStream_t)stream);
+}
+
+extern "C" SKPS_API int skps_letterbox_frames(const skps_det_src* src, int n, uint8_t* out, int in_h, int in_w,
+                                              void* stream) {
+    SKPS_CHECK(n >= 0 && n <= 65535 && in_h > 0 && in_h <= 65535 && in_w > 0,
+               "letterbox_frames: n %d outside 0..65535 or input %dx%d", n, in_h, in_w);
+    if (n == 0) return 0;
+    SKPS_CHECK(src && out, "letterbox_frames: bad arguments");
+    LetterboxArgs a = {};
+    a.src = src; a.out = out; a.out_stride = (size_t)in_h * in_w * 3; a.in_h = in_h; a.in_w = in_w;
+    return launch_letterbox(a, n, (cudaStream_t)stream);
 }
 
 extern "C" SKPS_API int skps_select_faces(const float* det_rows, const int32_t* det_count, int det_stride, const float* track,

@@ -4,6 +4,7 @@
 #include <stdint.h>
 
 struct skps_pipeline_cfg;
+struct skps_det_src;
 
 namespace skps {
 
@@ -53,9 +54,10 @@ struct MpStreamDesc {
 
 // Letterbox (face_detector.py:45-71) of frame g into out + g * out_stride, in_h x in_w x 3 RGB.
 struct LetterboxArgs {
-    const uint8_t* frame; int H, W, pitch;      // the one frame (desc null) ...
+    const uint8_t* frame; int H, W, pitch;      // the one frame (desc and src null) ...
     int rw, rh, top, left;                      // ... and its letterbox geometry
     const MpStreamDesc* desc;                   // or frame g's: desc[g], geometry included
+    const skps_det_src* src;                    // or frame g's: src[g] (skps_letterbox_frames), whole or in row pairs
     uint8_t* out; size_t out_stride;
     int in_h, in_w;
 };

@@ -76,6 +76,7 @@ SIGNATURES = {
                                       C.c_int, C.c_int, c_vp]),
     "skps_letterbox": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, C.c_int, C.c_int,
                                  C.c_int, C.c_int, C.c_int, C.c_int, c_vp]),
+    "skps_letterbox_frames": (C.c_int, [c_vp, C.c_int, c_vp, C.c_int, C.c_int, c_vp]),
     "skps_detect_post": (C.c_int, [c_vp, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
                                    c_vp, c_vp, c_vp, C.c_int, c_vp]),
     "skps_detect_post_workspace_size": (C.c_size_t, [C.c_int, C.c_int]),
