@@ -245,6 +245,23 @@ SKPS_API int skps_select_faces(const float* det_rows, const int32_t* det_count, 
                       float min_face, int top_k,
                       float* boxes4, int32_t* count, void* stream);
 
+/* skps_select_faces with no track boxes (FaceAna.run on a new or just-reset FaceAna) for n images (>= 0) at once, one
+ * block per image: image i selects from its det_count[i] [dev] rows of 16 floats at det_rows [dev] + i*det_cap*16 (the
+ * kept_rows / count layout of skps_detect_post_batch with capacity det_cap) and writes its count[i] [dev] boxes to
+ * boxes4 [dev] + i*top_k*4.  Same rule and same bytes as skps_select_faces on each image alone. */
+SKPS_API int skps_select_faces_batch(const float* det_rows, const int32_t* det_count, int det_cap, int n, float min_face,
+                                     int top_k, float* boxes4, int32_t* count, void* stream);
+
+/* The box FaceAna.run returns for a face on a frame with no history (facer.py:75-82, judge_boxs(boxes, rects(kps))),
+ * for n_faces (>= 0) faces of many images: face f has landmarks kps [dev] (n_faces,n_points,2) float32 and belongs to
+ * image face_image[f] [dev] int32, whose selected boxes are sel_boxes [dev] (images,top_k,4), sel_count [dev] of them.
+ * boxes_out[f] [dev] (n_faces,4) float32 is the landmarks' rectangle [min x, min y, max x, max y], or, when the first
+ * selected box of its image whose IoU with that rectangle is above iou_thres exists, alpha*rect + one_minus_alpha*box
+ * in float32 (rounded like numpy's float32 expression).  One warp per face. */
+SKPS_API int skps_landmark_boxes(const float* kps, int n_points, const int32_t* face_image, int n_faces,
+                                 const float* sel_boxes, const int32_t* sel_count, int top_k, float iou_thres, float alpha,
+                                 float one_minus_alpha, float* boxes_out, void* stream);
+
 /* FaceLandmark.preprocess (face_landmark.py:66-104) for all faces at once: zero-pad, square
  * crop, cv2.resize to (out_hw,out_hw), uint8 BGR NHWC.  `boxes4` [dev] (max_faces,4), `count`
  * [dev].  `detail` [dev] (max_faces,5) int32 = [h,w,y1,x1,add].  Faces >= *count are zeroed. */
@@ -513,6 +530,12 @@ SKPS_API int skps_mpipe_align_results(skps_mpipe* p, int slot, uint8_t* chips, d
  * is ordered on `stream`, and the call returns once that stream has reached it.  Synchronous. */
 SKPS_API int skps_pipeline_pose(skps_pipeline* p, const double* kps, int n, int H, int W, double* rvec, double* tvec,
                                 double* euler, double* reproject, void* stream);
+/* FaceAnaImages, whose faces come from many images: kps [dev] (n_faces,n_points,2) float32 (n_points >= 98), hw [dev]
+ * (n_faces,2) int32 the H, W of each face's own image; rvec, tvec, euler [dev] (n_faces,3), reproject [dev]
+ * (n_faces,8,2).  The same results as skps_pipeline_pose on the same landmarks promoted to float64.  Asynchronous on
+ * `stream`; allocates nothing. */
+SKPS_API int skps_head_pose_faces(const float* kps, int n_faces, int n_points, const int32_t* hw, double* rvec,
+                                  double* tvec, double* euler, double* reproject, void* stream);
 /* FaceAnaStreams: on != 0 makes every following skps_mpipe_submit solve the pose of every returned face from the smoothed
  * float64 landmarks, with each stream's own frame size, on the compute stream without a host synchronisation; the results
  * are copied back with the slot's other results.  on = 0 switches it off and frees the buffers (n_streams x top_k x 200

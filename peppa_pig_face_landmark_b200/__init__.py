@@ -13,6 +13,9 @@ def __getattr__(name):
     if name == "FaceAna":
         from .core.api.facer import FaceAna
         return FaceAna
+    if name == "FaceAnaImages":
+        from .core.api.images import FaceAnaImages
+        return FaceAnaImages
     if name == "FaceAnaStreams":
         from .core.api.streams import FaceAnaStreams
         return FaceAnaStreams
@@ -28,4 +31,4 @@ def __getattr__(name):
     raise AttributeError(name)
 
 
-__all__ = ["FaceAna", "FaceAnaStreams", "FaceDetector", "FaceLandmark", "ONNXEngine"]
+__all__ = ["FaceAna", "FaceAnaImages", "FaceAnaStreams", "FaceDetector", "FaceLandmark", "ONNXEngine"]

@@ -235,11 +235,13 @@ class FaceDetector:
             layout.append((H, W, pitch, geo, None if cuda else host_upload_rows(H, geo[2])))
         return frames, layout, cuda
 
-    def _enqueue(self, frames, out, detect):
+    def _enqueue(self, frames, out, detect, checked=None):
         """Stages the frames into the next slot and enqueues letterbox (and, with detect, network, NMS and the copy back
-        of host results) on the engine's stream; returns the slot."""
+        of host results) on the engine's stream; returns the slot.  out: None, or result buffers of new_results(n) the
+        kept rows go to, for host frames as well as CUDA frames (FaceAnaImages keeps them on the GPU); nothing is then
+        copied back.  checked: what _layout(frames) returned, when the caller has checked the frames already."""
         torch = rt.require_cuda()
-        frames, layout, cuda = self._layout(frames)
+        frames, layout, cuda = self._layout(frames) if checked is None else checked
         n, R, M = len(frames), self._rows, min(self.MAX_DET, self._rows)
         if self._slots is None:
             self._slots = [self._new_slot() for _ in range(2)]

@@ -175,9 +175,27 @@ class FaceLandmark:
         work queued on it after submit() returns runs after they have been read.
         out: None (collect() returns numpy arrays), or, with CUDA frames, a dict from new_results(n) with n >= the call's
         faces, not used by a call still in flight: the results are written there on the GPU."""
-        torch = rt.require_cuda()
         if len(self._pending) == 2:
             raise RuntimeError("FaceLandmark: two calls already in flight; call collect() first")
+        checked = self._check_call(frames, boxes)
+        if out is not None:
+            if not checked[3]:
+                raise ValueError("out= keeps results on the GPU and takes CUDA frames; these are host frames")
+            self._check_out(out, sum(checked[5]))
+        slot = self._enqueue(checked, out)
+        self._pending.append((slot, checked[5], out))
+
+    def _enqueue_to(self, frames, boxes, out):
+        """submit() with results left in out (a new_results(n) dict) for host frames as well as CUDA frames, and not
+        counted as a call in flight: FaceAnaImages orders its own work after it on the engine's stream.  Returns the
+        faces per frame."""
+        checked = self._check_call(frames, boxes)
+        self._check_out(out, sum(checked[5]))
+        self._enqueue(checked, out)
+        return checked[5]
+
+    def _check_call(self, frames, boxes):
+        """Checks the frames and boxes of a call: (frames, boxes, layout, cuda frames, cuda boxes, faces per frame)."""
         frames, boxes = list(frames), list(boxes)
         if len(frames) != len(boxes):
             raise ValueError("%d frames but %d box arrays" % (len(frames), len(boxes)))
@@ -203,13 +221,15 @@ class FaceLandmark:
             raise ValueError("CUDA boxes take CUDA frames: the host frames' upload is cut to the boxes on the host")
         boxes = [self._check_cuda_boxes(b, i) if cuda_boxes else self._check_host_boxes(b, i) for i, b in enumerate(boxes)]
         counts = [int(b.shape[0]) for b in boxes]
+        return frames, boxes, layout, cuda, cuda_boxes, counts
+
+    def _enqueue(self, checked, out):
+        """Stages a checked call into the next slot and enqueues crops, network and post-processing (and, without out,
+        the copy back) on the engine's stream; returns the slot."""
+        torch = rt.require_cuda()
+        frames, boxes, layout, cuda, cuda_boxes, counts = checked
         n = sum(counts)
         P = self.keypoints_num
-        if out is not None:
-            if not cuda:
-                raise ValueError("out= keeps results on the GPU and takes CUDA frames; these are host frames")
-            self._check_out(out, n)
-
         if self._slots is None:
             self._slots = [self._new_slot() for _ in range(2)]
         slot = self._next
@@ -292,8 +312,8 @@ class FaceLandmark:
                 st["hkps"][:n].copy_(kps[:n], non_blocking=True)
                 st["hscores"][:n].copy_(scores[:n], non_blocking=True)
         st["done"].record(s)
-        self._pending.append((slot, counts, out))
         self._next ^= 1
+        return slot
 
     def collect(self):
         """Results of the oldest call in flight: a list with one (kps (k_i, 98, 2), scores (k_i, 98)) pair per frame, as

@@ -449,6 +449,20 @@ extern "C" SKPS_API int skps_head_pose(const float* pts, int N, int img_w, int i
     return 0;
 }
 
+// get_head_pose of n faces that may each come from a different frame, on device data (FaceAnaImages).
+extern "C" SKPS_API int skps_head_pose_faces(const float* kps, int n_faces, int n_points, const int32_t* hw, double* rvec,
+                                             double* tvec, double* euler, double* reproject, void* stream) {
+    SKPS_CHECK(n_faces >= 0 && n_points >= 98, "head_pose_faces: %d faces of %d landmarks, expected >= 0 faces of >= 98",
+               n_faces, n_points);
+    if (n_faces == 0) return 0;
+    SKPS_CHECK(kps && hw && rvec && tvec && euler && reproject, "head_pose_faces: null argument");
+    PoseArgs a = {};
+    pose_model_98(a);
+    a.pts32 = kps; a.G = n_faces; a.K = 1; a.P = n_points; a.hw = hw;
+    a.rvec = rvec; a.tvec = tvec; a.euler = euler; a.reproj = reproject;
+    return launch_head_pose(a, (cudaStream_t)stream);
+}
+
 // The solver's rotation helpers on their own, in device code: R_out[i] = rodrigues(r_in[i]); r_out[i] = rodrigues_inv(R_in[i]);
 // euler_out[i] = euler_rq(R_in[i]).  r_in (n,3), R_in (n,3,3) row-major, all [host] float64.
 extern "C" SKPS_API int skps_debug_rotation(const double* r_in, const double* R_in, int n, double* R_out, double* r_out,

@@ -425,6 +425,37 @@ __global__ void __launch_bounds__(256) select_frames_kernel(const SelectArgs a) 
                       a.src ? a.src + (size_t)g * a.top_k : nullptr, !det);
 }
 
+// The box FaceAna returns for a face on a frame with no history (facer.py:75-82): judge_boxs(boxes_return, rects(kps)),
+// i.e. the face's landmark rectangle, EMA-blended with the first selected box of its image it overlaps with IoU >
+// iou_thres.  One warp per face: the rectangle's min / max by shuffles, then judged_box.
+__global__ void __launch_bounds__(256) landmark_boxes_kernel(const float* __restrict__ kps, int P,
+                                                             const int* __restrict__ face_image, int n,
+                                                             const float* __restrict__ sel_boxes,
+                                                             const int* __restrict__ sel_count, int top_k, float iou_thres,
+                                                             float alpha, float oma, float* __restrict__ out) {
+    const int f = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (f >= n) return;                             // whole warps leave together
+    const float* p = kps + (size_t)f * P * 2;
+    float x0 = INFINITY, y0 = INFINITY, x1 = -INFINITY, y1 = -INFINITY;
+    for (int i = lane; i < P; i += 32) {
+        const float x = p[2 * i], y = p[2 * i + 1];
+        x0 = fminf(x0, x); y0 = fminf(y0, y); x1 = fmaxf(x1, x); y1 = fmaxf(y1, y);
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        x0 = fminf(x0, __shfl_xor_sync(0xffffffffu, x0, o));
+        y0 = fminf(y0, __shfl_xor_sync(0xffffffffu, y0, o));
+        x1 = fmaxf(x1, __shfl_xor_sync(0xffffffffu, x1, o));
+        y1 = fmaxf(y1, __shfl_xor_sync(0xffffffffu, y1, o));
+    }
+    if (lane == 0) {
+        const int g = face_image[f];
+        const float rect[4] = {x0, y0, x1, y1};
+        float b[4];
+        judged_box(rect, sel_boxes + (size_t)g * top_k * 4, sel_count[g], iou_thres, alpha, oma, b);
+        for (int c = 0; c < 4; ++c) out[(size_t)f * 4 + c] = b[c];
+    }
+}
+
 // ------------------------------------------------------------------------------------------
 // FaceLandmark.postprocess (face_landmark.py:106-115): float32 product, then + x1 - add in
 // float64, stored as float32 (numpy>=2 promotion of `float32 * int + np.int32 - int`).
@@ -635,6 +666,33 @@ extern "C" SKPS_API int skps_select_faces(const float* det_rows, const int32_t* 
     a.iou_thres = iou_thres; a.alpha = alpha; a.one_minus_alpha = one_minus_alpha; a.min_face = min_face; a.top_k = top_k;
     a.boxes4 = boxes4; a.count = count;
     return launch_select(a, 1, (cudaStream_t)stream);
+}
+
+extern "C" SKPS_API int skps_select_faces_batch(const float* det_rows, const int32_t* det_count, int det_cap, int n,
+                                                float min_face, int top_k, float* boxes4, int32_t* count, void* stream) {
+    SKPS_CHECK(n >= 0 && top_k > 0 && top_k <= SEL_MAX_K && det_cap > 0,
+               "select_faces_batch: n %d < 0, top_k %d outside 1..%d or det_cap %d < 1", n, top_k, SEL_MAX_K, det_cap);
+    if (n == 0) return 0;
+    SKPS_CHECK(det_rows && det_count && boxes4 && count, "select_faces_batch: bad arguments");
+    SelectArgs a = {};
+    a.det_rows = det_rows; a.det_count = det_count; a.det_stride = 16; a.det_cap = det_cap; a.flag1 = 1;
+    a.min_face = min_face; a.top_k = top_k;
+    a.boxes4 = boxes4; a.count = count;
+    return launch_select(a, n, (cudaStream_t)stream);
+}
+
+extern "C" SKPS_API int skps_landmark_boxes(const float* kps, int n_points, const int32_t* face_image, int n_faces,
+                                            const float* sel_boxes, const int32_t* sel_count, int top_k, float iou_thres,
+                                            float alpha, float one_minus_alpha, float* boxes_out, void* stream) {
+    SKPS_CHECK(n_faces >= 0 && n_points > 0 && top_k > 0, "landmark_boxes: n_faces %d, n_points %d or top_k %d out of range",
+               n_faces, n_points, top_k);
+    if (n_faces == 0) return 0;
+    SKPS_CHECK(kps && face_image && sel_boxes && sel_count && boxes_out, "landmark_boxes: bad arguments");
+    const unsigned blocks = (unsigned)(((long long)n_faces + 7) / 8);
+    landmark_boxes_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(kps, n_points, face_image, n_faces, sel_boxes, sel_count,
+                                                                     top_k, iou_thres, alpha, one_minus_alpha, boxes_out);
+    SKPS_CUDA(cudaGetLastError());
+    return 0;
 }
 
 extern "C" SKPS_API int skps_crop_resize(const uint8_t* frame, int H, int W, int pitch, const float* boxes4,

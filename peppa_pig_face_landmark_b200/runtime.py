@@ -84,6 +84,9 @@ SIGNATURES = {
                                          c_vp, C.c_size_t, c_vp]),
     "skps_select_faces": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, C.c_int, C.c_float, C.c_float, C.c_float,
                                     C.c_float, C.c_int, c_vp, c_vp, c_vp]),
+    "skps_select_faces_batch": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_float, C.c_int, c_vp, c_vp, c_vp]),
+    "skps_landmark_boxes": (C.c_int, [c_vp, C.c_int, c_vp, C.c_int, c_vp, c_vp, C.c_int, C.c_float, C.c_float, C.c_float,
+                                      c_vp, c_vp]),
     "skps_crop_resize": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, C.c_int, C.c_float, C.c_float,
                                    c_vp, C.c_int, c_vp, c_vp]),
     "skps_crop_faces": (C.c_int, [c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, C.c_int, c_vp, c_vp]),
@@ -121,6 +124,7 @@ SIGNATURES = {
     "skps_mpipe_set_align": (C.c_int, [c_vp, C.c_int]),
     "skps_mpipe_align_results": (C.c_int, [c_vp, C.c_int, c_vp, c_vp]),
     "skps_pipeline_pose": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "skps_head_pose_faces": (C.c_int, [c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "skps_mpipe_set_pose": (C.c_int, [c_vp, C.c_int]),
     "skps_mpipe_pose_results": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp]),
     "skps_mpipe_set_detect_every": (C.c_int, [c_vp, C.c_int]),
