@@ -76,8 +76,9 @@ def warp_affine(image, M, dsize):
     frame = torch.from_numpy(image).cuda()
     m = torch.from_numpy(np.ascontiguousarray(M)).cuda()
     out = torch.empty((n, h, w, 3), dtype=torch.uint8, device=frame.device)
-    rt.check(lib.skps_warp_affine(frame.data_ptr(), H, W, W * 3, m.data_ptr(), None, n, h, w, out.data_ptr(),
-                                  torch.cuda.current_stream(frame.device).cuda_stream))
+    with torch.cuda.device(frame.device):
+        rt.check(lib.skps_warp_affine(frame.data_ptr(), H, W, W * 3, m.data_ptr(), None, n, h, w, out.data_ptr(),
+                                      torch.cuda.current_stream(frame.device).cuda_stream))
     return out.cpu().numpy()
 
 
@@ -96,6 +97,7 @@ def align_faces(image, kps, size=112):
     dk = torch.from_numpy(k).cuda()
     chips = torch.empty((n, size, size, 3), dtype=torch.uint8, device=frame.device)
     M = torch.empty((n, 2, 3), dtype=torch.float64, device=frame.device)
-    rt.check(lib.skps_align_faces(frame.data_ptr(), H, W, W * 3, dk.data_ptr(), None, n, k.shape[1], size, chips.data_ptr(),
-                                  M.data_ptr(), torch.cuda.current_stream(frame.device).cuda_stream))
+    with torch.cuda.device(frame.device):
+        rt.check(lib.skps_align_faces(frame.data_ptr(), H, W, W * 3, dk.data_ptr(), None, n, k.shape[1], size,
+                                      chips.data_ptr(), M.data_ptr(), torch.cuda.current_stream(frame.device).cuda_stream))
     return chips.cpu().numpy(), M.cpu().numpy()

@@ -303,16 +303,18 @@ class FaceDetector:
         inp = self.model.input_ptr()
         for c0 in range(0, n, K):
             m = min(K, n - c0)
-            rt.check(self.lib.skps_letterbox_frames(dev + DET_SRC.itemsize * c0, m, inp, in_h, in_w, s.cuda_stream))
+            with torch.cuda.device(self.device):      # the kernels launch on the current device
+                rt.check(self.lib.skps_letterbox_frames(dev + DET_SRC.itemsize * c0, m, inp, in_h, in_w, s.cuda_stream))
             if c0 + K >= n:
                 st["read"].record(s)
             if not detect:
                 continue
             rt.check(self.lib.skps_engine_forward(self.model.handle, inp, m, None, s.cuda_stream))
-            rt.check(self.lib.skps_detect_post_batch(self.model.output_ptr(0), R, m, self.score_thrs, self.iou_thrs,
-                                                     dev + rec_off + 12 * c0, rows_t.data_ptr() + 64 * R * c0,
-                                                     idx_t.data_ptr() + 4 * R * c0, count_t.data_ptr() + 4 * c0, R,
-                                                     self._ws.data_ptr(), self._ws_bytes, s.cuda_stream))
+            with torch.cuda.device(self.device):
+                rt.check(self.lib.skps_detect_post_batch(self.model.output_ptr(0), R, m, self.score_thrs, self.iou_thrs,
+                                                         dev + rec_off + 12 * c0, rows_t.data_ptr() + 64 * R * c0,
+                                                         idx_t.data_ptr() + 4 * R * c0, count_t.data_ptr() + 4 * c0, R,
+                                                         self._ws.data_ptr(), self._ws_bytes, s.cuda_stream))
         if n == 0:
             st["read"].record(s)
         torch.cuda.current_stream(self.device).wait_event(st["read"])

@@ -121,10 +121,11 @@ class FaceLandmark:
             self._boxes[:n].copy_(torch.from_numpy(np.ascontiguousarray(bboxes[:, :4])))
             self._count.fill_(n)
         S = self.input_size[0]
-        rt.check(self.lib.skps_crop_resize(frame.data_ptr(), h, w, w * 3, self._boxes.data_ptr(),
-                                           self._count.data_ptr(), self.max_faces, self.face_scale,
-                                           float(self.min_face), self.model.input_ptr(), S,
-                                           self._detail.data_ptr(), s.cuda_stream))
+        with torch.cuda.device(self.device):          # the kernel launches on the current device
+            rt.check(self.lib.skps_crop_resize(frame.data_ptr(), h, w, w * 3, self._boxes.data_ptr(),
+                                               self._count.data_ptr(), self.max_faces, self.face_scale,
+                                               float(self.min_face), self.model.input_ptr(), S,
+                                               self._detail.data_ptr(), s.cuda_stream))
         s.synchronize()
         out = np.empty((self.max_faces, S, S, 3), np.uint8)
         rt.check(self.lib.skps_engine_read_buffer(self.model.handle, self.model.plan.input.buf.idx, self.max_faces,
@@ -296,14 +297,17 @@ class FaceLandmark:
         det = st["detail"].data_ptr()
         for c0 in range(0, n, K):
             m = min(K, n - c0)
-            rt.check(self.lib.skps_crop_faces(dev + FACE_SRC.itemsize * c0, dev + box_off + 16 * c0, m, self.face_scale,
-                                              float(self.min_face), inp, S, det + 20 * c0, s.cuda_stream))
+            with torch.cuda.device(self.device):      # the kernels launch on the current device
+                rt.check(self.lib.skps_crop_faces(dev + FACE_SRC.itemsize * c0, dev + box_off + 16 * c0, m,
+                                                  self.face_scale, float(self.min_face), inp, S, det + 20 * c0,
+                                                  s.cuda_stream))
             if c0 + K >= n:
                 st["read"].record(s)
             outs = (C.c_void_p * 2)(None, scores.data_ptr() + 4 * P * c0)
             rt.check(self.lib.skps_engine_forward(self.model.handle, inp, m, outs, s.cuda_stream))
-            rt.check(self.lib.skps_landmark_post(self.model.output_ptr(0), det + 20 * c0, st["count"].data_ptr(), m, P,
-                                                 kps.data_ptr() + 8 * P * c0, s.cuda_stream))
+            with torch.cuda.device(self.device):
+                rt.check(self.lib.skps_landmark_post(self.model.output_ptr(0), det + 20 * c0, st["count"].data_ptr(), m,
+                                                     P, kps.data_ptr() + 8 * P * c0, s.cuda_stream))
         if n == 0:
             st["read"].record(s)
         torch.cuda.current_stream(self.device).wait_event(st["read"])

@@ -176,8 +176,10 @@ class FaceAnaImages:
         fd._enqueue(frames, st["det"], detect=True, checked=checked)
         # 2. face selection, all images in one launch; 3. the call's one read-back: counts and selected boxes
         sel = st["sel"]
-        rt.check(lib.skps_select_faces_batch(st["det"]["rows"].data_ptr(), st["det"]["count"].data_ptr(), fd._rows, n,
-                                             self.min_face, K, sel.data_ptr() + 4 * cpad, sel.data_ptr(), ds.cuda_stream))
+        with torch.cuda.device(self.device):          # the kernels launch on the current device
+            rt.check(lib.skps_select_faces_batch(st["det"]["rows"].data_ptr(), st["det"]["count"].data_ptr(), fd._rows,
+                                                 n, self.min_face, K, sel.data_ptr() + 4 * cpad, sel.data_ptr(),
+                                                 ds.cuda_stream))
         with torch.cuda.stream(ds):
             st["hsel"][:need].copy_(sel[:need], non_blocking=True)
         st["selected"].record(ds)
@@ -216,13 +218,14 @@ class FaceAnaImages:
                 out["count"][:n].copy_(dmap[n:2 * n])
         # 5. the returned box; 6. head pose
         face_ptr, hw_ptr = dmap.data_ptr() + 4 * 2 * n, dmap.data_ptr() + 4 * (2 * n + F)
-        rt.check(lib.skps_landmark_boxes(res["kps"].data_ptr(), P, face_ptr, F, sel.data_ptr() + 4 * cpad, sel.data_ptr(),
-                                         K, self.iou_thres, self.alpha, self.one_minus_alpha, res["box"].data_ptr(),
-                                         ls.cuda_stream))
-        if self.pose:
-            rt.check(lib.skps_head_pose_faces(res["kps"].data_ptr(), F, P, hw_ptr, res["rvec"].data_ptr(),
-                                              res["tvec"].data_ptr(), res["euler"].data_ptr(),
-                                              res["reproject"].data_ptr(), ls.cuda_stream))
+        with torch.cuda.device(self.device):
+            rt.check(lib.skps_landmark_boxes(res["kps"].data_ptr(), P, face_ptr, F, sel.data_ptr() + 4 * cpad,
+                                             sel.data_ptr(), K, self.iou_thres, self.alpha, self.one_minus_alpha,
+                                             res["box"].data_ptr(), ls.cuda_stream))
+            if self.pose:
+                rt.check(lib.skps_head_pose_faces(res["kps"].data_ptr(), F, P, hw_ptr, res["rvec"].data_ptr(),
+                                                  res["tvec"].data_ptr(), res["euler"].data_ptr(),
+                                                  res["reproject"].data_ptr(), ls.cuda_stream))
         # 7. results: back to pinned host memory, or left in out
         if out is None and F:
             with torch.cuda.stream(ls):

@@ -102,6 +102,58 @@ const char* get_error();
         }                                     \
     } while (0)
 
+// ---- per-device state: kernel attributes and allocations apply to the device current when they were made ----
+constexpr int MAX_DEVICES = 64;
+
+// Raises a kernel's dynamic shared-memory limit on the current device to `bytes` where it is lower.  set_bytes: the
+// kernel's limit per device so far, MAX_DEVICES entries kept by the caller (one static array per kernel).
+inline int smem_limit(const void* kernel, int* set_bytes, int bytes) {
+    int dev = 0;
+    SKPS_CUDA(cudaGetDevice(&dev));
+    SKPS_CHECK(dev >= 0 && dev < MAX_DEVICES, "device %d out of range", dev);
+    if (bytes > set_bytes[dev]) {
+        SKPS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        set_bytes[dev] = bytes;
+    }
+    return 0;
+}
+
+// 1024 zeros on the current device, standing in for a missing bias; one allocation per device, null on failure
+inline const float* zero_bias() {
+    static float* z[MAX_DEVICES] = {};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= MAX_DEVICES) return nullptr;
+    if (!z[dev]) {
+        if (cudaMalloc(&z[dev], 1024 * sizeof(float)) != cudaSuccess) { z[dev] = nullptr; return nullptr; }
+        if (cudaMemset(z[dev], 0, 1024 * sizeof(float)) != cudaSuccess) return nullptr;
+    }
+    return z[dev];
+}
+
+// Makes `dev` the calling thread's current device for the guard's life and gives the caller back its own current device
+// on every return path.  Every entry point on a handle opens one (SKPS_ON_DEVICE), so a call launches only on the
+// handle's device whatever device is current, and leaves the current device as it found it.
+class DeviceGuard {
+public:
+    explicit DeviceGuard(int dev) : dev_(dev) {
+        if (cudaGetDevice(&prev_) != cudaSuccess) prev_ = -1;
+        err_ = prev_ == dev ? cudaSuccess : cudaSetDevice(dev);
+    }
+    ~DeviceGuard() {
+        if (prev_ >= 0 && prev_ != dev_) cudaSetDevice(prev_);
+    }
+    DeviceGuard(const DeviceGuard&) = delete;
+    DeviceGuard& operator=(const DeviceGuard&) = delete;
+    cudaError_t status() const { return err_; }
+
+private:
+    int dev_, prev_ = -1;
+    cudaError_t err_;
+};
+#define SKPS_ON_DEVICE(dev)                         \
+    skps::DeviceGuard skps_device_guard_(dev);      \
+    SKPS_CUDA(skps_device_guard_.status())
+
 // The fail-and-destroy lambdas of the *_create functions report a failed step as "<fn>: <what>: <error set by the step>".
 inline void prefix_error(const char* fn, const char* what) {
     char tmp[900];

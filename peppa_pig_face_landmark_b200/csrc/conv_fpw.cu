@@ -321,7 +321,7 @@ int fpw_prepare(FpwLayer& L, const XfSetup& s) {
     SKPS_CHECK(smem, "conv_fpw: layer does not fit shared memory");
     L.smem_bytes = (int)smem + 1024;
     k.Cout = s.Cout; k.out_scale = s.out_scale;
-    k.bias = s.bias ? s.bias : xf_zero_bias();
+    k.bias = s.bias ? s.bias : zero_bias();
     SKPS_CHECK(k.bias, "conv_fpw: zero-bias allocation failed");
     k.res = s.res.base; k.res_fmt = s.res.fmt; k.res_plane = s.res.plane; k.res_ld = s.res.ld; k.res_coff = s.res.c_off;
     k.res_first = s.res.base ? s.res_first : 0;
@@ -330,8 +330,8 @@ int fpw_prepare(FpwLayer& L, const XfSetup& s) {
 
 template <int MODE, int N, int ACT, bool SPLIT>
 static int fpw_launch_t(const FpwLayer& L, const FpwK& k, int grid, cudaStream_t stream) {
-    static int attr_bytes[XF_MAX_DEVICES] = {};
-    if (xf_smem_limit((const void*)conv_fpw_kernel<MODE, N, ACT, SPLIT>, attr_bytes, L.smem_bytes)) return 1;
+    static int attr_bytes[MAX_DEVICES] = {};
+    if (smem_limit((const void*)conv_fpw_kernel<MODE, N, ACT, SPLIT>, attr_bytes, L.smem_bytes)) return 1;
     conv_fpw_kernel<MODE, N, ACT, SPLIT><<<grid, XF_THREADS, L.smem_bytes, stream>>>(
         L.src0, L.src1_hi, L.src1_lo, L.b_hi, L.b_lo, L.o_hi, L.o_lo, L.w_eff, k);
     SKPS_CUDA(cudaGetLastError());

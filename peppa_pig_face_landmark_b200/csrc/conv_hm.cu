@@ -242,11 +242,8 @@ Grid hm_grid(const HmLayer& L, int batch, int num_sms, HmK* kp) {
 }
 
 int hm_launch(const HmLayer& L, int batch, int num_sms, cudaStream_t stream) {
-    static int attr_bytes = 0;
-    if (L.smem_bytes > attr_bytes) {
-        SKPS_CUDA(cudaFuncSetAttribute(conv_hm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
-        attr_bytes = L.smem_bytes;
-    }
+    static int attr_bytes[MAX_DEVICES] = {};
+    if (smem_limit((const void*)conv_hm_kernel, attr_bytes, L.smem_bytes)) return 1;
     HmK k;
     const int grid = hm_grid(L, batch, num_sms, &k).ctas;
     conv_hm_kernel<<<grid, HM_THREADS, L.smem_bytes, stream>>>(L.x_hi, L.x_lo, L.w_hi, L.w_lo, k);

@@ -235,19 +235,21 @@ conv_mma_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant
 }
 
 // ------------------------------------------------------------------------------------------ host side
-// Shared-memory limit of the instantiation and its resident CTAs per SM
+// Shared-memory limit of the instantiation and its resident CTAs per SM, on the current device
 template <int CIN, int COUT>
 static int mma_setup_t(int* ctas_per_sm) {
-    static bool attr_set = false;
-    static int ctas = 1;
+    static int attr_bytes[MAX_DEVICES] = {};
+    static int ctas[MAX_DEVICES] = {};
     constexpr int smem = MmaCfg<CIN, COUT>::SMEM;
-    if (!attr_set) {
-        SKPS_CUDA(cudaFuncSetAttribute(conv_mma_kernel<CIN, COUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        SKPS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, conv_mma_kernel<CIN, COUT>, MMA_THREADS, smem));
-        if (ctas < 1) ctas = 1;
-        attr_set = true;
+    if (smem_limit((const void*)conv_mma_kernel<CIN, COUT>, attr_bytes, smem)) return 1;
+    int dev = 0;
+    SKPS_CUDA(cudaGetDevice(&dev));
+    if (!ctas[dev]) {
+        int n = 0;
+        SKPS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, conv_mma_kernel<CIN, COUT>, MMA_THREADS, smem));
+        ctas[dev] = n < 1 ? 1 : n;
     }
-    *ctas_per_sm = ctas;
+    *ctas_per_sm = ctas[dev];
     return 0;
 }
 

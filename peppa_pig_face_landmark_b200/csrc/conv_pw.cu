@@ -293,12 +293,8 @@ int pw_prepare(PwLayer& L, const TcSetup& s) {
 template <int NC, int ACT, bool SPLIT>
 static int pw_launch_t(const PwLayer& L, const PwK& k, const CUtensorMap& o_hi, const CUtensorMap& o_lo, int grid,
                        cudaStream_t stream) {
-    static int attr_bytes = 0;
-    if (L.smem_bytes > attr_bytes) {
-        SKPS_CUDA(cudaFuncSetAttribute(conv_pw_kernel<NC, ACT, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       L.smem_bytes));
-        attr_bytes = L.smem_bytes;
-    }
+    static int attr_bytes[MAX_DEVICES] = {};
+    if (smem_limit((const void*)conv_pw_kernel<NC, ACT, SPLIT>, attr_bytes, L.smem_bytes)) return 1;
     conv_pw_kernel<NC, ACT, SPLIT><<<grid, PW_THREADS, L.smem_bytes, stream>>>(L.a_hi, L.a_lo, L.b_hi, L.b_lo, o_hi, o_lo, k);
     SKPS_CUDA(cudaGetLastError());
     return 0;

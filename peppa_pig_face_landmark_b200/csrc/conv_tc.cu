@@ -403,15 +403,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
 }
 
 // ------------------------------------------------------------------------------------------ host side
-static const float* zero_bias() {
-    static float* z = nullptr;       // 1024 zeros for bias-free layers (ASPP), per process/device
-    if (!z) {
-        if (cudaMalloc(&z, 1024 * sizeof(float)) != cudaSuccess) return nullptr;
-        cudaMemset(z, 0, 1024 * sizeof(float));
-    }
-    return z;
-}
-
 // Tile width for an Ho x Wo OUTPUT map (0 = no tiling): 128-pixel tiles are bw x (128/bw) blocks of one image.
 // Maps whose width divides (or is a multiple of) 128 use row-block tiles (bw = min(W, 128)) that cover the map exactly.
 // Any other map (the detector's 48x80 / 24x40 / 12x20, re-targeted @192/@320 exports) gets the bw in {64,32,16,8} with the
@@ -563,12 +554,8 @@ int tc_prepare(TcLayer& L, const TcSetup& s) {
 
 template <int ACT, bool SPLIT>
 static int tc_launch_t(const TcLayer& L, const TcK& k, int grid, cudaStream_t stream) {
-    static bool attr_set = false;
-    if (!attr_set) {
-        SKPS_CUDA(cudaFuncSetAttribute(conv_tc_kernel<ACT, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       227 * 1024 - 1024));
-        attr_set = true;
-    }
+    static int attr_bytes[MAX_DEVICES] = {};
+    if (smem_limit((const void*)conv_tc_kernel<ACT, SPLIT>, attr_bytes, 227 * 1024 - 1024)) return 1;
     conv_tc_kernel<ACT, SPLIT><<<grid, TC_THREADS, L.smem_bytes, stream>>>(L.a_hi, L.a_lo, L.b_hi, L.b_lo, L.o_hi, L.o_lo, k);
     SKPS_CUDA(cudaGetLastError());
     return 0;

@@ -317,11 +317,8 @@ int tct_prepare(TctLayer& L, const TcSetup& s) {
 
 template <int ACT>
 static int tct_launch_t(const TctLayer& L, const TctK& k, int grid, cudaStream_t stream) {
-    static int attr_bytes = 0;
-    if (L.smem_bytes > attr_bytes) {
-        SKPS_CUDA(cudaFuncSetAttribute(conv_tct_kernel<ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, L.smem_bytes));
-        attr_bytes = L.smem_bytes;
-    }
+    static int attr_bytes[MAX_DEVICES] = {};
+    if (smem_limit((const void*)conv_tct_kernel<ACT>, attr_bytes, L.smem_bytes)) return 1;
     conv_tct_kernel<ACT><<<grid, TCT_THREADS, L.smem_bytes, stream>>>(L.x_hi, L.x_lo, L.w_hi, L.w_lo, L.o_hi, L.o_lo, k);
     SKPS_CUDA(cudaGetLastError());
     return 0;

@@ -250,28 +250,6 @@ conv_xf_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
 }
 
 // ------------------------------------------------------------------------------------------ host side
-const float* xf_zero_bias() {
-    static float* z[XF_MAX_DEVICES] = {};
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= XF_MAX_DEVICES) return nullptr;
-    if (!z[dev]) {
-        if (cudaMalloc(&z[dev], 1024 * sizeof(float)) != cudaSuccess) { z[dev] = nullptr; return nullptr; }
-        if (cudaMemset(z[dev], 0, 1024 * sizeof(float)) != cudaSuccess) return nullptr;
-    }
-    return z[dev];
-}
-
-int xf_smem_limit(const void* kernel, int* set_bytes, int bytes) {
-    int dev = 0;
-    SKPS_CUDA(cudaGetDevice(&dev));
-    SKPS_CHECK(dev >= 0 && dev < XF_MAX_DEVICES, "device %d out of range", dev);
-    if (bytes > set_bytes[dev]) {
-        SKPS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-        set_bytes[dev] = bytes;
-    }
-    return 0;
-}
-
 size_t xf_rings(XfProducer& k, int mode, size_t b_slot, size_t reserve, bool two_out_bufs, int& bs, int& out_bufs) {
     const size_t budget = 227 * 1024 - 1024 - 512 - reserve;
     const size_t w_bytes = mode == XF_DW ? (size_t)10 * k.cchunks * 64 * 4 : 0;
@@ -439,7 +417,7 @@ int xf_prepare(XfLayer& L, const XfSetup& s) {
     SKPS_CHECK(smem, "conv_xf: layer does not fit shared memory");
     L.smem_bytes = (int)(smem + XF_XS_BYTES + 1024);
     k.Cout = s.Cout; k.act = s.act; k.out_scale = s.out_scale;
-    k.bias = s.bias ? s.bias : xf_zero_bias();
+    k.bias = s.bias ? s.bias : zero_bias();
     SKPS_CHECK(k.bias, "conv_xf: zero-bias allocation failed");
     k.out = out.base; k.out_fmt = out.fmt; k.out_plane = out.plane; k.out_ld = out.ld; k.out_coff = out.c_off;
     k.out_cstride = out.c_stride;
@@ -450,8 +428,8 @@ int xf_prepare(XfLayer& L, const XfSetup& s) {
 
 template <int MODE, int ACT, bool SPLIT>
 static int xf_launch_t(const XfLayer& L, const XfK& k, int grid, cudaStream_t stream) {
-    static int attr_bytes[XF_MAX_DEVICES] = {};
-    if (xf_smem_limit((const void*)conv_xf_kernel<MODE, ACT, SPLIT>, attr_bytes, L.smem_bytes)) return 1;
+    static int attr_bytes[MAX_DEVICES] = {};
+    if (smem_limit((const void*)conv_xf_kernel<MODE, ACT, SPLIT>, attr_bytes, L.smem_bytes)) return 1;
     conv_xf_kernel<MODE, ACT, SPLIT><<<grid, XF_THREADS, L.smem_bytes, stream>>>(L.src0, L.src1_hi, L.src1_lo, L.b_hi, L.b_lo,
                                                                                   L.o_hi, L.o_lo, L.w_eff, k);
     SKPS_CUDA(cudaGetLastError());

@@ -373,11 +373,8 @@ int dw_tma_prepare(DwTmaLayer& L, const TView& in, const TView& out, const float
 template <int K, int S, int D, bool SPLIT>
 static int launch_variant(const DwTmaLayer& L, const DwTmaK& k, dim3 grid, cudaStream_t stream) {
     constexpr int RY = (K == 5 && S == 1) ? 2 : 1;      // dw_tile_rows(K, S) / TH
-    static bool attr_set = false;
-    if (!attr_set) {
-        SKPS_CUDA(cudaFuncSetAttribute(dw_tma_kernel<K, S, D, SPLIT, RY>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        attr_set = true;
-    }
+    static int attr_bytes[MAX_DEVICES] = {};
+    if (smem_limit((const void*)dw_tma_kernel<K, S, D, SPLIT, RY>, attr_bytes, 200 * 1024)) return 1;
     dw_tma_kernel<K, S, D, SPLIT, RY><<<grid, DW_THREADS, L.smem_bytes, stream>>>(L.hi, L.lo, k);
     SKPS_CUDA(cudaGetLastError());
     return 0;

@@ -21,6 +21,7 @@
 #include "conv_fpw.h"
 #include "conv_xf.h"
 #include "dw_tma.h"
+#include "mpipe_kernels.h"
 #include "stem_block.h"
 
 namespace skps {
@@ -354,6 +355,13 @@ static const char* prepare_op(skps_engine* e, int i) {
     return nullptr;
 }
 
+int skps::engine_pair_device(const skps_engine* det, const skps_engine* kps, const char* fn, int* device) {
+    SKPS_CHECK(det->device == kps->device, "%s: the detector engine is on device %d and the landmark engine on device %d; "
+               "a pipeline's engines must share one device", fn, det->device, kps->device);
+    *device = det->device;
+    return 0;
+}
+
 extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words, const float* weights, size_t n_floats,
                                   int max_batch, int device, skps_engine** out) {
     SKPS_CHECK(words && weights && out && n_words >= 8 && max_batch > 0, "engine_create: bad arguments");
@@ -361,7 +369,7 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
     int n_bufs = words[2], n_ops = words[3];
     const size_t body = (size_t)8 + 4 * (size_t)n_bufs + OP_WORDS * (size_t)n_ops;
     SKPS_CHECK(n_words == body, "engine_create: plan size mismatch");
-    SKPS_CUDA(cudaSetDevice(device));
+    SKPS_ON_DEVICE(device);
     skps_engine* e = new skps_engine();
     e->device = device;
     e->max_batch = max_batch;
@@ -420,7 +428,7 @@ extern "C" SKPS_API int skps_engine_create(const int32_t* words, size_t n_words,
 
 extern "C" SKPS_API void skps_engine_destroy(skps_engine* e) {
     if (!e) return;
-    cudaSetDevice(e->device);
+    DeviceGuard on(e->device);
     for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);
     for (void* p : e->dbuf) if (p) cudaFree(p);
     for (int i = 0; i < 2; ++i) {
@@ -467,7 +475,7 @@ extern "C" SKPS_API int skps_engine_buffer_dims(const skps_engine* e, int buf, i
 }
 extern "C" SKPS_API int skps_engine_read_buffer(skps_engine* e, int buf, int batch, void* dst) {
     SKPS_CHECK(e && buf >= 0 && buf < (int)e->bufs.size() && batch <= e->max_batch, "read_buffer: bad arguments");
-    SKPS_CUDA(cudaSetDevice(e->device));
+    SKPS_ON_DEVICE(e->device);
     SKPS_CUDA(cudaDeviceSynchronize());
     const BufDesc& b = e->bufs[buf];
     if (b.dtype == DT_SPLIT16) {
@@ -495,7 +503,7 @@ extern "C" SKPS_API int skps_engine_launches_for_batch(const skps_engine* e, int
 extern "C" SKPS_API int skps_engine_run_op(skps_engine* e, int op_index, int batch, void* stream) {
     SKPS_CHECK(e && op_index >= 0 && op_index < (int)e->ops.size(), "run_op: bad op index");
     SKPS_CHECK(batch > 0 && batch <= e->max_batch, "run_op: batch %d outside 1..%d", batch, e->max_batch);
-    SKPS_CUDA(cudaSetDevice(e->device));
+    SKPS_ON_DEVICE(e->device);
     return run_ops(e, batch, (cudaStream_t)stream, op_index, op_index + 1);
 }
 
@@ -535,7 +543,7 @@ extern "C" SKPS_API int skps_engine_op_kernel(const skps_engine* e, int op_index
 extern "C" SKPS_API int skps_engine_set_num_sms(skps_engine* e, int n) {
     SKPS_CHECK(e, "set_num_sms: null engine");
     SKPS_CHECK(n >= 0 && n <= e->device_sms, "set_num_sms: %d outside 0..%d", n, e->device_sms);
-    SKPS_CUDA(cudaSetDevice(e->device));
+    SKPS_ON_DEVICE(e->device);
     // a captured forward keeps the grids it was captured with
     for (auto& kv : e->graphs) cudaGraphExecDestroy(kv.second);
     e->graphs.clear();
@@ -604,7 +612,7 @@ extern "C" SKPS_API int skps_engine_forward(skps_engine* e, const uint8_t* input
     SKPS_CHECK(e && input, "forward: null argument");
     SKPS_CHECK(batch > 0 && batch <= e->max_batch, "forward: batch %d outside 1..%d", batch, e->max_batch);
     cudaStream_t s = (cudaStream_t)stream;
-    SKPS_CUDA(cudaSetDevice(e->device));
+    SKPS_ON_DEVICE(e->device);
     const BufDesc& ib = e->bufs[e->input_buf];
     SKPS_CHECK(ib.dtype == DT_U8, "forward: engine input is not uint8");
     if ((const void*)input != e->dbuf[e->input_buf])
@@ -632,7 +640,7 @@ extern "C" SKPS_API int skps_engine_forward_host_u8(skps_engine* e, const uint8_
     SKPS_CHECK(e && input, "forward_host_u8: null argument");
     SKPS_CHECK(batch > 0 && batch <= e->max_batch, "forward: batch %d outside 1..%d", batch, e->max_batch);
     cudaStream_t s = (cudaStream_t)stream;
-    SKPS_CUDA(cudaSetDevice(e->device));
+    SKPS_ON_DEVICE(e->device);
     const BufDesc& ib = e->bufs[e->input_buf];
     SKPS_CUDA(cudaMemcpyAsync(e->dbuf[e->input_buf], input, buf_bytes(ib) * batch, cudaMemcpyHostToDevice, s));
     if (enqueue(e, batch, s)) return 1;
@@ -646,7 +654,7 @@ extern "C" SKPS_API int skps_engine_forward_host_f32(skps_engine* e, const float
     SKPS_CHECK(e && input, "forward_host_f32: null argument");
     SKPS_CHECK(batch > 0 && batch <= e->max_batch, "forward: batch %d outside 1..%d", batch, e->max_batch);
     cudaStream_t s = (cudaStream_t)stream;
-    SKPS_CUDA(cudaSetDevice(e->device));
+    SKPS_ON_DEVICE(e->device);
     const BufDesc& ib = e->bufs[e->input_buf];
     long long total = (long long)buf_elems(ib) * batch;
     SKPS_CUDA(cudaMemcpyAsync(e->d_stage_f32, input, total * sizeof(float), cudaMemcpyHostToDevice, s));
@@ -684,7 +692,7 @@ extern "C" SKPS_API int skps_engine_submit_host_u8(skps_engine* e, int slot, con
                                                    float* const* outputs) {
     SKPS_CHECK(e && input && (slot == 0 || slot == 1), "submit: bad arguments");
     SKPS_CHECK(batch > 0 && batch <= e->max_batch, "submit: batch %d outside 1..%d", batch, e->max_batch);
-    SKPS_CUDA(cudaSetDevice(e->device));
+    SKPS_ON_DEVICE(e->device);
     if (ensure_streaming(e)) return 1;
     const BufDesc& ib = e->bufs[e->input_buf];
     const size_t in_bytes = buf_bytes(ib) * (size_t)batch;
@@ -703,7 +711,7 @@ extern "C" SKPS_API int skps_engine_submit_host_u8(skps_engine* e, int slot, con
 
 extern "C" SKPS_API int skps_engine_wait(skps_engine* e, int slot) {
     SKPS_CHECK(e && (slot == 0 || slot == 1) && e->s_copy, "wait: nothing submitted");
-    SKPS_CUDA(cudaSetDevice(e->device));
+    SKPS_ON_DEVICE(e->device);
     SKPS_CUDA(cudaEventSynchronize(e->ev_done[slot]));
     return 0;
 }

@@ -104,7 +104,7 @@ void skps::mp_temporal_constants(const skps_pipeline_cfg& c, MpTemporalArgs& a) 
 
 extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
     if (!p) return;
-    cudaSetDevice(p->device);
+    DeviceGuard on(p->device);
     if (p->s_compute) cudaStreamSynchronize(p->s_compute);
     if (p->s_copy) cudaStreamSynchronize(p->s_copy);
     for (uint8_t* f : p->d_frame) if (f) cudaFree(f);
@@ -130,7 +130,7 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
 
 extern "C" SKPS_API int skps_mpipe_reset(skps_mpipe* p, int stream) {
     SKPS_CHECK(p && stream >= -1 && stream < p->S, "mpipe_reset: bad stream %d", stream);
-    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_ON_DEVICE(p->device);
     SKPS_CUDA(cudaStreamSynchronize(p->s_compute));
     const int a = stream < 0 ? 0 : stream, b = stream < 0 ? p->S : stream + 1;
     for (int s = a; s < b; ++s) {
@@ -152,6 +152,9 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
                                           skps_mpipe** out) {
     SKPS_CHECK(det && kps && cfg && out && n_streams > 0 && n_streams <= 256, "mpipe_create: bad arguments");
     SKPS_CHECK(cfg->top_k > 0 && cfg->top_k <= 64, "mpipe_create: top_k %d outside 1..64", cfg->top_k);
+    int device = 0;
+    if (engine_pair_device(det, kps, "mpipe_create", &device)) return 1;
+    SKPS_ON_DEVICE(device);
     skps_mpipe* p = new skps_mpipe();
     p->det = det; p->kps = kps; p->cfg = *cfg; p->S = n_streams; p->K = cfg->top_k;
     int c = 0, kh = 0, kw = 0;
@@ -160,7 +163,7 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
     p->kps_hw = kh;
     p->det_rows = skps_engine_output_elems(det, 0) / 16;
     p->P = skps_engine_output_elems(kps, 1);
-    cudaGetDevice(&p->device);
+    p->device = device;
     auto fail = [&](const char* what) {
         prefix_error("mpipe_create", what);
         skps_mpipe_destroy(p);
@@ -228,7 +231,7 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     SKPS_CHECK(!out || !p->align_size || (out->chips && out->M), "mpipe_submit: alignment is on; device outputs need chips and M");
     SKPS_CHECK(!out || !p->pose_on || (out->rvec && out->tvec && out->euler && out->reproject),
                "mpipe_submit: pose is on; device outputs need rvec, tvec, euler and reproject");
-    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_ON_DEVICE(p->device);
     const skps_pipeline_cfg& c = p->cfg;
     const int S = p->S, K = p->K, P = p->P;
     cudaStream_t sc = p->s_copy, sx = p->s_compute;
@@ -406,7 +409,7 @@ extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8
 extern "C" SKPS_API int skps_mpipe_submit_device(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* pitches,
                                                  const int32_t* hw, int n, const skps_mpipe_outputs* out, void* producer_stream) {
     SKPS_CHECK(p && frames && pitches && hw && n > 0 && n <= p->S, "mpipe_submit_device: bad arguments");
-    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_ON_DEVICE(p->device);
     for (int s = 0; s < n; ++s)
         if (check_device_frame(frames[s], p->device, "mpipe_submit_device", s)) return 1;
     return submit_batch(p, slot_i, frames, hw, n, pitches, (cudaStream_t)producer_stream, out);
@@ -417,7 +420,7 @@ extern "C" SKPS_API int skps_mpipe_wait_stream(skps_mpipe* p, int slot_i, void* 
     skps_mpipe::Slot& sl = p->slot[slot_i];
     SKPS_CHECK(sl.busy, "mpipe_wait_stream: nothing submitted on slot %d", slot_i);
     SKPS_CHECK(sl.device_out, "mpipe_wait_stream: slot %d has host results (call skps_mpipe_wait)", slot_i);
-    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_ON_DEVICE(p->device);
     SKPS_CUDA(cudaStreamWaitEvent((cudaStream_t)consumer_stream, sl.ev_done, 0));
     sl.busy = false;
     return 0;
@@ -429,7 +432,7 @@ extern "C" SKPS_API int skps_mpipe_wait(skps_mpipe* p, int slot_i, int32_t* n_fa
     skps_mpipe::Slot& sl = p->slot[slot_i];
     SKPS_CHECK(sl.busy, "mpipe_wait: nothing submitted on slot %d", slot_i);
     SKPS_CHECK(!sl.device_out, "mpipe_wait: slot %d has device results (call skps_mpipe_wait_stream)", slot_i);
-    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_ON_DEVICE(p->device);
     SKPS_CUDA(cudaEventSynchronize(sl.ev_done));
     sl.busy = false;
     const int K = p->K, P = p->P, n = sl.n;
@@ -458,7 +461,7 @@ static void free_align(skps_mpipe* p) {
 extern "C" SKPS_API int skps_mpipe_set_align(skps_mpipe* p, int size) {
     SKPS_CHECK(p && (size == 0 || (size >= 16 && size <= 512)), "mpipe_set_align: size %d is neither 0 nor in 16..512", size);
     SKPS_CHECK(!p->slot[0].busy && !p->slot[1].busy, "mpipe_set_align: a batch is in flight (call skps_mpipe_wait first)");
-    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_ON_DEVICE(p->device);
     SKPS_CUDA(cudaStreamSynchronize(p->s_compute));
     if (size == p->align_size) return 0;
     free_align(p);
@@ -504,7 +507,7 @@ static void free_pose(skps_mpipe* p) {
 extern "C" SKPS_API int skps_mpipe_set_pose(skps_mpipe* p, int on) {
     SKPS_CHECK(p, "mpipe_set_pose: null");
     SKPS_CHECK(!p->slot[0].busy && !p->slot[1].busy, "mpipe_set_pose: a batch is in flight (call skps_mpipe_wait first)");
-    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_ON_DEVICE(p->device);
     SKPS_CUDA(cudaStreamSynchronize(p->s_compute));
     if ((on != 0) == p->pose_on) return 0;
     free_pose(p);

@@ -5,6 +5,7 @@
 
 struct skps_pipeline_cfg;
 struct skps_det_src;
+struct skps_engine;
 
 namespace skps {
 
@@ -110,6 +111,8 @@ int launch_frame_diff(const MpStreamDesc* d, int n, const MpStreamDesc& one, siz
 // device or managed memory of `device`; the error names the caller `fn` and, for index >= 0, the frame's index.
 int upload_host_frame(const uint8_t* frame, size_t bytes, uint8_t* stage, uint8_t* dst, cudaStream_t s);
 int check_device_frame(const void* frame, int device, const char* fn, int index);
+// The device of a pipeline's two engines (engine.cu); fails, naming both devices, when they are on different devices.
+int engine_pair_device(const skps_engine* det, const skps_engine* kps, const char* fn, int* device);
 
 // Detector post-processing (nms.cu): score filter, sort, greedy NMS and scale_coords of `batch` frames of `rows` raw rows each
 // (raw [batch][rows][16]), for any number of candidates.  Frame f keeps its boxes in kept_rows [f][capacity][16] /

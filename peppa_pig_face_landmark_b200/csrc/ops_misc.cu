@@ -977,11 +977,8 @@ int launch_se_fc(const TView& part, const TView& gate, const float* w1t, const f
     SKPS_CHECK(k.slices >= 1, "se_fc: %d hidden channels", Cr);
     if (k.slices > 32) k.slices = 32;
     const size_t smem = (size_t)(k.C + k.Cr + k.slices * k.jp) * SE_SAMPLES * sizeof(float);
-    static bool attr_set = false;
-    if (!attr_set) {
-        SKPS_CUDA(cudaFuncSetAttribute(se_fc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-        attr_set = true;
-    }
+    static int attr_bytes[MAX_DEVICES] = {};
+    if (smem_limit((const void*)se_fc_kernel, attr_bytes, 96 * 1024)) return 1;
     SKPS_CHECK(smem <= 96 * 1024, "se_fc: %d + %d channels do not fit shared memory", k.C, k.Cr);
     se_fc_kernel<<<(batch + SE_SAMPLES - 1) / SE_SAMPLES, SE_THREADS, smem, s>>>(k);
     SKPS_CUDA(cudaGetLastError());

@@ -58,7 +58,7 @@ struct skps_pipeline {
 
 extern "C" SKPS_API void skps_pipeline_destroy(skps_pipeline* p) {
     if (!p) return;
-    cudaSetDevice(p->device);
+    DeviceGuard on(p->device);
     for (int i = 0; i < 2; ++i) if (p->d_frame[i]) cudaFree(p->d_frame[i]);
     if (p->h_frame) cudaFreeHost(p->h_frame);
     void* dev[] = {p->d_det_rows, p->d_det_idx, p->d_det_count, p->d_nms_ws, p->d_track, p->d_boxes, p->d_count, p->d_detail,
@@ -79,6 +79,9 @@ extern "C" SKPS_API int skps_pipeline_create(skps_engine* det, skps_engine* kps,
     SKPS_CHECK(det && kps && cfg && out, "pipeline_create: null argument");
     SKPS_CHECK(cfg->top_k > 0 && cfg->top_k <= SKPS_MAX_TOP_K, "pipeline_create: top_k %d outside 1..%d", cfg->top_k,
                SKPS_MAX_TOP_K);
+    int device = 0;
+    if (engine_pair_device(det, kps, "pipeline_create", &device)) return 1;
+    SKPS_ON_DEVICE(device);
     int c = 0, det_h = 0, det_w = 0, kh = 0, kw = 0;
     skps_engine_input_dims(det, &det_h, &det_w, &c);
     skps_engine_input_dims(kps, &kh, &kw, &c);
@@ -90,7 +93,7 @@ extern "C" SKPS_API int skps_pipeline_create(skps_engine* det, skps_engine* kps,
     p->det = det; p->kps = kps; p->cfg = *cfg;
     p->det_h = det_h; p->det_w = det_w; p->kps_hw = kh; p->n_points = P;
     p->det_rows = skps_engine_output_elems(det, 0) / 16;
-    cudaGetDevice(&p->device);
+    p->device = device;
     auto fail = [&](const char* what) {
         prefix_error("pipeline_create", what);
         skps_pipeline_destroy(p);
@@ -158,7 +161,7 @@ extern "C" SKPS_API int skps_pipeline_frame_diff(skps_pipeline* p, const uint8_t
                                                  void* stream) {
     SKPS_CHECK(p && frame && mean_diff, "frame_diff: null argument");
     cudaStream_t s = (cudaStream_t)stream;
-    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_ON_DEVICE(p->device);
     if (check_frame_size(p, H, W)) return 1;
     const size_t n = (size_t)H * W * 3;
     if (upload_host_frame(frame, n, p->h_frame, p->d_frame[p->cur], s)) return 1;
@@ -182,7 +185,7 @@ extern "C" SKPS_API int skps_pipeline_frame_diff_device(skps_pipeline* p, const 
     SKPS_CHECK(p && frame && mean_diff, "frame_diff_device: null argument");
     SKPS_CHECK(H == 1 || pitch >= 3 * W, "frame_diff_device: row pitch %d is less than 3 x width %d", pitch, W);
     cudaStream_t s = (cudaStream_t)stream, producer = (cudaStream_t)producer_stream;
-    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_ON_DEVICE(p->device);
     if (check_device_frame(frame, p->device, "frame_diff_device", -1) || check_frame_size(p, H, W)) return 1;
     const bool diff = p->prev_h == H && p->prev_w == W;
     SKPS_CUDA(cudaEventRecord(p->ev_ready, producer));
@@ -226,7 +229,7 @@ extern "C" SKPS_API int skps_pipeline_run(skps_pipeline* p, int run_detector, in
     SKPS_CHECK(p->cur_h > 0, "pipeline_run: no frame staged (call skps_pipeline_frame_diff or _frame_diff_device first)");
     SKPS_CHECK(n_track >= 0 && n_track <= p->track_cap, "pipeline_run: n_track %d outside 0..%d", n_track, p->track_cap);
     cudaStream_t s = (cudaStream_t)stream;
-    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_ON_DEVICE(p->device);
     const skps_pipeline_cfg& c = p->cfg;
     const int K = c.top_k, P = p->n_points, H = p->cur_h, W = p->cur_w;
     const uint8_t* d_frame = p->d_frame[p->cur];
@@ -328,7 +331,7 @@ extern "C" SKPS_API int skps_pipeline_det_results(skps_pipeline* p, int capacity
     const int n = p->last_n_det;
     SKPS_CHECK(capacity >= n, "pipeline_det_results: the last detector run kept %d boxes, capacity is %d", n, capacity);
     if (n == 0) return 0;
-    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_ON_DEVICE(p->device);
     if (det_idx) SKPS_CUDA(cudaMemcpy(det_idx, p->d_det_idx, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
     if (det_rows) SKPS_CUDA(cudaMemcpy(det_rows, p->d_det_rows, sizeof(float) * 16 * n, cudaMemcpyDeviceToHost));
     return 0;
@@ -343,7 +346,7 @@ extern "C" SKPS_API int skps_pipeline_align(skps_pipeline* p, const double* kps,
     SKPS_CHECK(size >= 16 && size <= 512, "pipeline_align: size %d outside 16..512", size);
     SKPS_CHECK(p->prev_h > 0 && p->prev_w > 0, "pipeline_align: no frame (run the pipeline first)");
     cudaStream_t s = (cudaStream_t)stream;
-    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_ON_DEVICE(p->device);
     const int K = p->cfg.top_k, P = p->n_points;
     const size_t chip_bytes = (size_t)size * size * 3;
     if (p->align_size != size) {
@@ -375,7 +378,7 @@ extern "C" SKPS_API int skps_pipeline_pose(skps_pipeline* p, const double* kps, 
     SKPS_CHECK(H > 0 && W > 0, "pipeline_pose: bad frame size %dx%d", H, W);
     SKPS_CHECK(p->n_points >= 98, "pipeline_pose: %d landmarks per face, expected 98", p->n_points);
     cudaStream_t s = (cudaStream_t)stream;
-    SKPS_CUDA(cudaSetDevice(p->device));
+    SKPS_ON_DEVICE(p->device);
     const int K = p->cfg.top_k, P = p->n_points;
     if (!p->d_pose) {
         SKPS_CUDA(cudaMalloc((void**)&p->d_pose_kps, sizeof(double) * 2 * P * K));

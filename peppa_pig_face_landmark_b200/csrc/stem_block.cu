@@ -372,11 +372,8 @@ bool stem_block_supported(int H, int W, int E, const TView& out) {
 Grid stem_block_grid(const StemBlockK& k, int num_sms) { return persistent_grid(k.n_tiles, num_sms); }
 
 int stem_block_launch(const StemBlockK& k, const StemBlockW& w, int num_sms, cudaStream_t s) {
-    static bool attr_set = false;
-    if (!attr_set) {
-        SKPS_CUDA(cudaFuncSetAttribute(stem_block_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SB_SMEM));
-        attr_set = true;
-    }
+    static int attr_bytes[MAX_DEVICES] = {};
+    if (smem_limit((const void*)stem_block_kernel<64>, attr_bytes, SB_SMEM)) return 1;
     const int grid = stem_block_grid(k, num_sms).ctas;
     stem_block_kernel<64><<<grid, SB_THREADS, SB_SMEM, s>>>(k, w);
     SKPS_CUDA(cudaGetLastError());

@@ -26,7 +26,6 @@ namespace skps {
 enum { XF_SCALE = 0, XF_DW = 1 };                                   // kernel mode
 enum { XS_UP_F32 = 0, XS_DW_F32 = 1, XS_DW_SPLIT = 2 };             // source of one 32-channel sub-chunk (XF_DW)
 constexpr int XF_MAX_CHUNKS = 16;                                   // K <= 1024 channels
-constexpr int XF_MAX_DEVICES = 64;
 
 constexpr int XF_THREADS = 512;
 constexpr int XF_TW = 16, XF_TH = 8;                 // output tile
@@ -86,11 +85,6 @@ int xf_producer_prepare(XfProducer& k, CUtensorMap& src0, CUtensorMap& src1_hi, 
 // `reserve` bytes, goes on depth.  b_slot = bytes of one weight-ring slot; two_out_bufs: a second staging buffer is of use.
 // Returns the bytes of the rings and the depthwise weights, or 0 when even the minimal rings do not fit.
 size_t xf_rings(XfProducer& k, int mode, size_t b_slot, size_t reserve, bool two_out_bufs, int& bs, int& out_bufs);
-// zeros standing in for a missing bias (at least 1024 channels), one allocation per device
-const float* xf_zero_bias();
-// Raises a kernel's dynamic shared-memory limit on the current device to `bytes` where it is lower.  set_bytes: the
-// kernel's limit per device so far, XF_MAX_DEVICES entries kept by the caller.
-int xf_smem_limit(const void* kernel, int* set_bytes, int bytes);
 
 // ------------------------------------------------------------------------------------------ device side
 struct XfBarriers {

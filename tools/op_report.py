@@ -794,18 +794,21 @@ def crop_inputs(batch=3):
     return _with_noise(frames.crop_variants(1)[0], batch)
 
 
-def make_engine(which, hw=None, batch=3):
+def make_engine(which, hw=None, batch=3, device=None):
+    """(engine, input batch) for which = detector (at input size hw), student or teacher; device: None (the current
+    device) or the device the engine runs on."""
     from peppa_pig_face_landmark_b200.core.api.onnx_model_base import ONNXEngine
+    dev = "cuda" if device is None else device
     pre = os.path.join(ROOT, "peppa_pig_face_landmark_b200", "pretrained")
     if which == "detector":
         from peppa_pig_face_landmark_b200.graph_tools import detector_onnx_for
         path = detector_onnx_for(os.path.join(pre, "yolov5n-0.5.onnx"), hw)
-        return ONNXEngine(path, max_batch=batch), detector_inputs(hw, batch)
+        return ONNXEngine(path, device=dev, max_batch=batch), detector_inputs(hw, batch)
     if which == "student":
-        return ONNXEngine(os.path.join(pre, "kps_student.onnx"), max_batch=batch), crop_inputs(batch)
+        return ONNXEngine(os.path.join(pre, "kps_student.onnx"), device=dev, max_batch=batch), crop_inputs(batch)
     if which == "teacher":
         from peppa_pig_face_landmark_b200 import teacher_graph as T
-        return ONNXEngine(T.ensure_teacher_onnx(256), max_batch=batch), crop_inputs(batch)
+        return ONNXEngine(T.ensure_teacher_onnx(256), device=dev, max_batch=batch), crop_inputs(batch)
     raise ValueError(which)
 
 
