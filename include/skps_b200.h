@@ -270,7 +270,7 @@ SKPS_API int skps_crop_resize(const uint8_t* frame, int H, int W, int pitch,
                      float face_scale /* float32(1+2*extend) */, float min_face,
                      uint8_t* crops, int out_hw, int32_t* detail, void* stream);
 
-/* Where one face's pixels are, for skps_crop_faces: `base` [dev] holds the rectangle of an H x W
+/* Where one face's pixels are, for skps_crop_faces and skps_warp_faces: `base` [dev] holds the rectangle of an H x W
  * frame that starts at column ox, row oy and is rw x rh pixels, rows `pitch` bytes apart.  A face
  * in a whole frame has ox = oy = 0, rw = W, rh = H; a face may also point at just the rectangle its
  * crop can read (FaceLandmark's host frames upload only that). */
@@ -505,6 +505,17 @@ SKPS_API int skps_warp_affine(const uint8_t* frame, int H, int W, int pitch, con
  * (n,size,size,3) uint8 and M [dev] (n,2,3) float64.  count [dev] or NULL as above.  Asynchronous on `stream`. */
 SKPS_API int skps_align_faces(const uint8_t* frame, int H, int W, int pitch, const double* kps, const int32_t* count, int n,
                               int P, int size, uint8_t* chips, double* M, void* stream);
+/* skps_warp_affine for n faces (any n >= 0) that may each come from a different image, in one launch per 65535 faces: chip i
+ * is warped from src[i] [dev] (skps_face_src, as skps_crop_faces takes it) with M [dev] (n,2,3) float64 -> out [dev]
+ * (n,out_h,out_w,3) uint8, the bytes cv2.warpAffine writes on the whole image.  A tap outside the image reads 0, and so
+ * does a tap inside the image but outside src[i]'s rectangle, which is never dereferenced (FaceLandmark's host frames
+ * upload only core/api/align.py:chip_read_rects).  Asynchronous on `stream`; allocates nothing. */
+SKPS_API int skps_warp_faces(const skps_face_src* src, const double* M, int n, int out_h, int out_w, uint8_t* out,
+                             void* stream);
+/* The estimate of skps_align_faces for n faces (any n >= 0) from float32 landmarks kps [dev] (n,P,2), P >= 98, each promoted
+ * to float64: M [dev] (n,2,3) float64, bit for bit what skps_align_faces gives for kps.astype(float64) (and so what
+ * FaceAna(align=size) returns for its float32 'kps').  size 16..512.  Asynchronous on `stream`; allocates nothing. */
+SKPS_API int skps_align_estimate(const float* kps, int n, int P, int size, double* M, void* stream);
 /* skps_align_faces on the frame of the last skps_pipeline_run / skps_pipeline_commit_frame (still in HBM, not uploaded
  * again) for FaceAna, whose landmarks are smoothed on the host: kps [host] (n,n_points,2) float64, chips [host]
  * (n,size,size,3) uint8, M [host] (n,2,3) float64.  n <= top_k.  Synchronous. */

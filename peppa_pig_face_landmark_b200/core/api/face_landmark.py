@@ -12,6 +12,9 @@ Additive: landmarks for faces the caller already has, from many frames per call 
     # overlapped, results left on the GPU (CUDA frames; boxes may be CUDA tensors straight from a GPU detector):
     bufs = [fl.new_results(n), fl.new_results(n)]
     fl.submit(frames_0, boxes_0, out=bufs[0]); fl.submit(frames_1, boxes_1, out=bufs[1]); r0 = fl.collect(); ...
+    # aligned chips of the same faces (core/api/align.py), for a detector that feeds its own aligner:
+    fl = FaceLandmark(max_faces=256, align=112)
+    res = fl.run_batch(frames, boxes)      # [(kps, scores, chips (k_i,112,112,3) uint8, M (k_i,2,3) float64) per frame]
 """
 import ctypes as C
 import os
@@ -22,6 +25,7 @@ import numpy as np
 
 from ... import runtime as rt
 from ...logger.logger import logger
+from .align import check_size, chip_read_rects
 from .device_frames import check_cuda_frame, check_host_frame, is_cuda_tensor, is_tensor
 from .onnx_model_base import ONNXEngine
 
@@ -77,10 +81,16 @@ def _grow(t, n, make):
 
 
 class FaceLandmark:
-    def __init__(self, cfg=None, max_faces=16, device="cuda"):
+    def __init__(self, cfg=None, max_faces=16, device="cuda", align=None):
         """cfg: Skps.yml's Keypoints section (None: read it from Skps.yml).  max_faces: faces per network forward; the
         Student@256 plan holds about 47 MB of activations per face of it.  Calls of run_batch / submit take any number
-        of faces and run them in chunks of at most max_faces."""
+        of faces and run them in chunks of at most max_faces.
+
+        align: None, or a chip side in 16..512: run_batch / collect then also return every face's chip (align, align, 3)
+        uint8 BGR and M (2, 3) float64, what FaceAna(align=align) computes from its 'kps': M is the similarity from the
+        landmarks promoted to float64 to the ArcFace template, the chip cv2.warpAffine(frame, M, (align, align)) bit for
+        bit (core/api/align.py).  Each of the two call slots then keeps align^2 x 3 bytes per face of its largest call
+        on the device and as much pinned (37.6 kB at 112, 786 kB at 512).  __call__ returns (kps, scores) as before."""
         if cfg is None:
             from .facer import get_cfg
             cfg = get_cfg()['Skps']['Keypoints']
@@ -96,6 +106,7 @@ class FaceLandmark:
         self.input_size = cfg['input_shape']
         self.extend = cfg['base_extend_range']
         self.face_scale = face_scale(cfg)
+        self.align = None if align is None else check_size(align)
         self.lib = rt.load_library()
         torch = rt.require_cuda()
         K = self.max_faces
@@ -104,8 +115,9 @@ class FaceLandmark:
         self._detail = torch.zeros((K, 5), dtype=torch.int32, device=self.device)
         self.last_detail = None
         self._slots = None            # staging of the batched path, made on first use
-        self._pending = []            # [(slot, faces per frame, out or None)]
+        self._pending = []            # [(slot, faces per frame, out or None, host frames to align or None)]
         self._next = 0
+        self._chip_stage = None       # staging of the host frames' chip rectangles, made on first use
 
     def crops(self, img, bboxes):
         """The (K,S,S,3) uint8 crops the network sees (face_landmark.py:66-104), for parity tests."""
@@ -138,7 +150,7 @@ class FaceLandmark:
             return np.array([]), np.array([])
         bboxes = np.asarray(bboxes, dtype=np.float32)
         slot = self._next
-        (kps, scores), = self.run_batch([img], [bboxes])
+        kps, scores = self.run_batch([img], [bboxes])[0][:2]
         self.last_detail = self._slots[slot]["detail"][:len(kps)].cpu().numpy()
         duration = time.time() - t0
         logger.info('keypoints done, time consume: %.5f and %.5f per face' % (duration, duration / len(bboxes)))
@@ -148,7 +160,8 @@ class FaceLandmark:
     def run_batch(self, frames, boxes):
         """Landmarks for the faces the caller has, over many frames (blocking): frames[i] with boxes[i] -> the i-th
         (kps (k_i, 98, 2) float32, scores (k_i, 98) float32) of the returned list, bit for bit what
-        FaceLandmark(cfg)(frames[i], boxes[i]) returns.  See submit() for what frames and boxes may be."""
+        FaceLandmark(cfg)(frames[i], boxes[i]) returns; with align, (kps, scores, chips (k_i, s, s, 3) uint8,
+        M (k_i, 2, 3) float64).  See submit() for what frames and boxes may be."""
         if self._pending:
             raise RuntimeError("FaceLandmark: %d calls in flight; collect() them first" % len(self._pending))
         self.submit(frames, boxes)
@@ -156,11 +169,19 @@ class FaceLandmark:
 
     def new_results(self, n_faces):
         """Device result buffers for submit(cuda_frames, boxes, out=...) of up to n_faces faces: a dict of CUDA tensors
-        on this object's device, kps (n_faces, 98, 2) and scores (n_faces, 98) float32."""
+        on this object's device, kps (n_faces, 98, 2) and scores (n_faces, 98) float32; with align also chip
+        (n_faces, s, s, 3) uint8 and M (n_faces, 2, 3) float64."""
         torch = rt.require_cuda()
-        n, P = int(n_faces), self.keypoints_num
-        return {"kps": torch.empty((n, P, 2), dtype=torch.float32, device=self.device),
-                "scores": torch.empty((n, P), dtype=torch.float32, device=self.device)}
+        return {k: torch.empty((int(n_faces),) + tail, dtype=getattr(torch, dt), device=self.device)
+                for k, (tail, dt) in self._out_fields().items()}
+
+    def _out_fields(self):
+        """{name: (shape of one face, dtype name)} of new_results."""
+        P, A = self.keypoints_num, self.align
+        f = {"kps": ((P, 2), "float32"), "scores": ((P,), "float32")}
+        if A is not None:
+            f.update({"chip": ((A, A, 3), "uint8"), "M": ((2, 3), "float64")})
+        return f
 
     def submit(self, frames, boxes, out=None):
         """Enqueue landmarks for boxes[i] on frames[i]; at most two calls may be in flight and collect() returns them in
@@ -175,7 +196,13 @@ class FaceLandmark:
         Ordering on torch.cuda.current_stream(): CUDA frames and boxes are read after the work already queued on it, and
         work queued on it after submit() returns runs after they have been read.
         out: None (collect() returns numpy arrays), or, with CUDA frames, a dict from new_results(n) with n >= the call's
-        faces, not used by a call still in flight: the results are written there on the GPU."""
+        faces, not used by a call still in flight: the results are written there on the GPU.
+
+        With align, CUDA frames are warped into chips on the GPU right after the landmarks, with no host synchronisation,
+        and are read until then.  Host frames are warped at collect(): M comes back with kps and scores, and
+        core/api/align.py:chip_read_rects picks the rectangle of the frame each chip reads, which is uploaded and warped.
+        That is one more read-back and one more upload per call, and the host frames must stay unchanged until
+        collect() returns."""
         if len(self._pending) == 2:
             raise RuntimeError("FaceLandmark: two calls already in flight; call collect() first")
         checked = self._check_call(frames, boxes)
@@ -184,7 +211,8 @@ class FaceLandmark:
                 raise ValueError("out= keeps results on the GPU and takes CUDA frames; these are host frames")
             self._check_out(out, sum(checked[5]))
         slot = self._enqueue(checked, out)
-        self._pending.append((slot, checked[5], out))
+        align_host = self.align is not None and not checked[3]
+        self._pending.append((slot, checked[5], out, (checked[0], checked[2]) if align_host else None))
 
     def _enqueue_to(self, frames, boxes, out):
         """submit() with results left in out (a new_results(n) dict) for host frames as well as CUDA frames, and not
@@ -235,6 +263,8 @@ class FaceLandmark:
             self._slots = [self._new_slot() for _ in range(2)]
         slot = self._next
         st = self._slots[slot]
+        A = self.align
+        warp_now = A is not None and cuda          # CUDA frames are warped here, host frames at collect()
         rects = None if cuda else [crop_read_rects(b, H, W, self.face_scale, self.min_face)
                                    for b, (H, W, _) in zip(boxes, layout)]
         roi_bytes = 0 if cuda else [(r[:, 2] - r[:, 0]) * (r[:, 3] - r[:, 1]) * 3 for r in rects]
@@ -251,6 +281,12 @@ class FaceLandmark:
             st["detail"] = _grow(st["detail"], n, lambda k: torch.empty((k, 5), dtype=torch.int32, device=self.device))
             st["hkps"] = _grow(st["hkps"], n, lambda k: torch.empty((k, P, 2), dtype=torch.float32).pin_memory())
             st["hscores"] = _grow(st["hscores"], n, lambda k: torch.empty((k, P), dtype=torch.float32).pin_memory())
+        if A is not None and out is None and (st["chips"] is None or st["chips"].shape[0] < n):
+            st["done"].synchronize()
+            st["M"] = _grow(st["M"], n, lambda k: torch.empty((k, 2, 3), dtype=torch.float64, device=self.device))
+            st["hM"] = _grow(st["hM"], n, lambda k: torch.empty((k, 2, 3), dtype=torch.float64).pin_memory())
+            st["chips"] = _grow(st["chips"], n, lambda k: torch.empty((k, A, A, 3), dtype=torch.uint8, device=self.device))
+            st["hchips"] = _grow(st["hchips"], n, lambda k: torch.empty((k, A, A, 3), dtype=torch.uint8).pin_memory())
         st["copied"].synchronize()                    # the slot's last upload has left the pinned staging
         host = st["host"].numpy()
         dev = st["dev"].data_ptr()
@@ -301,53 +337,112 @@ class FaceLandmark:
                 rt.check(self.lib.skps_crop_faces(dev + FACE_SRC.itemsize * c0, dev + box_off + 16 * c0, m,
                                                   self.face_scale, float(self.min_face), inp, S, det + 20 * c0,
                                                   s.cuda_stream))
-            if c0 + K >= n:
+            if c0 + K >= n and not warp_now:
                 st["read"].record(s)
             outs = (C.c_void_p * 2)(None, scores.data_ptr() + 4 * P * c0)
             rt.check(self.lib.skps_engine_forward(self.model.handle, inp, m, outs, s.cuda_stream))
             with torch.cuda.device(self.device):
                 rt.check(self.lib.skps_landmark_post(self.model.output_ptr(0), det + 20 * c0, st["count"].data_ptr(), m,
                                                      P, kps.data_ptr() + 8 * P * c0, s.cuda_stream))
-        if n == 0:
+        if A is not None and n:
+            M = out["M"] if out is not None else st["M"]
+            chips = out["chip"] if out is not None else st["chips"]
+            with torch.cuda.device(self.device):
+                rt.check(self.lib.skps_align_estimate(kps.data_ptr(), n, P, A, M.data_ptr(), s.cuda_stream))
+                if warp_now:                          # the face descriptors hold the whole CUDA frames
+                    rt.check(self.lib.skps_warp_faces(dev, M.data_ptr(), n, A, A, chips.data_ptr(), s.cuda_stream))
+        if n == 0 or warp_now:
             st["read"].record(s)
         torch.cuda.current_stream(self.device).wait_event(st["read"])
         if out is None and n:
             with torch.cuda.stream(s):
                 st["hkps"][:n].copy_(kps[:n], non_blocking=True)
                 st["hscores"][:n].copy_(scores[:n], non_blocking=True)
+                if A is not None:
+                    st["hM"][:n].copy_(st["M"][:n], non_blocking=True)
+                    if warp_now:
+                        st["hchips"][:n].copy_(st["chips"][:n], non_blocking=True)
         st["done"].record(s)
         self._next ^= 1
         return slot
 
     def collect(self):
         """Results of the oldest call in flight: a list with one (kps (k_i, 98, 2), scores (k_i, 98)) pair per frame, as
-        float32 numpy arrays; for a call submitted with out=, views of out's rows, with no host synchronisation:
-        torch.cuda.current_stream() is made to wait for the call, so work queued on it afterwards sees the results."""
+        float32 numpy arrays (with align, (kps, scores, chips, M)); for a call submitted with out=, views of out's rows,
+        with no host synchronisation: torch.cuda.current_stream() is made to wait for the call, so work queued on it
+        afterwards sees the results.  A call of host frames with align is warped here (see submit())."""
         if not self._pending:
             raise RuntimeError("FaceLandmark: nothing submitted")
-        slot, counts, out = self._pending.pop(0)
+        slot, counts, out, host_frames = self._pending.pop(0)
         st = self._slots[slot]
+        names = list(self._out_fields())
         if out is not None:
             import torch
             torch.cuda.current_stream(self.device).wait_event(st["done"])
-            kps, scores = out["kps"], out["scores"]
+            arrays = [out[k] for k in names]
         else:
             st["done"].synchronize()
-            kps, scores = st["hkps"].numpy(), st["hscores"].numpy()
+            n = sum(counts)
+            if host_frames is not None and n:
+                self._warp_host_frames(*host_frames, counts, st["hM"].numpy()[:n], st["M"], st["chips"], st["hchips"])
+            arrays = [st[h].numpy() for h in ("hkps", "hscores", "hchips", "hM")[:len(names)]]
         res, o = [], 0
         for k in counts:
             if out is None:
-                res.append((kps[o:o + k].copy(), scores[o:o + k].copy()))
+                res.append(tuple(a[o:o + k].copy() for a in arrays))
             else:
-                res.append((kps[o:o + k], scores[o:o + k]))
+                res.append(tuple(a[o:o + k] for a in arrays))
             o += k
         return res
+
+    def _warp_host_frames(self, frames, layout, counts, M, d_M, chips, h_chips):
+        """The chip phase of host frames (blocking): counts[i] faces of frames[i] (layout[i] = (H, W, pitch)), whose
+        matrices M (n, 2, 3) float64 are on the host and, equal, in d_M on the device.  Uploads the rectangle of each
+        frame that each chip reads (chip_read_rects) through pinned staging on a copy stream, warps chips[:n] on the
+        engine's stream, where no other kernel runs beside it, and copies them to the pinned h_chips[:n]."""
+        torch = rt.require_cuda()
+        n, A = len(M), self.align
+        rects = np.concatenate([chip_read_rects(M[o:o + k], A, H, W) for o, k, (H, W, _)
+                                in zip(np.cumsum([0] + list(counts[:-1])), counts, layout)])
+        rw, rh = rects[:, 2] - rects[:, 0], rects[:, 3] - rects[:, 1]
+        nb = rw * rh * 3
+        roi_off = (n * FACE_SRC.itemsize + 15) // 16 * 16
+        total = roi_off + int(nb.sum())
+        cs = self._chip_stage
+        if cs is None:
+            cs = self._chip_stage = dict(copy=torch.cuda.Stream(device=self.device), host=None, dev=None,
+                                         copied=torch.cuda.Event(), done=torch.cuda.Event())
+        cs["host"] = _grow(cs["host"], total, lambda k: torch.empty((k,), dtype=torch.uint8).pin_memory())
+        cs["dev"] = _grow(cs["dev"], total, lambda k: torch.empty((k,), dtype=torch.uint8, device=self.device))
+        host, dev = cs["host"].numpy(), cs["dev"].data_ptr()
+        starts = roi_off + np.concatenate(([0], np.cumsum(nb)[:-1]))
+        desc = host[:n * FACE_SRC.itemsize].view(FACE_SRC)
+        img = np.repeat(np.arange(len(counts)), counts)
+        hw = np.array([l[:2] for l in layout], np.int64)[img]
+        desc["H"], desc["W"] = hw[:, 0], hw[:, 1]
+        desc["base"], desc["pitch"], desc["_pad"] = dev + starts, 3 * rw, 0
+        desc["ox"], desc["oy"], desc["rw"], desc["rh"] = rects[:, 0], rects[:, 1], rw, rh
+        for j in np.flatnonzero(nb):
+            x0, y0, x1, y1 = (int(v) for v in rects[j])
+            host[starts[j]:starts[j] + nb[j]].reshape(y1 - y0, 3 * (x1 - x0))[:] = \
+                frames[img[j]][y0:y1, x0:x1].reshape(y1 - y0, 3 * (x1 - x0))
+        s, cp = self.model.stream, cs["copy"]
+        with torch.cuda.stream(cp):
+            cs["dev"][:total].copy_(cs["host"][:total], non_blocking=True)
+        cs["copied"].record(cp)
+        s.wait_event(cs["copied"])
+        with torch.cuda.device(self.device):
+            rt.check(self.lib.skps_warp_faces(dev, d_M.data_ptr(), n, A, A, chips.data_ptr(), s.cuda_stream))
+        with torch.cuda.stream(s):
+            h_chips[:n].copy_(chips[:n], non_blocking=True)
+        cs["done"].record(s)
+        cs["done"].synchronize()                  # the staging is free again and h_chips holds the chips
 
     def _new_slot(self):
         import torch
         ev = {name: torch.cuda.Event() for name in ("copied", "read", "done")}
         return dict(copy=torch.cuda.Stream(device=self.device), host=None, dev=None, kps=None, scores=None, detail=None,
-                    hkps=None, hscores=None, count=torch.full((1,), self.max_faces, dtype=torch.int32, device=self.device),
+                    hkps=None, hscores=None, M=None, hM=None, chips=None, hchips=None, count=torch.full((1,), self.max_faces, dtype=torch.int32, device=self.device),
                     **ev)
 
     @staticmethod
@@ -374,16 +469,16 @@ class FaceLandmark:
 
     def _check_out(self, out, n):
         import torch
-        P = self.keypoints_num
-        if not isinstance(out, dict) or set(out) != {"kps", "scores"}:
-            raise ValueError("out: expected a dict with keys ['kps', 'scores'] (see new_results())")
-        for k, tail in (("kps", (P, 2)), ("scores", (P,))):
+        fields = self._out_fields()
+        if not isinstance(out, dict) or set(out) != set(fields):
+            raise ValueError("out: expected a dict with keys %s (see new_results())" % sorted(fields))
+        for k, (tail, dt) in fields.items():
             t = out[k]
-            if (not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or t.device != self.device
+            if (not isinstance(t, torch.Tensor) or t.dtype != getattr(torch, dt) or t.device != self.device
                     or not t.is_contiguous() or tuple(t.shape[1:]) != tail or t.shape[0] < n):
                 got = ("%s %s on %s" % (t.dtype, tuple(t.shape), t.device)) if is_tensor(t) else type(t).__name__
-                raise ValueError("out[%r]: expected a contiguous float32 tensor (>= %d, %s) on %s, got %s"
-                                 % (k, n, ", ".join(map(str, tail)), self.device, got))
-        busy = {t.data_ptr() for _, _, o in self._pending if o is not None for t in o.values()}
+                raise ValueError("out[%r]: expected a contiguous %s tensor (>= %d, %s) on %s, got %s"
+                                 % (k, dt, n, ", ".join(map(str, tail)), self.device, got))
+        busy = {t.data_ptr() for p in self._pending if p[2] is not None for t in p[2].values()}
         if any(t.data_ptr() in busy for t in out.values()):
             raise ValueError("out: these buffers belong to a call still in flight; collect() it first")

@@ -6,6 +6,7 @@ max_frames and the landmark net in batches of max_faces on exactly the faces fou
 
     fi = FaceAnaImages(top_k=16)
     res = fi.run_batch(images)          # one list of {'box','kps','scores'} per image, what FaceAna.run returns after reset()
+    fi = FaceAnaImages(top_k=16, align=112)     # also 'chip' and 'M' per face, as FaceAna(align=112) returns them
     # overlapped: while one call's landmarks run, the next call stages its images
     fi.submit(images_0); fi.submit(images_1); r0 = fi.collect(); fi.submit(images_2); r1 = fi.collect(); ...
     # CUDA images, results left on the GPU, packed by image:
@@ -14,12 +15,15 @@ max_frames and the landmark net in batches of max_faces on exactly the faces fou
 One call on the GPU: FaceDetector's batched letterbox, network and NMS; skps_select_faces_batch (sort_and_filter with no
 track boxes, one block per image); one read-back of the face counts and selected boxes, which size the landmark batch and,
 for host images, cut their upload to the crop rectangles; FaceLandmark's batched crops, network and de-normalisation;
-skps_landmark_boxes (the returned box, judge_boxs(boxes, rects(kps))); with pose, skps_head_pose_faces.
+skps_landmark_boxes (the returned box, judge_boxs(boxes, rects(kps))); with pose, skps_head_pose_faces.  With align,
+FaceLandmark's chip stage: skps_align_estimate right after the landmarks, and skps_warp_faces on CUDA images there too, or
+on the rectangles of host images each chip reads at collect().
 """
 import numpy as np
 
 from ... import runtime as rt
 from ...graph_tools import check_detector_input
+from .align import check_size
 from .device_frames import is_tensor
 from .face_detector import FaceDetector, _grow, _pad16
 from .face_landmark import FaceLandmark
@@ -37,21 +41,23 @@ def pack_faces(counts):
     return first.astype(np.int32), np.repeat(np.arange(len(counts)), counts).astype(np.int32)
 
 
-def result_fields(n_images, top_k, n_points, pose):
+def result_fields(n_images, top_k, n_points, pose, align=None):
     """{name: (shape, dtype name)} of new_results(n_images)."""
     rows = n_images * top_k
     f = {"count": ((n_images,), "int32"), "first": ((n_images,), "int32"), "box": ((rows, 4), "float32"),
          "kps": ((rows, n_points, 2), "float32"), "scores": ((rows, n_points), "float32")}
+    if align is not None:
+        f.update({"chip": ((rows, align, align, 3), "uint8"), "M": ((rows, 2, 3), "float64")})
     if pose:
         f.update({k: ((rows,) + tail, "float64") for k, tail in POSE_FIELDS})
     return f
 
 
-def check_results(out, n_images, top_k, n_points, pose, device, busy=()):
+def check_results(out, n_images, top_k, n_points, pose, device, busy=(), align=None):
     """ValueError unless out is a dict of result buffers (new_results) on `device` that holds a call of n_images images
     and shares no buffer with `busy` (the buffers of calls still in flight)."""
     import torch
-    want = result_fields(n_images, top_k, n_points, pose)
+    want = result_fields(n_images, top_k, n_points, pose, align)
     if not isinstance(out, dict) or set(out) != set(want):
         raise ValueError("out: expected a dict with keys %s (see new_results())" % sorted(want))
     for k, (shape, dt) in want.items():
@@ -66,21 +72,25 @@ def check_results(out, n_images, top_k, n_points, pose, device, busy=()):
 
 
 class FaceAnaImages:
-    def __init__(self, top_k=None, det_input=None, pose=False, max_frames=16, max_faces=64, device="cuda"):
+    def __init__(self, top_k=None, det_input=None, pose=False, max_frames=16, max_faces=64, device="cuda", align=None):
         """top_k: None (Skps.yml's Detect.topk, 5), or 1..1024 faces per image.  det_input: None (Skps.yml's 384x640), or
         the detector input size (h, w) as FaceAna(det_input=...) takes it.  pose: every result dict then also carries
-        'pose' as FaceAna(pose=True) returns it, each face with its own image's size for the camera.
+        'pose' as FaceAna(pose=True) returns it, each face with its own image's size for the camera.  align: None, or a
+        chip side in 16..512: every result dict then also carries 'chip' (align, align, 3) uint8 and 'M' (2, 3) float64
+        as FaceAna(align=align) returns them (FaceLandmark(align=...)'s chip stage).
 
-        run_batch(images)[i] is bit for bit what FaceAna(top_k=top_k, det_input=det_input, pose=pose).run(images[i])
-        returns on a new or just-reset FaceAna, for images of any size (FaceAna's max_frame_hw does not apply).
+        run_batch(images)[i] is bit for bit what FaceAna(top_k=top_k, det_input=det_input, pose=pose,
+        align=align).run(images[i]) returns on a new or just-reset FaceAna, for images of any size (FaceAna's
+        max_frame_hw does not apply).
 
         max_frames: images per detector forward; max_faces: faces per landmark forward.  A call takes any number of
         images and faces and runs them in chunks of these.  Memory: the detector holds about 39 MB of activations per
         frame of max_frames at 384x640 (0.35 GB at 1152x1920), the landmark net about 47 MB per face of max_faces (3 GB
         at 64).  Each of the two call slots keeps, per image of its largest call, every detector row as a possible kept
         row (rows x 68 bytes: 1.0 MB at 384x640, 9.3 MB at 1152x1920) and top_k selected boxes; per face of its
-        largest call, its results (about 1.2 kB, 1.4 kB with pose); and, for host images, the pinned staging of the
-        rows and crop rectangles it uploads."""
+        largest call, its results (about 1.2 kB, 1.4 kB with pose; with align, align^2 x 3 bytes more on the device and
+        as much pinned: 37.6 kB at 112, 786 kB at 512); and, for host images, the pinned staging of the rows and crop
+        rectangles it uploads.  With align, one more pinned staging holds the chip rectangles of the largest host call."""
         cfg = get_cfg()['Skps']
         self.top_k = int(top_k if top_k is not None else cfg['Detect']['topk'])
         if not 1 <= self.top_k <= MAX_TOP_K:
@@ -89,8 +99,9 @@ class FaceAnaImages:
             det_input = check_detector_input(det_input)
             cfg['Detect']['input_shape'] = [det_input[0], det_input[1], 3]
         self.pose = bool(pose)
+        self.align = None if align is None else check_size(align)
         self.detector = FaceDetector(cfg['Detect'], max_frames=max_frames, device=device)
-        self.landmark = FaceLandmark(cfg['Keypoints'], max_faces=max_faces, device=device)
+        self.landmark = FaceLandmark(cfg['Keypoints'], max_faces=max_faces, device=device, align=self.align)
         self.max_frames, self.max_faces = self.detector.max_frames, self.landmark.max_faces
         self.device = self.detector.device
         self.n_points = self.landmark.keypoints_num
@@ -101,13 +112,13 @@ class FaceAnaImages:
         self.one_minus_alpha = 1 - self.alpha
         self.lib = rt.load_library()
         self._slots = None            # device and pinned buffers of the two call slots, made on first use
-        self._pending = []            # [(slot, n images, out or None, counts, first)]
+        self._pending = []            # [(slot, n images, out or None, counts, first, host images to align or None)]
         self._next = 0
 
     # ------------------------------------------------------------------
     def run_batch(self, images):
-        """FaceAna.run after reset() for every image (blocking): one list of {'box', 'kps', 'scores'[, 'pose']} per
-        image, [] for an image without a face.  See submit() for what images may be."""
+        """FaceAna.run after reset() for every image (blocking): one list of {'box', 'kps', 'scores'[, 'chip', 'M']
+        [, 'pose']} per image, [] for an image without a face.  See submit() for what images may be."""
         if self._pending:
             raise RuntimeError("FaceAnaImages: %d calls in flight; collect() them first" % len(self._pending))
         self.submit(images)
@@ -116,12 +127,14 @@ class FaceAnaImages:
     def new_results(self, n_images):
         """Device result buffers for submit(cuda_images, out=...) of up to n_images images: a dict of CUDA tensors on
         this object's device.  count, first (n,) int32; box (n*top_k, 4), kps (n*top_k, P, 2), scores (n*top_k, P)
-        float32; with pose also rvec, tvec, euler (n*top_k, 3) and reproject (n*top_k, 8, 2) float64.  Faces are packed
+        float32; with align also chip (n*top_k, s, s, 3) uint8 and M (n*top_k, 2, 3) float64; with pose also rvec,
+        tvec, euler (n*top_k, 3) and reproject (n*top_k, 8, 2) float64.  Faces are packed
         in image order, each image's in FaceAna's order: image i's are rows first[i] .. first[i] + count[i] - 1.  Rows
         past the call's faces are unspecified."""
         torch = rt.require_cuda()
         return {k: torch.empty(shape, dtype=getattr(torch, dt), device=self.device)
-                for k, (shape, dt) in result_fields(int(n_images), self.top_k, self.n_points, self.pose).items()}
+                for k, (shape, dt) in result_fields(int(n_images), self.top_k, self.n_points, self.pose,
+                                                    self.align).items()}
 
     def submit(self, images, out=None):
         """Enqueue the analysis of images; at most two calls may be in flight and collect() returns them in submission
@@ -135,7 +148,12 @@ class FaceAnaImages:
         Ordering on torch.cuda.current_stream(): CUDA images are read after the work already queued on it, and work
         queued on it after submit() returns runs after they have been read, so the producer may reuse them at once.
         out: None (collect() returns lists of dicts), or, with CUDA images, a dict from new_results(n) with n >= the
-        call's images, not used by a call still in flight: the results are written there on the GPU."""
+        call's images, not used by a call still in flight: the results are written there on the GPU.
+
+        With align, CUDA images are warped into chips right after the landmarks, with no host synchronisation.  Host
+        images are warped at collect(): M comes back with the other results, and only the rectangle of an image each
+        chip reads is uploaded then.  That is one more read-back and one more upload per call, and the host images
+        must stay unchanged until collect() returns."""
         if len(self._pending) == 2:
             raise RuntimeError("FaceAnaImages: two calls already in flight; call collect() first")
         checked = self.detector._layout(list(images))
@@ -145,9 +163,9 @@ class FaceAnaImages:
             if not (n and cuda):
                 raise ValueError("out= keeps results on the GPU and takes CUDA images")
             check_results(out, n, self.top_k, self.n_points, self.pose, self.device,
-                          [t.data_ptr() for p in self._pending if p[2] is not None for t in p[2].values()])
+                          [t.data_ptr() for p in self._pending if p[2] is not None for t in p[2].values()], self.align)
         if n == 0:
-            self._pending.append((None, 0, None, None, None))
+            self._pending.append((None, 0, None, None, None, None))
             return
         torch = rt.require_cuda()
         if self._slots is None:
@@ -193,11 +211,11 @@ class FaceAnaImages:
         # 4. landmarks on exactly the faces found, packed in image order
         if out is None:
             self._grow_faces(st, max(F, 1))
-            res = {k: st[k] for k in ("box", "kps", "scores") + (tuple(k for k, _ in POSE_FIELDS) if self.pose else ())}
+            res = {k: st[k] for k in self._face_fields()}
         else:
             res = out
         fl._enqueue_to(frames, [boxes[i, :k] for i, k in enumerate(counts.tolist())],
-                       {"kps": res["kps"], "scores": res["scores"]})
+                       {k: res[k] for k in fl._out_fields()})
         # face -> image map and each face's image size; with out=, first and count too: one upload
         m = 2 * n + 3 * F
         if st["hmap"] is None or st["hmap"].shape[0] < m:
@@ -230,9 +248,11 @@ class FaceAnaImages:
         if out is None and F:
             with torch.cuda.stream(ls):
                 for k, t in res.items():
-                    st["h" + k][:F].copy_(t[:F], non_blocking=True)
+                    if k != "chip" or cuda:           # host images are warped at collect()
+                        st["h" + k][:F].copy_(t[:F], non_blocking=True)
         st["done"].record(ls)
-        self._pending.append((slot, n, out, counts, first))
+        align_host = self.align is not None and not cuda
+        self._pending.append((slot, n, out, counts, first, (frames, [f.shape for f in frames]) if align_host else None))
         self._next ^= 1
 
     def collect(self):
@@ -241,7 +261,7 @@ class FaceAnaImages:
         torch.cuda.current_stream() is made to wait for the call, so work queued on it afterwards sees the results."""
         if not self._pending:
             raise RuntimeError("FaceAnaImages: nothing submitted")
-        slot, n, out, counts, first = self._pending.pop(0)
+        slot, n, out, counts, first, host_images = self._pending.pop(0)
         if n == 0:
             return []
         st = self._slots[slot]
@@ -251,12 +271,17 @@ class FaceAnaImages:
             return out
         st["done"].synchronize()
         F = int(counts.sum())
-        host = {k: st["h" + k].numpy()[:F] for k in ("box", "kps", "scores") +
-                (tuple(k for k, _ in POSE_FIELDS) if self.pose else ())}
+        if host_images is not None and F:
+            self.landmark._warp_host_frames(*host_images, counts.tolist(), st["hM"].numpy()[:F], st["M"], st["chip"],
+                                            st["hchip"])
+        host = {k: st["h" + k].numpy()[:F] for k in self._face_fields()}
         res = []
         for o, k in zip(first.tolist(), counts.tolist()):
             part = {name: a[o:o + k].copy() for name, a in host.items()}
             faces = [{'box': part['box'][j], 'kps': part['kps'][j], 'scores': part['scores'][j]} for j in range(k)]
+            if self.align is not None:
+                for j, r in enumerate(faces):
+                    r['chip'], r['M'] = part['chip'][j], part['M'][j]
             if self.pose:
                 for j, r in enumerate(faces):
                     r['pose'] = {name: part[name][j] for name, _ in POSE_FIELDS}
@@ -269,6 +294,10 @@ class FaceAnaImages:
         ev = {name: torch.cuda.Event() for name in ("selected", "staged", "done")}
         return dict(det=None, sel=None, hsel=None, map=None, hmap=None, faces=0, **ev)
 
+    def _face_fields(self):
+        """Names of the per-face results, in new_results' order."""
+        return [k for k in result_fields(1, 1, self.n_points, self.pose, self.align) if k not in ("count", "first")]
+
     def _grow_faces(self, st, F):
         """The slot's device results and their pinned copies, for at least F faces."""
         import torch
@@ -276,7 +305,7 @@ class FaceAnaImages:
             return
         st["done"].synchronize()
         rows = max(F, 2 * st["faces"], 1)
-        for k, (shape, dt) in result_fields(rows, 1, self.n_points, self.pose).items():
+        for k, (shape, dt) in result_fields(rows, 1, self.n_points, self.pose, self.align).items():
             if k in ("count", "first"):
                 continue
             st[k] = torch.empty(shape, dtype=getattr(torch, dt), device=self.device)

@@ -7,7 +7,8 @@
 //
 // Two launches cover every face of every frame of a call: the estimate (a thread per face), then the warp (grid.y = face,
 // grid.x = runs of 256 pixels of the face's chip, stored with consecutive threads on consecutive bytes).  The frame is
-// read where it lies.
+// read where it lies.  A face's source is one frame for all faces, one MpStreamDesc per group of faces, or one
+// skps_face_src per face (faces of many images, or just the rectangle of an image a chip reads).
 #include <limits.h>
 
 #include "../../include/skps_b200.h"
@@ -26,19 +27,21 @@ __constant__ int kFive[5] = {96, 97, 54, 76, 82};
 // Least-squares similarity (rotation, uniform scale, translation; no reflection) mapping the five landmarks of `kps`
 // (P x 2) onto the template scaled by size/112.  The 2-D closed form of Umeyama 1991: with centred points a_i (source)
 // and b_i (template), scale*cos = sum(a.b) / sum|a|^2 and scale*sin = sum(a x b) / sum|a|^2.
-__device__ void similarity_to_template(const double* __restrict__ kps, int size, double* M) {
+// T: the landmarks' type, each promoted to double as it is read.
+template <typename T>
+__device__ void similarity_to_template(const T* __restrict__ kps, int size, double* M) {
     const double sc = size / 112.0;
     double msx = 0, msy = 0, mdx = 0, mdy = 0;
 #pragma unroll 1
     for (int i = 0; i < 5; ++i) {
-        msx += kps[2 * kFive[i]]; msy += kps[2 * kFive[i] + 1];
+        msx += (double)kps[2 * kFive[i]]; msy += (double)kps[2 * kFive[i] + 1];
         mdx += kTemplate112[2 * i] * sc; mdy += kTemplate112[2 * i + 1] * sc;
     }
     msx /= 5; msy /= 5; mdx /= 5; mdy /= 5;
     double dot = 0, cross = 0, den = 0;
 #pragma unroll 1
     for (int i = 0; i < 5; ++i) {
-        const double ax = kps[2 * kFive[i]] - msx, ay = kps[2 * kFive[i] + 1] - msy;
+        const double ax = (double)kps[2 * kFive[i]] - msx, ay = (double)kps[2 * kFive[i] + 1] - msy;
         const double bx = kTemplate112[2 * i] * sc - mdx, by = kTemplate112[2 * i + 1] * sc - mdy;
         dot += ax * bx + ay * by;
         cross += ax * by - ay * bx;
@@ -58,6 +61,7 @@ __device__ __forceinline__ int sat_short(int v) { return v < -32768 ? -32768 : (
 struct WarpArgs {
     const uint8_t* frame; int H, W, pitch;      // the frame of every face (desc == null)
     const MpStreamDesc* desc;                   // or per group: desc[g].cur, H, W (pitch W*3)
+    const skps_face_src* src;                   // or per face: src[f], taps outside its rectangle read 0
     const double* M;                            // [faces][2][3] frame -> chip
     const int* count; int per_group;            // face f = g * per_group + i is skipped when count && i >= count[g]
     int out_h, out_w;
@@ -65,7 +69,8 @@ struct WarpArgs {
 };
 
 // One thread per face: M[f] from the landmarks kps[f] (P x 2).
-__global__ void __launch_bounds__(128) align_estimate_kernel(const double* __restrict__ kps, int P, const int* __restrict__ count,
+template <typename T>
+__global__ void __launch_bounds__(128) align_estimate_kernel(const T* __restrict__ kps, int P, const int* __restrict__ count,
                                                              int per_group, int faces, int size, double* __restrict__ M) {
     const int f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= faces) return;
@@ -87,12 +92,17 @@ __global__ void __launch_bounds__(256) align_warp_kernel(const WarpArgs a) {
     const int pixels = a.out_w * a.out_h;
     const int p = blockIdx.x * 256 + threadIdx.x;
     if (p < pixels) {
-        const uint8_t* frame = a.frame;
-        int H = a.H, W = a.W, pitch = a.pitch;
+        // base holds the rectangle of an H x W image at column ox, row oy, rw x rh pixels
+        const uint8_t* base = a.frame;
+        int H = a.H, W = a.W, pitch = a.pitch, ox = 0, oy = 0, rw = a.W, rh = a.H;
         if (a.desc) {
             const MpStreamDesc& d = a.desc[g];
-            frame = d.cur; H = d.H; W = d.W; pitch = d.W * 3;
+            base = d.cur; H = d.H; W = d.W; pitch = d.W * 3; rw = W; rh = H;
+        } else if (a.src) {
+            const skps_face_src& s = a.src[f];
+            base = s.base; H = s.H; W = s.W; pitch = s.pitch; ox = s.ox; oy = s.oy; rw = s.rw; rh = s.rh;
         }
+        const int xa = max(ox, 0), xb = min(ox + rw, W), ya = max(oy, 0), yb = min(oy + rh, H);
         // the inverse map as warpAffine computes it (imgwarp.cpp), same order of operations; every thread of the face
         // computes the same values
         const double* Mf = a.M + (size_t)f * 6;
@@ -113,10 +123,10 @@ __global__ void __launch_bounds__(256) align_warp_kernel(const WarpArgs a) {
         const int sx = sat_short(X >> 5), sy = sat_short(Y >> 5);
         const int fx = X & 31, fy = Y & 31;
         const int w00 = (32 - fx) * (32 - fy), w01 = fx * (32 - fy), w10 = (32 - fx) * fy, w11 = fx * fy;
-        // taps outside the frame read the border value 0
-        const bool x0 = sx >= 0 && sx < W, x1 = sx + 1 >= 0 && sx + 1 < W;
-        const bool y0 = sy >= 0 && sy < H, y1 = sy + 1 >= 0 && sy + 1 < H;
-        const uint8_t* r0 = frame + (ptrdiff_t)sy * pitch + (ptrdiff_t)sx * 3;     // dereferenced only where inside
+        // taps outside the frame read the border value 0; so do taps outside the rectangle, which are never dereferenced
+        const bool x0 = sx >= xa && sx < xb, x1 = sx + 1 >= xa && sx + 1 < xb;
+        const bool y0 = sy >= ya && sy < yb, y1 = sy + 1 >= ya && sy + 1 < yb;
+        const uint8_t* r0 = base + (ptrdiff_t)(sy - oy) * pitch + (ptrdiff_t)(sx - ox) * 3;   // dereferenced only where inside
         const uint8_t* r1 = r0 + pitch;
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
@@ -142,7 +152,7 @@ int launch_warp(const WarpArgs& a, int faces, cudaStream_t s) {
 // estimate (one launch, a thread per face) then warp (one launch, a thread per output byte)
 int launch_align(const uint8_t* frame, int H, int W, int pitch, const MpStreamDesc* desc, const double* kps, int P,
                  const int* count, int per_group, int faces, int size, uint8_t* chips, double* M, cudaStream_t s) {
-    align_estimate_kernel<<<(faces + 127) / 128, 128, 0, s>>>(kps, P, count, per_group, faces, size, M);
+    align_estimate_kernel<double><<<(faces + 127) / 128, 128, 0, s>>>(kps, P, count, per_group, faces, size, M);
     SKPS_CUDA(cudaGetLastError());
     WarpArgs a = {};
     a.frame = frame; a.H = H; a.W = W; a.pitch = pitch; a.desc = desc;
@@ -180,4 +190,31 @@ extern "C" SKPS_API int skps_align_faces(const uint8_t* frame, int H, int W, int
     SKPS_CHECK(n > 0 && n <= 65535 && P >= 98, "align_faces: n %d or n_points %d out of range", n, P);
     SKPS_CHECK(size >= 16 && size <= 512, "align_faces: size %d outside 16..512", size);
     return launch_align(frame, H, W, pitch, nullptr, kps, P, count, n, n, size, chips, M, (cudaStream_t)stream);
+}
+
+extern "C" SKPS_API int skps_warp_faces(const skps_face_src* src, const double* M, int n, int out_h, int out_w, uint8_t* out,
+                                        void* stream) {
+    SKPS_CHECK(n >= 0 && out_h > 0 && out_w > 0 && out_h <= 4096 && out_w <= 4096,
+               "warp_faces: n %d or output %dx%d out of range", n, out_h, out_w);
+    if (n == 0) return 0;
+    SKPS_CHECK(src && M && out, "warp_faces: bad arguments");
+    // grid.y is the face: chunks of at most 65535 faces
+    for (int c0 = 0; c0 < n; c0 += 65535) {
+        const int m = min(65535, n - c0);
+        WarpArgs a = {};
+        a.src = src + c0; a.M = M + (size_t)c0 * 6; a.per_group = m;
+        a.out_h = out_h; a.out_w = out_w; a.out = out + (size_t)c0 * out_h * out_w * 3;
+        if (launch_warp(a, m, (cudaStream_t)stream)) return 1;
+    }
+    return 0;
+}
+
+extern "C" SKPS_API int skps_align_estimate(const float* kps, int n, int P, int size, double* M, void* stream) {
+    SKPS_CHECK(n >= 0 && P >= 98, "align_estimate: n %d or n_points %d out of range", n, P);
+    SKPS_CHECK(size >= 16 && size <= 512, "align_estimate: size %d outside 16..512", size);
+    if (n == 0) return 0;
+    SKPS_CHECK(kps && M, "align_estimate: bad arguments");
+    align_estimate_kernel<float><<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(kps, P, nullptr, n, n, size, M);
+    SKPS_CUDA(cudaGetLastError());
+    return 0;
 }

@@ -7,12 +7,14 @@
   (e) out      the same with CUDA images and out= (results left on the GPU);
   (f) engines  the detector engine alone at batch max_frames and the landmark engine alone at batch max_faces, as the
                ceiling: a call's engine time is n images x detector time per frame + its faces x landmark time per face.
+With --align SIZE, (c), (d) and (e) also run with FaceAnaImages(align=SIZE), as host_align, cuda_align and out_align,
+alternated with the others, and the host upload counts the chip rectangles (chip_read_rects) as well.
 Workloads: 16 x 1080p with 4 faces, 16 x 4K with 16 faces (top_k 16), and a photo collection of 16 images of mixed
 sizes (4000x3000, 3000x4000, 1920x1080, 1280x720, 640x480) with 0-6 faces each.  Prints one JSON line per workload and
 mode: median images/s over the rounds and its spread, faces/s, ms per call, call time over engine time, and for host
 images the bytes one call uploads; then the card's name and power limit read in the same run.
 
-    python tools/bench_images.py [--rounds 5] [--iters 10] [--images 16]"""
+    python tools/bench_images.py [--rounds 5] [--iters 10] [--images 16] [--align SIZE]"""
 import argparse
 import json
 import os
@@ -59,20 +61,29 @@ def card():
 
 def upload_bytes(fi, imgs):
     """Bytes one host-image call of FaceAnaImages sends: the detector's rows (host_upload_rows) and descriptors, and the
-    crop rectangles of the selected faces (crop_read_rects) with their descriptors and boxes."""
+    crop rectangles of the selected faces (crop_read_rects) with their descriptors and boxes; with align, also the chip
+    rectangles (chip_read_rects) with their descriptors."""
+    from peppa_pig_face_landmark_b200.core.api.align import chip_read_rects
     from oracle.host_ref import sort_and_filter
     from peppa_pig_face_landmark_b200.core.api.face_detector import DET_SRC, host_upload_rows, letterbox_geometry
     from peppa_pig_face_landmark_b200.core.api.face_landmark import FACE_SRC, crop_read_rects
     fd, fl = fi.detector, fi.landmark
-    n, det, kps = len(imgs), (DET_SRC.itemsize + 12) * len(imgs), 0
-    for img, rows in zip(imgs, fd.run_batch(imgs)):
+    n, det, kps, chips = len(imgs), (DET_SRC.itemsize + 12) * len(imgs), 0, 0
+    res = fi.run_batch(imgs) if fi.align is not None else [[]] * n
+    for img, rows, faces in zip(imgs, fd.run_batch(imgs), res):
         H, W = img.shape[:2]
         r = host_upload_rows(H, letterbox_geometry(H, W, *fd.input_size[:2])[2])
         det += (H if r is None else len(r)) * 3 * W
         boxes = np.asarray(sort_and_filter(rows, fi.min_face, fi.top_k), np.float32).reshape(-1, 16)
         rect = crop_read_rects(boxes, H, W, fl.face_scale)
         kps += int(((rect[:, 2] - rect[:, 0]) * (rect[:, 3] - rect[:, 1]) * 3).sum()) + (FACE_SRC.itemsize + 16) * len(rect)
-    return {"detector": det, "landmarks": kps, "whole_images": int(sum(f.nbytes for f in imgs)), "images": n}
+        if faces:
+            rect = chip_read_rects(np.stack([r["M"] for r in faces]), fi.align, H, W)
+            chips += int(((rect[:, 2] - rect[:, 0]) * (rect[:, 3] - rect[:, 1]) * 3).sum()) + FACE_SRC.itemsize * len(rect)
+    out = {"detector": det, "landmarks": kps, "whole_images": int(sum(f.nbytes for f in imgs)), "images": n}
+    if fi.align is not None:
+        out["chips"] = chips
+    return out
 
 
 def engine_times(fi, iters):
@@ -140,6 +151,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--iters", type=int, default=10, help="calls of --images images per mode and round")
     ap.add_argument("--images", type=int, default=16)
+    ap.add_argument("--align", type=int, default=None, help="chip side: also time FaceAnaImages(align=SIZE)")
     a = ap.parse_args()
     import logging
     import torch
@@ -158,24 +170,34 @@ def main():
         faces = sum(len(r) for r in fi.run_batch(imgs))
         faces_fit = sum(len(r) for r in fi.run_batch(fit)) if fit else 0
         up = upload_bytes(fi, imgs)
+        fis = {"": fi}
+        if a.align is not None:
+            fis["_align"] = FaceAnaImages(top_k=top_k, align=a.align)
+            up_align = upload_bytes(fis["_align"], imgs)
+            outs_align = [fis["_align"].new_results(B), fis["_align"].new_results(B)]
         # warm every mode once
-        in_flight(fi, imgs, 2)
-        in_flight(fi, dev, 2)
-        in_flight(fi, dev, 2, outs)
+        for suffix, f in fis.items():
+            o = outs if not suffix else outs_align
+            in_flight(f, imgs, 2)
+            in_flight(f, dev, 2)
+            in_flight(f, dev, 2, o)
         per_image(fa, imgs, 1)
         if fit:
             streams(fs, fit, 1)
         engine_times(fi, 3)
         n_one = max(1, a.iters // 5)
-        secs = {m: [] for m in ("faceana", "streams", "host", "cuda", "out")}
+        secs = {m + x: [] for m in ("faceana", "streams", "host", "cuda", "out") for x in fis
+                if not x or m in ("host", "cuda", "out")}
         eng = []
         for _ in range(a.rounds):
             secs["faceana"].append(per_image(fa, imgs, n_one) / n_one)
             if fit:
                 secs["streams"].append(streams(fs, fit, a.iters) / a.iters)
-            secs["host"].append(in_flight(fi, imgs, a.iters) / a.iters)
-            secs["cuda"].append(in_flight(fi, dev, a.iters) / a.iters)
-            secs["out"].append(in_flight(fi, dev, a.iters, outs) / a.iters)
+            for suffix, f in fis.items():
+                o = outs if not suffix else outs_align
+                secs["host" + suffix].append(in_flight(f, imgs, a.iters) / a.iters)
+                secs["cuda" + suffix].append(in_flight(f, dev, a.iters) / a.iters)
+                secs["out" + suffix].append(in_flight(f, dev, a.iters, o) / a.iters)
             eng.append(engine_times(fi, a.iters))
         det_ms, kps_ms = (float(np.median([e[i] for e in eng])) for i in range(2))
         engine_ms = B * det_ms + faces * kps_ms
@@ -189,15 +211,15 @@ def main():
                  "faces_per_s": n_face / ms * 1e3}
             if m == "streams":
                 r["skipped_images"] = B - len(fit)
-            if m in ("host", "cuda", "out"):
+            if m.split("_")[0] in ("host", "cuda", "out"):
                 r["call_over_engine_time"] = ms / engine_ms
-            if m in ("host", "faceana"):
-                r["host_upload_bytes_per_call"] = up if m == "host" else up["whole_images"]
+            if m in ("host", "host_align", "faceana"):
+                r["host_upload_bytes_per_call"] = {"host": up, "faceana": up["whole_images"]}.get(m) or up_align
             print(json.dumps(r), flush=True)
         print(json.dumps({"workload": name, "mode": "engines", "detector_ms_per_frame": det_ms,
                           "landmark_ms_per_face": kps_ms, "engine_ms_per_call": engine_ms,
                           "images_per_s": B / engine_ms * 1e3, "faces_per_s": faces / engine_ms * 1e3}), flush=True)
-        del fi, fa, fs, dev, outs
+        del fi, fa, fs, dev, outs, fis
         torch.cuda.empty_cache()
     print(json.dumps({"card": card()}), flush=True)
 

@@ -5,7 +5,10 @@
   (c) host     FaceLandmark.submit / collect on host 1024x1024 frames with one face each, through the rectangle upload;
                with the bytes uploaded per face beside the whole frame's
 
-    python tools/bench_landmarks.py [--max-faces 256] [--calls 40] [--warmup 5]
+  With --align SIZE, (b) and (c) also run on FaceLandmark(align=SIZE), alternated with the runs without it, and the
+  host upload per face counts the chip's rectangle (chip_read_rects) as well.
+
+    python tools/bench_landmarks.py [--max-faces 256] [--calls 40] [--warmup 5] [--align SIZE]
 Prints one JSON line; the card's name and power limit are part of it."""
 import argparse
 import json
@@ -69,6 +72,7 @@ def main():
     ap.add_argument("--max-faces", type=int, default=256)
     ap.add_argument("--calls", type=int, default=40)
     ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--align", type=int, default=None, help="chip side: also time FaceLandmark(align=SIZE)")
     args = ap.parse_args()
     import torch
     import frames
@@ -107,6 +111,24 @@ def main():
            "engine_faces_per_s": K / t_a, "device_faces_per_s": 4 * n_frames / t_b, "host_faces_per_s": K / t_c,
            "device_vs_engine": (4 * n_frames / t_b) / (K / t_a),
            "host_upload_bytes_per_face": roi, "whole_frame_bytes": 1024 * 1024 * 3}
+    if args.align is not None:
+        from peppa_pig_face_landmark_b200.core.api.align import chip_read_rects
+        fl_al = FaceLandmark(max_faces=K, align=args.align)
+        bufs_al = [fl_al.new_results(4 * n_frames) for _ in range(2)]
+        calls_b_al = [c[:2] + (bufs_al[i],) for i, c in enumerate(calls_b)]
+        # alternated: without, with, without, with
+        t = {"b": [t_b], "c": [t_c], "b_al": [], "c_al": []}
+        for _ in range(2):
+            t["b_al"].append(pipelined(fl_al, calls_b_al, args.calls, args.warmup))
+            t["c_al"].append(pipelined(fl_al, calls_c, args.calls, args.warmup))
+            t["b"].append(pipelined(fl, calls_b, args.calls, args.warmup))
+            t["c"].append(pipelined(fl, calls_c, args.calls, args.warmup))
+        med = {k: float(np.median(v)) for k, v in t.items()}
+        M = fl_al.run_batch([host[0]], [hb])[0][3]
+        c = chip_read_rects(M, args.align, 1024, 1024)[0]
+        res.update({"align": args.align, "device_faces_per_s": 4 * n_frames / med["b"], "host_faces_per_s": K / med["c"],
+                    "device_align_faces_per_s": 4 * n_frames / med["b_al"], "host_align_faces_per_s": K / med["c_al"],
+                    "host_align_upload_bytes_per_face": roi + int((c[2] - c[0]) * (c[3] - c[1]) * 3)})
     print(json.dumps(res))
 
 
