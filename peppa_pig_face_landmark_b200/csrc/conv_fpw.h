@@ -12,7 +12,7 @@ namespace skps {
 
 struct FpwK {
     XfProducer a;                                   // the A producer (no edge tiles: H % 8 == W % 16 == 0)
-    int units;                                      // work units of the launch: batch * tiles_per_img * nsplit
+    int units;                                      // work items of the launch: batch * tiles_per_img * nsplit (/ 2 paired)
     int nsplit;                                     // work units per tile: ceil(N tile / unit width)
     int bs, out_bufs;                               // ring depths: B tiles, epilogue staging buffers
     // epilogue: act(fmaf(acc, out_scale, bias) [+ res]) as in conv_xf
@@ -26,6 +26,7 @@ struct FpwLayer {
     CUtensorMap src0, src1_hi, src1_lo, b_hi, b_lo, o_hi, o_lo, w_eff;
     FpwK k;
     int mode = 0, n = 0, act = 0, out_fmt = 0;      // n: output channels per work unit (the kernel's N)
+    bool pair = false;                              // on conv_fpw_pair: work items of two units sharing each A tile
     int smem_bytes = 0;
 };
 

@@ -109,11 +109,12 @@ __device__ __forceinline__ XfSmem xf_smem(const uint8_t* smem_raw, const XfProdu
     return s;
 }
 
-// CTA set-up: tensor-map prefetch, mbarrier rings, the layer's depthwise weights.  Ends in __syncthreads.
+// CTA set-up: tensor-map prefetch, mbarrier rings, the layer's depthwise weights.  Ends in __syncthreads.  mma_warps: the
+// warps that read each A and B slot and release it (one MMA warpgroup, or two sharing every slot); nthreads: the CTA's.
 template <int MODE>
 __device__ __forceinline__ void xf_cta_init(const XfProducer& p, XfBarriers& bar, const XfSmem& sm, uint8_t* smem_raw,
                                             const CUtensorMap* tm0, const CUtensorMap* tm1_hi, const CUtensorMap* tmB_hi,
-                                            const CUtensorMap* tmB_lo) {
+                                            const CUtensorMap* tmB_lo, int mma_warps = 4, int nthreads = XF_THREADS) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (warp == 0 && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(tm0) : "memory");
@@ -127,16 +128,16 @@ __device__ __forceinline__ void xf_cta_init(const XfProducer& p, XfBarriers& bar
             mbar_init(smem_u32(&bar.raw_empty[s]), p.halves ? 4 : 8);   // one arrival per warp that consumes the slot
             mbar_init(smem_u32(&bar.a_raw[s]), 1);
             mbar_init(smem_u32(&bar.a_full[s]), 8);
-            mbar_init(smem_u32(&bar.a_empty[s]), 4);              // one arrival per MMA warp
+            mbar_init(smem_u32(&bar.a_empty[s]), mma_warps);      // one arrival per MMA warp
             mbar_init(smem_u32(&bar.b_full[s]), 1);
-            mbar_init(smem_u32(&bar.b_empty[s]), 4);
+            mbar_init(smem_u32(&bar.b_empty[s]), mma_warps);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     if (MODE == XF_DW) {
         // depthwise weights + bias of the whole layer stay in shared memory for the life of the (persistent) CTA
         float* dws = reinterpret_cast<float*>(smem_raw + (sm.w_off - smem_u32(smem_raw)));
-        for (int i = threadIdx.x; i < 10 * p.cchunks * 64; i += XF_THREADS) dws[i] = __ldg(p.dww + i);
+        for (int i = threadIdx.x; i < 10 * p.cchunks * 64; i += nthreads) dws[i] = __ldg(p.dww + i);
     }
     __syncthreads();
 }
