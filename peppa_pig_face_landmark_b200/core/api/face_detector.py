@@ -21,10 +21,9 @@ import numpy as np
 from ... import runtime as rt
 from ...graph_tools import detector_onnx_for
 from ...logger.logger import logger
-from .device_frames import check_cuda_frame, check_host_frame, is_cuda_tensor, is_tensor
+from .device_frames import check_host_frame
 from .onnx_model_base import ONNXEngine
-
-MAX_SIDE = 1 << 20         # largest frame side submit takes: keeps every row pitch in int32
+from .staging import Staging, check_frames, check_out, new_buffers, pad16
 
 # skps_det_src of include/skps_b200.h
 DET_SRC = np.dtype([("base", "<u8"), ("pitch", "<i4"), ("H", "<i4"), ("W", "<i4"), ("rw", "<i4"), ("rh", "<i4"),
@@ -63,15 +62,10 @@ def host_upload_rows(H, rh):
     return letterbox_rows(H, rh) if 2 * rh < H else None
 
 
-def _grow(t, n, make):
-    """t when it holds n elements, else make(max(n, 2 * len(t)))."""
-    if t is not None and t.shape[0] >= n:
-        return t
-    return make(max(n, 0 if t is None else 2 * t.shape[0], 1))
-
-
-def _pad16(n):
-    return (n + 15) // 16 * 16
+def result_fields(n_frames, rows):
+    """{name: (shape, dtype name)} of new_results(n_frames) of a detector with `rows` rows."""
+    return {"rows": ((n_frames, rows, 16), "float32"), "idx": ((n_frames, rows), "int32"),
+            "count": ((n_frames,), "int32")}
 
 
 class FaceDetector:
@@ -118,11 +112,11 @@ class FaceDetector:
         """face_detector.py:45-71: returns ((1,3,H,W) float32 RGB/255, [scale, left, top])."""
         if self._pending:
             raise RuntimeError("FaceDetector: %d calls in flight; collect() them first" % len(self._pending))
-        image = check_host_frame(image)
-        h, w = image.shape[:2]
+        call = check_frames([check_host_frame(image)], self.device)
+        layout = self._layout(call)
+        scale, _, _, top, left = layout[0][3]
         in_h, in_w = self.input_size[0], self.input_size[1]
-        scale, rw, rh, top, left = letterbox_geometry(h, w, in_h, in_w)
-        st = self._enqueue([image], None, detect=False)
+        st = self._enqueue(call, layout, None, detect=False)
         st["done"].synchronize()
         u8 = np.empty((in_h, in_w, 3), np.uint8)
         rt.check(self.lib.skps_engine_read_buffer(self.model.handle, self.model.plan.input.buf.idx, 1, u8.ctypes.data))
@@ -151,11 +145,8 @@ class FaceDetector:
         """Device result buffers for submit(cuda_frames, out=...) of up to n_frames frames: a dict of CUDA tensors on
         this object's device, rows (n, R, 16) float32, idx (n, R) int32 and count (n,) int32, where R is the detector's
         row count (15120 at 384x640): frame i keeps rows[i, :count[i]], the detector rows idx[i, :count[i]]."""
-        torch = rt.require_cuda()
-        n, R = int(n_frames), self._rows
-        return {"rows": torch.empty((n, R, 16), dtype=torch.float32, device=self.device),
-                "idx": torch.empty((n, R), dtype=torch.int32, device=self.device),
-                "count": torch.empty((n,), dtype=torch.int32, device=self.device)}
+        rt.require_cuda()
+        return new_buffers(result_fields(int(n_frames), self._rows), self.device)
 
     def submit(self, frames, out=None):
         """Enqueue the detector on frames; at most two calls may be in flight and collect() returns them in submission
@@ -173,14 +164,16 @@ class FaceDetector:
         GPU."""
         if len(self._pending) == 2:
             raise RuntimeError("FaceDetector: two calls already in flight; call collect() first")
-        frames = list(frames)
+        call = check_frames(frames, self.device)
+        layout = self._layout(call)
+        n = len(call.frames)
         if out is not None:
-            if not (frames and all(is_cuda_tensor(f) for f in frames)):
+            if not call.cuda:
                 raise ValueError("out= keeps results on the GPU and takes CUDA frames")
-            self._check_out(out, len(frames))
+            check_out(out, result_fields(n, self._rows), self.device, [p[2] for p in self._pending])
         slot = self._next
-        self._enqueue(frames, out, detect=True)
-        self._pending.append((slot, len(frames), out))
+        self._enqueue(call, layout, out, detect=True)
+        self._pending.append((slot, n, out))
 
     def collect(self):
         """Results of the oldest call in flight: a list with one (k_i, 16) float32 numpy array per frame, and
@@ -212,61 +205,42 @@ class FaceDetector:
         return res
 
     # ------------------------------------------------------------------
-    def _layout(self, frames):
-        """Checks every frame; [(H, W, row pitch, geometry, rows uploaded or None)] and whether they are CUDA frames."""
-        on_dev = [is_cuda_tensor(f) for f in frames]
-        cuda = bool(on_dev) and all(on_dev)
-        if any(on_dev) and not cuda:
-            raise ValueError("one call takes either host frames or CUDA frames, got both (frames %s are CUDA)"
-                             % [i for i, d in enumerate(on_dev) if d])
-        if cuda:
-            shapes = [check_cuda_frame(f, self.device, (MAX_SIDE, MAX_SIDE)) for f in frames]
-        else:
-            frames = [check_host_frame(f) for f in frames]
-            shapes = [(f.shape[0], f.shape[1], 3 * f.shape[1]) for f in frames]
+    def _layout(self, call):
+        """[(H, W, row pitch, letterbox geometry, rows uploaded or None)] of the frames of a call checked by
+        check_frames; ValueError for a frame whose letterbox is empty."""
         in_h, in_w = self.input_size[0], self.input_size[1]
         layout = []
-        for H, W, pitch in shapes:
-            if not (0 < H <= MAX_SIDE and 0 < W <= MAX_SIDE):
-                raise ValueError("frame %dx%d: sides must be in 1..%d" % (H, W, MAX_SIDE))
+        for H, W, pitch in call.shapes:
             geo = letterbox_geometry(H, W, in_h, in_w)
             if geo[1] < 1 or geo[2] < 1:
                 raise ValueError("frame %dx%d: its letterbox at %dx%d is %dx%d, empty" % (H, W, in_h, in_w, geo[2], geo[1]))
-            layout.append((H, W, pitch, geo, None if cuda else host_upload_rows(H, geo[2])))
-        return frames, layout, cuda
+            layout.append((H, W, pitch, geo, None if call.cuda else host_upload_rows(H, geo[2])))
+        return layout
 
-    def _enqueue(self, frames, out, detect, checked=None):
-        """Stages the frames into the next slot and enqueues letterbox (and, with detect, network, NMS and the copy back
-        of host results) on the engine's stream; returns the slot.  out: None, or result buffers of new_results(n) the
-        kept rows go to, for host frames as well as CUDA frames (FaceAnaImages keeps them on the GPU); nothing is then
-        copied back.  checked: what _layout(frames) returned, when the caller has checked the frames already."""
+    def _enqueue(self, call, layout, out, detect):
+        """Stages a checked call (check_frames, _layout) into the next slot and enqueues letterbox (and, with detect,
+        network, NMS and the copy back of host results) on the engine's stream; returns the slot.  out: None, or result
+        buffers of new_results(n) the kept rows go to, for host frames as well as CUDA frames (FaceAnaImages keeps them
+        on the GPU); nothing is then copied back."""
         torch = rt.require_cuda()
-        frames, layout, cuda = self._layout(frames) if checked is None else checked
+        frames, cuda = call.frames, call.cuda
         n, R, M = len(frames), self._rows, min(self.MAX_DET, self._rows)
         if self._slots is None:
             self._slots = [self._new_slot() for _ in range(2)]
         slot = self._next
         st = self._slots[slot]
-        rec_off = _pad16(n * DET_SRC.itemsize)
-        frame_off = rec_off + _pad16(n * 12)
-        sizes = [0 if cuda else _pad16((H if rows is None else len(rows)) * pitch) for H, W, pitch, geo, rows in layout]
+        rec_off = pad16(n * DET_SRC.itemsize)
+        frame_off = rec_off + pad16(n * 12)
+        sizes = [0 if cuda else pad16((H if rows is None else len(rows)) * pitch) for H, W, pitch, geo, rows in layout]
         total = frame_off + sum(sizes)
         own = detect and out is None                  # results go to the slot's buffers and come back to the host
-        if st["host"] is None or st["host"].shape[0] < total:
+        host, dev = st["stage"].reserve(total, st["done"])
+        if own and st["capacity"] < max(n, 1):
             st["done"].synchronize()                  # the slot's last call has finished with what is replaced
-            st["host"] = _grow(st["host"], total, lambda k: torch.empty((k,), dtype=torch.uint8).pin_memory())
-            st["dev"] = _grow(st["dev"], total, lambda k: torch.empty((k,), dtype=torch.uint8, device=self.device))
-        if own and (st["rows"] is None or st["rows"].shape[0] < n):
-            st["done"].synchronize()
-            st["rows"] = _grow(st["rows"], n, lambda k: torch.empty((k, R, 16), dtype=torch.float32, device=self.device))
-            st["idx"] = _grow(st["idx"], n, lambda k: torch.empty((k, R), dtype=torch.int32, device=self.device))
-            st["count"] = _grow(st["count"], n, lambda k: torch.empty((k,), dtype=torch.int32, device=self.device))
-            st["hrows"] = _grow(st["hrows"], n, lambda k: torch.empty((k, M, 16), dtype=torch.float32).pin_memory())
-            st["hidx"] = _grow(st["hidx"], n, lambda k: torch.empty((k, M), dtype=torch.int32).pin_memory())
-            st["hcount"] = _grow(st["hcount"], n, lambda k: torch.empty((k,), dtype=torch.int32).pin_memory())
-        st["copied"].synchronize()                    # the slot's last upload has left the pinned staging
-        host = st["host"].numpy()
-        dev = st["dev"].data_ptr()
+            st["capacity"] = k = max(n, 2 * st["capacity"], 1)
+            st.update(new_buffers(result_fields(k, R), self.device))
+            # the first M kept rows of every frame come back with the counts
+            st.update({"h" + name: t.pin_memory() for name, t in new_buffers(result_fields(k, M), "cpu").items()})
         # host staging = [n frame descriptors | n (scale, left, top) | the host frames' rows], sent with one copy
         desc = host[:n * DET_SRC.itemsize].view(DET_SRC)
         rec = host[rec_off:rec_off + 12 * n].view(np.float32).reshape(n, 3)
@@ -287,15 +261,10 @@ class FaceDetector:
                         mode="clip")
             at += nb
 
-        s, cp = self.model.stream, st["copy"]
-        sent = frame_off if cuda else total
-        if sent:
-            cp.wait_event(st["done"])                 # the slot's last call has read its device staging (NMS reads recover)
-            with torch.cuda.stream(cp):
-                st["dev"][:sent].copy_(st["host"][:sent], non_blocking=True)
-        st["copied"].record(cp)
+        s = self.model.stream
+        st["stage"].send(frame_off if cuda else total, st["done"])     # NMS reads the recoveries from the staging
         s.wait_stream(torch.cuda.current_stream(self.device))
-        s.wait_event(st["copied"])
+        s.wait_event(st["stage"].copied)
         res = out if out is not None else st
         rows_t, idx_t, count_t = res["rows"], res["idx"], res["count"]
         K = self.max_frames
@@ -329,22 +298,5 @@ class FaceDetector:
 
     def _new_slot(self):
         import torch
-        ev = {name: torch.cuda.Event() for name in ("copied", "read", "done")}
-        return dict(copy=torch.cuda.Stream(device=self.device), host=None, dev=None, rows=None, idx=None, count=None,
-                    hrows=None, hidx=None, hcount=None, **ev)
-
-    def _check_out(self, out, n):
-        import torch
-        R = self._rows
-        if not isinstance(out, dict) or set(out) != {"rows", "idx", "count"}:
-            raise ValueError("out: expected a dict with keys ['count', 'idx', 'rows'] (see new_results())")
-        for k, dt, tail in (("rows", torch.float32, (R, 16)), ("idx", torch.int32, (R,)), ("count", torch.int32, ())):
-            t = out[k]
-            if (not isinstance(t, torch.Tensor) or t.dtype != dt or t.device != self.device or not t.is_contiguous()
-                    or t.dim() != 1 + len(tail) or tuple(t.shape[1:]) != tail or t.shape[0] < n):
-                got = ("%s %s on %s" % (t.dtype, tuple(t.shape), t.device)) if is_tensor(t) else type(t).__name__
-                raise ValueError("out[%r]: expected a contiguous %s tensor (>= %d%s) on %s, got %s"
-                                 % (k, dt, n, "".join(", %d" % v for v in tail), self.device, got))
-        busy = {t.data_ptr() for _, _, o in self._pending if o is not None for t in o.values()}
-        if any(t.data_ptr() in busy for t in out.values()):
-            raise ValueError("out: these buffers belong to a call still in flight; collect() it first")
+        return dict(stage=Staging(self.device), capacity=0, rows=None, idx=None, count=None, read=torch.cuda.Event(),
+                    done=torch.cuda.Event())

@@ -26,11 +26,11 @@ import numpy as np
 from ... import runtime as rt
 from ...logger.logger import logger
 from .align import check_size, chip_read_rects
-from .device_frames import check_cuda_frame, check_host_frame, is_cuda_tensor, is_tensor
+from .device_frames import is_cuda_tensor
 from .onnx_model_base import ONNXEngine
+from .staging import Staging, check_frames, check_out, grow, new_buffers, pad16
 
 MIN_FACE = 20              # face_landmark.py:26,76: boxes with a side of at most this many pixels get no landmarks
-MAX_SIDE = 1 << 20         # largest frame side run_batch takes: keeps every crop coordinate in int32
 BOX_LIMIT = 2.0 ** 24      # largest |box coordinate| of host boxes: the host and device crop geometry stay exact in int32
 
 # skps_face_src of include/skps_b200.h
@@ -73,11 +73,35 @@ def crop_read_rects(boxes, H, W, face_scale, min_face=MIN_FACE):
     return out
 
 
-def _grow(t, n, make):
-    """t when it holds n elements, else make(max(n, 2 * len(t)))."""
-    if t is not None and t.shape[0] >= n:
-        return t
-    return make(max(n, 0 if t is None else 2 * t.shape[0], 1))
+def result_fields(n_faces, n_points, align=None):
+    """{name: (shape, dtype name)} of new_results(n_faces) of FaceLandmark(align=align) with n_points landmarks."""
+    f = {"kps": ((n_faces, n_points, 2), "float32"), "scores": ((n_faces, n_points), "float32")}
+    if align is not None:
+        f.update({"chip": ((n_faces, align, align, 3), "uint8"), "M": ((n_faces, 2, 3), "float64")})
+    return f
+
+
+def _rect_bytes(rects):
+    """Bytes of the BGR pixels of each [x0, y0, x1, y1) rectangle of rects (n, 4)."""
+    return (rects[:, 2] - rects[:, 0]) * (rects[:, 3] - rects[:, 1]) * 3
+
+
+def _gather_rects(frames, rects, image, host, at, dev):
+    """Stages the parts of host frames that kernels read through FACE_SRC descriptors: rectangle j, rects[j] of
+    frames[image[j]], goes into the pinned staging `host` from byte `at` on, one after the other, and descriptor j at the
+    start of `host` points at it in the device copy of the staging at address `dev`."""
+    nb = _rect_bytes(rects)
+    starts = at + np.cumsum(nb) - nb
+    rw, rh = rects[:, 2] - rects[:, 0], rects[:, 3] - rects[:, 1]
+    hw = np.array([f.shape[:2] for f in frames], np.int64)[image]
+    desc = host[:len(rects) * FACE_SRC.itemsize].view(FACE_SRC)
+    desc["H"], desc["W"], desc["_pad"] = hw[:, 0], hw[:, 1], 0
+    desc["base"], desc["pitch"] = dev + starts, 3 * rw
+    desc["ox"], desc["oy"], desc["rw"], desc["rh"] = rects[:, 0], rects[:, 1], rw, rh
+    for j in np.flatnonzero(nb):
+        x0, y0, x1, y1 = (int(v) for v in rects[j])
+        host[starts[j]:starts[j] + nb[j]].reshape(y1 - y0, 3 * (x1 - x0))[:] = \
+            frames[image[j]][y0:y1, x0:x1].reshape(y1 - y0, 3 * (x1 - x0))
 
 
 class FaceLandmark:
@@ -115,9 +139,9 @@ class FaceLandmark:
         self._detail = torch.zeros((K, 5), dtype=torch.int32, device=self.device)
         self.last_detail = None
         self._slots = None            # staging of the batched path, made on first use
-        self._pending = []            # [(slot, faces per frame, out or None, host frames to align or None)]
+        self._pending = []            # [(slot, faces per frame, out or None, checked host frames to align or None)]
         self._next = 0
-        self._chip_stage = None       # staging of the host frames' chip rectangles, made on first use
+        self._chip_stage = None       # (Staging, done event) of the host frames' chip rectangles, made on first use
 
     def crops(self, img, bboxes):
         """The (K,S,S,3) uint8 crops the network sees (face_landmark.py:66-104), for parity tests."""
@@ -171,17 +195,11 @@ class FaceLandmark:
         """Device result buffers for submit(cuda_frames, boxes, out=...) of up to n_faces faces: a dict of CUDA tensors
         on this object's device, kps (n_faces, 98, 2) and scores (n_faces, 98) float32; with align also chip
         (n_faces, s, s, 3) uint8 and M (n_faces, 2, 3) float64."""
-        torch = rt.require_cuda()
-        return {k: torch.empty((int(n_faces),) + tail, dtype=getattr(torch, dt), device=self.device)
-                for k, (tail, dt) in self._out_fields().items()}
+        rt.require_cuda()
+        return new_buffers(self._fields(int(n_faces)), self.device)
 
-    def _out_fields(self):
-        """{name: (shape of one face, dtype name)} of new_results."""
-        P, A = self.keypoints_num, self.align
-        f = {"kps": ((P, 2), "float32"), "scores": ((P,), "float32")}
-        if A is not None:
-            f.update({"chip": ((A, A, 3), "uint8"), "M": ((2, 3), "float64")})
-        return f
+    def _fields(self, n_faces):
+        return result_fields(n_faces, self.keypoints_num, self.align)
 
     def submit(self, frames, boxes, out=None):
         """Enqueue landmarks for boxes[i] on frames[i]; at most two calls may be in flight and collect() returns them in
@@ -205,129 +223,88 @@ class FaceLandmark:
         collect() returns."""
         if len(self._pending) == 2:
             raise RuntimeError("FaceLandmark: two calls already in flight; call collect() first")
-        checked = self._check_call(frames, boxes)
+        call = check_frames(frames, self.device)
+        boxes, cuda_boxes = self._check_boxes(call, boxes)
+        counts = [int(b.shape[0]) for b in boxes]
         if out is not None:
-            if not checked[3]:
+            if not call.cuda:
                 raise ValueError("out= keeps results on the GPU and takes CUDA frames; these are host frames")
-            self._check_out(out, sum(checked[5]))
-        slot = self._enqueue(checked, out)
-        align_host = self.align is not None and not checked[3]
-        self._pending.append((slot, checked[5], out, (checked[0], checked[2]) if align_host else None))
+            check_out(out, self._fields(sum(counts)), self.device, [p[2] for p in self._pending])
+        slot = self._enqueue(call, boxes, cuda_boxes, out)
+        align_host = self.align is not None and not call.cuda
+        self._pending.append((slot, counts, out, call if align_host else None))
 
-    def _enqueue_to(self, frames, boxes, out):
-        """submit() with results left in out (a new_results(n) dict) for host frames as well as CUDA frames, and not
-        counted as a call in flight: FaceAnaImages orders its own work after it on the engine's stream.  Returns the
-        faces per frame."""
-        checked = self._check_call(frames, boxes)
-        self._check_out(out, sum(checked[5]))
-        self._enqueue(checked, out)
-        return checked[5]
-
-    def _check_call(self, frames, boxes):
-        """Checks the frames and boxes of a call: (frames, boxes, layout, cuda frames, cuda boxes, faces per frame)."""
-        frames, boxes = list(frames), list(boxes)
-        if len(frames) != len(boxes):
-            raise ValueError("%d frames but %d box arrays" % (len(frames), len(boxes)))
-        on_dev = [is_cuda_tensor(f) for f in frames]
-        cuda = bool(on_dev) and all(on_dev)
-        if any(on_dev) and not cuda:
-            raise ValueError("one call takes either host frames or CUDA frames, got both (frames %s are CUDA)"
-                             % [i for i, d in enumerate(on_dev) if d])
-        if cuda:
-            layout = [check_cuda_frame(f, self.device, (MAX_SIDE, MAX_SIDE)) for f in frames]
-        else:
-            frames = [check_host_frame(f) for f in frames]
-            layout = [(f.shape[0], f.shape[1], 3 * f.shape[1]) for f in frames]
-        for H, W, _ in layout:
-            if not (0 < H <= MAX_SIDE and 0 < W <= MAX_SIDE):
-                raise ValueError("frame %dx%d: sides must be in 1..%d" % (H, W, MAX_SIDE))
+    def _check_boxes(self, call, boxes):
+        """Checks the boxes of a call whose frames check_frames has checked: (boxes, whether they are CUDA tensors)."""
+        boxes = list(boxes)
+        if len(call.frames) != len(boxes):
+            raise ValueError("%d frames but %d box arrays" % (len(call.frames), len(boxes)))
         box_dev = [is_cuda_tensor(b) for b in boxes]
         cuda_boxes = bool(box_dev) and all(box_dev)
         if any(box_dev) and not cuda_boxes:
             raise ValueError("boxes are either all host arrays or all CUDA tensors (boxes %s are CUDA)"
                              % [i for i, d in enumerate(box_dev) if d])
-        if cuda_boxes and not cuda:
+        if cuda_boxes and not call.cuda:
             raise ValueError("CUDA boxes take CUDA frames: the host frames' upload is cut to the boxes on the host")
-        boxes = [self._check_cuda_boxes(b, i) if cuda_boxes else self._check_host_boxes(b, i) for i, b in enumerate(boxes)]
-        counts = [int(b.shape[0]) for b in boxes]
-        return frames, boxes, layout, cuda, cuda_boxes, counts
+        check = self._check_cuda_boxes if cuda_boxes else self._check_host_boxes
+        return [check(b, i) for i, b in enumerate(boxes)], cuda_boxes
 
-    def _enqueue(self, checked, out):
-        """Stages a checked call into the next slot and enqueues crops, network and post-processing (and, without out,
-        the copy back) on the engine's stream; returns the slot."""
+    def _enqueue(self, call, boxes, cuda_boxes, out):
+        """Stages a call checked by check_frames and _check_boxes into the next slot and enqueues crops, network and
+        post-processing (and, without out, the copy back) on the engine's stream; returns the slot.  out: None, or
+        result buffers of new_results(n) the results go to, for host frames as well as CUDA frames (FaceAnaImages keeps
+        them on the GPU)."""
         torch = rt.require_cuda()
-        frames, boxes, layout, cuda, cuda_boxes, counts = checked
-        n = sum(counts)
-        P = self.keypoints_num
+        counts = [int(b.shape[0]) for b in boxes]
+        n, P, A = sum(counts), self.keypoints_num, self.align
         if self._slots is None:
             self._slots = [self._new_slot() for _ in range(2)]
         slot = self._next
         st = self._slots[slot]
-        A = self.align
-        warp_now = A is not None and cuda          # CUDA frames are warped here, host frames at collect()
-        rects = None if cuda else [crop_read_rects(b, H, W, self.face_scale, self.min_face)
-                                   for b, (H, W, _) in zip(boxes, layout)]
-        roi_bytes = 0 if cuda else [(r[:, 2] - r[:, 0]) * (r[:, 3] - r[:, 1]) * 3 for r in rects]
-        box_off = (n * FACE_SRC.itemsize + 15) // 16 * 16
-        roi_off = box_off + (n * 16 + 15) // 16 * 16
-        total = roi_off + (0 if cuda else int(sum(int(r.sum()) for r in roi_bytes)))
+        warp_now = A is not None and call.cuda     # CUDA frames are warped here, host frames at collect()
+        image = np.repeat(np.arange(len(counts)), counts)
+        rects = None if call.cuda or n == 0 else np.concatenate(
+            [crop_read_rects(b, H, W, self.face_scale, self.min_face) for b, (H, W, _) in zip(boxes, call.shapes)])
+        box_off = pad16(n * FACE_SRC.itemsize)
+        roi_off = box_off + pad16(n * 16)
+        total = roi_off + (0 if rects is None else int(_rect_bytes(rects).sum()))
         sent = box_off if cuda_boxes else total       # bytes of the host staging the call sends
-        if (st["host"] is None or st["host"].shape[0] < total or st["kps"] is None or st["kps"].shape[0] < n):
+        host, dev = st["stage"].reserve(total, st["done"])
+        if st["kps"] is None or st["kps"].shape[0] < n:
             st["done"].synchronize()                  # the slot's last call has finished with what is replaced
-            st["host"] = _grow(st["host"], total, lambda k: torch.empty((k,), dtype=torch.uint8).pin_memory())
-            st["dev"] = _grow(st["dev"], total, lambda k: torch.empty((k,), dtype=torch.uint8, device=self.device))
-            st["kps"] = _grow(st["kps"], n, lambda k: torch.empty((k, P, 2), dtype=torch.float32, device=self.device))
-            st["scores"] = _grow(st["scores"], n, lambda k: torch.empty((k, P), dtype=torch.float32, device=self.device))
-            st["detail"] = _grow(st["detail"], n, lambda k: torch.empty((k, 5), dtype=torch.int32, device=self.device))
-            st["hkps"] = _grow(st["hkps"], n, lambda k: torch.empty((k, P, 2), dtype=torch.float32).pin_memory())
-            st["hscores"] = _grow(st["hscores"], n, lambda k: torch.empty((k, P), dtype=torch.float32).pin_memory())
-        if A is not None and out is None and (st["chips"] is None or st["chips"].shape[0] < n):
+            st["kps"] = grow(st["kps"], n, lambda k: torch.empty((k, P, 2), dtype=torch.float32, device=self.device))
+            st["scores"] = grow(st["scores"], n, lambda k: torch.empty((k, P), dtype=torch.float32, device=self.device))
+            st["detail"] = grow(st["detail"], n, lambda k: torch.empty((k, 5), dtype=torch.int32, device=self.device))
+            st["hkps"] = grow(st["hkps"], n, lambda k: torch.empty((k, P, 2), dtype=torch.float32).pin_memory())
+            st["hscores"] = grow(st["hscores"], n, lambda k: torch.empty((k, P), dtype=torch.float32).pin_memory())
+        if A is not None and out is None and (st["chip"] is None or st["chip"].shape[0] < n):
             st["done"].synchronize()
-            st["M"] = _grow(st["M"], n, lambda k: torch.empty((k, 2, 3), dtype=torch.float64, device=self.device))
-            st["hM"] = _grow(st["hM"], n, lambda k: torch.empty((k, 2, 3), dtype=torch.float64).pin_memory())
-            st["chips"] = _grow(st["chips"], n, lambda k: torch.empty((k, A, A, 3), dtype=torch.uint8, device=self.device))
-            st["hchips"] = _grow(st["hchips"], n, lambda k: torch.empty((k, A, A, 3), dtype=torch.uint8).pin_memory())
-        st["copied"].synchronize()                    # the slot's last upload has left the pinned staging
-        host = st["host"].numpy()
-        dev = st["dev"].data_ptr()
+            st["M"] = grow(st["M"], n, lambda k: torch.empty((k, 2, 3), dtype=torch.float64, device=self.device))
+            st["hM"] = grow(st["hM"], n, lambda k: torch.empty((k, 2, 3), dtype=torch.float64).pin_memory())
+            st["chip"] = grow(st["chip"], n, lambda k: torch.empty((k, A, A, 3), dtype=torch.uint8, device=self.device))
+            st["hchip"] = grow(st["hchip"], n, lambda k: torch.empty((k, A, A, 3), dtype=torch.uint8).pin_memory())
         # host staging = [n face descriptors | n boxes | the host frames' rectangles], sent with one copy
-        desc = host[:n * FACE_SRC.itemsize].view(FACE_SRC)
-        o, at = 0, roi_off
-        for i, (f, (H, W, pitch), k) in enumerate(zip(frames, layout, counts)):
-            if k == 0:
-                continue
-            d = desc[o:o + k]
-            d["H"], d["W"], d["_pad"] = H, W, 0
-            if not cuda_boxes:
-                host[box_off + 16 * o:box_off + 16 * (o + k)].view(np.float32).reshape(k, 4)[:] = boxes[i]
-            if cuda:
-                d["base"], d["pitch"], d["ox"], d["oy"], d["rw"], d["rh"] = f.data_ptr(), pitch, 0, 0, W, H
-            else:
-                r, nb = rects[i], roi_bytes[i]
-                starts = at + np.concatenate(([0], np.cumsum(nb)[:-1]))
-                rw, rh = r[:, 2] - r[:, 0], r[:, 3] - r[:, 1]
-                d["base"], d["pitch"], d["ox"], d["oy"], d["rw"], d["rh"] = dev + starts, 3 * rw, r[:, 0], r[:, 1], rw, rh
-                for j in np.flatnonzero(nb):
-                    x0, y0, x1, y1 = (int(v) for v in r[j])
-                    host[starts[j]:starts[j] + nb[j]].reshape(y1 - y0, 3 * (x1 - x0))[:] = \
-                        f[y0:y1, x0:x1].reshape(y1 - y0, 3 * (x1 - x0))
-                at += int(nb.sum())
-            o += k
+        if n and not cuda_boxes:
+            host[box_off:box_off + 16 * n].view(np.float32).reshape(n, 4)[:] = np.concatenate(boxes)
+        if call.cuda:                                 # descriptors of the whole frames
+            desc = host[:n * FACE_SRC.itemsize].view(FACE_SRC)
+            H, W, pitch = np.array(call.shapes, np.int64)[image].T
+            desc["base"] = np.array([f.data_ptr() for f in call.frames], np.uint64)[image]
+            desc["pitch"], desc["H"], desc["W"], desc["rw"], desc["rh"] = pitch, H, W, W, H
+            desc["ox"], desc["oy"], desc["_pad"] = 0, 0, 0
+        elif n:
+            _gather_rects(call.frames, rects, image, host, roi_off, dev)
 
-        s, cp = self.model.stream, st["copy"]
-        if sent:
-            cp.wait_event(st["read"])                 # the slot's last crops have read its device staging
-            with torch.cuda.stream(cp):
-                st["dev"][:sent].copy_(st["host"][:sent], non_blocking=True)
-        st["copied"].record(cp)
+        s = self.model.stream
+        st["stage"].send(sent, st["read"])            # the slot's last crops have read its device staging
         s.wait_stream(torch.cuda.current_stream(self.device))
-        s.wait_event(st["copied"])
+        s.wait_event(st["stage"].copied)
         if cuda_boxes and n:
             with torch.cuda.stream(s):
-                dst = st["dev"][box_off:box_off + 16 * n].view(torch.float32).view(n, 4)
+                dst = st["stage"].dev[box_off:box_off + 16 * n].view(torch.float32).view(n, 4)
                 torch.cat([b[:, :4] for b in boxes if b.shape[0]], out=dst)
-        kps = out["kps"] if out is not None else st["kps"]
-        scores = out["scores"] if out is not None else st["scores"]
+        res = out if out is not None else st
+        kps, scores = res["kps"], res["scores"]
         K, S = self.max_faces, self.input_size[0]
         inp = self.model.input_ptr()
         det = st["detail"].data_ptr()
@@ -345,8 +322,7 @@ class FaceLandmark:
                 rt.check(self.lib.skps_landmark_post(self.model.output_ptr(0), det + 20 * c0, st["count"].data_ptr(), m,
                                                      P, kps.data_ptr() + 8 * P * c0, s.cuda_stream))
         if A is not None and n:
-            M = out["M"] if out is not None else st["M"]
-            chips = out["chip"] if out is not None else st["chips"]
+            M, chips = res["M"], res["chip"]
             with torch.cuda.device(self.device):
                 rt.check(self.lib.skps_align_estimate(kps.data_ptr(), n, P, A, M.data_ptr(), s.cuda_stream))
                 if warp_now:                          # the face descriptors hold the whole CUDA frames
@@ -356,12 +332,9 @@ class FaceLandmark:
         torch.cuda.current_stream(self.device).wait_event(st["read"])
         if out is None and n:
             with torch.cuda.stream(s):
-                st["hkps"][:n].copy_(kps[:n], non_blocking=True)
-                st["hscores"][:n].copy_(scores[:n], non_blocking=True)
-                if A is not None:
-                    st["hM"][:n].copy_(st["M"][:n], non_blocking=True)
-                    if warp_now:
-                        st["hchips"][:n].copy_(st["chips"][:n], non_blocking=True)
+                for k in self._fields(0):
+                    if k != "chip" or warp_now:       # host frames are warped at collect()
+                        st["h" + k][:n].copy_(st[k][:n], non_blocking=True)
         st["done"].record(s)
         self._next ^= 1
         return slot
@@ -373,9 +346,9 @@ class FaceLandmark:
         afterwards sees the results.  A call of host frames with align is warped here (see submit())."""
         if not self._pending:
             raise RuntimeError("FaceLandmark: nothing submitted")
-        slot, counts, out, host_frames = self._pending.pop(0)
+        slot, counts, out, host_call = self._pending.pop(0)
         st = self._slots[slot]
-        names = list(self._out_fields())
+        names = list(self._fields(0))
         if out is not None:
             import torch
             torch.cuda.current_stream(self.device).wait_event(st["done"])
@@ -383,9 +356,9 @@ class FaceLandmark:
         else:
             st["done"].synchronize()
             n = sum(counts)
-            if host_frames is not None and n:
-                self._warp_host_frames(*host_frames, counts, st["hM"].numpy()[:n], st["M"], st["chips"], st["hchips"])
-            arrays = [st[h].numpy() for h in ("hkps", "hscores", "hchips", "hM")[:len(names)]]
+            if host_call is not None and n:
+                self._warp_host_frames(host_call, counts, st["hM"].numpy()[:n], st["M"], st["chip"], st["hchip"])
+            arrays = [st["h" + k].numpy() for k in names]
         res, o = [], 0
         for k in counts:
             if out is None:
@@ -395,55 +368,38 @@ class FaceLandmark:
             o += k
         return res
 
-    def _warp_host_frames(self, frames, layout, counts, M, d_M, chips, h_chips):
-        """The chip phase of host frames (blocking): counts[i] faces of frames[i] (layout[i] = (H, W, pitch)), whose
-        matrices M (n, 2, 3) float64 are on the host and, equal, in d_M on the device.  Uploads the rectangle of each
-        frame that each chip reads (chip_read_rects) through pinned staging on a copy stream, warps chips[:n] on the
+    def _warp_host_frames(self, call, counts, M, d_M, chips, h_chips):
+        """The chip phase of host frames (blocking): counts[i] faces of call.frames[i] (a call checked by check_frames),
+        whose matrices M (n, 2, 3) float64 are on the host and, equal, in d_M on the device.  Uploads the rectangle of
+        each frame that each chip reads (chip_read_rects) through the chip stage's pinned staging, warps chips[:n] on the
         engine's stream, where no other kernel runs beside it, and copies them to the pinned h_chips[:n]."""
         torch = rt.require_cuda()
         n, A = len(M), self.align
         rects = np.concatenate([chip_read_rects(M[o:o + k], A, H, W) for o, k, (H, W, _)
-                                in zip(np.cumsum([0] + list(counts[:-1])), counts, layout)])
-        rw, rh = rects[:, 2] - rects[:, 0], rects[:, 3] - rects[:, 1]
-        nb = rw * rh * 3
-        roi_off = (n * FACE_SRC.itemsize + 15) // 16 * 16
-        total = roi_off + int(nb.sum())
-        cs = self._chip_stage
-        if cs is None:
-            cs = self._chip_stage = dict(copy=torch.cuda.Stream(device=self.device), host=None, dev=None,
-                                         copied=torch.cuda.Event(), done=torch.cuda.Event())
-        cs["host"] = _grow(cs["host"], total, lambda k: torch.empty((k,), dtype=torch.uint8).pin_memory())
-        cs["dev"] = _grow(cs["dev"], total, lambda k: torch.empty((k,), dtype=torch.uint8, device=self.device))
-        host, dev = cs["host"].numpy(), cs["dev"].data_ptr()
-        starts = roi_off + np.concatenate(([0], np.cumsum(nb)[:-1]))
-        desc = host[:n * FACE_SRC.itemsize].view(FACE_SRC)
-        img = np.repeat(np.arange(len(counts)), counts)
-        hw = np.array([l[:2] for l in layout], np.int64)[img]
-        desc["H"], desc["W"] = hw[:, 0], hw[:, 1]
-        desc["base"], desc["pitch"], desc["_pad"] = dev + starts, 3 * rw, 0
-        desc["ox"], desc["oy"], desc["rw"], desc["rh"] = rects[:, 0], rects[:, 1], rw, rh
-        for j in np.flatnonzero(nb):
-            x0, y0, x1, y1 = (int(v) for v in rects[j])
-            host[starts[j]:starts[j] + nb[j]].reshape(y1 - y0, 3 * (x1 - x0))[:] = \
-                frames[img[j]][y0:y1, x0:x1].reshape(y1 - y0, 3 * (x1 - x0))
-        s, cp = self.model.stream, cs["copy"]
-        with torch.cuda.stream(cp):
-            cs["dev"][:total].copy_(cs["host"][:total], non_blocking=True)
-        cs["copied"].record(cp)
-        s.wait_event(cs["copied"])
+                                in zip(np.cumsum([0] + list(counts[:-1])), counts, call.shapes)])
+        roi_off = pad16(n * FACE_SRC.itemsize)
+        total = roi_off + int(_rect_bytes(rects).sum())
+        if self._chip_stage is None:
+            self._chip_stage = (Staging(self.device), torch.cuda.Event())
+        cs, done = self._chip_stage
+        host, dev = cs.reserve(total, done)
+        _gather_rects(call.frames, rects, np.repeat(np.arange(len(counts)), counts), host, roi_off, dev)
+        s = self.model.stream
+        cs.send(total, done)
+        s.wait_event(cs.copied)
         with torch.cuda.device(self.device):
             rt.check(self.lib.skps_warp_faces(dev, d_M.data_ptr(), n, A, A, chips.data_ptr(), s.cuda_stream))
         with torch.cuda.stream(s):
             h_chips[:n].copy_(chips[:n], non_blocking=True)
-        cs["done"].record(s)
-        cs["done"].synchronize()                  # the staging is free again and h_chips holds the chips
+        done.record(s)
+        done.synchronize()                            # the staging is free again and h_chips holds the chips
 
     def _new_slot(self):
         import torch
-        ev = {name: torch.cuda.Event() for name in ("copied", "read", "done")}
-        return dict(copy=torch.cuda.Stream(device=self.device), host=None, dev=None, kps=None, scores=None, detail=None,
-                    hkps=None, hscores=None, M=None, hM=None, chips=None, hchips=None, count=torch.full((1,), self.max_faces, dtype=torch.int32, device=self.device),
-                    **ev)
+        return dict(stage=Staging(self.device), kps=None, scores=None, detail=None, hkps=None, hscores=None, M=None,
+                    hM=None, chip=None, hchip=None,
+                    count=torch.full((1,), self.max_faces, dtype=torch.int32, device=self.device),
+                    read=torch.cuda.Event(), done=torch.cuda.Event())
 
     @staticmethod
     def _check_host_boxes(b, i):
@@ -466,19 +422,3 @@ class FaceLandmark:
         if b.dim() != 2 or b.shape[1] < 4:
             raise ValueError("boxes[%d]: expected a (k, >= 4) tensor, got shape %s" % (i, tuple(b.shape)))
         return b
-
-    def _check_out(self, out, n):
-        import torch
-        fields = self._out_fields()
-        if not isinstance(out, dict) or set(out) != set(fields):
-            raise ValueError("out: expected a dict with keys %s (see new_results())" % sorted(fields))
-        for k, (tail, dt) in fields.items():
-            t = out[k]
-            if (not isinstance(t, torch.Tensor) or t.dtype != getattr(torch, dt) or t.device != self.device
-                    or not t.is_contiguous() or tuple(t.shape[1:]) != tail or t.shape[0] < n):
-                got = ("%s %s on %s" % (t.dtype, tuple(t.shape), t.device)) if is_tensor(t) else type(t).__name__
-                raise ValueError("out[%r]: expected a contiguous %s tensor (>= %d, %s) on %s, got %s"
-                                 % (k, dt, n, ", ".join(map(str, tail)), self.device, got))
-        busy = {t.data_ptr() for p in self._pending if p[2] is not None for t in p[2].values()}
-        if any(t.data_ptr() in busy for t in out.values()):
-            raise ValueError("out: these buffers belong to a call still in flight; collect() it first")

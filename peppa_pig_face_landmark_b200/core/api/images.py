@@ -24,10 +24,10 @@ import numpy as np
 from ... import runtime as rt
 from ...graph_tools import check_detector_input
 from .align import check_size
-from .device_frames import is_tensor
-from .face_detector import FaceDetector, _grow, _pad16
+from .face_detector import FaceDetector
 from .face_landmark import FaceLandmark
 from .facer import MAX_TOP_K, get_cfg
+from .staging import check_frames, check_out, grow, new_buffers, pad16
 
 POSE_FIELDS = (("rvec", (3,)), ("tvec", (3,)), ("euler", (3,)), ("reproject", (8, 2)))
 
@@ -51,24 +51,6 @@ def result_fields(n_images, top_k, n_points, pose, align=None):
     if pose:
         f.update({k: ((rows,) + tail, "float64") for k, tail in POSE_FIELDS})
     return f
-
-
-def check_results(out, n_images, top_k, n_points, pose, device, busy=(), align=None):
-    """ValueError unless out is a dict of result buffers (new_results) on `device` that holds a call of n_images images
-    and shares no buffer with `busy` (the buffers of calls still in flight)."""
-    import torch
-    want = result_fields(n_images, top_k, n_points, pose, align)
-    if not isinstance(out, dict) or set(out) != set(want):
-        raise ValueError("out: expected a dict with keys %s (see new_results())" % sorted(want))
-    for k, (shape, dt) in want.items():
-        t, dt = out[k], getattr(torch, dt)
-        if (not isinstance(t, torch.Tensor) or t.dtype != dt or t.device != device or not t.is_contiguous()
-                or t.dim() != len(shape) or tuple(t.shape[1:]) != shape[1:] or t.shape[0] < shape[0]):
-            got = ("%s %s on %s" % (t.dtype, tuple(t.shape), t.device)) if is_tensor(t) else type(t).__name__
-            raise ValueError("out[%r]: expected a contiguous %s tensor (>= %d%s) on %s, got %s"
-                             % (k, dt, shape[0], "".join(", %d" % v for v in shape[1:]), device, got))
-    if any(t.data_ptr() in set(busy) for t in out.values()):
-        raise ValueError("out: these buffers belong to a call still in flight; collect() it first")
 
 
 class FaceAnaImages:
@@ -131,10 +113,8 @@ class FaceAnaImages:
         tvec, euler (n*top_k, 3) and reproject (n*top_k, 8, 2) float64.  Faces are packed
         in image order, each image's in FaceAna's order: image i's are rows first[i] .. first[i] + count[i] - 1.  Rows
         past the call's faces are unspecified."""
-        torch = rt.require_cuda()
-        return {k: torch.empty(shape, dtype=getattr(torch, dt), device=self.device)
-                for k, (shape, dt) in result_fields(int(n_images), self.top_k, self.n_points, self.pose,
-                                                    self.align).items()}
+        rt.require_cuda()
+        return new_buffers(result_fields(int(n_images), self.top_k, self.n_points, self.pose, self.align), self.device)
 
     def submit(self, images, out=None):
         """Enqueue the analysis of images; at most two calls may be in flight and collect() returns them in submission
@@ -156,14 +136,15 @@ class FaceAnaImages:
         must stay unchanged until collect() returns."""
         if len(self._pending) == 2:
             raise RuntimeError("FaceAnaImages: two calls already in flight; call collect() first")
-        checked = self.detector._layout(list(images))
-        frames, _, cuda = checked
-        n = len(frames)
+        fd, fl = self.detector, self.landmark
+        call = check_frames(images, self.device)
+        layout = fd._layout(call)
+        n = len(call.frames)
         if out is not None:
-            if not (n and cuda):
+            if not call.cuda:
                 raise ValueError("out= keeps results on the GPU and takes CUDA images")
-            check_results(out, n, self.top_k, self.n_points, self.pose, self.device,
-                          [t.data_ptr() for p in self._pending if p[2] is not None for t in p[2].values()], self.align)
+            check_out(out, result_fields(n, self.top_k, self.n_points, self.pose, self.align), self.device,
+                      [p[2] for p in self._pending])
         if n == 0:
             self._pending.append((None, 0, None, None, None, None))
             return
@@ -173,25 +154,24 @@ class FaceAnaImages:
         slot = self._next
         st = self._slots[slot]
         K, P, lib = self.top_k, self.n_points, self.lib
-        fd, fl = self.detector, self.landmark
         ds, ls = fd.model.stream, fl.model.stream
 
         # 1. detector: every kept row of every image stays on the device
-        cpad = _pad16(n)
+        cpad = pad16(n)
         if st["det"] is None or st["det"]["count"].shape[0] < n:
             st["done"].synchronize()                  # the slot's last call has finished with what is replaced
             st["det"] = fd.new_results(max(n, 0 if st["det"] is None else 2 * st["det"]["count"].shape[0]))
         need = cpad + 4 * n * K
         if st["sel"] is None or st["sel"].shape[0] < need:
             st["done"].synchronize()
-            st["sel"] = _grow(st["sel"], need, lambda k: torch.empty((k,), dtype=torch.float32, device=self.device))
-            st["hsel"] = _grow(st["hsel"], need, lambda k: torch.empty((k,), dtype=torch.float32).pin_memory())
+            st["sel"] = grow(st["sel"], need, lambda k: torch.empty((k,), dtype=torch.float32, device=self.device))
+            st["hsel"] = grow(st["hsel"], need, lambda k: torch.empty((k,), dtype=torch.float32).pin_memory())
         # The detector starts after the previous call's landmark phase, so the two engines never run at the same time:
         # landmarks computed while the other engine ran on another stream have been seen to vary from run to run.  The
         # next call's host staging still overlaps the GPU work.  This also orders the slot's last reads of its boxes.
         ds.wait_event(self._slots[slot ^ 1]["done"])
         ds.wait_event(st["done"])
-        fd._enqueue(frames, st["det"], detect=True, checked=checked)
+        fd._enqueue(call, layout, st["det"], detect=True)
         # 2. face selection, all images in one launch; 3. the call's one read-back: counts and selected boxes
         sel = st["sel"]
         with torch.cuda.device(self.device):          # the kernels launch on the current device
@@ -211,21 +191,21 @@ class FaceAnaImages:
         # 4. landmarks on exactly the faces found, packed in image order
         if out is None:
             self._grow_faces(st, max(F, 1))
-            res = {k: st[k] for k in self._face_fields()}
+            res = {k: st[k] for k in self._face_fields(0)}
         else:
             res = out
-        fl._enqueue_to(frames, [boxes[i, :k] for i, k in enumerate(counts.tolist())],
-                       {k: res[k] for k in fl._out_fields()})
+        fl._enqueue(call, *fl._check_boxes(call, [boxes[i, :k] for i, k in enumerate(counts.tolist())]),
+                    {k: res[k] for k in fl._fields(0)})
         # face -> image map and each face's image size; with out=, first and count too: one upload
         m = 2 * n + 3 * F
         if st["hmap"] is None or st["hmap"].shape[0] < m:
             st["done"].synchronize()
-            st["hmap"] = _grow(st["hmap"], m, lambda k: torch.empty((k,), dtype=torch.int32).pin_memory())
-            st["map"] = _grow(st["map"], m, lambda k: torch.empty((k,), dtype=torch.int32, device=self.device))
+            st["hmap"] = grow(st["hmap"], m, lambda k: torch.empty((k,), dtype=torch.int32).pin_memory())
+            st["map"] = grow(st["map"], m, lambda k: torch.empty((k,), dtype=torch.int32, device=self.device))
         st["staged"].synchronize()                    # the slot's last upload has left the pinned map
         hmap = st["hmap"].numpy()
         hmap[:n], hmap[n:2 * n], hmap[2 * n:2 * n + F] = first, counts, face_image
-        hw = np.array([f.shape[:2] for f in frames], np.int32)
+        hw = np.array([shape[:2] for shape in call.shapes], np.int32)
         hmap[2 * n + F:m].reshape(F, 2)[:] = hw[face_image]
         dmap = st["map"]
         with torch.cuda.stream(ls):
@@ -248,11 +228,11 @@ class FaceAnaImages:
         if out is None and F:
             with torch.cuda.stream(ls):
                 for k, t in res.items():
-                    if k != "chip" or cuda:           # host images are warped at collect()
+                    if k != "chip" or call.cuda:      # host images are warped at collect()
                         st["h" + k][:F].copy_(t[:F], non_blocking=True)
         st["done"].record(ls)
-        align_host = self.align is not None and not cuda
-        self._pending.append((slot, n, out, counts, first, (frames, [f.shape for f in frames]) if align_host else None))
+        align_host = self.align is not None and not call.cuda
+        self._pending.append((slot, n, out, counts, first, call if align_host else None))
         self._next ^= 1
 
     def collect(self):
@@ -261,7 +241,7 @@ class FaceAnaImages:
         torch.cuda.current_stream() is made to wait for the call, so work queued on it afterwards sees the results."""
         if not self._pending:
             raise RuntimeError("FaceAnaImages: nothing submitted")
-        slot, n, out, counts, first, host_images = self._pending.pop(0)
+        slot, n, out, counts, first, host_call = self._pending.pop(0)
         if n == 0:
             return []
         st = self._slots[slot]
@@ -271,10 +251,10 @@ class FaceAnaImages:
             return out
         st["done"].synchronize()
         F = int(counts.sum())
-        if host_images is not None and F:
-            self.landmark._warp_host_frames(*host_images, counts.tolist(), st["hM"].numpy()[:F], st["M"], st["chip"],
+        if host_call is not None and F:
+            self.landmark._warp_host_frames(host_call, counts.tolist(), st["hM"].numpy()[:F], st["M"], st["chip"],
                                             st["hchip"])
-        host = {k: st["h" + k].numpy()[:F] for k in self._face_fields()}
+        host = {k: st["h" + k].numpy()[:F] for k in self._face_fields(0)}
         res = []
         for o, k in zip(first.tolist(), counts.tolist()):
             part = {name: a[o:o + k].copy() for name, a in host.items()}
@@ -294,20 +274,19 @@ class FaceAnaImages:
         ev = {name: torch.cuda.Event() for name in ("selected", "staged", "done")}
         return dict(det=None, sel=None, hsel=None, map=None, hmap=None, faces=0, **ev)
 
-    def _face_fields(self):
-        """Names of the per-face results, in new_results' order."""
-        return [k for k in result_fields(1, 1, self.n_points, self.pose, self.align) if k not in ("count", "first")]
+    def _face_fields(self, rows):
+        """The per-face fields of result_fields, for `rows` faces."""
+        f = result_fields(rows, 1, self.n_points, self.pose, self.align)
+        del f["count"], f["first"]
+        return f
 
     def _grow_faces(self, st, F):
         """The slot's device results and their pinned copies, for at least F faces."""
-        import torch
         if st["faces"] >= F:
             return
         st["done"].synchronize()
         rows = max(F, 2 * st["faces"], 1)
-        for k, (shape, dt) in result_fields(rows, 1, self.n_points, self.pose, self.align).items():
-            if k in ("count", "first"):
-                continue
-            st[k] = torch.empty(shape, dtype=getattr(torch, dt), device=self.device)
-            st["h" + k] = torch.empty(shape, dtype=getattr(torch, dt)).pin_memory()
+        fields = self._face_fields(rows)
+        st.update(new_buffers(fields, self.device))
+        st.update({"h" + k: t.pin_memory() for k, t in new_buffers(fields, "cpu").items()})
         st["faces"] = rows

@@ -53,31 +53,3 @@ def test_packing_equals_numpy(top_k):
             assert np.all(face_image[first[i]:first[i] + k] == i)
     first, face_image = pack_faces([top_k] * 3)
     assert first.tolist() == [0, top_k, 2 * top_k] and len(face_image) == 3 * top_k
-
-
-@pytest.mark.parametrize("pose", [False, True])
-def test_out_capacity_check(pose):
-    import torch
-    from peppa_pig_face_landmark_b200.core.api.images import check_results, result_fields
-    cpu, K, P = torch.device("cpu"), 16, 98
-
-    def new(n):
-        return {k: torch.zeros(shape, dtype=getattr(torch, dt)) for k, (shape, dt) in result_fields(n, K, P, pose).items()}
-
-    out = new(4)
-    assert out["box"].shape == (64, 4) and out["kps"].shape == (64, P, 2) and out["count"].shape == (4,)
-    for n in (0, 1, 4):
-        check_results(out, n, K, P, pose, cpu)
-    with pytest.raises(ValueError):
-        check_results(out, 5, K, P, pose, cpu)                          # one image too many
-    with pytest.raises(ValueError):
-        check_results(out, 4, K + 1, P, pose, cpu)                      # rows for a smaller top_k
-    with pytest.raises(ValueError):
-        check_results(out, 1, K, P, not pose, cpu)                      # the pose fields missing or extra
-    bent = [dict(out, box=out["box"].double()), dict(out, count=out["count"].long()), dict(out, kps=out["kps"][:, :97]),
-            dict(out, scores=out["scores"].t()), {k: v for k, v in out.items() if k != "first"}, dict(out, first=[0] * 4)]
-    for b in bent:
-        with pytest.raises(ValueError):
-            check_results(b, 1, K, P, pose, cpu)
-    with pytest.raises(ValueError):
-        check_results(out, 1, K, P, pose, cpu, busy=[out["kps"].data_ptr()])
