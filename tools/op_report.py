@@ -453,24 +453,99 @@ def _stored(op):
     return list(op.outs)
 
 
+# Output tile of every tiled kernel: kernel -> (f(info, H, W) -> (rows, columns) of one tile of an H x W output map, whether
+# a tile can hang over the map's border).  info is the tiling skps_engine_op_kernel reports.  A kernel whose applicability
+# test only takes maps made of whole tiles has no border tiles; launch_signature() asserts that of every launch it sees.
+# conv_pw tiles the flat (n, y, x) pixel index of the batch instead (PW_BM); conv_simt's pixel tile is picked per launch
+# from the SM count and is not reported, so it has no entry.
+TILES = {
+    # 128-pixel blocks of bw x bh = 128 / bw pixels of one image, ragged at the right and bottom border (tc_pick_bw);
+    # maps under 128 pixels: ipt whole images per tile (bw = W, bh = ipt H), the batch's last tile partial
+    K_TC: (lambda info, H, W: (info[1], info[0]), True),
+    # whole-row store boxes: bh = 256 / W rows of the full width; tct_applicable takes only W | 256 and H % bh == 0
+    K_TCT: (lambda info, H, W: (info[0], W), False),
+    # 256-pixel blocks of whole rows; hm_shape_ok takes only W | 256 and (H W) % 256 == 0
+    K_HM: (lambda info, H, W: (256 // W, W), False),
+    # 8 x 16 pixel tiles over the (stride-1) map, ceil-divided (conv_mma.cu MT_H, MT_W)
+    K_MMA: (lambda info, H, W: (8, 16), True),
+    # 16 x 8 pixel tiles (xf_producer.h XF_TW, XF_TH), ceil-divided
+    K_XF: (lambda info, H, W: (8, 16), True),
+    # conv_xf's tiles; fpw_supported takes only H % 8 == W % 16 == 0
+    K_FPW: (lambda info, H, W: (8, 16), False),
+    # dw_tile_rows(k, s) rows x 16 columns, ceil-divided
+    K_DW_TMA: (lambda info, H, W: (info[0], P.DW_TILE_W), True),
+    # 8 x 16 output tiles for the up-sampled channels and a 3x3 stride-1 dw_tma launch (8 x 16) for the skip channels
+    K_UPCAT_TMA: (lambda info, H, W: (8, 16), True),
+    # 8 x 16 tiles of the quarter-resolution output; stem_block_supported takes only input maps with H % 32 == W % 64 == 0
+    K_STEM: (lambda info, H, W: (8, 16), False),
+    # the fallback depthwise kernel: one thread per 4 consecutive pixels of a row where W % 4 == 0, else per pixel
+    K_DW: (lambda info, H, W: (1, 4 if W % 4 == 0 else 1), False),
+}
+
+
 def edge_tile(kernel, info, H, W, y, x, n=None, batch=None):
-    """Whether output pixel (y, x) of an H x W map lies in a tile that hangs over the map's border; for conv_pw, whether
-    pixel (n, y, x) lies in the last, partial tile of a batch of `batch` maps.  conv_fpw only takes maps made of whole 16 x 8
-    tiles, so none of its pixels is in an edge tile."""
-    if kernel == K_FPW:
-        return False
-    if kernel == K_PW:
+    """Whether output pixel (y, x) of an H x W map lies in a tile that hangs over the map's border (TILES); for conv_pw, and
+    for conv_tc's multi-image tiles, whether pixel (n, y, x) lies in the last, partial tile of a batch of `batch` maps.
+    None where the kernel's tiling is not known."""
+    if kernel == K_PW or (kernel == K_TC and info[2] > 1):
         if n is None or batch is None:
             return None
+        if kernel == K_TC:
+            return bool(batch % info[2] and n >= batch // info[2] * info[2])
         rows = batch * H * W
         return bool(rows % PW_BM and (n * H + y) * W + x >= rows // PW_BM * PW_BM)
-    if kernel == K_TC and info[2] == 1:
-        bw, bh = info[0], info[1]
-    elif kernel == K_DW_TMA:
-        bw, bh = P.DW_TILE_W, info[0]
-    else:
+    if kernel not in TILES:
+        return None
+    tile, border = TILES[kernel]
+    if not border:
+        return False
+    bh, bw = tile(info, H, W)
+    if bh <= 0 or bw <= 0:                     # no tiling reported (the float32 interpreter standing in for the engine)
         return None
     return bool((x // bw + 1) * bw > W or (y // bh + 1) * bh > H)
+
+
+def plan_structure(plan):
+    """The sequence of (op type, op flags) of a plan: which ops the lowering emits, fused how, routed to which family."""
+    return tuple((op.type, op.flags) for op in plan.ops)
+
+
+def launch_signature(op, kernel, info, H, W, batch):
+    """What decides which code paths one op's launch runs: the op's layer (type, flags, kernel size, stride, channels,
+    activation), the kernel and its tiling (info), and where the map's border falls in the kernel's tile.  H x W is the
+    op's output map.
+
+    For the kernels in TILES the border is (H mod tile rows > 0, W mod tile columns > 0, the map is smaller than one
+    tile).  Whether a side is ragged, not by how much, is what selects code: conv_tc masks every row of an edge tile
+    (row_ok) and its TMA stores clip, dw_tma masks every pixel, conv_xf stores row by row, so the remainder itself picks
+    no other path.  conv_xf adds whether the map is one tile across: it then loads a wider up-sample weight box (wcx,
+    conv_xf.cu).  conv_pw: whether the last 128-pixel tile of the batch's batch H W pixels is partial.  conv_tc adds
+    the images in the last multi-image tile (ipt > 1) and, with two pixel tiles per weight load (mt = 2), the parity
+    of the launch's tile count.  A kernel without border tiles is asserted to have no ragged side.  The op's place in
+    the plan is left out: the same layer at another place runs the same code."""
+    info = tuple(int(v) for v in info)
+    if kernel == K_PW:
+        border = ((batch * H * W) % PW_BM > 0,)
+    elif kernel in TILES:
+        tile, has_border = TILES[kernel]
+        th, tw = tile(info, H, W)
+        border = (H % th > 0, W % tw > 0, H < th or W < tw)
+        assert has_border or not (border[0] or border[1]), "%s has no border tiles, but its %dx%d tile does not " \
+            "divide %dx%d" % (KERNELS[kernel], th, tw, H, W)
+        if kernel == K_XF:
+            border += (W <= tw,)
+        if kernel == K_TC:
+            bw, bh, ipt, mt = info
+            if ipt > 1:
+                border += (batch % ipt,)
+            if mt == 2:
+                tiles = -(-batch // ipt) if ipt > 1 else batch * (-(-H // bh)) * (-(-W // bw))
+                border += (tiles % 2,)
+    else:
+        border = None
+    layer = (op.type, op.flags, tuple(op.k), tuple(op.s), op.ins[0].C if op.ins and op.ins[0] is not None else 0,
+             op.outs[0].C, op.act)
+    return layer, kernel, info, border
 
 
 def _to64(t, buf):
@@ -777,6 +852,64 @@ def detector_inputs(hw, batch=3):
     x, _ = H.letterbox(frames.frame_4k(), *hw)
     real = np.round(x[0].transpose(1, 2, 0) * 255).astype(np.uint8)
     return _with_noise(real, batch)
+
+
+def detector_domain_sample():
+    """Detector input sizes that take every value of each axis of the accepted range (check_detector_input): every h with
+    w at the range's minimum, Skps.yml's default 640 and the maximum, every w with h at the minimum, the default 384 and
+    the maximum -- the four corners included.  The minima bring the small maps, where conv_tc's multi-image tiles start."""
+    from peppa_pig_face_landmark_b200.graph_tools import DET_INPUT_MAX as hi, DET_INPUT_MIN as lo
+    hs, ws = range(lo[0], hi[0] + 1, 32), range(lo[1], hi[1] + 1, 32)
+    return sorted({(h, w) for h in hs for w in (lo[1], 640, hi[1])} | {(h, w) for w in ws for h in (lo[0], 384, hi[0])})
+
+
+def retarget_and_lower(args):
+    """(hw, directory, keep) -> (hw, path, plan_structure of the plan): the shipped detector retargeted to hw, written to
+    `path` in directory and lowered.  The file (2 MB at 128x128, 84 MB at 2176x3840) is deleted unless keep, and path is
+    then None.  A module-level function so that a process pool can run it."""
+    from peppa_pig_face_landmark_b200 import lowering
+    from peppa_pig_face_landmark_b200.graph_tools import retarget_detector_input
+    hw, d, keep = args
+    src = os.path.join(ROOT, "peppa_pig_face_landmark_b200", "pretrained", "yolov5n-0.5.onnx")
+    path = retarget_detector_input(src, os.path.join(d, "det_%dx%d.onnx" % hw), hw)
+    try:
+        structure = plan_structure(lowering.lower(path, hw))
+    finally:
+        if not keep:
+            os.remove(path)
+    return hw, path if keep else None, structure
+
+
+def lower_detector_domain(sizes, directory, keep=False):
+    """retarget_and_lower over `sizes` on every CPU: yields (hw, path, plan structure) in the order of `sizes`.  With
+    keep, the caller deletes each file once done with it; the pool runs at most two sizes per worker ahead of the
+    caller, so only those files exist at one time."""
+    import multiprocessing
+    from collections import deque
+    from concurrent.futures import ProcessPoolExecutor
+    n = min(16, os.cpu_count() or 1)
+    todo = iter(sizes)
+    with ProcessPoolExecutor(n, mp_context=multiprocessing.get_context("spawn")) as ex:
+        ahead = deque()
+        for hw in todo:
+            ahead.append(ex.submit(retarget_and_lower, (hw, directory, keep)))
+            if len(ahead) >= 2 * n:
+                yield ahead.popleft().result()
+        while ahead:
+            yield ahead.popleft().result()
+
+
+def greedy_cover(sigs):
+    """{size: set of signatures} -> sizes whose signatures together are all of them: greedy weighted set cover at cost
+    h w, i.e. repeatedly the size with the least cost per signature it adds (the smaller size on a tie)."""
+    left = set().union(*sigs.values())
+    cover = []
+    while left:
+        hw = min((hw for hw in sigs if sigs[hw] & left),
+                 key=lambda hw: (hw[0] * hw[1] / len(sigs[hw] & left), hw[0] * hw[1], hw))
+        cover.append(hw)
+        left -= sigs[hw]
+    return cover
 
 
 def _with_noise(real, batch):
