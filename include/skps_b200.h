@@ -485,6 +485,18 @@ SKPS_API int skps_debug_mp_temporal(const skps_pipeline_cfg* cfg, int n_streams,
                                     int32_t* n_prev, int32_t* prev_f32, int32_t* state_idx, double* track_box,
                                     float* track_f32, int32_t* n_track, int64_t* ids, int64_t* next_id, double* out_kps,
                                     void* stream);
+/* skps_debug_mp_temporal with the id memory of skps_mpipe_set_id_memory: id_memory >= 0 frames, and the memory state [dev],
+ * updated in place, laid out as skps_mpipe keeps it: mem_ids (S,K) int64 ids of the lost tracks, most recently lost first;
+ * mem_box (S,K,4) float32 their boxes of the frame that last returned them; mem_gap (S,K) int32 the frames in a row each has
+ * been missing so far; mem_n (S) entries held, 0 after skps_mpipe_create / skps_mpipe_reset.  With id_memory = 0 the four
+ * may be NULL and the launch is skps_debug_mp_temporal's.  Asynchronous on `stream`. */
+SKPS_API int skps_debug_mp_temporal_mem(const skps_pipeline_cfg* cfg, int n_streams, int top_k, int n_points,
+                                        const float* kps_now, const int32_t* count, const int32_t* flag, const int32_t* hw,
+                                        const float* boxes4, const int32_t* src, double* prev_lm, double* prev_dx,
+                                        int32_t* n_prev, int32_t* prev_f32, int32_t* state_idx, double* track_box,
+                                        float* track_f32, int32_t* n_track, int64_t* ids, int64_t* next_id, double* out_kps,
+                                        int id_memory, int64_t* mem_ids, float* mem_box, int32_t* mem_gap, int32_t* mem_n,
+                                        void* stream);
 
 /* ---- Aligned face chips (csrc/align.cu; additive) -----------------------------------------------------------------------
  * What a caller does with the 98 landmarks before a recognition / attribute model: estimate the least-squares similarity
@@ -566,6 +578,17 @@ SKPS_API int skps_mpipe_pose_results(skps_mpipe* p, int slot, double* rvec, doub
 SKPS_API int skps_mpipe_set_detect_every(skps_mpipe* p, int every);
 /* The number of frames the detector ran on in the slot's last submitted batch (0..n; 0 skips the detector). */
 SKPS_API int skps_mpipe_detector_frames(const skps_mpipe* p, int slot, int* m);
+
+/* ---- Id memory (csrc/temporal.cu; additive) ------------------------------------------------------------------------------
+ * FaceAna(track_ids=True, id_memory=frames) for every stream.  A track box returned at a stream's frame a whose id no face of
+ * its frame a + 1 carries is lost: the stream remembers its id and float32 box, most recently lost first, tracks lost at the
+ * same frame in return order, at most top_k (about 28 bytes each, allocated by skps_mpipe_create).  A face that would get the
+ * stream's next number first takes back the id of the first remembered track that it overlaps with IoU > track_iou (its
+ * float32 landmark-stage box against the remembered one) and that has been missing for at most `frames` frames in a row; the
+ * entry is then forgotten.  When more than top_k are held, the oldest go first.  A stream's frames are those of the submits
+ * that include it.  frames = 0 (the default) remembers nothing; switching to 0 forgets every stream's lost tracks.
+ * skps_mpipe_reset forgets the stream's.  May be called at any time; takes effect from the next submit. */
+SKPS_API int skps_mpipe_set_id_memory(skps_mpipe* p, int frames);
 
 #ifdef __cplusplus
 }

@@ -16,7 +16,7 @@ import yaml
 from ... import runtime as rt
 from ...graph_tools import check_detector_input
 from ...logger.logger import logger
-from ..smoother.lk import EmaFilter, GroupTrack, assign_track_ids, first_match, rects
+from ..smoother.lk import MAX_ID_MEMORY, EmaFilter, GroupTrack, IdMemory, assign_track_ids, first_match, rects
 from .face_detector import FaceDetector, letterbox_geometry
 from .face_landmark import MIN_FACE, FaceLandmark, face_scale
 from .align import check_size
@@ -36,6 +36,16 @@ def check_detect_every(every, offset=0):
     if not is_int(offset) or not 0 <= offset < every:
         raise ValueError("detect_offset must be an int in 0..%d, got %r" % (every - 1, offset))
     return int(every), int(offset)
+
+
+def check_id_memory(frames, track_ids):
+    """id_memory as an int in 0..MAX_ID_MEMORY, and > 0 only with track_ids, else ValueError."""
+    if (not isinstance(frames, (int, np.integer)) or isinstance(frames, (bool, np.bool_))
+            or not 0 <= frames <= MAX_ID_MEMORY):
+        raise ValueError("id_memory must be an int in 0..%d, got %r" % (MAX_ID_MEMORY, frames))
+    if frames and not track_ids:
+        raise ValueError("id_memory=%d keeps the ids of lost tracks and needs track_ids=True" % frames)
+    return int(frames)
 
 
 class DetectCadence:
@@ -75,7 +85,7 @@ def pipeline_cfg(cfg, top_k, max_frame_hw):
 
 class FaceAna():
     def __init__(self, verbose=False, top_k=None, max_frame_hw=(2160, 3840), align=None, pose=False, det_input=None,
-                 track_ids=False, detect_every=1, detect_offset=0):
+                 track_ids=False, detect_every=1, detect_offset=0, id_memory=0):
         """align: None, or a chip side in 16..512: every result dict then also carries 'chip' ((align, align, 3) uint8
         BGR, the face warped to the ArcFace five-point template) and 'M' ((2, 3) float64, the frame -> chip matrix for
         cv2.warpAffine), computed on the GPU from the returned 'kps' and the frame already in HBM (core/api/align.py).
@@ -93,8 +103,15 @@ class FaceAna():
         the detector, the first of the previous call's faces whose box its detection overlaps with IoU > Trace.iou_thres
         (the match judge_boxs smooths the box with), or none; on a frame the difference gate skipped, the previous face
         it is.  In the order of the returned list, a face inherits its source's id unless an earlier face of the same
-        call already took it, and every other face gets the next unused number.  A face the tracker loses for one frame
-        comes back with a new id: there is no re-identification.
+        call already took it, and every other face gets the next unused number.  With id_memory=0 (the default) a face
+        the tracker loses for one frame comes back with a new id.
+        id_memory: 0..2**31 - 1 frames (track_ids only).  A track returned at frame a that no face of frame a + 1 carries
+        is lost; its id and its float32 box of frame a are remembered, up to top_k of them.  A face that would get the
+        next unused number first takes back the id of the first remembered track, most recently lost first, that it
+        overlaps with IoU > Trace.iou_thres (its float32 landmark-stage box against the remembered one) and that has been
+        missing for at most id_memory frames in a row.  Only 'id' changes: such a face's box, landmarks and smoothing
+        start afresh as without the memory.  Frames are counted from construction or reset(), which forgets the lost
+        tracks too.
         detect_every, detect_offset: the detection cadence.  Frames are counted from construction or reset(), i = 0, 1,
         2, ...; frame i runs the detector when there is no previous frame of its size (the first frame, a size change),
         or when (i + detect_offset) % detect_every == 0 and the frame-difference gate fires.  Every other frame takes the
@@ -102,6 +119,7 @@ class FaceAna():
         found at the next keyframe, up to detect_every - 1 frames late, and a face that leaves is followed by its
         landmark box until the next keyframe.  detect_every=1 (the default) is the reference's behaviour.
         last_ran_detector tells whether the last run() used the detector."""
+        self.id_memory = check_id_memory(id_memory, track_ids)
         self._cadence = DetectCadence(detect_every, detect_offset)
         self.detect_every, self.detect_offset = self._cadence.every, self._cadence.offset
         cfg = get_cfg()
@@ -149,6 +167,7 @@ class FaceAna():
         self._det_rows = np.zeros((FaceDetector.MAX_DET, 16), np.float32)
         self._have_prev = False
         self._ids, self._next_id = [], 0     # ids of the track boxes (index-aligned with track_box), next unused id
+        self._memory = IdMemory(self.id_memory, self.top_k, self.iou_thres) if self.id_memory else None
         self.last_det_idx = None       # kept detector rows of the last detector run (parity checks)
         self.last_ran_detector = None
         self.last_det_rows = None
@@ -182,7 +201,7 @@ class FaceAna():
         track32 = None
         if n_track:
             track32 = np.ascontiguousarray(np.asarray(track)[:, :4], dtype=np.float32)
-        ids = []
+        src = np.zeros((0,), np.int32)
         if not run_det and n_track == 0:
             # facer.py:61 with an empty/None track: nothing to do (the reference would fail on None)
             boxes_return = np.zeros((0, 4), np.float32)
@@ -200,7 +219,6 @@ class FaceAna():
             if self.track_ids and n:
                 src = np.empty((n,), np.int32)
                 rt.check(self.lib.skps_pipeline_face_sources(self._pipe, n, src.ctypes.data))
-                ids, self._next_id = assign_track_ids(src, self._ids, self._next_id)
             if run_det:
                 nd = self._ndet.value
                 idx, rows = self._det_idx, self._det_rows
@@ -212,6 +230,12 @@ class FaceAna():
                 self.last_det_rows = rows[:nd].copy()
         if run_det:
             self.trace.previous_landmarks_set = None
+        ids = []
+        if self._memory is not None:          # every call, faceless ones included: they lose every track
+            prev = track32 if n_track else np.zeros((0, 4), np.float32)
+            ids, self._next_id = self._memory.assign(src, boxes_return, self._ids, prev, self._next_id)
+        elif len(src):
+            ids, self._next_id = assign_track_ids(src, self._ids, self._next_id)
 
         landmarks = self.trace.calculate(image, landmarks)
 
@@ -316,6 +340,8 @@ class FaceAna():
         self.previous_image = None
         self.previous_box = None
         self._ids, self._next_id = [], 0
+        if self._memory is not None:
+            self._memory.reset()
         self._cadence.reset()
         rt.check(self.lib.skps_pipeline_reset(self._pipe))
 

@@ -11,6 +11,7 @@ device (csrc/mpipe.cu, csrc/temporal.cu) and two batches can be in flight so tha
     # FaceAnaStreams(..., pose=True): each dict also has 'pose' {'euler', 'rvec', 'tvec', 'reproject'} as FaceAna returns it
     # FaceAnaStreams(..., track_ids=True): each dict also has 'id', the track id FaceAna(track_ids=True) gives the face
     # FaceAnaStreams(..., detect_every=4): stream s runs the detector on a quarter of its frames, staggered by s % 4
+    # FaceAnaStreams(..., track_ids=True, id_memory=30): a face lost for up to 30 frames gets its old id back
     # or, overlapped:
     fa.submit(frames_t0); fa.submit(frames_t1); r0 = fa.collect(); fa.submit(frames_t2); r1 = fa.collect(); ...
     # frames already on the GPU (torch.uint8 CUDA tensors (H, W, 3), any row pitch), results left on the GPU:
@@ -27,13 +28,13 @@ from ... import runtime as rt
 from ...graph_tools import check_detector_input, detector_onnx_for
 from .align import check_size
 from .device_frames import check_cuda_frame, check_host_frame, is_cuda_tensor
-from .facer import check_detect_every, get_cfg, pipeline_cfg
+from .facer import check_detect_every, check_id_memory, get_cfg, pipeline_cfg
 from .onnx_model_base import ONNXEngine
 
 
 class FaceAnaStreams:
     def __init__(self, n_streams, top_k=None, max_frame_hw=(2160, 3840), device="cuda", align=None, pose=False,
-                 det_input=None, track_ids=False, detect_every=1):
+                 det_input=None, track_ids=False, detect_every=1, id_memory=0):
         """align: None, or a chip side in 16..512: every result dict then also carries 'chip' and 'M' as FaceAna(align=...)
         returns them, warped inside the same submit on the device from the smoothed landmarks and the frame in the ring.
         pose: every result dict then also carries 'pose' as FaceAna(pose=True) returns it, solved inside the same submit
@@ -44,6 +45,9 @@ class FaceAnaStreams:
         track_ids: every result dict then also carries 'id', the int FaceAna(track_ids=True) returns for the face: ids
         are numbered per stream from 0, reset(stream) starts that stream again from 0, and the rule that assigns them is
         FaceAna's.  The ids are kept on the device next to the track boxes, whether or not they are returned.
+        id_memory: FaceAna(track_ids=True, id_memory=...) for every stream: up to top_k lost tracks per stream (about 28
+        bytes each) whose ids a face that reappears where one was lost takes back, kept and matched on the device.  A
+        stream's frames are the calls that include it; reset(stream) forgets its lost tracks.
         detect_every: the detection cadence of FaceAna(detect_every=N, detect_offset=s % N) for stream s, which it
         returns bit for bit.  A stream counts its frames from construction or reset(stream), advancing only on calls
         that include a frame for it; frame i runs the detector when the stream has no previous frame of its size, or
@@ -53,6 +57,7 @@ class FaceAnaStreams:
         call, packed into one batch, and not at all on a call without keyframes (last_detector_frames).  The detector
         engine keeps one CUDA graph per batch size it meets; with the stagger those are only a few sizes."""
         self.detect_every = check_detect_every(detect_every)[0]
+        self.id_memory = check_id_memory(id_memory, track_ids)
         self.align = None if align is None else check_size(align)
         self.pose = bool(pose)
         self.track_ids = bool(track_ids)
@@ -81,6 +86,8 @@ class FaceAnaStreams:
         self._h = h
         if self.detect_every != 1:
             rt.check(self.lib.skps_mpipe_set_detect_every(h, self.detect_every))
+        if self.id_memory:
+            rt.check(self.lib.skps_mpipe_set_id_memory(h, self.id_memory))
         S, K, P = self.n_streams, self.top_k, self.n_points
         self._out = [dict(n=np.zeros(S, np.int32), box=np.zeros((S, K, 4), np.float64), kps=np.zeros((S, K, P, 2), np.float64),
                           sc=np.zeros((S, K, P), np.float32), det=np.zeros(S, np.int32), ids=np.zeros((S, K), np.int64))

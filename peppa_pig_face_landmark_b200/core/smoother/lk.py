@@ -27,14 +27,20 @@ def rects(sets):
 
 def first_match(r1, r2, thres):
     """For every row of r1 (n, 4), the first row of r2 (m, 4) with iou > thres, else -1: what the reference's loop
-    `for prev in r2: if iou(now, prev) > thres: break` finds with _iou on numpy scalars.
+    `for prev in r2: if iou(now, prev) > thres: break` finds with _iou on numpy scalars."""
+    n, m = r1.shape[0], r2.shape[0]
+    if n == 0 or m == 0:
+        return np.full(n, -1, np.int64)
+    hit = iou_hits(r1, r2, thres)
+    return np.where(hit.any(1), hit.argmax(1), -1)
+
+
+def iou_hits(r1, r2, thres):
+    """(n, m) bool: _iou(r1[i], r2[j]) > thres on numpy scalars of the rows' own dtypes, for n, m >= 1.
 
     Python's min / max return one of their operands, each with its own dtype, and numpy then computes in float32 only
     when both operands are float32 (float64 otherwise).  With r1 and r2 of different dtypes that choice is made per
     element, so each intermediate carries a "float32" flag next to its float64 value."""
-    n, m = r1.shape[0], r2.shape[0]
-    if n == 0 or m == 0:
-        return np.full(n, -1, np.int64)
     f32, f64 = np.float32, np.float64
     a32, b32 = r1.dtype == f32, r2.dtype == f32
     a, b = r1.astype(f64)[:, None, :], r2.astype(f64)[None, :, :]
@@ -58,8 +64,7 @@ def first_match(r1, r2, thres):
         inter = inter.astype(s.dtype)
         iou = inter / (s - inter)
         # max(0, w) * max(0, h) is 0 (iou 0 or nan) unless both are positive
-        hit = (w[0] > 0) & (h[0] > 0) & (iou > thres)
-    return np.where(hit.any(1), hit.argmax(1), -1)
+        return (w[0] > 0) & (h[0] > 0) & (iou > thres)
 
 
 def assign_track_ids(sources, prev_ids, next_id):
@@ -77,6 +82,60 @@ def assign_track_ids(sources, prev_ids, next_id):
             next_id += 1
         taken.add(ids[-1])
     return ids, next_id
+
+
+MAX_ID_MEMORY = 2 ** 31 - 1      # frames: the device keeps each lost track's gap as an int32
+
+
+class IdMemory:
+    """Track ids with a memory of lost tracks (SORT's max_age, applied to ids only).  A track returned by one call and
+    carried by no face of the next is lost; its id and its float32 box of the call that last returned it are remembered.
+    A face that assign_track_ids would give a fresh number first takes the id of the first remembered track it overlaps
+    with iou > iou_thres (both boxes float32, as judge_boxs compares two float32 rows) that has been missing for at most
+    `frames` calls in a row; that entry is then forgotten.
+
+    Entries are kept most recently lost first, tracks lost at the same call in the order their faces were returned.  At
+    most `capacity` are kept: the oldest go first, and among tracks lost at the same call the last returned.  An entry
+    whose gap can no longer qualify is dropped.  frames=0 keeps nothing, and assign() then gives assign_track_ids's ids."""
+
+    def __init__(self, frames, capacity, iou_thres):
+        self.frames, self.capacity, self.iou_thres = int(frames), int(capacity), iou_thres
+        self.reset()
+
+    def reset(self):
+        self.ids = []                                # most recently lost first
+        self.boxes = np.zeros((0, 4), np.float32)
+        self.gaps = []                               # calls in a row without the track so far
+
+    def assign(self, sources, boxes, prev_ids, prev_boxes, next_id):
+        """One call: sources as for assign_track_ids, boxes (n, 4) the float32 boxes of this call's faces (the boxes the
+        landmark stage used), prev_ids / prev_boxes (len(prev_ids), 4) the ids and float32 boxes of the previous call's
+        faces.  Returns (ids as a list of ints, the new next_id) and remembers the tracks this call loses."""
+        n, m = len(sources), len(self.ids)
+        hit = None
+        if n and m:
+            hit = iou_hits(np.asarray(boxes, np.float32).reshape(-1, 4), self.boxes, self.iou_thres)
+        ids, taken, used = [], set(), set()
+        for i, s in enumerate(sources):
+            s = int(s)
+            if 0 <= s < len(prev_ids) and prev_ids[s] not in taken:
+                ids.append(prev_ids[s])
+            else:
+                k = next((k for k in range(m) if k not in used and self.gaps[k] <= self.frames and hit[i, k]), None)
+                if k is not None:
+                    used.add(k)
+                    ids.append(self.ids[k])
+                else:
+                    ids.append(next_id)
+                    next_id += 1
+            taken.add(ids[-1])
+        lost = ([j for j, v in enumerate(prev_ids) if v not in taken] if self.frames else [])[:self.capacity]
+        keep = [k for k in range(m) if k not in used and self.gaps[k] < self.frames][:self.capacity - len(lost)]
+        prev_boxes = np.asarray(prev_boxes, np.float32).reshape(-1, 4)
+        self.ids = [prev_ids[j] for j in lost] + [self.ids[k] for k in keep]
+        self.boxes = np.concatenate([prev_boxes[lost], self.boxes[keep]]).reshape(-1, 4)
+        self.gaps = [1] * len(lost) + [self.gaps[k] + 1 for k in keep]
+        return ids, next_id
 
 
 def _iou(r1, r2):

@@ -174,15 +174,33 @@ extern "C" SKPS_API int skps_debug_mp_temporal(const skps_pipeline_cfg* cfg, int
                                                double* prev_dx, int32_t* n_prev, int32_t* prev_f32, int32_t* state_idx,
                                                double* track_box, float* track_f32, int32_t* n_track, int64_t* ids,
                                                int64_t* next_id, double* out_kps, void* stream) {
+    return skps_debug_mp_temporal_mem(cfg, n_streams, top_k, n_points, kps_now, count, flag, hw, boxes4, src, prev_lm, prev_dx,
+                                      n_prev, prev_f32, state_idx, track_box, track_f32, n_track, ids, next_id, out_kps, 0,
+                                      nullptr, nullptr, nullptr, nullptr, stream);
+}
+
+// The same launch with the id memory of skps_mpipe_set_id_memory: id_memory frames, and the memory state in the caller's
+// device buffers (needed when id_memory > 0).
+extern "C" SKPS_API int skps_debug_mp_temporal_mem(const skps_pipeline_cfg* cfg, int n_streams, int top_k, int n_points,
+                                                   const float* kps_now, const int32_t* count, const int32_t* flag,
+                                                   const int32_t* hw, const float* boxes4, const int32_t* src,
+                                                   double* prev_lm, double* prev_dx, int32_t* n_prev, int32_t* prev_f32,
+                                                   int32_t* state_idx, double* track_box, float* track_f32, int32_t* n_track,
+                                                   int64_t* ids, int64_t* next_id, double* out_kps, int id_memory,
+                                                   int64_t* mem_ids, float* mem_box, int32_t* mem_gap, int32_t* mem_n,
+                                                   void* stream) {
     SKPS_CHECK(cfg && kps_now && count && flag && hw && boxes4 && src && prev_lm && prev_dx && n_prev && prev_f32 &&
                state_idx && track_box && track_f32 && n_track && ids && next_id && out_kps, "debug_mp_temporal: null argument");
     SKPS_CHECK(top_k > 0 && top_k <= 64, "debug_mp_temporal: top_k %d outside 1..64", top_k);
     SKPS_CHECK(n_streams > 0 && n_points > 0, "debug_mp_temporal: %d streams of %d points", n_streams, n_points);
-    MpTemporalArgs a;
+    SKPS_CHECK(id_memory >= 0, "debug_mp_temporal: id_memory %d is not >= 0", id_memory);
+    SKPS_CHECK(!id_memory || (mem_ids && mem_box && mem_gap && mem_n), "debug_mp_temporal: id memory on with a null buffer");
+    MpTemporalArgs a = {};
     a.top_k = top_k; a.n_points = n_points;
     a.kps_now = kps_now; a.count = count; a.flag = flag; a.hw = hw; a.boxes4 = boxes4;
     a.prev_lm = prev_lm; a.prev_dx = prev_dx; a.n_prev = n_prev; a.prev_f32 = prev_f32; a.state_idx = state_idx;
     a.track_box = track_box; a.track_f32 = track_f32; a.n_track = n_track; a.src = src; a.ids = ids; a.next_id = next_id;
+    a.id_memory = id_memory; a.mem_ids = mem_ids; a.mem_box = mem_box; a.mem_gap = mem_gap; a.mem_n = mem_n;
     a.out_kps = out_kps;
     mp_temporal_constants(*cfg, a);
     return launch_mp_temporal(a, n_streams, (cudaStream_t)stream);

@@ -80,6 +80,11 @@ struct skps_mpipe {
     int32_t* d_src = nullptr;                 // [S][K]
     int64_t* d_ids = nullptr;                 // [S][K]
     int64_t* d_next_id = nullptr;             // [S]
+    // id memory (skps_mpipe_set_id_memory): each stream's lost tracks, at most K, most recently lost first
+    int id_memory = 0;
+    int64_t* d_mem_ids = nullptr;             // [S][K]
+    float* d_mem_box = nullptr;               // [S][K][4]
+    int32_t *d_mem_gap = nullptr, *d_mem_n = nullptr;     // [S][K], [S]
 };
 
 static void letterbox_geometry(int H, int W, int in_h, int in_w, float* scale, int* rw, int* rh, int* top, int* left) {
@@ -121,7 +126,8 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
     void* dev[] = {p->d_desc, p->d_hw, p->d_have_prev, p->d_flag, p->d_det_count, p->d_det_idx, p->d_count, p->d_detail, p->d_diff,
                    p->d_det_rows, p->d_boxes, p->d_kps_now, p->d_prev_lm, p->d_prev_dx, p->d_track, p->d_out_kps,
                    p->d_track_f32, p->d_n_prev, p->d_prev_f32, p->d_state_idx, p->d_n_track, p->d_chips, p->d_align_M, p->d_pose,
-                   p->d_nms_ws, p->d_src, p->d_ids, p->d_next_id, p->d_det_slot};
+                   p->d_nms_ws, p->d_src, p->d_ids, p->d_next_id, p->d_det_slot, p->d_mem_ids, p->d_mem_box, p->d_mem_gap,
+                   p->d_mem_n};
     for (void* q : dev) if (q) cudaFree(q);
     if (p->s_copy) cudaStreamDestroy(p->s_copy);
     if (p->s_compute) cudaStreamDestroy(p->s_compute);
@@ -135,12 +141,13 @@ extern "C" SKPS_API int skps_mpipe_reset(skps_mpipe* p, int stream) {
     const int a = stream < 0 ? 0 : stream, b = stream < 0 ? p->S : stream + 1;
     for (int s = a; s < b; ++s) {
         // FaceAna.reset (facer.py:200-208) + a fresh GroupTrack: no previous frame, no track boxes, no landmark history;
-        // track ids number from 0 again
+        // track ids number from 0 again, with no lost tracks remembered
         p->prev_h[s] = p->prev_w[s] = 0;
         p->frame_idx[s] = 0;
         const int32_t zero = 0, none = -1, one = 1;
         SKPS_CUDA(cudaMemcpy(p->d_n_track + s, &zero, 4, cudaMemcpyHostToDevice));
         SKPS_CUDA(cudaMemsetAsync(p->d_next_id + s, 0, 8, p->s_compute));
+        SKPS_CUDA(cudaMemsetAsync(p->d_mem_n + s, 0, 4, p->s_compute));
         SKPS_CUDA(cudaMemsetAsync(p->d_ids + (size_t)s * p->K, 0xff, 8 * (size_t)p->K, p->s_compute));
         SKPS_CUDA(cudaMemcpy(p->d_n_prev + s, &none, 4, cudaMemcpyHostToDevice));
         SKPS_CUDA(cudaMemcpy(p->d_prev_f32 + s, &one, 4, cudaMemcpyHostToDevice));
@@ -206,6 +213,8 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
     SKPS_DEV_ALLOC(p->d_n_prev, 4 * S); SKPS_DEV_ALLOC(p->d_prev_f32, 4 * S); SKPS_DEV_ALLOC(p->d_state_idx, 4 * S);
     SKPS_DEV_ALLOC(p->d_n_track, 4 * S);
     SKPS_DEV_ALLOC(p->d_src, 4 * (size_t)K * S); SKPS_DEV_ALLOC(p->d_ids, 8 * (size_t)K * S); SKPS_DEV_ALLOC(p->d_next_id, 8 * S);
+    SKPS_DEV_ALLOC(p->d_mem_ids, 8 * (size_t)K * S); SKPS_DEV_ALLOC(p->d_mem_box, 4 * 4 * (size_t)K * S);
+    SKPS_DEV_ALLOC(p->d_mem_gap, 4 * (size_t)K * S); SKPS_DEV_ALLOC(p->d_mem_n, 4 * S);
     cudaMemset(p->d_prev_lm, 0, 8 * 2 * 2 * (size_t)P * K * S); cudaMemset(p->d_prev_dx, 0, 8 * 2 * 2 * (size_t)P * K * S);
     cudaMemset(p->d_state_idx, 0, 4 * S); cudaMemset(p->d_track_f32, 0, 4 * 4 * (size_t)K * S);
     cudaMemset(p->d_track, 0, 8 * 4 * (size_t)K * S);
@@ -350,6 +359,8 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     a.prev_lm = p->d_prev_lm; a.prev_dx = p->d_prev_dx; a.n_prev = p->d_n_prev; a.prev_f32 = p->d_prev_f32;
     a.state_idx = p->d_state_idx; a.track_box = p->d_track; a.track_f32 = p->d_track_f32; a.n_track = p->d_n_track;
     a.src = p->d_src; a.ids = p->d_ids; a.next_id = p->d_next_id;
+    a.id_memory = p->id_memory;
+    a.mem_ids = p->d_mem_ids; a.mem_box = p->d_mem_box; a.mem_gap = p->d_mem_gap; a.mem_n = p->d_mem_n;
     a.out_kps = p->d_out_kps;
     mp_temporal_constants(c, a);
     if (launch_mp_temporal(a, n, sx)) return 1;
@@ -552,6 +563,15 @@ extern "C" SKPS_API int skps_mpipe_track_ids(skps_mpipe* p, int slot_i, int64_t*
 extern "C" SKPS_API int skps_mpipe_set_detect_every(skps_mpipe* p, int every) {
     SKPS_CHECK(p && every >= 1, "mpipe_set_detect_every: every %d is not >= 1", every);
     p->detect_every = every;
+    return 0;
+}
+
+extern "C" SKPS_API int skps_mpipe_set_id_memory(skps_mpipe* p, int frames) {
+    SKPS_CHECK(p && frames >= 0, "mpipe_set_id_memory: frames %d is not >= 0", frames);
+    SKPS_ON_DEVICE(p->device);
+    // switched off, every stream forgets its lost tracks; submits already queued keep the value they were made with
+    if (frames == 0 && p->id_memory > 0) SKPS_CUDA(cudaMemsetAsync(p->d_mem_n, 0, 4 * (size_t)p->S, p->s_compute));
+    p->id_memory = frames;
     return 0;
 }
 

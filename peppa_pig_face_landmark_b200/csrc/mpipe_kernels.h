@@ -28,6 +28,13 @@ struct MpTemporalArgs {
     const int* src;              // [S][K] source of each face this frame (launch_select), an index into the old track
     int64_t* ids;                // [S][K] track id of each track box
     int64_t* next_id;            // [S] the next unused id of the stream
+    // id memory (skps_mpipe_set_id_memory): the lost tracks of each stream, most recently lost first.  id_memory 0: off,
+    // the four pointers are not read and may be null
+    int id_memory;               // frames in a row a lost track may be missing and still give its id back
+    int64_t* mem_ids;            // [S][K] ids of the lost tracks
+    float* mem_box;              // [S][K][4] their float32 boxes of the frame that last returned them
+    int* mem_gap;                // [S][K] frames in a row each has been missing so far
+    int* mem_n;                  // [S] entries held
     // outputs
     double* out_kps;             // [S][K][P][2]
     // constants (python floats computed on the host exactly as lk.py does)

@@ -95,6 +95,36 @@ __global__ void __launch_bounds__(128) mp_temporal_kernel(const MpTemporalArgs a
     __shared__ int s_match;
     __shared__ int64_t s_ids[64];                                     // the old track ids (skps_mpipe_create: top_k <= 64)
     const int n = a.count[s];
+    // id memory: the old track boxes (overwritten below before the ids are assigned), the stream's lost tracks, and per
+    // face the entries it overlaps with IoU > iou_thres (bit k: entry k), all float32 as judge_boxs compares two such rows
+    __shared__ float s_old_box[64][4], s_mem_box[64][4];
+    __shared__ int64_t s_mem_id[64];
+    __shared__ int s_mem_gap[64];
+    __shared__ unsigned long long s_hit[64];
+    const bool mem_on = a.id_memory > 0;
+    int mem_n = 0;
+    if (mem_on) {
+        mem_n = a.mem_n[s];
+        const int n_old = a.n_track[s];
+        const float* tf = a.track_f32 + (long long)s * K * 4;
+        const float* mb = a.mem_box + (long long)s * K * 4;
+        for (int e = tid; e < 4 * n_old; e += blockDim.x) s_old_box[e >> 2][e & 3] = tf[e];
+        for (int e = tid; e < 4 * mem_n; e += blockDim.x) s_mem_box[e >> 2][e & 3] = mb[e];
+        for (int e = tid; e < mem_n; e += blockDim.x) {
+            s_mem_id[e] = a.mem_ids[(long long)s * K + e];
+            s_mem_gap[e] = a.mem_gap[(long long)s * K + e];
+        }
+        for (int e = tid; e < n; e += blockDim.x) s_hit[e] = 0ull;
+        __syncthreads();
+        const float* b4 = a.boxes4 + (long long)s * K * 4;
+        for (int e = tid; e < n * mem_n; e += blockDim.x) {
+            const int i = e / mem_n, k = e - i * mem_n;
+            Num r1[4], r2[4];
+            for (int c = 0; c < 4; ++c) { r1[c] = mk((double)b4[i * 4 + c], true); r2[c] = mk((double)s_mem_box[k][c], true); }
+            if (iou_gt(r1, r2, a.iou_thres)) atomicOr(&s_hit[i], 1ull << k);
+        }
+        __syncthreads();
+    }
     const float* now = a.kps_now + (long long)s * K * set;            // float32 (n, P, 2)
     const int cur = a.state_idx[s], nxt = cur ^ 1;
     const double* prev = a.prev_lm + ((long long)(s * 2 + cur) * K) * set;
@@ -190,22 +220,57 @@ __global__ void __launch_bounds__(128) mp_temporal_kernel(const MpTemporalArgs a
     }
     if (tid == 0) {
         // track ids, in output order: a face inherits the id of its source track box unless an earlier face of this frame
-        // took it; every other face gets the stream's next number.  The new ids are index-aligned with the new track boxes.
+        // took it; every other face takes back the id of the first lost track it overlaps that has been missing for at most
+        // id_memory frames, or else gets the stream's next number.  The new ids are index-aligned with the new track boxes.
         int64_t* ids = a.ids + (long long)s * K;
         const int n_old = a.n_track[s];
         for (int j = 0; j < n_old; ++j) s_ids[j] = ids[j];
         unsigned long long taken = 0ull;                              // bit j: track box j's id is given out (K <= 64)
+        unsigned long long used = 0ull;                               // bit k: memory entry k's id is given back
         int64_t next = a.next_id[s];
         for (int i = 0; i < n; ++i) {
             const int j = a.src[(long long)s * K + i];
             if (j >= 0 && j < n_old && !((taken >> j) & 1ull)) {
                 taken |= 1ull << j;
                 ids[i] = s_ids[j];
+                continue;
+            }
+            int k = -1;
+            if (mem_on) {
+                for (unsigned long long c = s_hit[i] & ~used; c && k < 0; c &= c - 1) {
+                    const int b = __ffsll((long long)c) - 1;
+                    if (s_mem_gap[b] <= a.id_memory) k = b;
+                }
+            }
+            if (k >= 0) {
+                used |= 1ull << k;
+                ids[i] = s_mem_id[k];
             } else {
                 ids[i] = next++;
             }
         }
         a.next_id[s] = next;
+        if (mem_on) {
+            // the new memory: the tracks this frame lost, in the order they were returned, then the older entries not given
+            // back that may still qualify at the next frame, oldest last; at most K
+            int64_t* mid = a.mem_ids + (long long)s * K;
+            float* mb = a.mem_box + (long long)s * K * 4;
+            int* mg = a.mem_gap + (long long)s * K;
+            int m = 0;
+            for (int j = 0; j < n_old && m < K; ++j) {
+                if ((taken >> j) & 1ull) continue;
+                mid[m] = s_ids[j]; mg[m] = 1;
+                for (int c = 0; c < 4; ++c) mb[m * 4 + c] = s_old_box[j][c];
+                ++m;
+            }
+            for (int k = 0; k < mem_n && m < K; ++k) {
+                if (((used >> k) & 1ull) || s_mem_gap[k] >= a.id_memory) continue;
+                mid[m] = s_mem_id[k]; mg[m] = s_mem_gap[k] + 1;
+                for (int c = 0; c < 4; ++c) mb[m * 4 + c] = s_mem_box[k][c];
+                ++m;
+            }
+            a.mem_n[s] = m;
+        }
         a.n_prev[s] = n;
         a.prev_f32[s] = all_f32 ? 1 : 0;
         a.n_track[s] = n;

@@ -131,6 +131,9 @@ SIGNATURES = {
     "skps_mpipe_pose_results": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp]),
     "skps_mpipe_set_detect_every": (C.c_int, [c_vp, C.c_int]),
     "skps_mpipe_detector_frames": (C.c_int, [c_vp, C.c_int, c_i32p]),
+    "skps_mpipe_set_id_memory": (C.c_int, [c_vp, C.c_int]),
+    "skps_debug_mp_temporal_mem": (C.c_int, [C.POINTER(PipelineCfg), C.c_int, C.c_int, C.c_int] + [c_vp] * 17 + [C.c_int]
+                                   + [c_vp] * 5),
 }
 
 _lib = None

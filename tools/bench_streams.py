@@ -7,7 +7,7 @@ host results out: every H2D / D2H is inside the timed region.
     python tools/bench_streams.py --align 112 [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
     python tools/bench_streams.py --pose [--parent-headpose OLD_headpose.cu --out DIR] [--rounds 5] [--configs ...]
     python tools/bench_streams.py --det-input H W [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
-    python tools/bench_streams.py --track-ids [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
+    python tools/bench_streams.py --track-ids [--id-memory N] [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
     python tools/bench_streams.py --detect-every N [--det-input H W] [--rounds 5] [--streams 16] [--batches 12] [--configs ...]
 
 --align SIZE times every config with and without aligned face chips (FaceAnaStreams(align=SIZE)) in the same process,
@@ -22,7 +22,8 @@ run and reports the largest difference of its skps_head_pose results from this b
 
 --det-input H W does the same with the detector at Skps.yml's 384x640 and at H x W (FaceAnaStreams(det_input=(H, W))).
 
---track-ids does the same without and with track ids in the results (FaceAnaStreams(track_ids=True)).
+--track-ids does the same without and with track ids in the results (FaceAnaStreams(track_ids=True)).  With --id-memory N
+it compares FaceAnaStreams(track_ids=True) and FaceAnaStreams(track_ids=True, id_memory=N) instead.
 
 --detect-every N does the same with FaceAnaStreams(detect_every=1) and (detect_every=N), at Skps.yml's detector input or,
 with --det-input H W, at H x W, and reports detector_frames_per_call of both (the mean of last_detector_frames).  Every
@@ -177,8 +178,8 @@ def time_align_kernel(torch, frame, kps, size, iters=200):
 
 def run_align_pair(name, size, n_streams=16, batches=12, warmup=3, rounds=5, length=6, feature="align"):
     """The same config with and without alignment (feature="align", chip side `size`), head pose (feature="pose"), track
-    ids (feature="track_ids") or the detector at input size `size` = (h, w) (feature="det_input"), alternating; median
-    ms_per_call of each."""
+    ids (feature="track_ids"), the memory of lost track ids (feature="id_memory", `size` frames, both with track ids) or
+    the detector at input size `size` = (h, w) (feature="det_input"), alternating; median ms_per_call of each."""
     import torch
     import frames
     from Skps import FaceAnaStreams
@@ -186,8 +187,9 @@ def run_align_pair(name, size, n_streams=16, batches=12, warmup=3, rounds=5, len
     seqs = make_streams(torch, frames, maker, n_streams, length=length)
     H, W = seqs[0][0].shape[:2]
     on = {"align": {"align": size}, "pose": {"pose": True}, "det_input": {"det_input": size},
-          "track_ids": {"track_ids": True}}[feature]
-    fas = {"off": FaceAnaStreams(n_streams=n_streams, top_k=topk, max_frame_hw=(H, W)),
+          "track_ids": {"track_ids": True}, "id_memory": {"track_ids": True, "id_memory": size}}[feature]
+    off = {"track_ids": True} if feature == "id_memory" else {}
+    fas = {"off": FaceAnaStreams(n_streams=n_streams, top_k=topk, max_frame_hw=(H, W), **off),
            "on": FaceAnaStreams(n_streams=n_streams, top_k=topk, max_frame_hw=(H, W), **on)}
     L = len(seqs[0])
 
@@ -237,6 +239,15 @@ def run_align_pair(name, size, n_streams=16, batches=12, warmup=3, rounds=5, len
                 "ms_per_call_track_ids_rounds": [1e3 * v / batches for v in times["on"]],
                 "faces_per_frame": faces["on"] / (n_streams * batches),
                 "api": "FaceAnaStreams.submit/collect, pinned host frames, 2 calls in flight; ids kept on the device"}
+    if feature == "id_memory":
+        del fas
+        ms = {k: 1e3 * float(np.median(v)) / batches for k, v in times.items()}
+        return {"config": name, "streams_per_gpu": n_streams, "calls": batches, "rounds": rounds, "id_memory": size,
+                "ms_per_call_id_memory_0": ms["off"], "ms_per_call_id_memory": ms["on"],
+                "ms_per_call_id_memory_0_rounds": [1e3 * v / batches for v in times["off"]],
+                "ms_per_call_id_memory_rounds": [1e3 * v / batches for v in times["on"]],
+                "faces_per_frame": faces["on"] / (n_streams * batches),
+                "api": "FaceAnaStreams(track_ids=True).submit/collect, pinned host frames, 2 calls in flight"}
     if feature == "pose":
         del fas
         return {"config": name, "streams_per_gpu": n_streams, "calls": batches, "rounds": rounds,
@@ -466,7 +477,11 @@ def main():
         rounds = int(opt("--rounds", 5))
         print(json.dumps(gpu_info(torch)))
         for name in names:
-            print(json.dumps(run_align_pair(name, 0, n_streams, batches, rounds=rounds, feature="track_ids")))
+            if "--id-memory" in a:
+                r = run_align_pair(name, int(opt("--id-memory", 0)), n_streams, batches, rounds=rounds, feature="id_memory")
+            else:
+                r = run_align_pair(name, 0, n_streams, batches, rounds=rounds, feature="track_ids")
+            print(json.dumps(r))
             sys.stdout.flush()
         return
     if "--align" in a:
