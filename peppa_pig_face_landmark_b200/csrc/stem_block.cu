@@ -11,8 +11,13 @@
 // tensor, everything in between lives in shared memory.  The work is ~1.2 M FMAs per tile on tensors with 3 / 16 input
 // channels.  The stem, the block-0 depthwise and its 16->16 pointwise run on the FP32 pipes with every dense weight taken from
 // the kernel-parameter (constant) bank (FFMA with a constant operand, each activation read from shared memory once per 16
-// outputs); the 16->E expansion - half of the FMAs - is a single wgmma K-step per 128 window pixels; the next tile's input
+// outputs); the 16->E expansion - half of the FMAs - is a single wgmma K-step per 64 window pixels; the next tile's input
 // window is prefetched into registers.
+//
+// Per tile, between CTA-wide barriers: S0 input window -> S1 stem -> S2 block-0 depthwise (warp-uniform channel group) ->
+// S3 block-0 pointwise into the fp16 hi/lo A operand -> then, per 16-channel chunk ch of the expansion, one interval that
+// issues the wgmma of chunk ch, runs the stride-2 depthwise and output store of chunk ch - 1 while it is in flight, and
+// writes chunk ch through bias / ReLU / mask into the other of two chunk buffers.  A tile takes 4 + E / 16 + 1 barriers.
 #include <cuda_fp16.h>
 #include <string.h>
 
@@ -30,15 +35,15 @@ constexpr int SB_IH = 2 * SB_SH + 1, SB_IW = 2 * SB_SW + 1;   // 39 x 71: input 
 constexpr int SB_PS = 20;                                  // floats per pixel in shared memory (16 + pad: conflict-free float4 rows)
 constexpr int SB_NE = SB_EH * SB_EW, SB_NS = SB_SH * SB_SW, SB_NI = SB_IH * SB_IW;
 constexpr int SB_A_FLOATS = (SB_NI * 4 > SB_NE * SB_PS) ? SB_NI * 4 : SB_NE * SB_PS;    // input window, later block-0 depthwise output
-constexpr int SB_B_FLOATS = SB_NS * SB_PS;                 // stem output, later one 16-channel chunk of the expanded tensor
+constexpr int SB_B_FLOATS = SB_NS * SB_PS;                 // stem output, later the even 16-channel chunks of the expanded tensor
 // The 16 -> E expansion (half of the block's FMAs) is ONE wgmma K-step.  S3 writes the block-0 output as float16 hi/lo rows
-// (64-byte swizzled rows of which only the first 32 bytes = 16 channels are used), five 128-row MMA tiles cover the 561
-// window pixels, per 16-channel chunk the accumulators live in registers and S4 is wgmma -> bias/ReLU/mask -> shared
-// memory.  Same fp16 hi/lo three-product scheme as conv_tc.cu.
+// (64-byte swizzled rows of which only the first 32 bytes = 16 channels are used), nine 64-row MMA blocks cover the 561
+// window pixels (warpgroup 0 takes three, warpgroups 1-3 two each), per 16-channel chunk the accumulators live in
+// registers and S4 is wgmma -> bias/ReLU/mask -> shared memory.  Same fp16 hi/lo three-product scheme as conv_tc.cu.
 constexpr int SB_T_TILES = (SB_NE + 127) / 128;            // 5
 constexpr int SB_T_PLANE = SB_T_TILES * 128 * 64;          // one plane of the A operand: 640 rows x 64 B
 constexpr int SB_WB_PLANE = SB_MAX_E * 64;                 // one plane of the B operand: E rows x 64 B
-constexpr int SB_SMEM = (SB_A_FLOATS + SB_B_FLOATS + 10 * SB_MAX_E + 256) * 4 + 1024 + 2 * SB_T_PLANE + 2 * SB_WB_PLANE;
+constexpr int SB_SMEM = (SB_A_FLOATS + SB_B_FLOATS + 11 * SB_MAX_E + 256) * 4 + 1024 + 2 * SB_T_PLANE + 2 * SB_WB_PLANE;
 
 // 8 floats -> 16 bytes of float16 hi and 16 bytes of float16 lo (v = hi + lo)
 __device__ __forceinline__ void split8(const float* v, uint4& hi, uint4& lo) {
@@ -56,25 +61,26 @@ __device__ __forceinline__ void split8(const float* v, uint4& hi, uint4& lo) {
 
 __device__ __forceinline__ float hswish_f(float v) { return v * hsigmoid_f(v); }
 
-// block-0 depthwise: 4 consecutive pixels of one window row x channel group G (weights as constant operands)
+// block-0 depthwise: 3 consecutive pixels of one window row x channel group G (weights as constant operands).  Strips of
+// 3 tile the 33-pixel row exactly, and 8 lanes on consecutive strips of a row read 8 distinct bank quads (pixel stride 20
+// floats, strip stride 60 floats = 7 quads mod 8)
+constexpr int SB_STRIP = 3;
 template <int G>
 __device__ __forceinline__ void dw16_strip(const float* __restrict__ s1, float* __restrict__ s2, int row, int x0, const StemBlockW& Wt) {
-    float4 acc[4];
+    float4 acc[SB_STRIP];
 #pragma unroll
-    for (int q = 0; q < 4; ++q) acc[q] = make_float4(Wt.dw0_b[4 * G], Wt.dw0_b[4 * G + 1], Wt.dw0_b[4 * G + 2], Wt.dw0_b[4 * G + 3]);
+    for (int q = 0; q < SB_STRIP; ++q) acc[q] = make_float4(Wt.dw0_b[4 * G], Wt.dw0_b[4 * G + 1], Wt.dw0_b[4 * G + 2], Wt.dw0_b[4 * G + 3]);
 #pragma unroll
     for (int ky = 0; ky < 3; ++ky) {
-        float4 in[6];
+        float4 in[SB_STRIP + 2];
 #pragma unroll
-        for (int i = 0; i < 6; ++i) {
-            const int xx = min(x0 + i, SB_SW - 1);          // the last strip of a row hangs over by up to 3 columns
-            in[i] = *reinterpret_cast<const float4*>(s1 + ((row + ky) * SB_SW + xx) * SB_PS + 4 * G);
-        }
+        for (int i = 0; i < SB_STRIP + 2; ++i)
+            in[i] = *reinterpret_cast<const float4*>(s1 + ((row + ky) * SB_SW + x0 + i) * SB_PS + 4 * G);
 #pragma unroll
         for (int kx = 0; kx < 3; ++kx) {
             const int t = ky * 3 + kx;
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
+            for (int q = 0; q < SB_STRIP; ++q) {
                 acc[q].x = fmaf(in[q + kx].x, Wt.dw0_w[t * 16 + 4 * G], acc[q].x);
                 acc[q].y = fmaf(in[q + kx].y, Wt.dw0_w[t * 16 + 4 * G + 1], acc[q].y);
                 acc[q].z = fmaf(in[q + kx].z, Wt.dw0_w[t * 16 + 4 * G + 2], acc[q].z);
@@ -83,8 +89,7 @@ __device__ __forceinline__ void dw16_strip(const float* __restrict__ s1, float* 
         }
     }
 #pragma unroll
-    for (int q = 0; q < 4; ++q) {
-        if (x0 + q >= SB_EW) break;
+    for (int q = 0; q < SB_STRIP; ++q) {
         float4 v = acc[q];
         v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
         *reinterpret_cast<float4*>(s2 + (row * SB_EW + x0 + q) * SB_PS + 4 * G) = v;
@@ -113,16 +118,18 @@ __global__ void __launch_bounds__(SB_THREADS, 1)
 stem_block_kernel(const StemBlockK p, const __grid_constant__ StemBlockW Wt) {
     extern __shared__ __align__(16) float sm[];
     __shared__ float s_wmax[SB_THREADS / 32];
-    float* sA = sm;                                    // input window (float4 per pixel: b, g, r, 0), later s2
-    float* sB = sA + SB_A_FLOATS;                      // stem output s1, later the expanded chunk
+    float* sA = sm;                                    // input window (float4 per pixel: b, g, r, 0), later s2, then odd chunks
+    float* sB = sA + SB_A_FLOATS;                      // stem output s1, later the even expanded chunks
     float* sW = sB + SB_B_FLOATS;                      // stride-2 depthwise weights [9][E] + bias [E]
-    float* lut = sW + 10 * SB_MAX_E;                   // i / 255
+    float* sPB = sW + 10 * SB_MAX_E;                   // expansion bias [E]
+    float* lut = sPB + SB_MAX_E;                       // i / 255
     // A operand (block-0 output as fp16 hi/lo rows), then the B operand (expand weights), 1024-byte aligned
     const uint32_t sT = (smem_u32(lut + 256) + 1023u) & ~1023u;
     const uint32_t sWB = sT + 2u * SB_T_PLANE;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     for (int i = tid; i < 256; i += SB_THREADS) lut[i] = __fdiv_rn((float)i, 255.f);
     for (int i = tid; i < 10 * E; i += SB_THREADS) sW[i] = p.dw1[i];
+    for (int i = tid; i < E; i += SB_THREADS) sPB[i] = Wt.pw1_b[i];
     const int tiles_x = p.Wq / SB_TW, tiles_per_img = tiles_x * (p.Hq / SB_TH);
     const int Hh = p.H / 2, Wh = p.W / 2;              // half-resolution map
     // expand weights -> fp16 hi/lo B operand [E rows][16 K], pre-multiplied by an exact power of two (undone after the
@@ -251,11 +258,13 @@ stem_block_kernel(const StemBlockK p, const __grid_constant__ StemBlockW Wt) {
             *reinterpret_cast<float4*>(o + 4) = make_float4(acc[4], acc[5], acc[6], acc[7]);
         }
         __syncthreads();
-        // ---- S2: blocks.0.0 depthwise 3x3 + ReLU over the 17 x 33 window; item = (4-pixel strip, 4-channel group)
+        // ---- S2: blocks.0.0 depthwise 3x3 + ReLU over the 17 x 33 window; item = (3-pixel strip, 4-channel group)
         {
-            constexpr int STRIPS = (SB_EW + 3) / 4;            // 9 strips per row, the last one 1 pixel wide
-            for (int it = tid; it < SB_EH * STRIPS * 4; it += SB_THREADS) {
-                const int g = it & 3, sidx = it >> 2, row = sidx / STRIPS, x0 = (sidx - row * STRIPS) * 4;
+            constexpr int STRIPS = SB_EW / SB_STRIP, NSTRIP = SB_EH * STRIPS;     // 11 strips per row, 187 in all
+            for (int it = tid; it < 4 * ((NSTRIP + 31) / 32) * 32; it += SB_THREADS) {
+                const int g = (it >> 5) & 3, sidx = ((it >> 7) << 5) | (it & 31);    // the channel group is warp-uniform
+                if (sidx >= NSTRIP) continue;
+                const int row = sidx / STRIPS, x0 = (sidx - row * STRIPS) * SB_STRIP;
                 switch (g) {
                     case 0: dw16_strip<0>(sB, sA, row, x0, Wt); break;
                     case 1: dw16_strip<1>(sB, sA, row, x0, Wt); break;
@@ -288,78 +297,103 @@ stem_block_kernel(const StemBlockK p, const __grid_constant__ StemBlockW Wt) {
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
-        // ---- S4/S5 per 16-channel chunk of the expanded tensor: 1x1 16->E + ReLU into sB, then depthwise 3x3 s2 + ReLU
+        // ---- S4/S5 per 16-channel chunk ch of the expanded tensor: 1x1 16->E + ReLU into xb[ch & 1] (S4), then depthwise
+        // 3x3 s2 + ReLU from it to the output (S5).  Warpgroups 0-3 run both; one barrier interval holds S4 of chunk ch and
+        // S5 of chunk ch - 1, whose shared-memory reads and FMAs cover the wgmma of chunk ch.  sA (block-0 depthwise output)
+        // is dead after S3 and holds the odd chunks.
         if (!p.in_f32 && tile + (int)gridDim.x < p.n_tiles) prefetch(tile + gridDim.x);     // in flight during S4 / S5
         const int y_ok0 = max(0, -ey0), y_ok1 = min(SB_EH, Hh - ey0), x_ok0 = max(0, -ex0), x_ok1 = min(SB_EW, Wh - ex0);
+        float* const xb[2] = {sB, sA};
+        const int wg = warp >> 2, w = warp & 3;
+        // warpgroup wg multiplies the 64-row MMA blocks wg and wg + 4 of the window pixels, warpgroup 0 also block 8
+        float acc[3][8];
+        auto mma_issue = [&](int ch) {
+            const uint64_t b_hi = make_smem_desc_sw64(sWB + (uint32_t)(ch * 16 * 64));
+            const uint64_t b_lo = make_smem_desc_sw64(sWB + (uint32_t)SB_WB_PLANE + (uint32_t)(ch * 16 * 64));
+            auto blk = [&](float* d, int m) {
+                const uint32_t ao = sT + (uint32_t)m * 4096u;
+                wg_mma3<16>(d, make_smem_desc_sw64(ao), make_smem_desc_sw64(ao + (uint32_t)SB_T_PLANE), b_hi, b_lo, 0u);
+            };
+            // straight-line issue per warpgroup role (a branch inside the group would serialise the wgmma)
+            if (wg == 0) {
+                wg_fence();
+                blk(acc[0], 0);
+                blk(acc[1], 4);
+                blk(acc[2], 8);
+                wg_commit();
+            } else {
+                wg_fence();
+                blk(acc[0], wg);
+                blk(acc[1], wg + 4);
+                wg_commit();
+            }
+        };
+        // accumulator fragment of block m: rows 64m + 16w + lane/4 (+8), columns 8i + 2(lane%4) (+1), written as column pairs
+        // through bias / ReLU / mask
+        auto epilogue = [&](int ch, float* dst) {
 #pragma unroll
-        for (int ch = 0; ch < E / 16; ++ch) {
-            // warpgroup g < 4 multiplies MMA tile g (window pixels 128g ..) by the 16 expand weights of chunk ch, warpgroup 0
-            // also tile 4; each thread then writes its accumulator fragment (rows 64h + 16w + lane/4 (+8), columns
-            // 8i + 2(lane%4) (+1)) through bias / ReLU / mask straight into sB
-            const int wg = warp >> 2, w = warp & 3;
-            if (wg < 4) {
-                const uint64_t b_hi = make_smem_desc_sw64(sWB + (uint32_t)(ch * 16 * 64));
-                const uint64_t b_lo = make_smem_desc_sw64(sWB + (uint32_t)SB_WB_PLANE + (uint32_t)(ch * 16 * 64));
-                float acc[2][16];
-                // straight-line issue per warpgroup role (a branch inside the group would serialise the wgmma)
-                auto mma_tile = [&](float* d, int m) {
+            for (int t = 0; t < 3; ++t) {
+                if (t == 2 && wg) break;
+                const int m = t == 2 ? 8 : wg + 4 * t;
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const uint32_t ao = sT + (uint32_t)m * 8192u + (uint32_t)h * 4096u;
-                        wg_mma3<16>(d + 8 * h, make_smem_desc_sw64(ao), make_smem_desc_sw64(ao + (uint32_t)SB_T_PLANE), b_hi,
-                                    b_lo, 0u);
-                    }
-                };
-                if (wg == 0) {
-                    wg_fence();
-                    mma_tile(acc[0], 0);
-                    mma_tile(acc[1], 4);
-                    wg_commit();
-                    wg_wait0();
-                } else {
-                    wg_fence();
-                    mma_tile(acc[0], wg);
-                    wg_commit();
-                    wg_wait0();
-                }
+                for (int rr = 0; rr < 2; ++rr) {
+                    const int px = 64 * m + 16 * w + (lane >> 2) + 8 * rr;
+                    if (px < SB_NE) {
+                        const int r = px / SB_EW, c = px - r * SB_EW;
+                        const bool inside = r >= y_ok0 && r < y_ok1 && c >= x_ok0 && c < x_ok1;
 #pragma unroll
-                for (int t = 0; t < 2; ++t) {
-                    const int m = t ? 4 : wg;
-                    if (t && wg) break;
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int h = j >> 3, i = (j >> 2) & 1, e = j & 3;
-                        const int px = 128 * m + 64 * h + 16 * w + (lane >> 2) + 8 * (e >> 1);
-                        const int co = 8 * i + 2 * (lane & 3) + (e & 1);
-                        if (px < SB_NE) {
-                            const int r = px / SB_EW, c = px - r * SB_EW;
-                            const bool inside = r >= y_ok0 && r < y_ok1 && c >= x_ok0 && c < x_ok1;
-                            sB[px * SB_PS + co] = inside ? fmaxf(fmaf(acc[t][j], w_inv, Wt.pw1_b[ch * 16 + co]), 0.f) : 0.f;
+                        for (int i = 0; i < 2; ++i) {
+                            const int co = 8 * i + 2 * (lane & 3);
+                            const float2 bb = *reinterpret_cast<const float2*>(sPB + ch * 16 + co);
+                            float2 v;
+                            v.x = inside ? fmaxf(fmaf(acc[t][4 * i + 2 * rr], w_inv, bb.x), 0.f) : 0.f;
+                            v.y = inside ? fmaxf(fmaf(acc[t][4 * i + 2 * rr + 1], w_inv, bb.y), 0.f) : 0.f;
+                            *reinterpret_cast<float2*>(dst + px * SB_PS + co) = v;
                         }
                     }
                 }
             }
-            __syncthreads();
-            // depthwise 3x3 stride 2: item = (output pixel, 4-channel group) = 128 x 4 = 512 items
-            if (tid < SB_TH * SB_TW * 4) {
-                const int g = tid & 3, opx = tid >> 2, orow = opx / SB_TW, ocol = opx - orow * SB_TW;
-                const int c0 = ch * 16 + 4 * g;
-                float4 acc = *reinterpret_cast<const float4*>(sW + 9 * E + c0);
+        };
+        // depthwise 3x3 stride 2: item = (output pixel, 4-channel group), 128 x 4 = 512 items on warpgroups 0-3.  A quarter
+        // warp takes 4 consecutive output columns x 2 groups: 8 distinct bank quads of the 20-float pixel rows.
+        auto dw_s2 = [&](int ch, const float* src) {
+            const int g = (lane & 1) | ((lane >> 2) & 2);
+            const int ocol = ((lane >> 1) & 3) | ((lane >> 2) & 4) | ((warp & 1) << 3), orow = warp >> 1;
+            const int c0 = ch * 16 + 4 * g;
+            float4 a = *reinterpret_cast<const float4*>(sW + 9 * E + c0);
 #pragma unroll
-                for (int ky = 0; ky < 3; ++ky)
+            for (int ky = 0; ky < 3; ++ky)
 #pragma unroll
-                    for (int kx = 0; kx < 3; ++kx) {
-                        const float4 v = *reinterpret_cast<const float4*>(sB + ((2 * orow + ky) * SB_EW + 2 * ocol + kx) * SB_PS + 4 * g);
-                        const float4 w = *reinterpret_cast<const float4*>(sW + (ky * 3 + kx) * E + c0);
-                        acc.x = fmaf(v.x, w.x, acc.x); acc.y = fmaf(v.y, w.y, acc.y);
-                        acc.z = fmaf(v.z, w.z, acc.z); acc.w = fmaf(v.w, w.w, acc.w);
-                    }
-                acc.x = fmaxf(acc.x, 0.f); acc.y = fmaxf(acc.y, 0.f); acc.z = fmaxf(acc.z, 0.f); acc.w = fmaxf(acc.w, 0.f);
-                const long long o = (((long long)img * p.Hq + oy0 + orow) * p.Wq + ox0 + ocol) * p.out_ld + p.out_coff + c0;
-                st4(p.out, p.out_fmt, p.out_plane, o, acc);
+                for (int kx = 0; kx < 3; ++kx) {
+                    const float4 v = *reinterpret_cast<const float4*>(src + ((2 * orow + ky) * SB_EW + 2 * ocol + kx) * SB_PS + 4 * g);
+                    const float4 wv = *reinterpret_cast<const float4*>(sW + (ky * 3 + kx) * E + c0);
+                    a.x = fmaf(v.x, wv.x, a.x); a.y = fmaf(v.y, wv.y, a.y);
+                    a.z = fmaf(v.z, wv.z, a.z); a.w = fmaf(v.w, wv.w, a.w);
+                }
+            a.x = fmaxf(a.x, 0.f); a.y = fmaxf(a.y, 0.f); a.z = fmaxf(a.z, 0.f); a.w = fmaxf(a.w, 0.f);
+            const long long o = (((long long)img * p.Hq + oy0 + orow) * p.Wq + ox0 + ocol) * p.out_ld + p.out_coff + c0;
+            st4(p.out, p.out_fmt, p.out_plane, o, a);
+        };
+        if (wg < 4) {
+            mma_issue(0);
+            wg_wait0();
+            wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]);
+            epilogue(0, xb[0]);
+        }
+        __syncthreads();
+#pragma unroll
+        for (int ch = 1; ch < E / 16; ++ch) {
+            if (wg < 4) {
+                mma_issue(ch);
+                dw_s2(ch - 1, xb[(ch - 1) & 1]);
+                wg_wait0();
+                wg_fence_acc(acc[0]); wg_fence_acc(acc[1]); wg_fence_acc(acc[2]);
+                epilogue(ch, xb[ch & 1]);
             }
             __syncthreads();
         }
+        if (wg < 4) dw_s2(E / 16 - 1, xb[(E / 16 - 1) & 1]);
+        __syncthreads();
     }
 }
 
