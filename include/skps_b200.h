@@ -429,6 +429,14 @@ SKPS_API int skps_mpipe_dims(const skps_mpipe* p, int* n_streams, int* top_k, in
  * Pinned frames must stay valid until skps_mpipe_wait(slot).  Frames on the device go through skps_mpipe_submit_device.
  * Asynchronous. */
 SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot, const uint8_t* const* frames, const int32_t* hw, int n);
+/* skps_mpipe_submit for any subset of the streams, in any order: frame i is the next frame of stream streams[i].  streams
+ * [host] int32 (n), distinct ids in 0..n_streams-1, or NULL for stream i (what skps_mpipe_submit does).  Everything per
+ * call stays in call order: hw, and every result of the batch (entry i of skps_mpipe_wait, the track ids, chips, pose and
+ * device outputs belongs to frame i).  A stream the call does not feed is untouched: its frame count, previous frame,
+ * track boxes, landmark history, ids and lost tracks stay as they are.  Duplicate or out-of-range ids fail before anything
+ * is enqueued.  A batch costs what its n frames cost, whatever n_streams is. */
+SKPS_API int skps_mpipe_submit_streams(skps_mpipe* p, int slot, const int32_t* streams, const uint8_t* const* frames,
+                                       const int32_t* hw, int n);
 /* Block until the slot's results are in host memory.  Per stream s < n: n_faces[s]; boxes (n, top_k, 4) float64 = the
  * refreshed track boxes (the 'box' entries of FaceAna.run); kps (n, top_k, n_points, 2) float64 smoothed landmarks;
  * scores (n, top_k, n_points) float32; ran_detector[s] (may be NULL) = the frame used the detector's rows (the
@@ -458,6 +466,11 @@ typedef struct skps_mpipe_outputs {
  * completed by skps_mpipe_wait_stream.  Asynchronous. */
 SKPS_API int skps_mpipe_submit_device(skps_mpipe* p, int slot, const uint8_t* const* frames, const int32_t* pitches,
                                       const int32_t* hw, int n, const skps_mpipe_outputs* out, void* producer_stream);
+/* skps_mpipe_submit_device for any subset of the streams, in any order, as skps_mpipe_submit_streams: frame i is the next
+ * frame of stream streams[i] (streams NULL: stream i); pitches, hw and the rows of *out are in call order. */
+SKPS_API int skps_mpipe_submit_device_streams(skps_mpipe* p, int slot, const int32_t* streams, const uint8_t* const* frames,
+                                              const int32_t* pitches, const int32_t* hw, int n, const skps_mpipe_outputs* out,
+                                              void* producer_stream);
 /* Completes a slot submitted with device outputs without blocking the host: work queued on `consumer_stream` after this
  * call runs after the batch's results are in the caller's buffers.  The slot can then be submitted again. */
 SKPS_API int skps_mpipe_wait_stream(skps_mpipe* p, int slot, void* consumer_stream);

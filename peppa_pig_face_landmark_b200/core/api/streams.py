@@ -2,11 +2,15 @@
 
 The reference serves one stream per FaceAna instance and keeps the temporal state (previous frame, track boxes,
 GroupTrack / One-Euro history; facer.py:28-50, lk.py:6-91) in Python.  Here one object owns S streams: each call takes
-one frame per stream and runs ONE detector forward and ONE landmark forward for all of them, the state lives on the
-device (csrc/mpipe.cu, csrc/temporal.cu) and two batches can be in flight so that frame uploads overlap compute.
+one frame for each of any subset of the streams and runs ONE detector forward and ONE landmark forward for all of them,
+the state lives on the device (csrc/mpipe.cu, csrc/temporal.cu) and two batches can be in flight so that frame uploads
+overlap compute.
 
     fa = FaceAnaStreams(n_streams=16, top_k=4)
     results = fa.run(frames)            # list of S lists of {'box','kps','scores'} - what S FaceAna.run calls return
+    # cameras at their own frame rates: frames for streams 5, 2 and 9 only; results[i] is stream [5, 2, 9][i]'s, and the
+    # other streams are untouched (no frame counted, no filter step, no id_memory gap)
+    results = fa.run([f5, f2, f9], streams=[5, 2, 9])
     # FaceAnaStreams(..., align=112): each dict also has 'chip' (112x112x3 uint8, aligned) and 'M' (2x3 float64)
     # FaceAnaStreams(..., pose=True): each dict also has 'pose' {'euler', 'rvec', 'tvec', 'reproject'} as FaceAna returns it
     # FaceAnaStreams(..., track_ids=True): each dict also has 'id', the track id FaceAna(track_ids=True) gives the face
@@ -32,6 +36,29 @@ from .facer import check_detect_every, check_id_memory, get_cfg, pipeline_cfg
 from .onnx_model_base import ONNXEngine
 
 
+def check_streams(streams, n, n_streams):
+    """The streams of a call of n frames as a list of ints, or None for streams 0..n-1 (streams None): a sequence of n
+    distinct ints in 0..n_streams-1, one per frame, else ValueError."""
+    if streams is None:
+        return None
+    if isinstance(streams, (str, bytes)) or not hasattr(streams, "__len__"):
+        raise ValueError("streams must be a sequence of ints, got %r" % (streams,))
+    ids = list(streams)
+    if len(ids) != n:
+        raise ValueError("streams: %d ids for %d frames" % (len(ids), n))
+    for i, t in enumerate(ids):
+        if not isinstance(t, (int, np.integer)) or isinstance(t, (bool, np.bool_)):
+            raise ValueError("streams[%d] must be an int, got %r" % (i, t))
+        if not 0 <= t < n_streams:
+            raise ValueError("streams[%d] = %d is outside 0..%d" % (i, t, n_streams - 1))
+    ids = [int(t) for t in ids]
+    if len(set(ids)) != n:
+        # two frames of one stream in one call would depend on each other: the second's previous frame is the first
+        dup = sorted({t for t in ids if ids.count(t) > 1})
+        raise ValueError("streams: each stream takes at most one frame per call, got %s more than once" % dup)
+    return ids
+
+
 class FaceAnaStreams:
     def __init__(self, n_streams, top_k=None, max_frame_hw=(2160, 3840), device="cuda", align=None, pose=False,
                  det_input=None, track_ids=False, detect_every=1, id_memory=0):
@@ -47,7 +74,8 @@ class FaceAnaStreams:
         FaceAna's.  The ids are kept on the device next to the track boxes, whether or not they are returned.
         id_memory: FaceAna(track_ids=True, id_memory=...) for every stream: up to top_k lost tracks per stream (about 28
         bytes each) whose ids a face that reappears where one was lost takes back, kept and matched on the device.  A
-        stream's frames are the calls that include it; reset(stream) forgets its lost tracks.
+        stream's frames are the calls that include it (submit(streams=...)): a call without it does not age its lost
+        tracks; reset(stream) forgets them.
         detect_every: the detection cadence of FaceAna(detect_every=N, detect_offset=s % N) for stream s, which it
         returns bit for bit.  A stream counts its frames from construction or reset(stream), advancing only on calls
         that include a frame for it; frame i runs the detector when the stream has no previous frame of its size, or
@@ -55,7 +83,13 @@ class FaceAnaStreams:
         enters is found up to N - 1 frames late; one that leaves is followed by its landmark box until the next keyframe.
         The staggered offsets spread the keyframes over the calls: the detector runs on about n_streams / N frames per
         call, packed into one batch, and not at all on a call without keyframes (last_detector_frames).  The detector
-        engine keeps one CUDA graph per batch size it meets; with the stagger those are only a few sizes."""
+        engine keeps one CUDA graph per batch size it meets; with the stagger those are only a few sizes.  The offset is
+        keyed to the stream id, not to the frame's position in a call.
+
+        Streams need not be frame-synchronous: a call feeds any subset of them, in any order (submit(streams=...)), and
+        costs what its frames cost - the detector batch is its keyframes, the landmark batch len(frames) * top_k faces.
+        A stream a call does not feed is untouched: no frame is counted, no filter step runs, no id_memory gap is counted,
+        its cadence phase does not move and its previous frame stays."""
         self.detect_every = check_detect_every(detect_every)[0]
         self.id_memory = check_id_memory(id_memory, track_ids)
         self.align = None if align is None else check_size(align)
@@ -121,9 +155,16 @@ class FaceAnaStreams:
             self.collect()
         rt.check(self.lib.skps_mpipe_reset(self._h, -1 if stream is None else int(stream)))
 
-    def submit(self, frames, out=None):
-        """Enqueue one frame per stream (frames[i] -> stream i, len(frames) <= n_streams).  At most two batches may be
-        pending; results come back from collect() in submission order.
+    def submit(self, frames, out=None, streams=None):
+        """Enqueue one frame for each of some streams.  At most two batches may be pending; results come back from
+        collect() in submission order.
+
+        streams: None, frames[i] -> stream i (len(frames) <= n_streams); or a sequence of distinct ints in
+        0..n_streams-1, one per frame in any order, frames[i] being the next frame of stream streams[i].  Everything per
+        call stays in call order: collect()'s entry i, last_ran_detector[i] and, with out=, row i of every result tensor
+        belong to frames[i].  A stream the call does not feed is untouched (its frame count, cadence phase, filters,
+        previous frame, track boxes, ids and lost tracks stay as they are).  A length mismatch, a duplicate, an id out of
+        range or one that is not an int raises ValueError before anything is enqueued.
 
         frames: all HxWx3 uint8 BGR numpy arrays, or all torch.uint8 CUDA tensors (H, W, 3) in BGR order on this object's
         device with stride(2) == 1, stride(1) == 3 and any row pitch stride(0) >= 3W (packed tensors, pitched decoder
@@ -139,12 +180,14 @@ class FaceAnaStreams:
         n = len(frames)
         if not 0 < n <= self.n_streams:
             raise ValueError("expected 1..%d frames, got %d" % (self.n_streams, n))
+        ids = check_streams(streams, n, self.n_streams)
+        smap = None if ids is None else np.array(ids, np.int32)
         on_device = [is_cuda_tensor(f) for f in frames]
         if any(on_device):
             if not all(on_device):
                 raise ValueError("one batch takes either host frames or CUDA frames, got both (streams %s are CUDA)"
                                  % [i for i, d in enumerate(on_device) if d])
-            self._submit_device(frames, out)
+            self._submit_device(frames, out, smap)
             return
         if out is not None:
             raise ValueError("out= keeps results on the GPU and takes CUDA frames; these are host frames")
@@ -152,11 +195,12 @@ class FaceAnaStreams:
         ptrs = (C.c_void_p * n)(*[f.ctypes.data for f in keep])
         hw = np.array([[f.shape[0], f.shape[1]] for f in keep], np.int32)
         slot = self._next
-        rt.check(self.lib.skps_mpipe_submit(self._h, slot, ptrs, hw.ctypes.data, n))
+        rt.check(self.lib.skps_mpipe_submit_streams(self._h, slot, None if smap is None else smap.ctypes.data, ptrs,
+                                                    hw.ctypes.data, n))
         self._pending.append((slot, n, keep, None))
         self._next ^= 1
 
-    def _submit_device(self, frames, out):
+    def _submit_device(self, frames, out, smap):
         import torch
         n = len(frames)
         layout = [check_cuda_frame(f, self.device, self.max_frame_hw) for f in frames]
@@ -173,9 +217,10 @@ class FaceAnaStreams:
         pitches = np.array([p for _, _, p in layout], np.int32)
         hw = np.array([[h, w] for h, w, _ in layout], np.int32)
         slot = self._next
-        rt.check(self.lib.skps_mpipe_submit_device(self._h, slot, ptrs, pitches.ctypes.data, hw.ctypes.data, n,
-                                                   None if outs is None else C.byref(outs),
-                                                   torch.cuda.current_stream(self.device).cuda_stream))
+        rt.check(self.lib.skps_mpipe_submit_device_streams(self._h, slot, None if smap is None else smap.ctypes.data, ptrs,
+                                                           pitches.ctypes.data, hw.ctypes.data, n,
+                                                           None if outs is None else C.byref(outs),
+                                                           torch.cuda.current_stream(self.device).cuda_stream))
         self._pending.append((slot, n, list(frames), out))
         self._next ^= 1
 
@@ -196,11 +241,12 @@ class FaceAnaStreams:
 
     def new_results(self):
         """Device result buffers for submit(cuda_frames, out=...): a dict of CUDA tensors on this object's device,
-        n (S,) int32 faces per stream; ran_detector (S,) int32, whether the frame used the detector's rows (a keyframe
+        n (S,) int32 faces per frame; ran_detector (S,) int32, whether the frame used the detector's rows (a keyframe
         whose frame-difference gate fired, or with no previous frame of its size); box (S,K,4) and kps
         (S,K,P,2) float64; scores (S,K,P) float32; with align, chip (S,K,size,size,3) uint8 and M (S,K,2,3) float64; with
-        pose, rvec, tvec, euler (S,K,3) and reproject (S,K,8,2) float64; with track_ids, id (S,K) int64.  Per stream s,
-        face rows i >= n[s] (and streams past the batch's length) are unspecified."""
+        pose, rvec, tvec, euler (S,K,3) and reproject (S,K,8,2) float64; with track_ids, id (S,K) int64.  Row i belongs
+        to frames[i] of the submit, in call order whatever its streams=; face rows j >= n[i] of row i, and rows
+        i >= len(frames), are unspecified."""
         import torch
         return {k: torch.empty(shape, dtype=dt, device=self.device) for k, (shape, dt) in self._result_layout().items()}
 
@@ -222,8 +268,8 @@ class FaceAnaStreams:
             raise ValueError("out: these buffers belong to a batch still in flight; collect() it first")
 
     def collect(self):
-        """Results of the oldest pending batch: a list (one entry per stream) of lists of {'box','kps','scores'}; for a
-        batch submitted with out=, that dict, with no host synchronisation: torch.cuda.current_stream() is made to wait
+        """Results of the oldest pending batch: a list, entry i for frames[i] of its submit (stream i, or streams[i]),
+        of lists of {'box','kps','scores'}; last_ran_detector[i] likewise; for a batch submitted with out=, that dict, with no host synchronisation: torch.cuda.current_stream() is made to wait
         for the batch, so work queued on it afterwards sees the results (last_ran_detector is then None; the gate's
         decisions are out['ran_detector'])."""
         if not self._pending:
@@ -265,7 +311,7 @@ class FaceAnaStreams:
                     r['id'] = int(o["ids"][s, i])
         return res
 
-    def run(self, frames):
-        """One frame per stream in, per-stream results out (blocking)."""
-        self.submit(frames)
+    def run(self, frames, streams=None):
+        """One frame for each of some streams in (submit's streams=), their results out in call order (blocking)."""
+        self.submit(frames, streams=streams)
         return self.collect()

@@ -408,11 +408,11 @@ __device__ __forceinline__ void select_faces_body(const float* __restrict__ det,
 }
 
 // block = frame: judge_boxs(track, detector rows) when the frame ran the detector (facer.py:58), else its track boxes
-// (facer.py:61), then sort_and_filter
+// (facer.py:61), then sort_and_filter; the track boxes are the frame's stream's, the outputs are row g
 __global__ void __launch_bounds__(256) select_frames_kernel(const SelectArgs a) {
-    const int g = blockIdx.x;
-    const float* trk = a.track + (size_t)g * a.top_k * 4;
-    const int n_trk = a.track ? (a.n_track ? a.n_track[g] : a.n_track1) : 0;
+    const int g = blockIdx.x, t = a.stream ? a.stream[g] : g;
+    const float* trk = a.track + (size_t)t * a.top_k * 4;
+    const int n_trk = a.track ? (a.n_track ? a.n_track[t] : a.n_track1) : 0;
     const bool det = a.flag ? a.flag[g] != 0 : a.flag1 != 0;
     const float* rows = trk;
     int n_rows = n_trk, stride = 4;

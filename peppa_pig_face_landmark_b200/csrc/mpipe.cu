@@ -1,7 +1,7 @@
 // skps_mpipe: FaceAna.run (Skps/core/api/facer.py:52-85) for MANY concurrent video streams on one GPU.
 //
-// One call takes one frame from each of up to S streams and runs, batched across the streams and with every piece of
-// per-stream state resident in HBM:
+// One call takes one frame from each of up to S streams, any subset of them in any order, and runs, batched across the
+// call's frames and with every piece of per-stream state resident in HBM:
 //   H2D (copy stream, overlapped with the previous batch's compute) -> |prev - cur| gate (which gathers frames already on
 //   the device into the ring in the same pass) -> letterbox x m ->
 //   ONE detector forward (batch m: the keyframes of skps_mpipe_set_detect_every, all S streams by default) -> NMS x m ->
@@ -43,6 +43,7 @@ struct skps_mpipe {
         MpStreamDesc* h_desc = nullptr;       // pinned [2S]: per-stream frame pointers + letterbox geometry of this batch,
                                               // then those of its keyframes, packed
         int32_t* h_det_slot = nullptr;        // pinned [S]: detector frame of each stream, -1 for none
+        int32_t* h_stream = nullptr;          // pinned [S]: stream of each frame of the batch (uploaded when not the identity)
         int32_t* h_count = nullptr; int32_t* h_flag = nullptr;
         double* h_box = nullptr; double* h_kps = nullptr; float* h_scores = nullptr;
         uint8_t* h_chips = nullptr; double* h_M = nullptr;     // pinned, only while alignment is on
@@ -68,6 +69,7 @@ struct skps_mpipe {
     // device scratch (one set: batches are serialised on s_compute)
     int32_t *d_hw = nullptr, *d_have_prev = nullptr, *d_flag = nullptr, *d_det_count = nullptr, *d_det_idx = nullptr;
     int32_t *d_count = nullptr, *d_detail = nullptr, *d_det_slot = nullptr;
+    int32_t* d_stream = nullptr;              // [S] the batch's call -> stream map, when it is not the identity
     unsigned long long* d_diff = nullptr;
     MpStreamDesc* d_desc = nullptr;           // this batch's descriptors (uploaded on the compute stream, in order) [2S]
     void* d_nms_ws = nullptr;                 // NMS workspace, det_rows candidates per stream
@@ -80,6 +82,9 @@ struct skps_mpipe {
     int32_t* d_src = nullptr;                 // [S][K]
     int64_t* d_ids = nullptr;                 // [S][K]
     int64_t* d_next_id = nullptr;             // [S]
+    // the batch's track boxes and ids in call order, copied out by the temporal step when the map is not the identity
+    double* d_out_box = nullptr;              // [S][K][4]
+    int64_t* d_out_ids = nullptr;             // [S][K]
     // id memory (skps_mpipe_set_id_memory): each stream's lost tracks, at most K, most recently lost first
     int id_memory = 0;
     int64_t* d_mem_ids = nullptr;             // [S][K]
@@ -114,7 +119,7 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
     if (p->s_copy) cudaStreamSynchronize(p->s_copy);
     for (uint8_t* f : p->d_frame) if (f) cudaFree(f);
     for (auto& sl : p->slot) {
-        void* host[] = {sl.h_desc, sl.h_det_slot, sl.h_stage, sl.h_hw, sl.h_have_prev, sl.h_geom, sl.h_count, sl.h_flag, sl.h_box,
+        void* host[] = {sl.h_desc, sl.h_det_slot, sl.h_stream, sl.h_stage, sl.h_hw, sl.h_have_prev, sl.h_geom, sl.h_count, sl.h_flag, sl.h_box,
                         sl.h_kps, sl.h_scores, sl.h_chips, sl.h_M, sl.h_pose, sl.h_ids};
         for (void* q : host) if (q) cudaFreeHost(q);
         if (sl.ev_in) cudaEventDestroy(sl.ev_in);
@@ -127,7 +132,7 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
                    p->d_det_rows, p->d_boxes, p->d_kps_now, p->d_prev_lm, p->d_prev_dx, p->d_track, p->d_out_kps,
                    p->d_track_f32, p->d_n_prev, p->d_prev_f32, p->d_state_idx, p->d_n_track, p->d_chips, p->d_align_M, p->d_pose,
                    p->d_nms_ws, p->d_src, p->d_ids, p->d_next_id, p->d_det_slot, p->d_mem_ids, p->d_mem_box, p->d_mem_gap,
-                   p->d_mem_n};
+                   p->d_mem_n, p->d_stream, p->d_out_box, p->d_out_ids};
     for (void* q : dev) if (q) cudaFree(q);
     if (p->s_copy) cudaStreamDestroy(p->s_copy);
     if (p->s_compute) cudaStreamDestroy(p->s_compute);
@@ -190,6 +195,7 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
         SKPS_HOST_ALLOC(sl.h_hw, sizeof(int32_t) * 2 * S); SKPS_HOST_ALLOC(sl.h_have_prev, sizeof(int32_t) * S);
         SKPS_HOST_ALLOC(sl.h_geom, sizeof(int32_t) * 8 * S);
         SKPS_HOST_ALLOC(sl.h_desc, sizeof(MpStreamDesc) * 2 * S); SKPS_HOST_ALLOC(sl.h_det_slot, sizeof(int32_t) * S);
+        SKPS_HOST_ALLOC(sl.h_stream, sizeof(int32_t) * S);
         SKPS_HOST_ALLOC(sl.h_count, sizeof(int32_t) * S); SKPS_HOST_ALLOC(sl.h_flag, sizeof(int32_t) * S);
         SKPS_HOST_ALLOC(sl.h_box, sizeof(double) * 4 * K * S); SKPS_HOST_ALLOC(sl.h_kps, sizeof(double) * 2 * P * K * S);
         SKPS_HOST_ALLOC(sl.h_scores, sizeof(float) * P * K * S);
@@ -215,6 +221,8 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
     SKPS_DEV_ALLOC(p->d_src, 4 * (size_t)K * S); SKPS_DEV_ALLOC(p->d_ids, 8 * (size_t)K * S); SKPS_DEV_ALLOC(p->d_next_id, 8 * S);
     SKPS_DEV_ALLOC(p->d_mem_ids, 8 * (size_t)K * S); SKPS_DEV_ALLOC(p->d_mem_box, 4 * 4 * (size_t)K * S);
     SKPS_DEV_ALLOC(p->d_mem_gap, 4 * (size_t)K * S); SKPS_DEV_ALLOC(p->d_mem_n, 4 * S);
+    SKPS_DEV_ALLOC(p->d_stream, 4 * S); SKPS_DEV_ALLOC(p->d_out_box, 8 * 4 * (size_t)K * S);
+    SKPS_DEV_ALLOC(p->d_out_ids, 8 * (size_t)K * S);
     cudaMemset(p->d_prev_lm, 0, 8 * 2 * 2 * (size_t)P * K * S); cudaMemset(p->d_prev_dx, 0, 8 * 2 * 2 * (size_t)P * K * S);
     cudaMemset(p->d_state_idx, 0, 4 * S); cudaMemset(p->d_track_f32, 0, 4 * 4 * (size_t)K * S);
     cudaMemset(p->d_track, 0, 8 * 4 * (size_t)K * S);
@@ -225,14 +233,36 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
     return 0;
 }
 
-// One batch.  Host frames (pitches null) are uploaded on the copy stream into the next ring position; device frames (rows
-// pitches[i] bytes apart) are gathered there by the frame-difference launch on the compute stream, after the work queued on
-// `producer`, whose later work waits for that launch.  out: results into caller buffers on the device instead of the slot's
-// pinned ones.
-static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* hw, int n,
-                        const int32_t* pitches, cudaStream_t producer, const skps_mpipe_outputs* out) {
+// The call -> stream map of a submit: streams [host] null, or n distinct ids in 0..S-1.  Returns 1 with skps_last_error set
+// for anything else, before the submit enqueues anything; *identity = the map is null or streams[i] == i for every i.
+static int check_stream_map(const skps_mpipe* p, const int32_t* streams, int n, bool* identity) {
+    *identity = true;
+    if (!streams) return 0;
+    std::vector<char> seen(p->S, 0);
+    for (int i = 0; i < n; ++i) {
+        const int t = streams[i];
+        SKPS_CHECK(t >= 0 && t < p->S, "mpipe_submit: frame %d is for stream %d, outside 0..%d", i, t, p->S - 1);
+        SKPS_CHECK(!seen[t], "mpipe_submit: frame %d is for stream %d, which an earlier frame of the call already feeds", i, t);
+        seen[t] = 1;
+        if (t != i) *identity = false;
+    }
+    return 0;
+}
+
+// One batch.  Frame i is the next frame of stream streams[i] (streams null: stream i); the streams are distinct, and a
+// stream the batch does not feed keeps its state as it is.  Everything per frame of the batch (descriptors, staging,
+// detector frames, results) is in call order; everything per stream (ring, previous frame size, frame count, the device
+// state of temporal.cu) is indexed by the stream.  Host frames (pitches null) are uploaded on the copy stream into the
+// stream's next ring position; device frames (rows pitches[i] bytes apart) are gathered there by the frame-difference launch
+// on the compute stream, after the work queued on `producer`, whose later work waits for that launch.  out: results into
+// caller buffers on the device instead of the slot's pinned ones.
+static int submit_batch(skps_mpipe* p, int slot_i, const int32_t* streams, const uint8_t* const* frames, const int32_t* hw,
+                        int n, const int32_t* pitches, cudaStream_t producer, const skps_mpipe_outputs* out) {
     const bool on_device = pitches != nullptr;
     SKPS_CHECK(p && frames && hw && (slot_i == 0 || slot_i == 1) && n > 0 && n <= p->S, "mpipe_submit: bad arguments");
+    bool identity = true;
+    if (check_stream_map(p, streams, n, &identity)) return 1;
+    if (identity) streams = nullptr;      // the launches of a submit without a map, byte for byte
     skps_mpipe::Slot& sl = p->slot[slot_i];
     SKPS_CHECK(!sl.busy, "mpipe_submit: slot %d still holds results (call skps_mpipe_wait first)", slot_i);
     SKPS_CHECK(!out || (out->n_faces && out->ran_detector && out->boxes && out->kps && out->scores),
@@ -247,22 +277,26 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     // a slot completed by skps_mpipe_wait_stream was not waited for on the host: its last batch may still be reading the
     // pinned per-batch buffers rewritten below
     SKPS_CUDA(cudaEventSynchronize(sl.ev_staged));
-    // and it may still read the ring position that host frames are about to be uploaded into
-    if (!on_device && sl.device_out) SKPS_CUDA(cudaStreamWaitEvent(sc, sl.ev_done, 0));
-    // ---- uploads on the copy stream: frame i of stream i into the next ring position
-    for (int s = 0; s < n; ++s) {
-        const int H = hw[2 * s], W = hw[2 * s + 1];
-        SKPS_CHECK(frames[s] && H > 0 && W > 0 && (size_t)H * W * 3 <= p->frame_bytes,
-                   "mpipe_submit: frame %d is %dx%d, larger than the pipeline maximum %dx%d", s, H, W, c.max_h, c.max_w);
+    // and it may still read ring positions that later host frames are uploaded into (see the ring discipline below): order
+    // the copy stream after it whether or not this batch uploads, so that every batch but the other slot's latest is
+    // behind the copy stream, or waited for on the host, whenever a batch uploads
+    if (sl.device_out) SKPS_CUDA(cudaStreamWaitEvent(sc, sl.ev_done, 0));
+    // ---- uploads on the copy stream: frame i of stream t = streams[i] into t's next ring position
+    for (int i = 0; i < n; ++i) {
+        const int t = streams ? streams[i] : i;
+        const int H = hw[2 * i], W = hw[2 * i + 1];
+        SKPS_CHECK(frames[i] && H > 0 && W > 0 && (size_t)H * W * 3 <= p->frame_bytes,
+                   "mpipe_submit: frame %d is %dx%d, larger than the pipeline maximum %dx%d", i, H, W, c.max_h, c.max_w);
         if (on_device) {
-            SKPS_CHECK(H == 1 || pitches[s] >= 3 * W, "mpipe_submit: frame %d has row pitch %d, less than 3 x width %d", s,
-                       pitches[s], W);
-        } else if (upload_host_frame(frames[s], (size_t)H * W * 3, sl.h_stage + p->frame_bytes * s,
-                                     p->d_frame[(size_t)s * 3 + (p->ring_pos[s] + 1) % 3], sc)) {
+            SKPS_CHECK(H == 1 || pitches[i] >= 3 * W, "mpipe_submit: frame %d has row pitch %d, less than 3 x width %d", i,
+                       pitches[i], W);
+        } else if (upload_host_frame(frames[i], (size_t)H * W * 3, sl.h_stage + p->frame_bytes * i,
+                                     p->d_frame[(size_t)t * 3 + (p->ring_pos[t] + 1) % 3], sc)) {
             return 1;
         }
-        sl.h_hw[2 * s] = H; sl.h_hw[2 * s + 1] = W;
-        sl.h_have_prev[s] = (p->prev_h[s] == H && p->prev_w[s] == W) ? 1 : 0;
+        sl.h_hw[2 * i] = H; sl.h_hw[2 * i + 1] = W;
+        sl.h_have_prev[i] = (p->prev_h[t] == H && p->prev_w[t] == W) ? 1 : 0;
+        sl.h_stream[i] = t;
     }
     if (on_device) {
         SKPS_CUDA(cudaEventRecord(p->ev_ready, producer));
@@ -279,39 +313,46 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     const size_t det_in_bytes = (size_t)p->det_h * p->det_w * 3;
     // per-stream frame pointers + letterbox geometry: one small upload, then every pre/post-processing step is ONE launch for
     // all streams (it was 5 launches per stream and call - ~80 launch gaps of a 5 ms call at 16 streams).
-    // Keyframes (skps_mpipe_set_detect_every): stream s's frame i is one when the stream has no previous frame of this size
-    // or (i + s % N) % N == 0.  Only keyframes go through the letterbox, the detector and NMS, as detector frames 0..m-1 in
-    // stream order; the host knows them now, so the detector batch shrinks with no read-back.
+    // Keyframes (skps_mpipe_set_detect_every): stream t's frame j is one when the stream has no previous frame of this size
+    // or (j + t % N) % N == 0, wherever the frame sits in the call.  Only keyframes go through the letterbox, the detector and
+    // NMS, as detector frames 0..m-1 in call order; the host knows them now, so the detector batch shrinks with no read-back.
     const int N = p->detect_every;
     int m = 0;
     size_t max_bytes = 0;
-    for (int s = 0; s < n; ++s) {
-        const int H = hw[2 * s], W = hw[2 * s + 1];
-        const bool key = !sl.h_have_prev[s] || (p->frame_idx[s] + s % N) % N == 0;
-        sl.h_det_slot[s] = key ? m++ : -1;
-        MpStreamDesc& D = sl.h_desc[s];
-        D.cur = p->d_frame[(size_t)s * 3 + (p->ring_pos[s] + 1) % 3];
-        // the difference sum only decides keyframes: the other streams skip it (a device frame is still gathered into cur)
-        D.have_prev = sl.h_have_prev[s] && key;
-        D.prev = D.have_prev ? p->d_frame[(size_t)s * 3 + p->ring_pos[s]] : nullptr;
+    for (int i = 0; i < n; ++i) {
+        const int t = sl.h_stream[i];
+        const int H = hw[2 * i], W = hw[2 * i + 1];
+        const bool key = !sl.h_have_prev[i] || (p->frame_idx[t] + t % N) % N == 0;
+        sl.h_det_slot[i] = key ? m++ : -1;
+        MpStreamDesc& D = sl.h_desc[i];
+        D.cur = p->d_frame[(size_t)t * 3 + (p->ring_pos[t] + 1) % 3];
+        // the difference sum only decides keyframes: the other frames skip it (a device frame is still gathered into cur)
+        D.have_prev = sl.h_have_prev[i] && key;
+        D.prev = D.have_prev ? p->d_frame[(size_t)t * 3 + p->ring_pos[t]] : nullptr;
         D.H = H; D.W = W;
-        D.src = on_device ? frames[s] : nullptr;
-        D.src_pitch = on_device ? pitches[s] : W * 3;
+        D.src = on_device ? frames[i] : nullptr;
+        D.src_pitch = on_device ? pitches[i] : W * 3;
         letterbox_geometry(H, W, p->det_h, p->det_w, &D.scale, &D.rw, &D.rh, &D.top, &D.left);
-        memcpy(&sl.h_geom[8 * s], &D.scale, 4); sl.h_geom[8 * s + 1] = D.top; sl.h_geom[8 * s + 2] = D.left;
+        memcpy(&sl.h_geom[8 * i], &D.scale, 4); sl.h_geom[8 * i + 1] = D.top; sl.h_geom[8 * i + 2] = D.left;
         if ((size_t)H * W * 3 > max_bytes) max_bytes = (size_t)H * W * 3;
     }
-    // the keyframes' descriptors, packed after the batch's; when every stream is a keyframe the batch is that list, and the
-    // kernels take det_slot = null (frame s is stream s's), exactly as without a cadence
+    // the keyframes' descriptors, packed after the batch's; when every frame is a keyframe the batch is that list, and the
+    // kernels take det_slot = null (detector frame i is frame i), exactly as without a cadence
     const MpStreamDesc* d_key_desc = p->d_desc;
     const int32_t* det_slot = nullptr;
     int n_desc = n;
     if (m < n) {
-        for (int s = 0; s < n; ++s)
-            if (sl.h_det_slot[s] >= 0) sl.h_desc[n + sl.h_det_slot[s]] = sl.h_desc[s];
+        for (int i = 0; i < n; ++i)
+            if (sl.h_det_slot[i] >= 0) sl.h_desc[n + sl.h_det_slot[i]] = sl.h_desc[i];
         d_key_desc = p->d_desc + n; n_desc = n + m;
         det_slot = p->d_det_slot;
         SKPS_CUDA(cudaMemcpyAsync(p->d_det_slot, sl.h_det_slot, 4 * n, cudaMemcpyHostToDevice, sx));
+    }
+    // the call -> stream map of the two kernels that touch per-stream device state (select, temporal); null: the identity
+    const int32_t* stream_map = nullptr;
+    if (streams) {
+        stream_map = p->d_stream;
+        SKPS_CUDA(cudaMemcpyAsync(p->d_stream, sl.h_stream, 4 * n, cudaMemcpyHostToDevice, sx));
     }
     SKPS_CUDA(cudaMemcpyAsync(p->d_desc, sl.h_desc, sizeof(MpStreamDesc) * n_desc, cudaMemcpyHostToDevice, sx));
     SKPS_CUDA(cudaEventRecord(sl.ev_staged, sx));
@@ -341,7 +382,7 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     }
     SelectArgs sa = {};
     sa.det_rows = p->d_det_rows; sa.det_count = p->d_det_count; sa.det_stride = 16; sa.det_cap = p->det_rows;
-    sa.det_slot = det_slot; sa.flag = p->d_flag; sa.track = p->d_track_f32; sa.n_track = p->d_n_track;
+    sa.det_slot = det_slot; sa.flag = p->d_flag; sa.track = p->d_track_f32; sa.n_track = p->d_n_track; sa.stream = stream_map;
     sa.iou_thres = c.track_iou; sa.alpha = c.alpha; sa.one_minus_alpha = (float)(1.0 - (double)c.alpha);
     sa.min_face = c.min_face; sa.top_k = K;
     sa.boxes4 = p->d_boxes; sa.count = p->d_count; sa.src = p->d_src;
@@ -354,7 +395,7 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     if (skps_engine_forward(p->kps, kps_in, n * K, nullptr, sx)) return 1;
     if (launch_landmark_post(skps_engine_output_ptr(p->kps, 0), p->d_detail, p->d_count, K, P, p->d_kps_now, n, sx)) return 1;
     MpTemporalArgs a;
-    a.top_k = K; a.n_points = P;
+    a.top_k = K; a.n_points = P; a.stream = stream_map;
     a.kps_now = p->d_kps_now; a.count = p->d_count; a.flag = p->d_flag; a.hw = p->d_hw; a.boxes4 = p->d_boxes;
     a.prev_lm = p->d_prev_lm; a.prev_dx = p->d_prev_dx; a.n_prev = p->d_n_prev; a.prev_f32 = p->d_prev_f32;
     a.state_idx = p->d_state_idx; a.track_box = p->d_track; a.track_f32 = p->d_track_f32; a.n_track = p->d_n_track;
@@ -362,6 +403,9 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     a.id_memory = p->id_memory;
     a.mem_ids = p->d_mem_ids; a.mem_box = p->d_mem_box; a.mem_gap = p->d_mem_gap; a.mem_n = p->d_mem_n;
     a.out_kps = p->d_out_kps;
+    // with a map, the stream state's rows 0..n-1 are not the batch's: the kernel packs the returned boxes and ids by frame
+    a.out_box = streams ? p->d_out_box : nullptr;
+    a.out_ids = streams ? p->d_out_ids : nullptr;
     mp_temporal_constants(c, a);
     if (launch_mp_temporal(a, n, sx)) return 1;
     sl.align = p->align_size;
@@ -393,18 +437,31 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     }
     SKPS_CUDA(cudaMemcpyAsync(out ? out->n_faces : sl.h_count, p->d_count, 4 * n, result_kind, sx));
     SKPS_CUDA(cudaMemcpyAsync(out ? out->ran_detector : sl.h_flag, p->d_flag, 4 * n, result_kind, sx));
-    SKPS_CUDA(cudaMemcpyAsync(out ? out->boxes : sl.h_box, p->d_track, 8 * 4 * (size_t)K * n, result_kind, sx));
+    SKPS_CUDA(cudaMemcpyAsync(out ? out->boxes : sl.h_box, streams ? p->d_out_box : p->d_track, 8 * 4 * (size_t)K * n,
+                              result_kind, sx));
     SKPS_CUDA(cudaMemcpyAsync(out ? out->kps : sl.h_kps, p->d_out_kps, 8 * 2 * (size_t)P * K * n, result_kind, sx));
     SKPS_CUDA(cudaMemcpyAsync(out ? out->scores : sl.h_scores, skps_engine_output_ptr(p->kps, 1), 4 * (size_t)P * K * n,
                               result_kind, sx));
-    if (!out || out->ids) SKPS_CUDA(cudaMemcpyAsync(out ? out->ids : sl.h_ids, p->d_ids, 8 * (size_t)K * n, result_kind, sx));
+    if (!out || out->ids)
+        SKPS_CUDA(cudaMemcpyAsync(out ? out->ids : sl.h_ids, streams ? p->d_out_ids : p->d_ids, 8 * (size_t)K * n, result_kind,
+                                  sx));
     SKPS_CUDA(cudaEventRecord(sl.ev_done, sx));
-    // ring discipline: this batch read positions r (previous) and r+1 (current); the next batch uploads into r+2 (free), the
-    // one after into r again - and that one reuses this slot, so the caller has passed skps_mpipe_wait(slot) by then
-    for (int s = 0; s < n; ++s) {
-        p->ring_pos[s] = (p->ring_pos[s] + 1) % 3;
-        p->prev_h[s] = hw[2 * s]; p->prev_w[s] = hw[2 * s + 1];
-        ++p->frame_idx[s];
+    // ring discipline, per stream t of the batch: this batch reads t's positions r (previous) and r+1 (current); the next
+    // batch that feeds t uploads into r+2 (free), and the one after that into r again.  That third batch B comes at least
+    // two submits after this one A, whichever slots and calls the stream's frames land in: at least one other submit, the
+    // one feeding t in between, separates them.  Every batch computes on the one serial compute stream, so any batch that
+    // is done implies all batches before it are done.  When B is submitted on slot j, its slot's previous batch q has been
+    // completed: waited for on the host (skps_mpipe_wait), or, if completed by skps_mpipe_wait_stream, the copy stream was
+    // made to wait for q's ev_done at the top of B's submit.  Every earlier submit did the same for its own slot's previous
+    // batch, so every batch except the latest one on the other slot, o, is done or behind the copy stream.  A is not o: if
+    // o is the most recent submit, A, two or more submits back, comes before it, and if q is more recent than o, q done
+    // implies o done.  So B's upload into r cannot overtake A's reads.  Device frames are gathered on the compute stream
+    // itself, after A.
+    for (int i = 0; i < n; ++i) {
+        const int t = sl.h_stream[i];
+        p->ring_pos[t] = (p->ring_pos[t] + 1) % 3;
+        p->prev_h[t] = hw[2 * i]; p->prev_w[t] = hw[2 * i + 1];
+        ++p->frame_idx[t];
     }
     sl.n = n;
     sl.m = m;
@@ -413,17 +470,30 @@ static int submit_batch(skps_mpipe* p, int slot_i, const uint8_t* const* frames,
     return 0;
 }
 
+extern "C" SKPS_API int skps_mpipe_submit_streams(skps_mpipe* p, int slot_i, const int32_t* streams, const uint8_t* const* frames,
+                                                  const int32_t* hw, int n) {
+    return submit_batch(p, slot_i, streams, frames, hw, n, nullptr, nullptr, nullptr);
+}
+
 extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* hw, int n) {
-    return submit_batch(p, slot_i, frames, hw, n, nullptr, nullptr, nullptr);
+    return skps_mpipe_submit_streams(p, slot_i, nullptr, frames, hw, n);
+}
+
+extern "C" SKPS_API int skps_mpipe_submit_device_streams(skps_mpipe* p, int slot_i, const int32_t* streams,
+                                                         const uint8_t* const* frames, const int32_t* pitches, const int32_t* hw,
+                                                         int n, const skps_mpipe_outputs* out, void* producer_stream) {
+    SKPS_CHECK(p && frames && pitches && hw && n > 0 && n <= p->S, "mpipe_submit_device: bad arguments");
+    bool identity = true;
+    if (check_stream_map(p, streams, n, &identity)) return 1;
+    SKPS_ON_DEVICE(p->device);
+    for (int i = 0; i < n; ++i)
+        if (check_device_frame(frames[i], p->device, "mpipe_submit_device", i)) return 1;
+    return submit_batch(p, slot_i, streams, frames, hw, n, pitches, (cudaStream_t)producer_stream, out);
 }
 
 extern "C" SKPS_API int skps_mpipe_submit_device(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* pitches,
                                                  const int32_t* hw, int n, const skps_mpipe_outputs* out, void* producer_stream) {
-    SKPS_CHECK(p && frames && pitches && hw && n > 0 && n <= p->S, "mpipe_submit_device: bad arguments");
-    SKPS_ON_DEVICE(p->device);
-    for (int s = 0; s < n; ++s)
-        if (check_device_frame(frames[s], p->device, "mpipe_submit_device", s)) return 1;
-    return submit_batch(p, slot_i, frames, hw, n, pitches, (cudaStream_t)producer_stream, out);
+    return skps_mpipe_submit_device_streams(p, slot_i, nullptr, frames, pitches, hw, n, out, producer_stream);
 }
 
 extern "C" SKPS_API int skps_mpipe_wait_stream(skps_mpipe* p, int slot_i, void* consumer_stream) {

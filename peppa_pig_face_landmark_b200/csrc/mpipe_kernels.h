@@ -9,13 +9,17 @@ struct skps_engine;
 
 namespace skps {
 
+// Block g of a launch over n calls' frames serves stream stream[g] (stream null: g).  The per-frame inputs and outputs are
+// in call order, rows g < n; the state is indexed by the stream, rows [S].
 struct MpTemporalArgs {
     int top_k, n_points;
-    const float* kps_now;        // [S][K][P][2] float32 landmarks in frame pixels (landmark_post)
-    const int* count;            // [S] faces this frame
-    const int* flag;             // [S] detector ran this frame
-    const int* hw;               // [S][2] frame height, width
-    const float* boxes4;         // [S][K][4] boxes the landmark stage used (boxes_return, facer.py:66)
+    const int* stream;           // [n] [dev] stream of each frame of the call, distinct, or null: frame g is stream g's
+    const float* kps_now;        // [n][K][P][2] float32 landmarks in frame pixels (landmark_post)
+    const int* count;            // [n] faces this frame
+    const int* flag;             // [n] detector ran this frame
+    const int* hw;               // [n][2] frame height, width
+    const float* boxes4;         // [n][K][4] boxes the landmark stage used (boxes_return, facer.py:66)
+    const int* src;              // [n][K] source of each face this frame (launch_select), an index into the old track
     // state, updated in place
     double* prev_lm;             // [S][2][K][P][2] previous landmark sets (ping-pong)
     double* prev_dx;             // [S][2][K][P][2] previous - filtered
@@ -25,7 +29,6 @@ struct MpTemporalArgs {
     double* track_box;           // [S][K][4] float64 track boxes (returned as 'box')
     float* track_f32;            // [S][K][4] the same, as float32 (next frame's judge_boxs / crop input)
     int* n_track;                // [S]
-    const int* src;              // [S][K] source of each face this frame (launch_select), an index into the old track
     int64_t* ids;                // [S][K] track id of each track box
     int64_t* next_id;            // [S] the next unused id of the stream
     // id memory (skps_mpipe_set_id_memory): the lost tracks of each stream, most recently lost first.  id_memory 0: off,
@@ -36,7 +39,9 @@ struct MpTemporalArgs {
     int* mem_gap;                // [S][K] frames in a row each has been missing so far
     int* mem_n;                  // [S] entries held
     // outputs
-    double* out_kps;             // [S][K][P][2]
+    double* out_kps;             // [n][K][P][2]
+    double* out_box;             // [n][K][4] copies of the new track boxes and their ids in call order, or null (not
+    int64_t* out_ids;            // [n][K]    written; without a stream map they are rows 0..n-1 of track_box and ids)
     // constants (python floats computed on the host exactly as lk.py does)
     double iou_thres, alpha, one_minus_alpha, a_d, one_minus_a_d, min_cutoff, beta, two_pi;
 };
@@ -86,6 +91,7 @@ int launch_crop(const CropArgs& a, int n, cudaStream_t s);
 // judge_boxs + sort_and_filter (facer.py:58-64), one block per frame.  Frame g selects from the rows of its detector frame
 // f = det_slot[g] (det_slot null: f = g), det_count[f] rows of det_stride floats at det_rows + f * det_cap * det_stride,
 // IoU-matched against its track boxes, when it ran the detector; else from its track boxes themselves (facer.py:61).
+// Its track boxes are those of stream t = stream[g] (stream null: t = g): track [t], n_track[t].
 // src [n][top_k] [dev] or null: each selected face's source for the track ids, the row it came from when the rows are the
 // track boxes, else the index of the track box its detection matched, -1 for none.
 struct SelectArgs {
@@ -93,8 +99,9 @@ struct SelectArgs {
     int det_stride, det_cap;
     const int* det_slot;                            // [n] [dev] or null
     const int* flag;                                // [n] [dev]: frame g ran the detector, or null: flag1
-    const float* track;                             // [n][top_k][4] [dev], or null (no track boxes)
-    const int* n_track;                             // [n] [dev], or null: n_track1
+    const float* track;                             // [streams][top_k][4] [dev], or null (no track boxes)
+    const int* n_track;                             // [streams] [dev], or null: n_track1
+    const int* stream;                              // [n] [dev] stream of frame g, or null: g
     int flag1, n_track1;
     float iou_thres, alpha, one_minus_alpha, min_face;
     int top_k;                                      // 1..SKPS_MAX_TOP_K
@@ -146,7 +153,7 @@ int launch_nms(const NmsArgs& a, cudaStream_t s);
 // difference > 5)
 int launch_mp_decide(const unsigned long long* diff, const int* hw, const int* have_prev, const int* det_slot, int* flag, int n,
                      cudaStream_t s);
-int launch_mp_temporal(const MpTemporalArgs& a, int n_streams, cudaStream_t s);
+int launch_mp_temporal(const MpTemporalArgs& a, int n, cudaStream_t s);
 // Aligned face chips (align.cu): per face of stream g < n with i < count[g], M = similarity of kps[g][i] (P x 2 float64) to the
 // ArcFace template at `size`, chips[g][i] = cv2.warpAffine(desc[g].cur, M, (size, size)); chips [n][K][size][size][3], M [n][K][2][3].
 int launch_mp_align(const MpStreamDesc* d, const double* kps, const int* count, int K, int P, int size, uint8_t* chips,

@@ -3,8 +3,9 @@
 //   GroupTrack.calculate      Skps/core/smoother/lk.py:19-59   (IoU match to last frame's landmark sets)
 //   OneEuroFilter.__call__    lk.py:115-149                    (unit time step, displacement-norm derivative)
 //   track box refresh         facer.py:74-82 + judge_boxs :144-189 + EmaFilter lk.py:155-162
-// One CTA per stream; all state (previous landmark sets, their deltas, track boxes) stays in HBM between frames, so a
-// batch of streams needs no host round trip between frames.  The reference does this arithmetic in numpy with mixed
+// One CTA per frame of the call, i.e. per stream the call feeds; all state (previous landmark sets, their deltas, track
+// boxes) stays in HBM between frames, indexed by the stream, so a batch of streams needs no host round trip between frames
+// and a stream the call does not feed is not touched.  The reference does this arithmetic in numpy with mixed
 // float32/float64 operands; the kernel follows numpy's promotion rules operation by operation (float64 wherever one
 // operand is float64, float32 where both are), which is why this file is compiled with -fmad=false.
 #include <math.h>
@@ -87,14 +88,15 @@ __global__ void mp_decide_kernel(const unsigned long long* __restrict__ diff, co
 }
 
 __global__ void __launch_bounds__(128) mp_temporal_kernel(const MpTemporalArgs a) {
-    const int s = blockIdx.x, tid = threadIdx.x;
+    // frame g of the call (its inputs and outputs), stream s (its state)
+    const int g = blockIdx.x, s = a.stream ? a.stream[g] : g, tid = threadIdx.x;
     const int K = a.top_k, P = a.n_points;
     const long long set = (long long)2 * P;
     __shared__ double red[16];
     __shared__ double rect_now[4], rect_prev[4];
     __shared__ int s_match;
     __shared__ int64_t s_ids[64];                                     // the old track ids (skps_mpipe_create: top_k <= 64)
-    const int n = a.count[s];
+    const int n = a.count[g];
     // id memory: the old track boxes (overwritten below before the ids are assigned), the stream's lost tracks, and per
     // face the entries it overlaps with IoU > iou_thres (bit k: entry k), all float32 as judge_boxs compares two such rows
     __shared__ float s_old_box[64][4], s_mem_box[64][4];
@@ -116,7 +118,7 @@ __global__ void __launch_bounds__(128) mp_temporal_kernel(const MpTemporalArgs a
         }
         for (int e = tid; e < n; e += blockDim.x) s_hit[e] = 0ull;
         __syncthreads();
-        const float* b4 = a.boxes4 + (long long)s * K * 4;
+        const float* b4 = a.boxes4 + (long long)g * K * 4;
         for (int e = tid; e < n * mem_n; e += blockDim.x) {
             const int i = e / mem_n, k = e - i * mem_n;
             Num r1[4], r2[4];
@@ -125,16 +127,16 @@ __global__ void __launch_bounds__(128) mp_temporal_kernel(const MpTemporalArgs a
         }
         __syncthreads();
     }
-    const float* now = a.kps_now + (long long)s * K * set;            // float32 (n, P, 2)
+    const float* now = a.kps_now + (long long)g * K * set;            // float32 (n, P, 2)
     const int cur = a.state_idx[s], nxt = cur ^ 1;
     const double* prev = a.prev_lm + ((long long)(s * 2 + cur) * K) * set;
     const double* prev_dx = a.prev_dx + ((long long)(s * 2 + cur) * K) * set;
     double* res = a.prev_lm + ((long long)(s * 2 + nxt) * K) * set;  // result = next frame's "previous"
     double* res_dx = a.prev_dx + ((long long)(s * 2 + nxt) * K) * set;
-    double* out = a.out_kps + (long long)s * K * set;
-    int n_prev = a.flag[s] ? -1 : a.n_prev[s];                        // facer.py:59: previous_landmarks_set = None
+    double* out = a.out_kps + (long long)g * K * set;
+    int n_prev = a.flag[g] ? -1 : a.n_prev[s];                        // facer.py:59: previous_landmarks_set = None
     const bool prev_f32 = a.prev_f32[s] != 0;
-    const double W = (double)a.hw[2 * s + 1], H = (double)a.hw[2 * s];
+    const double W = (double)a.hw[2 * g + 1], H = (double)a.hw[2 * g];
     bool all_f32 = true;                                              // dtype of np.array(result)
     for (int i = 0; i < n; ++i) {
         const float* cur_pts = now + i * set;
@@ -186,7 +188,7 @@ __global__ void __launch_bounds__(128) mp_temporal_kernel(const MpTemporalArgs a
         __syncthreads();
     }
     // outputs + track boxes: tmp_box = min/max of the refined landmarks, judge_boxs(boxes_return, tmp_box) (facer.py:74-82)
-    const float* boxes_ret = a.boxes4 + (long long)s * K * 4;         // float32, n rows
+    const float* boxes_ret = a.boxes4 + (long long)g * K * 4;         // float32, n rows
     for (int i = 0; i < n; ++i) {
         const double* r_i = res + i * set;
         for (int p = tid; p < 2 * P; p += blockDim.x) out[i * set + p] = r_i[p];
@@ -214,6 +216,7 @@ __global__ void __launch_bounds__(128) mp_temporal_kernel(const MpTemporalArgs a
                 }
                 tb[c] = v;
                 tf[c] = (float)v;                                      // facer.py: the next frame's boxes go through float32
+                if (a.out_box) a.out_box[((long long)g * K + i) * 4 + c] = v;
             }
         }
         __syncthreads();
@@ -229,10 +232,11 @@ __global__ void __launch_bounds__(128) mp_temporal_kernel(const MpTemporalArgs a
         unsigned long long used = 0ull;                               // bit k: memory entry k's id is given back
         int64_t next = a.next_id[s];
         for (int i = 0; i < n; ++i) {
-            const int j = a.src[(long long)s * K + i];
+            const int j = a.src[(long long)g * K + i];
             if (j >= 0 && j < n_old && !((taken >> j) & 1ull)) {
                 taken |= 1ull << j;
                 ids[i] = s_ids[j];
+                if (a.out_ids) a.out_ids[(long long)g * K + i] = ids[i];
                 continue;
             }
             int k = -1;
@@ -248,6 +252,7 @@ __global__ void __launch_bounds__(128) mp_temporal_kernel(const MpTemporalArgs a
             } else {
                 ids[i] = next++;
             }
+            if (a.out_ids) a.out_ids[(long long)g * K + i] = ids[i];
         }
         a.next_id[s] = next;
         if (mem_on) {
@@ -285,8 +290,8 @@ int launch_mp_decide(const unsigned long long* diff, const int* hw, const int* h
     return 0;
 }
 
-int launch_mp_temporal(const MpTemporalArgs& a, int n_streams, cudaStream_t s) {
-    mp_temporal_kernel<<<n_streams, 128, 0, s>>>(a);
+int launch_mp_temporal(const MpTemporalArgs& a, int n, cudaStream_t s) {
+    mp_temporal_kernel<<<n, 128, 0, s>>>(a);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }

@@ -111,6 +111,9 @@ SIGNATURES = {
     "skps_mpipe_submit": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, C.c_int]),
     "skps_mpipe_wait": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "skps_mpipe_submit_device": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int, C.POINTER(MpipeOutputs), c_vp]),
+    "skps_mpipe_submit_streams": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, C.c_int]),
+    "skps_mpipe_submit_device_streams": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp, C.c_int, C.POINTER(MpipeOutputs),
+                                                   c_vp]),
     "skps_mpipe_wait_stream": (C.c_int, [c_vp, C.c_int, c_vp]),
     "skps_mpipe_track_ids": (C.c_int, [c_vp, C.c_int, c_vp]),
     "skps_debug_mp_temporal": (C.c_int, [C.POINTER(PipelineCfg), C.c_int, C.c_int, C.c_int] + [c_vp] * 18),
