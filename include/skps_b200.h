@@ -182,6 +182,24 @@ SKPS_API int skps_debug_conv_mma(const float* x, int N, int H, int W, int C, con
 
 /* ------------------------------------------------------------------ image kernels */
 
+/* Pixel layouts of frames already in device memory (the `layout` arguments and skps_frame_layout below).  Pixel (y, x)
+ * of a frame at `base` with row pitch `pitch` has its blue, green and red bytes at
+ *     base + y*pitch + x*xstep + off[c]
+ * with, per layout, xstep and off[B, G, R]:
+ *     SKPS_LAYOUT_BGR         3, {0, 1, 2}          HxWx3, the reference's own layout
+ *     SKPS_LAYOUT_RGB         3, {2, 1, 0}          HxWx3 (DALI's default)
+ *     SKPS_LAYOUT_BGRA        4, {0, 1, 2}          HxWx4, the 4th byte's value is never used
+ *     SKPS_LAYOUT_RGBA        4, {2, 1, 0}
+ *     SKPS_LAYOUT_BGR_PLANAR  1, {0, P, 2P}         3xHxW, planes P = plane_pitch bytes apart
+ *     SKPS_LAYOUT_RGB_PLANAR  1, {2P, P, 0}         (torchvision.io.decode_jpeg on the GPU, NCHW video decoders)
+ * Row pitches are >= xstep * W (any value for a one-row frame), plane pitches >= 0; both fit int32.  The kernels only
+ * compute addresses this way and keep their arithmetic: a frame gives, bit for bit, the results of the same pixels
+ * passed as interleaved BGR.  0 is BGR, so a zeroed skps_frame_layout describes a BGR frame. */
+enum {
+    SKPS_LAYOUT_BGR = 0, SKPS_LAYOUT_RGB = 1, SKPS_LAYOUT_BGRA = 2, SKPS_LAYOUT_RGBA = 3, SKPS_LAYOUT_BGR_PLANAR = 4,
+    SKPS_LAYOUT_RGB_PLANAR = 5
+};
+
 /* FaceDetector.preprocess (face_detector.py:45-71): BGR->RGB, cv2.resize INTER_LINEAR
  * (bit-exact 11-bit fixed point) to (rw,rh), pad with 114 to (in_h,in_w).  `frame` [dev]
  * HxWx3 uint8 with row pitch `pitch` bytes; `out` [dev] in_h*in_w*3 uint8 RGB.  The /255 is
@@ -209,6 +227,19 @@ typedef struct skps_det_src {
  * [dev], is letterboxed into out [dev] + i*in_h*in_w*3.  The bytes of each frame are those
  * skps_letterbox writes for the whole frame with the same geometry. */
 SKPS_API int skps_letterbox_frames(const skps_det_src* src, int n, uint8_t* out, int in_h, int in_w, void* stream);
+
+/* The pixel layout of one frame for the *_layout entries: a SKPS_LAYOUT_* code and, for the planar layouts, the bytes
+ * from one plane to the next.  A zeroed entry is interleaved BGR, what the descriptors alone describe. */
+typedef struct skps_frame_layout {
+    int32_t layout;
+    int32_t plane_pitch;
+} skps_frame_layout;
+
+/* skps_letterbox_frames for frames in any SKPS_LAYOUT_*: frame i's pixels are laid out as lay[i] [dev] (n) says, its row
+ * pitch src[i].pitch >= xstep * W; lay NULL: every frame is BGR (skps_letterbox_frames).  The bytes are those of the
+ * same pixels as an interleaved BGR frame.  row_pairs frames are BGR. */
+SKPS_API int skps_letterbox_frames_layout(const skps_det_src* src, const skps_frame_layout* lay, int n, uint8_t* out,
+                                          int in_h, int in_w, void* stream);
 
 /* xywh2xyxy + py_nms + scale_coords (face_detector.py:73-136) on the raw (rows,16) output.
  * Writes up to max_det (<= 256) kept rows (16 floats each, cols 0-3 mapped back to frame pixels),
@@ -289,6 +320,11 @@ typedef struct skps_face_src {
  * every pixel of the frame the crop reads. */
 SKPS_API int skps_crop_faces(const skps_face_src* src, const float* boxes4, int n, float face_scale,
                              float min_face, uint8_t* crops, int out_hw, int32_t* detail, void* stream);
+/* skps_crop_faces for faces of frames in any SKPS_LAYOUT_*: face i's frame is laid out as lay[i] [dev] (n) says; lay NULL:
+ * every frame is BGR (skps_crop_faces).  The crops stay BGR: the bytes of the same pixels as an interleaved BGR frame. */
+SKPS_API int skps_crop_faces_layout(const skps_face_src* src, const skps_frame_layout* lay, const float* boxes4, int n,
+                                    float face_scale, float min_face, uint8_t* crops, int out_hw, int32_t* detail,
+                                    void* stream);
 
 /* FaceLandmark.postprocess (face_landmark.py:106-115): x*w + x1 - add, y*h + y1 - add. */
 SKPS_API int skps_landmark_post(const float* xy_norm, const int32_t* detail, const int32_t* count,
@@ -304,6 +340,11 @@ SKPS_API int skps_frame_absdiff_sum(const uint8_t* a, const uint8_t* b, size_t n
  * NULL (copy only, *sum = 0).  Asynchronous on `stream`. */
 SKPS_API int skps_frame_ingest(const uint8_t* frame, int H, int W, int pitch, uint8_t* packed, const uint8_t* prev,
                                unsigned long long* sum, void* stream);
+/* skps_frame_ingest for a frame in any SKPS_LAYOUT_*: `packed` gets the frame as interleaved BGR (H*W*3 bytes) and *sum
+ * is sum |packed - prev|, the bytes and the sum skps_frame_ingest gives for the same pixels passed as BGR.  pitch >=
+ * xstep * W (H == 1: any); plane_pitch is read for the planar layouts only.  skps_frame_ingest is this entry with BGR. */
+SKPS_API int skps_frame_ingest_layout(const uint8_t* frame, int H, int W, int pitch, int layout, int plane_pitch,
+                                      uint8_t* packed, const uint8_t* prev, unsigned long long* sum, void* stream);
 
 /* ------------------------------------------------------------------ FaceAna.run (facer.py:52-85) */
 
@@ -378,6 +419,12 @@ SKPS_API int skps_pipeline_frame_diff(skps_pipeline* p, const uint8_t* frame, in
  * queued on producer_stream after this call returns runs after the read, so the producer may overwrite the frame at once. */
 SKPS_API int skps_pipeline_frame_diff_device(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch,
                                              void* producer_stream, double* mean_diff, void* stream);
+/* skps_pipeline_frame_diff_device for a frame in any SKPS_LAYOUT_* (pitch and plane_pitch as skps_frame_ingest_layout
+ * takes them): the frame is staged as interleaved BGR, so everything after it sees the frame the BGR entry stages for the
+ * same pixels.  skps_pipeline_frame_diff_device is this entry with BGR. */
+SKPS_API int skps_pipeline_frame_diff_device_layout(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch,
+                                                    int layout, int plane_pitch, void* producer_stream, double* mean_diff,
+                                                    void* stream);
 /* Adopt the staged frame as the previous frame without running the chain: the skip path of FaceAna.run (facer.py:57-62
  * replaces previous_image on every call, also when nothing is detected or tracked).  Fails when no frame is staged. */
 SKPS_API int skps_pipeline_commit_frame(skps_pipeline* p);
@@ -471,6 +518,15 @@ SKPS_API int skps_mpipe_submit_device(skps_mpipe* p, int slot, const uint8_t* co
 SKPS_API int skps_mpipe_submit_device_streams(skps_mpipe* p, int slot, const int32_t* streams, const uint8_t* const* frames,
                                               const int32_t* pitches, const int32_t* hw, int n, const skps_mpipe_outputs* out,
                                               void* producer_stream);
+/* skps_mpipe_submit_device_streams for frames in any SKPS_LAYOUT_*, one layout for the whole call: pitches[i] >= xstep *
+ * W_i (H_i == 1: any); plane_pitches [host] int32 (n) the plane pitch of each frame, read for the planar layouts only
+ * (may be NULL otherwise).  Every frame is gathered into its stream's ring as interleaved BGR, so the gate, the detection
+ * cadence, track ids and smoothing see what the BGR entry stages for the same pixels, and consecutive calls may use
+ * different layouts.  skps_mpipe_submit_device_streams is this entry with BGR. */
+SKPS_API int skps_mpipe_submit_device_layout(skps_mpipe* p, int slot, const int32_t* streams, const uint8_t* const* frames,
+                                             const int32_t* pitches, const int32_t* hw, int n, int layout,
+                                             const int32_t* plane_pitches, const skps_mpipe_outputs* out,
+                                             void* producer_stream);
 /* Completes a slot submitted with device outputs without blocking the host: work queued on `consumer_stream` after this
  * call runs after the batch's results are in the caller's buffers.  The slot can then be submitted again. */
 SKPS_API int skps_mpipe_wait_stream(skps_mpipe* p, int slot, void* consumer_stream);
@@ -537,6 +593,10 @@ SKPS_API int skps_align_faces(const uint8_t* frame, int H, int W, int pitch, con
  * upload only core/api/align.py:chip_read_rects).  Asynchronous on `stream`; allocates nothing. */
 SKPS_API int skps_warp_faces(const skps_face_src* src, const double* M, int n, int out_h, int out_w, uint8_t* out,
                              void* stream);
+/* skps_warp_faces for faces of images in any SKPS_LAYOUT_*: chip i's image is laid out as lay[i] [dev] (n) says; lay NULL:
+ * every image is BGR (skps_warp_faces).  The chips are BGR, the bytes of the same pixels as an interleaved BGR image. */
+SKPS_API int skps_warp_faces_layout(const skps_face_src* src, const skps_frame_layout* lay, const double* M, int n, int out_h,
+                                    int out_w, uint8_t* out, void* stream);
 /* The estimate of skps_align_faces for n faces (any n >= 0) from float32 landmarks kps [dev] (n,P,2), P >= 98, each promoted
  * to float64: M [dev] (n,2,3) float64, bit for bit what skps_align_faces gives for kps.astype(float64) (and so what
  * FaceAna(align=size) returns for its float32 'kps').  size 16..512.  Asynchronous on `stream`; allocates nothing. */

@@ -1,10 +1,75 @@
 """The frames FaceAna.run and FaceAnaStreams.submit accept, checked before anything is enqueued: numpy arrays, and frames
-already in GPU memory (a decoder surface, a tensor from NVDEC / DALI / torchvision, an ROI view of either).  Pixels stay
-HxWx3 uint8 BGR as the reference's run(image) takes them; only where the frame lives and its row pitch differ between the
-two."""
+already in GPU memory (a decoder surface, a tensor from NVDEC / DALI / torchvision, an ROI view of either).  Host frames
+are HxWx3 uint8 BGR as the reference's run(image) takes them.  CUDA frames are read where they are, at any row pitch, in
+the pixel layout the caller names with layout= (LAYOUTS): interleaved BGR (the default), RGB, BGRA or RGBA, or planar
+(3, H, W) BGR or RGB.  Every layout gives, bit for bit, the results of the same pixels passed as interleaved BGR."""
+import collections
 import sys
 
 import numpy as np
+
+# layout= name -> SKPS_LAYOUT_* code of include/skps_b200.h
+LAYOUTS = {"bgr": 0, "rgb": 1, "bgra": 2, "rgba": 3, "bgr_planar": 4, "rgb_planar": 5}
+PLANAR = ("bgr_planar", "rgb_planar")
+# skps_frame_layout of include/skps_b200.h: a frame's layout code and plane pitch, beside its skps_det_src / skps_face_src
+FRAME_LAYOUT = np.dtype([("layout", "<i4"), ("plane_pitch", "<i4")])
+
+FrameLayout = collections.namedtuple("FrameLayout", "H W pitch plane code")
+FrameLayout.__doc__ = """Where a CUDA frame's pixels are: its height and width, the bytes from one row to the next (pitch)
+and from one plane to the next (plane, 0 for interleaved layouts), and its SKPS_LAYOUT_* code."""
+
+
+def check_layout(layout, cuda=True):
+    """The SKPS_LAYOUT_* code of layout=, one of LAYOUTS.  ValueError for anything else, and for a layout other than "bgr"
+    with host frames (cuda False), which are HxWx3 BGR."""
+    if not isinstance(layout, str) or layout not in LAYOUTS:
+        raise ValueError("layout: expected one of %s, got %r" % (", ".join(repr(k) for k in LAYOUTS), layout))
+    if not cuda and layout != "bgr":
+        raise ValueError("layout=%r takes CUDA frames; host frames are HxWx3 uint8 BGR (layout='bgr')" % layout)
+    return LAYOUTS[layout]
+
+
+def frame_layout(shape, strides, layout):
+    """FrameLayout of a uint8 frame with this shape and these strides (in bytes) in layout `layout`:
+      "bgr", "rgb"            (H, W, 3), strides (>= 3W, 3, 1)
+      "bgra", "rgba"          (H, W, 4), strides (>= 4W, 4, 1); the 4th channel's values are never used
+      "bgr_planar", "rgb_planar"  (3, H, W), strides (any, >= W, 1): planes at any distance
+    A stride that never moves (the row stride of a one-row frame, the column stride of a one-column one) may be anything.
+    Row and plane pitches must fit 32 bits.  ValueError for anything else: the layout is what the caller says, never
+    guessed from the shape (a (3, W, 3) tensor fits two of them)."""
+    code = check_layout(layout)
+    shape, strides = tuple(int(v) for v in shape), tuple(int(v) for v in strides)
+    if len(shape) != 3 or len(strides) != 3:
+        raise ValueError("layout=%r: expected a 3-d frame, got shape %s" % (layout, shape))
+    if layout in PLANAR:
+        (C, H, W), (plane, sy, sx) = shape, strides
+        if C != 3:
+            raise ValueError("layout=%r: expected a (3, H, W) frame, got shape %s" % (layout, shape))
+        if H < 1 or W < 1:
+            raise ValueError("empty frame %s" % (shape,))
+        if (W > 1 and sx != 1) or (H > 1 and sy < W) or plane < 0:
+            raise ValueError("layout=%r: expected planes of rows, strides (any, >= W, 1); got strides %s for shape %s "
+                             "(an HxWxC tensor takes an interleaved layout such as layout='rgb')" % (layout, strides, shape))
+        pitch = sy if H > 1 else W
+    else:
+        C = 4 if layout in ("bgra", "rgba") else 3
+        (H, W, c), (sy, sx, sc) = shape, strides
+        if c != C:
+            raise ValueError("layout=%r: expected an (H, W, %d) frame, got shape %s%s"
+                             % (layout, C, shape, " (a planar tensor takes layout='rgb_planar' or 'bgr_planar')"
+                                if shape[0] == 3 else ""))
+        if H < 1 or W < 1:
+            raise ValueError("empty frame %s" % (shape,))
+        if sc != 1 or (W > 1 and sx != C) or (H > 1 and sy < C * W):
+            raise ValueError("layout=%r: expected interleaved pixels, strides (>= %dW, %d, 1); got strides %s for shape %s "
+                             "(name the frame's layout with layout=, e.g. 'rgb_planar' for a (3, H, W) tensor)"
+                             % (layout, C, C, strides, shape))
+        pitch, plane = (sy if H > 1 else C * W), 0
+    if pitch >= 2 ** 31:
+        raise ValueError("row pitch %d does not fit 32 bits" % pitch)
+    if plane >= 2 ** 31:
+        raise ValueError("plane pitch %d does not fit 32 bits" % plane)
+    return FrameLayout(H, W, pitch, plane, code)
 
 
 def check_host_frame(frame):
@@ -26,28 +91,20 @@ def is_tensor(x):
     return torch is not None and isinstance(x, torch.Tensor)
 
 
-def check_cuda_frame(frame, device, max_hw):
-    """(H, W, row pitch in bytes) of `frame`, a torch.uint8 CUDA tensor (H, W, 3) on `device` with interleaved channels:
-    stride(2) == 1, stride(1) == 3 and stride(0) >= 3 W, so packed tensors, pitched surfaces and big[y0:y1, x0:x1] views
-    all qualify.  ValueError for anything else, or for more pixels than max_hw = (max_h, max_w) allows."""
+def check_cuda_frame(frame, device, max_hw, layout="bgr"):
+    """FrameLayout of `frame`, a torch.uint8 CUDA tensor on `device` in layout `layout` (frame_layout): with the default
+    "bgr", (H, W, 3) with stride(2) == 1, stride(1) == 3 and stride(0) >= 3 W, so packed tensors, pitched surfaces and
+    big[y0:y1, x0:x1] views all qualify.  ValueError for anything else, or for more pixels than max_hw = (max_h, max_w)
+    allows."""
     if not is_tensor(frame):
         raise ValueError("expected a CUDA tensor, got %s" % type(frame).__name__)
     if not frame.is_cuda:
         raise ValueError("expected a CUDA tensor, got a tensor on %s" % frame.device)
-    if str(frame.dtype) != "torch.uint8" or frame.dim() != 3 or frame.shape[2] != 3:
-        raise ValueError("expected an HxWx3 uint8 BGR frame, got %s %s" % (frame.dtype, tuple(frame.shape)))
+    if str(frame.dtype) != "torch.uint8" or frame.dim() != 3:
+        raise ValueError("expected a uint8 frame in layout=%r, got %s %s" % (layout, frame.dtype, tuple(frame.shape)))
     if frame.device != device:
         raise ValueError("the frame is on %s, the pipeline on %s" % (frame.device, device))
-    H, W = int(frame.shape[0]), int(frame.shape[1])
-    if H < 1 or W < 1:
-        raise ValueError("empty frame %s" % (tuple(frame.shape),))
-    sy, sx, sc = frame.stride()
-    if sc != 1 or (W > 1 and sx != 3) or (H > 1 and sy < 3 * W):
-        raise ValueError("expected interleaved BGR pixels, strides (>= 3W, 3, 1); got strides %s for shape %s "
-                         "(a planar or permuted view: pass .contiguous())" % ((sy, sx, sc), tuple(frame.shape)))
-    if H * W > max_hw[0] * max_hw[1]:
-        raise ValueError("frame %dx%d has more pixels than max_frame_hw %dx%d" % (H, W, max_hw[0], max_hw[1]))
-    pitch = sy if H > 1 else 3 * W
-    if pitch >= 2 ** 31:
-        raise ValueError("row pitch %d does not fit 32 bits" % pitch)
-    return H, W, pitch
+    fl = frame_layout(frame.shape, frame.stride(), layout)
+    if fl.H * fl.W > max_hw[0] * max_hw[1]:
+        raise ValueError("frame %dx%d has more pixels than max_frame_hw %dx%d" % (fl.H, fl.W, max_hw[0], max_hw[1]))
+    return fl

@@ -21,7 +21,7 @@ import numpy as np
 from ... import runtime as rt
 from ...graph_tools import detector_onnx_for
 from ...logger.logger import logger
-from .device_frames import check_host_frame
+from .device_frames import FRAME_LAYOUT, check_host_frame
 from .onnx_model_base import ONNXEngine
 from .staging import Staging, check_frames, check_out, new_buffers, pad16
 
@@ -132,13 +132,13 @@ class FaceDetector:
         return bboxes
 
     # ------------------------------------------------------------------ batched path
-    def run_batch(self, frames):
+    def run_batch(self, frames, layout="bgr"):
         """The detector over many frames (blocking): the i-th (k_i, 16) float32 array of the returned list is bit for bit
         what FaceDetector(cfg)(frames[i]) returns; last_keep_idx is then the list of the frames' kept row indices (int64).
-        See submit() for what frames may be."""
+        See submit() for what frames and layout may be."""
         if self._pending:
             raise RuntimeError("FaceDetector: %d calls in flight; collect() them first" % len(self._pending))
-        self.submit(frames)
+        self.submit(frames, layout=layout)
         return self.collect()
 
     def new_results(self, n_frames):
@@ -148,7 +148,7 @@ class FaceDetector:
         rt.require_cuda()
         return new_buffers(result_fields(int(n_frames), self._rows), self.device)
 
-    def submit(self, frames, out=None):
+    def submit(self, frames, out=None, layout="bgr"):
         """Enqueue the detector on frames; at most two calls may be in flight and collect() returns them in submission
         order.  Everything is checked before anything is enqueued.
 
@@ -157,6 +157,9 @@ class FaceDetector:
         differ, as long as their letterbox fills the input (letterbox_geometry).  A host frame sends only the rows the
         letterbox reads when that is fewer than its rows (host_upload_rows), else the whole frame; a CUDA frame is read
         where it is.
+        layout: the pixel layout of all CUDA frames of the call (device_frames.frame_layout): "bgr" (the default), "rgb",
+        "bgra", "rgba" (H, W, 4), "bgr_planar" or "rgb_planar" (3, H, W).  The letterbox reads them in place, and the
+        results are, bit for bit, those of the same pixels passed as interleaved BGR.  Host frames are BGR only.
         Ordering on torch.cuda.current_stream(): CUDA frames are read after the work already queued on it, and work
         queued on it after submit() returns runs after they have been read.
         out: None (collect() returns numpy arrays), or, with CUDA frames, a dict from new_results(n) with n >= the call's
@@ -164,15 +167,15 @@ class FaceDetector:
         GPU."""
         if len(self._pending) == 2:
             raise RuntimeError("FaceDetector: two calls already in flight; call collect() first")
-        call = check_frames(frames, self.device)
-        layout = self._layout(call)
+        call = check_frames(frames, self.device, layout)
+        geo = self._layout(call)
         n = len(call.frames)
         if out is not None:
             if not call.cuda:
                 raise ValueError("out= keeps results on the GPU and takes CUDA frames")
             check_out(out, result_fields(n, self._rows), self.device, [p[2] for p in self._pending])
         slot = self._next
-        self._enqueue(call, layout, out, detect=True)
+        self._enqueue(call, geo, out, detect=True)
         self._pending.append((slot, n, out))
 
     def collect(self):
@@ -210,7 +213,7 @@ class FaceDetector:
         check_frames; ValueError for a frame whose letterbox is empty."""
         in_h, in_w = self.input_size[0], self.input_size[1]
         layout = []
-        for H, W, pitch in call.shapes:
+        for H, W, pitch, _, _ in call.shapes:
             geo = letterbox_geometry(H, W, in_h, in_w)
             if geo[1] < 1 or geo[2] < 1:
                 raise ValueError("frame %dx%d: its letterbox at %dx%d is %dx%d, empty" % (H, W, in_h, in_w, geo[2], geo[1]))
@@ -229,8 +232,11 @@ class FaceDetector:
             self._slots = [self._new_slot() for _ in range(2)]
         slot = self._next
         st = self._slots[slot]
+        # CUDA frames in a layout other than BGR: one skps_frame_layout per frame after the recoveries
+        lay = cuda and n > 0 and call.shapes[0].code != 0
         rec_off = pad16(n * DET_SRC.itemsize)
-        frame_off = rec_off + pad16(n * 12)
+        lay_off = rec_off + pad16(n * 12)
+        frame_off = lay_off + (pad16(n * FRAME_LAYOUT.itemsize) if lay else 0)
         sizes = [0 if cuda else pad16((H if rows is None else len(rows)) * pitch) for H, W, pitch, geo, rows in layout]
         total = frame_off + sum(sizes)
         own = detect and out is None                  # results go to the slot's buffers and come back to the host
@@ -241,9 +247,13 @@ class FaceDetector:
             st.update(new_buffers(result_fields(k, R), self.device))
             # the first M kept rows of every frame come back with the counts
             st.update({"h" + name: t.pin_memory() for name, t in new_buffers(result_fields(k, M), "cpu").items()})
-        # host staging = [n frame descriptors | n (scale, left, top) | the host frames' rows], sent with one copy
+        # host staging = [n frame descriptors | n (scale, left, top) | n layouts | the host frames' rows], sent with one copy
         desc = host[:n * DET_SRC.itemsize].view(DET_SRC)
         rec = host[rec_off:rec_off + 12 * n].view(np.float32).reshape(n, 3)
+        if lay:
+            fl = host[lay_off:lay_off + n * FRAME_LAYOUT.itemsize].view(FRAME_LAYOUT)
+            fl["layout"] = [f.code for f in call.shapes]
+            fl["plane_pitch"] = [f.plane for f in call.shapes]
         at = frame_off
         for i, (f, (H, W, pitch, (scale, rw, rh, top, left), rows), nb) in enumerate(zip(frames, layout, sizes)):
             rec[i] = (scale, left, top)
@@ -273,7 +283,9 @@ class FaceDetector:
         for c0 in range(0, n, K):
             m = min(K, n - c0)
             with torch.cuda.device(self.device):      # the kernels launch on the current device
-                rt.check(self.lib.skps_letterbox_frames(dev + DET_SRC.itemsize * c0, m, inp, in_h, in_w, s.cuda_stream))
+                rt.check(self.lib.skps_letterbox_frames_layout(dev + DET_SRC.itemsize * c0,
+                                                               dev + lay_off + FRAME_LAYOUT.itemsize * c0 if lay else None,
+                                                               m, inp, in_h, in_w, s.cuda_stream))
             if c0 + K >= n:
                 st["read"].record(s)
             if not detect:

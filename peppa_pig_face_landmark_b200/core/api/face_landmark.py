@@ -26,7 +26,7 @@ import numpy as np
 from ... import runtime as rt
 from ...logger.logger import logger
 from .align import check_size, chip_read_rects
-from .device_frames import is_cuda_tensor
+from .device_frames import FRAME_LAYOUT, is_cuda_tensor
 from .onnx_model_base import ONNXEngine
 from .staging import Staging, check_frames, check_out, grow, new_buffers, pad16
 
@@ -181,14 +181,14 @@ class FaceLandmark:
         return kps, scores
 
     # ------------------------------------------------------------------ batched path
-    def run_batch(self, frames, boxes):
+    def run_batch(self, frames, boxes, layout="bgr"):
         """Landmarks for the faces the caller has, over many frames (blocking): frames[i] with boxes[i] -> the i-th
         (kps (k_i, 98, 2) float32, scores (k_i, 98) float32) of the returned list, bit for bit what
         FaceLandmark(cfg)(frames[i], boxes[i]) returns; with align, (kps, scores, chips (k_i, s, s, 3) uint8,
-        M (k_i, 2, 3) float64).  See submit() for what frames and boxes may be."""
+        M (k_i, 2, 3) float64).  See submit() for what frames, boxes and layout may be."""
         if self._pending:
             raise RuntimeError("FaceLandmark: %d calls in flight; collect() them first" % len(self._pending))
-        self.submit(frames, boxes)
+        self.submit(frames, boxes, layout=layout)
         return self.collect()
 
     def new_results(self, n_faces):
@@ -201,7 +201,7 @@ class FaceLandmark:
     def _fields(self, n_faces):
         return result_fields(n_faces, self.keypoints_num, self.align)
 
-    def submit(self, frames, boxes, out=None):
+    def submit(self, frames, boxes, out=None, layout="bgr"):
         """Enqueue landmarks for boxes[i] on frames[i]; at most two calls may be in flight and collect() returns them in
         submission order.  Everything is checked before anything is enqueued.
 
@@ -215,6 +215,9 @@ class FaceLandmark:
         work queued on it after submit() returns runs after they have been read.
         out: None (collect() returns numpy arrays), or, with CUDA frames, a dict from new_results(n) with n >= the call's
         faces, not used by a call still in flight: the results are written there on the GPU.
+        layout: the pixel layout of all CUDA frames of the call (device_frames.frame_layout): "bgr" (the default), "rgb",
+        "bgra", "rgba" (H, W, 4), "bgr_planar" or "rgb_planar" (3, H, W).  Crops and chips read them in place and come
+        out BGR, bit for bit those of the same pixels passed as interleaved BGR.  Host frames are BGR only.
 
         With align, CUDA frames are warped into chips on the GPU right after the landmarks, with no host synchronisation,
         and are read until then.  Host frames are warped at collect(): M comes back with kps and scores, and
@@ -223,7 +226,7 @@ class FaceLandmark:
         collect() returns."""
         if len(self._pending) == 2:
             raise RuntimeError("FaceLandmark: two calls already in flight; call collect() first")
-        call = check_frames(frames, self.device)
+        call = check_frames(frames, self.device, layout)
         boxes, cuda_boxes = self._check_boxes(call, boxes)
         counts = [int(b.shape[0]) for b in boxes]
         if out is not None:
@@ -264,8 +267,11 @@ class FaceLandmark:
         warp_now = A is not None and call.cuda     # CUDA frames are warped here, host frames at collect()
         image = np.repeat(np.arange(len(counts)), counts)
         rects = None if call.cuda or n == 0 else np.concatenate(
-            [crop_read_rects(b, H, W, self.face_scale, self.min_face) for b, (H, W, _) in zip(boxes, call.shapes)])
-        box_off = pad16(n * FACE_SRC.itemsize)
+            [crop_read_rects(b, f.H, f.W, self.face_scale, self.min_face) for b, f in zip(boxes, call.shapes)])
+        # CUDA frames in a layout other than BGR: one skps_frame_layout per face after the descriptors
+        lay = call.cuda and n > 0 and call.shapes[0].code != 0
+        lay_off = pad16(n * FACE_SRC.itemsize)
+        box_off = lay_off + (pad16(n * FRAME_LAYOUT.itemsize) if lay else 0)
         roi_off = box_off + pad16(n * 16)
         total = roi_off + (0 if rects is None else int(_rect_bytes(rects).sum()))
         sent = box_off if cuda_boxes else total       # bytes of the host staging the call sends
@@ -283,15 +289,18 @@ class FaceLandmark:
             st["hM"] = grow(st["hM"], n, lambda k: torch.empty((k, 2, 3), dtype=torch.float64).pin_memory())
             st["chip"] = grow(st["chip"], n, lambda k: torch.empty((k, A, A, 3), dtype=torch.uint8, device=self.device))
             st["hchip"] = grow(st["hchip"], n, lambda k: torch.empty((k, A, A, 3), dtype=torch.uint8).pin_memory())
-        # host staging = [n face descriptors | n boxes | the host frames' rectangles], sent with one copy
+        # host staging = [n face descriptors | n layouts | n boxes | the host frames' rectangles], sent with one copy
         if n and not cuda_boxes:
             host[box_off:box_off + 16 * n].view(np.float32).reshape(n, 4)[:] = np.concatenate(boxes)
         if call.cuda:                                 # descriptors of the whole frames
             desc = host[:n * FACE_SRC.itemsize].view(FACE_SRC)
-            H, W, pitch = np.array(call.shapes, np.int64)[image].T
+            H, W, pitch, plane, code = np.array(call.shapes, np.int64).reshape(-1, 5)[image].T
             desc["base"] = np.array([f.data_ptr() for f in call.frames], np.uint64)[image]
             desc["pitch"], desc["H"], desc["W"], desc["rw"], desc["rh"] = pitch, H, W, W, H
             desc["ox"], desc["oy"], desc["_pad"] = 0, 0, 0
+            if lay:
+                fl = host[lay_off:lay_off + n * FRAME_LAYOUT.itemsize].view(FRAME_LAYOUT)
+                fl["layout"], fl["plane_pitch"] = code, plane
         elif n:
             _gather_rects(call.frames, rects, image, host, roi_off, dev)
 
@@ -311,9 +320,10 @@ class FaceLandmark:
         for c0 in range(0, n, K):
             m = min(K, n - c0)
             with torch.cuda.device(self.device):      # the kernels launch on the current device
-                rt.check(self.lib.skps_crop_faces(dev + FACE_SRC.itemsize * c0, dev + box_off + 16 * c0, m,
-                                                  self.face_scale, float(self.min_face), inp, S, det + 20 * c0,
-                                                  s.cuda_stream))
+                rt.check(self.lib.skps_crop_faces_layout(dev + FACE_SRC.itemsize * c0,
+                                                         dev + lay_off + FRAME_LAYOUT.itemsize * c0 if lay else None,
+                                                         dev + box_off + 16 * c0, m, self.face_scale, float(self.min_face),
+                                                         inp, S, det + 20 * c0, s.cuda_stream))
             if c0 + K >= n and not warp_now:
                 st["read"].record(s)
             outs = (C.c_void_p * 2)(None, scores.data_ptr() + 4 * P * c0)
@@ -326,7 +336,8 @@ class FaceLandmark:
             with torch.cuda.device(self.device):
                 rt.check(self.lib.skps_align_estimate(kps.data_ptr(), n, P, A, M.data_ptr(), s.cuda_stream))
                 if warp_now:                          # the face descriptors hold the whole CUDA frames
-                    rt.check(self.lib.skps_warp_faces(dev, M.data_ptr(), n, A, A, chips.data_ptr(), s.cuda_stream))
+                    rt.check(self.lib.skps_warp_faces_layout(dev, dev + lay_off if lay else None, M.data_ptr(), n, A, A,
+                                                             chips.data_ptr(), s.cuda_stream))
         if n == 0 or warp_now:
             st["read"].record(s)
         torch.cuda.current_stream(self.device).wait_event(st["read"])
@@ -375,7 +386,7 @@ class FaceLandmark:
         engine's stream, where no other kernel runs beside it, and copies them to the pinned h_chips[:n]."""
         torch = rt.require_cuda()
         n, A = len(M), self.align
-        rects = np.concatenate([chip_read_rects(M[o:o + k], A, H, W) for o, k, (H, W, _)
+        rects = np.concatenate([chip_read_rects(M[o:o + k], A, f.H, f.W) for o, k, f
                                 in zip(np.cumsum([0] + list(counts[:-1])), counts, call.shapes)])
         roi_off = pad16(n * FACE_SRC.itemsize)
         total = roi_off + int(_rect_bytes(rects).sum())

@@ -20,7 +20,7 @@ from ..smoother.lk import MAX_ID_MEMORY, EmaFilter, GroupTrack, IdMemory, assign
 from .face_detector import FaceDetector, letterbox_geometry
 from .face_landmark import MIN_FACE, FaceLandmark, face_scale
 from .align import check_size
-from .device_frames import check_cuda_frame, check_host_frame, is_cuda_tensor
+from .device_frames import PLANAR, check_cuda_frame, check_host_frame, check_layout, is_cuda_tensor
 
 
 MAX_TOP_K = 1024           # SKPS_MAX_TOP_K of include/skps_b200.h
@@ -179,15 +179,23 @@ class FaceAna():
             self._pipe = None
 
     # ------------------------------------------------------------------ facer.py:52-85
-    def run(self, image):
+    def run(self, image, layout="bgr"):
         """image: an HxWx3 uint8 BGR numpy array, or a torch.uint8 CUDA tensor (H, W, 3) in BGR order on this object's
         device with stride(2) == 1, stride(1) == 3 and any row pitch stride(0) >= 3W (a packed tensor, a pitched decoder
         surface, big[y0:y1, x0:x1]).  A CUDA frame is copied once on the GPU, never through the host, and the results are
         those of image.cpu().numpy() bit for bit.  Ordering on torch.cuda.current_stream(): the frame is read after all
         work already queued on it, and work queued on it after run() returns runs after the frame has been read, so a
-        decoder may overwrite the surface at once."""
+        decoder may overwrite the surface at once.
+
+        layout: the pixel layout of a CUDA frame (device_frames.frame_layout): "bgr" (the default), "rgb", "bgra",
+        "rgba" (H, W, 4), or "bgr_planar", "rgb_planar" (3, H, W) with any row and plane pitch.  The frame is packed
+        into BGR by the same GPU copy, and the results are, bit for bit, those of the same pixels passed as an
+        interleaved BGR frame.  Calls may change layouts from frame to frame.  Host frames are BGR only."""
+        check_layout(layout, is_cuda_tensor(image))
         image = image if is_cuda_tensor(image) else check_host_frame(image)
-        d = self._frame_diff(image)     # checks a CUDA frame, stages the frame on the device
+        d = self._frame_diff(image, layout)     # checks a CUDA frame, stages the frame on the device as BGR
+        if layout in PLANAR:
+            image = image.permute(1, 2, 0)      # an (H, W, 3) view: from here on only the frame's size is read
         forced = self.previous_image is None or d < 0       # no previous frame of this size
         run_det = self._cadence.step(forced) and (forced or d > self.diff_thres)
         self.last_ran_detector = run_det
@@ -287,16 +295,16 @@ class FaceAna():
             return True
         return bool(d > self.diff_thres)
 
-    def _frame_diff(self, image):
-        """Stages `image` on the device and returns the mean |prev - cur| against the previous staged frame, or a
-        negative number when that frame has another size (or there is none)."""
+    def _frame_diff(self, image, layout="bgr"):
+        """Stages `image` (a CUDA frame in layout `layout`) on the device as BGR and returns the mean |prev - cur|
+        against the previous staged frame, or a negative number when that frame has another size (or there is none)."""
         d = C.c_double(0.0)
         if is_cuda_tensor(image):
             import torch
-            H, W, pitch = check_cuda_frame(image, self._device, self._max_hw)
-            rt.check(self.lib.skps_pipeline_frame_diff_device(self._pipe, image.data_ptr(), H, W, pitch,
-                                                              torch.cuda.current_stream(self._device).cuda_stream,
-                                                              C.byref(d), self._stream.cuda_stream))
+            f = check_cuda_frame(image, self._device, self._max_hw, layout)
+            rt.check(self.lib.skps_pipeline_frame_diff_device_layout(
+                self._pipe, image.data_ptr(), f.H, f.W, f.pitch, f.code, f.plane,
+                torch.cuda.current_stream(self._device).cuda_stream, C.byref(d), self._stream.cuda_stream))
         else:
             rt.check(self.lib.skps_pipeline_frame_diff(self._pipe, image.ctypes.data, *image.shape[:2], C.byref(d),
                                                        self._stream.cuda_stream))

@@ -98,12 +98,12 @@ class FaceAnaImages:
         self._next = 0
 
     # ------------------------------------------------------------------
-    def run_batch(self, images):
+    def run_batch(self, images, layout="bgr"):
         """FaceAna.run after reset() for every image (blocking): one list of {'box', 'kps', 'scores'[, 'chip', 'M']
-        [, 'pose']} per image, [] for an image without a face.  See submit() for what images may be."""
+        [, 'pose']} per image, [] for an image without a face.  See submit() for what images and layout may be."""
         if self._pending:
             raise RuntimeError("FaceAnaImages: %d calls in flight; collect() them first" % len(self._pending))
-        self.submit(images)
+        self.submit(images, layout=layout)
         return self.collect()
 
     def new_results(self, n_images):
@@ -116,7 +116,7 @@ class FaceAnaImages:
         rt.require_cuda()
         return new_buffers(result_fields(int(n_images), self.top_k, self.n_points, self.pose, self.align), self.device)
 
-    def submit(self, images, out=None):
+    def submit(self, images, out=None, layout="bgr"):
         """Enqueue the analysis of images; at most two calls may be in flight and collect() returns them in submission
         order.  Everything is checked before anything is enqueued.  submit() returns once the call's landmark phase is
         enqueued: the face counts are read back once on the way, so it waits for the call's detector phase.
@@ -129,6 +129,10 @@ class FaceAnaImages:
         queued on it after submit() returns runs after they have been read, so the producer may reuse them at once.
         out: None (collect() returns lists of dicts), or, with CUDA images, a dict from new_results(n) with n >= the
         call's images, not used by a call still in flight: the results are written there on the GPU.
+        layout: the pixel layout of all CUDA images of the call (device_frames.frame_layout): "bgr" (the default),
+        "rgb", "bgra", "rgba" (H, W, 4), "bgr_planar" or "rgb_planar" (3, H, W).  Letterbox, crops and chips read them in
+        place, and the results are, bit for bit, those of the same pixels passed as interleaved BGR.  Host images are
+        BGR only.
 
         With align, CUDA images are warped into chips right after the landmarks, with no host synchronisation.  Host
         images are warped at collect(): M comes back with the other results, and only the rectangle of an image each
@@ -137,7 +141,7 @@ class FaceAnaImages:
         if len(self._pending) == 2:
             raise RuntimeError("FaceAnaImages: two calls already in flight; call collect() first")
         fd, fl = self.detector, self.landmark
-        call = check_frames(images, self.device)
+        call = check_frames(images, self.device, layout)
         layout = fd._layout(call)
         n = len(call.frames)
         if out is not None:

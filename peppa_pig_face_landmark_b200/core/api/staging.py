@@ -3,31 +3,32 @@ allocation of result buffers given as {name: (shape, dtype name)}, and the growa
 descriptors and host pixels with one copy."""
 import collections
 
-from .device_frames import check_cuda_frame, check_host_frame, is_cuda_tensor, is_tensor
+from .device_frames import FrameLayout, check_cuda_frame, check_host_frame, check_layout, is_cuda_tensor, is_tensor
 
 MAX_SIDE = 1 << 20         # largest frame side a call takes: keeps every row pitch and crop coordinate in int32
 
 Frames = collections.namedtuple("Frames", "frames shapes cuda")
-Frames.__doc__ = """A call's checked frames: the frames (host frames C-contiguous), (H, W, row pitch in bytes) of each,
-and whether they are CUDA tensors."""
+Frames.__doc__ = """A call's checked frames: the frames (host frames C-contiguous), the FrameLayout of each (H, W, row
+pitch and plane pitch in bytes, layout code; host frames are packed BGR) and whether they are CUDA tensors."""
 
 
-def check_frames(frames, device):
+def check_frames(frames, device, layout="bgr"):
     """Frames of a call, checked before anything is enqueued: all HxWx3 uint8 BGR numpy arrays, or all torch.uint8 CUDA
-    tensors (H, W, 3) on `device` that check_cuda_frame takes, with sides in 1..MAX_SIDE.  ValueError otherwise, and for
-    a mix of the two."""
+    tensors on `device` in layout `layout` that check_cuda_frame takes, with sides in 1..MAX_SIDE.  ValueError otherwise,
+    for a mix of the two, and for a layout other than "bgr" with host frames."""
     frames = list(frames)
     on_dev = [is_cuda_tensor(f) for f in frames]
     cuda = bool(on_dev) and all(on_dev)
     if any(on_dev) and not cuda:
         raise ValueError("one call takes either host frames or CUDA frames, got both (frames %s are CUDA)"
                          % [i for i, d in enumerate(on_dev) if d])
+    check_layout(layout, cuda or not frames)
     if cuda:
-        shapes = [check_cuda_frame(f, device, (MAX_SIDE, MAX_SIDE)) for f in frames]
+        shapes = [check_cuda_frame(f, device, (MAX_SIDE, MAX_SIDE), layout) for f in frames]
     else:
         frames = [check_host_frame(f) for f in frames]
-        shapes = [(f.shape[0], f.shape[1], 3 * f.shape[1]) for f in frames]
-    for H, W, _ in shapes:
+        shapes = [FrameLayout(f.shape[0], f.shape[1], 3 * f.shape[1], 0, 0) for f in frames]
+    for H, W, *_ in shapes:
         if not (0 < H <= MAX_SIDE and 0 < W <= MAX_SIDE):
             raise ValueError("frame %dx%d: sides must be in 1..%d" % (H, W, MAX_SIDE))
     return Frames(frames, shapes, cuda)

@@ -31,7 +31,7 @@ import numpy as np
 from ... import runtime as rt
 from ...graph_tools import check_detector_input, detector_onnx_for
 from .align import check_size
-from .device_frames import check_cuda_frame, check_host_frame, is_cuda_tensor
+from .device_frames import check_cuda_frame, check_host_frame, check_layout, is_cuda_tensor
 from .facer import check_detect_every, check_id_memory, get_cfg, pipeline_cfg
 from .onnx_model_base import ONNXEngine
 
@@ -155,7 +155,7 @@ class FaceAnaStreams:
             self.collect()
         rt.check(self.lib.skps_mpipe_reset(self._h, -1 if stream is None else int(stream)))
 
-    def submit(self, frames, out=None, streams=None):
+    def submit(self, frames, out=None, streams=None, layout="bgr"):
         """Enqueue one frame for each of some streams.  At most two batches may be pending; results come back from
         collect() in submission order.
 
@@ -173,6 +173,12 @@ class FaceAnaStreams:
         work already queued on it, and work queued on it after submit() returns runs after they have been read, so a
         decoder may reuse its surfaces at once.
 
+        layout: the pixel layout of all CUDA frames of the call (device_frames.frame_layout): "bgr" (the default),
+        "rgb", "bgra", "rgba" (H, W, 4), or "bgr_planar", "rgb_planar" (3, H, W) with any row and plane pitch.  The
+        gathering kernel packs them into the ring as BGR, so the results are, bit for bit, those of the same pixels
+        passed as interleaved BGR, and the gate, detect_every, track ids and smoothing do not see the layout: calls may
+        change it.  Host frames are BGR only.
+
         out: None (collect() returns host results), or, with CUDA frames, a dict from new_results() not used by a batch
         still in flight: the batch's results are written into it on the GPU and nothing is copied to the host."""
         if len(self._pending) == 2:
@@ -183,11 +189,12 @@ class FaceAnaStreams:
         ids = check_streams(streams, n, self.n_streams)
         smap = None if ids is None else np.array(ids, np.int32)
         on_device = [is_cuda_tensor(f) for f in frames]
+        check_layout(layout, any(on_device))
         if any(on_device):
             if not all(on_device):
                 raise ValueError("one batch takes either host frames or CUDA frames, got both (streams %s are CUDA)"
                                  % [i for i, d in enumerate(on_device) if d])
-            self._submit_device(frames, out, smap)
+            self._submit_device(frames, out, smap, layout)
             return
         if out is not None:
             raise ValueError("out= keeps results on the GPU and takes CUDA frames; these are host frames")
@@ -200,10 +207,10 @@ class FaceAnaStreams:
         self._pending.append((slot, n, keep, None))
         self._next ^= 1
 
-    def _submit_device(self, frames, out, smap):
+    def _submit_device(self, frames, out, smap, layout):
         import torch
         n = len(frames)
-        layout = [check_cuda_frame(f, self.device, self.max_frame_hw) for f in frames]
+        shapes = [check_cuda_frame(f, self.device, self.max_frame_hw, layout) for f in frames]
         outs = None
         if out is not None:
             self._check_out(out)
@@ -214,13 +221,14 @@ class FaceAnaStreams:
                 if k in out:
                     setattr(outs, field, out[k].data_ptr())
         ptrs = (C.c_void_p * n)(*[f.data_ptr() for f in frames])
-        pitches = np.array([p for _, _, p in layout], np.int32)
-        hw = np.array([[h, w] for h, w, _ in layout], np.int32)
+        pitches = np.array([f.pitch for f in shapes], np.int32)
+        planes = np.array([f.plane for f in shapes], np.int32)
+        hw = np.array([[f.H, f.W] for f in shapes], np.int32)
         slot = self._next
-        rt.check(self.lib.skps_mpipe_submit_device_streams(self._h, slot, None if smap is None else smap.ctypes.data, ptrs,
-                                                           pitches.ctypes.data, hw.ctypes.data, n,
-                                                           None if outs is None else C.byref(outs),
-                                                           torch.cuda.current_stream(self.device).cuda_stream))
+        rt.check(self.lib.skps_mpipe_submit_device_layout(self._h, slot, None if smap is None else smap.ctypes.data, ptrs,
+                                                          pitches.ctypes.data, hw.ctypes.data, n, shapes[0].code,
+                                                          planes.ctypes.data, None if outs is None else C.byref(outs),
+                                                          torch.cuda.current_stream(self.device).cuda_stream))
         self._pending.append((slot, n, list(frames), out))
         self._next ^= 1
 
@@ -311,7 +319,8 @@ class FaceAnaStreams:
                     r['id'] = int(o["ids"][s, i])
         return res
 
-    def run(self, frames, streams=None):
-        """One frame for each of some streams in (submit's streams=), their results out in call order (blocking)."""
-        self.submit(frames, streams=streams)
+    def run(self, frames, streams=None, layout="bgr"):
+        """One frame for each of some streams in (submit's streams= and layout=), their results out in call order
+        (blocking)."""
+        self.submit(frames, streams=streams, layout=layout)
         return self.collect()

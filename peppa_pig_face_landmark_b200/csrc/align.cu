@@ -8,7 +8,8 @@
 // Two launches cover every face of every frame of a call: the estimate (a thread per face), then the warp (grid.y = face,
 // grid.x = runs of 256 pixels of the face's chip, stored with consecutive threads on consecutive bytes).  The frame is
 // read where it lies.  A face's source is one frame for all faces, one MpStreamDesc per group of faces, or one
-// skps_face_src per face (faces of many images, or just the rectangle of an image a chip reads).
+// skps_face_src per face (faces of many images, or just the rectangle of an image a chip reads), which may give any pixel
+// layout of skps_b200.h: only the address of a tap depends on it, the chip is BGR.
 #include <limits.h>
 
 #include "../../include/skps_b200.h"
@@ -61,7 +62,8 @@ __device__ __forceinline__ int sat_short(int v) { return v < -32768 ? -32768 : (
 struct WarpArgs {
     const uint8_t* frame; int H, W, pitch;      // the frame of every face (desc == null)
     const MpStreamDesc* desc;                   // or per group: desc[g].cur, H, W (pitch W*3)
-    const skps_face_src* src;                   // or per face: src[f], taps outside its rectangle read 0
+    const skps_face_src* src;                   // or per face: src[f], taps outside its rectangle read 0,
+    const skps_frame_layout* lay;               // its pixels laid out as lay[f] says (null: BGR)
     const double* M;                            // [faces][2][3] frame -> chip
     const int* count; int per_group;            // face f = g * per_group + i is skipped when count && i >= count[g]
     int out_h, out_w;
@@ -95,12 +97,14 @@ __global__ void __launch_bounds__(256) align_warp_kernel(const WarpArgs a) {
         // base holds the rectangle of an H x W image at column ox, row oy, rw x rh pixels
         const uint8_t* base = a.frame;
         int H = a.H, W = a.W, pitch = a.pitch, ox = 0, oy = 0, rw = a.W, rh = a.H;
+        PxLayout lay = px_layout(SKPS_LAYOUT_BGR, 0);
         if (a.desc) {
             const MpStreamDesc& d = a.desc[g];
             base = d.cur; H = d.H; W = d.W; pitch = d.W * 3; rw = W; rh = H;
         } else if (a.src) {
             const skps_face_src& s = a.src[f];
             base = s.base; H = s.H; W = s.W; pitch = s.pitch; ox = s.ox; oy = s.oy; rw = s.rw; rh = s.rh;
+            if (a.lay) lay = px_layout(a.lay[f].layout, a.lay[f].plane_pitch);
         }
         const int xa = max(ox, 0), xb = min(ox + rw, W), ya = max(oy, 0), yb = min(oy + rh, H);
         // the inverse map as warpAffine computes it (imgwarp.cpp), same order of operations; every thread of the face
@@ -126,12 +130,15 @@ __global__ void __launch_bounds__(256) align_warp_kernel(const WarpArgs a) {
         // taps outside the frame read the border value 0; so do taps outside the rectangle, which are never dereferenced
         const bool x0 = sx >= xa && sx < xb, x1 = sx + 1 >= xa && sx + 1 < xb;
         const bool y0 = sy >= ya && sy < yb, y1 = sy + 1 >= ya && sy + 1 < yb;
-        const uint8_t* r0 = base + (ptrdiff_t)(sy - oy) * pitch + (ptrdiff_t)(sx - ox) * 3;   // dereferenced only where inside
+        const uint8_t* r0 = base + (ptrdiff_t)(sy - oy) * pitch + (ptrdiff_t)(sx - ox) * lay.xs;   // dereferenced only where inside
         const uint8_t* r1 = r0 + pitch;
+        const int xs = lay.xs;
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
-            const int acc = (y0 && x0 ? (int)__ldg(r0 + c) : 0) * w00 + (y0 && x1 ? (int)__ldg(r0 + 3 + c) : 0) * w01 +
-                            (y1 && x0 ? (int)__ldg(r1 + c) : 0) * w10 + (y1 && x1 ? (int)__ldg(r1 + 3 + c) : 0) * w11;
+            const uint8_t* p0 = r0 + lay.off[c];
+            const uint8_t* p1 = r1 + lay.off[c];
+            const int acc = (y0 && x0 ? (int)__ldg(p0) : 0) * w00 + (y0 && x1 ? (int)__ldg(p0 + xs) : 0) * w01 +
+                            (y1 && x0 ? (int)__ldg(p1) : 0) * w10 + (y1 && x1 ? (int)__ldg(p1 + xs) : 0) * w11;
             // weights * 32 sum to 2^15: (sum * 32 + 2^14) >> 15 == (sum + 2^9) >> 10; at most 255
             px[threadIdx.x * 3 + c] = (uint8_t)min((acc + 512) >> 10, 255);
         }
@@ -192,8 +199,8 @@ extern "C" SKPS_API int skps_align_faces(const uint8_t* frame, int H, int W, int
     return launch_align(frame, H, W, pitch, nullptr, kps, P, count, n, n, size, chips, M, (cudaStream_t)stream);
 }
 
-extern "C" SKPS_API int skps_warp_faces(const skps_face_src* src, const double* M, int n, int out_h, int out_w, uint8_t* out,
-                                        void* stream) {
+extern "C" SKPS_API int skps_warp_faces_layout(const skps_face_src* src, const skps_frame_layout* lay, const double* M, int n,
+                                               int out_h, int out_w, uint8_t* out, void* stream) {
     SKPS_CHECK(n >= 0 && out_h > 0 && out_w > 0 && out_h <= 4096 && out_w <= 4096,
                "warp_faces: n %d or output %dx%d out of range", n, out_h, out_w);
     if (n == 0) return 0;
@@ -202,11 +209,16 @@ extern "C" SKPS_API int skps_warp_faces(const skps_face_src* src, const double* 
     for (int c0 = 0; c0 < n; c0 += 65535) {
         const int m = min(65535, n - c0);
         WarpArgs a = {};
-        a.src = src + c0; a.M = M + (size_t)c0 * 6; a.per_group = m;
+        a.src = src + c0; a.lay = lay ? lay + c0 : nullptr; a.M = M + (size_t)c0 * 6; a.per_group = m;
         a.out_h = out_h; a.out_w = out_w; a.out = out + (size_t)c0 * out_h * out_w * 3;
         if (launch_warp(a, m, (cudaStream_t)stream)) return 1;
     }
     return 0;
+}
+
+extern "C" SKPS_API int skps_warp_faces(const skps_face_src* src, const double* M, int n, int out_h, int out_w, uint8_t* out,
+                                        void* stream) {
+    return skps_warp_faces_layout(src, nullptr, M, n, out_h, out_w, out, stream);
 }
 
 extern "C" SKPS_API int skps_align_estimate(const float* kps, int n, int P, int size, double* M, void* stream) {

@@ -2,6 +2,9 @@
 // with cv2.resize INTER_LINEAR on uint8), face selection (IoU track match + EMA, area filter, top-k), landmark
 // de-normalisation and the frame-difference gate.  All HBM-bound byte/index work; compiled with
 // -fmad=false so float32 expressions round exactly like the numpy expressions they restate.
+// The caller's device frames may be in any pixel layout of skps_b200.h (interleaved BGR / RGB / BGRA / RGBA, planar
+// BGR / RGB): the letterbox and the face crop read them where they are, through PxLayout, and the frame ingest repacks
+// them into interleaved BGR.  Only the address of a sample depends on the layout, never the arithmetic.
 #include <string.h>
 
 #include "../../include/skps_b200.h"
@@ -46,9 +49,10 @@ __device__ __forceinline__ int vblend(int h0, int h1, int b0, int b1) {
 // output pixel (3 channels); output is uint8 RGB NHWC, /255 happens in the first conv.
 // ------------------------------------------------------------------------------------------
 // `frame` holds the whole frame, or with row_pairs only the two rows each resized row reads: rows 2 dy and 2 dy + 1.
+// Its pixels are laid out as `lay` says (BGR: xs 3, off {0, 1, 2}).
 __device__ __forceinline__ void letterbox_px(const uint8_t* __restrict__ frame, int H, int W, int pitch, int row_pairs,
-                                             uint8_t* __restrict__ out, int in_h, int in_w, int rw, int rh, int top, int left,
-                                             int x, int y) {
+                                             const PxLayout& lay, uint8_t* __restrict__ out, int in_h, int in_w, int rw,
+                                             int rh, int top, int left, int x, int y) {
     if (x >= in_w) return;
     uint8_t* o = out + ((long long)y * in_w + x) * 3;
     int dx = x - left, dy = y - top;
@@ -60,10 +64,13 @@ __device__ __forceinline__ void letterbox_px(const uint8_t* __restrict__ frame, 
     Tap ty = linear_tap(dy, rh, H, false);
     const uint8_t* r0 = frame + (long long)(row_pairs ? 2 * dy : ty.i0) * pitch;
     const uint8_t* r1 = frame + (long long)(row_pairs ? 2 * dy + 1 : ty.i1) * pitch;
+    const int x0 = tx.i0 * lay.xs, x1 = tx.i1 * lay.xs;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-        int h0 = r0[tx.i0 * 3 + c] * tx.w0 + r0[tx.i1 * 3 + c] * tx.w1;
-        int h1 = r1[tx.i0 * 3 + c] * tx.w0 + r1[tx.i1 * 3 + c] * tx.w1;
+        const uint8_t* a = r0 + lay.off[c];
+        const uint8_t* b = r1 + lay.off[c];
+        int h0 = a[x0] * tx.w0 + a[x1] * tx.w1;
+        int h1 = b[x0] * tx.w0 + b[x1] * tx.w1;
         o[2 - c] = (uint8_t)vblend(h0, h1, ty.w0, ty.w1);      // BGR -> RGB
     }
 }
@@ -71,6 +78,7 @@ __device__ __forceinline__ void letterbox_px(const uint8_t* __restrict__ frame, 
 __global__ void __launch_bounds__(256) letterbox_frames_kernel(const LetterboxArgs a) {
     const uint8_t* frame = a.frame;
     int H = a.H, W = a.W, pitch = a.pitch, rw = a.rw, rh = a.rh, top = a.top, left = a.left, row_pairs = 0;
+    PxLayout lay = px_layout(SKPS_LAYOUT_BGR, 0);
     if (a.desc) {
         const MpStreamDesc D = a.desc[blockIdx.z];
         frame = D.cur; H = D.H; W = D.W; pitch = D.W * 3; rw = D.rw; rh = D.rh; top = D.top; left = D.left;
@@ -78,8 +86,9 @@ __global__ void __launch_bounds__(256) letterbox_frames_kernel(const LetterboxAr
         const skps_det_src F = a.src[blockIdx.z];
         frame = F.base; H = F.H; W = F.W; pitch = F.pitch; rw = F.rw; rh = F.rh; top = F.top; left = F.left;
         row_pairs = F.row_pairs;
+        if (a.lay) lay = px_layout(a.lay[blockIdx.z].layout, a.lay[blockIdx.z].plane_pitch);
     }
-    letterbox_px(frame, H, W, pitch, row_pairs, a.out + a.out_stride * blockIdx.z, a.in_h, a.in_w, rw, rh, top, left,
+    letterbox_px(frame, H, W, pitch, row_pairs, lay, a.out + a.out_stride * blockIdx.z, a.in_h, a.in_w, rw, rh, top, left,
                  blockIdx.x * blockDim.x + threadIdx.x, blockIdx.y);
 }
 
@@ -112,12 +121,13 @@ __device__ __forceinline__ CropGeo crop_geometry(const float* b, int H, int W, f
 }
 
 // Output pixel (x, y) of the crop of one face with box b into o, and at (0, 0) its detail d = [h, w, y1, x1, add].  The
-// frame is H x W; `base` holds only its rectangle starting at column ox, row oy, rows `pitch` bytes apart.  Whether a tap
-// is in the frame or in the zero border is decided against the whole frame, so a caller that holds only the rectangle
-// the taps can reach gets the same bytes as one that holds the whole frame (ox = oy = 0).
+// frame is H x W; `base` holds only its rectangle starting at column ox, row oy, rows `pitch` bytes apart, pixels laid
+// out as `lay` says.  Whether a tap is in the frame or in the zero border is decided against the whole frame, so a caller
+// that holds only the rectangle the taps can reach gets the same bytes as one that holds the whole frame (ox = oy = 0).
 __device__ __forceinline__ void crop_face_px(const uint8_t* __restrict__ base, int H, int W, int pitch, int ox, int oy,
-                                             const float* __restrict__ b, float face_scale, float min_face,
-                                             uint8_t* __restrict__ o, int S, int* __restrict__ d, int x, int y) {
+                                             const PxLayout& lay, const float* __restrict__ b, float face_scale,
+                                             float min_face, uint8_t* __restrict__ o, int S, int* __restrict__ d, int x,
+                                             int y) {
     CropGeo g = crop_geometry(b, H, W, face_scale, min_face);
     if (x == 0 && y == 0) {
         d[0] = g.h; d[1] = g.w; d[2] = g.y1; d[3] = g.x1; d[4] = g.add;
@@ -132,10 +142,13 @@ __device__ __forceinline__ void crop_face_px(const uint8_t* __restrict__ base, i
     bool vy0 = fy0 >= 0 && fy0 < H, vy1 = fy1 >= 0 && fy1 < H;
     const uint8_t* r0 = base + (long long)((vy0 ? fy0 : oy) - oy) * pitch;
     const uint8_t* r1 = base + (long long)((vy1 ? fy1 : oy) - oy) * pitch;
+    const int x0 = (fx0 - ox) * lay.xs, x1 = (fx1 - ox) * lay.xs;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-        int p00 = (vy0 && vx0) ? r0[(fx0 - ox) * 3 + c] : 0, p01 = (vy0 && vx1) ? r0[(fx1 - ox) * 3 + c] : 0;
-        int p10 = (vy1 && vx0) ? r1[(fx0 - ox) * 3 + c] : 0, p11 = (vy1 && vx1) ? r1[(fx1 - ox) * 3 + c] : 0;
+        const uint8_t* a = r0 + lay.off[c];
+        const uint8_t* e = r1 + lay.off[c];
+        int p00 = (vy0 && vx0) ? a[x0] : 0, p01 = (vy0 && vx1) ? a[x1] : 0;
+        int p10 = (vy1 && vx0) ? e[x0] : 0, p11 = (vy1 && vx1) ? e[x1] : 0;
         int h0 = p00 * tx.w0 + p01 * tx.w1;
         int h1 = p10 * tx.w0 + p11 * tx.w1;
         o[c] = (uint8_t)vblend(h0, h1, ty.w0, ty.w1);          // stays BGR (face_landmark.py:44)
@@ -154,7 +167,8 @@ __device__ __forceinline__ void crop_px(const uint8_t* __restrict__ frame, int H
         if (x == 0 && y == 0) { for (int k = 0; k < 5; ++k) detail[face * 5 + k] = 0; }
         return;
     }
-    crop_face_px(frame, H, W, pitch, 0, 0, boxes + face * 4, face_scale, min_face, o, S, detail + face * 5, x, y);
+    crop_face_px(frame, H, W, pitch, 0, 0, px_layout(SKPS_LAYOUT_BGR, 0), boxes + face * 4, face_scale, min_face, o, S,
+                 detail + face * 5, x, y);
 }
 // block z = face of a frame (K per frame)
 __global__ void __launch_bounds__(256) crop_frames_kernel(const CropArgs a) {
@@ -169,14 +183,17 @@ __global__ void __launch_bounds__(256) crop_frames_kernel(const CropArgs a) {
             a.crops + (size_t)a.S * a.S * 3 * a.K * g, a.S, a.detail + (size_t)5 * a.K * g, face,
             blockIdx.x * blockDim.x + threadIdx.x, blockIdx.y);
 }
-// Face table variant (FaceLandmark.submit): block z = face, each face with its own frame or frame rectangle.
-__global__ void __launch_bounds__(256) crop_faces_kernel(const skps_face_src* __restrict__ src, const float* __restrict__ boxes,
-                                                         float face_scale, float min_face, uint8_t* __restrict__ crops, int S,
-                                                         int* __restrict__ detail) {
+// Face table variant (FaceLandmark.submit): block z = face, each face with its own frame or frame rectangle, laid out as
+// lay[face] says (lay null: BGR).
+__global__ void __launch_bounds__(256) crop_faces_kernel(const skps_face_src* __restrict__ src,
+                                                         const skps_frame_layout* __restrict__ lay,
+                                                         const float* __restrict__ boxes, float face_scale, float min_face,
+                                                         uint8_t* __restrict__ crops, int S, int* __restrict__ detail) {
     const int face = blockIdx.z, x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
     if (x >= S) return;
     const skps_face_src F = src[face];
-    crop_face_px(F.base, F.H, F.W, F.pitch, F.ox, F.oy, boxes + face * 4, face_scale, min_face,
+    const PxLayout L = lay ? px_layout(lay[face].layout, lay[face].plane_pitch) : px_layout(SKPS_LAYOUT_BGR, 0);
+    crop_face_px(F.base, F.H, F.W, F.pitch, F.ox, F.oy, L, boxes + face * 4, face_scale, min_face,
                  crops + (((long long)face * S + y) * S + x) * 3, S, detail + face * 5, x, y);
 }
 
@@ -504,14 +521,8 @@ __device__ __forceinline__ unsigned long long absdiff_bytes(const uint8_t* __res
     return local;
 }
 
-// 16 bytes from an address of any alignment: the one or two aligned 16-byte blocks that hold them, shifted into place.
-// Every block loaded holds a byte of the range, so no load leaves the allocation.
-__device__ __forceinline__ uint4 load16_any(const uint8_t* p) {
-    const unsigned off = (unsigned)((uintptr_t)p & 15);
-    const uint4* a = reinterpret_cast<const uint4*>(p - off);
-    const uint4 lo = __ldg(a);
-    if (off == 0) return lo;
-    const uint4 hi = __ldg(a + 1);
+// The 16 bytes that start `off` (0..15) bytes into the 32 bytes lo, hi (lo when off is 0).
+__device__ __forceinline__ uint4 shift16(const uint4& lo, const uint4& hi, unsigned off) {
     unsigned w0, w1, w2, w3, w4;
     switch (off >> 2) {
         case 0: w0 = lo.x; w1 = lo.y; w2 = lo.z; w3 = lo.w; w4 = hi.x; break;
@@ -522,6 +533,52 @@ __device__ __forceinline__ uint4 load16_any(const uint8_t* p) {
     const unsigned sh = (off & 3) * 8;
     return make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh),
                       __funnelshift_r(w3, w4, sh));
+}
+
+// 16 bytes from an address of any alignment: the one or two aligned 16-byte blocks that hold them, shifted into place.
+// Every block loaded holds a byte of the range, so no load leaves the allocation.
+__device__ __forceinline__ uint4 load16_any(const uint8_t* p) {
+    const unsigned off = (unsigned)((uintptr_t)p & 15);
+    const uint4* a = reinterpret_cast<const uint4*>(p - off);
+    const uint4 lo = __ldg(a);
+    if (off == 0) return lo;
+    return shift16(lo, __ldg(a + 1), off);
+}
+
+// 16 N bytes from an address of any alignment into w[0 .. 4N): the N + 1 aligned blocks that hold them (N when aligned),
+// each loaded once.  As in load16_any, every block loaded holds a byte of the range.
+template <int N>
+__device__ __forceinline__ void load_any(const uint8_t* p, unsigned (&w)[4 * N]) {
+    const unsigned off = (unsigned)((uintptr_t)p & 15);
+    const uint4* a = reinterpret_cast<const uint4*>(p - off);
+    uint4 blk[N + 1];
+#pragma unroll
+    for (int k = 0; k < N; ++k) blk[k] = __ldg(a + k);
+    blk[N] = off ? __ldg(a + N) : make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+        const uint4 v = shift16(blk[k], blk[k + 1], off);
+        w[4 * k] = v.x; w[4 * k + 1] = v.y; w[4 * k + 2] = v.z; w[4 * k + 3] = v.w;
+    }
+}
+
+// Ingest of a layout other than BGR, 16 pixels at a time.  The unit's source bytes are loaded as they lie: 48 (RGB) or
+// 64 (BGRA, RGBA) interleaved bytes, or 16 bytes of each plane, in the order B, G, R (planar).  Byte o of the packed BGR
+// unit, channel c = o % 3 of pixel p = o / 3, is their byte in_byte(o).
+template <int L>
+__device__ __forceinline__ constexpr int in_byte(int o) {
+    return L == SKPS_LAYOUT_RGB    ? 3 * (o / 3) + 2 - o % 3
+         : L == SKPS_LAYOUT_BGRA   ? 4 * (o / 3) + o % 3
+         : L == SKPS_LAYOUT_RGBA   ? 4 * (o / 3) + 2 - o % 3
+                                   : 16 * (o % 3) + o / 3;          // planar
+}
+// Word k of the packed unit: three byte permutes.
+template <int L, int NW>
+__device__ __forceinline__ unsigned packed_word(const unsigned (&in)[NW], int k) {
+    const int i0 = in_byte<L>(4 * k), i1 = in_byte<L>(4 * k + 1), i2 = in_byte<L>(4 * k + 2), i3 = in_byte<L>(4 * k + 3);
+    const unsigned lo = __byte_perm(in[i0 >> 2], in[i1 >> 2], (i0 & 3) | (((i1 & 3) + 4) << 4));
+    const unsigned hi = __byte_perm(in[i2 >> 2], in[i3 >> 2], (i2 & 3) | (((i3 & 3) + 4) << 4));
+    return __byte_perm(lo, hi, 0x5410);
 }
 
 // Ingest of one frame: the packed frame cur is cut into 16-byte units; unit u takes bytes [16u, 16u + 16) of the frame
@@ -559,13 +616,82 @@ __device__ __forceinline__ unsigned long long ingest_units(const MpStreamDesc& D
     return local;
 }
 
-// block y = frame (integer sums: the order of the atomic adds does not matter)
+// Ingest of one frame in layout L (not BGR): the packed frame cur is cut into units of 16 pixels, 48 bytes; unit u takes
+// pixels [16u, 16u + 16) of the frame, from row y = 16u / W.  A unit inside one row is loaded with 16-byte loads
+// (load_any), repacked in registers (packed_word) and stored as three 16-byte stores; a unit that crosses a row end, and
+// the partial last unit, go pixel by pixel.  Returns this thread's part of sum |cur - prev|, the same integer sum as for
+// BGR pixels, whose units it regroups.
+template <int L>
+__device__ __forceinline__ unsigned long long ingest_pixels(const MpStreamDesc& D) {
+    constexpr bool planar = L == SKPS_LAYOUT_BGR_PLANAR || L == SKPS_LAYOUT_RGB_PLANAR;
+    constexpr int xs = planar ? 1 : (L == SKPS_LAYOUT_RGB ? 3 : 4);
+    const PxLayout lay = px_layout(L, D.src_plane);
+    const unsigned W = (unsigned)D.W, n = W * (unsigned)D.H, units = (n + 15) / 16;
+    const uint8_t* __restrict__ src = D.src;
+    uint8_t* __restrict__ cur = D.cur;
+    const uint8_t* __restrict__ prev = D.have_prev ? D.prev : nullptr;
+    unsigned long long local = 0;
+    for (unsigned u = blockIdx.x * blockDim.x + threadIdx.x; u < units; u += gridDim.x * blockDim.x) {
+        const unsigned p = u * 16, y = p / W, x = p - y * W;
+        const uint8_t* row = src + (size_t)y * D.src_pitch;
+        if (x + 16 <= W) {
+            unsigned in[planar ? 12 : 4 * xs];
+            if constexpr (planar) {
+                unsigned b[4], g[4], r[4];
+                load_any<1>(row + lay.off[0] + x, b);
+                load_any<1>(row + lay.off[1] + x, g);
+                load_any<1>(row + lay.off[2] + x, r);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) { in[k] = b[k]; in[4 + k] = g[k]; in[8 + k] = r[k]; }
+            } else {
+                load_any<xs>(row + (size_t)x * xs, in);
+            }
+            unsigned o[12];
+#pragma unroll
+            for (int k = 0; k < 12; ++k) o[k] = packed_word<L>(in, k);
+            uint4* c4 = reinterpret_cast<uint4*>(cur + (size_t)p * 3);
+#pragma unroll
+            for (int k = 0; k < 3; ++k) c4[k] = make_uint4(o[4 * k], o[4 * k + 1], o[4 * k + 2], o[4 * k + 3]);
+            if (prev) {
+                const uint4* q4 = reinterpret_cast<const uint4*>(prev + (size_t)p * 3);
+#pragma unroll
+                for (int k = 0; k < 3; ++k) {
+                    const uint4 q = q4[k];
+                    local += __vsadu4(o[4 * k], q.x) + __vsadu4(o[4 * k + 1], q.y) + __vsadu4(o[4 * k + 2], q.z) +
+                             __vsadu4(o[4 * k + 3], q.w);
+                }
+            }
+        } else {
+            unsigned yy = y, xx = x;
+            const unsigned end = p + 16 < n ? p + 16 : n;
+            for (unsigned i = p; i < end; ++i) {
+                const uint8_t* px = src + (size_t)yy * D.src_pitch + (size_t)xx * xs;
+#pragma unroll
+                for (int c = 0; c < 3; ++c) {
+                    const uint8_t v = px[lay.off[c]];
+                    cur[(size_t)i * 3 + c] = v;
+                    if (prev) {
+                        const int dd = (int)v - (int)prev[(size_t)i * 3 + c];
+                        local += (unsigned)(dd < 0 ? -dd : dd);
+                    }
+                }
+                if (++xx == W) { xx = 0; ++yy; }
+            }
+        }
+    }
+    return local;
+}
+
+// block y = frame (integer sums: the order of the atomic adds does not matter); L: the layout of the frames with src set
+template <int L>
 __global__ void __launch_bounds__(256) diff_frames_kernel(const MpStreamDesc* __restrict__ d, MpStreamDesc one, size_t one_bytes,
                                                           unsigned long long* __restrict__ sum) {
     const MpStreamDesc D = d ? d[blockIdx.y] : one;
     const size_t n = d ? (size_t)D.H * D.W * 3 : one_bytes;
     if (!D.have_prev && !D.src) return;
-    unsigned long long local = D.src ? ingest_units(D) : absdiff_bytes(D.prev, D.cur, n);
+    unsigned long long local;
+    if constexpr (L == SKPS_LAYOUT_BGR) local = D.src ? ingest_units(D) : absdiff_bytes(D.prev, D.cur, n);
+    else local = D.src ? ingest_pixels<L>(D) : absdiff_bytes(D.prev, D.cur, n);
     for (int o = 16; o > 0; o >>= 1) local += __shfl_down_sync(0xffffffffu, local, o);
     __shared__ unsigned long long warp_sum[8];
     if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = local;
@@ -578,14 +704,25 @@ __global__ void __launch_bounds__(256) diff_frames_kernel(const MpStreamDesc* __
 }
 
 int launch_frame_diff(const MpStreamDesc* d, int n, const MpStreamDesc& one, size_t bytes, unsigned long long* sum,
-                      cudaStream_t s) {
-    // ingest_units counts the 16-byte units of a frame in 32 bits
+                      cudaStream_t s, int layout) {
+    // ingest_units counts the 16-byte units of a frame in 32 bits, ingest_pixels its packed bytes
     SKPS_CHECK(bytes < (1ull << 32) - 16 || !(d || one.src), "frame_diff: a %zu-byte frame is larger than 4 GB", bytes);
-    // a 16-byte unit per thread, at most 8 blocks per SM per frame
-    size_t blocks = (bytes / 16 + 255) / 256;
+    SKPS_CHECK(layout_ok(layout), "frame_diff: unknown pixel layout %d", layout);
+    // a unit per thread (16 bytes; 16 pixels for the other layouts), at most 8 blocks per SM per frame
+    const size_t units = layout == SKPS_LAYOUT_BGR ? bytes / 16 : bytes / 48;
+    size_t blocks = (units + 255) / 256;
     if (blocks > (size_t)sm_count() * 8) blocks = (size_t)sm_count() * 8;
     if (blocks < 1) blocks = 1;
-    diff_frames_kernel<<<dim3((unsigned)blocks, n), 256, 0, s>>>(d, one, bytes, sum);
+    const dim3 grid((unsigned)blocks, n);
+    switch (layout) {
+        case SKPS_LAYOUT_BGR: diff_frames_kernel<SKPS_LAYOUT_BGR><<<grid, 256, 0, s>>>(d, one, bytes, sum); break;
+        case SKPS_LAYOUT_RGB: diff_frames_kernel<SKPS_LAYOUT_RGB><<<grid, 256, 0, s>>>(d, one, bytes, sum); break;
+        case SKPS_LAYOUT_BGRA: diff_frames_kernel<SKPS_LAYOUT_BGRA><<<grid, 256, 0, s>>>(d, one, bytes, sum); break;
+        case SKPS_LAYOUT_RGBA: diff_frames_kernel<SKPS_LAYOUT_RGBA><<<grid, 256, 0, s>>>(d, one, bytes, sum); break;
+        case SKPS_LAYOUT_BGR_PLANAR:
+            diff_frames_kernel<SKPS_LAYOUT_BGR_PLANAR><<<grid, 256, 0, s>>>(d, one, bytes, sum); break;
+        default: diff_frames_kernel<SKPS_LAYOUT_RGB_PLANAR><<<grid, 256, 0, s>>>(d, one, bytes, sum); break;
+    }
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }
@@ -645,15 +782,20 @@ extern "C" SKPS_API int skps_letterbox(const uint8_t* frame, int H, int W, int p
     return launch_letterbox(a, 1, (cudaStream_t)stream);
 }
 
-extern "C" SKPS_API int skps_letterbox_frames(const skps_det_src* src, int n, uint8_t* out, int in_h, int in_w,
-                                              void* stream) {
+extern "C" SKPS_API int skps_letterbox_frames_layout(const skps_det_src* src, const skps_frame_layout* lay, int n,
+                                                     uint8_t* out, int in_h, int in_w, void* stream) {
     SKPS_CHECK(n >= 0 && n <= 65535 && in_h > 0 && in_h <= 65535 && in_w > 0,
                "letterbox_frames: n %d outside 0..65535 or input %dx%d", n, in_h, in_w);
     if (n == 0) return 0;
     SKPS_CHECK(src && out, "letterbox_frames: bad arguments");
     LetterboxArgs a = {};
-    a.src = src; a.out = out; a.out_stride = (size_t)in_h * in_w * 3; a.in_h = in_h; a.in_w = in_w;
+    a.src = src; a.lay = lay; a.out = out; a.out_stride = (size_t)in_h * in_w * 3; a.in_h = in_h; a.in_w = in_w;
     return launch_letterbox(a, n, (cudaStream_t)stream);
+}
+
+extern "C" SKPS_API int skps_letterbox_frames(const skps_det_src* src, int n, uint8_t* out, int in_h, int in_w,
+                                              void* stream) {
+    return skps_letterbox_frames_layout(src, nullptr, n, out, in_h, in_w, stream);
 }
 
 extern "C" SKPS_API int skps_select_faces(const float* det_rows, const int32_t* det_count, int det_stride, const float* track,
@@ -705,15 +847,21 @@ extern "C" SKPS_API int skps_crop_resize(const uint8_t* frame, int H, int W, int
     return launch_crop(a, 1, (cudaStream_t)stream);
 }
 
-extern "C" SKPS_API int skps_crop_faces(const skps_face_src* src, const float* boxes4, int n, float face_scale, float min_face,
-                                        uint8_t* crops, int out_hw, int32_t* detail, void* stream) {
+extern "C" SKPS_API int skps_crop_faces_layout(const skps_face_src* src, const skps_frame_layout* lay, const float* boxes4,
+                                               int n, float face_scale, float min_face, uint8_t* crops, int out_hw,
+                                               int32_t* detail, void* stream) {
     SKPS_CHECK(n >= 0 && n <= 65535 && out_hw > 0, "crop_faces: n %d outside 0..65535 or out_hw %d", n, out_hw);
     if (n == 0) return 0;
     SKPS_CHECK(src && boxes4 && crops && detail, "crop_faces: bad arguments");
     dim3 grid((out_hw + 255) / 256, out_hw, n);
-    crop_faces_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src, boxes4, face_scale, min_face, crops, out_hw, detail);
+    crop_faces_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src, lay, boxes4, face_scale, min_face, crops, out_hw, detail);
     SKPS_CUDA(cudaGetLastError());
     return 0;
+}
+
+extern "C" SKPS_API int skps_crop_faces(const skps_face_src* src, const float* boxes4, int n, float face_scale, float min_face,
+                                        uint8_t* crops, int out_hw, int32_t* detail, void* stream) {
+    return skps_crop_faces_layout(src, nullptr, boxes4, n, face_scale, min_face, crops, out_hw, detail, stream);
 }
 
 extern "C" SKPS_API int skps_crop_rect(const uint8_t* frame, int H, int W, int pitch, int rx, int ry, int rw, int rh,
@@ -750,13 +898,20 @@ extern "C" SKPS_API int skps_frame_absdiff_sum(const uint8_t* a, const uint8_t* 
     return launch_frame_diff(nullptr, 1, D, n, sum, (cudaStream_t)stream);
 }
 
-extern "C" SKPS_API int skps_frame_ingest(const uint8_t* frame, int H, int W, int pitch, uint8_t* packed, const uint8_t* prev,
-                                          unsigned long long* sum, void* stream) {
-    SKPS_CHECK(frame && packed && sum && H > 0 && W > 0 && (H == 1 || pitch >= 3 * W), "ingest: bad arguments");
+extern "C" SKPS_API int skps_frame_ingest_layout(const uint8_t* frame, int H, int W, int pitch, int layout, int plane_pitch,
+                                                 uint8_t* packed, const uint8_t* prev, unsigned long long* sum, void* stream) {
+    SKPS_CHECK(layout_ok(layout), "ingest: unknown pixel layout %d", layout);
+    SKPS_CHECK(frame && packed && sum && H > 0 && W > 0 && (H == 1 || pitch >= layout_xstep(layout) * W) &&
+               (layout < SKPS_LAYOUT_BGR_PLANAR || plane_pitch >= 0), "ingest: bad arguments");
     SKPS_CHECK(((uintptr_t)packed % 16 == 0) && ((uintptr_t)prev % 16 == 0), "ingest: packed and prev must be 16-byte aligned");
     SKPS_CUDA(cudaMemsetAsync(sum, 0, sizeof(unsigned long long), (cudaStream_t)stream));
     MpStreamDesc D = {};
     D.cur = packed; D.prev = prev; D.have_prev = prev != nullptr; D.H = H; D.W = W;
-    D.src = frame; D.src_pitch = pitch;
-    return launch_frame_diff(nullptr, 1, D, (size_t)H * W * 3, sum, (cudaStream_t)stream);
+    D.src = frame; D.src_pitch = pitch; D.src_plane = plane_pitch;
+    return launch_frame_diff(nullptr, 1, D, (size_t)H * W * 3, sum, (cudaStream_t)stream, layout);
+}
+
+extern "C" SKPS_API int skps_frame_ingest(const uint8_t* frame, int H, int W, int pitch, uint8_t* packed, const uint8_t* prev,
+                                          unsigned long long* sum, void* stream) {
+    return skps_frame_ingest_layout(frame, H, W, pitch, SKPS_LAYOUT_BGR, 0, packed, prev, sum, stream);
 }

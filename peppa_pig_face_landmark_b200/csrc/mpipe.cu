@@ -254,10 +254,12 @@ static int check_stream_map(const skps_mpipe* p, const int32_t* streams, int n, 
 // detector frames, results) is in call order; everything per stream (ring, previous frame size, frame count, the device
 // state of temporal.cu) is indexed by the stream.  Host frames (pitches null) are uploaded on the copy stream into the
 // stream's next ring position; device frames (rows pitches[i] bytes apart) are gathered there by the frame-difference launch
-// on the compute stream, after the work queued on `producer`, whose later work waits for that launch.  out: results into
-// caller buffers on the device instead of the slot's pinned ones.
+// on the compute stream, after the work queued on `producer`, whose later work waits for that launch; they are in pixel
+// layout `layout` (planes plane_pitches[i] bytes apart for the planar layouts) and land in the ring as BGR.  out: results
+// into caller buffers on the device instead of the slot's pinned ones.
 static int submit_batch(skps_mpipe* p, int slot_i, const int32_t* streams, const uint8_t* const* frames, const int32_t* hw,
-                        int n, const int32_t* pitches, cudaStream_t producer, const skps_mpipe_outputs* out) {
+                        int n, const int32_t* pitches, cudaStream_t producer, const skps_mpipe_outputs* out,
+                        int layout = SKPS_LAYOUT_BGR, const int32_t* plane_pitches = nullptr) {
     const bool on_device = pitches != nullptr;
     SKPS_CHECK(p && frames && hw && (slot_i == 0 || slot_i == 1) && n > 0 && n <= p->S, "mpipe_submit: bad arguments");
     bool identity = true;
@@ -288,8 +290,10 @@ static int submit_batch(skps_mpipe* p, int slot_i, const int32_t* streams, const
         SKPS_CHECK(frames[i] && H > 0 && W > 0 && (size_t)H * W * 3 <= p->frame_bytes,
                    "mpipe_submit: frame %d is %dx%d, larger than the pipeline maximum %dx%d", i, H, W, c.max_h, c.max_w);
         if (on_device) {
-            SKPS_CHECK(H == 1 || pitches[i] >= 3 * W, "mpipe_submit: frame %d has row pitch %d, less than 3 x width %d", i,
-                       pitches[i], W);
+            SKPS_CHECK(H == 1 || pitches[i] >= layout_xstep(layout) * W,
+                       "mpipe_submit: frame %d has row pitch %d, less than %d x width %d", i, pitches[i], layout_xstep(layout), W);
+            SKPS_CHECK(layout < SKPS_LAYOUT_BGR_PLANAR || plane_pitches[i] >= 0, "mpipe_submit: frame %d has plane pitch %d",
+                       i, plane_pitches[i]);
         } else if (upload_host_frame(frames[i], (size_t)H * W * 3, sl.h_stage + p->frame_bytes * i,
                                      p->d_frame[(size_t)t * 3 + (p->ring_pos[t] + 1) % 3], sc)) {
             return 1;
@@ -332,6 +336,7 @@ static int submit_batch(skps_mpipe* p, int slot_i, const int32_t* streams, const
         D.H = H; D.W = W;
         D.src = on_device ? frames[i] : nullptr;
         D.src_pitch = on_device ? pitches[i] : W * 3;
+        D.src_plane = on_device && layout >= SKPS_LAYOUT_BGR_PLANAR ? plane_pitches[i] : 0;
         letterbox_geometry(H, W, p->det_h, p->det_w, &D.scale, &D.rw, &D.rh, &D.top, &D.left);
         memcpy(&sl.h_geom[8 * i], &D.scale, 4); sl.h_geom[8 * i + 1] = D.top; sl.h_geom[8 * i + 2] = D.left;
         if ((size_t)H * W * 3 > max_bytes) max_bytes = (size_t)H * W * 3;
@@ -356,7 +361,8 @@ static int submit_batch(skps_mpipe* p, int slot_i, const int32_t* streams, const
     }
     SKPS_CUDA(cudaMemcpyAsync(p->d_desc, sl.h_desc, sizeof(MpStreamDesc) * n_desc, cudaMemcpyHostToDevice, sx));
     SKPS_CUDA(cudaEventRecord(sl.ev_staged, sx));
-    if (launch_frame_diff(p->d_desc, n, MpStreamDesc{}, max_bytes, p->d_diff, sx)) return 1;
+    if (launch_frame_diff(p->d_desc, n, MpStreamDesc{}, max_bytes, p->d_diff, sx, on_device ? layout : SKPS_LAYOUT_BGR))
+        return 1;
     if (on_device) {
         SKPS_CUDA(cudaEventRecord(p->ev_read, sx));
         SKPS_CUDA(cudaStreamWaitEvent(producer, p->ev_read, 0));
@@ -479,16 +485,26 @@ extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8
     return skps_mpipe_submit_streams(p, slot_i, nullptr, frames, hw, n);
 }
 
-extern "C" SKPS_API int skps_mpipe_submit_device_streams(skps_mpipe* p, int slot_i, const int32_t* streams,
-                                                         const uint8_t* const* frames, const int32_t* pitches, const int32_t* hw,
-                                                         int n, const skps_mpipe_outputs* out, void* producer_stream) {
+extern "C" SKPS_API int skps_mpipe_submit_device_layout(skps_mpipe* p, int slot_i, const int32_t* streams,
+                                                        const uint8_t* const* frames, const int32_t* pitches, const int32_t* hw,
+                                                        int n, int layout, const int32_t* plane_pitches,
+                                                        const skps_mpipe_outputs* out, void* producer_stream) {
     SKPS_CHECK(p && frames && pitches && hw && n > 0 && n <= p->S, "mpipe_submit_device: bad arguments");
+    SKPS_CHECK(layout_ok(layout), "mpipe_submit_device: unknown pixel layout %d", layout);
+    SKPS_CHECK(layout < SKPS_LAYOUT_BGR_PLANAR || plane_pitches, "mpipe_submit_device: a planar layout needs plane pitches");
     bool identity = true;
     if (check_stream_map(p, streams, n, &identity)) return 1;
     SKPS_ON_DEVICE(p->device);
     for (int i = 0; i < n; ++i)
         if (check_device_frame(frames[i], p->device, "mpipe_submit_device", i)) return 1;
-    return submit_batch(p, slot_i, streams, frames, hw, n, pitches, (cudaStream_t)producer_stream, out);
+    return submit_batch(p, slot_i, streams, frames, hw, n, pitches, (cudaStream_t)producer_stream, out, layout, plane_pitches);
+}
+
+extern "C" SKPS_API int skps_mpipe_submit_device_streams(skps_mpipe* p, int slot_i, const int32_t* streams,
+                                                         const uint8_t* const* frames, const int32_t* pitches, const int32_t* hw,
+                                                         int n, const skps_mpipe_outputs* out, void* producer_stream) {
+    return skps_mpipe_submit_device_layout(p, slot_i, streams, frames, pitches, hw, n, SKPS_LAYOUT_BGR, nullptr, out,
+                                           producer_stream);
 }
 
 extern "C" SKPS_API int skps_mpipe_submit_device(skps_mpipe* p, int slot_i, const uint8_t* const* frames, const int32_t* pitches,

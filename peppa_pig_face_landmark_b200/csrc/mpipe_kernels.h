@@ -5,9 +5,29 @@
 
 struct skps_pipeline_cfg;
 struct skps_det_src;
+struct skps_frame_layout;
 struct skps_engine;
 
 namespace skps {
+
+// Where the pixels of a frame in layout SKPS_LAYOUT_* (skps_b200.h) are: pixel (y, x) has its B, G, R bytes at
+// base + y * pitch + x * xs + off[0..2].  `plane` is the plane pitch of the planar layouts.  layout_ok: a known code.
+struct PxLayout {
+    int xs;
+    long long off[3];
+};
+__host__ __device__ __forceinline__ bool layout_ok(int layout) { return layout >= 0 && layout <= 5; }
+__host__ __device__ __forceinline__ int layout_xstep(int layout) { return layout >= 4 ? 1 : (layout >= 2 ? 4 : 3); }
+__host__ __device__ __forceinline__ PxLayout px_layout(int layout, int plane) {
+    PxLayout l;
+    l.xs = layout_xstep(layout);
+    const long long step = layout >= 4 ? (long long)plane : 1;       // channel c is c steps from the first in memory
+    const bool rgb = layout & 1;
+    l.off[0] = rgb ? 2 * step : 0;
+    l.off[1] = step;
+    l.off[2] = rgb ? 0 : 2 * step;
+    return l;
+}
 
 // Block g of a launch over n calls' frames serves stream stream[g] (stream null: g).  The per-frame inputs and outputs are
 // in call order, rows g < n; the state is indexed by the stream, rows [S].
@@ -56,7 +76,8 @@ struct MpStreamDesc {
     float scale;                 // letterbox geometry (face_detector.py:49-62)
     int rw, rh, top, left;
     const uint8_t* src;          // the caller's device frame, gathered into cur by launch_frame_diff, or null (cur holds it)
-    int src_pitch;               // bytes from one row of src to the next, >= 3 W, any alignment
+    int src_pitch;               // bytes from one row of src to the next, >= xstep W, any alignment
+    int src_plane;               // bytes from one plane of src to the next (planar layouts)
 };
 
 // Image ops (image_ops.cu): one kernel per op, launched by skps_pipeline (FaceAna), skps_mpipe (FaceAnaStreams) and the
@@ -70,7 +91,8 @@ struct LetterboxArgs {
     const uint8_t* frame; int H, W, pitch;      // the one frame (desc and src null) ...
     int rw, rh, top, left;                      // ... and its letterbox geometry
     const MpStreamDesc* desc;                   // or frame g's: desc[g], geometry included
-    const skps_det_src* src;                    // or frame g's: src[g] (skps_letterbox_frames), whole or in row pairs
+    const skps_det_src* src;                    // or frame g's: src[g] (skps_letterbox_frames), whole or in row pairs,
+    const skps_frame_layout* lay;               // with src: its pixel layout lay[g] [dev], or null (BGR)
     uint8_t* out; size_t out_stride;
     int in_h, in_w;
 };
@@ -114,10 +136,11 @@ int launch_select(const SelectArgs& a, int n, cudaStream_t s);
 int launch_landmark_post(const float* xy, const int* detail, const int* count, int K, int P, float* kps, int n, cudaStream_t s);
 
 // The frame-difference gate (facer.py:111-113): sum[g] += sum |cur - prev| over frame g's bytes when have_prev.  A frame
-// with src set is first gathered into cur in the same pass (the same integer sum as from a packed cur).  Frame g is d[g]
-// [dev], or (d null, n = 1) `one` of `bytes` bytes, any count when one.src is null; with d, bytes is the largest frame's.
+// with src set is first gathered into cur in the same pass (the same integer sum as from a packed cur); its pixels are in
+// `layout` (SKPS_LAYOUT_*, one for the launch; cur gets them as BGR).  Frame g is d[g] [dev], or (d null, n = 1) `one` of
+// `bytes` bytes, any count when one.src is null; with d, bytes is the largest frame's packed size.
 int launch_frame_diff(const MpStreamDesc* d, int n, const MpStreamDesc& one, size_t bytes, unsigned long long* sum,
-                      cudaStream_t s);
+                      cudaStream_t s, int layout = 0);
 
 // Frame staging on the host side, shared by skps_pipeline and skps_mpipe.  upload_host_frame queues the H2D copy of a [host]
 // frame of `bytes` bytes into dst on s: a pinned frame is copied as it is, a pageable one first into `stage` (pinned, at
