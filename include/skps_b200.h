@@ -597,6 +597,25 @@ SKPS_API int skps_warp_faces(const skps_face_src* src, const double* M, int n, i
  * every image is BGR (skps_warp_faces).  The chips are BGR, the bytes of the same pixels as an interleaved BGR image. */
 SKPS_API int skps_warp_faces_layout(const skps_face_src* src, const skps_frame_layout* lay, const double* M, int n, int out_h,
                                     int out_w, uint8_t* out, void* stream);
+/* skps_warp_faces_layout for the kept faces of n_frames frames, with the face counts known only on the device:
+ * n_frames * per_frame slots (per_frame 1..65535) are launched, and slot j of frame i, chip i*per_frame + j of
+ * out [dev] (n_frames*per_frame,out_h,out_w,3) uint8, is warped with M [dev] + (i*per_frame + j)*6 only when
+ * j < count[i] [dev] (n_frames) int32; the other chips are left as they were.  One source per frame: src[i] [dev] and,
+ * unless NULL, lay[i] [dev] (n_frames) describe frame i for all its slots (the whole frame at any pitch and layout).
+ * Asynchronous on `stream`; allocates nothing. */
+SKPS_API int skps_warp_faces_count(const skps_face_src* src, const skps_frame_layout* lay, const int32_t* count,
+                                   int n_frames, int per_frame, const double* M, int out_h, int out_w, uint8_t* out,
+                                   void* stream);
+/* The estimate for the detector's own five landmarks (yolov5-face columns 5..14: eyes, nose tip, mouth corners, the
+ * template's order).  rows [dev] (n_frames,det_cap,16), count [dev] (n_frames) and recover [dev] (n_frames,3) float32 are
+ * skps_detect_post_batch's kept_rows, count and recover with capacity det_cap.  For slot j < min(count[i], max_chips)
+ * of frame i, points [dev] + (i*max_chips + j)*10 (5,2) float32 gets the five points in frame pixels, ((x - pad_x) /
+ * scale, (y - pad_y) / scale) in float32 as scale_coords maps columns 0..3, and M [dev] + (i*max_chips + j)*6 (2,3)
+ * float64 the similarity from those points promoted to float64 to the template scaled by size/112, the estimator of
+ * skps_align_faces bit for bit.  Other slots are left as they were.  max_chips 1..det_cap, size 16..512.  One thread
+ * per slot; asynchronous on `stream`; allocates nothing. */
+SKPS_API int skps_det_align_estimate(const float* rows, const int32_t* count, int det_cap, const float* recover,
+                                     int n_frames, int max_chips, int size, float* points, double* M, void* stream);
 /* The estimate of skps_align_faces for n faces (any n >= 0) from float32 landmarks kps [dev] (n,P,2), P >= 98, each promoted
  * to float64: M [dev] (n,2,3) float64, bit for bit what skps_align_faces gives for kps.astype(float64) (and so what
  * FaceAna(align=size) returns for its float32 'kps').  size 16..512.  Asynchronous on `stream`; allocates nothing. */

@@ -11,6 +11,9 @@ Additive: the detector over many frames per call (SURVEY.md 8b):
     # overlapped, results left on the GPU (CUDA frames):
     bufs = [fd.new_results(n), fd.new_results(n)]
     fd.submit(frames_0, out=bufs[0]); fd.submit(frames_1, out=bufs[1]); r0 = fd.collect(); ...
+    # ArcFace chips from the detector's own five landmarks, for a recognition model without the landmark net:
+    fd = FaceDetector(align=112)
+    res = fd.run_batch(frames)             # [(rows, points (k_i,5,2), chips (k_i,112,112,3) uint8, M (k_i,2,3)) per frame]
 """
 import os
 import pathlib
@@ -21,9 +24,11 @@ import numpy as np
 from ... import runtime as rt
 from ...graph_tools import detector_onnx_for
 from ...logger.logger import logger
+from .align import check_size
 from .device_frames import FRAME_LAYOUT, check_host_frame
+from .face_landmark import FACE_SRC, HostChips
 from .onnx_model_base import ONNXEngine
-from .staging import Staging, check_frames, check_out, new_buffers, pad16
+from .staging import Staging, check_frames, check_out, grow, new_buffers, pad16
 
 # skps_det_src of include/skps_b200.h
 DET_SRC = np.dtype([("base", "<u8"), ("pitch", "<i4"), ("H", "<i4"), ("W", "<i4"), ("rw", "<i4"), ("rh", "<i4"),
@@ -62,16 +67,57 @@ def host_upload_rows(H, rh):
     return letterbox_rows(H, rh) if 2 * rh < H else None
 
 
-def result_fields(n_frames, rows):
-    """{name: (shape, dtype name)} of new_results(n_frames) of a detector with `rows` rows."""
-    return {"rows": ((n_frames, rows, 16), "float32"), "idx": ((n_frames, rows), "int32"),
-            "count": ((n_frames,), "int32")}
+MAX_CHIPS = 1024            # largest max_chips
+
+
+def check_max_chips(max_chips):
+    """Chips per frame: an int in 1..MAX_CHIPS (ValueError otherwise)."""
+    if isinstance(max_chips, (bool, np.bool_)) or not isinstance(max_chips, (int, np.integer)) \
+            or not 1 <= max_chips <= MAX_CHIPS:
+        raise ValueError("max_chips must be an int in 1..%d, got %r" % (MAX_CHIPS, max_chips))
+    return int(max_chips)
+
+
+def landmark_points(rows, recover):
+    """(k, 5, 2) float32: the five landmarks of kept rows (k, 16) float32 (columns 5..14, letterbox coordinates) in frame
+    pixels, with the letterbox's recover = [scale, left, top]: what scale_coords (face_detector.py:82-93) does to columns
+    0..3, in the same float32 arithmetic, so that the points and the box share one frame.  The host restatement of
+    skps_det_align_estimate's points."""
+    scale, left, top = recover
+    p = np.array(rows, np.float32).reshape(-1, 16)[:, 5:15].reshape(-1, 5, 2)
+    p[:, :, 0] -= np.float32(left)
+    p[:, :, 1] -= np.float32(top)
+    p /= np.float32(scale)
+    return p
+
+
+def result_fields(n_frames, rows, align=None, max_chips=None):
+    """{name: (shape, dtype name)} of new_results(n_frames) of FaceDetector(align=align, max_chips=max_chips) with `rows`
+    rows."""
+    f = {"rows": ((n_frames, rows, 16), "float32"), "idx": ((n_frames, rows), "int32"),
+         "count": ((n_frames,), "int32")}
+    if align is not None:
+        f.update({"points": ((n_frames, max_chips, 5, 2), "float32"), "M": ((n_frames, max_chips, 2, 3), "float64"),
+                  "chip": ((n_frames, max_chips, align, align, 3), "uint8")})
+    return f
+
+
+def align_results(rows, count, points, chips, M, max_chips):
+    """collect()'s list with align: (rows[i], points[i, :k], chips of frame i, M[i, :k]) per frame i, as copies, with
+    k = min(count[i], max_chips).  points (n, max_chips, 5, 2) and M (n, max_chips, 2, 3) hold a slot per chip; chips
+    (>= sum k, s, s, 3) holds them packed in frame order."""
+    res, o = [], 0
+    for i, c in enumerate(count):
+        k = min(int(c), max_chips)
+        res.append((rows[i], points[i, :k].copy(), chips[o:o + k].copy(), M[i, :k].copy()))
+        o += k
+    return res
 
 
 class FaceDetector:
     MAX_DET = 256           # kept rows per frame copied back with the counts (the rest only for frames that keep more)
 
-    def __init__(self, cfg=None, max_frames=16, device="cuda"):
+    def __init__(self, cfg=None, max_frames=16, device="cuda", align=None, max_chips=64):
         """cfg: Skps.yml's Detect section (None: read it from Skps.yml).  The engine is built for cfg['input_shape']
         ([h, w, 3]): from the export itself when that is its input size, else from the export retargeted to (h, w)
         (graph_tools.detector_onnx_for; h and w multiples of 32 in 128..2176 x 128..3840), so the letterbox and the
@@ -82,7 +128,20 @@ class FaceDetector:
         384x640 and 0.35 GB at 1152x1920, plus an NMS workspace of skps_detect_post_workspace_size(rows, max_frames)
         bytes (rows = 15120 at 384x640).  Each of the two call slots keeps, per frame of its largest call, every
         detector row as a possible kept box (rows x 68 bytes, about 1 MB at 384x640) and, for host frames, the pinned
-        staging of the rows it uploads."""
+        staging of the rows it uploads.
+
+        align: None, or a chip side in 16..512: run_batch / collect then return, per frame, (rows, points, chips, M)
+        for the first min(count, max_chips) kept rows, in NMS order (score descending): points (k, 5, 2) float32, the
+        row's five landmarks (eyes, nose tip, mouth corners) mapped back to the frame the way scale_coords maps the box
+        (landmark_points; the rows themselves keep them in letterbox coordinates, as the reference does); M (k, 2, 3)
+        float64, the similarity from the points promoted to float64 to the ArcFace template scaled by align/112, the
+        estimator of core/api/align.py:align_faces; chips (k, align, align, 3) uint8 BGR, cv2.warpAffine(frame, M,
+        (align, align)) byte for byte.  max_chips: chips per frame, an int in 1..1024.  Each call slot then keeps
+        max_chips x align^2 x 3 bytes of chips on the device per frame of its largest call with CUDA frames (38.5 MB
+        for a call of 16 frames at the default max_chips and align 112), and the points and matrices (88 bytes per chip
+        slot) on the device and pinned.  A bad align or max_chips raises ValueError before anything is allocated."""
+        self.align = None if align is None else check_size(align)
+        self.max_chips = check_max_chips(max_chips)
         if cfg is None:
             from .facer import get_cfg
             cfg = get_cfg()['Skps']['Detect']
@@ -104,8 +163,9 @@ class FaceDetector:
         self._ws = torch.empty((self._ws_bytes,), dtype=torch.uint8, device=self.device)
         self.last_keep_idx = None
         self._slots = None            # staging and results of the two call slots, made on first use
-        self._pending = []            # [(slot, frames, out or None)]
+        self._pending = []            # [(slot, frames, out or None, checked host frames to align or None)]
         self._next = 0
+        self.host_chips = None if self.align is None else HostChips(self.device, self.align)
 
     # ------------------------------------------------------------------ reference contract
     def preprocess(self, image, color=(114, 114, 114)):
@@ -127,6 +187,8 @@ class FaceDetector:
     def __call__(self, image):
         t0 = time.time()
         bboxes, = self.run_batch([image])
+        if self.align is not None:
+            bboxes = bboxes[0]
         self.last_keep_idx = self.last_keep_idx[0]
         logger.info('detect done, time consume: %.5f' % (time.time() - t0))
         return bboxes
@@ -135,7 +197,8 @@ class FaceDetector:
     def run_batch(self, frames, layout="bgr"):
         """The detector over many frames (blocking): the i-th (k_i, 16) float32 array of the returned list is bit for bit
         what FaceDetector(cfg)(frames[i]) returns; last_keep_idx is then the list of the frames' kept row indices (int64).
-        See submit() for what frames and layout may be."""
+        With align, the i-th entry is (rows, points, chips, M) (see __init__).  See submit() for what frames and layout
+        may be."""
         if self._pending:
             raise RuntimeError("FaceDetector: %d calls in flight; collect() them first" % len(self._pending))
         self.submit(frames, layout=layout)
@@ -144,9 +207,15 @@ class FaceDetector:
     def new_results(self, n_frames):
         """Device result buffers for submit(cuda_frames, out=...) of up to n_frames frames: a dict of CUDA tensors on
         this object's device, rows (n, R, 16) float32, idx (n, R) int32 and count (n,) int32, where R is the detector's
-        row count (15120 at 384x640): frame i keeps rows[i, :count[i]], the detector rows idx[i, :count[i]]."""
+        row count (15120 at 384x640): frame i keeps rows[i, :count[i]], the detector rows idx[i, :count[i]].  With
+        align, also points (n, max_chips, 5, 2) float32, M (n, max_chips, 2, 3) float64 and chip
+        (n, max_chips, align, align, 3) uint8: slot j < min(count[i], max_chips) of frame i holds row j's; the other
+        slots are unspecified."""
         rt.require_cuda()
-        return new_buffers(result_fields(int(n_frames), self._rows), self.device)
+        return new_buffers(self._fields(int(n_frames)), self.device)
+
+    def _fields(self, n_frames):
+        return result_fields(n_frames, self._rows, self.align, self.max_chips)
 
     def submit(self, frames, out=None, layout="bgr"):
         """Enqueue the detector on frames; at most two calls may be in flight and collect() returns them in submission
@@ -163,8 +232,13 @@ class FaceDetector:
         Ordering on torch.cuda.current_stream(): CUDA frames are read after the work already queued on it, and work
         queued on it after submit() returns runs after they have been read.
         out: None (collect() returns numpy arrays), or, with CUDA frames, a dict from new_results(n) with n >= the call's
-        frames, not used by a call still in flight: the kept rows, their indices and counts are written there on the
-        GPU."""
+        frames, not used by a call still in flight: the kept rows, their indices and counts (with align, the points,
+        matrices and chips) are written there on the GPU.
+
+        With align, CUDA frames are warped into chips on the GPU right after the NMS, with no host synchronisation, and
+        are read until then.  Host frames are warped at collect(): the points and M come back with the rows, and only
+        the rectangle of the frame each chip reads (core/api/align.py:chip_read_rects) is uploaded and warped.  That is
+        one more upload per call, and the host frames must stay unchanged until collect() returns."""
         if len(self._pending) == 2:
             raise RuntimeError("FaceDetector: two calls already in flight; call collect() first")
         call = check_frames(frames, self.device, layout)
@@ -173,19 +247,20 @@ class FaceDetector:
         if out is not None:
             if not call.cuda:
                 raise ValueError("out= keeps results on the GPU and takes CUDA frames")
-            check_out(out, result_fields(n, self._rows), self.device, [p[2] for p in self._pending])
+            check_out(out, self._fields(n), self.device, [p[2] for p in self._pending])
         slot = self._next
         self._enqueue(call, geo, out, detect=True)
-        self._pending.append((slot, n, out))
+        self._pending.append((slot, n, out, call if self.align is not None and not call.cuda else None))
 
     def collect(self):
         """Results of the oldest call in flight: a list with one (k_i, 16) float32 numpy array per frame, and
-        last_keep_idx the list of their kept row indices; for a call submitted with out=, the out dict, with no host
-        synchronisation: torch.cuda.current_stream() is made to wait for the call, so work queued on it afterwards sees
-        the results."""
+        last_keep_idx the list of their kept row indices; with align, one (rows, points, chips, M) tuple per frame.  For
+        a call submitted with out=, the out dict, with no host synchronisation: torch.cuda.current_stream() is made to
+        wait for the call, so work queued on it afterwards sees the results.  A call of host frames with align is warped
+        here (see submit())."""
         if not self._pending:
             raise RuntimeError("FaceDetector: nothing submitted")
-        slot, n, out = self._pending.pop(0)
+        slot, n, out, host_call = self._pending.pop(0)
         st = self._slots[slot]
         if out is not None:
             import torch
@@ -205,7 +280,36 @@ class FaceDetector:
                 res.append(st["rows"][i, :k].cpu().numpy())
                 keep.append(st["idx"][i, :k].cpu().numpy().astype(np.int64))
         self.last_keep_idx = keep
-        return res
+        if self.align is None:
+            return res
+        chips = self._chips(st, host_call, count.tolist())
+        return align_results(res, count, st["hpoints"].numpy(), chips, st["hM"].numpy(), self.max_chips)
+
+    def _chips(self, st, host_call, count):
+        """The chips of a collected call without out=, packed in frame order, min(count[i], max_chips) for frame i: a
+        pinned (n, align, align, 3) uint8 array.  CUDA frames were warped into the slot's chips at submit(); host frames
+        are warped here."""
+        torch = rt.require_cuda()
+        A, ks = self.align, [min(k, self.max_chips) for k in count]
+        F = sum(ks)
+        make = lambda k: torch.empty((k, A, A, 3), dtype=torch.uint8)
+        st["hchip"] = grow(st["hchip"], F, lambda k: make(k).pin_memory())
+        if host_call is not None:
+            if F:
+                st["dchip"] = grow(st["dchip"], F, lambda k: make(k).to(self.device))
+                hM = st["hM"].numpy()
+                M = np.concatenate([hM[i, :k] for i, k in enumerate(ks)])
+                self.host_chips.warp(self.lib, self.model.stream, host_call, ks, M, st["dchip"], st["hchip"])
+        else:
+            cs = st["stage"].copy                     # idle until this slot's next call: the call is done
+            with torch.cuda.stream(cs):
+                o = 0
+                for i, k in enumerate(ks):
+                    if k:
+                        st["hchip"][o:o + k].copy_(st["chip"][i, :k], non_blocking=True)
+                    o += k
+            cs.synchronize()
+        return st["hchip"].numpy()
 
     # ------------------------------------------------------------------
     def _layout(self, call):
@@ -228,6 +332,9 @@ class FaceDetector:
         torch = rt.require_cuda()
         frames, cuda = call.frames, call.cuda
         n, R, M = len(frames), self._rows, min(self.MAX_DET, self._rows)
+        A, C = self.align, self.max_chips
+        align = detect and A is not None
+        warp_now = align and cuda                     # CUDA frames are warped here, host frames at collect()
         if self._slots is None:
             self._slots = [self._new_slot() for _ in range(2)]
         slot = self._next
@@ -236,7 +343,8 @@ class FaceDetector:
         lay = cuda and n > 0 and call.shapes[0].code != 0
         rec_off = pad16(n * DET_SRC.itemsize)
         lay_off = rec_off + pad16(n * 12)
-        frame_off = lay_off + (pad16(n * FRAME_LAYOUT.itemsize) if lay else 0)
+        face_off = lay_off + (pad16(n * FRAME_LAYOUT.itemsize) if lay else 0)
+        frame_off = face_off + (pad16(n * FACE_SRC.itemsize) if warp_now else 0)
         sizes = [0 if cuda else pad16((H if rows is None else len(rows)) * pitch) for H, W, pitch, geo, rows in layout]
         total = frame_off + sum(sizes)
         own = detect and out is None                  # results go to the slot's buffers and come back to the host
@@ -244,16 +352,30 @@ class FaceDetector:
         if own and st["capacity"] < max(n, 1):
             st["done"].synchronize()                  # the slot's last call has finished with what is replaced
             st["capacity"] = k = max(n, 2 * st["capacity"], 1)
-            st.update(new_buffers(result_fields(k, R), self.device))
-            # the first M kept rows of every frame come back with the counts
-            st.update({"h" + name: t.pin_memory() for name, t in new_buffers(result_fields(k, M), "cpu").items()})
-        # host staging = [n frame descriptors | n (scale, left, top) | n layouts | the host frames' rows], sent with one copy
+            fields = result_fields(k, R, A, C)
+            fields.pop("chip", None)                  # warped at submit() for CUDA frames only: below
+            st.update(new_buffers(fields, self.device))
+            # the first M kept rows of every frame come back with the counts, and with align the points and matrices
+            fields = result_fields(k, M, A, C)
+            fields.pop("chip", None)
+            st.update({"h" + name: t.pin_memory() for name, t in new_buffers(fields, "cpu").items()})
+        if own and warp_now and (st["chip"] is None or st["chip"].shape[0] < n):
+            st["done"].synchronize()
+            st["chip"] = grow(st["chip"], n, lambda k: torch.empty((k, C, A, A, 3), dtype=torch.uint8, device=self.device))
+        # host staging = [n frame descriptors | n (scale, left, top) | n layouts | n face sources | the host frames' rows],
+        # sent with one copy
         desc = host[:n * DET_SRC.itemsize].view(DET_SRC)
         rec = host[rec_off:rec_off + 12 * n].view(np.float32).reshape(n, 3)
         if lay:
             fl = host[lay_off:lay_off + n * FRAME_LAYOUT.itemsize].view(FRAME_LAYOUT)
             fl["layout"] = [f.code for f in call.shapes]
             fl["plane_pitch"] = [f.plane for f in call.shapes]
+        if warp_now:                                  # the chips' sources: the whole frames
+            fs = host[face_off:face_off + n * FACE_SRC.itemsize].view(FACE_SRC)
+            H, W, pitch = np.array([f[:3] for f in call.shapes], np.int64).reshape(-1, 3).T
+            fs["base"] = [f.data_ptr() for f in frames]
+            fs["pitch"], fs["H"], fs["W"], fs["rw"], fs["rh"] = pitch, H, W, W, H
+            fs["ox"], fs["oy"], fs["_pad"] = 0, 0, 0
         at = frame_off
         for i, (f, (H, W, pitch, (scale, rw, rh, top, left), rows), nb) in enumerate(zip(frames, layout, sizes)):
             rec[i] = (scale, left, top)
@@ -286,7 +408,7 @@ class FaceDetector:
                 rt.check(self.lib.skps_letterbox_frames_layout(dev + DET_SRC.itemsize * c0,
                                                                dev + lay_off + FRAME_LAYOUT.itemsize * c0 if lay else None,
                                                                m, inp, in_h, in_w, s.cuda_stream))
-            if c0 + K >= n:
+            if c0 + K >= n and not warp_now:
                 st["read"].record(s)
             if not detect:
                 continue
@@ -296,7 +418,16 @@ class FaceDetector:
                                                          dev + rec_off + 12 * c0, rows_t.data_ptr() + 64 * R * c0,
                                                          idx_t.data_ptr() + 4 * R * c0, count_t.data_ptr() + 4 * c0, R,
                                                          self._ws.data_ptr(), self._ws_bytes, s.cuda_stream))
-        if n == 0:
+        if align and n:
+            points, mats = res["points"], res["M"]
+            with torch.cuda.device(self.device):
+                rt.check(self.lib.skps_det_align_estimate(rows_t.data_ptr(), count_t.data_ptr(), R, dev + rec_off, n, C, A,
+                                                          points.data_ptr(), mats.data_ptr(), s.cuda_stream))
+                if warp_now:
+                    rt.check(self.lib.skps_warp_faces_count(dev + face_off, dev + lay_off if lay else None,
+                                                            count_t.data_ptr(), n, C, mats.data_ptr(), A, A,
+                                                            res["chip"].data_ptr(), s.cuda_stream))
+        if n == 0 or warp_now:
             st["read"].record(s)
         torch.cuda.current_stream(self.device).wait_event(st["read"])
         if own and n:
@@ -304,11 +435,14 @@ class FaceDetector:
                 st["hrows"][:n].copy_(rows_t[:n, :M], non_blocking=True)
                 st["hidx"][:n].copy_(idx_t[:n, :M], non_blocking=True)
                 st["hcount"][:n].copy_(count_t[:n], non_blocking=True)
+                if align:
+                    st["hpoints"][:n].copy_(res["points"][:n], non_blocking=True)
+                    st["hM"][:n].copy_(res["M"][:n], non_blocking=True)
         st["done"].record(s)
         self._next ^= 1
         return st
 
     def _new_slot(self):
         import torch
-        return dict(stage=Staging(self.device), capacity=0, rows=None, idx=None, count=None, read=torch.cuda.Event(),
-                    done=torch.cuda.Event())
+        return dict(stage=Staging(self.device), capacity=0, rows=None, idx=None, count=None, chip=None, hchip=None,
+                    dchip=None, read=torch.cuda.Event(), done=torch.cuda.Event())

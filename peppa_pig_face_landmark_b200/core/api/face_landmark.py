@@ -104,6 +104,43 @@ def _gather_rects(frames, rects, image, host, at, dev):
             frames[image[j]][y0:y1, x0:x1].reshape(y1 - y0, 3 * (x1 - x0))
 
 
+class HostChips:
+    """The chip stage of host frames, which FaceLandmark, FaceAnaImages and FaceDetector with align run at collect(): of
+    each frame only the rectangle each chip reads (core/api/align.py:chip_read_rects) crosses PCIe, through a pinned
+    staging on a copy stream, and is warped with skps_warp_faces."""
+
+    def __init__(self, device, size):
+        self.device, self.size = device, size
+        self._stage = None            # (Staging, done event), made on first use
+
+    def warp(self, lib, stream, call, counts, M, chips, h_chips):
+        """(blocking) counts[i] faces of call.frames[i] (a call checked by check_frames), whose matrices M (n, 2, 3)
+        float64 are on the host.  Uploads the matrices and the rectangles, warps chips[:n] (a device (>= n, size, size, 3)
+        uint8 tensor) on `stream`, where no other kernel runs beside it, and copies them to the pinned h_chips[:n]."""
+        torch = rt.require_cuda()
+        n, A = len(M), self.size
+        rects = np.concatenate([chip_read_rects(M[o:o + k], A, f.H, f.W) for o, k, f
+                                in zip(np.cumsum([0] + list(counts[:-1])), counts, call.shapes)])
+        m_off = pad16(n * FACE_SRC.itemsize)
+        roi_off = m_off + 48 * n
+        total = roi_off + int(_rect_bytes(rects).sum())
+        if self._stage is None:
+            self._stage = (Staging(self.device), torch.cuda.Event())
+        cs, done = self._stage
+        host, dev = cs.reserve(total, done)
+        # host staging = [n face descriptors | n matrices | the frames' rectangles], sent with one copy
+        host[m_off:roi_off].view(np.float64)[:] = np.asarray(M, np.float64).reshape(-1)
+        _gather_rects(call.frames, rects, np.repeat(np.arange(len(counts)), counts), host, roi_off, dev)
+        cs.send(total, done)
+        stream.wait_event(cs.copied)
+        with torch.cuda.device(self.device):
+            rt.check(lib.skps_warp_faces(dev, dev + m_off, n, A, A, chips.data_ptr(), stream.cuda_stream))
+        with torch.cuda.stream(stream):
+            h_chips[:n].copy_(chips[:n], non_blocking=True)
+        done.record(stream)
+        done.synchronize()                            # the staging is free again and h_chips holds the chips
+
+
 class FaceLandmark:
     def __init__(self, cfg=None, max_faces=16, device="cuda", align=None):
         """cfg: Skps.yml's Keypoints section (None: read it from Skps.yml).  max_faces: faces per network forward; the
@@ -141,7 +178,7 @@ class FaceLandmark:
         self._slots = None            # staging of the batched path, made on first use
         self._pending = []            # [(slot, faces per frame, out or None, checked host frames to align or None)]
         self._next = 0
-        self._chip_stage = None       # (Staging, done event) of the host frames' chip rectangles, made on first use
+        self.host_chips = None if self.align is None else HostChips(self.device, self.align)
 
     def crops(self, img, bboxes):
         """The (K,S,S,3) uint8 crops the network sees (face_landmark.py:66-104), for parity tests."""
@@ -368,7 +405,8 @@ class FaceLandmark:
             st["done"].synchronize()
             n = sum(counts)
             if host_call is not None and n:
-                self._warp_host_frames(host_call, counts, st["hM"].numpy()[:n], st["M"], st["chip"], st["hchip"])
+                self.host_chips.warp(self.lib, self.model.stream, host_call, counts, st["hM"].numpy()[:n], st["chip"],
+                                     st["hchip"])
             arrays = [st["h" + k].numpy() for k in names]
         res, o = [], 0
         for k in counts:
@@ -378,32 +416,6 @@ class FaceLandmark:
                 res.append(tuple(a[o:o + k] for a in arrays))
             o += k
         return res
-
-    def _warp_host_frames(self, call, counts, M, d_M, chips, h_chips):
-        """The chip phase of host frames (blocking): counts[i] faces of call.frames[i] (a call checked by check_frames),
-        whose matrices M (n, 2, 3) float64 are on the host and, equal, in d_M on the device.  Uploads the rectangle of
-        each frame that each chip reads (chip_read_rects) through the chip stage's pinned staging, warps chips[:n] on the
-        engine's stream, where no other kernel runs beside it, and copies them to the pinned h_chips[:n]."""
-        torch = rt.require_cuda()
-        n, A = len(M), self.align
-        rects = np.concatenate([chip_read_rects(M[o:o + k], A, f.H, f.W) for o, k, f
-                                in zip(np.cumsum([0] + list(counts[:-1])), counts, call.shapes)])
-        roi_off = pad16(n * FACE_SRC.itemsize)
-        total = roi_off + int(_rect_bytes(rects).sum())
-        if self._chip_stage is None:
-            self._chip_stage = (Staging(self.device), torch.cuda.Event())
-        cs, done = self._chip_stage
-        host, dev = cs.reserve(total, done)
-        _gather_rects(call.frames, rects, np.repeat(np.arange(len(counts)), counts), host, roi_off, dev)
-        s = self.model.stream
-        cs.send(total, done)
-        s.wait_event(cs.copied)
-        with torch.cuda.device(self.device):
-            rt.check(self.lib.skps_warp_faces(dev, d_M.data_ptr(), n, A, A, chips.data_ptr(), s.cuda_stream))
-        with torch.cuda.stream(s):
-            h_chips[:n].copy_(chips[:n], non_blocking=True)
-        done.record(s)
-        done.synchronize()                            # the staging is free again and h_chips holds the chips
 
     def _new_slot(self):
         import torch

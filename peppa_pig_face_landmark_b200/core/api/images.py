@@ -256,8 +256,9 @@ class FaceAnaImages:
         st["done"].synchronize()
         F = int(counts.sum())
         if host_call is not None and F:
-            self.landmark._warp_host_frames(host_call, counts.tolist(), st["hM"].numpy()[:F], st["M"], st["chip"],
-                                            st["hchip"])
+            fl = self.landmark
+            fl.host_chips.warp(fl.lib, fl.model.stream, host_call, counts.tolist(), st["hM"].numpy()[:F], st["chip"],
+                               st["hchip"])
         host = {k: st["h" + k].numpy()[:F] for k in self._face_fields(0)}
         res = []
         for o, k in zip(first.tolist(), counts.tolist()):

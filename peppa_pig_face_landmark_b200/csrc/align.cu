@@ -8,8 +8,10 @@
 // Two launches cover every face of every frame of a call: the estimate (a thread per face), then the warp (grid.y = face,
 // grid.x = runs of 256 pixels of the face's chip, stored with consecutive threads on consecutive bytes).  The frame is
 // read where it lies.  A face's source is one frame for all faces, one MpStreamDesc per group of faces, or one
-// skps_face_src per face (faces of many images, or just the rectangle of an image a chip reads), which may give any pixel
-// layout of skps_b200.h: only the address of a tap depends on it, the chip is BGR.
+// skps_face_src per face (faces of many images, or just the rectangle of an image a chip reads) or per group (the frame
+// of a detector's slots), which may give any pixel layout of skps_b200.h: only the address of a tap depends on it, the
+// chip is BGR.  The detector's five landmarks have an estimate of their own (det_align_estimate_kernel) that maps them
+// back from the letterbox first.
 #include <limits.h>
 
 #include "../../include/skps_b200.h"
@@ -25,24 +27,26 @@ __constant__ double kTemplate112[10] = {38.2946, 51.6963, 73.5318, 51.5014, 56.0
                                         41.5493, 92.3655, 70.7299, 92.2041};
 __constant__ int kFive[5] = {96, 97, 54, 76, 82};
 
-// Least-squares similarity (rotation, uniform scale, translation; no reflection) mapping the five landmarks of `kps`
-// (P x 2) onto the template scaled by size/112.  The 2-D closed form of Umeyama 1991: with centred points a_i (source)
-// and b_i (template), scale*cos = sum(a.b) / sum|a|^2 and scale*sin = sum(a x b) / sum|a|^2.
-// T: the landmarks' type, each promoted to double as it is read.
-template <typename T>
-__device__ void similarity_to_template(const T* __restrict__ kps, int size, double* M) {
+// Least-squares similarity (rotation, uniform scale, translation; no reflection) mapping five points onto the template
+// scaled by size/112; five(i) gives point i (template order) as a double2.  The 2-D closed form of Umeyama 1991: with
+// centred points a_i (source) and b_i (template), scale*cos = sum(a.b) / sum|a|^2 and scale*sin = sum(a x b) / sum|a|^2.
+// The one estimator of the library: the 98-point path (Five98) and the detector's five points (DetFive) both call it.
+template <typename Five>
+__device__ void similarity_to_template(const Five& five, int size, double* M) {
     const double sc = size / 112.0;
     double msx = 0, msy = 0, mdx = 0, mdy = 0;
 #pragma unroll 1
     for (int i = 0; i < 5; ++i) {
-        msx += (double)kps[2 * kFive[i]]; msy += (double)kps[2 * kFive[i] + 1];
+        const double2 p = five(i);
+        msx += p.x; msy += p.y;
         mdx += kTemplate112[2 * i] * sc; mdy += kTemplate112[2 * i + 1] * sc;
     }
     msx /= 5; msy /= 5; mdx /= 5; mdy /= 5;
     double dot = 0, cross = 0, den = 0;
 #pragma unroll 1
     for (int i = 0; i < 5; ++i) {
-        const double ax = (double)kps[2 * kFive[i]] - msx, ay = (double)kps[2 * kFive[i] + 1] - msy;
+        const double2 p = five(i);
+        const double ax = p.x - msx, ay = p.y - msy;
         const double bx = kTemplate112[2 * i] * sc - mdx, by = kTemplate112[2 * i + 1] * sc - mdy;
         dot += ax * bx + ay * by;
         cross += ax * by - ay * bx;
@@ -53,6 +57,25 @@ __device__ void similarity_to_template(const T* __restrict__ kps, int size, doub
     M[3] = b; M[4] = a;  M[5] = mdy - (b * msx + a * msy);
 }
 
+// The five alignment points kFive of WFLW-98 landmarks `kps` (P x 2) of type T, each promoted to double.
+template <typename T>
+struct Five98 {
+    const T* kps;
+    __device__ double2 operator()(int i) const {
+        return make_double2((double)kps[2 * kFive[i]], (double)kps[2 * kFive[i] + 1]);
+    }
+};
+
+// The five landmarks of a detector row (columns 5..14, letterbox coordinates) in frame pixels: scale_coords' float32
+// (v - pad) / scale, the NMS gather's arithmetic for columns 0..3 (nms.cu), promoted to double.
+struct DetFive {
+    const float* lm;                            // row + 5
+    float scale, left, top;
+    __device__ float x(int i) const { return (lm[2 * i] - left) / scale; }
+    __device__ float y(int i) const { return (lm[2 * i + 1] - top) / scale; }
+    __device__ double2 operator()(int i) const { return make_double2((double)x(i), (double)y(i)); }
+};
+
 // cvRound on x86 (cvtsd2si): half to even; NaN or outside int32 -> INT_MIN
 __device__ __forceinline__ int cv_round(double v) { return fabs(v) < 2147483647.5 ? __double2int_rn(v) : INT_MIN; }
 // int32 addition with the two's-complement wrap OpenCV's int arithmetic has in practice
@@ -62,8 +85,8 @@ __device__ __forceinline__ int sat_short(int v) { return v < -32768 ? -32768 : (
 struct WarpArgs {
     const uint8_t* frame; int H, W, pitch;      // the frame of every face (desc == null)
     const MpStreamDesc* desc;                   // or per group: desc[g].cur, H, W (pitch W*3)
-    const skps_face_src* src;                   // or per face: src[f], taps outside its rectangle read 0,
-    const skps_frame_layout* lay;               // its pixels laid out as lay[f] says (null: BGR)
+    const skps_face_src* src;                   // or per group: src[g], taps outside its rectangle read 0,
+    const skps_frame_layout* lay;               // its pixels laid out as lay[g] says (null: BGR)
     const double* M;                            // [faces][2][3] frame -> chip
     const int* count; int per_group;            // face f = g * per_group + i is skipped when count && i >= count[g]
     int out_h, out_w;
@@ -79,9 +102,31 @@ __global__ void __launch_bounds__(128) align_estimate_kernel(const T* __restrict
     const int g = f / per_group, i = f - g * per_group;
     if (count && i >= count[g]) return;
     double m[6];
-    similarity_to_template(kps + (size_t)f * P * 2, size, m);
+    similarity_to_template(Five98<T>{kps + (size_t)f * P * 2}, size, m);
 #pragma unroll
     for (int j = 0; j < 6; ++j) M[(size_t)f * 6 + j] = m[j];
+}
+
+// One thread per (frame f, slot j) of the detector's kept rows: rows (n, det_cap, 16) with count[f] rows kept, in NMS
+// order.  Slot j < min(count[f], max_chips) gets its five landmarks (columns 5..14, letterbox coordinates) mapped back to
+// the frame with recover[f] = (scale, left, top) exactly as the NMS gather maps columns 0..3 (scale_coords in float32),
+// written to points[f][j] (5 x 2 float32), and M[f][j] from those points promoted to double.  Other slots are skipped.
+__global__ void __launch_bounds__(128) det_align_estimate_kernel(const float* __restrict__ rows, const int* __restrict__ count,
+                                                                 int det_cap, const float* __restrict__ recover, int n,
+                                                                 int max_chips, int size, float* __restrict__ points,
+                                                                 double* __restrict__ M) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (long long)n * max_chips) return;
+    const int f = (int)(t / max_chips), j = (int)(t - (long long)f * max_chips);
+    if (j >= count[f]) return;
+    const DetFive five{rows + ((size_t)f * det_cap + j) * 16 + 5, recover[3 * f], recover[3 * f + 1], recover[3 * f + 2]};
+    float* pt = points + (size_t)t * 10;
+#pragma unroll
+    for (int i = 0; i < 5; ++i) { pt[2 * i] = five.x(i); pt[2 * i + 1] = five.y(i); }
+    double m[6];
+    similarity_to_template(five, size, m);
+#pragma unroll
+    for (int k = 0; k < 6; ++k) M[(size_t)t * 6 + k] = m[k];
 }
 
 // A block warps 256 consecutive pixels of one chip: each thread finds its pixel's four taps and weights once and blends the
@@ -102,9 +147,9 @@ __global__ void __launch_bounds__(256) align_warp_kernel(const WarpArgs a) {
             const MpStreamDesc& d = a.desc[g];
             base = d.cur; H = d.H; W = d.W; pitch = d.W * 3; rw = W; rh = H;
         } else if (a.src) {
-            const skps_face_src& s = a.src[f];
+            const skps_face_src& s = a.src[g];
             base = s.base; H = s.H; W = s.W; pitch = s.pitch; ox = s.ox; oy = s.oy; rw = s.rw; rh = s.rh;
-            if (a.lay) lay = px_layout(a.lay[f].layout, a.lay[f].plane_pitch);
+            if (a.lay) lay = px_layout(a.lay[g].layout, a.lay[g].plane_pitch);
         }
         const int xa = max(ox, 0), xb = min(ox + rw, W), ya = max(oy, 0), yb = min(oy + rh, H);
         // the inverse map as warpAffine computes it (imgwarp.cpp), same order of operations; every thread of the face
@@ -209,9 +254,32 @@ extern "C" SKPS_API int skps_warp_faces_layout(const skps_face_src* src, const s
     for (int c0 = 0; c0 < n; c0 += 65535) {
         const int m = min(65535, n - c0);
         WarpArgs a = {};
-        a.src = src + c0; a.lay = lay ? lay + c0 : nullptr; a.M = M + (size_t)c0 * 6; a.per_group = m;
+        a.src = src + c0; a.lay = lay ? lay + c0 : nullptr; a.M = M + (size_t)c0 * 6; a.per_group = 1;   // a source per face
         a.out_h = out_h; a.out_w = out_w; a.out = out + (size_t)c0 * out_h * out_w * 3;
         if (launch_warp(a, m, (cudaStream_t)stream)) return 1;
+    }
+    return 0;
+}
+
+extern "C" SKPS_API int skps_warp_faces_count(const skps_face_src* src, const skps_frame_layout* lay, const int32_t* count,
+                                              int n_frames, int per_frame, const double* M, int out_h, int out_w,
+                                              uint8_t* out, void* stream) {
+    SKPS_CHECK(n_frames >= 0 && per_frame > 0 && per_frame <= 65535 && out_h > 0 && out_w > 0 && out_h <= 4096 &&
+               out_w <= 4096, "warp_faces_count: n_frames %d, per_frame %d or output %dx%d out of range", n_frames,
+               per_frame, out_h, out_w);
+    if (n_frames == 0) return 0;
+    SKPS_CHECK(src && count && M && out, "warp_faces_count: bad arguments");
+    // grid.y is the slot: chunks of whole frames, at most 65535 slots each
+    const int step = 65535 / per_frame;
+    const size_t chip = (size_t)out_h * out_w * 3;
+    for (int g0 = 0; g0 < n_frames; g0 += step) {
+        const int m = min(step, n_frames - g0);
+        const size_t f0 = (size_t)g0 * per_frame;
+        WarpArgs a = {};
+        a.src = src + g0; a.lay = lay ? lay + g0 : nullptr; a.M = M + f0 * 6;
+        a.count = count + g0; a.per_group = per_frame;
+        a.out_h = out_h; a.out_w = out_w; a.out = out + f0 * chip;
+        if (launch_warp(a, m * per_frame, (cudaStream_t)stream)) return 1;
     }
     return 0;
 }
@@ -227,6 +295,21 @@ extern "C" SKPS_API int skps_align_estimate(const float* kps, int n, int P, int 
     if (n == 0) return 0;
     SKPS_CHECK(kps && M, "align_estimate: bad arguments");
     align_estimate_kernel<float><<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(kps, P, nullptr, n, n, size, M);
+    SKPS_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" SKPS_API int skps_det_align_estimate(const float* rows, const int32_t* count, int det_cap, const float* recover,
+                                                int n_frames, int max_chips, int size, float* points, double* M,
+                                                void* stream) {
+    SKPS_CHECK(n_frames >= 0 && max_chips > 0 && max_chips <= det_cap,
+               "det_align_estimate: n_frames %d or max_chips %d out of range (det_cap %d)", n_frames, max_chips, det_cap);
+    SKPS_CHECK(size >= 16 && size <= 512, "det_align_estimate: size %d outside 16..512", size);
+    if (n_frames == 0) return 0;
+    SKPS_CHECK(rows && count && recover && points && M, "det_align_estimate: bad arguments");
+    const long long slots = (long long)n_frames * max_chips;
+    det_align_estimate_kernel<<<(unsigned)((slots + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+        rows, count, det_cap, recover, n_frames, max_chips, size, points, M);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }

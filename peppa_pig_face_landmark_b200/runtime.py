@@ -133,6 +133,8 @@ SIGNATURES = {
     "skps_warp_faces": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
     "skps_warp_faces_layout": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
     "skps_align_estimate": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
+    "skps_warp_faces_count": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_int, c_vp, C.c_int, C.c_int, c_vp, c_vp]),
+    "skps_det_align_estimate": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp]),
     "skps_pipeline_align": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp]),
     "skps_mpipe_set_align": (C.c_int, [c_vp, C.c_int]),
     "skps_mpipe_align_results": (C.c_int, [c_vp, C.c_int, c_vp, c_vp]),
