@@ -200,6 +200,21 @@ enum {
     SKPS_LAYOUT_RGB_PLANAR = 5
 };
 
+/* Frames stored turned (the *_rotate entries): `turns` is the number of quarter turns clockwise, 0..3, by which the stored
+ * frame must be turned to be upright; the frame is analysed as cv2.rotate(frame, code) with 1 ROTATE_90_CLOCKWISE,
+ * 2 ROTATE_180 and 3 ROTATE_90_COUNTERCLOCKWISE.  A frame's H, W and pitch describe it as stored; pixel (y, x) of the
+ * upright frame (W x H for odd turns) is at
+ *     base + org + y*ystep + x*xstep + off[c]
+ * with, for a row pitch p and the layout's xstep s:
+ *     0: org 0,                    ystep  p, xstep  s
+ *     1: org (H-1)p,               ystep  s, xstep -p
+ *     2: org (H-1)p + (W-1)s,      ystep -p, xstep -s
+ *     3: org (W-1)s,               ystep -s, xstep  p
+ * The kernels only compute addresses this way and keep their arithmetic: every result, in upright coordinates, is bit for
+ * bit that of the upright frame passed as a contiguous frame.  Entries taking a [dev] turns array read its low two bits
+ * only; the others fail on a value outside 0..3.  A NULL turns array, or turns 0, means no turn and runs the kernels of
+ * the entries without it. */
+
 /* FaceDetector.preprocess (face_detector.py:45-71): BGR->RGB, cv2.resize INTER_LINEAR
  * (bit-exact 11-bit fixed point) to (rw,rh), pad with 114 to (in_h,in_w).  `frame` [dev]
  * HxWx3 uint8 with row pitch `pitch` bytes; `out` [dev] in_h*in_w*3 uint8 RGB.  The /255 is
@@ -240,6 +255,11 @@ typedef struct skps_frame_layout {
  * same pixels as an interleaved BGR frame.  row_pairs frames are BGR. */
 SKPS_API int skps_letterbox_frames_layout(const skps_det_src* src, const skps_frame_layout* lay, int n, uint8_t* out,
                                           int in_h, int in_w, void* stream);
+/* skps_letterbox_frames_layout for frames stored turned: frame i must be turned turns[i] [dev] (n) quarter turns clockwise
+ * (see SKPS_LAYOUT_* above); src[i].H, W and pitch describe it as stored, its letterbox geometry (rw, rh, top, left) that of
+ * the upright frame.  row_pairs frames are read unturned.  turns NULL: skps_letterbox_frames_layout. */
+SKPS_API int skps_letterbox_frames_rotate(const skps_det_src* src, const skps_frame_layout* lay, const int32_t* turns, int n,
+                                          uint8_t* out, int in_h, int in_w, void* stream);
 
 /* xywh2xyxy + py_nms + scale_coords (face_detector.py:73-136) on the raw (rows,16) output.
  * Writes up to max_det (<= 256) kept rows (16 floats each, cols 0-3 mapped back to frame pixels),
@@ -325,6 +345,12 @@ SKPS_API int skps_crop_faces(const skps_face_src* src, const float* boxes4, int 
 SKPS_API int skps_crop_faces_layout(const skps_face_src* src, const skps_frame_layout* lay, const float* boxes4, int n,
                                     float face_scale, float min_face, uint8_t* crops, int out_hw, int32_t* detail,
                                     void* stream);
+/* skps_crop_faces_layout for faces of frames stored turned: face i's frame must be turned turns[i] [dev] (n) quarter turns
+ * clockwise and its box is in the upright frame.  A turned frame is read whole (its ox, oy, rw, rh are not read); one of
+ * turn 0 may be a rectangle as for skps_crop_faces.  turns NULL: skps_crop_faces_layout. */
+SKPS_API int skps_crop_faces_rotate(const skps_face_src* src, const skps_frame_layout* lay, const int32_t* turns,
+                                    const float* boxes4, int n, float face_scale, float min_face, uint8_t* crops, int out_hw,
+                                    int32_t* detail, void* stream);
 
 /* FaceLandmark.postprocess (face_landmark.py:106-115): x*w + x1 - add, y*h + y1 - add. */
 SKPS_API int skps_landmark_post(const float* xy_norm, const int32_t* detail, const int32_t* count,
@@ -344,6 +370,11 @@ SKPS_API int skps_frame_ingest(const uint8_t* frame, int H, int W, int pitch, ui
  * is sum |packed - prev|, the bytes and the sum skps_frame_ingest gives for the same pixels passed as BGR.  pitch >=
  * xstep * W (H == 1: any); plane_pitch is read for the planar layouts only.  skps_frame_ingest is this entry with BGR. */
 SKPS_API int skps_frame_ingest_layout(const uint8_t* frame, int H, int W, int pitch, int layout, int plane_pitch,
+                                      uint8_t* packed, const uint8_t* prev, unsigned long long* sum, void* stream);
+/* skps_frame_ingest_layout for a frame stored turned `turns` (0..3) quarter turns clockwise: H, W and pitch describe the
+ * stored frame, `packed` gets the upright frame (W x H for odd turns) as interleaved BGR and *sum is sum |packed - prev|,
+ * the bytes and the sum skps_frame_ingest gives for the upright frame.  turns 0: skps_frame_ingest_layout. */
+SKPS_API int skps_frame_ingest_rotate(const uint8_t* frame, int H, int W, int pitch, int layout, int plane_pitch, int turns,
                                       uint8_t* packed, const uint8_t* prev, unsigned long long* sum, void* stream);
 
 /* ------------------------------------------------------------------ FaceAna.run (facer.py:52-85) */
@@ -425,6 +456,12 @@ SKPS_API int skps_pipeline_frame_diff_device(skps_pipeline* p, const uint8_t* fr
 SKPS_API int skps_pipeline_frame_diff_device_layout(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch,
                                                     int layout, int plane_pitch, void* producer_stream, double* mean_diff,
                                                     void* stream);
+/* skps_pipeline_frame_diff_device_layout for a frame stored turned `turns` (0..3) quarter turns clockwise (H, W, pitch as
+ * stored): the frame is staged upright, so the gate, skps_pipeline_run, pose and alignment see the upright frame, of size
+ * W x H for odd turns, and consecutive frames may change turns.  turns 0: skps_pipeline_frame_diff_device_layout. */
+SKPS_API int skps_pipeline_frame_diff_device_rotate(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch,
+                                                    int layout, int plane_pitch, int turns, void* producer_stream,
+                                                    double* mean_diff, void* stream);
 /* Adopt the staged frame as the previous frame without running the chain: the skip path of FaceAna.run (facer.py:57-62
  * replaces previous_image on every call, also when nothing is detected or tracked).  Fails when no frame is staged. */
 SKPS_API int skps_pipeline_commit_frame(skps_pipeline* p);
@@ -527,6 +564,14 @@ SKPS_API int skps_mpipe_submit_device_layout(skps_mpipe* p, int slot, const int3
                                              const int32_t* pitches, const int32_t* hw, int n, int layout,
                                              const int32_t* plane_pitches, const skps_mpipe_outputs* out,
                                              void* producer_stream);
+/* skps_mpipe_submit_device_layout for frames stored turned: frame i must be turned turns[i] [host] int32 (n, each 0..3)
+ * quarter turns clockwise; hw and pitches describe it as stored.  It is gathered into its stream's ring upright, so the
+ * stream sees the upright frame: a stream whose frames change between odd and even turns changes frame size (the next
+ * frame is a keyframe), one that changes between 0 and 2 does not.  turns NULL: skps_mpipe_submit_device_layout. */
+SKPS_API int skps_mpipe_submit_device_rotate(skps_mpipe* p, int slot, const int32_t* streams, const uint8_t* const* frames,
+                                             const int32_t* pitches, const int32_t* hw, int n, int layout,
+                                             const int32_t* plane_pitches, const int32_t* turns,
+                                             const skps_mpipe_outputs* out, void* producer_stream);
 /* Completes a slot submitted with device outputs without blocking the host: work queued on `consumer_stream` after this
  * call runs after the batch's results are in the caller's buffers.  The slot can then be submitted again. */
 SKPS_API int skps_mpipe_wait_stream(skps_mpipe* p, int slot, void* consumer_stream);
@@ -597,6 +642,11 @@ SKPS_API int skps_warp_faces(const skps_face_src* src, const double* M, int n, i
  * every image is BGR (skps_warp_faces).  The chips are BGR, the bytes of the same pixels as an interleaved BGR image. */
 SKPS_API int skps_warp_faces_layout(const skps_face_src* src, const skps_frame_layout* lay, const double* M, int n, int out_h,
                                     int out_w, uint8_t* out, void* stream);
+/* skps_warp_faces_layout for faces of images stored turned: chip i's image must be turned turns[i] [dev] (n) quarter turns
+ * clockwise and M maps the upright image.  A turned image is read whole; one of turn 0 may be a rectangle as for
+ * skps_warp_faces.  turns NULL: skps_warp_faces_layout. */
+SKPS_API int skps_warp_faces_rotate(const skps_face_src* src, const skps_frame_layout* lay, const int32_t* turns,
+                                    const double* M, int n, int out_h, int out_w, uint8_t* out, void* stream);
 /* skps_warp_faces_layout for the kept faces of n_frames frames, with the face counts known only on the device:
  * n_frames * per_frame slots (per_frame 1..65535) are launched, and slot j of frame i, chip i*per_frame + j of
  * out [dev] (n_frames*per_frame,out_h,out_w,3) uint8, is warped with M [dev] + (i*per_frame + j)*6 only when
@@ -606,6 +656,11 @@ SKPS_API int skps_warp_faces_layout(const skps_face_src* src, const skps_frame_l
 SKPS_API int skps_warp_faces_count(const skps_face_src* src, const skps_frame_layout* lay, const int32_t* count,
                                    int n_frames, int per_frame, const double* M, int out_h, int out_w, uint8_t* out,
                                    void* stream);
+/* skps_warp_faces_count for frames stored turned: frame i must be turned turns[i] [dev] (n_frames) quarter turns clockwise
+ * and its matrices map the upright frame (FaceDetector(align=...) on turned frames).  turns NULL: skps_warp_faces_count. */
+SKPS_API int skps_warp_faces_count_rotate(const skps_face_src* src, const skps_frame_layout* lay, const int32_t* turns,
+                                          const int32_t* count, int n_frames, int per_frame, const double* M, int out_h,
+                                          int out_w, uint8_t* out, void* stream);
 /* The estimate for the detector's own five landmarks (yolov5-face columns 5..14: eyes, nose tip, mouth corners, the
  * template's order).  rows [dev] (n_frames,det_cap,16), count [dev] (n_frames) and recover [dev] (n_frames,3) float32 are
  * skps_detect_post_batch's kept_rows, count and recover with capacity det_cap.  For slot j < min(count[i], max_chips)

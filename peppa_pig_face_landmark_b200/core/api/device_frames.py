@@ -2,8 +2,11 @@
 already in GPU memory (a decoder surface, a tensor from NVDEC / DALI / torchvision, an ROI view of either).  Host frames
 are HxWx3 uint8 BGR as the reference's run(image) takes them.  CUDA frames are read where they are, at any row pitch, in
 the pixel layout the caller names with layout= (LAYOUTS): interleaved BGR (the default), RGB, BGRA or RGBA, or planar
-(3, H, W) BGR or RGB.  Every layout gives, bit for bit, the results of the same pixels passed as interleaved BGR."""
+(3, H, W) BGR or RGB.  Every layout gives, bit for bit, the results of the same pixels passed as interleaved BGR.
+CUDA frames stored sideways or upside down (a portrait clip from NVDEC, a photo whose EXIF orientation nvJPEG did not
+apply, a ceiling camera) are read in place as the upright frame with rotate= (check_rotate)."""
 import collections
+import numbers
 import sys
 
 import numpy as np
@@ -70,6 +73,49 @@ def frame_layout(shape, strides, layout):
     if plane >= 2 ** 31:
         raise ValueError("plane pitch %d does not fit 32 bits" % plane)
     return FrameLayout(H, W, pitch, plane, code)
+
+
+ROTATIONS = (0, 90, 180, 270)
+
+
+def _turns(rotate):
+    if isinstance(rotate, (bool, np.bool_)) or not isinstance(rotate, numbers.Integral) or int(rotate) not in ROTATIONS:
+        raise ValueError("rotate: expected one of %s (degrees clockwise), got %r" % (", ".join(map(str, ROTATIONS)), rotate))
+    return int(rotate) // 90
+
+
+def check_rotate(rotate, n=None, cuda=True):
+    """Quarter turns clockwise (0..3) of rotate=: the clockwise angle in degrees, one of ROTATIONS, by which a stored
+    frame must be turned to be upright.  The frame is analysed as cv2.rotate(frame, code), 90 being ROTATE_90_CLOCKWISE,
+    180 ROTATE_180 and 270 ROTATE_90_COUNTERCLOCKWISE; for an (H, W, C) tensor that is
+    torch.rot90(frame, -rotate // 90, dims=(0, 1)), for a planar one the same with dims=(1, 2).
+    n None: rotate is one int, and so is the result.  n an int: rotate is one int for all n frames or a sequence of n,
+    and the result a list of n turns.  ValueError for a value outside ROTATIONS, a bool or a non-int, a sequence of
+    another length, and any turn with host frames (cuda False): cv2.imread and VideoCapture give them upright already,
+    and the caller can cv2.rotate them."""
+    if n is None or isinstance(rotate, (numbers.Number, np.bool_, str, bytes)) or not hasattr(rotate, "__len__"):
+        t = _turns(rotate)
+        turns = t if n is None else [t] * n
+    else:
+        if len(rotate) != n:
+            raise ValueError("rotate: expected one value or one per frame (%d), got %d values" % (n, len(rotate)))
+        turns = [_turns(r) for r in rotate]
+    if not cuda and any(turns if n is not None else [turns]):
+        raise ValueError("rotate=%r takes CUDA frames; host frames are upright as cv2 decodes them (cv2.rotate them)"
+                         % (rotate,))
+    return turns
+
+
+def upright_hw(H, W, turns):
+    """(H, W) of the upright frame of an H x W frame stored `turns` quarter turns from upright."""
+    return (W, H) if turns & 1 else (H, W)
+
+
+def upright_shape(shape, strides, layout="bgr", rotate=0):
+    """(H, W) of the upright frame a call analyses for a uint8 frame with this shape and these strides (in bytes) in
+    layout `layout` (frame_layout) stored turned by rotate= degrees (check_rotate).  ValueError as those two raise it."""
+    fl = frame_layout(shape, strides, layout)
+    return upright_hw(fl.H, fl.W, check_rotate(rotate))
 
 
 def check_host_frame(frame):

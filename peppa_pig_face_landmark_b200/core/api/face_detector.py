@@ -194,14 +194,14 @@ class FaceDetector:
         return bboxes
 
     # ------------------------------------------------------------------ batched path
-    def run_batch(self, frames, layout="bgr"):
+    def run_batch(self, frames, layout="bgr", rotate=0):
         """The detector over many frames (blocking): the i-th (k_i, 16) float32 array of the returned list is bit for bit
         what FaceDetector(cfg)(frames[i]) returns; last_keep_idx is then the list of the frames' kept row indices (int64).
-        With align, the i-th entry is (rows, points, chips, M) (see __init__).  See submit() for what frames and layout
-        may be."""
+        With align, the i-th entry is (rows, points, chips, M) (see __init__).  See submit() for what frames, layout and
+        rotate may be."""
         if self._pending:
             raise RuntimeError("FaceDetector: %d calls in flight; collect() them first" % len(self._pending))
-        self.submit(frames, layout=layout)
+        self.submit(frames, layout=layout, rotate=rotate)
         return self.collect()
 
     def new_results(self, n_frames):
@@ -217,7 +217,7 @@ class FaceDetector:
     def _fields(self, n_frames):
         return result_fields(n_frames, self._rows, self.align, self.max_chips)
 
-    def submit(self, frames, out=None, layout="bgr"):
+    def submit(self, frames, out=None, layout="bgr", rotate=0):
         """Enqueue the detector on frames; at most two calls may be in flight and collect() returns them in submission
         order.  Everything is checked before anything is enqueued.
 
@@ -229,6 +229,10 @@ class FaceDetector:
         layout: the pixel layout of all CUDA frames of the call (device_frames.frame_layout): "bgr" (the default), "rgb",
         "bgra", "rgba" (H, W, 4), "bgr_planar" or "rgb_planar" (3, H, W).  The letterbox reads them in place, and the
         results are, bit for bit, those of the same pixels passed as interleaved BGR.  Host frames are BGR only.
+        rotate: the clockwise angle in degrees (0, 90, 180 or 270) by which CUDA frames, as stored, must be turned to be
+        upright (device_frames.check_rotate), one for the call or one per frame (each photo has its own EXIF
+        orientation).  They are read in place, and every result (rows, kept indices, points, M, chips) is in the
+        upright frame's pixels, bit for bit that of the upright frame passed as a contiguous tensor.  Host frames take 0.
         Ordering on torch.cuda.current_stream(): CUDA frames are read after the work already queued on it, and work
         queued on it after submit() returns runs after they have been read.
         out: None (collect() returns numpy arrays), or, with CUDA frames, a dict from new_results(n) with n >= the call's
@@ -241,7 +245,7 @@ class FaceDetector:
         one more upload per call, and the host frames must stay unchanged until collect() returns."""
         if len(self._pending) == 2:
             raise RuntimeError("FaceDetector: two calls already in flight; call collect() first")
-        call = check_frames(frames, self.device, layout)
+        call = check_frames(frames, self.device, layout, rotate)
         geo = self._layout(call)
         n = len(call.frames)
         if out is not None:
@@ -314,13 +318,14 @@ class FaceDetector:
     # ------------------------------------------------------------------
     def _layout(self, call):
         """[(H, W, row pitch, letterbox geometry, rows uploaded or None)] of the frames of a call checked by
-        check_frames; ValueError for a frame whose letterbox is empty."""
+        check_frames, H, W and pitch as stored, the geometry that of the upright frame; ValueError for a frame whose
+        letterbox is empty."""
         in_h, in_w = self.input_size[0], self.input_size[1]
         layout = []
-        for H, W, pitch, _, _ in call.shapes:
-            geo = letterbox_geometry(H, W, in_h, in_w)
+        for (H, W, pitch, _, _), (Hu, Wu) in zip(call.shapes, call.upright):
+            geo = letterbox_geometry(Hu, Wu, in_h, in_w)
             if geo[1] < 1 or geo[2] < 1:
-                raise ValueError("frame %dx%d: its letterbox at %dx%d is %dx%d, empty" % (H, W, in_h, in_w, geo[2], geo[1]))
+                raise ValueError("frame %dx%d: its letterbox at %dx%d is %dx%d, empty" % (Hu, Wu, in_h, in_w, geo[2], geo[1]))
             layout.append((H, W, pitch, geo, None if call.cuda else host_upload_rows(H, geo[2])))
         return layout
 
@@ -339,11 +344,14 @@ class FaceDetector:
             self._slots = [self._new_slot() for _ in range(2)]
         slot = self._next
         st = self._slots[slot]
-        # CUDA frames in a layout other than BGR: one skps_frame_layout per frame after the recoveries
+        # CUDA frames in a layout other than BGR: one skps_frame_layout per frame after the recoveries; a call holding a
+        # turned frame: then the quarter turns of every frame, int32
         lay = cuda and n > 0 and call.shapes[0].code != 0
+        turned = cuda and call.turned
         rec_off = pad16(n * DET_SRC.itemsize)
         lay_off = rec_off + pad16(n * 12)
-        face_off = lay_off + (pad16(n * FRAME_LAYOUT.itemsize) if lay else 0)
+        turn_off = lay_off + (pad16(n * FRAME_LAYOUT.itemsize) if lay else 0)
+        face_off = turn_off + (pad16(n * 4) if turned else 0)
         frame_off = face_off + (pad16(n * FACE_SRC.itemsize) if warp_now else 0)
         sizes = [0 if cuda else pad16((H if rows is None else len(rows)) * pitch) for H, W, pitch, geo, rows in layout]
         total = frame_off + sum(sizes)
@@ -362,14 +370,16 @@ class FaceDetector:
         if own and warp_now and (st["chip"] is None or st["chip"].shape[0] < n):
             st["done"].synchronize()
             st["chip"] = grow(st["chip"], n, lambda k: torch.empty((k, C, A, A, 3), dtype=torch.uint8, device=self.device))
-        # host staging = [n frame descriptors | n (scale, left, top) | n layouts | n face sources | the host frames' rows],
-        # sent with one copy
+        # host staging = [n frame descriptors | n (scale, left, top) | n layouts | n turns | n face sources | the host
+        # frames' rows], sent with one copy
         desc = host[:n * DET_SRC.itemsize].view(DET_SRC)
         rec = host[rec_off:rec_off + 12 * n].view(np.float32).reshape(n, 3)
         if lay:
             fl = host[lay_off:lay_off + n * FRAME_LAYOUT.itemsize].view(FRAME_LAYOUT)
             fl["layout"] = [f.code for f in call.shapes]
             fl["plane_pitch"] = [f.plane for f in call.shapes]
+        if turned:
+            host[turn_off:turn_off + 4 * n].view(np.int32)[:] = call.turns
         if warp_now:                                  # the chips' sources: the whole frames
             fs = host[face_off:face_off + n * FACE_SRC.itemsize].view(FACE_SRC)
             H, W, pitch = np.array([f[:3] for f in call.shapes], np.int64).reshape(-1, 3).T
@@ -405,8 +415,9 @@ class FaceDetector:
         for c0 in range(0, n, K):
             m = min(K, n - c0)
             with torch.cuda.device(self.device):      # the kernels launch on the current device
-                rt.check(self.lib.skps_letterbox_frames_layout(dev + DET_SRC.itemsize * c0,
+                rt.check(self.lib.skps_letterbox_frames_rotate(dev + DET_SRC.itemsize * c0,
                                                                dev + lay_off + FRAME_LAYOUT.itemsize * c0 if lay else None,
+                                                               dev + turn_off + 4 * c0 if turned else None,
                                                                m, inp, in_h, in_w, s.cuda_stream))
             if c0 + K >= n and not warp_now:
                 st["read"].record(s)
@@ -424,9 +435,10 @@ class FaceDetector:
                 rt.check(self.lib.skps_det_align_estimate(rows_t.data_ptr(), count_t.data_ptr(), R, dev + rec_off, n, C, A,
                                                           points.data_ptr(), mats.data_ptr(), s.cuda_stream))
                 if warp_now:
-                    rt.check(self.lib.skps_warp_faces_count(dev + face_off, dev + lay_off if lay else None,
-                                                            count_t.data_ptr(), n, C, mats.data_ptr(), A, A,
-                                                            res["chip"].data_ptr(), s.cuda_stream))
+                    rt.check(self.lib.skps_warp_faces_count_rotate(dev + face_off, dev + lay_off if lay else None,
+                                                                   dev + turn_off if turned else None, count_t.data_ptr(),
+                                                                   n, C, mats.data_ptr(), A, A, res["chip"].data_ptr(),
+                                                                   s.cuda_stream))
         if n == 0 or warp_now:
             st["read"].record(s)
         torch.cuda.current_stream(self.device).wait_event(st["read"])

@@ -218,14 +218,14 @@ class FaceLandmark:
         return kps, scores
 
     # ------------------------------------------------------------------ batched path
-    def run_batch(self, frames, boxes, layout="bgr"):
+    def run_batch(self, frames, boxes, layout="bgr", rotate=0):
         """Landmarks for the faces the caller has, over many frames (blocking): frames[i] with boxes[i] -> the i-th
         (kps (k_i, 98, 2) float32, scores (k_i, 98) float32) of the returned list, bit for bit what
         FaceLandmark(cfg)(frames[i], boxes[i]) returns; with align, (kps, scores, chips (k_i, s, s, 3) uint8,
-        M (k_i, 2, 3) float64).  See submit() for what frames, boxes and layout may be."""
+        M (k_i, 2, 3) float64).  See submit() for what frames, boxes, layout and rotate may be."""
         if self._pending:
             raise RuntimeError("FaceLandmark: %d calls in flight; collect() them first" % len(self._pending))
-        self.submit(frames, boxes, layout=layout)
+        self.submit(frames, boxes, layout=layout, rotate=rotate)
         return self.collect()
 
     def new_results(self, n_faces):
@@ -238,7 +238,7 @@ class FaceLandmark:
     def _fields(self, n_faces):
         return result_fields(n_faces, self.keypoints_num, self.align)
 
-    def submit(self, frames, boxes, out=None, layout="bgr"):
+    def submit(self, frames, boxes, out=None, layout="bgr", rotate=0):
         """Enqueue landmarks for boxes[i] on frames[i]; at most two calls may be in flight and collect() returns them in
         submission order.  Everything is checked before anything is enqueued.
 
@@ -255,6 +255,10 @@ class FaceLandmark:
         layout: the pixel layout of all CUDA frames of the call (device_frames.frame_layout): "bgr" (the default), "rgb",
         "bgra", "rgba" (H, W, 4), "bgr_planar" or "rgb_planar" (3, H, W).  Crops and chips read them in place and come
         out BGR, bit for bit those of the same pixels passed as interleaved BGR.  Host frames are BGR only.
+        rotate: the clockwise angle in degrees (0, 90, 180 or 270) by which CUDA frames, as stored, must be turned to be
+        upright (device_frames.check_rotate), one for the call or one per frame.  The boxes are in the upright frame's
+        pixels, and so are the results, bit for bit those of the upright frame passed as a contiguous tensor; crops and
+        chips read the stored frame in place.  Host frames take 0.
 
         With align, CUDA frames are warped into chips on the GPU right after the landmarks, with no host synchronisation,
         and are read until then.  Host frames are warped at collect(): M comes back with kps and scores, and
@@ -263,7 +267,7 @@ class FaceLandmark:
         collect() returns."""
         if len(self._pending) == 2:
             raise RuntimeError("FaceLandmark: two calls already in flight; call collect() first")
-        call = check_frames(frames, self.device, layout)
+        call = check_frames(frames, self.device, layout, rotate)
         boxes, cuda_boxes = self._check_boxes(call, boxes)
         counts = [int(b.shape[0]) for b in boxes]
         if out is not None:
@@ -305,10 +309,13 @@ class FaceLandmark:
         image = np.repeat(np.arange(len(counts)), counts)
         rects = None if call.cuda or n == 0 else np.concatenate(
             [crop_read_rects(b, f.H, f.W, self.face_scale, self.min_face) for b, f in zip(boxes, call.shapes)])
-        # CUDA frames in a layout other than BGR: one skps_frame_layout per face after the descriptors
+        # CUDA frames in a layout other than BGR: one skps_frame_layout per face after the descriptors; a call holding a
+        # turned frame: then the quarter turns of every face's frame, int32
         lay = call.cuda and n > 0 and call.shapes[0].code != 0
+        turned = call.cuda and n > 0 and call.turned
         lay_off = pad16(n * FACE_SRC.itemsize)
-        box_off = lay_off + (pad16(n * FRAME_LAYOUT.itemsize) if lay else 0)
+        turn_off = lay_off + (pad16(n * FRAME_LAYOUT.itemsize) if lay else 0)
+        box_off = turn_off + (pad16(n * 4) if turned else 0)
         roi_off = box_off + pad16(n * 16)
         total = roi_off + (0 if rects is None else int(_rect_bytes(rects).sum()))
         sent = box_off if cuda_boxes else total       # bytes of the host staging the call sends
@@ -326,7 +333,8 @@ class FaceLandmark:
             st["hM"] = grow(st["hM"], n, lambda k: torch.empty((k, 2, 3), dtype=torch.float64).pin_memory())
             st["chip"] = grow(st["chip"], n, lambda k: torch.empty((k, A, A, 3), dtype=torch.uint8, device=self.device))
             st["hchip"] = grow(st["hchip"], n, lambda k: torch.empty((k, A, A, 3), dtype=torch.uint8).pin_memory())
-        # host staging = [n face descriptors | n layouts | n boxes | the host frames' rectangles], sent with one copy
+        # host staging = [n face descriptors | n layouts | n turns | n boxes | the host frames' rectangles], sent with one
+        # copy
         if n and not cuda_boxes:
             host[box_off:box_off + 16 * n].view(np.float32).reshape(n, 4)[:] = np.concatenate(boxes)
         if call.cuda:                                 # descriptors of the whole frames
@@ -338,6 +346,8 @@ class FaceLandmark:
             if lay:
                 fl = host[lay_off:lay_off + n * FRAME_LAYOUT.itemsize].view(FRAME_LAYOUT)
                 fl["layout"], fl["plane_pitch"] = code, plane
+            if turned:
+                host[turn_off:turn_off + 4 * n].view(np.int32)[:] = np.array(call.turns, np.int32)[image]
         elif n:
             _gather_rects(call.frames, rects, image, host, roi_off, dev)
 
@@ -357,8 +367,9 @@ class FaceLandmark:
         for c0 in range(0, n, K):
             m = min(K, n - c0)
             with torch.cuda.device(self.device):      # the kernels launch on the current device
-                rt.check(self.lib.skps_crop_faces_layout(dev + FACE_SRC.itemsize * c0,
+                rt.check(self.lib.skps_crop_faces_rotate(dev + FACE_SRC.itemsize * c0,
                                                          dev + lay_off + FRAME_LAYOUT.itemsize * c0 if lay else None,
+                                                         dev + turn_off + 4 * c0 if turned else None,
                                                          dev + box_off + 16 * c0, m, self.face_scale, float(self.min_face),
                                                          inp, S, det + 20 * c0, s.cuda_stream))
             if c0 + K >= n and not warp_now:
@@ -373,7 +384,8 @@ class FaceLandmark:
             with torch.cuda.device(self.device):
                 rt.check(self.lib.skps_align_estimate(kps.data_ptr(), n, P, A, M.data_ptr(), s.cuda_stream))
                 if warp_now:                          # the face descriptors hold the whole CUDA frames
-                    rt.check(self.lib.skps_warp_faces_layout(dev, dev + lay_off if lay else None, M.data_ptr(), n, A, A,
+                    rt.check(self.lib.skps_warp_faces_rotate(dev, dev + lay_off if lay else None,
+                                                             dev + turn_off if turned else None, M.data_ptr(), n, A, A,
                                                              chips.data_ptr(), s.cuda_stream))
         if n == 0 or warp_now:
             st["read"].record(s)

@@ -20,7 +20,7 @@ from ..smoother.lk import MAX_ID_MEMORY, EmaFilter, GroupTrack, IdMemory, assign
 from .face_detector import FaceDetector, letterbox_geometry
 from .face_landmark import MIN_FACE, FaceLandmark, face_scale
 from .align import check_size
-from .device_frames import PLANAR, check_cuda_frame, check_host_frame, check_layout, is_cuda_tensor
+from .device_frames import PLANAR, check_cuda_frame, check_host_frame, check_layout, check_rotate, is_cuda_tensor
 
 
 MAX_TOP_K = 1024           # SKPS_MAX_TOP_K of include/skps_b200.h
@@ -179,7 +179,7 @@ class FaceAna():
             self._pipe = None
 
     # ------------------------------------------------------------------ facer.py:52-85
-    def run(self, image, layout="bgr"):
+    def run(self, image, layout="bgr", rotate=0):
         """image: an HxWx3 uint8 BGR numpy array, or a torch.uint8 CUDA tensor (H, W, 3) in BGR order on this object's
         device with stride(2) == 1, stride(1) == 3 and any row pitch stride(0) >= 3W (a packed tensor, a pitched decoder
         surface, big[y0:y1, x0:x1]).  A CUDA frame is copied once on the GPU, never through the host, and the results are
@@ -190,12 +190,21 @@ class FaceAna():
         layout: the pixel layout of a CUDA frame (device_frames.frame_layout): "bgr" (the default), "rgb", "bgra",
         "rgba" (H, W, 4), or "bgr_planar", "rgb_planar" (3, H, W) with any row and plane pitch.  The frame is packed
         into BGR by the same GPU copy, and the results are, bit for bit, those of the same pixels passed as an
-        interleaved BGR frame.  Calls may change layouts from frame to frame.  Host frames are BGR only."""
+        interleaved BGR frame.  Calls may change layouts from frame to frame.  Host frames are BGR only.
+
+        rotate: the clockwise angle in degrees (0, 90, 180 or 270) by which a CUDA frame, as stored, must be turned to
+        be upright (device_frames.check_rotate): a portrait clip NVDEC returns as coded, a ceiling camera.  The same GPU
+        copy stages the frame upright, and the results are in the upright frame's pixels, bit for bit those of the
+        upright frame passed as a contiguous tensor; the gate, tracking and smoothing see the upright frame, so a change
+        between 0 and 90 is a change of frame size.  Host frames take 0."""
         check_layout(layout, is_cuda_tensor(image))
+        turns = check_rotate(rotate, cuda=is_cuda_tensor(image))
         image = image if is_cuda_tensor(image) else check_host_frame(image)
-        d = self._frame_diff(image, layout)     # checks a CUDA frame, stages the frame on the device as BGR
+        d = self._frame_diff(image, layout, turns)     # checks a CUDA frame, stages the frame on the device as upright BGR
         if layout in PLANAR:
             image = image.permute(1, 2, 0)      # an (H, W, 3) view: from here on only the frame's size is read
+        if turns & 1:
+            image = image.permute(1, 0, 2)      # a view of the upright frame's size
         forced = self.previous_image is None or d < 0       # no previous frame of this size
         run_det = self._cadence.step(forced) and (forced or d > self.diff_thres)
         self.last_ran_detector = run_det
@@ -295,16 +304,22 @@ class FaceAna():
             return True
         return bool(d > self.diff_thres)
 
-    def _frame_diff(self, image, layout="bgr"):
-        """Stages `image` (a CUDA frame in layout `layout`) on the device as BGR and returns the mean |prev - cur|
-        against the previous staged frame, or a negative number when that frame has another size (or there is none)."""
+    def _frame_diff(self, image, layout="bgr", turns=0):
+        """Stages `image` (a CUDA frame in layout `layout`, stored `turns` quarter turns clockwise from upright) on the
+        device as upright BGR and returns the mean |prev - cur| against the previous staged frame, or a negative number
+        when that frame has another size (or there is none)."""
         d = C.c_double(0.0)
         if is_cuda_tensor(image):
             import torch
             f = check_cuda_frame(image, self._device, self._max_hw, layout)
-            rt.check(self.lib.skps_pipeline_frame_diff_device_layout(
-                self._pipe, image.data_ptr(), f.H, f.W, f.pitch, f.code, f.plane,
-                torch.cuda.current_stream(self._device).cuda_stream, C.byref(d), self._stream.cuda_stream))
+            if turns:
+                rt.check(self.lib.skps_pipeline_frame_diff_device_rotate(
+                    self._pipe, image.data_ptr(), f.H, f.W, f.pitch, f.code, f.plane, turns,
+                    torch.cuda.current_stream(self._device).cuda_stream, C.byref(d), self._stream.cuda_stream))
+            else:
+                rt.check(self.lib.skps_pipeline_frame_diff_device_layout(
+                    self._pipe, image.data_ptr(), f.H, f.W, f.pitch, f.code, f.plane,
+                    torch.cuda.current_stream(self._device).cuda_stream, C.byref(d), self._stream.cuda_stream))
         else:
             rt.check(self.lib.skps_pipeline_frame_diff(self._pipe, image.ctypes.data, *image.shape[:2], C.byref(d),
                                                        self._stream.cuda_stream))

@@ -98,12 +98,13 @@ class FaceAnaImages:
         self._next = 0
 
     # ------------------------------------------------------------------
-    def run_batch(self, images, layout="bgr"):
+    def run_batch(self, images, layout="bgr", rotate=0):
         """FaceAna.run after reset() for every image (blocking): one list of {'box', 'kps', 'scores'[, 'chip', 'M']
-        [, 'pose']} per image, [] for an image without a face.  See submit() for what images and layout may be."""
+        [, 'pose']} per image, [] for an image without a face.  See submit() for what images, layout and rotate may
+        be."""
         if self._pending:
             raise RuntimeError("FaceAnaImages: %d calls in flight; collect() them first" % len(self._pending))
-        self.submit(images, layout=layout)
+        self.submit(images, layout=layout, rotate=rotate)
         return self.collect()
 
     def new_results(self, n_images):
@@ -116,7 +117,7 @@ class FaceAnaImages:
         rt.require_cuda()
         return new_buffers(result_fields(int(n_images), self.top_k, self.n_points, self.pose, self.align), self.device)
 
-    def submit(self, images, out=None, layout="bgr"):
+    def submit(self, images, out=None, layout="bgr", rotate=0):
         """Enqueue the analysis of images; at most two calls may be in flight and collect() returns them in submission
         order.  Everything is checked before anything is enqueued.  submit() returns once the call's landmark phase is
         enqueued: the face counts are read back once on the way, so it waits for the call's detector phase.
@@ -133,6 +134,10 @@ class FaceAnaImages:
         "rgb", "bgra", "rgba" (H, W, 4), "bgr_planar" or "rgb_planar" (3, H, W).  Letterbox, crops and chips read them in
         place, and the results are, bit for bit, those of the same pixels passed as interleaved BGR.  Host images are
         BGR only.
+        rotate: the clockwise angle in degrees (0, 90, 180 or 270) by which CUDA images, as stored, must be turned to be
+        upright (device_frames.check_rotate), one for the call or one per image (a photo's EXIF orientation, which GPU
+        JPEG decoders do not apply).  They are read in place, and every result, pose included, is in the upright
+        image's pixels, bit for bit that of the upright image passed as a contiguous tensor.  Host images take 0.
 
         With align, CUDA images are warped into chips right after the landmarks, with no host synchronisation.  Host
         images are warped at collect(): M comes back with the other results, and only the rectangle of an image each
@@ -141,7 +146,7 @@ class FaceAnaImages:
         if len(self._pending) == 2:
             raise RuntimeError("FaceAnaImages: two calls already in flight; call collect() first")
         fd, fl = self.detector, self.landmark
-        call = check_frames(images, self.device, layout)
+        call = check_frames(images, self.device, layout, rotate)
         layout = fd._layout(call)
         n = len(call.frames)
         if out is not None:
@@ -209,7 +214,7 @@ class FaceAnaImages:
         st["staged"].synchronize()                    # the slot's last upload has left the pinned map
         hmap = st["hmap"].numpy()
         hmap[:n], hmap[n:2 * n], hmap[2 * n:2 * n + F] = first, counts, face_image
-        hw = np.array([shape[:2] for shape in call.shapes], np.int32)
+        hw = np.array(call.upright, np.int32).reshape(-1, 2)
         hmap[2 * n + F:m].reshape(F, 2)[:] = hw[face_image]
         dmap = st["map"]
         with torch.cuda.stream(ls):

@@ -3,19 +3,24 @@ allocation of result buffers given as {name: (shape, dtype name)}, and the growa
 descriptors and host pixels with one copy."""
 import collections
 
-from .device_frames import FrameLayout, check_cuda_frame, check_host_frame, check_layout, is_cuda_tensor, is_tensor
+from .device_frames import (FrameLayout, check_cuda_frame, check_host_frame, check_layout, check_rotate, is_cuda_tensor,
+                            is_tensor, upright_hw)
 
 MAX_SIDE = 1 << 20         # largest frame side a call takes: keeps every row pitch and crop coordinate in int32
 
-Frames = collections.namedtuple("Frames", "frames shapes cuda")
+Frames = collections.namedtuple("Frames", "frames shapes cuda turns", defaults=(None,))
 Frames.__doc__ = """A call's checked frames: the frames (host frames C-contiguous), the FrameLayout of each (H, W, row
-pitch and plane pitch in bytes, layout code; host frames are packed BGR) and whether they are CUDA tensors."""
+pitch and plane pitch in bytes, layout code, all as stored; host frames are packed BGR), whether they are CUDA tensors,
+and the quarter turns clockwise that make each upright (check_rotate; Frames.upright gives the upright sizes)."""
+Frames.upright = property(lambda self: [upright_hw(f.H, f.W, t) for f, t in zip(self.shapes, self.turns)])
+Frames.turned = property(lambda self: any(self.turns))
 
 
-def check_frames(frames, device, layout="bgr"):
+def check_frames(frames, device, layout="bgr", rotate=0):
     """Frames of a call, checked before anything is enqueued: all HxWx3 uint8 BGR numpy arrays, or all torch.uint8 CUDA
-    tensors on `device` in layout `layout` that check_cuda_frame takes, with sides in 1..MAX_SIDE.  ValueError otherwise,
-    for a mix of the two, and for a layout other than "bgr" with host frames."""
+    tensors on `device` in layout `layout` that check_cuda_frame takes, with sides in 1..MAX_SIDE, stored turned by
+    rotate= (check_rotate: one angle for the call or one per frame).  ValueError otherwise, for a mix of the two, for a
+    layout other than "bgr" and for a turn with host frames."""
     frames = list(frames)
     on_dev = [is_cuda_tensor(f) for f in frames]
     cuda = bool(on_dev) and all(on_dev)
@@ -23,6 +28,7 @@ def check_frames(frames, device, layout="bgr"):
         raise ValueError("one call takes either host frames or CUDA frames, got both (frames %s are CUDA)"
                          % [i for i, d in enumerate(on_dev) if d])
     check_layout(layout, cuda or not frames)
+    turns = check_rotate(rotate, len(frames), cuda or not frames)
     if cuda:
         shapes = [check_cuda_frame(f, device, (MAX_SIDE, MAX_SIDE), layout) for f in frames]
     else:
@@ -31,7 +37,7 @@ def check_frames(frames, device, layout="bgr"):
     for H, W, *_ in shapes:
         if not (0 < H <= MAX_SIDE and 0 < W <= MAX_SIDE):
             raise ValueError("frame %dx%d: sides must be in 1..%d" % (H, W, MAX_SIDE))
-    return Frames(frames, shapes, cuda)
+    return Frames(frames, shapes, cuda, turns)
 
 
 def new_buffers(fields, device):

@@ -31,7 +31,7 @@ import numpy as np
 from ... import runtime as rt
 from ...graph_tools import check_detector_input, detector_onnx_for
 from .align import check_size
-from .device_frames import check_cuda_frame, check_host_frame, check_layout, is_cuda_tensor
+from .device_frames import check_cuda_frame, check_host_frame, check_layout, check_rotate, is_cuda_tensor
 from .facer import check_detect_every, check_id_memory, get_cfg, pipeline_cfg
 from .onnx_model_base import ONNXEngine
 
@@ -155,7 +155,7 @@ class FaceAnaStreams:
             self.collect()
         rt.check(self.lib.skps_mpipe_reset(self._h, -1 if stream is None else int(stream)))
 
-    def submit(self, frames, out=None, streams=None, layout="bgr"):
+    def submit(self, frames, out=None, streams=None, layout="bgr", rotate=0):
         """Enqueue one frame for each of some streams.  At most two batches may be pending; results come back from
         collect() in submission order.
 
@@ -179,6 +179,13 @@ class FaceAnaStreams:
         passed as interleaved BGR, and the gate, detect_every, track ids and smoothing do not see the layout: calls may
         change it.  Host frames are BGR only.
 
+        rotate: the clockwise angle in degrees (0, 90, 180 or 270) by which CUDA frames, as stored, must be turned to be
+        upright (device_frames.check_rotate), one for the call or one per frame, so cameras mounted differently are fed
+        in one call.  The gathering kernel puts each frame into the ring upright, and the results are in the upright
+        frame's pixels, bit for bit those of the upright frames passed as contiguous tensors.  A stream sees the upright
+        frame: a change between 0 and 90 changes its frame size (the next frame runs the detector), one between 0 and
+        180 does not.  Host frames take 0.
+
         out: None (collect() returns host results), or, with CUDA frames, a dict from new_results() not used by a batch
         still in flight: the batch's results are written into it on the GPU and nothing is copied to the host."""
         if len(self._pending) == 2:
@@ -190,11 +197,12 @@ class FaceAnaStreams:
         smap = None if ids is None else np.array(ids, np.int32)
         on_device = [is_cuda_tensor(f) for f in frames]
         check_layout(layout, any(on_device))
+        turns = check_rotate(rotate, n, any(on_device))
         if any(on_device):
             if not all(on_device):
                 raise ValueError("one batch takes either host frames or CUDA frames, got both (streams %s are CUDA)"
                                  % [i for i, d in enumerate(on_device) if d])
-            self._submit_device(frames, out, smap, layout)
+            self._submit_device(frames, out, smap, layout, turns)
             return
         if out is not None:
             raise ValueError("out= keeps results on the GPU and takes CUDA frames; these are host frames")
@@ -207,7 +215,7 @@ class FaceAnaStreams:
         self._pending.append((slot, n, keep, None))
         self._next ^= 1
 
-    def _submit_device(self, frames, out, smap, layout):
+    def _submit_device(self, frames, out, smap, layout, turns):
         import torch
         n = len(frames)
         shapes = [check_cuda_frame(f, self.device, self.max_frame_hw, layout) for f in frames]
@@ -225,9 +233,11 @@ class FaceAnaStreams:
         planes = np.array([f.plane for f in shapes], np.int32)
         hw = np.array([[f.H, f.W] for f in shapes], np.int32)
         slot = self._next
-        rt.check(self.lib.skps_mpipe_submit_device_layout(self._h, slot, None if smap is None else smap.ctypes.data, ptrs,
+        q = np.array(turns, np.int32)                 # as stored: hw, pitches; the ring gets them upright
+        rt.check(self.lib.skps_mpipe_submit_device_rotate(self._h, slot, None if smap is None else smap.ctypes.data, ptrs,
                                                           pitches.ctypes.data, hw.ctypes.data, n, shapes[0].code,
-                                                          planes.ctypes.data, None if outs is None else C.byref(outs),
+                                                          planes.ctypes.data, q.ctypes.data if any(turns) else None,
+                                                          None if outs is None else C.byref(outs),
                                                           torch.cuda.current_stream(self.device).cuda_stream))
         self._pending.append((slot, n, list(frames), out))
         self._next ^= 1
@@ -319,8 +329,8 @@ class FaceAnaStreams:
                     r['id'] = int(o["ids"][s, i])
         return res
 
-    def run(self, frames, streams=None, layout="bgr"):
-        """One frame for each of some streams in (submit's streams= and layout=), their results out in call order
-        (blocking)."""
-        self.submit(frames, streams=streams, layout=layout)
+    def run(self, frames, streams=None, layout="bgr", rotate=0):
+        """One frame for each of some streams in (submit's streams=, layout= and rotate=), their results out in call
+        order (blocking)."""
+        self.submit(frames, streams=streams, layout=layout, rotate=rotate)
         return self.collect()

@@ -91,6 +91,8 @@ struct WarpArgs {
     const int* count; int per_group;            // face f = g * per_group + i is skipped when count && i >= count[g]
     int out_h, out_w;
     uint8_t* out;                               // [faces][out_h][out_w][3]
+    const int* turns;                           // with src: group g's image is stored turned turns[g] quarter turns
+                                                // clockwise (align_warp_turned_kernel only)
 };
 
 // One thread per face: M[f] from the landmarks kps[f] (P x 2).
@@ -131,7 +133,10 @@ __global__ void __launch_bounds__(128) det_align_estimate_kernel(const float* __
 
 // A block warps 256 consecutive pixels of one chip: each thread finds its pixel's four taps and weights once and blends the
 // three channels into shared memory, then the block stores the 768 bytes with consecutive threads on consecutive bytes.
-__global__ void __launch_bounds__(256) align_warp_kernel(const WarpArgs a) {
+// TURNED: a source image is stored turned a.turns[g] quarter turns clockwise, read through px_view as the upright image; a
+// turned image is read whole, one of turn 0 may be a rectangle as without TURNED.
+template <bool TURNED>
+__device__ __forceinline__ void warp_chip(const WarpArgs& a) {
     const int f = blockIdx.y;
     const int g = f / a.per_group, i = f - g * a.per_group;
     if (a.count && i >= a.count[g]) return;
@@ -143,6 +148,7 @@ __global__ void __launch_bounds__(256) align_warp_kernel(const WarpArgs a) {
         const uint8_t* base = a.frame;
         int H = a.H, W = a.W, pitch = a.pitch, ox = 0, oy = 0, rw = a.W, rh = a.H;
         PxLayout lay = px_layout(SKPS_LAYOUT_BGR, 0);
+        PxView v;
         if (a.desc) {
             const MpStreamDesc& d = a.desc[g];
             base = d.cur; H = d.H; W = d.W; pitch = d.W * 3; rw = W; rh = H;
@@ -150,6 +156,13 @@ __global__ void __launch_bounds__(256) align_warp_kernel(const WarpArgs a) {
             const skps_face_src& s = a.src[g];
             base = s.base; H = s.H; W = s.W; pitch = s.pitch; ox = s.ox; oy = s.oy; rw = s.rw; rh = s.rh;
             if (a.lay) lay = px_layout(a.lay[g].layout, a.lay[g].plane_pitch);
+        }
+        if constexpr (TURNED) {
+            const skps_frame_layout L = a.src && a.lay ? a.lay[g] : skps_frame_layout{SKPS_LAYOUT_BGR, 0};
+            const int t = a.src ? a.turns[g] & 3 : 0;
+            v = px_view(L.layout, L.plane_pitch, pitch, H, W, t);
+            if (t) { H = v.H; W = v.W; ox = oy = 0; rw = W; rh = H; }
+            else v.org = -((long long)oy * pitch + (long long)ox * v.xstep);
         }
         const int xa = max(ox, 0), xb = min(ox + rw, W), ya = max(oy, 0), yb = min(oy + rh, H);
         // the inverse map as warpAffine computes it (imgwarp.cpp), same order of operations; every thread of the face
@@ -175,17 +188,31 @@ __global__ void __launch_bounds__(256) align_warp_kernel(const WarpArgs a) {
         // taps outside the frame read the border value 0; so do taps outside the rectangle, which are never dereferenced
         const bool x0 = sx >= xa && sx < xb, x1 = sx + 1 >= xa && sx + 1 < xb;
         const bool y0 = sy >= ya && sy < yb, y1 = sy + 1 >= ya && sy + 1 < yb;
-        const uint8_t* r0 = base + (ptrdiff_t)(sy - oy) * pitch + (ptrdiff_t)(sx - ox) * lay.xs;   // dereferenced only where inside
-        const uint8_t* r1 = r0 + pitch;
-        const int xs = lay.xs;
+        if constexpr (TURNED) {
+            const uint8_t* r0 = base + v.org + (long long)sy * v.ystep + (long long)sx * v.xstep;   // dereferenced only where inside
+            const uint8_t* r1 = r0 + v.ystep;
+            const long long xs = v.xstep;
 #pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            const uint8_t* p0 = r0 + lay.off[c];
-            const uint8_t* p1 = r1 + lay.off[c];
-            const int acc = (y0 && x0 ? (int)__ldg(p0) : 0) * w00 + (y0 && x1 ? (int)__ldg(p0 + xs) : 0) * w01 +
-                            (y1 && x0 ? (int)__ldg(p1) : 0) * w10 + (y1 && x1 ? (int)__ldg(p1 + xs) : 0) * w11;
-            // weights * 32 sum to 2^15: (sum * 32 + 2^14) >> 15 == (sum + 2^9) >> 10; at most 255
-            px[threadIdx.x * 3 + c] = (uint8_t)min((acc + 512) >> 10, 255);
+            for (int c = 0; c < 3; ++c) {
+                const uint8_t* p0 = r0 + v.off[c];
+                const uint8_t* p1 = r1 + v.off[c];
+                const int acc = (y0 && x0 ? (int)__ldg(p0) : 0) * w00 + (y0 && x1 ? (int)__ldg(p0 + xs) : 0) * w01 +
+                                (y1 && x0 ? (int)__ldg(p1) : 0) * w10 + (y1 && x1 ? (int)__ldg(p1 + xs) : 0) * w11;
+                px[threadIdx.x * 3 + c] = (uint8_t)min((acc + 512) >> 10, 255);
+            }
+        } else {
+            const uint8_t* r0 = base + (ptrdiff_t)(sy - oy) * pitch + (ptrdiff_t)(sx - ox) * lay.xs;   // dereferenced only where inside
+            const uint8_t* r1 = r0 + pitch;
+            const int xs = lay.xs;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const uint8_t* p0 = r0 + lay.off[c];
+                const uint8_t* p1 = r1 + lay.off[c];
+                const int acc = (y0 && x0 ? (int)__ldg(p0) : 0) * w00 + (y0 && x1 ? (int)__ldg(p0 + xs) : 0) * w01 +
+                                (y1 && x0 ? (int)__ldg(p1) : 0) * w10 + (y1 && x1 ? (int)__ldg(p1 + xs) : 0) * w11;
+                // weights * 32 sum to 2^15: (sum * 32 + 2^14) >> 15 == (sum + 2^9) >> 10; at most 255
+                px[threadIdx.x * 3 + c] = (uint8_t)min((acc + 512) >> 10, 255);
+            }
         }
     }
     __syncthreads();
@@ -193,10 +220,14 @@ __global__ void __launch_bounds__(256) align_warp_kernel(const WarpArgs a) {
     uint8_t* out = a.out + (size_t)f * pixels * 3 + first;
     for (int j = threadIdx.x; j < n; j += 256) out[j] = px[j];
 }
+__global__ void __launch_bounds__(256) align_warp_kernel(const WarpArgs a) { warp_chip<false>(a); }
+__global__ void __launch_bounds__(256) align_warp_turned_kernel(const WarpArgs a) { warp_chip<true>(a); }
 
 int launch_warp(const WarpArgs& a, int faces, cudaStream_t s) {
     const int pixels = a.out_w * a.out_h;
-    align_warp_kernel<<<dim3((pixels + 255) / 256, faces), 256, 0, s>>>(a);
+    const dim3 grid((pixels + 255) / 256, faces);
+    if (a.src && a.turns) align_warp_turned_kernel<<<grid, 256, 0, s>>>(a);
+    else align_warp_kernel<<<grid, 256, 0, s>>>(a);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }
@@ -244,8 +275,8 @@ extern "C" SKPS_API int skps_align_faces(const uint8_t* frame, int H, int W, int
     return launch_align(frame, H, W, pitch, nullptr, kps, P, count, n, n, size, chips, M, (cudaStream_t)stream);
 }
 
-extern "C" SKPS_API int skps_warp_faces_layout(const skps_face_src* src, const skps_frame_layout* lay, const double* M, int n,
-                                               int out_h, int out_w, uint8_t* out, void* stream) {
+extern "C" SKPS_API int skps_warp_faces_rotate(const skps_face_src* src, const skps_frame_layout* lay, const int32_t* turns,
+                                               const double* M, int n, int out_h, int out_w, uint8_t* out, void* stream) {
     SKPS_CHECK(n >= 0 && out_h > 0 && out_w > 0 && out_h <= 4096 && out_w <= 4096,
                "warp_faces: n %d or output %dx%d out of range", n, out_h, out_w);
     if (n == 0) return 0;
@@ -255,15 +286,21 @@ extern "C" SKPS_API int skps_warp_faces_layout(const skps_face_src* src, const s
         const int m = min(65535, n - c0);
         WarpArgs a = {};
         a.src = src + c0; a.lay = lay ? lay + c0 : nullptr; a.M = M + (size_t)c0 * 6; a.per_group = 1;   // a source per face
+        a.turns = turns ? turns + c0 : nullptr;
         a.out_h = out_h; a.out_w = out_w; a.out = out + (size_t)c0 * out_h * out_w * 3;
         if (launch_warp(a, m, (cudaStream_t)stream)) return 1;
     }
     return 0;
 }
 
-extern "C" SKPS_API int skps_warp_faces_count(const skps_face_src* src, const skps_frame_layout* lay, const int32_t* count,
-                                              int n_frames, int per_frame, const double* M, int out_h, int out_w,
-                                              uint8_t* out, void* stream) {
+extern "C" SKPS_API int skps_warp_faces_layout(const skps_face_src* src, const skps_frame_layout* lay, const double* M, int n,
+                                               int out_h, int out_w, uint8_t* out, void* stream) {
+    return skps_warp_faces_rotate(src, lay, nullptr, M, n, out_h, out_w, out, stream);
+}
+
+extern "C" SKPS_API int skps_warp_faces_count_rotate(const skps_face_src* src, const skps_frame_layout* lay,
+                                                     const int32_t* turns, const int32_t* count, int n_frames, int per_frame,
+                                                     const double* M, int out_h, int out_w, uint8_t* out, void* stream) {
     SKPS_CHECK(n_frames >= 0 && per_frame > 0 && per_frame <= 65535 && out_h > 0 && out_w > 0 && out_h <= 4096 &&
                out_w <= 4096, "warp_faces_count: n_frames %d, per_frame %d or output %dx%d out of range", n_frames,
                per_frame, out_h, out_w);
@@ -277,11 +314,18 @@ extern "C" SKPS_API int skps_warp_faces_count(const skps_face_src* src, const sk
         const size_t f0 = (size_t)g0 * per_frame;
         WarpArgs a = {};
         a.src = src + g0; a.lay = lay ? lay + g0 : nullptr; a.M = M + f0 * 6;
+        a.turns = turns ? turns + g0 : nullptr;
         a.count = count + g0; a.per_group = per_frame;
         a.out_h = out_h; a.out_w = out_w; a.out = out + f0 * chip;
         if (launch_warp(a, m * per_frame, (cudaStream_t)stream)) return 1;
     }
     return 0;
+}
+
+extern "C" SKPS_API int skps_warp_faces_count(const skps_face_src* src, const skps_frame_layout* lay, const int32_t* count,
+                                              int n_frames, int per_frame, const double* M, int out_h, int out_w,
+                                              uint8_t* out, void* stream) {
+    return skps_warp_faces_count_rotate(src, lay, nullptr, count, n_frames, per_frame, M, out_h, out_w, out, stream);
 }
 
 extern "C" SKPS_API int skps_warp_faces(const skps_face_src* src, const double* M, int n, int out_h, int out_w, uint8_t* out,

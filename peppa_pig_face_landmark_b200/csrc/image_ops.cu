@@ -92,6 +92,42 @@ __global__ void __launch_bounds__(256) letterbox_frames_kernel(const LetterboxAr
                  blockIdx.x * blockDim.x + threadIdx.x, blockIdx.y);
 }
 
+// letterbox_px of a frame read through the view v (px_view), H x W being the upright frame's size; row_pairs frames are read
+// with a view of no turn.  The same taps and blend: only the addresses differ.
+__device__ __forceinline__ void letterbox_turned_px(const uint8_t* __restrict__ frame, int H, int W, int row_pairs,
+                                                    const PxView& v, uint8_t* __restrict__ out, int in_h, int in_w, int rw,
+                                                    int rh, int top, int left, int x, int y) {
+    if (x >= in_w) return;
+    uint8_t* o = out + ((long long)y * in_w + x) * 3;
+    int dx = x - left, dy = y - top;
+    if (dx < 0 || dx >= rw || dy < 0 || dy >= rh) {
+        o[0] = 114; o[1] = 114; o[2] = 114;
+        return;
+    }
+    Tap tx = linear_tap(dx, rw, W, true);
+    Tap ty = linear_tap(dy, rh, H, false);
+    const uint8_t* r0 = frame + v.org + (long long)(row_pairs ? 2 * dy : ty.i0) * v.ystep;
+    const uint8_t* r1 = frame + v.org + (long long)(row_pairs ? 2 * dy + 1 : ty.i1) * v.ystep;
+    const long long x0 = tx.i0 * v.xstep, x1 = tx.i1 * v.xstep;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const uint8_t* a = r0 + v.off[c];
+        const uint8_t* b = r1 + v.off[c];
+        int h0 = a[x0] * tx.w0 + a[x1] * tx.w1;
+        int h1 = b[x0] * tx.w0 + b[x1] * tx.w1;
+        o[2 - c] = (uint8_t)vblend(h0, h1, ty.w0, ty.w1);      // BGR -> RGB
+    }
+}
+// block z = frame a.src[z], stored turned a.turns[z] quarter turns clockwise (skps_letterbox_frames_rotate); its geometry
+// is that of the upright frame
+__global__ void __launch_bounds__(256) letterbox_turned_kernel(const LetterboxArgs a) {
+    const skps_det_src F = a.src[blockIdx.z];
+    const skps_frame_layout L = a.lay ? a.lay[blockIdx.z] : skps_frame_layout{SKPS_LAYOUT_BGR, 0};
+    const PxView v = px_view(L.layout, L.plane_pitch, F.pitch, F.H, F.W, F.row_pairs ? 0 : a.turns[blockIdx.z]);
+    letterbox_turned_px(F.base, v.H, v.W, F.row_pairs, v, a.out + a.out_stride * blockIdx.z, a.in_h, a.in_w, F.rw, F.rh,
+                        F.top, F.left, blockIdx.x * blockDim.x + threadIdx.x, blockIdx.y);
+}
+
 // ------------------------------------------------------------------------------------------
 // Per-face crop + resize (face_landmark.py:74-98).  Geometry in float32 exactly as numpy>=2
 // evaluates it; the zero border of copyMakeBorder is virtual.
@@ -155,6 +191,37 @@ __device__ __forceinline__ void crop_face_px(const uint8_t* __restrict__ base, i
     }
 }
 
+// crop_face_px of a frame read through the view v (px_view), H x W being the upright frame's size.  The same geometry, taps
+// and blend: only the addresses differ.
+__device__ __forceinline__ void crop_face_turned_px(const uint8_t* __restrict__ base, int H, int W, const PxView& v,
+                                                    const float* __restrict__ b, float face_scale, float min_face,
+                                                    uint8_t* __restrict__ o, int S, int* __restrict__ d, int x, int y) {
+    CropGeo g = crop_geometry(b, H, W, face_scale, min_face);
+    if (x == 0 && y == 0) {
+        d[0] = g.h; d[1] = g.w; d[2] = g.y1; d[3] = g.x1; d[4] = g.add;
+    }
+    if (!g.ok) { o[0] = 0; o[1] = 0; o[2] = 0; return; }
+    Tap tx = linear_tap(x, S, g.w, true);
+    Tap ty = linear_tap(y, S, g.h, false);
+    int fx0 = g.x1 + tx.i0 - g.add, fx1 = g.x1 + tx.i1 - g.add;
+    int fy0 = g.y1 + ty.i0 - g.add, fy1 = g.y1 + ty.i1 - g.add;
+    bool vx0 = fx0 >= 0 && fx0 < W, vx1 = fx1 >= 0 && fx1 < W;
+    bool vy0 = fy0 >= 0 && fy0 < H, vy1 = fy1 >= 0 && fy1 < H;
+    const uint8_t* r0 = base + v.org + (long long)(vy0 ? fy0 : 0) * v.ystep;
+    const uint8_t* r1 = base + v.org + (long long)(vy1 ? fy1 : 0) * v.ystep;
+    const long long x0 = (long long)(vx0 ? fx0 : 0) * v.xstep, x1 = (long long)(vx1 ? fx1 : 0) * v.xstep;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const uint8_t* a = r0 + v.off[c];
+        const uint8_t* e = r1 + v.off[c];
+        int p00 = (vy0 && vx0) ? a[x0] : 0, p01 = (vy0 && vx1) ? a[x1] : 0;
+        int p10 = (vy1 && vx0) ? e[x0] : 0, p11 = (vy1 && vx1) ? e[x1] : 0;
+        int h0 = p00 * tx.w0 + p01 * tx.w1;
+        int h1 = p10 * tx.w0 + p11 * tx.w1;
+        o[c] = (uint8_t)vblend(h0, h1, ty.w0, ty.w1);
+    }
+}
+
 __device__ __forceinline__ void crop_px(const uint8_t* __restrict__ frame, int H, int W, int pitch,
                                         const float* __restrict__ boxes, const int* __restrict__ count, float face_scale,
                                         float min_face, uint8_t* __restrict__ crops, int S, int* __restrict__ detail,
@@ -195,6 +262,24 @@ __global__ void __launch_bounds__(256) crop_faces_kernel(const skps_face_src* __
     const PxLayout L = lay ? px_layout(lay[face].layout, lay[face].plane_pitch) : px_layout(SKPS_LAYOUT_BGR, 0);
     crop_face_px(F.base, F.H, F.W, F.pitch, F.ox, F.oy, L, boxes + face * 4, face_scale, min_face,
                  crops + (((long long)face * S + y) * S + x) * 3, S, detail + face * 5, x, y);
+}
+// crop_faces_kernel for faces whose frames are stored turned turns[face] quarter turns clockwise (skps_crop_faces_rotate):
+// the boxes are in the upright frame.  A turned frame is read whole; one of turn 0 may be a rectangle, as above.
+__global__ void __launch_bounds__(256) crop_faces_turned_kernel(const skps_face_src* __restrict__ src,
+                                                                const skps_frame_layout* __restrict__ lay,
+                                                                const int* __restrict__ turns,
+                                                                const float* __restrict__ boxes, float face_scale,
+                                                                float min_face, uint8_t* __restrict__ crops, int S,
+                                                                int* __restrict__ detail) {
+    const int face = blockIdx.z, x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+    if (x >= S) return;
+    const skps_face_src F = src[face];
+    const skps_frame_layout L = lay ? lay[face] : skps_frame_layout{SKPS_LAYOUT_BGR, 0};
+    const int t = turns[face] & 3;
+    PxView v = px_view(L.layout, L.plane_pitch, F.pitch, F.H, F.W, t);
+    if (t == 0) v.org = -((long long)F.oy * F.pitch + (long long)F.ox * v.xstep);
+    crop_face_turned_px(F.base, v.H, v.W, v, boxes + face * 4, face_scale, min_face,
+                        crops + (((long long)face * S + y) * S + x) * 3, S, detail + face * 5, x, y);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -703,25 +788,106 @@ __global__ void __launch_bounds__(256) diff_frames_kernel(const MpStreamDesc* __
     }
 }
 
+// Ingest of one frame stored turned: cur gets the D.H x D.W upright frame (px_view of the stored frame, turned `turns`
+// quarter turns clockwise), as packed BGR.  The upright frame is cut into 32 x 32 pixel tiles staged through shared memory:
+// the tile is gathered with consecutive threads on consecutive stored pixels (down an upright column for odd turns, along an
+// upright row otherwise), then its upright rows are stored with consecutive threads on consecutive bytes, whatever their
+// alignment.  Returns this thread's part of sum |cur - prev|, the same integer sum as for the upright frame passed as it is.
+constexpr int TURN_TILE = 32;
+template <int L>
+__device__ __forceinline__ unsigned long long ingest_turned(const MpStreamDesc& D, int turns) {
+    __shared__ uint8_t tile[TURN_TILE][TURN_TILE * 3 + 4];       // rows 100 bytes apart: a gathered column hits 32 banks
+    const int Hs = (turns & 1) ? D.W : D.H, Ws = (turns & 1) ? D.H : D.W;
+    const PxView v = px_view(L, D.src_plane, D.src_pitch, Hs, Ws, turns);
+    const uint8_t* __restrict__ src = D.src;
+    uint8_t* __restrict__ cur = D.cur;
+    const uint8_t* __restrict__ prev = D.have_prev ? D.prev : nullptr;
+    const bool down = turns & 1;
+    const int tiles_x = (D.W + TURN_TILE - 1) / TURN_TILE, tiles = tiles_x * ((D.H + TURN_TILE - 1) / TURN_TILE);
+    unsigned long long local = 0;
+    for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+        const int y0 = t / tiles_x * TURN_TILE, x0 = (t % tiles_x) * TURN_TILE;
+        const int ny = min(TURN_TILE, D.H - y0), nx = min(TURN_TILE, D.W - x0);
+        for (int i = threadIdx.x; i < TURN_TILE * TURN_TILE; i += blockDim.x) {
+            const int a = i % TURN_TILE, b = i / TURN_TILE, yy = down ? a : b, xx = down ? b : a;
+            if (yy < ny && xx < nx) {
+                const uint8_t* px = src + v.org + (long long)(y0 + yy) * v.ystep + (long long)(x0 + xx) * v.xstep;
+#pragma unroll
+                for (int c = 0; c < 3; ++c) tile[yy][3 * xx + c] = px[v.off[c]];
+            }
+        }
+        __syncthreads();
+        const int row = 3 * nx;
+        for (int i = threadIdx.x; i < ny * row; i += blockDim.x) {
+            const int yy = i / row, b = i - yy * row;
+            const size_t o = ((size_t)(y0 + yy) * D.W + x0) * 3 + b;
+            const uint8_t val = tile[yy][b];
+            cur[o] = val;
+            if (prev) {
+                const int dd = (int)val - (int)prev[o];
+                local += (unsigned)(dd < 0 ? -dd : dd);
+            }
+        }
+        __syncthreads();
+    }
+    return local;
+}
+
+// sum[g] += the block's `local`s, as diff_frames_kernel adds them (integer sums: the order of the atomic adds does not matter)
+__device__ __forceinline__ void block_sum_add(unsigned long long local, unsigned long long* sum) {
+    for (int o = 16; o > 0; o >>= 1) local += __shfl_down_sync(0xffffffffu, local, o);
+    __shared__ unsigned long long warp_sum[8];
+    if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = local;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        unsigned long long t = 0;
+        for (int w = 0; w < 8; ++w) t += warp_sum[w];
+        atomicAdd(sum, t);
+    }
+}
+
+// diff_frames_kernel for launches holding a turned frame: frame g's src is turned turns[g] (d set) or one_turns quarter
+// turns clockwise, 0 included
+template <int L>
+__global__ void __launch_bounds__(256) diff_frames_turned_kernel(const MpStreamDesc* __restrict__ d, MpStreamDesc one,
+                                                                 size_t one_bytes, const int* __restrict__ turns,
+                                                                 int one_turns, unsigned long long* __restrict__ sum) {
+    const MpStreamDesc D = d ? d[blockIdx.y] : one;
+    const size_t n = d ? (size_t)D.H * D.W * 3 : one_bytes;
+    if (!D.have_prev && !D.src) return;
+    const unsigned long long local = D.src ? ingest_turned<L>(D, (d ? turns[blockIdx.y] : one_turns) & 3)
+                                           : absdiff_bytes(D.prev, D.cur, n);
+    block_sum_add(local, sum + blockIdx.y);
+}
+
+template <int L>
+static void launch_diff(dim3 grid, cudaStream_t s, const MpStreamDesc* d, const MpStreamDesc& one, size_t bytes,
+                        unsigned long long* sum, bool turned, const int* turns, int one_turns) {
+    if (turned) diff_frames_turned_kernel<L><<<grid, 256, 0, s>>>(d, one, bytes, turns, one_turns, sum);
+    else diff_frames_kernel<L><<<grid, 256, 0, s>>>(d, one, bytes, sum);
+}
+
 int launch_frame_diff(const MpStreamDesc* d, int n, const MpStreamDesc& one, size_t bytes, unsigned long long* sum,
-                      cudaStream_t s, int layout) {
+                      cudaStream_t s, int layout, const int* turns, int one_turns) {
     // ingest_units counts the 16-byte units of a frame in 32 bits, ingest_pixels its packed bytes
     SKPS_CHECK(bytes < (1ull << 32) - 16 || !(d || one.src), "frame_diff: a %zu-byte frame is larger than 4 GB", bytes);
     SKPS_CHECK(layout_ok(layout), "frame_diff: unknown pixel layout %d", layout);
-    // a unit per thread (16 bytes; 16 pixels for the other layouts), at most 8 blocks per SM per frame
-    const size_t units = layout == SKPS_LAYOUT_BGR ? bytes / 16 : bytes / 48;
+    const bool turned = d ? turns != nullptr : one_turns != 0;
+    // a unit per thread (16 bytes; 16 pixels for the other layouts; a 32 x 32 tile per block when turned), at most 8
+    // blocks per SM per frame
+    const size_t units = turned ? bytes / 3072 * 256 : layout == SKPS_LAYOUT_BGR ? bytes / 16 : bytes / 48;
     size_t blocks = (units + 255) / 256;
     if (blocks > (size_t)sm_count() * 8) blocks = (size_t)sm_count() * 8;
     if (blocks < 1) blocks = 1;
     const dim3 grid((unsigned)blocks, n);
     switch (layout) {
-        case SKPS_LAYOUT_BGR: diff_frames_kernel<SKPS_LAYOUT_BGR><<<grid, 256, 0, s>>>(d, one, bytes, sum); break;
-        case SKPS_LAYOUT_RGB: diff_frames_kernel<SKPS_LAYOUT_RGB><<<grid, 256, 0, s>>>(d, one, bytes, sum); break;
-        case SKPS_LAYOUT_BGRA: diff_frames_kernel<SKPS_LAYOUT_BGRA><<<grid, 256, 0, s>>>(d, one, bytes, sum); break;
-        case SKPS_LAYOUT_RGBA: diff_frames_kernel<SKPS_LAYOUT_RGBA><<<grid, 256, 0, s>>>(d, one, bytes, sum); break;
+        case SKPS_LAYOUT_BGR: launch_diff<SKPS_LAYOUT_BGR>(grid, s, d, one, bytes, sum, turned, turns, one_turns); break;
+        case SKPS_LAYOUT_RGB: launch_diff<SKPS_LAYOUT_RGB>(grid, s, d, one, bytes, sum, turned, turns, one_turns); break;
+        case SKPS_LAYOUT_BGRA: launch_diff<SKPS_LAYOUT_BGRA>(grid, s, d, one, bytes, sum, turned, turns, one_turns); break;
+        case SKPS_LAYOUT_RGBA: launch_diff<SKPS_LAYOUT_RGBA>(grid, s, d, one, bytes, sum, turned, turns, one_turns); break;
         case SKPS_LAYOUT_BGR_PLANAR:
-            diff_frames_kernel<SKPS_LAYOUT_BGR_PLANAR><<<grid, 256, 0, s>>>(d, one, bytes, sum); break;
-        default: diff_frames_kernel<SKPS_LAYOUT_RGB_PLANAR><<<grid, 256, 0, s>>>(d, one, bytes, sum); break;
+            launch_diff<SKPS_LAYOUT_BGR_PLANAR>(grid, s, d, one, bytes, sum, turned, turns, one_turns); break;
+        default: launch_diff<SKPS_LAYOUT_RGB_PLANAR>(grid, s, d, one, bytes, sum, turned, turns, one_turns); break;
     }
     SKPS_CUDA(cudaGetLastError());
     return 0;
@@ -745,7 +911,9 @@ int check_device_frame(const void* frame, int device, const char* fn, int index)
     return 1;
 }
 int launch_letterbox(const LetterboxArgs& a, int n, cudaStream_t s) {
-    letterbox_frames_kernel<<<dim3((a.in_w + 255) / 256, a.in_h, n), 256, 0, s>>>(a);
+    const dim3 grid((a.in_w + 255) / 256, a.in_h, n);
+    if (a.src && a.turns) letterbox_turned_kernel<<<grid, 256, 0, s>>>(a);
+    else letterbox_frames_kernel<<<grid, 256, 0, s>>>(a);
     SKPS_CUDA(cudaGetLastError());
     return 0;
 }
@@ -782,15 +950,22 @@ extern "C" SKPS_API int skps_letterbox(const uint8_t* frame, int H, int W, int p
     return launch_letterbox(a, 1, (cudaStream_t)stream);
 }
 
-extern "C" SKPS_API int skps_letterbox_frames_layout(const skps_det_src* src, const skps_frame_layout* lay, int n,
-                                                     uint8_t* out, int in_h, int in_w, void* stream) {
+extern "C" SKPS_API int skps_letterbox_frames_rotate(const skps_det_src* src, const skps_frame_layout* lay,
+                                                     const int32_t* turns, int n, uint8_t* out, int in_h, int in_w,
+                                                     void* stream) {
     SKPS_CHECK(n >= 0 && n <= 65535 && in_h > 0 && in_h <= 65535 && in_w > 0,
                "letterbox_frames: n %d outside 0..65535 or input %dx%d", n, in_h, in_w);
     if (n == 0) return 0;
     SKPS_CHECK(src && out, "letterbox_frames: bad arguments");
     LetterboxArgs a = {};
-    a.src = src; a.lay = lay; a.out = out; a.out_stride = (size_t)in_h * in_w * 3; a.in_h = in_h; a.in_w = in_w;
+    a.src = src; a.lay = lay; a.turns = turns; a.out = out; a.out_stride = (size_t)in_h * in_w * 3; a.in_h = in_h;
+    a.in_w = in_w;
     return launch_letterbox(a, n, (cudaStream_t)stream);
+}
+
+extern "C" SKPS_API int skps_letterbox_frames_layout(const skps_det_src* src, const skps_frame_layout* lay, int n,
+                                                     uint8_t* out, int in_h, int in_w, void* stream) {
+    return skps_letterbox_frames_rotate(src, lay, nullptr, n, out, in_h, in_w, stream);
 }
 
 extern "C" SKPS_API int skps_letterbox_frames(const skps_det_src* src, int n, uint8_t* out, int in_h, int in_w,
@@ -847,16 +1022,26 @@ extern "C" SKPS_API int skps_crop_resize(const uint8_t* frame, int H, int W, int
     return launch_crop(a, 1, (cudaStream_t)stream);
 }
 
-extern "C" SKPS_API int skps_crop_faces_layout(const skps_face_src* src, const skps_frame_layout* lay, const float* boxes4,
-                                               int n, float face_scale, float min_face, uint8_t* crops, int out_hw,
-                                               int32_t* detail, void* stream) {
+extern "C" SKPS_API int skps_crop_faces_rotate(const skps_face_src* src, const skps_frame_layout* lay, const int32_t* turns,
+                                               const float* boxes4, int n, float face_scale, float min_face, uint8_t* crops,
+                                               int out_hw, int32_t* detail, void* stream) {
     SKPS_CHECK(n >= 0 && n <= 65535 && out_hw > 0, "crop_faces: n %d outside 0..65535 or out_hw %d", n, out_hw);
     if (n == 0) return 0;
     SKPS_CHECK(src && boxes4 && crops && detail, "crop_faces: bad arguments");
     dim3 grid((out_hw + 255) / 256, out_hw, n);
-    crop_faces_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src, lay, boxes4, face_scale, min_face, crops, out_hw, detail);
+    if (turns)
+        crop_faces_turned_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src, lay, turns, boxes4, face_scale, min_face, crops,
+                                                                         out_hw, detail);
+    else
+        crop_faces_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src, lay, boxes4, face_scale, min_face, crops, out_hw, detail);
     SKPS_CUDA(cudaGetLastError());
     return 0;
+}
+
+extern "C" SKPS_API int skps_crop_faces_layout(const skps_face_src* src, const skps_frame_layout* lay, const float* boxes4,
+                                               int n, float face_scale, float min_face, uint8_t* crops, int out_hw,
+                                               int32_t* detail, void* stream) {
+    return skps_crop_faces_rotate(src, lay, nullptr, boxes4, n, face_scale, min_face, crops, out_hw, detail, stream);
 }
 
 extern "C" SKPS_API int skps_crop_faces(const skps_face_src* src, const float* boxes4, int n, float face_scale, float min_face,
@@ -898,17 +1083,25 @@ extern "C" SKPS_API int skps_frame_absdiff_sum(const uint8_t* a, const uint8_t* 
     return launch_frame_diff(nullptr, 1, D, n, sum, (cudaStream_t)stream);
 }
 
-extern "C" SKPS_API int skps_frame_ingest_layout(const uint8_t* frame, int H, int W, int pitch, int layout, int plane_pitch,
-                                                 uint8_t* packed, const uint8_t* prev, unsigned long long* sum, void* stream) {
+extern "C" SKPS_API int skps_frame_ingest_rotate(const uint8_t* frame, int H, int W, int pitch, int layout, int plane_pitch,
+                                                 int turns, uint8_t* packed, const uint8_t* prev, unsigned long long* sum,
+                                                 void* stream) {
     SKPS_CHECK(layout_ok(layout), "ingest: unknown pixel layout %d", layout);
+    SKPS_CHECK(turns >= 0 && turns <= 3, "ingest: turns %d outside 0..3", turns);
     SKPS_CHECK(frame && packed && sum && H > 0 && W > 0 && (H == 1 || pitch >= layout_xstep(layout) * W) &&
                (layout < SKPS_LAYOUT_BGR_PLANAR || plane_pitch >= 0), "ingest: bad arguments");
     SKPS_CHECK(((uintptr_t)packed % 16 == 0) && ((uintptr_t)prev % 16 == 0), "ingest: packed and prev must be 16-byte aligned");
     SKPS_CUDA(cudaMemsetAsync(sum, 0, sizeof(unsigned long long), (cudaStream_t)stream));
     MpStreamDesc D = {};
-    D.cur = packed; D.prev = prev; D.have_prev = prev != nullptr; D.H = H; D.W = W;
+    D.cur = packed; D.prev = prev; D.have_prev = prev != nullptr;
+    D.H = (turns & 1) ? W : H; D.W = (turns & 1) ? H : W;        // the upright frame
     D.src = frame; D.src_pitch = pitch; D.src_plane = plane_pitch;
-    return launch_frame_diff(nullptr, 1, D, (size_t)H * W * 3, sum, (cudaStream_t)stream, layout);
+    return launch_frame_diff(nullptr, 1, D, (size_t)H * W * 3, sum, (cudaStream_t)stream, layout, nullptr, turns);
+}
+
+extern "C" SKPS_API int skps_frame_ingest_layout(const uint8_t* frame, int H, int W, int pitch, int layout, int plane_pitch,
+                                                 uint8_t* packed, const uint8_t* prev, unsigned long long* sum, void* stream) {
+    return skps_frame_ingest_rotate(frame, H, W, pitch, layout, plane_pitch, 0, packed, prev, sum, stream);
 }
 
 extern "C" SKPS_API int skps_frame_ingest(const uint8_t* frame, int H, int W, int pitch, uint8_t* packed, const uint8_t* prev,

@@ -44,6 +44,7 @@ struct skps_mpipe {
                                               // then those of its keyframes, packed
         int32_t* h_det_slot = nullptr;        // pinned [S]: detector frame of each stream, -1 for none
         int32_t* h_stream = nullptr;          // pinned [S]: stream of each frame of the batch (uploaded when not the identity)
+        int32_t* h_turns = nullptr;           // pinned [S]: quarter turns of each device frame (uploaded when one is turned)
         int32_t* h_count = nullptr; int32_t* h_flag = nullptr;
         double* h_box = nullptr; double* h_kps = nullptr; float* h_scores = nullptr;
         uint8_t* h_chips = nullptr; double* h_M = nullptr;     // pinned, only while alignment is on
@@ -70,6 +71,7 @@ struct skps_mpipe {
     int32_t *d_hw = nullptr, *d_have_prev = nullptr, *d_flag = nullptr, *d_det_count = nullptr, *d_det_idx = nullptr;
     int32_t *d_count = nullptr, *d_detail = nullptr, *d_det_slot = nullptr;
     int32_t* d_stream = nullptr;              // [S] the batch's call -> stream map, when it is not the identity
+    int32_t* d_turns = nullptr;               // [S] the batch's quarter turns, when a frame is turned
     unsigned long long* d_diff = nullptr;
     MpStreamDesc* d_desc = nullptr;           // this batch's descriptors (uploaded on the compute stream, in order) [2S]
     void* d_nms_ws = nullptr;                 // NMS workspace, det_rows candidates per stream
@@ -119,7 +121,7 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
     if (p->s_copy) cudaStreamSynchronize(p->s_copy);
     for (uint8_t* f : p->d_frame) if (f) cudaFree(f);
     for (auto& sl : p->slot) {
-        void* host[] = {sl.h_desc, sl.h_det_slot, sl.h_stream, sl.h_stage, sl.h_hw, sl.h_have_prev, sl.h_geom, sl.h_count, sl.h_flag, sl.h_box,
+        void* host[] = {sl.h_desc, sl.h_det_slot, sl.h_stream, sl.h_turns, sl.h_stage, sl.h_hw, sl.h_have_prev, sl.h_geom, sl.h_count, sl.h_flag, sl.h_box,
                         sl.h_kps, sl.h_scores, sl.h_chips, sl.h_M, sl.h_pose, sl.h_ids};
         for (void* q : host) if (q) cudaFreeHost(q);
         if (sl.ev_in) cudaEventDestroy(sl.ev_in);
@@ -132,7 +134,7 @@ extern "C" SKPS_API void skps_mpipe_destroy(skps_mpipe* p) {
                    p->d_det_rows, p->d_boxes, p->d_kps_now, p->d_prev_lm, p->d_prev_dx, p->d_track, p->d_out_kps,
                    p->d_track_f32, p->d_n_prev, p->d_prev_f32, p->d_state_idx, p->d_n_track, p->d_chips, p->d_align_M, p->d_pose,
                    p->d_nms_ws, p->d_src, p->d_ids, p->d_next_id, p->d_det_slot, p->d_mem_ids, p->d_mem_box, p->d_mem_gap,
-                   p->d_mem_n, p->d_stream, p->d_out_box, p->d_out_ids};
+                   p->d_mem_n, p->d_stream, p->d_turns, p->d_out_box, p->d_out_ids};
     for (void* q : dev) if (q) cudaFree(q);
     if (p->s_copy) cudaStreamDestroy(p->s_copy);
     if (p->s_compute) cudaStreamDestroy(p->s_compute);
@@ -195,7 +197,7 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
         SKPS_HOST_ALLOC(sl.h_hw, sizeof(int32_t) * 2 * S); SKPS_HOST_ALLOC(sl.h_have_prev, sizeof(int32_t) * S);
         SKPS_HOST_ALLOC(sl.h_geom, sizeof(int32_t) * 8 * S);
         SKPS_HOST_ALLOC(sl.h_desc, sizeof(MpStreamDesc) * 2 * S); SKPS_HOST_ALLOC(sl.h_det_slot, sizeof(int32_t) * S);
-        SKPS_HOST_ALLOC(sl.h_stream, sizeof(int32_t) * S);
+        SKPS_HOST_ALLOC(sl.h_stream, sizeof(int32_t) * S); SKPS_HOST_ALLOC(sl.h_turns, sizeof(int32_t) * S);
         SKPS_HOST_ALLOC(sl.h_count, sizeof(int32_t) * S); SKPS_HOST_ALLOC(sl.h_flag, sizeof(int32_t) * S);
         SKPS_HOST_ALLOC(sl.h_box, sizeof(double) * 4 * K * S); SKPS_HOST_ALLOC(sl.h_kps, sizeof(double) * 2 * P * K * S);
         SKPS_HOST_ALLOC(sl.h_scores, sizeof(float) * P * K * S);
@@ -206,7 +208,7 @@ extern "C" SKPS_API int skps_mpipe_create(skps_engine* det, skps_engine* kps, co
     }
     if (cudaEventCreateWithFlags(&p->ev_ready, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&p->ev_read, cudaEventDisableTiming) != cudaSuccess) { set_error("cudaEventCreate"); return fail("event"); }
-    SKPS_DEV_ALLOC(p->d_desc, sizeof(MpStreamDesc) * 2 * S); SKPS_DEV_ALLOC(p->d_det_slot, 4 * S); SKPS_DEV_ALLOC(p->d_hw, 8 * S); SKPS_DEV_ALLOC(p->d_have_prev, 4 * S);
+    SKPS_DEV_ALLOC(p->d_desc, sizeof(MpStreamDesc) * 2 * S); SKPS_DEV_ALLOC(p->d_det_slot, 4 * S); SKPS_DEV_ALLOC(p->d_turns, 4 * S); SKPS_DEV_ALLOC(p->d_hw, 8 * S); SKPS_DEV_ALLOC(p->d_have_prev, 4 * S);
     SKPS_DEV_ALLOC(p->d_flag, 4 * S); SKPS_DEV_ALLOC(p->d_det_count, 4 * S);
     SKPS_DEV_ALLOC(p->d_det_idx, 4 * (size_t)p->det_rows * S); SKPS_DEV_ALLOC(p->d_count, 4 * S);
     SKPS_DEV_ALLOC(p->d_detail, 4 * 5 * (size_t)K * S);
@@ -255,11 +257,14 @@ static int check_stream_map(const skps_mpipe* p, const int32_t* streams, int n, 
 // state of temporal.cu) is indexed by the stream.  Host frames (pitches null) are uploaded on the copy stream into the
 // stream's next ring position; device frames (rows pitches[i] bytes apart) are gathered there by the frame-difference launch
 // on the compute stream, after the work queued on `producer`, whose later work waits for that launch; they are in pixel
-// layout `layout` (planes plane_pitches[i] bytes apart for the planar layouts) and land in the ring as BGR.  out: results
-// into caller buffers on the device instead of the slot's pinned ones.
+// layout `layout` (planes plane_pitches[i] bytes apart for the planar layouts) and land in the ring as BGR.  A device frame
+// stored turned turns[i] quarter turns clockwise (turns null: none) lands there upright, and from then on the batch sees
+// the upright frame: hw[i] is the stored size.  out: results into caller buffers on the device instead of the slot's
+// pinned ones.
 static int submit_batch(skps_mpipe* p, int slot_i, const int32_t* streams, const uint8_t* const* frames, const int32_t* hw,
                         int n, const int32_t* pitches, cudaStream_t producer, const skps_mpipe_outputs* out,
-                        int layout = SKPS_LAYOUT_BGR, const int32_t* plane_pitches = nullptr) {
+                        int layout = SKPS_LAYOUT_BGR, const int32_t* plane_pitches = nullptr,
+                        const int32_t* turns = nullptr) {
     const bool on_device = pitches != nullptr;
     SKPS_CHECK(p && frames && hw && (slot_i == 0 || slot_i == 1) && n > 0 && n <= p->S, "mpipe_submit: bad arguments");
     bool identity = true;
@@ -284,9 +289,10 @@ static int submit_batch(skps_mpipe* p, int slot_i, const int32_t* streams, const
     // behind the copy stream, or waited for on the host, whenever a batch uploads
     if (sl.device_out) SKPS_CUDA(cudaStreamWaitEvent(sc, sl.ev_done, 0));
     // ---- uploads on the copy stream: frame i of stream t = streams[i] into t's next ring position
+    bool turned = false;
     for (int i = 0; i < n; ++i) {
         const int t = streams ? streams[i] : i;
-        const int H = hw[2 * i], W = hw[2 * i + 1];
+        int H = hw[2 * i], W = hw[2 * i + 1];
         SKPS_CHECK(frames[i] && H > 0 && W > 0 && (size_t)H * W * 3 <= p->frame_bytes,
                    "mpipe_submit: frame %d is %dx%d, larger than the pipeline maximum %dx%d", i, H, W, c.max_h, c.max_w);
         if (on_device) {
@@ -294,6 +300,11 @@ static int submit_batch(skps_mpipe* p, int slot_i, const int32_t* streams, const
                        "mpipe_submit: frame %d has row pitch %d, less than %d x width %d", i, pitches[i], layout_xstep(layout), W);
             SKPS_CHECK(layout < SKPS_LAYOUT_BGR_PLANAR || plane_pitches[i] >= 0, "mpipe_submit: frame %d has plane pitch %d",
                        i, plane_pitches[i]);
+            const int q = turns ? turns[i] : 0;
+            SKPS_CHECK(q >= 0 && q <= 3, "mpipe_submit: frame %d has turns %d, outside 0..3", i, q);
+            sl.h_turns[i] = q;
+            turned |= q != 0;
+            if (q & 1) { H = hw[2 * i + 1]; W = hw[2 * i]; }       // the upright frame
         } else if (upload_host_frame(frames[i], (size_t)H * W * 3, sl.h_stage + p->frame_bytes * i,
                                      p->d_frame[(size_t)t * 3 + (p->ring_pos[t] + 1) % 3], sc)) {
             return 1;
@@ -325,7 +336,7 @@ static int submit_batch(skps_mpipe* p, int slot_i, const int32_t* streams, const
     size_t max_bytes = 0;
     for (int i = 0; i < n; ++i) {
         const int t = sl.h_stream[i];
-        const int H = hw[2 * i], W = hw[2 * i + 1];
+        const int H = sl.h_hw[2 * i], W = sl.h_hw[2 * i + 1];
         const bool key = !sl.h_have_prev[i] || (p->frame_idx[t] + t % N) % N == 0;
         sl.h_det_slot[i] = key ? m++ : -1;
         MpStreamDesc& D = sl.h_desc[i];
@@ -359,9 +370,12 @@ static int submit_batch(skps_mpipe* p, int slot_i, const int32_t* streams, const
         stream_map = p->d_stream;
         SKPS_CUDA(cudaMemcpyAsync(p->d_stream, sl.h_stream, 4 * n, cudaMemcpyHostToDevice, sx));
     }
+    // the turns of a batch holding a turned frame: its ingest is the turned kernel, any other the unturned one
+    if (turned) SKPS_CUDA(cudaMemcpyAsync(p->d_turns, sl.h_turns, 4 * n, cudaMemcpyHostToDevice, sx));
     SKPS_CUDA(cudaMemcpyAsync(p->d_desc, sl.h_desc, sizeof(MpStreamDesc) * n_desc, cudaMemcpyHostToDevice, sx));
     SKPS_CUDA(cudaEventRecord(sl.ev_staged, sx));
-    if (launch_frame_diff(p->d_desc, n, MpStreamDesc{}, max_bytes, p->d_diff, sx, on_device ? layout : SKPS_LAYOUT_BGR))
+    if (launch_frame_diff(p->d_desc, n, MpStreamDesc{}, max_bytes, p->d_diff, sx, on_device ? layout : SKPS_LAYOUT_BGR,
+                          turned ? p->d_turns : nullptr))
         return 1;
     if (on_device) {
         SKPS_CUDA(cudaEventRecord(p->ev_read, sx));
@@ -466,7 +480,7 @@ static int submit_batch(skps_mpipe* p, int slot_i, const int32_t* streams, const
     for (int i = 0; i < n; ++i) {
         const int t = sl.h_stream[i];
         p->ring_pos[t] = (p->ring_pos[t] + 1) % 3;
-        p->prev_h[t] = hw[2 * i]; p->prev_w[t] = hw[2 * i + 1];
+        p->prev_h[t] = sl.h_hw[2 * i]; p->prev_w[t] = sl.h_hw[2 * i + 1];
         ++p->frame_idx[t];
     }
     sl.n = n;
@@ -485,19 +499,30 @@ extern "C" SKPS_API int skps_mpipe_submit(skps_mpipe* p, int slot_i, const uint8
     return skps_mpipe_submit_streams(p, slot_i, nullptr, frames, hw, n);
 }
 
-extern "C" SKPS_API int skps_mpipe_submit_device_layout(skps_mpipe* p, int slot_i, const int32_t* streams,
+extern "C" SKPS_API int skps_mpipe_submit_device_rotate(skps_mpipe* p, int slot_i, const int32_t* streams,
                                                         const uint8_t* const* frames, const int32_t* pitches, const int32_t* hw,
-                                                        int n, int layout, const int32_t* plane_pitches,
+                                                        int n, int layout, const int32_t* plane_pitches, const int32_t* turns,
                                                         const skps_mpipe_outputs* out, void* producer_stream) {
     SKPS_CHECK(p && frames && pitches && hw && n > 0 && n <= p->S, "mpipe_submit_device: bad arguments");
     SKPS_CHECK(layout_ok(layout), "mpipe_submit_device: unknown pixel layout %d", layout);
     SKPS_CHECK(layout < SKPS_LAYOUT_BGR_PLANAR || plane_pitches, "mpipe_submit_device: a planar layout needs plane pitches");
+    for (int i = 0; turns && i < n; ++i)
+        SKPS_CHECK(turns[i] >= 0 && turns[i] <= 3, "mpipe_submit_device: frame %d has turns %d, outside 0..3", i, turns[i]);
     bool identity = true;
     if (check_stream_map(p, streams, n, &identity)) return 1;
     SKPS_ON_DEVICE(p->device);
     for (int i = 0; i < n; ++i)
         if (check_device_frame(frames[i], p->device, "mpipe_submit_device", i)) return 1;
-    return submit_batch(p, slot_i, streams, frames, hw, n, pitches, (cudaStream_t)producer_stream, out, layout, plane_pitches);
+    return submit_batch(p, slot_i, streams, frames, hw, n, pitches, (cudaStream_t)producer_stream, out, layout, plane_pitches,
+                        turns);
+}
+
+extern "C" SKPS_API int skps_mpipe_submit_device_layout(skps_mpipe* p, int slot_i, const int32_t* streams,
+                                                        const uint8_t* const* frames, const int32_t* pitches, const int32_t* hw,
+                                                        int n, int layout, const int32_t* plane_pitches,
+                                                        const skps_mpipe_outputs* out, void* producer_stream) {
+    return skps_mpipe_submit_device_rotate(p, slot_i, streams, frames, pitches, hw, n, layout, plane_pitches, nullptr, out,
+                                           producer_stream);
 }
 
 extern "C" SKPS_API int skps_mpipe_submit_device_streams(skps_mpipe* p, int slot_i, const int32_t* streams,

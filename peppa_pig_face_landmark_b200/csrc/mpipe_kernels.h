@@ -29,6 +29,31 @@ __host__ __device__ __forceinline__ PxLayout px_layout(int layout, int plane) {
     return l;
 }
 
+// A frame stored H x W (row pitch `pitch`, layout and plane pitch as px_layout takes them) that must be turned `turns`
+// quarter turns clockwise to be upright (cv2.rotate: 1 ROTATE_90_CLOCKWISE, 2 ROTATE_180, 3 ROTATE_90_COUNTERCLOCKWISE):
+// pixel (y, x) of the upright frame, H' x W' (W x H for odd turns), has its B, G, R bytes at
+// base + org + y * ystep + x * xstep + off[0..2].  Only the low two bits of `turns` are read.
+struct PxView {
+    long long org, ystep, xstep;
+    long long off[3];
+    int H, W;                    // the upright frame's size
+};
+__host__ __device__ __forceinline__ PxView px_view(int layout, int plane, int pitch, int H, int W, int turns) {
+    const PxLayout l = px_layout(layout, plane);
+    const long long p = pitch, s = l.xs;
+    PxView v;
+    v.off[0] = l.off[0]; v.off[1] = l.off[1]; v.off[2] = l.off[2];
+    switch (turns & 3) {
+        case 0: v.org = 0; v.ystep = p; v.xstep = s; break;
+        case 1: v.org = (H - 1) * p; v.ystep = s; v.xstep = -p; break;
+        case 2: v.org = (H - 1) * p + (W - 1) * s; v.ystep = -p; v.xstep = -s; break;
+        default: v.org = (W - 1) * s; v.ystep = -s; v.xstep = p; break;
+    }
+    v.H = (turns & 1) ? W : H;
+    v.W = (turns & 1) ? H : W;
+    return v;
+}
+
 // Block g of a launch over n calls' frames serves stream stream[g] (stream null: g).  The per-frame inputs and outputs are
 // in call order, rows g < n; the state is indexed by the stream, rows [S].
 struct MpTemporalArgs {
@@ -95,6 +120,7 @@ struct LetterboxArgs {
     const skps_frame_layout* lay;               // with src: its pixel layout lay[g] [dev], or null (BGR)
     uint8_t* out; size_t out_stride;
     int in_h, in_w;
+    const int* turns;                           // with src: quarter turns clockwise of frame g [dev], or null (none)
 };
 int launch_letterbox(const LetterboxArgs& a, int n, cudaStream_t s);
 
@@ -139,8 +165,11 @@ int launch_landmark_post(const float* xy, const int* detail, const int* count, i
 // with src set is first gathered into cur in the same pass (the same integer sum as from a packed cur); its pixels are in
 // `layout` (SKPS_LAYOUT_*, one for the launch; cur gets them as BGR).  Frame g is d[g] [dev], or (d null, n = 1) `one` of
 // `bytes` bytes, any count when one.src is null; with d, bytes is the largest frame's packed size.
+// Rotated frames: src of frame g must be turned turns[g] [dev] (d set) or one_turns (d null) quarter turns clockwise to be
+// upright (px_view), and cur gets the upright frame, D.H x D.W; the sum is that of the upright frame.  A launch with turns
+// null and one_turns 0 runs the unrotated kernels.
 int launch_frame_diff(const MpStreamDesc* d, int n, const MpStreamDesc& one, size_t bytes, unsigned long long* sum,
-                      cudaStream_t s, int layout = 0);
+                      cudaStream_t s, int layout = 0, const int* turns = nullptr, int one_turns = 0);
 
 // Frame staging on the host side, shared by skps_pipeline and skps_mpipe.  upload_host_frame queues the H2D copy of a [host]
 // frame of `bytes` bytes into dst on s: a pinned frame is copied as it is, a pageable one first into `stage` (pinned, at

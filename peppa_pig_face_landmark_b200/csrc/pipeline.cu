@@ -180,33 +180,44 @@ extern "C" SKPS_API int skps_pipeline_frame_diff(skps_pipeline* p, const uint8_t
 // One ingest pass gathers the [dev] frame, in any pixel layout, into d_frame[cur] as BGR and, against a previous frame of
 // the same size, sums the difference.  The read waits for the work queued on the producer stream so far, and the
 // producer's later work waits for the read.
-extern "C" SKPS_API int skps_pipeline_frame_diff_device_layout(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch,
-                                                               int layout, int plane_pitch, void* producer_stream,
+// A frame stored turned `turns` quarter turns clockwise is staged upright by the same pass: from then on the pipeline sees
+// the upright frame, of size W x H for odd turns.
+extern "C" SKPS_API int skps_pipeline_frame_diff_device_rotate(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch,
+                                                               int layout, int plane_pitch, int turns, void* producer_stream,
                                                                double* mean_diff, void* stream) {
     SKPS_CHECK(p && frame && mean_diff, "frame_diff_device: null argument");
     SKPS_CHECK(layout_ok(layout), "frame_diff_device: unknown pixel layout %d", layout);
+    SKPS_CHECK(turns >= 0 && turns <= 3, "frame_diff_device: turns %d outside 0..3", turns);
     SKPS_CHECK(H == 1 || pitch >= layout_xstep(layout) * W, "frame_diff_device: row pitch %d is less than %d x width %d",
                pitch, layout_xstep(layout), W);
     SKPS_CHECK(layout < SKPS_LAYOUT_BGR_PLANAR || plane_pitch >= 0, "frame_diff_device: plane pitch %d < 0", plane_pitch);
     cudaStream_t s = (cudaStream_t)stream, producer = (cudaStream_t)producer_stream;
     SKPS_ON_DEVICE(p->device);
     if (check_device_frame(frame, p->device, "frame_diff_device", -1) || check_frame_size(p, H, W)) return 1;
-    const bool diff = p->prev_h == H && p->prev_w == W;
+    const int Hu = (turns & 1) ? W : H, Wu = (turns & 1) ? H : W;         // the upright frame
+    const bool diff = p->prev_h == Hu && p->prev_w == Wu;
     SKPS_CUDA(cudaEventRecord(p->ev_ready, producer));
     SKPS_CUDA(cudaStreamWaitEvent(s, p->ev_ready, 0));
     MpStreamDesc D = {};
     D.cur = p->d_frame[p->cur]; D.prev = diff ? p->d_frame[p->cur ^ 1] : nullptr; D.have_prev = diff;
-    D.H = H; D.W = W; D.src = frame; D.src_pitch = pitch; D.src_plane = plane_pitch;
+    D.H = Hu; D.W = Wu; D.src = frame; D.src_pitch = pitch; D.src_plane = plane_pitch;
     if (diff) SKPS_CUDA(cudaMemsetAsync(p->d_diff, 0, sizeof(unsigned long long), s));
-    if (launch_frame_diff(nullptr, 1, D, (size_t)H * W * 3, p->d_diff, s, layout)) return 1;
+    if (launch_frame_diff(nullptr, 1, D, (size_t)H * W * 3, p->d_diff, s, layout, nullptr, turns)) return 1;
     SKPS_CUDA(cudaEventRecord(p->ev_read, s));
     SKPS_CUDA(cudaStreamWaitEvent(producer, p->ev_read, 0));
-    p->cur_h = H; p->cur_w = W;
+    p->cur_h = Hu; p->cur_w = Wu;
     if (!diff) {
         *mean_diff = -1.0;
         return 0;
     }
-    return read_mean_diff(p, H, W, mean_diff, s);
+    return read_mean_diff(p, Hu, Wu, mean_diff, s);
+}
+
+extern "C" SKPS_API int skps_pipeline_frame_diff_device_layout(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch,
+                                                               int layout, int plane_pitch, void* producer_stream,
+                                                               double* mean_diff, void* stream) {
+    return skps_pipeline_frame_diff_device_rotate(p, frame, H, W, pitch, layout, plane_pitch, 0, producer_stream, mean_diff,
+                                                  stream);
 }
 
 extern "C" SKPS_API int skps_pipeline_frame_diff_device(skps_pipeline* p, const uint8_t* frame, int H, int W, int pitch,

@@ -78,6 +78,7 @@ SIGNATURES = {
                                  C.c_int, C.c_int, C.c_int, C.c_int, c_vp]),
     "skps_letterbox_frames": (C.c_int, [c_vp, C.c_int, c_vp, C.c_int, C.c_int, c_vp]),
     "skps_letterbox_frames_layout": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, C.c_int, C.c_int, c_vp]),
+    "skps_letterbox_frames_rotate": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, c_vp, C.c_int, C.c_int, c_vp]),
     "skps_detect_post": (C.c_int, [c_vp, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
                                    c_vp, c_vp, c_vp, C.c_int, c_vp]),
     "skps_detect_post_workspace_size": (C.c_size_t, [C.c_int, C.c_int]),
@@ -92,10 +93,13 @@ SIGNATURES = {
                                    c_vp, C.c_int, c_vp, c_vp]),
     "skps_crop_faces": (C.c_int, [c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, C.c_int, c_vp, c_vp]),
     "skps_crop_faces_layout": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, C.c_int, c_vp, c_vp]),
+    "skps_crop_faces_rotate": (C.c_int, [c_vp, c_vp, c_vp, c_vp, C.c_int, C.c_float, C.c_float, c_vp, C.c_int, c_vp, c_vp]),
     "skps_landmark_post": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_int, c_vp, c_vp]),
     "skps_frame_absdiff_sum": (C.c_int, [c_vp, c_vp, C.c_size_t, c_vp, c_vp]),
     "skps_frame_ingest": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp]),
     "skps_frame_ingest_layout": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp]),
+    "skps_frame_ingest_rotate": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp,
+                                           c_vp]),
     "skps_pipeline_create": (C.c_int, [c_vp, c_vp, C.POINTER(PipelineCfg), C.POINTER(c_vp)]),
     "skps_pipeline_destroy": (None, [c_vp]),
     "skps_pipeline_reset": (C.c_int, [c_vp]),
@@ -119,6 +123,8 @@ SIGNATURES = {
                                                    c_vp]),
     "skps_mpipe_submit_device_layout": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp, C.c_int, C.c_int, c_vp,
                                                   C.POINTER(MpipeOutputs), c_vp]),
+    "skps_mpipe_submit_device_rotate": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_vp, c_vp, C.c_int, C.c_int, c_vp, c_vp,
+                                                  C.POINTER(MpipeOutputs), c_vp]),
     "skps_mpipe_wait_stream": (C.c_int, [c_vp, C.c_int, c_vp]),
     "skps_mpipe_track_ids": (C.c_int, [c_vp, C.c_int, c_vp]),
     "skps_debug_mp_temporal": (C.c_int, [C.POINTER(PipelineCfg), C.c_int, C.c_int, C.c_int] + [c_vp] * 18),
@@ -127,13 +133,18 @@ SIGNATURES = {
     "skps_pipeline_frame_diff_device": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, C.POINTER(C.c_double), c_vp]),
     "skps_pipeline_frame_diff_device_layout": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_vp,
                                                          C.POINTER(C.c_double), c_vp]),
+    "skps_pipeline_frame_diff_device_rotate": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                         c_vp, C.POINTER(C.c_double), c_vp]),
     "skps_warp_affine": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
     "skps_align_faces": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp,
                                    c_vp]),
     "skps_warp_faces": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
     "skps_warp_faces_layout": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
+    "skps_warp_faces_rotate": (C.c_int, [c_vp, c_vp, c_vp, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
     "skps_align_estimate": (C.c_int, [c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
     "skps_warp_faces_count": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_int, c_vp, C.c_int, C.c_int, c_vp, c_vp]),
+    "skps_warp_faces_count_rotate": (C.c_int, [c_vp, c_vp, c_vp, c_vp, C.c_int, C.c_int, c_vp, C.c_int, C.c_int, c_vp,
+                                               c_vp]),
     "skps_det_align_estimate": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp]),
     "skps_pipeline_align": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, c_vp, c_vp, c_vp]),
     "skps_mpipe_set_align": (C.c_int, [c_vp, C.c_int]),
